@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Headline benchmark: NeuTTS-Air synthetic 500-prefill / 250-decode utterances -> 24 kHz PCM.
 
-    python bench.py --gpus N --steps K --warmup W            # B200 path (this repo)
+    python bench.py --gpus N --steps K --warmup W            # the CUDA path of this repo (H100)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's PyTorch CPU path
 
 One "step" = one pass of the hot path over one batch of utterances per GPU: prefill(500) ->
@@ -48,6 +48,8 @@ def parse():
                     help="fixed: every prompt 500 tokens (configs[1]); mixed: prompt lengths U{200..1400}, seeded (configs[2])")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-sweep", action="store_true", help="skip the batch 8 / 64 lines reported under 'batches' (N=1 runs only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (PCM, generated ids) as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -56,7 +58,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 # ----------------------------------------------------------------------------------------------
@@ -77,7 +79,7 @@ def synth_prompts(n, vocab, speech_base, seed, mixed=False):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -113,6 +115,16 @@ class ClockSampler:
                         reasons.add(nme)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": sorted(reasons), "samples": len(sm)}
+
+
+def gpu_identity(gpu_index):
+    """Card name and power limit (read-only nvidia-smi query): an absolute number is only meaningful with both."""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
+                              "-i", str(gpu_index)], capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        return {"name": out[0].strip(), "power_limit_w": float(out[1]), "sm_max_mhz": float(out[2])}
+    except Exception:
+        return {"name": torch.cuda.get_device_name(gpu_index), "power_limit_w": None, "sm_max_mhz": None}
 
 
 # ----------------------------------------------------------------------------------------------
@@ -226,13 +238,11 @@ def main_reference(args):
 
 
 # ----------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ----------------------------------------------------------------------------------------------
 _WEIGHTS = {}
 SPEECH_BASE, EOS = 151936, 151670
-# dram__bytes_read.sum + dram__bytes_write.sum of ONE decode_tc_kernel launch (249 steps, batch 1, contexts 500..749)
-# from profiles/decode_tc_b1_r2_ncu_summary.txt (ncu --set full); None until a capture of the current kernel exists
-NCU_TRAFFIC_B1 = 278.50e9
+DUMP_BYTES = 64 << 20   # --dump-outputs writes at most this much
 
 
 def build_engines(device, batch, prefill_tokens=None):
@@ -298,10 +308,8 @@ def decode_roofline(lm, B, lens, t_dec, n_steps, launches_per_step):
     t = t_dec if persistent else t_dec / n_steps
     return {"bound": "hbm",
             "kernel": ("decode_tc_kernel (persistent: all layers + lm_head + sampler, %d decode steps per launch)" % n_steps) if persistent
-            else "decode step = CUDA graph of %d kernels (tcgen05 GEMMs, attention, norms, sampler)" % launches_per_step,
+            else "decode step = CUDA graph of %d kernels (wgmma GEMMs, attention, norms, sampler)" % launches_per_step,
             "achieved": alg / t / 1e9, "peak": peak, "unit": "GB/s", "frac": alg / t / 1e9 / peak,
-            "traffic": NCU_TRAFFIC_B1 if (persistent and B == 1) else None,
-            "traffic_source": "profiles/decode_tc_b1_r2_ncu_summary.txt (dram__bytes_read.sum + dram__bytes_write.sum, one launch)",
             "peak_source": how, "algorithmic_bytes_per_launch": alg, "us_per_launch": t * 1e6,
             "us_per_decode_step": t_dec / n_steps * 1e6, "algorithmic_bytes_per_step": sb}
 
@@ -404,6 +412,22 @@ def stream_line(dev, B=8, frames_per_chunk=50, L=None):
             "api": "neutts.NeuTTS._stream_batch (engine loop of infer_stream_batch)"}
 
 
+def dump_outputs(out_dir, arrays):
+    """Writes {name: tensor} as out_dir/<name>.npy (float32, or float64 for integer ids so they stay exact).  When the
+    whole set exceeds DUMP_BYTES, every array keeps the same fixed, seeded sample of its rows."""
+    os.makedirs(out_dir, exist_ok=True)
+    host = {k: (v.detach().cpu().double() if not v.is_floating_point() else v.detach().cpu().float()) for k, v in arrays.items()}
+    total = sum(v.numel() * v.element_size() for v in host.values())
+    rows = min(v.shape[0] for v in host.values())
+    if total > DUMP_BYTES:
+        keep = max(1, int(rows * DUMP_BYTES // total))
+        idx = torch.randperm(rows, generator=torch.Generator().manual_seed(0))[:keep].sort().values
+        host = {k: v[idx] for k, v in host.items()}
+        host["sampled_rows"] = idx.double()
+    for k, v in host.items():
+        np.save(os.path.join(out_dir, k + ".npy"), v.numpy())
+
+
 def main_b200(args):
     import torch.distributed as td
 
@@ -486,12 +510,14 @@ def main_b200(args):
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     ev0.record()
     for i in range(args.steps):
-        gather(step_device(100 + i))
+        pcm = gather(step_device(100 + i))
     ev1.record()
     barrier()
     t_dev = ev0.elapsed_time(ev1) / 1e3
     launches = L.nt_launch_count() - n0
     clk = clocks.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:   # the last timed step's results, as its caller receives them
+        dump_outputs(args.dump_outputs, {"pcm": pcm.reshape(pcm.shape[0], -1), "generated_ids": lm.out_tokens[:B, :DECODE]})
 
     # the parts, each timed alone with CUDA events
     t_dec, dec_launches = time_decode(lm, prompts)
@@ -542,7 +568,7 @@ def main_b200(args):
                                  f"configs[1]: 500 prefill / 250 decode tokens + NeuCodec decode to 24 kHz, batch={B} per GPU")),
                    "per_gpu_batch": B, "global_batch": B * world, "sharding": "utterances one-per-GPU-slot, weights replicated, "
                    "one all-gather of waveforms" if world > 1 else "single GPU",
-                   "l2": "inputs larger than L2: 1.1 GB of weights stream per decode step (L2 = 126 MB)", "weights": "seeded random, inferred Air/NeuCodec shapes"},
+                   "l2": "inputs larger than L2: 1.1 GB of weights stream per decode step (H100 L2 = 50 MB)", "weights": "seeded random, inferred Air/NeuCodec shapes"},
         "decode_tok_s": B * world * (DECODE - 1) / t_dec,
         "roofline": roof,
         "breakdown_ms": {"prefill": t_pre * 1e3, "decode_249_steps": t_dec * 1e3, "codec": t_codec * 1e3},
@@ -550,6 +576,7 @@ def main_b200(args):
                 "ms_per_step": t_e2e / args.steps * 1e3, "api": "neutts.NeuTTS.infer_from_prompt_ids" + (" + dist.all_gather_waveforms" if world > 1 else "")},
         "gpu_launches": int(launches),
         "clocks": clk,
+        "device": gpu_identity(local),
     }
     if world == 1 and not args.no_sweep:
         del lm, codec, tts
@@ -569,6 +596,8 @@ def main_b200(args):
 
 if __name__ == "__main__":
     a = parse()
+    if a.steps < 1:
+        raise SystemExit("--steps must be >= 1")
     if a.impl == "reference":
         main_reference(a)
     else:

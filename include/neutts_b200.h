@@ -1,4 +1,4 @@
-/* neutts_b200 — C-ABI of the B200 (sm_100a) implementation of NeuTTS-Air's two inference
+/* neutts_b200 — C-ABI of the H100 (sm_90a) implementation of NeuTTS-Air's two inference
  * hot paths.  Plain pointers and sizes only; no torch / C++ types cross this boundary.
  *
  * The reference has no FFI of its own (it is 465 lines of Python over `transformers` and
@@ -47,7 +47,7 @@ int nt_abi_version(void);   /* 2: nt_sampling gained limits + slot_base; 3: nt_c
 uint64_t nt_launch_count(void);
 
 /* ------------------------------------------------------------------------------------------
- * Generic tensor-core GEMM (tcgen05 + TMEM + TMA):  C[M,N] = epilogue(A[M,K] . W[N,K]^T)
+ * Generic tensor-core GEMM (wgmma + TMA):  C[M,N] = epilogue(A[M,K] . W[N,K]^T)
  * Used by prefill, batched decode and the codec.  Replaces torch addmm/mm as reached from
  * transformers modeling_qwen2.py:46-48,217-219,244,475 and the codec's Linear/Conv1d layers.
  * ------------------------------------------------------------------------------------------ */

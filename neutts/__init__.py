@@ -1,4 +1,4 @@
-"""Public name of the reference package (`from neutts import NeuTTS`), served by the B200 build.
+"""Public name of the reference package (`from neutts import NeuTTS`), served by the H100 build.
 
 The class lives in :mod:`neutts.neutts`; everything below its two inner seams is ``libneutts_b200.so``
 (see INTEGRATION.md)."""

@@ -1,11 +1,11 @@
-"""Drop-in ``neutts.NeuTTS`` on the B200 engine.
+"""Drop-in ``neutts.NeuTTS`` on the H100 engine.
 
 Same public surface as the reference facade (``/root/reference/neutts/neutts.py:73-465``):
 constructor signature and attributes (``:75-98``), ``infer`` (``:216``), ``infer_stream`` (``:245``),
 ``encode_reference`` (``:266``), the private seams ``_apply_chat_template`` / ``_infer_torch`` /
 ``_decode`` / ``_to_phones``, and the same error convention (``ValueError`` / ``ImportError`` /
 ``NotImplementedError``).  Behind it, hot path A (speech-LM prefill + decode) and hot path B
-(NeuCodec decoder) run in ``libneutts_b200.so`` on an sm_100a GPU; there is no CPU fallback and no
+(NeuCodec decoder) run in ``libneutts_b200.so`` on an sm_90a GPU; there is no CPU fallback and no
 llama.cpp / ONNX / vLLM dispatch.
 
 What differs from the reference, on purpose:
@@ -64,7 +64,7 @@ class NeuTTS:
         """Same positional signature and defaults as the reference (``neutts/neutts.py:75-81``), so
         ``examples/basic_example.py:12-17`` runs unmodified.  The device strings keep their reference
         meaning for the CALLER -- ``"cpu"`` = results come back as host arrays, which this facade always
-        does -- but the engines themselves only exist for sm_100a: a ``"cpu"`` request runs on the current
+        does -- but the engines themselves only exist for sm_90a: a ``"cpu"`` request runs on the current
         CUDA device and says so once (there is no CPU fallback)."""
         # constants the reference exposes (neutts/neutts.py:84-91)
         self.sample_rate = 24_000
@@ -107,7 +107,7 @@ class NeuTTS:
             self.backbone = backbone
             return
         if str(backbone_repo).endswith("gguf"):
-            raise ValueError("GGUF / llama.cpp backbones are not dispatched by the B200 build; "
+            raise ValueError("GGUF / llama.cpp backbones are not dispatched by the H100 build; "
                              "use the safetensors checkpoint (e.g. neuphonic/neutts-air)")
         backbone_device = self._engine_device(backbone_device, "backbone")
         from neutts_air_b200 import loader
@@ -122,7 +122,7 @@ class NeuTTS:
             self.codec = codec
             return
         if str(codec_repo).endswith(".onnx") or codec_repo == "neuphonic/neucodec-onnx-decoder":
-            raise ValueError("ONNX codec decoders are not dispatched by the B200 build; use 'neuphonic/neucodec'")
+            raise ValueError("ONNX codec decoders are not dispatched by the H100 build; use 'neuphonic/neucodec'")
         if codec_repo not in ("neuphonic/neucodec", "neuphonic/distill-neucodec") and not Path(str(codec_repo)).exists():
             raise ValueError("Invalid codec repo! Must be one of: 'neuphonic/neucodec', 'neuphonic/distill-neucodec' "
                              "(or a local checkpoint directory).")
@@ -134,16 +134,16 @@ class NeuTTS:
 
     @staticmethod
     def _engine_device(requested, what: str):
-        """Reference device string -> the CUDA device the B200 engine runs on."""
+        """Reference device string -> the CUDA device the H100 engine runs on."""
         dev = torch.device(requested)
         if dev.type == "cuda":
             return dev
         if dev.type != "cpu":
             raise ValueError(f"unsupported {what}_device {requested!r}")
         if not torch.cuda.is_available():
-            raise RuntimeError(f"neutts (B200 build): {what}_device={requested!r} was requested, but the engines exist only for "
-                               "CUDA sm_100a and no CUDA device is visible (there is no CPU fallback)")
-        warnings.warn(f"neutts (B200 build): {what}_device={requested!r} -> running on cuda:{torch.cuda.current_device()}; "
+            raise RuntimeError(f"neutts (H100 build): {what}_device={requested!r} was requested, but the engines exist only for "
+                               "CUDA sm_90a and no CUDA device is visible (there is no CPU fallback)")
+        warnings.warn(f"neutts (H100 build): {what}_device={requested!r} -> running on cuda:{torch.cuda.current_device()}; "
                       "outputs are returned on the host as with the reference's CPU path", stacklevel=3)
         return torch.device("cuda", torch.cuda.current_device())
 
@@ -289,7 +289,7 @@ class NeuTTS:
         every 25 new frames (once 5 look-ahead frames exist) the codec re-decodes
         [n - 50 - 1, n + 25 + 5 + 1) and the chunk is cross-faded with triangular weights."""
         if self._is_quantized_model:  # kept for signature parity; never true on this build
-            raise NotImplementedError("GGUF streaming is not part of the B200 build")
+            raise NotImplementedError("GGUF streaming is not part of the H100 build")
         prompt = self._apply_chat_template(ref_codes, ref_text, text)
         return self._stream(prompt, [int(c) for c in (ref_codes.tolist() if hasattr(ref_codes, "tolist") else ref_codes)])
 

@@ -1,4 +1,4 @@
-"""neutts_air_b200 — B200 (sm_100a) implementation of NeuTTS-Air's two inference hot paths
+"""neutts_air_b200 — H100 (sm_90a) implementation of NeuTTS-Air's two inference hot paths
 (speech-LM prefill/decode and the NeuCodec decoder) behind a C-ABI shared library.
 
 Only what the path needs lives here: ``csrc/`` (CUDA kernels + C-ABI), ``_lib`` (ctypes binding),

@@ -103,12 +103,12 @@ def lib() -> C.CDLL:
     if _lib is not None:
         return _lib
     path = LIB_PATH
-    if os.environ.get("NT_LIB_PATH"):      # A/B measurements against an older build of the library (profiles/ab/)
+    if os.environ.get("NT_LIB_PATH"):      # A/B measurements against another build of the library
         path = Path(os.environ["NT_LIB_PATH"])
     if not path.exists():
         raise RuntimeError(
             f"{path} is missing: build it with `python -m neutts_air_b200.build` "
-            "(nvcc, sm_100a). neutts_air_b200 has no CPU or PyTorch fallback.")
+            "(nvcc, sm_90a). neutts_air_b200 has no CPU or PyTorch fallback.")
     L = C.CDLL(str(path))
     L.nt_last_error.restype = C.c_char_p
     L.nt_abi_version.restype = C.c_int

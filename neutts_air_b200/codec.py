@@ -90,7 +90,7 @@ class CodecDecoder:
         if precision not in self.PRECISIONS:
             raise ValueError(f"precision must be one of {sorted(self.PRECISIONS)}")
         if not torch.cuda.is_available():
-            raise RuntimeError("neutts_air_b200.CodecDecoder needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("neutts_air_b200.CodecDecoder needs a CUDA device (sm_90a); there is no CPU fallback")
         if shape.rope_axis not in ("time", "head"):
             raise ValueError(f"rope_axis {shape.rope_axis!r}")
         self.L = _lib.lib()
@@ -131,7 +131,7 @@ class CodecDecoder:
 
     def to(self, device):
         if torch.device(device).type != "cuda":
-            raise ValueError("neutts_air_b200.CodecDecoder runs on CUDA (sm_100a) only")
+            raise ValueError("neutts_air_b200.CodecDecoder runs on CUDA (sm_90a) only")
         return self
 
     @torch.no_grad()

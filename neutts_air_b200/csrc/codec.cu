@@ -1,8 +1,8 @@
-// NeuCodec decoder (seam 2: neutts/neutts.py:288-291 -> codec.decode_code) for sm_100a.
+// NeuCodec decoder (seam 2: neutts/neutts.py:288-291 -> codec.decode_code) for sm_90a.
 //
 // Activations are channels-last fp32 in a padded-batch layout: item b owns rows
 // [b*Tp, (b+1)*Tp) with Tp = N + 6; frame t sits at row b*Tp + 3 + t and the 3 rows on either
-// side stay zero, so every Conv1d (k=7 and k=3, "same" padding) is a plain TMA-fed tcgen05
+// side stay zero, so every Conv1d (k=7 and k=3, "same" padding) is a plain TMA-fed wgmma
 // GEMM whose K loop walks the taps (gemm_tc.cu) — no im2col buffer, no per-item launches.
 // All dense math runs on the tensor cores as TF32 with fp32 accumulation (the <=1e-3 RMS PCM
 // bar of BASELINE.json rules out bf16 operands here); norms, attention softmax, exp/sin/cos
@@ -376,9 +376,10 @@ extern "C" int nt_codec_create(const nt_codec_config* cfg, const nt_codec_weight
     for (int j = 0; j < cfg->depth; ++j) k->blk[i].push_back(bsrc[i][j]);
   int dev = 0;
   cudaDeviceProp prop;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaGetDeviceProperties(&prop, dev) != cudaSuccess || prop.major != 10) {
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaGetDeviceProperties(&prop, dev) != cudaSuccess || prop.major != 9 ||
+      prop.minor != 0) {
     delete k;
-    return set_error(NT_ERR_CUDA, "no sm_100 CUDA device: this library has no CPU fallback");
+    return set_error(NT_ERR_CUDA, "no sm_90 CUDA device: this library has no CPU fallback");
   }
   float invf[64] = {0};
   for (int i = 0; i < 32; ++i) invf[i] = static_cast<float>(1.0 / std::pow(static_cast<double>(cfg->rope_base), (2.0 * i) / 64.0));
@@ -424,7 +425,7 @@ struct CodecRun {
   // masked GEMM on the padded layout: out rows r+3 for r with (r % Tp) < N.
   // A points at the first row the tap window of output row 0 touches.
   // sw (optional): the weight's hi / lo halves -> 3xTF32 in one pass of the GEMM kernel (A_lo.W_hi + A_hi.W_lo +
-  // A_hi.W_hi into one TMEM accumulator); the activations are split into a hi / lo pair of buffers first.
+  // A_hi.W_hi into one accumulator); the activations are split into a hi / lo pair of buffers first.
   int gemm(const float* A, int K, int lda, const float* W, const float* bias, const float* residual, nt_act act, float* out,
            int ldc, int Nout, bool masked, const SplitW* sw = nullptr, int ldw = 0) {
     nt_gemm_args a;

@@ -1,5 +1,5 @@
-// Shared device helpers for the sm_100a kernels: mbarrier, bulk/TMA copies, tcgen05
-// (UMMA + TMEM), programmatic dependent launch, small math utilities.
+// Shared device helpers for the sm_90a kernels: mbarrier, bulk/TMA copies, wgmma (warpgroup MMA),
+// programmatic dependent launch, small math utilities.
 // Everything is inline PTX; no CUTLASS/CuTe headers are included.
 #pragma once
 #include <cuda_runtime.h>
@@ -9,6 +9,8 @@
 #include <stdio.h>
 
 #define NT_DEVINL __device__ __forceinline__
+
+#include "wgmma.cuh"
 
 // Spin bound for every mbarrier wait: a protocol bug becomes a trap (the launch fails with
 // an error the host reports) instead of a hung GPU box.  try_wait itself suspends the thread for
@@ -25,11 +27,11 @@ constexpr int kWarp = 32;
 NT_DEVINL uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 NT_DEVINL int lane_id() { return threadIdx.x & 31; }
 // One lane of a fully converged warp (the same lane on every call).  Code issuing uniform-datapath instructions
-// (tcgen05.mma / commit, TMA) must sit under THIS predicate inside warp-uniform control flow: behind a plain
-// `if (lane == 0)` the compiler cannot prove that a single thread is active and wraps every such instruction in an
-// ELECT / BRA.U.ANY loop with R2UR moves -- measured ~160 cycles per tcgen05.mma issue instead of back-to-back issue.
+// (TMA) must sit under THIS predicate inside warp-uniform control flow: behind a plain `if (lane == 0)` the compiler
+// cannot prove that a single thread is active and wraps every such instruction in an ELECT / BRA.U.ANY loop with
+// R2UR moves.
 // Call it AT the use site, after any data-dependent wait loop: elect.sync (full mask) is also the reconvergence point,
-// and the compiler emits the guarded UTMALDG / UTCHMMA unpredicated (only the operand moves carry the predicate), so
+// and the compiler emits the guarded UTMALDG unpredicated (only the operand moves carry the predicate), so
 // a diverged lane group without the leader would execute it with stale uniform registers (memcheck: out-of-range
 // shared address; found with a cached `leader` flag behind an mbarrier spin).
 NT_DEVINL bool elect_one() {
@@ -74,12 +76,18 @@ NT_DEVINL bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
+#ifdef NT_WGMMA_KERNELS
+// Translation units with wgmma kernels: a function call anywhere in such a kernel makes ptxas serialize its wgmma
+// pipeline, so a timeout traps in line without the report.
+NT_DEVINL void nt_timeout(const char*) { __trap(); }
+#else
 // out of line on purpose: the report is cold code, inlined it would sit (printf argument set-up and all) in the
 // instruction stream of every wait loop of kernels that already fight for the instruction cache
 __device__ __noinline__ inline void nt_timeout(const char* what) {
   printf("neutts_b200: timed out waiting for %s (block %d,%d thread %d)\n", what, blockIdx.x, blockIdx.y, threadIdx.x);
   __trap();
 }
+#endif
 NT_DEVINL void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
@@ -112,7 +120,7 @@ NT_DEVINL void tma_load_2d(void* smem_dst, const CUtensorMap* m, int c0, int c1,
 }
 
 // Same with an L2 eviction-priority hint (createpolicy): weights that stream through once per decode step are loaded
-// evict_first so that they do not push the small hot set (KV pages, hand-off buffers, logits) out of the 126 MB L2.
+// evict_first so that they do not push the small hot set (KV pages, hand-off buffers, logits) out of the 50 MB L2.
 NT_DEVINL uint64_t l2_policy_evict_first() {
   uint64_t pol;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
@@ -126,77 +134,44 @@ NT_DEVINL void tma_load_2d_hint(void* smem_dst, const CUtensorMap* m, int c0, in
       : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-NT_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-NT_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// Whole warp.  Writes the TMEM base address to *smem_slot.  ncols: power of two in [32, 512].
-NT_DEVINL void tmem_alloc(uint32_t* smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-NT_DEVINL void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
+// ---------------------------------------------------------------- wgmma (warpgroup MMA)
 // K-major operand tile in shared memory written by TMA with CU_TENSOR_MAP_SWIZZLE_128B:
-// rows of 128 bytes, 8-row groups 1024 bytes apart (SBO), descriptor version 1 (sm_100),
-// layout type 2 (SWIZZLE_128B).  Field layout follows the UMMA shared-memory descriptor
-// (start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version [46,48), layout [61,64)).
-NT_DEVINL uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// rows of 128 bytes, 8-row groups 1024 bytes apart (SBO), layout type 1 (SWIZZLE_128B).
+// Field layout of the sm_90 wgmma matrix descriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46),
+// base offset [49,52) (0: tiles are 1024-byte aligned), layout [62,64).  Adding 2 to the descriptor advances the
+// start by 32 bytes = one K step of a bf16 (16) or tf32 (8) instruction; adding 512 advances by 64 rows.
+NT_DEVINL uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;            // LBO (ignored for swizzled K-major), canonical value 1
   d |= static_cast<uint64_t>(1024 >> 4) << 32;    // SBO = 1024 B between 8-row core groups
-  d |= static_cast<uint64_t>(1) << 46;            // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;            // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;            // SWIZZLE_128B
   return d;
 }
-
-// Instruction descriptor for kind::f16 / kind::tf32, fp32 accumulate, both operands K-major.
-// fmt: 0 = f16, 1 = bf16, 2 = tf32.
-__host__ __device__ constexpr uint32_t umma_idesc(int fmt, int M, int N) {
-  return (1u << 4)                      // C format = F32
-         | (uint32_t(fmt) << 7)         // A format
-         | (uint32_t(fmt) << 10)        // B format
-         | (0u << 15) | (0u << 16)      // A, B K-major
-         | (uint32_t(N >> 3) << 17)     // N / 8
-         | (uint32_t(M >> 4) << 24);    // M / 16
+// Register fence before the first wgmma that reads accumulators this thread wrote (or a new batch of MMAs).
+NT_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+NT_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// Wait until at most N committed groups of this warp are pending: their shared-memory operands may then be reused.
+template <int N>
+NT_DEVINL void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Keep the compiler from moving accumulator reads / writes across an asynchronous wgmma.
+template <int R>
+NT_DEVINL void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i]) : : "memory");
 }
-
-NT_DEVINL void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// Accumulator fragments of one warp (rows [16 w, 16 w + 16) of a 64-row wgmma tile, see wgmma.cuh) -> fp32 rows in
+// shared memory: dst[row * ld + col], rows offset by row0.
+template <int N>
+NT_DEVINL void wgmma_store_rows(const float (&d)[N / 2], float* dst, int ld, int row0) {
+  const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+  const int r = row0 + 16 * w + (l >> 2), c = 2 * (l & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    *reinterpret_cast<float2*>(dst + static_cast<long long>(r) * ld + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(dst + static_cast<long long>(r + 8) * ld + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
 }
-NT_DEVINL void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-NT_DEVINL void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns.
-NT_DEVINL void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-NT_DEVINL void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ---------------------------------------------------------------- math / conversion
 NT_DEVINL float warp_sum(float v) {

@@ -1,11 +1,12 @@
-// tcgen05 GEMM for sm_100a:  C[M,N] = epilogue(A[M,K] . W[N,K]^T), fp32 accumulation in TMEM.
+// wgmma GEMM for sm_90a:  C[M,N] = epilogue(A[M,K] . W[N,K]^T), fp32 accumulation in registers.
 //
 //   - operands K-major in global memory, tiles of 128 bytes along K (64 bf16 / 32 tf32)
 //     staged by TMA (SWIZZLE_128B) into a multi-stage shared-memory ring;
-//   - one elected thread issues tcgen05.mma (M=128, N=BN, K=16|8 per instruction), the
-//     accumulator tile lives in TMEM (BN fp32 columns x 128 lanes);
-//   - four epilogue warps read TMEM with tcgen05.ld (32 lanes x 32 columns each) and apply
-//     bias / residual / SiLU / SwiGLU before writing fp32 and/or bf16 rows;
+//   - one warpgroup (warps 4..7) issues wgmma.mma_async (two M=64 halves of the 128-row tile, N=BN,
+//     K=16|8 per instruction) and keeps the accumulator tile in registers;
+//   - once the K loop has drained the ring, the accumulators go through shared memory (the ring) so that each
+//     thread owns one output row, and the same four warps apply bias / residual / SiLU / SwiGLU before writing
+//     fp32 and/or bf16 rows;
 //   - Conv1d is the same kernel: the K loop walks (tap, channel-block) and shifts the A row
 //     coordinate by `tap`, so no im2col buffer exists anywhere.
 //
@@ -14,6 +15,7 @@
 // layers (SURVEY.md §8a rows A2, A4, A8-A10, B2-B6).
 #include <cstdlib>
 
+#define NT_WGMMA_KERNELS
 #include "common.cuh"
 #include "internal.h"
 
@@ -36,12 +38,11 @@ struct GemmEpilogue {
                            //   tile-max sampler); plain fp32 epilogue only
 };
 
-// kShallow: half-depth ring (<= 113 KB) so two CTAs share an SM -- used when the grid is between one and two
-// waves of single-occupancy CTAs (e.g. gate/up at batched decode: 152 tiles on 148 SMs would take two rounds).
+// kShallow: half-depth ring (<= 113 KB of shared memory) for grids of more than one wave of CTAs.
 // kS3 (tf32 only): 3xTF32 in ONE pass.  Both operands arrive as hi/lo halves (hi = the value rounded to TF32, lo = the
 // exact remainder), the lo half stored `*_lo_rows` rows below the hi half in the same matrix, so one tensor map per
 // operand serves both; a stage holds A_hi | A_lo | W_hi | W_lo and every k-block issues A_lo.W_hi, A_hi.W_lo, A_hi.W_hi
-// into the same TMEM accumulator: fp32-grade products on the TF32 pipe without intermediate round trips to HBM.
+// into the same accumulators: fp32-grade products on the TF32 pipe without intermediate round trips to HBM.
 template <int BN, bool kShallow = false, bool kS3 = false>
 struct GemmCfg {
   static constexpr int BM = 128;
@@ -51,6 +52,8 @@ struct GemmCfg {
   static constexpr int STAGES = kS3 ? (BN == 128 ? 3 : (BN == 64 ? 4 : 5))
                                     : (kShallow ? (BN <= 64 ? 4 : 3) : ((BN <= 64) ? 8 : (BN == 128 ? 6 : 4)));
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int OUT_LD = BN + 4;   // fp32 row stride of the accumulator tile staged in the drained ring
+  static_assert(BM * OUT_LD * 4 <= STAGES * STAGE_BYTES, "accumulator staging must fit the ring");
 };
 
 template <int kFmt, int BN, bool kShallow, bool kS3 = false>
@@ -69,9 +72,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint64_t* bars = reinterpret_cast<uint64_t*>(tiles + STAGES * Cfg::STAGE_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* acc_bar = bars + 2 * STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 1);
-
   const int warp = uniform(warp_id());   // provably warp-uniform: role branches below stay convergent (elect_one())
   const int lane = lane_id();
   const int n0 = blockIdx.x * BN;
@@ -87,16 +87,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 4);   // one arrival per MMA warp
     }
-    mbar_init(acc_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // Programmatic dependent launch: let the next kernel's CTAs start their prologue now (they block in their own
   // griddepcontrol.wait until this grid has completed), and start streaming this kernel's weights -- which no
@@ -119,8 +114,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
   pdl_wait();  // inputs (A, residual) may come from the previous kernel in the stream
 
-  // Producer and MMA warps: warp-uniform loops, the TMA / tcgen05 instructions under the elect.sync predicate (see
-  // elect_one() in common.cuh: behind `if (lane == 0)` every UTCHMMA costs ~160 cycles of issue overhead).
+  // Producer warp: warp-uniform loop, the TMA instructions under the elect.sync predicate (see elect_one() in
+  // common.cuh).
   if (warp == 0) {
     // ------------------------------------------------------------ TMA producer
     for (int kb = kb_lo; kb < kb_hi; ++kb) {
@@ -142,62 +137,78 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = umma_idesc(kFmt, 128, BN);
+  } else if (warp >= 4) {
+    // ------------------------------------------------------------ MMA warpgroup + epilogue
+    // acc0 = rows [0, 64) of the tile, acc1 = rows [64, 128); one k-block's MMAs form a commit group, and the ring
+    // slot of a k-block is released once the next group has been issued and the older one retired.
+    float acc0[BN / 2], acc1[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i] = 0.f;
     const uint32_t tiles_addr = smem_u32(tiles);
+    auto mma = [&](uint64_t ad, uint64_t bd) {
+      if constexpr (kFmt == 2) {
+        wgmma_tf32<BN>(acc0, ad, bd, 1u);
+        wgmma_tf32<BN>(acc1, ad + 512, bd, 1u);
+      } else {
+        wgmma_bf16<BN>(acc0, ad, bd, 1u);
+        wgmma_bf16<BN>(acc1, ad + 512, bd, 1u);
+      }
+    };
+    int prev = -1;
     for (int kb = kb_lo; kb < kb_hi; ++kb) {
       const int s = (kb - kb_lo) % STAGES;
       const uint32_t ph = ((kb - kb_lo) / STAGES) & 1;
       mbar_wait(&full_bar[s], ph);
-      tc_fence_after();
-      if (elect_one()) {   // same lane every time (all 32 present): tcgen05.commit tracks the issuing thread's MMAs
-        const uint32_t sa = tiles_addr + static_cast<uint32_t>(s) * Cfg::STAGE_BYTES;
-        const uint32_t sb = sa + W_OFF;
-        const uint64_t adesc = umma_desc_sw128(sa);
-        const uint64_t bdesc = umma_desc_sw128(sb);
-        if (kS3) {   // small terms first: A_lo.W_hi, A_hi.W_lo, then A_hi.W_hi
-          const uint64_t alo = umma_desc_sw128(sa + Cfg::A_BYTES), blo = umma_desc_sw128(sb + Cfg::B_BYTES);
+      const uint32_t sa = tiles_addr + static_cast<uint32_t>(s) * Cfg::STAGE_BYTES;
+      const uint32_t sb = sa + W_OFF;
+      const uint64_t adesc = wgmma_desc_sw128(sa);
+      const uint64_t bdesc = wgmma_desc_sw128(sb);
+      wgmma_fence();
+      if (kS3) {   // small terms first: A_lo.W_hi, A_hi.W_lo, then A_hi.W_hi
+        const uint64_t alo = wgmma_desc_sw128(sa + Cfg::A_BYTES), blo = wgmma_desc_sw128(sb + Cfg::B_BYTES);
 #pragma unroll
-          for (int k = 0; k < 4; ++k) umma_tf32(tmem_base, alo + 2 * k, bdesc + 2 * k, idesc, (kb > kb_lo || k > 0) ? 1u : 0u);
+        for (int k = 0; k < 4; ++k) mma(alo + 2 * k, bdesc + 2 * k);
 #pragma unroll
-          for (int k = 0; k < 4; ++k) umma_tf32(tmem_base, adesc + 2 * k, blo + 2 * k, idesc, 1u);
+        for (int k = 0; k < 4; ++k) mma(adesc + 2 * k, blo + 2 * k);
 #pragma unroll
-          for (int k = 0; k < 4; ++k) umma_tf32(tmem_base, adesc + 2 * k, bdesc + 2 * k, idesc, 1u);
-        } else {
+        for (int k = 0; k < 4; ++k) mma(adesc + 2 * k, bdesc + 2 * k);
+      } else {
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {  // 4 x 32 bytes of K per stage
-            const uint32_t acc = (kb > kb_lo || k > 0) ? 1u : 0u;
-            if (kFmt == 2)
-              umma_tf32(tmem_base, adesc + 2 * k, bdesc + 2 * k, idesc, acc);
-            else
-              umma_bf16(tmem_base, adesc + 2 * k, bdesc + 2 * k, idesc, acc);
-          }
-        }
-        umma_commit(&empty_bar[s]);  // frees the smem slot when these MMAs retire
+        for (int k = 0; k < 4; ++k) mma(adesc + 2 * k, bdesc + 2 * k);  // 4 x 32 bytes of K per stage
       }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);   // frees the smem slot of the previous k-block
+      }
+      prev = s;
     }
-    if (elect_one()) umma_commit(acc_bar);  // accumulator complete
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------ epilogue
-    const int q = warp - 4;  // TMEM lane quarter (== warp % 4)
-    mbar_wait(acc_bar, 0);
-    tc_fence_after();
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc0);
+    wgmma_fence_regs(acc1);
+    // every TMA load of this CTA has been consumed: the ring is free to hold the fp32 tile [128][OUT_LD]
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    float* stage = reinterpret_cast<float*>(tiles);
+    wgmma_store_rows<BN>(acc0, stage, Cfg::OUT_LD, 0);
+    wgmma_store_rows<BN>(acc1, stage, Cfg::OUT_LD, 64);
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    const int q = warp - 4;  // rows [32 q, 32 q + 32) of the tile, one per lane
+    const float* srow = stage + (q * 32 + lane) * Cfg::OUT_LD;
     const int row = m0 + q * 32 + lane;
     bool row_ok = row < M;
     if (ep.valid_period > 0 && (row % ep.valid_period) >= ep.valid_len) row_ok = false;
-    const uint32_t trow = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
     float tmx = -INFINITY;
 #pragma unroll 1
     for (int c = 0; c < BN / 32; ++c) {
-      uint32_t raw[32];
-      tmem_ld32(trow + c * 32, raw);
-      tmem_ld_wait();
       const int col0 = n0 + c * 32;
       if (!row_ok || col0 >= N) continue;
       float v[32];
 #pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(raw[j]);
+      for (int j = 0; j < 8; ++j) {
+        const float4 t = reinterpret_cast<const float4*>(srow + c * 32)[j];
+        v[4 * j] = t.x, v[4 * j + 1] = t.y, v[4 * j + 2] = t.z, v[4 * j + 3] = t.w;
+      }
       const bool full = (col0 + 32 <= N);
       if (ep.split_k > 1) {
         float* dst = ep.out_f32 + blockIdx.z * ep.split_stride + row * ep.ldc + col0;
@@ -295,9 +306,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
     if (ep.tile_max && row_ok) ep.tile_max[static_cast<long long>(row) * gridDim.x + blockIdx.x] = tmx;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, BN);
 }
 
 // ------------------------------------------------------------------------------------------ host side
@@ -352,7 +360,7 @@ static int num_sms() {
   if (!n) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
 }
@@ -361,8 +369,8 @@ static int num_sms() {
 int gemm_tile_n(int M, int N, bool swiglu) {
   const int mt = (M + 127) / 128;
   int bn = 128;
-  if (mt * ((N + 127) / 128) < 120) bn = 64;
-  if (mt * ((N + 63) / 64) < 100) bn = 32;
+  if (mt * ((N + 127) / 128) < num_sms() * 13 / 16) bn = 64;
+  if (mt * ((N + 63) / 64) < num_sms() * 11 / 16) bn = 32;
   if (swiglu && bn < 64) bn = 64;
   return bn;
 }
@@ -432,7 +440,7 @@ int gemm_dispatch(const nt_gemm_args& a, cudaStream_t stream, SplitK* split, boo
     const bool in_place = a.residual == a.out_f32 && a.ldr == a.ldc;
     if (tiles <= 48 && taps == 1 && a.act == NT_ACT_NONE && !a.out_bf16 && a.out_f32 && (in_place || !a.residual) &&
         a.valid_period == 0 && num_kb >= 8) {
-      int sk = 144 / tiles;
+      int sk = (num_sms() - 4) / tiles;
       if (sk > num_kb / 4) sk = num_kb / 4;
       if (sk > 8) sk = 8;
       const size_t slice = size_t(a.M) * size_t(a.ldc);
@@ -446,9 +454,8 @@ int gemm_dispatch(const nt_gemm_args& a, cudaStream_t stream, SplitK* split, boo
 
   const int ctas = mt * ((a.N + bn - 1) / bn) * (ep.split_k > 1 ? ep.split_k : 1);
   // Two CTAs per SM (half-depth ring) for every grid of more than one wave: one CTA's prologue / epilogue overlaps
-  // the other's main loop, and grids just over a multiple of the SM count lose their short last wave.  Measured at
-  // batch 64: prefill 63 -> 45 ms, codec 36.8 -> 28.8 ms.  NT_GEMM_DEEP_RINGS=1 restores one deep-ring CTA per SM
-  // for grids beyond two waves with several row tiles.
+  // the other's main loop, and grids just over a multiple of the SM count lose their short last wave.
+  // NT_GEMM_DEEP_RINGS=1 restores one deep-ring CTA per SM for grids beyond two waves with several row tiles.
   static const bool deep_rings = [] {
     const char* e = getenv("NT_GEMM_DEEP_RINGS");
     return e && e[0] && e[0] != '0';

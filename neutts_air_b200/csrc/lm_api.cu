@@ -32,7 +32,7 @@ static bool env_flag(const char* name) {
   const char* v = getenv(name);
   return v && v[0] && v[0] != '0';
 }
-// largest batch the per-op GEMV chain takes when the megakernel is off (above it: tcgen05 GEMM chain with M = batch)
+// largest batch the per-op GEMV chain takes when the megakernel is off (above it: tensor-core GEMM chain with M = batch)
 static int gemv_max_batch() {
   const char* e = getenv("NT_GEMV_MAX_BATCH");
   const int n = e ? atoi(e) : 4;
@@ -85,7 +85,7 @@ bool pdl_disabled() {
   return off;
 }
 
-// launch-latency probe: a chain of dependent trivial kernels (profiles/probe_launch.py)
+// launch-latency probe: a chain of dependent trivial kernels
 __global__ void noop_chain_kernel(int* p) {
   pdl_launch_dependents();
   pdl_wait();
@@ -123,9 +123,9 @@ struct nt_lm {
   uint64_t graph_kernels = 0;         // kernel nodes in the captured step (for nt_launch_count)
   bool prefilled = false;
   int debug_layers = -1;              // >= 0: run only this many layers (per-stage parity tests)
-  long long* prof = nullptr;          // megakernel timeline buffer (profiles/probe_mega.py)
+  long long* prof = nullptr;          // megakernel timeline buffer
   int prof_step = 0;
-  // persistent tcgen05 decode kernel (lm_decode_tc.cu): plan, tensor maps and buffers live in the workspace
+  // persistent wgmma decode kernel (lm_decode_tc.cu): plan, tensor maps and buffers live in the workspace
   bool tc_ok = false, tc_flat_ok = false;
   TcPlanInfo tc_info[2] = {};         // [0]: whole-K gate/up plan (any batch), [1]: flat plan (batch <= 4)
   int tc_rows = 0;
@@ -257,9 +257,9 @@ extern "C" int nt_lm_create(const nt_lm_config* cfg, const nt_lm_weights* w, voi
     delete lm;
     return set_error(NT_ERR_CUDA, "no CUDA device: this library has no CPU fallback");
   }
-  if (prop.major != 10) {
+  if (prop.major != 9 || prop.minor != 0) {
     delete lm;
-    return set_error(NT_ERR_CUDA, "device is sm_%d%d; this library is built for sm_100a only", prop.major, prop.minor);
+    return set_error(NT_ERR_CUDA, "device is sm_%d%d; this library is built for sm_90a only", prop.major, prop.minor);
   }
   lm->num_sms = prop.multiProcessorCount;
   // rotary inverse frequencies (modeling_qwen2.py:95-100), iota, zeroed split counters
@@ -294,8 +294,8 @@ extern "C" int nt_lm_create(const nt_lm_config* cfg, const nt_lm_weights* w, voi
     }
   }
   {
-    // persistent tcgen05 decode kernel: work plan + every tensor map, built once (VERDICT r1 item 6: maps were
-    // re-encoded on every GEMM call).  A shape the plan cannot take leaves tc_ok false -> older decode paths.
+    // persistent wgmma decode kernel: work plan + every tensor map, built once (re-encoding the maps on every GEMM
+    // call costs host time on each step).  A shape the plan cannot take leaves tc_ok false -> older decode paths.
     std::vector<TcPlan> plan(512);
     std::vector<unsigned char> nsl(4096, 0);
     TcShape ts{c.hidden, c.inter, c.n_heads, c.n_kv_heads, lm->qkv_n, c.vocab_size};
@@ -615,11 +615,11 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
   if (n_steps < 0) return set_error(NT_ERR_INVALID, "negative step count");
 
   if (n_steps == 0) return NT_OK;
-  // NT_DECODE_IMPL = tc (default: persistent tcgen05 kernel, every batch size) | mega | perop (round-1 paths, kept
-  // for A/B measurements and as the fallback for shapes the tcgen05 plan does not take)
+  // NT_DECODE_IMPL = tc (default: persistent wgmma kernel, every batch size) | mega | perop (older paths, kept
+  // for A/B measurements and as the fallback for shapes the persistent kernel's plan does not take)
   const char* impl = getenv("NT_DECODE_IMPL");
-  // default: the tcgen05 kernel up to NT_TC_MAX_BATCH sequences (measured on B200, ms / step: 0.72 / 0.83 / 0.90 / 1.03
-  // at batch 1 / 4 / 8 / 16, then 1.35 / 2.04 at 32 / 64, where the per-op chain's 1.25 - 1.31 ms (flat in the batch) wins)
+  // default: the persistent kernel up to NT_TC_MAX_BATCH sequences; its step time grows with the batch while the
+  // per-op chain's is nearly flat, so the chain takes the larger batches
   int tc_cap = 16;
   if (const char* e = getenv("NT_TC_MAX_BATCH")) tc_cap = atoi(e);
   const bool want_tc = (impl && impl[0] == 't') || ((!impl || !impl[0]) && B <= tc_cap);

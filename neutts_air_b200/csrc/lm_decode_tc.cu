@@ -1,15 +1,16 @@
-// Persistent tcgen05 decode kernel: ALL layers, the lm_head, the sampler and the whole multi-step decode loop in
+// Persistent wgmma decode kernel: ALL layers, the lm_head, the sampler and the whole multi-step decode loop in
 // ONE cooperative launch of one CTA per SM, for every batch size 1..64.
 //
-//   GEMM phases (qkv | o_proj | gate/up | down | lm_head) run on the 5th-generation tensor cores:
+//   GEMM phases (qkv | o_proj | gate/up | down | lm_head) run on the tensor cores (warpgroup MMA):
 //     * A operand = WEIGHTS, exactly as they lie in HBM (K-major): 128 rows x 64 k tiles (16 KB) fetched by 2-D TMA
 //       (SWIZZLE_128B) through per-matrix tensor maps built once at nt_lm_create; one warp streams this CTA's tiles
 //       of the WHOLE step into a deep mbarrier ring and runs ahead across phase boundaries (weights are immutable);
-//     * B operand = ACTIVATIONS, K-major [tokens x 64 k] chunks in shared memory: tokens sit on the UMMA N axis
+//     * B operand = ACTIVATIONS, K-major [tokens x 64 k] chunks in shared memory: tokens sit on the MMA N axis
 //       (N = 16 | 32 | 64).  Batch <= 8 feeds every activation as a bf16 hi + lo pair on two N columns (~16 mantissa
 //       bits, the decode path keeps fp32-grade activations); larger batches use plain bf16 like the prefill path;
-//     * accumulators in TMEM (128 lanes = weight rows, N fp32 columns), double-buffered: one elected thread issues
-//       tcgen05.mma, four epilogue warps tcgen05.ld their 32 lanes and run the fused epilogues.
+//     * one MMA warpgroup issues wgmma (two M = 64 halves of the 128-row tile) with the accumulators in registers,
+//       then hands each finished tile [128 weight rows x N] to the four epilogue warps through shared memory (one
+//       fp32 row per epilogue lane) while it already accumulates the next item.
 //   Work split: every weight matrix is cut into (128-row tile, K slice) items spread over the CTAs so that each
 //   SM streams the same number of bytes per layer; matrices with few row tiles (qkv 9, o 7, down 7) split K and
 //   write raw partial sums, folded IN SLICE ORDER by their consumer (bit-reproducible, no atomics).  gate/up keeps
@@ -26,6 +27,7 @@
 //
 // Replaces transformers generation/utils.py:2743-2805 + modeling_qwen2.py:280-309,353-413 for the decode loop
 // (SURVEY.md §8a rows A1, A3-A12); supersedes the CUDA-core megakernel (lm_mega.cu) and the 196-launch chain.
+#define NT_WGMMA_KERNELS
 #include "lm_device.cuh"
 #include "lm_decode_tc.cuh"
 
@@ -47,15 +49,6 @@ NT_DEVINL long long tc_ns() {
   long long t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
-}
-NT_DEVINL void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
 }
 // (value, stamp) pairs: relaxed gpu-scope loads (served by L2, never by a stale L1 line)
 NT_DEVINL float4 ldp2(const float2* p) {
@@ -149,10 +142,9 @@ struct TcMisc {
   uint64_t full_bar[16];
   uint64_t empty_bar[16];
   uint64_t bop_bar;
-  uint64_t acc_full[2];
-  uint64_t acc_empty[2];
+  uint64_t acc_full;      // the accumulator tile in shared memory is written (MMA warpgroup -> epilogue warps)
+  uint64_t acc_empty;     // ... and has been read
   uint64_t att_bar[kAttWarpsMax];
-  uint32_t tmem_slot;
   uint64_t go_bar;        // step gate of the stream / MMA warps: one completion per released decode step
   int stop;               // set before the last completion: leave instead of running the step
   int pos[kTcMaxBatch];   // this step's seq_lens snapshot
@@ -180,16 +172,13 @@ template <int NT, bool HILO, bool FOLD>
 __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_constant__ TcParams P) {
   constexpr int CHUNK = NT * 128;            // bytes of one B-operand k-block
   constexpr int NTOK = HILO ? 8 : NT;        // token slots on the N axis
-  // MMAs into one accumulator tile form a dependent chain (~150 cycles each at N = 16): the four 16-wide k-steps of
-  // a k-block go to NACC independent TMEM tiles instead, summed by the epilogue (fixed order).
-  constexpr int NACC = NT == 16 ? 4 : (NT == 32 ? 2 : 1);
-  constexpr int ACOLS = NACC * NT;           // TMEM columns of one accumulator buffer
-  constexpr int TMEM_COLS = 2 * ACOLS < 32 ? 32 : 2 * ACOLS;
+  constexpr int ACC_LD = NT + 4;             // fp32 row stride of the accumulator tile in shared memory
   extern __shared__ uint8_t tc_smem_raw[];
   uint8_t* smem = tc_smem_raw + ((1024u - (smem_u32(tc_smem_raw) & 1023u)) & 1023u);
   uint8_t* ring = smem;
   uint8_t* uni = smem + P.uni_off;
   TcMisc* ms = reinterpret_cast<TcMisc*>(smem + P.misc_off);
+  float* accs = reinterpret_cast<float*>(smem + P.acc_off);   // [128][ACC_LD]
   const int tid = threadIdx.x, warp = uniform(tid >> 5), lane = tid & 31;
   const int NS = P.nstages;
   const int L = P.n_layers;
@@ -203,13 +192,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
   if (tid == 0) {
     for (int s = 0; s < NS; ++s) {
       mbar_init(&ms->full_bar[s], 1);
-      mbar_init(&ms->empty_bar[s], 1);
+      mbar_init(&ms->empty_bar[s], 4);   // one arrival per MMA warp
     }
     mbar_init(&ms->bop_bar, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&ms->acc_full[i], 1);
-      mbar_init(&ms->acc_empty[i], 4);
-    }
+    mbar_init(&ms->acc_full, 4);         // the four MMA warps
+    mbar_init(&ms->acc_empty, 4);        // the four epilogue warps
     for (int i = 0; i < kAttWarpsMax; ++i) mbar_init(&ms->att_bar[i], 1);
     mbar_init(&ms->go_bar, 1);
     fence_barrier_init();
@@ -218,11 +205,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
   }
   for (int i = tid; i < static_cast<int>(sizeof(TcPlan) / 4); i += kTcThreads)
     reinterpret_cast<int*>(&ms->plan)[i] = reinterpret_cast<const int*>(P.plan + blockIdx.x)[i];
-  if (warp == 9) tmem_alloc(&ms->tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = ms->tmem_slot;
   const TcPlan& plan = ms->plan;
   if (tid < 4) {  // chunk tables of the split phases (items in plan order, k-blocks ascending)
     int c = 0;
@@ -239,7 +222,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     mbar_wait(&ms->go_bar, static_cast<uint32_t>(step) & 1u);
     return *reinterpret_cast<volatile int*>(&ms->stop) == 0;
   };
-  if (warp == 8) {
+  if (warp == kTcStreamWarp) {
     // ================================================================== weight stream
     // The whole warp walks the plan (warp-uniform control flow); one elected lane issues the copies.  elect.sync is
     // re-executed at every use: it is also the point where the lanes RECONVERGE after a data-dependent wait loop --
@@ -275,13 +258,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
       for (int t = t0; t < t1; ++t)
         for (int kb = 0; kb < KBH; ++kb) push(hm, kb * 64, t * 128);
     }
-  } else if (warp == 9) {
-    // ================================================================== MMA issuer
-    // Warp-uniform control flow, tcgen05.mma / commit under the elect.sync predicate: this is what lets the compiler
-    // keep descriptors in uniform registers and issue the MMAs back to back (see elect_one() in common.cuh); elect.sync
-    // after every wait (reconvergence, see the stream warp).  With all 32 lanes present it names the same lane every
-    // time, which tcgen05.commit needs (it tracks the MMAs of the issuing thread).
-    constexpr uint32_t idesc = umma_idesc(1, 128, NT);
+  } else if (warp >= kTcMmaWarp0) {
+    // ================================================================== MMA warpgroup (warps kTcMmaWarp0 .. + 3)
+    // acc0 = weight rows [0, 64) of the tile, acc1 = rows [64, 128).  One k-block's MMAs form a commit group; a ring
+    // slot is released (one arrival per warp) once the next group has been issued and the older one retired.
     int slot = 0;
     uint32_t par = 0;
     uint32_t bop_n = 0, acc_n = 0;
@@ -289,24 +269,39 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     const uint32_t ring_addr = smem_u32(ring);
     // one item: nkb ring tiles against B chunks chunk0, chunk0 + 1, ...
     auto run_item = [&](int nkb, int chunk0) {
-      const uint32_t buf = acc_n & 1;
-      mbar_wait(&ms->acc_empty[buf], ((acc_n >> 1) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t dst = tmem_base + buf * ACOLS;
+      float acc0[NT / 2], acc1[NT / 2];
+#pragma unroll
+      for (int i = 0; i < NT / 2; ++i) acc0[i] = acc1[i] = 0.f;
+      int prev = -1;
       for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(&ms->full_bar[slot], par);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t adesc = umma_desc_sw128(ring_addr + static_cast<uint32_t>(slot) * 16384u);
-          const uint64_t bdesc = umma_desc_sw128(bop_addr + static_cast<uint32_t>(chunk0 + kb) * CHUNK);
+        const uint64_t adesc = wgmma_desc_sw128(ring_addr + static_cast<uint32_t>(slot) * 16384u);
+        const uint64_t bdesc = wgmma_desc_sw128(bop_addr + static_cast<uint32_t>(chunk0 + kb) * CHUNK);
+        wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16(dst + (k % NACC) * NT, adesc + 2 * k, bdesc + 2 * k, idesc, (kb > 0 || k >= NACC) ? 1u : 0u);
-          umma_commit(&ms->empty_bar[slot]);
+        for (int k = 0; k < 4; ++k) {
+          wgmma_bf16<NT>(acc0, adesc + 2 * k, bdesc + 2 * k, 1u);
+          wgmma_bf16<NT>(acc1, adesc + 512 + 2 * k, bdesc + 2 * k, 1u);
         }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&ms->empty_bar[prev]);
+        }
+        prev = slot;
         if (++slot == NS) slot = 0, par ^= 1;
       }
-      if (elect_one()) umma_commit(&ms->acc_full[buf]);
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc0);
+      wgmma_fence_regs(acc1);
+      __syncwarp();
+      if (prev >= 0 && lane == 0) mbar_arrive(&ms->empty_bar[prev]);
+      mbar_wait(&ms->acc_empty, (acc_n & 1) ^ 1);
+      wgmma_store_rows<NT>(acc0, accs, ACC_LD, 0);
+      wgmma_store_rows<NT>(acc1, accs, ACC_LD, 64);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&ms->acc_full);
       ++acc_n;
     };
     const int gu_split = uniform(plan.gu_split);
@@ -319,7 +314,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
           if (n_it == 0) continue;
           mbar_wait(&ms->bop_bar, bop_n & 1);
           ++bop_n;
-          tc_fence_after();
           int chunk = 0;
           for (int i = 0; i < n_it; ++i) {
             const int nkb = uniform(plan.it[ph][i].nkb);
@@ -334,7 +328,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
       if (n_head > 0) {
         mbar_wait(&ms->bop_bar, bop_n & 1);
         ++bop_n;
-        tc_fence_after();
         for (int t = 0; t < n_head; ++t) run_item(KBH, 0);
       }
     }
@@ -415,38 +408,15 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
 
     // ---- accumulator of the next item -> registers (epilogue warps 0..3; lane = weight row of the tile)
     auto acc_take = [&](float (&v)[NT]) {
-      const uint32_t buf = acc_n & 1;
-      mbar_wait(&ms->acc_full[buf], (acc_n >> 1) & 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + buf * ACOLS;
-      if constexpr (NT == 16) {   // 4 sub-accumulators of 16 columns
-        uint32_t r0[32], r1[32];
-        tmem_ld32(taddr, r0);
-        tmem_ld32(taddr + 32, r1);
-        tmem_ld_wait();
+      mbar_wait(&ms->acc_full, acc_n & 1);
+      const float4* src = reinterpret_cast<const float4*>(accs + (warp * 32 + lane) * ACC_LD);
 #pragma unroll
-        for (int j = 0; j < 16; ++j)
-          v[j] = (__uint_as_float(r0[j]) + __uint_as_float(r0[16 + j])) + (__uint_as_float(r1[j]) + __uint_as_float(r1[16 + j]));
-      } else if constexpr (NT == 32) {   // 2 sub-accumulators of 32 columns
-        uint32_t r0[32], r1[32];
-        tmem_ld32(taddr, r0);
-        tmem_ld32(taddr + 32, r1);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r0[j]) + __uint_as_float(r1[j]);
-      } else {
-#pragma unroll
-        for (int c = 0; c < NT / 32; ++c) {
-          uint32_t r[32];
-          tmem_ld32(taddr + c * 32, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[c * 32 + j] = __uint_as_float(r[j]);
-        }
+      for (int j = 0; j < NT / 4; ++j) {
+        const float4 t = src[j];
+        v[4 * j] = t.x, v[4 * j + 1] = t.y, v[4 * j + 2] = t.z, v[4 * j + 3] = t.w;
       }
-      tc_fence_before();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&ms->acc_empty[buf]);
+      if (lane == 0) mbar_arrive(&ms->acc_empty);
       ++acc_n;
       if constexpr (HILO) {
 #pragma unroll
@@ -809,7 +779,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     };
 
     // ---- o_proj input: merge the split-KV partials of the heads this CTA's items need, straight into B chunks
+    // The B chunks of the previous GEMM phase are free once the epilogue warps have taken its last accumulator: the MMA
+    // warpgroup has then retired every wgmma that reads them.  Warps 4..7 skip the epilogue (and a CTA without an
+    // attention split skips the attention barriers), so the staging below starts with a consumer barrier.
     auto stage_attn = [&](int stamp) {
+      csync();
       const int nch = ms->nchunks[kPhO];
       const int per = B * 64;
       for (int e = tid; e < nch * per; e += kConsumerThreads) {
@@ -864,6 +838,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
 
     // ---- batch <= 4: down_proj input from the (value, stamp) SwiGLU outputs, two elements per thread
     auto stage_act = [&](int stamp) {
+      csync();   // the B chunks of the gate/up phase are free (see stage_attn)
       const int nch = ms->nchunks[kPhD];
       const int per = B * 32;
       for (int e = tid; e < nch * per; e += kConsumerThreads) {
@@ -1138,9 +1113,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
       mbar_arrive(&ms->go_bar);
     }
   }
-  tc_fence_before();
   __syncthreads();
-  if (warp == 9) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 // ------------------------------------------------------------------------------------------ host side
@@ -1151,8 +1124,8 @@ static size_t tc_chunk_bytes(int nt) {   // B chunks (+ fold_in_cta: fp32 rows a
 static size_t tc_attn_bytes(int aw) { return (tc_attn_layout_bytes(aw) + 1023) & ~size_t(1023); }
 
 bool tc_fold_in_cta(int B, int hidden) {
-  // Measured on B200 (us / step, NeuTTS-Air): in-CTA fold 719 / 916 / 1111 / 1283 at batch 1 / 2 / 3 / 4, fold phases
-  // 806 / 805 / 826 / 830: every consumer re-folding ALL rows stops paying at two sequences.
+  // Every consumer re-folds ALL rows in the in-CTA fold, so its cost grows with the batch while the fold phases' is
+  // flat: the in-CTA fold is the default at batch 1 only.
   // NT_TC_FOLD: "phase" forces the fold phases at batch 1, "cta" the in-CTA fold up to batch 4 (experiments).
   const char* fe = getenv("NT_TC_FOLD");
   const int cap = (fe && fe[0] == 'c') ? 4 : 1;
@@ -1265,6 +1238,7 @@ static int launch_tc(TcParams& P, int num_sms, cudaStream_t stream) {
   auto kern = decode_tc_kernel<NT, HILO, FOLD>;
   const size_t budget = 227 * 1024;
   const size_t misc = (sizeof(TcMisc) + 127) & ~size_t(127);
+  const size_t acc = (size_t(128) * (NT + 4) * 4 + 127) & ~size_t(127);   // accumulator tile [128][NT + 4] fp32
   // batch <= 4: the attention staging sits BEHIND the B chunks, so a layer's KV pages are fetched while the qkv
   // projection still runs; otherwise the two alias (a phase uses one or the other)
   const bool separate = P.fold_in_cta != 0 && !getenv("NT_TC_NO_PREFETCH");
@@ -1272,15 +1246,16 @@ static int launch_tc(TcParams& P, int num_sms, cudaStream_t stream) {
   P.att_warps = separate ? 2 : 4;
   const size_t chunks = tc_chunk_bytes(NT), att = tc_attn_bytes(P.att_warps);
   const size_t uni = separate ? chunks + att : (chunks > att ? chunks : att);
-  int ns = int((budget - uni - misc - 1024) / 16384);
+  int ns = int((budget - uni - misc - acc - 1024) / 16384);
   if (ns > 16) ns = 16;
   if (ns < 3) return set_error(NT_ERR_INVALID, "decode_tc: shared memory plan leaves %d ring stages", ns);
-  const size_t smem = size_t(ns) * 16384 + uni + misc + 1024;
+  const size_t smem = size_t(ns) * 16384 + uni + misc + acc + 1024;
   P.nstages = ns;
   P.uni_off = unsigned(size_t(ns) * 16384);
   P.uni_bytes = unsigned(uni);
   P.att_off = P.uni_off + (separate ? unsigned(chunks) : 0u);
   P.misc_off = P.uni_off + P.uni_bytes;
+  P.acc_off = P.misc_off + unsigned(misc);
   NT_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
   int per_sm = 0;
   NT_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kTcThreads, smem));

@@ -1,4 +1,4 @@
-// Parameter block + work plan of the persistent tcgen05 decode kernel (lm_decode_tc.cu): ONE cooperative launch
+// Parameter block + work plan of the persistent wgmma decode kernel (lm_decode_tc.cu): ONE cooperative launch
 // runs every layer, the lm_head, the sampler and the whole multi-step decode loop for batch 1..64.
 #pragma once
 #include <cuda.h>
@@ -8,7 +8,9 @@
 namespace nt {
 
 constexpr int kTcMaxItems = 4;      // work items of one GEMM phase a CTA may own
-constexpr int kTcThreads = 320;     // 8 worker warps + 1 weight-stream warp + 1 MMA warp
+constexpr int kTcMmaWarp0 = 8;      // warps 8..11: the MMA warpgroup (warpgroup-aligned)
+constexpr int kTcStreamWarp = 12;   // the weight-stream warp
+constexpr int kTcThreads = 416;     // 8 worker warps + 1 MMA warpgroup + 1 weight-stream warp
 constexpr int kTcMaxBatch = 64;
 constexpr int kTcMaxSlices = 16;
 constexpr int kTcMaxGuSlices = 4;   // K slices of one gate/up tile in the flat plan (batch <= 4)
@@ -79,7 +81,7 @@ struct TcParams {
   int prof_step;
   // shared-memory plan
   int nstages;
-  unsigned uni_off, uni_bytes, misc_off;
+  unsigned uni_off, uni_bytes, misc_off, acc_off;
   int att_warps;                  // page-walking warps of the attention phase (2 | 4)
   unsigned att_off;               // attention staging: inside the union region (aliased) or behind it (batch <= 4: pages prefetched)
   int fold_in_cta;                // 1: batch <= 4, consumers fold the split-K slices themselves (no fold phases)

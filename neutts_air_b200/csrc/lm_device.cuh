@@ -263,7 +263,7 @@ NT_DEVINL void gemv_consume_stage(const GemvParams& p, const uint8_t* st, const 
   }
 }
 
-// ---- legacy tensor-core path used by both attention kernels (tcgen05 needs 64+ rows of M; these tiles have 7-16)
+// ---- legacy tensor-core path used by both attention kernels (wgmma needs 64 rows of M; these tiles have 7-16)
 NT_DEVINL void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile(
       "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"

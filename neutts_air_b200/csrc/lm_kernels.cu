@@ -1,4 +1,4 @@
-// Speech-LM kernels for sm_100a (SURVEY.md §8a, rows A1-A12).
+// Speech-LM kernels for sm_90a (SURVEY.md §8a, rows A1-A12).
 //
 // Decode (memory-bound, batch <= 4 on CUDA cores):
 //   gemv_kernel        weight rows stream HBM -> shared memory through a cp.async.bulk (TMA
@@ -38,7 +38,7 @@ static GemvSmemPlan gemv_plan(int K, int nb) {
   p.units_per_stage = (p.wpu == 1) ? kConsumerWarps : 1;
   p.stage_bytes = unit_bytes * p.units_per_stage;
   p.nstages = (p.wpu == 1) ? 3 : 4;
-  if (const char* e = getenv("NT_GEMV_STAGES")) {  // experiments (profiles/probe_head_stages.py)
+  if (const char* e = getenv("NT_GEMV_STAGES")) {  // experiments
     const int n = atoi(e);
     if (n >= 2 && n <= 8) p.nstages = n;
   }

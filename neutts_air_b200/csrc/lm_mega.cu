@@ -48,10 +48,8 @@ struct Prof {
 
 // Grid-wide barrier over the consumer warps of all CTAs: one relaxed L2 atomic per CTA on a
 // monotonically growing counter (release fence before it), then thread 0 spins with acquire loads
-// until the counter reaches this barrier's target.  Measured on B200 (profiles/mega_timeline_r1.md):
-// ~0.5 us to publish + ~1.3-2.6 us until the slowest CTA has arrived.  A flag-array variant (one word
-// per CTA, coalesced polling, no atomics) was tried and is 2x slower: 148 pollers hammering the flag
-// lines delay the flag stores themselves.
+// until the counter reaches this barrier's target.  A flag-array variant (one word per CTA, coalesced
+// polling, no atomics) was slower: one poller per SM hammering the flag lines delays the flag stores themselves.
 NT_DEVINL void grid_sync(unsigned* gbar, unsigned& target, unsigned nblocks, Prof& prof) {
   asm volatile("bar.sync 1, 256;" ::: "memory");
   if (threadIdx.x == 0) {

@@ -32,7 +32,7 @@ struct MegaParams {
   int n_steps;
   float* logits_out;  // optional: this group's first row of [n_steps][batch][vocab]
   long long logits_step_stride;  // elements between consecutive steps in logits_out (batch * vocab)
-  long long* prof;    // optional timeline buffer [2 CTAs][kProfMarks] of %globaltimer ns (profiles/probe_mega.py)
+  long long* prof;    // optional timeline buffer [2 CTAs][kProfMarks] of %globaltimer ns
   int prof_step;
   // shared-memory plan and tuning (filled by launch_decode_mega)
   int nstages, stage_bytes;

@@ -113,7 +113,7 @@ class SpeechLM:
     def __init__(self, shape: LMShape, state_dict: dict, device="cuda", max_batch: int = 1, max_ctx: int = 2048,
                  max_new: int | None = None, max_prefill_tokens: int | None = None, page_shuffle_seed: int | None = None):
         if not torch.cuda.is_available():
-            raise RuntimeError("neutts_air_b200.SpeechLM needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("neutts_air_b200.SpeechLM needs a CUDA device (sm_90a); there is no CPU fallback")
         self.L = _lib.lib()
         self.shape = shape
         self.device = torch.device(device)

@@ -60,7 +60,7 @@ def load_speech_lm(repo: str, device="cuda", **kw) -> SpeechLM:
     # Mistral share; q/k/v biases are optional (absent in Llama-style checkpoints -> zeros)
     family = ("Qwen2", "Llama", "Mistral", "Qwen3")
     if not any(f in arch for f in family) and cfg.get("model_type") not in ("qwen2", "llama", "mistral"):
-        raise ValueError(f"unsupported backbone architecture {arch!r}: the B200 kernels implement the "
+        raise ValueError(f"unsupported backbone architecture {arch!r}: the sm_90a kernels implement the "
                          f"Qwen2/Llama-family decoder (RMSNorm, RoPE, GQA, SwiGLU)")
     if cfg.get("rope_scaling") not in (None, {}) and (cfg["rope_scaling"] or {}).get("rope_type", "default") != "default":
         raise ValueError("scaled RoPE variants are not implemented")

@@ -2,7 +2,7 @@
 
 No checkpoint, tokenizer or codec source exists offline (SURVEY.md fact 2), so benchmarks and the
 smoke test run on these.  Plain tensors only: the LM comes out as an HF-named Qwen2 state_dict, the
-codec as the dict layout ``codec.pack_weights`` consumes.  Both arms of bench.py (B200 and the CPU
+codec as the dict layout ``codec.pack_weights`` consumes.  Both arms of bench.py (the GPU and the CPU
 reference) are built from the same tensors.
 """
 from __future__ import annotations

@@ -171,7 +171,7 @@ def forward(cfg: LMConfig, w: LMWeights, ids: torch.Tensor, cache: KVCache | Non
     the kernels can be checked to ~fp32 accuracy against their own specification (it is
     not part of the reference semantics; ``mirror=None`` is the reference):
       "decode"  (CUDA-core GEMV chain): K/V rounded to bf16 when cached, all else fp32;
-      "decode_tc" (persistent tcgen05 decode kernel, batch <= 8): as "decode" (activations travel as bf16 hi + lo
+      "decode_tc" (persistent wgmma decode kernel, batch <= 8): as "decode" (activations travel as bf16 hi + lo
                 pairs, fp32-grade), but attention runs on bf16 tensor-core operands (scaled query, probabilities);
       "prefill" (tensor-core path): additionally the normalised activations, the
                 attention output and the SwiGLU output are rounded to bf16 (GEMM A operands), and

@@ -1,4 +1,4 @@
-"""GPU: the drop-in facade end to end on the B200 engines (synthetic weights, injected tokenizer /
+"""GPU: the drop-in facade end to end on the H100 engines (synthetic weights, injected tokenizer /
 phonemizer): the reference's own smoke assertions (tests/test_neutts.py:55-58), batched inference,
 and streaming with the reference's window geometry."""
 import warnings

@@ -4,7 +4,7 @@ oracle would take minutes per forward.  Parity there is checked through size-ind
   * prefill / decode consistency: the logits after prefill(P) + k teacher-forced decode steps equal the logits at
     the last position of prefill(P + k) — two different kernel families (tensor-core GEMMs + flash attention vs the
     persistent GEMV megakernel with split-KV attention) over the same paged KV cache, RoPE positions and weights;
-  * batch invariance: a sequence decoded alone (megakernel) and inside a batch of 6 (per-op tcgen05 chain) agrees;
+  * batch invariance: a sequence decoded alone (megakernel) and inside a batch of 6 (per-op wgmma chain) agrees;
   * reproducibility: the same seed gives the same sampled tokens twice.
 """
 import pytest

@@ -1,4 +1,4 @@
-"""GPU parity tests of single kernels through the C-ABI (tcgen05 GEMM, RMSNorm, sampler).
+"""GPU parity tests of single kernels through the C-ABI (wgmma GEMM, RMSNorm, sampler).
 
 The comparison target for these float kernels is a plain PyTorch fp32 evaluation of the same
 op on the same (rounded) operands; tolerances are stated next to each assertion."""

@@ -81,7 +81,7 @@ def test_lm_decode_path_tight(cuda, cfgkw, mega, monkeypatch):
     prompt = torch.randint(0, cfg.vocab_size, (1,), generator=g)
     forced = torch.randint(0, cfg.vocab_size, (1, n_new), generator=g)
     got = _teacher_forced(cfg, w, lm, [prompt.tolist()], forced, n_new, eos)[0]
-    # the persistent tcgen05 kernel keeps fp32-grade activations (bf16 hi + lo pairs) but runs the attention products
+    # the persistent wgmma kernel keeps fp32-grade activations (bf16 hi + lo pairs) but runs the attention products
     # on bf16 tensor-core operands like the prefill kernel: mirror "decode_tc"; the per-op chain is all fp32: "decode"
     _, mir = O.generate(cfg, w, prompt, eos, max_length=256, max_new_tokens=n_new, forced=forced[0], mirror=True,
                         decode_mirror="decode_tc" if mega else None)
@@ -109,7 +109,7 @@ def test_lm_ragged_batch_prefill_and_decode(cuda, mega, monkeypatch):
 @pytest.mark.parametrize("B,impl", [(6, None), (10, None), (18, None), (18, "tc"), (34, "tc"), (7, "perop")],
                          ids=["persistent-b6-hilo", "persistent-b10-bf16", "chain-b18", "persistent-b18-n32", "persistent-b34-n64", "chain-b7"])
 def test_lm_batched_decode(cuda, B, impl, monkeypatch):
-    """Batched decode, every kernel variant: the persistent tcgen05 kernel with bf16 hi+lo activations (batch <= 8),
+    """Batched decode, every kernel variant: the persistent wgmma kernel with bf16 hi+lo activations (batch <= 8),
     with plain bf16 activations on N = 16 / 32 / 64 token columns (the default up to batch 16; larger batches forced
     with NT_DECODE_IMPL=tc), and the per-op chain (default from batch 17; forced at batch 7).  Prefill is the
     tensor-core path in every case, so the bar is the pure-reference one."""

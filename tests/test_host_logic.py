@@ -375,25 +375,21 @@ def test_reference_signature_defaults():
                    ("codec_repo", "neuphonic/neucodec"), ("codec_device", "cpu")]
 
 
-REF_EXAMPLE = "/root/reference/examples/basic_example.py"
+BASIC_EXAMPLE_CALLS = os.path.join(os.path.dirname(__file__), "golden", "basic_example_calls.json")
 
 
-@pytest.mark.skipif(not os.path.exists(REF_EXAMPLE), reason="reference checkout not mounted (GPU box)")
-def test_reference_basic_example_runs_unmodified(tmp_path, monkeypatch):
-    """SURVEY §8c golden (4): the reference's examples/basic_example.py, imported as it is, drives THIS repo's
-    ``neutts.NeuTTS`` (ctor with the reference's device strings, encode_reference, infer, soundfile.write) and
-    writes a wav of 480 * N samples.  Checkpoints, tokenizer and espeak do not exist offline, so the three loaders
-    are replaced by the fakes of this file; everything else -- the example and the facade -- runs unmodified."""
-    import importlib.util
-    import sys
-    import types
+def test_reference_basic_example_call_trace(tmp_path, monkeypatch):
+    """SURVEY §8c golden (4): the calls the reference's examples/basic_example.py makes -- recorded from the original
+    project into tests/golden/basic_example_calls.json (ctor with the reference's device strings, encode_reference,
+    infer, soundfile.write) -- replayed on THIS repo's ``neutts.NeuTTS`` write a wav of 480 * N samples.  Checkpoints,
+    tokenizer and espeak do not exist offline, so the three loaders are replaced by the fakes of this file."""
+    import json
 
     import neutts.neutts as NN
+    from neutts import NeuTTS
 
-    written = {}
-    sf = types.ModuleType("soundfile")
-    sf.write = lambda path, wav, sr: written.update(path=path, wav=np.asarray(wav), sr=sr)
-    monkeypatch.setitem(sys.modules, "soundfile", sf)
+    calls = json.load(open(BASIC_EXAMPLE_CALLS))["calls"]
+    assert [c["call"] for c in calls] == ["NeuTTS", "encode_reference", "infer", "soundfile.write"]
     tok = FakeTokenizer()
     tail = [tok.speech_base + c for c in (5, 9, 11, 70000, 13)] + [65, tok.special_base + 5]   # 4 valid codes, junk, EOS
     seen = {}
@@ -413,16 +409,22 @@ def test_reference_basic_example_runs_unmodified(tmp_path, monkeypatch):
     # reference voice: audio file + the pre-encoded codes next to it, as the reference ships them (samples/dave.{wav,pt})
     (tmp_path / "dave.wav").write_bytes(b"RIFF....WAVE")
     torch.save(torch.tensor([54, 65493, 7], dtype=torch.int32), tmp_path / "dave.pt")
-    (tmp_path / "dave.txt").write_text("hello there\n")
-    spec = importlib.util.spec_from_file_location("ref_basic_example", REF_EXAMPLE)
-    mod = importlib.util.module_from_spec(spec)
+    values = {"<ref_audio_path>": str(tmp_path / "dave.wav"), "<output_path>": str(tmp_path / "out.wav")}
+    written = {}
     import warnings
     with warnings.catch_warnings():
         warnings.simplefilter("ignore")
-        spec.loader.exec_module(mod)            # `from neutts import NeuTTS` resolves to this repo's package
-        assert mod.NeuTTS is NN.NeuTTS
-        mod.main("Testing.", str(tmp_path / "dave.wav"), str(tmp_path / "dave.txt"), "neuphonic/neutts-air",
-                 output_path=str(tmp_path / "out.wav"))
+        for c in calls:
+            args = [values.get(a, a) if isinstance(a, str) else a for a in c["args"]]
+            if c["call"] == "NeuTTS":
+                tts = NeuTTS(*args, **c["kwargs"])
+            elif c["call"] == "encode_reference":
+                values["<ref_codes>"] = tts.encode_reference(*args, **c["kwargs"])
+            elif c["call"] == "infer":
+                values["<wav>"] = tts.infer(*args, **c["kwargs"])
+            else:
+                path, wav, sr = [values.get(a, a) if isinstance(a, str) else a for a in c["args"]]
+                written.update(path=path, wav=np.asarray(wav), sr=sr)
     assert seen == {"backbone": ("neuphonic/neutts-air", "cpu"), "codec": ("neuphonic/neucodec", "cpu")}
     assert written["sr"] == 24000 and written["path"].endswith("out.wav")
     assert written["wav"].dtype == np.float32 and written["wav"].shape == (480 * 4,) and np.isfinite(written["wav"]).all()
