@@ -167,8 +167,8 @@ int nt_lm_debug_set_layers(nt_lm* lm, int n_layers);
 /* launch-latency probe: n dependent trivial kernels (grid x block) each incrementing *counter */
 int nt_debug_launch_chain(int n, int grid, int block, int* counter, void* stream);
 void* nt_lm_debug_ptr(nt_lm* lm, const char* name);
-/* megakernel timeline: buf = device int64 [2][1024] receiving %globaltimer marks of decode step `step`
- * from the first and the last CTA (NULL disables) */
+/* persistent decode kernel timeline: buf = device int64 [2][1024] receiving %globaltimer marks of decode
+ * step `step` from CTAs 0 and 1 (NULL disables) */
 int nt_lm_debug_set_profile(nt_lm* lm, long long* buf, int step);
 
 /* ------------------------------------------------------------------------------------------

@@ -15,7 +15,7 @@ from pathlib import Path
 PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 LIB = PKG / "libneutts_b200.so"
-SOURCES = ["lm_api.cu", "lm_kernels.cu", "lm_mega.cu", "lm_decode_tc.cu", "gemm_tc.cu", "codec.cu"]
+SOURCES = ["lm_api.cu", "lm_kernels.cu", "lm_decode_tc.cu", "gemm_tc.cu", "codec.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC",

@@ -402,11 +402,7 @@ int gemm_dispatch(const nt_gemm_args& a, cudaStream_t stream, SplitK* split, boo
 
   // tile-N choice: keep >= ~1 wave of CTAs when the problem allows it
   const int mt = (a.M + 127) / 128;
-  int bn = gemm_tile_n(a.M, a.N, a.act == NT_ACT_SWIGLU);
-  if (a.act == NT_ACT_SWIGLU && mt == 1) {   // experiments: tile width of the batched-decode gate/up GEMM
-    static const int force = [] { const char* e = getenv("NT_GEMM_GU_BN"); return e ? atoi(e) : 0; }();
-    if (force == 64 || force == 128) bn = force;
-  }
+  const int bn = gemm_tile_n(a.M, a.N, a.act == NT_ACT_SWIGLU);
   if (tile_max && (split || a.act != NT_ACT_NONE || a.out_bf16)) return set_error(NT_ERR_INVALID, "gemm: tile maxima need the plain fp32 epilogue");
 
   if (s3 && (a.dtype != NT_TF32 || split)) return set_error(NT_ERR_INVALID, "gemm: 3xTF32 needs tf32 operands and no split-K");
@@ -433,7 +429,7 @@ int gemm_dispatch(const nt_gemm_args& a, cudaStream_t stream, SplitK* split, boo
   ep.split_stride = 0;
   ep.w_const = w_const ? 1 : 0;
   ep.tile_max = tile_max;
-  ep.w_stream = (w_const && mt == 1 && !getenv("NT_GEMM_NO_EVICT_FIRST")) ? 1 : 0;
+  ep.w_stream = (w_const && mt == 1) ? 1 : 0;
   if (split) {
     split->used = 1;
     const int tiles = mt * ((a.N + bn - 1) / bn);
@@ -455,12 +451,7 @@ int gemm_dispatch(const nt_gemm_args& a, cudaStream_t stream, SplitK* split, boo
   const int ctas = mt * ((a.N + bn - 1) / bn) * (ep.split_k > 1 ? ep.split_k : 1);
   // Two CTAs per SM (half-depth ring) for every grid of more than one wave: one CTA's prologue / epilogue overlaps
   // the other's main loop, and grids just over a multiple of the SM count lose their short last wave.
-  // NT_GEMM_DEEP_RINGS=1 restores one deep-ring CTA per SM for grids beyond two waves with several row tiles.
-  static const bool deep_rings = [] {
-    const char* e = getenv("NT_GEMM_DEEP_RINGS");
-    return e && e[0] && e[0] != '0';
-  }();
-  const bool shallow = ctas > num_sms() && (ctas <= 2 * num_sms() || mt == 1 || !deep_rings);
+  const bool shallow = ctas > num_sms();
 #define NT_GEMM_CASE(FMT, BNV)                                                                           \
   return shallow ? launch_gemm<FMT, BNV, true>(ta, tb, ep, a.M, a.N, num_kb, kb_per_tap, stream)         \
                  : launch_gemm<FMT, BNV, false>(ta, tb, ep, a.M, a.N, num_kb, kb_per_tap, stream)

@@ -14,7 +14,6 @@ namespace nt {
 
 int set_error(int code, const char* fmt, ...);
 extern std::atomic<uint64_t> g_launches;
-bool pdl_disabled();  // NT_NO_PDL=1: launch without the programmatic-dependent-launch attribute (experiments)
 // Every kernel of the library asks for the maximum shared-memory carveout, so consecutive kernels never force the
 // SM to switch its L1 / shared-memory split (the big-tile kernels need ~180 KB; the small ones do not use L1 much).
 void prefer_max_smem_carveout(const void* kernel);
@@ -44,7 +43,7 @@ int launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, 
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = (pdl && !pdl_disabled()) ? 1 : 0;
+  cfg.numAttrs = pdl ? 1 : 0;
   cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(std::forward<Args>(args))...);
   if (e != cudaSuccess) return set_error(NT_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
   g_launches.fetch_add(1, std::memory_order_relaxed);

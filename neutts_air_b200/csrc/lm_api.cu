@@ -13,7 +13,6 @@
 
 #include "lm_decode_tc.cuh"
 #include "lm_kernels.cuh"
-#include "lm_mega.cuh"
 
 namespace nt {
 
@@ -28,22 +27,6 @@ int set_error(int code, const char* fmt, ...) {
   return code;
 }
 
-static bool env_flag(const char* name) {
-  const char* v = getenv(name);
-  return v && v[0] && v[0] != '0';
-}
-// largest batch the per-op GEMV chain takes when the megakernel is off (above it: tensor-core GEMM chain with M = batch)
-static int gemv_max_batch() {
-  const char* e = getenv("NT_GEMV_MAX_BATCH");
-  const int n = e ? atoi(e) : 4;
-  return n < 0 ? 0 : (n > 4 ? 4 : n);
-}
-// largest batch the persistent decode megakernel takes (default 4; up to 16 via concurrent instances)
-static int mega_max_batch() {
-  const char* e = getenv("NT_MEGA_MAX_BATCH");
-  const int n = e ? atoi(e) : 4;
-  return n < 1 ? 1 : (n > 16 ? 16 : n);
-}
 // Function attributes are per device context: a process that runs engines on two GPUs (backbone on cuda:0, codec on
 // cuda:1) must set them on both.  One table keyed by (kernel, device ordinal) serves the carve-out preference and the
 // dynamic shared-memory limit of every launch that goes through launch_kernel().
@@ -63,12 +46,11 @@ static KernelAttrState& kernel_attr_state(const void* kernel, std::unique_lock<s
   return table.back().second;
 }
 void prefer_max_smem_carveout(const void* kernel) {
-  static const bool off = env_flag("NT_NO_CARVEOUT");
   std::unique_lock<std::mutex> lock;
   KernelAttrState& st = kernel_attr_state(kernel, lock);
   if (st.carveout) return;
   st.carveout = true;
-  if (!off) cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
 }
 int ensure_dynamic_smem(const void* kernel, size_t bytes) {
   if (bytes <= 48 * 1024) return NT_OK;
@@ -79,10 +61,6 @@ int ensure_dynamic_smem(const void* kernel, size_t bytes) {
   if (e != cudaSuccess) return set_error(NT_ERR_CUDA, "cudaFuncSetAttribute(%zu B of dynamic shared memory) failed: %s", bytes, cudaGetErrorString(e));
   st.dyn_smem = bytes;
   return NT_OK;
-}
-bool pdl_disabled() {
-  static const bool off = env_flag("NT_NO_PDL");
-  return off;
 }
 
 // launch-latency probe: a chain of dependent trivial kernels
@@ -105,25 +83,22 @@ struct nt_lm {
   std::vector<const float*> ln1, bqkv, ln2;
   std::vector<const __nv_bfloat16*> wqkv, wo, wgu, wd;
   // workspace
-  float *h, *q, *attn, *act, *logits, *part_o, *part_ml, *cand_val, *inv_freq, *qkv, *h_last, *splitk_ws;
+  float *h, *q, *attn, *act, *logits, *cand_val, *inv_freq, *qkv, *h_last, *splitk_ws;
   size_t splitk_floats;
-  int *counters, *cand_idx, *tok_seq, *tok_pos, *cu_dev, *last_rows, *iota;
+  int *cand_idx, *tok_seq, *tok_pos, *cu_dev, *last_rows, *iota;
   __nv_bfloat16 *xn, *attn_bf16, *act_bf16;
-  // megakernel tables (device)
-  MegaPhase* phase_tab;
+  // persistent decode kernel tables (device)
   const float** ptr_tab;   // [3][n_layers]: ln1, bqkv, ln2
-  unsigned* gbar;
+  unsigned* gbar;          // grid barrier counters
   // cached decode-step graph
   cudaGraphExec_t graph = nullptr;
   std::vector<uint8_t> graph_key;
-  cudaStream_t grp_stream[4] = {nullptr, nullptr, nullptr, nullptr};  // concurrent megakernel instances (batch 5..16)
-  cudaEvent_t grp_fork = nullptr, grp_join[4] = {nullptr, nullptr, nullptr, nullptr};
   cudaStream_t cap_stream = nullptr;  // capture happens here (torch's default stream is the legacy
                                       // stream, which cannot be captured); replay on the caller's stream
   uint64_t graph_kernels = 0;         // kernel nodes in the captured step (for nt_launch_count)
   bool prefilled = false;
   int debug_layers = -1;              // >= 0: run only this many layers (per-stage parity tests)
-  long long* prof = nullptr;          // megakernel timeline buffer
+  long long* prof = nullptr;          // persistent decode kernel timeline buffer
   int prof_step = 0;
   // persistent wgmma decode kernel (lm_decode_tc.cu): plan, tensor maps and buffers live in the workspace
   bool tc_ok = false, tc_flat_ok = false;
@@ -158,14 +133,11 @@ static size_t lm_carve(const nt_lm_config& c, void* ws, size_t bytes, F&& assign
     (L)->attn = a.take<float>(size_t(c.max_batch) * c.n_heads * 64);                           \
     (L)->act = a.take<float>(size_t(c.max_batch) * I);                                         \
     (L)->logits = a.take<float>(size_t(c.max_batch) * V);                                      \
-    (L)->part_o = a.take<float>(size_t(c.max_batch) * c.n_heads * max_splits * 64);            \
-    (L)->part_ml = a.take<float>(size_t(c.max_batch) * c.n_heads * max_splits * 2);            \
     (L)->cand_val = a.take<float>(sampler_scratch_floats(c.max_batch, V));                     \
     (L)->cand_idx = a.take<int>(sampler_scratch_floats(c.max_batch, V));                       \
     (L)->inv_freq = a.take<float>(64);                                                         \
     (L)->qkv = a.take<float>(size_t(rows) * qkv_n);                                            \
     (L)->h_last = a.take<float>(size_t(c.max_batch) * H);                                      \
-    (L)->counters = a.take<int>(size_t(c.max_batch) * c.n_kv_heads);                           \
     (L)->tok_seq = a.take<int>(rows);                                                          \
     (L)->tok_pos = a.take<int>(rows);                                                          \
     (L)->cu_dev = a.take<int>(c.max_batch + 1);                                                \
@@ -174,9 +146,8 @@ static size_t lm_carve(const nt_lm_config& c, void* ws, size_t bytes, F&& assign
     (L)->xn = a.take<__nv_bfloat16>(size_t(rows) * H);                                         \
     (L)->attn_bf16 = a.take<__nv_bfloat16>(size_t(rows) * c.n_heads * 64);                     \
     (L)->act_bf16 = a.take<__nv_bfloat16>(size_t(rows) * I);                                   \
-    (L)->phase_tab = a.take<MegaPhase>(size_t(4) * c.n_layers + 1);                            \
     (L)->ptr_tab = a.take<const float*>(size_t(3) * c.n_layers);                               \
-    (L)->gbar = a.take<unsigned>(256);                                                         \
+    (L)->gbar = a.take<unsigned>(64);                                                          \
     (L)->splitk_floats = size_t(8) * 128 * (qkv_n > H ? qkv_n : H);                            \
     (L)->splitk_ws = a.take<float>(size_t(8) * 128 * (qkv_n > H ? qkv_n : H));                 \
     (L)->tc_rows = c.max_batch < kTcMaxBatch ? c.max_batch : kTcMaxBatch;                      \
@@ -262,45 +233,31 @@ extern "C" int nt_lm_create(const nt_lm_config* cfg, const nt_lm_weights* w, voi
     return set_error(NT_ERR_CUDA, "device is sm_%d%d; this library is built for sm_90a only", prop.major, prop.minor);
   }
   lm->num_sms = prop.multiProcessorCount;
-  // rotary inverse frequencies (modeling_qwen2.py:95-100), iota, zeroed split counters
+  // rotary inverse frequencies (modeling_qwen2.py:95-100), iota, per-layer norm / bias pointers
   float invf[64] = {0};
   for (int i = 0; i < 32; ++i) invf[i] = static_cast<float>(1.0 / std::pow(static_cast<double>(c.rope_theta), (2.0 * i) / 64.0));
   std::vector<int> iota(c.max_batch);
   for (int i = 0; i < c.max_batch; ++i) iota[i] = i;
+  std::vector<const float*> pt(size_t(3) * c.n_layers);
+  for (int l = 0; l < c.n_layers; ++l) {
+    pt[l] = lm->ln1[l];
+    pt[c.n_layers + l] = lm->bqkv[l];
+    pt[2 * c.n_layers + l] = lm->ln2[l];
+  }
   if (cudaMemcpy(lm->inv_freq, invf, sizeof(invf), cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemcpy(lm->iota, iota.data(), iota.size() * sizeof(int), cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemset(lm->counters, 0, size_t(c.max_batch) * c.n_kv_heads * sizeof(int)) != cudaSuccess) {
+      cudaMemcpy(lm->ptr_tab, pt.data(), pt.size() * sizeof(const float*), cudaMemcpyHostToDevice) != cudaSuccess) {
     delete lm;
     return set_error(NT_ERR_CUDA, "workspace initialisation failed: %s", cudaGetErrorString(cudaGetLastError()));
   }
   {
-    std::vector<MegaPhase> ph(size_t(4) * c.n_layers + 1);
-    std::vector<const float*> pt(size_t(3) * c.n_layers);
-    const int HD = c.n_heads * 64;
-    for (int l = 0; l < c.n_layers; ++l) {
-      ph[4 * l + 0] = MegaPhase{lm->wqkv[l], lm->qkv_n, c.hidden};
-      ph[4 * l + 1] = MegaPhase{lm->wo[l], c.hidden, HD};
-      ph[4 * l + 2] = MegaPhase{lm->wgu[l], 2 * c.inter, c.hidden};
-      ph[4 * l + 3] = MegaPhase{lm->wd[l], c.hidden, c.inter};
-      pt[l] = lm->ln1[l];
-      pt[c.n_layers + l] = lm->bqkv[l];
-      pt[2 * c.n_layers + l] = lm->ln2[l];
-    }
-    ph[4 * c.n_layers] = MegaPhase{lm->lm_head, c.vocab_size, c.hidden};
-    if (cudaMemcpy(lm->phase_tab, ph.data(), ph.size() * sizeof(MegaPhase), cudaMemcpyHostToDevice) != cudaSuccess ||
-        cudaMemcpy(lm->ptr_tab, pt.data(), pt.size() * sizeof(const float*), cudaMemcpyHostToDevice) != cudaSuccess) {
-      delete lm;
-      return set_error(NT_ERR_CUDA, "megakernel table upload failed");
-    }
-  }
-  {
     // persistent wgmma decode kernel: work plan + every tensor map, built once (re-encoding the maps on every GEMM
-    // call costs host time on each step).  A shape the plan cannot take leaves tc_ok false -> older decode paths.
+    // call costs host time on each step).  A shape the plan cannot take leaves tc_ok false -> the per-op chain.
     std::vector<TcPlan> plan(512);
     std::vector<unsigned char> nsl(4096, 0);
     TcShape ts{c.hidden, c.inter, c.n_heads, c.n_kv_heads, lm->qkv_n, c.vocab_size};
     const int G = lm->num_sms > 256 ? 256 : lm->num_sms;
-    lm->tc_flat_ok = (2 * c.inter + 127) / 128 <= 4096 && !env_flag("NT_TC_NO_FLAT") &&
+    lm->tc_flat_ok = (2 * c.inter + 127) / 128 <= 4096 &&
                      tc_build_plan(ts, G, true, plan.data() + 256, nsl.data(), &lm->tc_info[1]) == NT_OK;
     if (tc_build_plan(ts, G, false, plan.data(), nullptr, &lm->tc_info[0]) == NT_OK) {
       const size_t nmaps = size_t(4) * c.n_layers + 1 + 6;
@@ -329,14 +286,9 @@ extern "C" int nt_lm_create(const nt_lm_config* cfg, const nt_lm_weights* w, voi
         lm->tc_ok = true;
     }
   }
-  bool ok = cudaStreamCreateWithFlags(&lm->cap_stream, cudaStreamNonBlocking) == cudaSuccess &&
-            cudaEventCreateWithFlags(&lm->grp_fork, cudaEventDisableTiming) == cudaSuccess;
-  for (int i = 0; i < 4 && ok; ++i)
-    ok = cudaStreamCreateWithFlags(&lm->grp_stream[i], cudaStreamNonBlocking) == cudaSuccess &&
-         cudaEventCreateWithFlags(&lm->grp_join[i], cudaEventDisableTiming) == cudaSuccess;
-  if (!ok) {
+  if (cudaStreamCreateWithFlags(&lm->cap_stream, cudaStreamNonBlocking) != cudaSuccess) {
     delete lm;
-    return set_error(NT_ERR_CUDA, "stream / event creation failed");
+    return set_error(NT_ERR_CUDA, "stream creation failed");
   }
   *out = lm;
   return NT_OK;
@@ -346,11 +298,6 @@ extern "C" int nt_lm_destroy(nt_lm* lm) {
   if (!lm) return NT_OK;
   if (lm->graph) cudaGraphExecDestroy(lm->graph);
   if (lm->cap_stream) cudaStreamDestroy(lm->cap_stream);
-  if (lm->grp_fork) cudaEventDestroy(lm->grp_fork);
-  for (int i = 0; i < 4; ++i) {
-    if (lm->grp_stream[i]) cudaStreamDestroy(lm->grp_stream[i]);
-    if (lm->grp_join[i]) cudaEventDestroy(lm->grp_join[i]);
-  }
   delete lm;
   return NT_OK;
 }
@@ -404,8 +351,7 @@ static int check_sampling(const nt_lm* lm, const nt_lm_state* st, const nt_sampl
 // lm_head on B hidden rows (fp32, un-normalised) -> lm->logits / `logits`
 // tile-max sampler after the tensor-core lm_head (batch > 4): the GEMM must tile the vocabulary by 128 columns
 static bool use_tile_sampler(const nt_lm* lm, int B) {
-  return B > gemv_max_batch() && B <= lm->tc_rows && lm->tc_tmax && gemm_tile_n(B, lm->cfg.vocab_size, false) == 128 &&
-         !env_flag("NT_NO_TILE_SAMPLER");
+  return B > kGemvMaxBatch && B <= lm->tc_rows && lm->tc_tmax && gemm_tile_n(B, lm->cfg.vocab_size, false) == 128;
 }
 static int run_sampler(nt_lm* lm, const SamplerParams& s, int B, cudaStream_t stream) {
   if (use_tile_sampler(lm, B)) return launch_sampler_tiles(s, B, lm->tc_tmax, (lm->cfg.vocab_size + 127) / 128, stream);
@@ -414,7 +360,7 @@ static int run_sampler(nt_lm* lm, const SamplerParams& s, int B, cudaStream_t st
 
 static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cudaStream_t stream, const SplitK* pend = nullptr) {
   const nt_lm_config& c = lm->cfg;
-  if (B <= gemv_max_batch()) {
+  if (B <= kGemvMaxBatch) {
     GemvParams g;
     memset(&g, 0, sizeof(g));
     g.W = lm->lm_head, g.rows = c.vocab_size, g.K = c.hidden;
@@ -425,7 +371,6 @@ static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cud
   }
   // pend: the last down_proj left split-K slices that still have to be folded into hrows (batched decode only)
   const bool fold = pend && pend->used > 1;
-  if (fold && B <= gemv_max_batch()) return set_error(NT_ERR_STATE, "lm_head: pending split-K slices on the GEMV path");
   int rc = launch_rmsnorm_rows(hrows, lm->final_norm, c.rms_eps, B, c.hidden, nullptr, lm->xn, stream, fold ? pend->ws : nullptr,
                                fold ? pend->used : 0, fold ? pend->slice_stride : 0);
   if (rc) return rc;
@@ -453,7 +398,6 @@ static int layers_gemm(nt_lm* lm, const nt_lm_state* st, int rows, int B, int mo
   // norm of lm_head_rows reads lm->h next); in prefill a row gather comes first, so it stays whole.
   SplitK pend;
   pend.ws = lm->splitk_ws, pend.ws_floats = lm->splitk_floats, pend.used = 1, pend.slice_stride = 0;
-  const bool allow_split = !env_flag("NT_NO_SPLITK");
   for (int l = 0; l < n_layers; ++l) {
     if ((rc = launch_rmsnorm_rows(lm->h, lm->ln1[l], c.rms_eps, rows, H, nullptr, lm->xn, stream,
                                   pend.used > 1 ? pend.ws : nullptr, pend.used > 1 ? pend.used : 0, pend.slice_stride)))
@@ -466,11 +410,11 @@ static int layers_gemm(nt_lm* lm, const nt_lm_state* st, int rows, int B, int mo
     // few row tiles: the projection splits K into slices that rope_append sums (the bias rides on slice 0)
     SplitK qsplit;
     qsplit.ws = lm->splitk_ws, qsplit.ws_floats = lm->splitk_floats, qsplit.used = 1, qsplit.slice_stride = 0;
-    if ((rc = gemm_dispatch(a, stream, allow_split ? &qsplit : nullptr, true))) return rc;
+    if ((rc = gemm_dispatch(a, stream, &qsplit, true))) return rc;
     const int32_t* tseq = mode == 0 ? lm->tok_seq : lm->iota;
     const int32_t* tpos = mode == 0 ? lm->tok_pos : st->seq_lens;
     // decode on the tensor-core attention kernel (batch > 4): RoPE + KV append run in that kernel's prologue
-    const bool fuse_rope = mode == 1 && B > 4 && !env_flag("NT_NO_FUSED_ROPE");
+    const bool fuse_rope = mode == 1 && B > 4;
     if (!fuse_rope &&
         (rc = launch_rope_append(qsplit.used > 1 ? qsplit.ws : lm->qkv, rows, QN, tseq, tpos, c.n_heads, lm->inv_freq, lm->q, kv, l, stream,
                                  qsplit.used, qsplit.slice_stride)))
@@ -484,8 +428,7 @@ static int layers_gemm(nt_lm* lm, const nt_lm_state* st, int rows, int B, int mo
       AttnDecParams ad;
       memset(&ad, 0, sizeof(ad));
       ad.q = lm->q, ad.kv = kv, ad.layer = l, ad.n_heads = c.n_heads, ad.n_rep = c.n_heads / c.n_kv_heads;
-      ad.scale_log2 = scale_log2, ad.part_o = lm->part_o, ad.part_ml = lm->part_ml, ad.counters = lm->counters;
-      ad.out = lm->attn, ad.out_bf16 = lm->attn_bf16, ad.max_splits = lm->max_splits;
+      ad.scale_log2 = scale_log2, ad.out = lm->attn, ad.out_bf16 = lm->attn_bf16;
       if (fuse_rope) {
         ad.qkv = qsplit.used > 1 ? qsplit.ws : lm->qkv, ad.qkv_n = QN, ad.qkv_parts = qsplit.used;
         ad.qkv_pstride = qsplit.slice_stride, ad.inv_freq = lm->inv_freq;
@@ -495,7 +438,7 @@ static int layers_gemm(nt_lm* lm, const nt_lm_state* st, int rows, int B, int mo
     memset(&a, 0, sizeof(a));
     a.dtype = NT_BF16, a.M = rows, a.N = H, a.K = HD, a.A = lm->attn_bf16, a.lda = HD, a.W = lm->wo[l], a.ldw = HD;
     a.residual = lm->h, a.ldr = H, a.out_f32 = lm->h, a.ldc = H;
-    if ((rc = gemm_dispatch(a, stream, allow_split ? &pend : nullptr, true))) return rc;
+    if ((rc = gemm_dispatch(a, stream, &pend, true))) return rc;
     if ((rc = launch_rmsnorm_rows(lm->h, lm->ln2[l], c.rms_eps, rows, H, nullptr, lm->xn, stream,
                                   pend.used > 1 ? pend.ws : nullptr, pend.used > 1 ? pend.used : 0, pend.slice_stride)))
       return rc;
@@ -507,7 +450,7 @@ static int layers_gemm(nt_lm* lm, const nt_lm_state* st, int rows, int B, int mo
     memset(&a, 0, sizeof(a));
     a.dtype = NT_BF16, a.M = rows, a.N = H, a.K = I, a.A = lm->act_bf16, a.lda = I, a.W = lm->wd[l], a.ldw = I;
     a.residual = lm->h, a.ldr = H, a.out_f32 = lm->h, a.ldc = H;
-    if ((rc = gemm_dispatch(a, stream, (allow_split && (l + 1 < n_layers || tail)) ? &pend : nullptr, true))) return rc;
+    if ((rc = gemm_dispatch(a, stream, (l + 1 < n_layers || tail) ? &pend : nullptr, true))) return rc;
   }
   if (tail) *tail = pend;
   return NT_OK;
@@ -558,7 +501,7 @@ static int decode_step(nt_lm* lm, const nt_lm_state* st, int B, const nt_samplin
   int rc;
   SplitK tail;
   tail.ws = nullptr, tail.ws_floats = 0, tail.used = 1, tail.slice_stride = 0;
-  if (B <= gemv_max_batch()) {
+  if (B <= kGemvMaxBatch) {
     const KVLayout kv = make_kv(lm, st);
     const int H = c.hidden, I = c.inter, HD = c.n_heads * 64;
     const float scale_log2 = (1.0f / 8.0f) * 1.4426950408889634f;
@@ -574,8 +517,7 @@ static int decode_step(nt_lm* lm, const nt_lm_state* st, int B, const nt_samplin
       AttnDecParams ad;
       memset(&ad, 0, sizeof(ad));
       ad.q = lm->q, ad.kv = kv, ad.layer = l, ad.n_heads = c.n_heads, ad.n_rep = c.n_heads / c.n_kv_heads;
-      ad.scale_log2 = scale_log2, ad.part_o = lm->part_o, ad.part_ml = lm->part_ml, ad.counters = lm->counters;
-      ad.out = lm->attn, ad.out_bf16 = nullptr, ad.max_splits = lm->max_splits;
+      ad.scale_log2 = scale_log2, ad.out = lm->attn, ad.out_bf16 = nullptr;
       if ((rc = launch_attn_decode(ad, B, c.n_layers, stream))) return rc;
 
       memset(&g, 0, sizeof(g));
@@ -614,17 +556,19 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
   if (rc) return rc;
   if (n_steps < 0) return set_error(NT_ERR_INVALID, "negative step count");
 
-  if (n_steps == 0) return NT_OK;
-  // NT_DECODE_IMPL = tc (default: persistent wgmma kernel, every batch size) | mega | perop (older paths, kept
-  // for A/B measurements and as the fallback for shapes the persistent kernel's plan does not take)
+  // NT_DECODE_IMPL = tc (persistent wgmma kernel) | perop (per-op kernel chain).  Unset: the persistent kernel up to
+  // kTcDefaultMaxBatch sequences; its step time grows with the batch while the chain's is nearly flat, so the chain
+  // takes the larger batches.  The chain also serves every shape the persistent kernel's plan does not take.
   const char* impl = getenv("NT_DECODE_IMPL");
-  // default: the persistent kernel up to NT_TC_MAX_BATCH sequences; its step time grows with the batch while the
-  // per-op chain's is nearly flat, so the chain takes the larger batches
-  int tc_cap = 16;
-  if (const char* e = getenv("NT_TC_MAX_BATCH")) tc_cap = atoi(e);
-  const bool want_tc = (impl && impl[0] == 't') || ((!impl || !impl[0]) && B <= tc_cap);
+  bool want_tc = B <= kTcDefaultMaxBatch;
+  if (impl && impl[0]) {
+    if (strcmp(impl, "tc") && strcmp(impl, "perop"))
+      return set_error(NT_ERR_INVALID, "NT_DECODE_IMPL=%s: valid values are tc and perop", impl);
+    want_tc = impl[0] == 't';
+  }
+  if (n_steps == 0) return NT_OK;
   const int tc_layers = lm->debug_layers >= 0 ? lm->debug_layers : c.n_layers;
-  if (want_tc && lm->tc_ok && B <= lm->tc_rows && B * c.n_kv_heads <= lm->num_sms && !env_flag("NT_NO_MEGA")) {
+  if (want_tc && lm->tc_ok && B <= lm->tc_rows && B * c.n_kv_heads <= lm->num_sms) {
     TcParams P;
     memset(&P, 0, sizeof(P));
     P.n_layers = tc_layers, P.total_layers = c.n_layers;
@@ -665,65 +609,10 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
     if ((rc = launch_sampler_check(P.samp))) return rc;
     return launch_decode_tc(P, B, lm->num_sms > 256 ? 256 : lm->num_sms, info, stream);
   }
-  if (B <= mega_max_batch() && !env_flag("NT_NO_MEGA") && !(impl && impl[0] == 'p') && c.hidden % 64 == 0) {
-    // Persistent megakernel: every layer, the lm_head, the sampler and all n_steps in one launch.
-    // It wins up to 4 sequences (0.86 ms / step at batch 1 against 1.65 ms for the per-op chain, whose step time
-    // is the same from batch 5 to 64).  NT_MEGA_MAX_BATCH=5..16 instead runs up to four concurrent instances of
-    // <= 4 sequences on disjoint SM subsets (measured 1.78 ms at batch 8, 2.5 ms at 16: slower than per-op).
-    const int ngroups = (B + 3) / 4;
-    const int per = (B + ngroups - 1) / ngroups;
-    const int sms = lm->num_sms / ngroups;
-    const int splits_stride = lm->max_splits;
-    if (ngroups > 1) NT_CUDA_CHECK(cudaEventRecord(lm->grp_fork, stream));
-    for (int gi = 0; gi < ngroups; ++gi) {
-      const int b0 = gi * per, nb = (B - b0 < per) ? (B - b0) : per;
-      cudaStream_t gs = ngroups > 1 ? lm->grp_stream[gi] : stream;
-      if (ngroups > 1) NT_CUDA_CHECK(cudaStreamWaitEvent(gs, lm->grp_fork, 0));
-      MegaParams P;
-      memset(&P, 0, sizeof(P));
-      P.n_layers = lm->debug_layers >= 0 ? lm->debug_layers : c.n_layers;
-      P.total_layers = c.n_layers;
-      P.hidden = c.hidden, P.inter = c.inter, P.n_heads = c.n_heads, P.qkv_n = lm->qkv_n, P.vocab = c.vocab_size;
-      P.eps = c.rms_eps, P.scale_log2 = (1.0f / 8.0f) * 1.4426950408889634f;
-      P.phases = lm->phase_tab;
-      P.ln1 = lm->ptr_tab, P.bqkv = lm->ptr_tab + c.n_layers, P.ln2 = lm->ptr_tab + 2 * c.n_layers;
-      P.final_norm = lm->final_norm, P.inv_freq = lm->inv_freq;
-      const int HD = c.n_heads * 64;
-      P.h = lm->h + size_t(b0) * c.hidden, P.q = lm->q + size_t(b0) * HD, P.attn = lm->attn + size_t(b0) * HD;
-      P.act = lm->act + size_t(b0) * c.inter, P.logits = lm->logits + size_t(b0) * c.vocab_size;
-      P.kv = make_kv(lm, st);
-      P.kv.page_table += size_t(b0) * P.kv.max_pages_per_seq;
-      P.kv.seq_lens += b0;
-      P.part_o = lm->part_o + size_t(b0) * c.n_heads * splits_stride * 64;
-      P.part_ml = lm->part_ml + size_t(b0) * c.n_heads * splits_stride * 2;
-      P.counters = lm->counters, P.max_splits = lm->max_splits;
-      P.samp = make_sampler(lm, st, sp);
-      P.samp.advance = 1;
-      P.samp.slot_base = sp->slot_base + b0;
-      P.samp.logits = P.logits;
-      P.samp.seq_lens += b0, P.samp.cur_token += b0, P.samp.n_generated += b0, P.samp.done += b0;
-      P.samp.out_tokens += size_t(b0) * st->max_new;
-      if (P.samp.sp.forced) P.samp.sp.forced += size_t(b0) * st->max_new;
-      P.samp.cand_val += size_t(b0) * 256 * 64, P.samp.cand_idx += size_t(b0) * 256 * 64;
-      P.samp.h = P.h;
-      P.gbar = lm->gbar + 64 * gi;
-      P.n_steps = n_steps;
-      P.logits_out = logits_out ? logits_out + size_t(b0) * c.vocab_size : nullptr;
-      P.logits_step_stride = static_cast<long long>(B) * c.vocab_size;
-      P.prof = gi == 0 ? lm->prof : nullptr, P.prof_step = lm->prof_step;
-      if ((rc = launch_sampler_check(P.samp))) return rc;
-      if ((rc = launch_decode_mega(P, nb, sms, gs))) return rc;
-      if (ngroups > 1) {
-        NT_CUDA_CHECK(cudaEventRecord(lm->grp_join[gi], gs));
-        NT_CUDA_CHECK(cudaStreamWaitEvent(stream, lm->grp_join[gi], 0));
-      }
-    }
-    return NT_OK;
-  }
 
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   NT_CUDA_CHECK(cudaStreamIsCapturing(stream, &cap));
-  const bool use_graph = !logits_out && cap == cudaStreamCaptureStatusNone && !env_flag("NT_NO_GRAPH") && n_steps > 1;
+  const bool use_graph = !logits_out && cap == cudaStreamCaptureStatusNone && n_steps > 1;
   if (!use_graph) {
     for (int i = 0; i < n_steps; ++i) {
       if ((rc = decode_step(lm, st, B, sp, stream))) return rc;

@@ -26,7 +26,7 @@
 //   ~10 us on one CTA per sequence instead of a pass over the vocabulary.
 //
 // Replaces transformers generation/utils.py:2743-2805 + modeling_qwen2.py:280-309,353-413 for the decode loop
-// (SURVEY.md §8a rows A1, A3-A12); supersedes the CUDA-core megakernel (lm_mega.cu) and the 196-launch chain.
+// (SURVEY.md §8a rows A1, A3-A12); up to batch 16 it takes the place of the 196-launch per-op chain.
 #define NT_WGMMA_KERNELS
 #include "lm_device.cuh"
 #include "lm_decode_tc.cuh"
@@ -1125,11 +1125,8 @@ static size_t tc_attn_bytes(int aw) { return (tc_attn_layout_bytes(aw) + 1023) &
 
 bool tc_fold_in_cta(int B, int hidden) {
   // Every consumer re-folds ALL rows in the in-CTA fold, so its cost grows with the batch while the fold phases' is
-  // flat: the in-CTA fold is the default at batch 1 only.
-  // NT_TC_FOLD: "phase" forces the fold phases at batch 1, "cta" the in-CTA fold up to batch 4 (experiments).
-  const char* fe = getenv("NT_TC_FOLD");
-  const int cap = (fe && fe[0] == 'c') ? 4 : 1;
-  return B <= cap && size_t(B) * hidden * 4 <= 16 * 1024 && hidden <= 1024 && !(fe && fe[0] == 'p');
+  // flat: the in-CTA fold runs at batch 1 only.
+  return B == 1 && size_t(hidden) * 4 <= 16 * 1024 && hidden <= 1024;
 }
 
 int tc_build_plan(const TcShape& s, int G, bool flat, TcPlan* plan, unsigned char* gu_nsl, TcPlanInfo* info) {
@@ -1186,13 +1183,9 @@ int tc_build_plan(const TcShape& s, int G, bool flat, TcPlan* plan, unsigned cha
   }
   const int nr = int(rest.size());
   int rot = 0;
-  int ov[3] = {0, 0, 0};   // NT_TC_SLICES="q,o,d": K slices per phase (experiments; 0 = automatic)
-  if (const char* e = getenv("NT_TC_SLICES")) sscanf(e, "%d,%d,%d", &ov[0], &ov[1], &ov[2]);
   auto split_phase = [&](int ph, int T, int KB, int* slices) -> bool {
     int S = nr / T;
-    const int want = ph == kPhQ ? ov[0] : (ph == kPhO ? ov[1] : ov[2]);
     if (flat && ph != kPhD && S > (KB + 1) / 2) S = (KB + 1) / 2;   // measured at batch 1: 7 slices 702 us / step, 14 slices 759
-    if (want > 0) S = want;
     if (S < 1) S = 1;
     if (S > KB) S = KB;
     if (S > kTcMaxSlices) S = kTcMaxSlices;
@@ -1241,7 +1234,7 @@ static int launch_tc(TcParams& P, int num_sms, cudaStream_t stream) {
   const size_t acc = (size_t(128) * (NT + 4) * 4 + 127) & ~size_t(127);   // accumulator tile [128][NT + 4] fp32
   // batch <= 4: the attention staging sits BEHIND the B chunks, so a layer's KV pages are fetched while the qkv
   // projection still runs; otherwise the two alias (a phase uses one or the other)
-  const bool separate = P.fold_in_cta != 0 && !getenv("NT_TC_NO_PREFETCH");
+  const bool separate = P.fold_in_cta != 0;
   // dedicated staging: two page-walking warps (a split is 1..4 pages at batch <= 4), which leaves the weight ring 8 stages
   P.att_warps = separate ? 2 : 4;
   const size_t chunks = tc_chunk_bytes(NT), att = tc_attn_bytes(P.att_warps);
@@ -1281,7 +1274,7 @@ int launch_decode_tc(TcParams& P, int B, int num_sms, const TcPlanInfo& info, cu
   const int nt = B <= 16 ? 16 : (B <= 32 ? 32 : 64);
   if (info.max_chunks > 14) return set_error(NT_ERR_INVALID, "decode_tc: %d k-blocks per CTA exceed the staging area", info.max_chunks);
   P.fold_in_cta = tc_fold_in_cta(B, P.hidden) ? 1 : 0;
-  P.weights_evict_first = getenv("NT_TC_NO_EVICT_FIRST") ? 0 : 1;
+  P.weights_evict_first = 1;
   if (info.gu_split && !P.fold_in_cta) return set_error(NT_ERR_INVALID, "decode_tc: the flat plan needs the in-CTA fold (batch <= 4)");
   const bool hilo = B <= 8;
   if (hilo) return P.fold_in_cta ? launch_tc<16, true, true>(P, num_sms, stream) : launch_tc<16, true, false>(P, num_sms, stream);

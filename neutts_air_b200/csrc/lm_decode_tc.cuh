@@ -12,6 +12,7 @@ constexpr int kTcMmaWarp0 = 8;      // warps 8..11: the MMA warpgroup (warpgroup
 constexpr int kTcStreamWarp = 12;   // the weight-stream warp
 constexpr int kTcThreads = 416;     // 8 worker warps + 1 MMA warpgroup + 1 weight-stream warp
 constexpr int kTcMaxBatch = 64;
+constexpr int kTcDefaultMaxBatch = 16;  // nt_lm_decode's default: larger batches take the per-op chain
 constexpr int kTcMaxSlices = 16;
 constexpr int kTcMaxGuSlices = 4;   // K slices of one gate/up tile in the flat plan (batch <= 4)
 

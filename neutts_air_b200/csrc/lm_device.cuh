@@ -1,7 +1,7 @@
-// Device-side building blocks of the decode path, shared by the per-op kernels (lm_kernels.cu)
-// and the persistent decode megakernel (lm_mega.cu).  Every block-cooperative function takes a
-// `Sync` functor: SyncAll (= __syncthreads, per-op kernels) or SyncConsumers (named barrier
-// over the 256 consumer threads of the megakernel, whose producer warp never joins).
+// Device-side building blocks shared by the per-op kernels (lm_kernels.cu) and the persistent wgmma decode kernel
+// (lm_decode_tc.cu): sync functors, ld_cg, the mma.sync helpers, the split-KV geometry and the sampler pieces.
+// Every block-cooperative function takes a `Sync` functor: SyncAll (= __syncthreads, per-op kernels) or
+// SyncConsumers (named barrier over 256 consumer threads, for kernels whose other warps never join).
 // All functions assume the cooperating threads are threadIdx.x in [0, 256).
 #pragma once
 #include "lm_kernels.cuh"
@@ -24,245 +24,6 @@ NT_DEVINL T ld_cg(const T* p) {
   return __ldcg(p);
 }
 
-// =================================================================================== GEMV pieces
-// x planes: element k = 8c + j of batch row b lives in xs[(2b + j/4) * nch + c] component j%4, so
-// the two float4 reads that pair with one 16-byte bf16 weight chunk are conflict-free.
-template <int NB, typename Sync>
-NT_DEVINL void load_x_planes(const float* x, long long ldx, int K, const float* norm_w /*global or shared*/, float eps, float4* xs,
-                             float* s_part /*[8][4]*/, Sync sync) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int nch = K >> 3, nvec = K >> 2;
-  float ssq[NB];
-#pragma unroll
-  for (int b = 0; b < NB; ++b) ssq[b] = 0.f;
-#pragma unroll
-  for (int b = 0; b < NB; ++b) {
-    const float4* src = reinterpret_cast<const float4*>(x + b * ldx);
-    for (int m0 = 0; m0 < nvec; m0 += 4 * kConsumerThreads) {  // 4 independent loads in flight per thread
-      float4 v[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int m = m0 + j * kConsumerThreads + tid;
-        v[j] = (m < nvec) ? __ldcg(src + m) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int m = m0 + j * kConsumerThreads + tid;
-        if (m < nvec) {
-          xs[(2 * b + (m & 1)) * nch + (m >> 1)] = v[j];
-          ssq[b] += v[j].x * v[j].x + v[j].y * v[j].y + v[j].z * v[j].z + v[j].w * v[j].w;
-        }
-      }
-    }
-  }
-  if (norm_w) {
-#pragma unroll
-    for (int b = 0; b < NB; ++b) {
-      const float t = warp_sum(ssq[b]);
-      if (lane == 0) s_part[warp * 4 + b] = t;
-    }
-    sync();
-    // every thread rebuilds the row scale from the 8 warp partials and rescales the elements it wrote itself
-    const float4* nw = reinterpret_cast<const float4*>(norm_w);
-#pragma unroll
-    for (int b = 0; b < NB; ++b) {
-      float t = 0.f;
-#pragma unroll
-      for (int w = 0; w < kConsumerWarps; ++w) t += s_part[w * 4 + b];
-      const float sc = rsqrtf(t / static_cast<float>(K) + eps);
-      for (int m = tid; m < nvec; m += kConsumerThreads) {
-        float4& v = xs[(2 * b + (m & 1)) * nch + (m >> 1)];
-        const float4 g = nw[m];
-        v.x = v.x * sc * g.x, v.y = v.y * sc * g.y, v.z = v.z * sc * g.z, v.w = v.w * sc * g.w;
-      }
-    }
-  }
-  sync();
-}
-
-// dot products of one unit (two adjacent bf16 rows in shared memory) with the NB x-vectors over
-// 16-byte chunks [c_lo, c_hi), strided by lane.  Partial sums stay per lane.
-template <int NB>
-NT_DEVINL void unit_dot(const uint4* r0, const uint4* r1, const float4* xs, int nch, int c_lo, int c_hi, int lane,
-                        float (&d0)[NB], float (&d1)[NB]) {
-  for (int c = c_lo + lane; c < c_hi; c += 32) {
-    float f0[8], f1[8];
-    bf16x8_to_f32(r0[c], f0);
-    bf16x8_to_f32(r1[c], f1);
-#pragma unroll
-    for (int b = 0; b < NB; ++b) {
-      const float4 xa = xs[(2 * b) * nch + c];
-      const float4 xb = xs[(2 * b + 1) * nch + c];
-      d0[b] += f0[0] * xa.x + f0[1] * xa.y + f0[2] * xa.z + f0[3] * xa.w + f0[4] * xb.x + f0[5] * xb.y + f0[6] * xb.z +
-               f0[7] * xb.w;
-      d1[b] += f1[0] * xa.x + f1[1] * xa.y + f1[2] * xa.z + f1[3] * xa.w + f1[4] * xb.x + f1[5] * xb.y + f1[6] * xb.z +
-               f1[7] * xb.w;
-    }
-  }
-}
-
-// Batch-1 fast path for warp slices of <= 128 chunks (K <= 1024 per unit, or K <= 8192 split over the 8 warps):
-// the lane's slice of the input vector (chunks c_lo + lane + 32 k, k < 4) stays in registers for the whole phase, so a unit costs two 16-byte shared loads per chunk instead of four, and
-// the fully unrolled loop puts all weight loads of the unit in flight at once.
-struct XRegs {
-  float4 a[4], b[4];
-};
-NT_DEVINL void load_xregs(const float4* xs, int nch, int c_lo, int c_hi, int lane, XRegs& xr) {
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const int c = c_lo + lane + 32 * k;
-    const bool ok = c < c_hi;
-    xr.a[k] = ok ? xs[c] : make_float4(0.f, 0.f, 0.f, 0.f);
-    xr.b[k] = ok ? xs[nch + c] : make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-}
-NT_DEVINL void unit_dot_x1(const uint4* r0, const uint4* r1, int c_lo, int c_hi, int lane, const XRegs& xr, float& d0,
-                            float& d1) {
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const int c = c_lo + lane + 32 * k;
-    if (c < c_hi) {
-      float f0[8], f1[8];
-      bf16x8_to_f32(r0[c], f0);
-      bf16x8_to_f32(r1[c], f1);
-      const float4 xa = xr.a[k], xb = xr.b[k];
-      d0 += f0[0] * xa.x + f0[1] * xa.y + f0[2] * xa.z + f0[3] * xa.w + f0[4] * xb.x + f0[5] * xb.y + f0[6] * xb.z + f0[7] * xb.w;
-      d1 += f1[0] * xa.x + f1[1] * xa.y + f1[2] * xa.z + f1[3] * xa.w + f1[4] * xb.x + f1[5] * xb.y + f1[6] * xb.z + f1[7] * xb.w;
-    }
-  }
-}
-
-// Epilogue of one unit (rows 2u, 2u+1).  All lanes hold the full sums; lane b finishes batch row b.
-template <int NB>
-NT_DEVINL void gemv_epilogue(const GemvParams& p, int u, float (&d0)[NB], float (&d1)[NB], int lane) {
-  if (lane >= NB) return;
-  const int b = lane;
-  float a0 = d0[0], a1 = d1[0];
-#pragma unroll
-  for (int i = 1; i < NB; ++i)
-    if (b == i) a0 = d0[i], a1 = d1[i];
-  const int r0 = 2 * u;
-  if (p.bias_smem) {
-    a0 += p.bias_smem[r0 - p.row0];
-    a1 += p.bias_smem[r0 - p.row0 + 1];
-  } else if (p.bias) {
-    a0 += __ldg(p.bias + r0);
-    a1 += __ldg(p.bias + r0 + 1);
-  }
-  if (p.epi == GEMV_STORE) {
-    if (p.residual) {
-      const float2 r = __ldcg(reinterpret_cast<const float2*>(p.residual + b * p.ldr + r0));
-      a0 += r.x;
-      a1 += r.y;
-    }
-    *reinterpret_cast<float2*>(p.out + b * p.ldo + r0) = make_float2(a0, a1);
-    if (p.smem_out) {
-      p.smem_out[b * p.smem_ld + r0 - p.row0] = a0;
-      p.smem_out[b * p.smem_ld + r0 - p.row0 + 1] = a1;
-    }
-  } else if (p.epi == GEMV_SWIGLU) {
-    p.out[b * p.ldo + u] = silu(a0) * a1;
-  } else {  // GEMV_QKV_ROPE
-    const int head = u >> 5;  // 32 units per 64-row head
-    const int i = u & 31;
-    const int pos = p.pos_cache ? p.pos_cache[b] : __ldcg(p.kv.seq_lens + b);
-    const int n_kv = p.kv.n_kv_heads;
-    if (head < p.n_heads + n_kv) {
-      // rows (i, i+32) of a q/k head: half-split rotation (modeling_qwen2.py:116-146)
-      float s, c;
-      sincosf(static_cast<float>(pos) * __ldg(p.inv_freq + i), &s, &c);
-      const float lo = a0 * c - a1 * s;
-      const float hi = a1 * c + a0 * s;
-      if (head < p.n_heads) {
-        float* q = p.q_out + (static_cast<long long>(b) * p.n_heads + head) * 64;
-        q[i] = lo;
-        q[i + 32] = hi;
-      } else if (pos < p.kv.max_ctx) {
-        const int page = p.page_cache ? p.page_cache[b] : __ldcg(p.kv.page_table + b * p.kv.max_pages_per_seq + (pos >> 6));
-        __nv_bfloat16* kp = p.kv.page_ptr(p.layer, 0, page, head - p.n_heads) + (pos & 63) * 64;
-        kp[i] = __float2bfloat16(lo);
-        kp[i + 32] = __float2bfloat16(hi);
-      }
-    } else if (pos < p.kv.max_ctx) {
-      const int page = p.page_cache ? p.page_cache[b] : __ldcg(p.kv.page_table + b * p.kv.max_pages_per_seq + (pos >> 6));
-      __nv_bfloat16* vp = p.kv.page_ptr(p.layer, 1, page, head - p.n_heads - n_kv) + (pos & 63) * 64;
-      *reinterpret_cast<__nv_bfloat162*>(vp + 2 * i) = __floats2bfloat162_rn(a0, a1);
-    }
-  }
-}
-
-// One ring stage of a GEMV phase, executed by the 8 consumer warps.
-//   wpu == 1: the stage holds up to 8 units, warp w owns unit w;
-//   wpu == 8: the stage holds one unit, the warps split K and reduce through `red` (double-buffered
-//             by `parity`), warp 0 finishes.
-// `release` is called once per warp as soon as the warp has finished reading the stage.
-template <int NB, typename Release>
-NT_DEVINL void gemv_consume_stage(const GemvParams& p, const uint8_t* st, const float4* xs, float* red, int wpu,
-                                  int first_unit_local, int units_in_stage, int u_begin, int parity, Release release,
-                                  const XRegs& xr, bool use_xr) {
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int nch = p.K >> 3;
-  const int unit_bytes = 4 * p.K;
-  float d0[NB], d1[NB];
-#pragma unroll
-  for (int b = 0; b < NB; ++b) d0[b] = d1[b] = 0.f;
-  if (wpu == 1) {
-    const bool has = warp < units_in_stage;
-    if (has) {
-      const uint4* r0 = reinterpret_cast<const uint4*>(st + static_cast<size_t>(warp) * unit_bytes);
-      if (NB == 1 && use_xr)
-        unit_dot_x1(r0, r0 + nch, 0, nch, lane, xr, d0[0], d1[0]);
-      else
-        unit_dot<NB>(r0, r0 + nch, xs, nch, 0, nch, lane, d0, d1);
-    }
-    __syncwarp();
-    release();
-    if (has) {
-#pragma unroll
-      for (int b = 0; b < NB; ++b) {
-        d0[b] = warp_sum(d0[b]);
-        d1[b] = warp_sum(d1[b]);
-      }
-      gemv_epilogue<NB>(p, u_begin + first_unit_local + warp, d0, d1, lane);
-    }
-  } else {
-    const int c_lo = (nch * warp) / kConsumerWarps, c_hi = (nch * (warp + 1)) / kConsumerWarps;
-    const uint4* r0 = reinterpret_cast<const uint4*>(st);
-    if (NB == 1 && use_xr)
-      unit_dot_x1(r0, r0 + nch, c_lo, c_hi, lane, xr, d0[0], d1[0]);
-    else
-      unit_dot<NB>(r0, r0 + nch, xs, nch, c_lo, c_hi, lane, d0, d1);
-    __syncwarp();
-    release();
-    float* rbuf = red + parity * (kConsumerWarps * 2 * 4);
-#pragma unroll
-    for (int b = 0; b < NB; ++b) {
-      d0[b] = warp_sum(d0[b]);
-      d1[b] = warp_sum(d1[b]);
-    }
-    if (lane == 0) {
-#pragma unroll
-      for (int b = 0; b < NB; ++b) {
-        rbuf[(warp * 2 + 0) * 4 + b] = d0[b];
-        rbuf[(warp * 2 + 1) * 4 + b] = d1[b];
-      }
-    }
-    asm volatile("bar.sync 1, 256;" ::: "memory");  // the 8 consumer warps (also the whole CTA minus the producer)
-    if (warp == 0) {
-#pragma unroll
-      for (int b = 0; b < NB; ++b) {
-        float t0 = 0.f, t1 = 0.f;
-        for (int w = 0; w < kConsumerWarps; ++w) {
-          t0 += rbuf[(w * 2 + 0) * 4 + b];
-          t1 += rbuf[(w * 2 + 1) * 4 + b];
-        }
-        d0[b] = t0, d1[b] = t1;
-      }
-      gemv_epilogue<NB>(p, u_begin + first_unit_local, d0, d1, lane);
-    }
-  }
-}
-
 // ---- legacy tensor-core path used by both attention kernels (wgmma needs 64 rows of M; these tiles have 7-16)
 NT_DEVINL void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile(
@@ -281,128 +42,6 @@ NT_DEVINL void ldmatrix_x4_trans(uint32_t (&r)[4], uint32_t addr) {
                : "r"(addr));
 }
 
-
-// =================================================================================== decode attention
-struct AttnSmem {
-  __nv_bfloat16 k[64 * 64];
-  __nv_bfloat16 v[64 * 64];
-  float q[8][64];
-  float s[8][64];
-  float ml[8][2];
-  float corr[8];
-  float red[4][8][64];
-};
-struct AttnSync {      // lives outside any aliased shared-memory region
-  uint64_t bar;        // mbarrier (count 1) completed by the K/V bulk copies
-  uint32_t uses;       // completed phases so far (parity bookkeeping across items)
-  int last;
-};
-
-// A work item covers `pps` consecutive 64-token pages of one (sequence, kv head): K and V pages staged by bulk
-// copies, fp32 scores, an online softmax across pages, and a partial (m, l, unnormalised o) written per split.
-// The per-op kernel merges the partials in its last-arriving CTA; in the megakernel the consumer of the
-// attention output merges them itself (load_attn_merged), so that phase has no atomic / last-arriver chain.
-// sy->bar must be initialised (count 1) and sy->uses must count its completed phases.
-NT_DEVINL void attn_issue_page(const AttnDecParams& p, int b, int kvh, int page_idx, AttnSmem* sm, AttnSync* sy) {
-  const int page = __ldcg(p.kv.page_table + b * p.kv.max_pages_per_seq + page_idx);
-  asm volatile("fence.proxy.async;" ::: "memory");  // K/V rows may have been written through the generic proxy
-  mbar_arrive_expect_tx(&sy->bar, 2 * 8192);
-  bulk_g2s(sm->k, p.kv.page_ptr(p.layer, 0, page, kvh), 8192, &sy->bar);
-  bulk_g2s(sm->v, p.kv.page_ptr(p.layer, 1, page, kvh), 8192, &sy->bar);
-}
-
-template <typename Sync>
-NT_DEVINL void attn_split_item(const AttnDecParams& p, int b, int kvh, int split, int pps, int npages, int n_ctx, AttnSmem* sm,
-                               AttnSync* sy, bool first_page_in_flight, Sync sync) {
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int n_rep = p.n_rep;
-  for (int i = tid; i < n_rep * 64; i += kConsumerThreads)
-    sm->q[i >> 6][i & 63] = __ldcg(p.q + (static_cast<long long>(b) * p.n_heads + kvh * n_rep + (i >> 6)) * 64 + (i & 63));
-  if (tid < 8) sm->ml[tid][0] = -INFINITY, sm->ml[tid][1] = 0.f;
-  float acc[8];
-#pragma unroll
-  for (int h = 0; h < 8; ++h) acc[h] = 0.f;
-  const int p0 = split * pps, p1 = min(p0 + pps, npages);
-  for (int pg = p0; pg < p1; ++pg) {
-    const uint32_t parity = sy->uses & 1;
-    sync();  // previous page fully consumed; q / running stats visible; everyone has read `uses`
-    if (tid == 0) {
-      if (!(first_page_in_flight && pg == p0)) attn_issue_page(p, b, kvh, pg, sm, sy);
-      sy->uses += 1;
-    }
-    mbar_wait(&sy->bar, parity);
-    {  // scores: thread = (token, quarter of the head dim)
-      const int tok = tid >> 2, part = tid & 3;
-      const uint4* kr = reinterpret_cast<const uint4*>(sm->k + tok * 64 + part * 16);
-      float kf[16];
-      {
-        float t[8];
-        bf16x8_to_f32(kr[0], t);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) kf[j] = t[j];
-        bf16x8_to_f32(kr[1], t);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) kf[8 + j] = t[j];
-      }
-      const bool valid = (pg * 64 + tok) < n_ctx;
-      for (int h = 0; h < n_rep; ++h) {
-        float d = 0.f;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) d += kf[j] * sm->q[h][part * 16 + j];
-        d += __shfl_xor_sync(0xffffffffu, d, 1);
-        d += __shfl_xor_sync(0xffffffffu, d, 2);
-        if (part == 0) sm->s[h][tok] = valid ? d * p.scale_log2 : -INFINITY;
-      }
-    }
-    sync();
-    if (warp < n_rep) {  // online softmax update of head `warp`
-      const float s0 = sm->s[warp][lane], s1 = sm->s[warp][lane + 32];
-      const float m_old = sm->ml[warp][0];
-      const float m_new = fmaxf(m_old, warp_max(fmaxf(s0, s1)));  // every page of a live split has a valid token
-      const float p0v = exp2f(s0 - m_new), p1v = exp2f(s1 - m_new);
-      const float lsum = warp_sum(p0v + p1v);
-      sm->s[warp][lane] = p0v;
-      sm->s[warp][lane + 32] = p1v;
-      if (lane == 0) {
-        const float c = exp2f(m_old - m_new);  // 0 on the first page (m_old = -inf)
-        sm->corr[warp] = c;
-        sm->ml[warp][0] = m_new;
-        sm->ml[warp][1] = sm->ml[warp][1] * c + lsum;
-      }
-    }
-    sync();
-    {  // P.V : thread = (dim, token group of 16), accumulators carried across pages
-      const int d = tid & 63, g = tid >> 6;
-#pragma unroll
-      for (int h = 0; h < 8; ++h)
-        if (h < n_rep) acc[h] *= sm->corr[h];
-      for (int t = g * 16; t < g * 16 + 16; ++t) {
-        const float v = __bfloat162float(sm->v[t * 64 + d]);
-#pragma unroll
-        for (int h = 0; h < 8; ++h)
-          if (h < n_rep) acc[h] += sm->s[h][t] * v;
-      }
-    }
-  }
-  {
-    const int d = tid & 63, g = tid >> 6;
-#pragma unroll
-    for (int h = 0; h < 8; ++h)
-      if (h < n_rep) sm->red[g][h][d] = acc[h];
-  }
-  sync();
-  for (int i = tid; i < n_rep * 64; i += kConsumerThreads) {
-    const int h = i >> 6, d = i & 63;
-    const float o = sm->red[0][h][d] + sm->red[1][h][d] + sm->red[2][h][d] + sm->red[3][h][d];
-    const long long hh = static_cast<long long>(b) * p.n_heads + kvh * n_rep + h;
-    p.part_o[(hh * p.max_splits + split) * 64 + d] = o;
-    if (d == 0) {
-      p.part_ml[(hh * p.max_splits + split) * 2 + 0] = sm->ml[h][0];
-      p.part_ml[(hh * p.max_splits + split) * 2 + 1] = sm->ml[h][1];
-    }
-  }
-}
-
 // split geometry shared by the producer of the partials and their consumer
 struct SplitGeom {
   int n_ctx, npages, pps, nsplit;
@@ -414,58 +53,6 @@ NT_DEVINL SplitGeom split_geom(int seq_len, int max_ctx, int max_splits) {
   g.pps = (g.npages + max_splits - 1) / max_splits;
   g.nsplit = (g.npages + g.pps - 1) / g.pps;
   return g;
-}
-
-// Input staging of the o_proj phase: merge the split partials (in split order) straight into the x planes.
-// Two round trips to L2 in total: (1) all (m, l) pairs of the batch -> shared memory, turned into
-// per-split weights w_s = 2^(m_s - M) / L;  (2) every output element gathers its <= 16 partial values with
-// independent loads.  wbuf: shared float [NB * n_heads * 16].
-template <int NB, typename Sync>
-NT_DEVINL void load_attn_merged(const AttnDecParams& p, const int* pos_cache, int split_cap, float4* xs, float* wbuf, Sync sync) {
-  const int tid = threadIdx.x;
-  const int HD = p.n_heads * 64, nch = HD >> 3;
-  float* xf = reinterpret_cast<float*>(xs);
-  // (1) one thread per (sequence, head): read its nsplit (m, l) pairs, write normalised weights
-  for (int i = tid; i < NB * p.n_heads; i += kConsumerThreads) {
-    const int b = i / p.n_heads;
-    const SplitGeom g = split_geom(pos_cache[b], p.kv.max_ctx, split_cap);
-    const float2* ml = reinterpret_cast<const float2*>(p.part_ml) + static_cast<long long>(i) * p.max_splits;
-    float2 v[16];
-#pragma unroll
-    for (int s = 0; s < 16; ++s) v[s] = (s < g.nsplit) ? __ldcg(ml + s) : make_float2(-INFINITY, 0.f);
-    float M = -INFINITY;
-#pragma unroll
-    for (int s = 0; s < 16; ++s) M = fmaxf(M, v[s].x);
-    float L = 0.f;
-#pragma unroll
-    for (int s = 0; s < 16; ++s) {
-      v[s].x = exp2f(v[s].x - M);  // exactly 0 for the unused slots
-      L += v[s].x * v[s].y;
-    }
-    const float inv = 1.0f / L;
-#pragma unroll
-    for (int s = 0; s < 16; ++s) wbuf[i * 16 + s] = v[s].x * inv;
-  }
-  sync();
-  // (2) gather
-#pragma unroll
-  for (int b = 0; b < NB; ++b) {
-    const SplitGeom g = split_geom(pos_cache[b], p.kv.max_ctx, split_cap);
-    for (int e = tid; e < HD; e += kConsumerThreads) {
-      const int h = e >> 6, d = e & 63;
-      const long long hh = static_cast<long long>(b) * p.n_heads + h;
-      const float* po = p.part_o + hh * p.max_splits * 64 + d;
-      float o[16];
-#pragma unroll
-      for (int s = 0; s < 16; ++s) o[s] = (s < g.nsplit) ? __ldcg(po + s * 64) : 0.f;
-      float acc = 0.f;
-#pragma unroll
-      for (int s = 0; s < 16; ++s) acc += wbuf[hh * 16 + s] * o[s];
-      const int m4 = e >> 2;
-      xf[(((2 * b + (m4 & 1)) * nch + (m4 >> 1)) << 2) + (e & 3)] = acc;
-    }
-  }
-  sync();
 }
 
 // =================================================================================== sampler pieces

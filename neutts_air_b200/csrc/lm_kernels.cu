@@ -18,13 +18,243 @@
 #include <cuda.h>
 
 #include <cfloat>
-#include <cstdlib>
 #include <mutex>
 
 namespace nt {
 
 // =================================================================================== GEMV
 constexpr int kGemvThreads = (kConsumerWarps + 1) * 32;
+
+// x planes: element k = 8c + j of batch row b lives in xs[(2b + j/4) * nch + c] component j%4, so
+// the two float4 reads that pair with one 16-byte bf16 weight chunk are conflict-free.
+template <int NB, typename Sync>
+NT_DEVINL void load_x_planes(const float* x, long long ldx, int K, const float* norm_w /*global or shared*/, float eps, float4* xs,
+                             float* s_part /*[8][4]*/, Sync sync) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int nch = K >> 3, nvec = K >> 2;
+  float ssq[NB];
+#pragma unroll
+  for (int b = 0; b < NB; ++b) ssq[b] = 0.f;
+#pragma unroll
+  for (int b = 0; b < NB; ++b) {
+    const float4* src = reinterpret_cast<const float4*>(x + b * ldx);
+    for (int m0 = 0; m0 < nvec; m0 += 4 * kConsumerThreads) {  // 4 independent loads in flight per thread
+      float4 v[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int m = m0 + j * kConsumerThreads + tid;
+        v[j] = (m < nvec) ? __ldcg(src + m) : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int m = m0 + j * kConsumerThreads + tid;
+        if (m < nvec) {
+          xs[(2 * b + (m & 1)) * nch + (m >> 1)] = v[j];
+          ssq[b] += v[j].x * v[j].x + v[j].y * v[j].y + v[j].z * v[j].z + v[j].w * v[j].w;
+        }
+      }
+    }
+  }
+  if (norm_w) {
+#pragma unroll
+    for (int b = 0; b < NB; ++b) {
+      const float t = warp_sum(ssq[b]);
+      if (lane == 0) s_part[warp * 4 + b] = t;
+    }
+    sync();
+    // every thread rebuilds the row scale from the 8 warp partials and rescales the elements it wrote itself
+    const float4* nw = reinterpret_cast<const float4*>(norm_w);
+#pragma unroll
+    for (int b = 0; b < NB; ++b) {
+      float t = 0.f;
+#pragma unroll
+      for (int w = 0; w < kConsumerWarps; ++w) t += s_part[w * 4 + b];
+      const float sc = rsqrtf(t / static_cast<float>(K) + eps);
+      for (int m = tid; m < nvec; m += kConsumerThreads) {
+        float4& v = xs[(2 * b + (m & 1)) * nch + (m >> 1)];
+        const float4 g = nw[m];
+        v.x = v.x * sc * g.x, v.y = v.y * sc * g.y, v.z = v.z * sc * g.z, v.w = v.w * sc * g.w;
+      }
+    }
+  }
+  sync();
+}
+
+// dot products of one unit (two adjacent bf16 rows in shared memory) with the NB x-vectors over
+// 16-byte chunks [c_lo, c_hi), strided by lane.  Partial sums stay per lane.
+template <int NB>
+NT_DEVINL void unit_dot(const uint4* r0, const uint4* r1, const float4* xs, int nch, int c_lo, int c_hi, int lane,
+                        float (&d0)[NB], float (&d1)[NB]) {
+  for (int c = c_lo + lane; c < c_hi; c += 32) {
+    float f0[8], f1[8];
+    bf16x8_to_f32(r0[c], f0);
+    bf16x8_to_f32(r1[c], f1);
+#pragma unroll
+    for (int b = 0; b < NB; ++b) {
+      const float4 xa = xs[(2 * b) * nch + c];
+      const float4 xb = xs[(2 * b + 1) * nch + c];
+      d0[b] += f0[0] * xa.x + f0[1] * xa.y + f0[2] * xa.z + f0[3] * xa.w + f0[4] * xb.x + f0[5] * xb.y + f0[6] * xb.z +
+               f0[7] * xb.w;
+      d1[b] += f1[0] * xa.x + f1[1] * xa.y + f1[2] * xa.z + f1[3] * xa.w + f1[4] * xb.x + f1[5] * xb.y + f1[6] * xb.z +
+               f1[7] * xb.w;
+    }
+  }
+}
+
+// Batch-1 fast path for warp slices of <= 128 chunks (K <= 1024 per unit, or K <= 8192 split over the 8 warps):
+// the lane's slice of the input vector (chunks c_lo + lane + 32 k, k < 4) stays in registers for the whole phase, so a unit costs two 16-byte shared loads per chunk instead of four, and
+// the fully unrolled loop puts all weight loads of the unit in flight at once.
+struct XRegs {
+  float4 a[4], b[4];
+};
+NT_DEVINL void load_xregs(const float4* xs, int nch, int c_lo, int c_hi, int lane, XRegs& xr) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int c = c_lo + lane + 32 * k;
+    const bool ok = c < c_hi;
+    xr.a[k] = ok ? xs[c] : make_float4(0.f, 0.f, 0.f, 0.f);
+    xr.b[k] = ok ? xs[nch + c] : make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+}
+NT_DEVINL void unit_dot_x1(const uint4* r0, const uint4* r1, int c_lo, int c_hi, int lane, const XRegs& xr, float& d0,
+                            float& d1) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int c = c_lo + lane + 32 * k;
+    if (c < c_hi) {
+      float f0[8], f1[8];
+      bf16x8_to_f32(r0[c], f0);
+      bf16x8_to_f32(r1[c], f1);
+      const float4 xa = xr.a[k], xb = xr.b[k];
+      d0 += f0[0] * xa.x + f0[1] * xa.y + f0[2] * xa.z + f0[3] * xa.w + f0[4] * xb.x + f0[5] * xb.y + f0[6] * xb.z + f0[7] * xb.w;
+      d1 += f1[0] * xa.x + f1[1] * xa.y + f1[2] * xa.z + f1[3] * xa.w + f1[4] * xb.x + f1[5] * xb.y + f1[6] * xb.z + f1[7] * xb.w;
+    }
+  }
+}
+
+// Epilogue of one unit (rows 2u, 2u+1).  All lanes hold the full sums; lane b finishes batch row b.
+template <int NB>
+NT_DEVINL void gemv_epilogue(const GemvParams& p, int u, float (&d0)[NB], float (&d1)[NB], int lane) {
+  if (lane >= NB) return;
+  const int b = lane;
+  float a0 = d0[0], a1 = d1[0];
+#pragma unroll
+  for (int i = 1; i < NB; ++i)
+    if (b == i) a0 = d0[i], a1 = d1[i];
+  const int r0 = 2 * u;
+  if (p.bias) {
+    a0 += __ldg(p.bias + r0);
+    a1 += __ldg(p.bias + r0 + 1);
+  }
+  if (p.epi == GEMV_STORE) {
+    if (p.residual) {
+      const float2 r = __ldcg(reinterpret_cast<const float2*>(p.residual + b * p.ldr + r0));
+      a0 += r.x;
+      a1 += r.y;
+    }
+    *reinterpret_cast<float2*>(p.out + b * p.ldo + r0) = make_float2(a0, a1);
+  } else if (p.epi == GEMV_SWIGLU) {
+    p.out[b * p.ldo + u] = silu(a0) * a1;
+  } else {  // GEMV_QKV_ROPE
+    const int head = u >> 5;  // 32 units per 64-row head
+    const int i = u & 31;
+    const int pos = __ldcg(p.kv.seq_lens + b);
+    const int n_kv = p.kv.n_kv_heads;
+    if (head < p.n_heads + n_kv) {
+      // rows (i, i+32) of a q/k head: half-split rotation (modeling_qwen2.py:116-146)
+      float s, c;
+      sincosf(static_cast<float>(pos) * __ldg(p.inv_freq + i), &s, &c);
+      const float lo = a0 * c - a1 * s;
+      const float hi = a1 * c + a0 * s;
+      if (head < p.n_heads) {
+        float* q = p.q_out + (static_cast<long long>(b) * p.n_heads + head) * 64;
+        q[i] = lo;
+        q[i + 32] = hi;
+      } else if (pos < p.kv.max_ctx) {
+        const int page = __ldcg(p.kv.page_table + b * p.kv.max_pages_per_seq + (pos >> 6));
+        __nv_bfloat16* kp = p.kv.page_ptr(p.layer, 0, page, head - p.n_heads) + (pos & 63) * 64;
+        kp[i] = __float2bfloat16(lo);
+        kp[i + 32] = __float2bfloat16(hi);
+      }
+    } else if (pos < p.kv.max_ctx) {
+      const int page = __ldcg(p.kv.page_table + b * p.kv.max_pages_per_seq + (pos >> 6));
+      __nv_bfloat16* vp = p.kv.page_ptr(p.layer, 1, page, head - p.n_heads - n_kv) + (pos & 63) * 64;
+      *reinterpret_cast<__nv_bfloat162*>(vp + 2 * i) = __floats2bfloat162_rn(a0, a1);
+    }
+  }
+}
+
+// One ring stage of a GEMV phase, executed by the 8 consumer warps.
+//   wpu == 1: the stage holds up to 8 units, warp w owns unit w;
+//   wpu == 8: the stage holds one unit, the warps split K and reduce through `red` (double-buffered
+//             by `parity`), warp 0 finishes.
+// `release` is called once per warp as soon as the warp has finished reading the stage.
+template <int NB, typename Release>
+NT_DEVINL void gemv_consume_stage(const GemvParams& p, const uint8_t* st, const float4* xs, float* red, int wpu,
+                                  int first_unit_local, int units_in_stage, int u_begin, int parity, Release release,
+                                  const XRegs& xr, bool use_xr) {
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int nch = p.K >> 3;
+  const int unit_bytes = 4 * p.K;
+  float d0[NB], d1[NB];
+#pragma unroll
+  for (int b = 0; b < NB; ++b) d0[b] = d1[b] = 0.f;
+  if (wpu == 1) {
+    const bool has = warp < units_in_stage;
+    if (has) {
+      const uint4* r0 = reinterpret_cast<const uint4*>(st + static_cast<size_t>(warp) * unit_bytes);
+      if (NB == 1 && use_xr)
+        unit_dot_x1(r0, r0 + nch, 0, nch, lane, xr, d0[0], d1[0]);
+      else
+        unit_dot<NB>(r0, r0 + nch, xs, nch, 0, nch, lane, d0, d1);
+    }
+    __syncwarp();
+    release();
+    if (has) {
+#pragma unroll
+      for (int b = 0; b < NB; ++b) {
+        d0[b] = warp_sum(d0[b]);
+        d1[b] = warp_sum(d1[b]);
+      }
+      gemv_epilogue<NB>(p, u_begin + first_unit_local + warp, d0, d1, lane);
+    }
+  } else {
+    const int c_lo = (nch * warp) / kConsumerWarps, c_hi = (nch * (warp + 1)) / kConsumerWarps;
+    const uint4* r0 = reinterpret_cast<const uint4*>(st);
+    if (NB == 1 && use_xr)
+      unit_dot_x1(r0, r0 + nch, c_lo, c_hi, lane, xr, d0[0], d1[0]);
+    else
+      unit_dot<NB>(r0, r0 + nch, xs, nch, c_lo, c_hi, lane, d0, d1);
+    __syncwarp();
+    release();
+    float* rbuf = red + parity * (kConsumerWarps * 2 * 4);
+#pragma unroll
+    for (int b = 0; b < NB; ++b) {
+      d0[b] = warp_sum(d0[b]);
+      d1[b] = warp_sum(d1[b]);
+    }
+    if (lane == 0) {
+#pragma unroll
+      for (int b = 0; b < NB; ++b) {
+        rbuf[(warp * 2 + 0) * 4 + b] = d0[b];
+        rbuf[(warp * 2 + 1) * 4 + b] = d1[b];
+      }
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");  // the 8 consumer warps (also the whole CTA minus the producer)
+    if (warp == 0) {
+#pragma unroll
+      for (int b = 0; b < NB; ++b) {
+        float t0 = 0.f, t1 = 0.f;
+        for (int w = 0; w < kConsumerWarps; ++w) {
+          t0 += rbuf[(w * 2 + 0) * 4 + b];
+          t1 += rbuf[(w * 2 + 1) * 4 + b];
+        }
+        d0[b] = t0, d1[b] = t1;
+      }
+      gemv_epilogue<NB>(p, u_begin + first_unit_local, d0, d1, lane);
+    }
+  }
+}
 
 struct GemvSmemPlan {
   int stage_bytes, nstages, units_per_stage, wpu;
@@ -38,10 +268,6 @@ static GemvSmemPlan gemv_plan(int K, int nb) {
   p.units_per_stage = (p.wpu == 1) ? kConsumerWarps : 1;
   p.stage_bytes = unit_bytes * p.units_per_stage;
   p.nstages = (p.wpu == 1) ? 3 : 4;
-  if (const char* e = getenv("NT_GEMV_STAGES")) {  // experiments
-    const int n = atoi(e);
-    if (n >= 2 && n <= 8) p.nstages = n;
-  }
   size_t off = 0;
   p.ring_off = off;
   off += size_t(p.stage_bytes) * p.nstages;
@@ -517,7 +743,8 @@ int launch_attn_decode(const AttnDecParams& p, int B, int n_layers, cudaStream_t
 
 // =================================================================================== sampler
 int sampler_nchunks(int V) { return (V + kTopChunk - 1) / kTopChunk; }
-// candidate arrays: [sequence][chunk][64]; the megakernel indexes chunks by CTA (<= 256), the per-op path by 2048-logit chunk
+// candidate arrays: [sequence][chunk][64], indexed by 2048-logit chunk.  At least 256 chunks per sequence: the general
+// path of sample_tiles_seq writes up to 256 * kTopKeep candidates per sequence (row pitch kCandPitch).
 size_t sampler_scratch_floats(int B, int V) {
   const int chunks = sampler_nchunks(V) > 256 ? sampler_nchunks(V) : 256;
   return size_t(B) * chunks * kTopKeep;

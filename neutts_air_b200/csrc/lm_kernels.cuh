@@ -39,27 +39,20 @@ struct GemvParams {
   KVLayout kv;
   int layer, n_heads;
   const float* inv_freq;   // [32]
-  // optional shared-memory side channels (megakernel; all null/0 in the per-op kernels)
-  const int* pos_cache;    // [nb] this step's seq_lens snapshot
-  const int* page_cache;   // [nb] page id holding the new token
-  const float* bias_smem;  // this CTA's bias slice, indexed by (row - row0)
-  float* smem_out;         // GEMV_STORE: also keep the result at smem_out[b * smem_ld + row - row0]
-  int smem_ld, row0;
 };
 
+constexpr int kGemvMaxBatch = 4;  // gemv_kernel has one instance per batch size 1..4
 int launch_gemv(const GemvParams& p, int nb, int num_sms, cudaStream_t stream);
 
 struct AttnDecParams {
   const float* q;   // [B, n_heads*64]
   KVLayout kv;
   int layer, n_heads, n_rep;
-  float scale_log2;  // head_dim^-0.5 * log2(e)
-  float* part_o;     // [B, n_heads, max_splits, 64]  (unnormalised: sum_t 2^(s_t - m) v_t)
-  float* part_ml;    // [B, n_heads, max_splits, 2]   (m, l) in the log2 domain
-  int* counters;     // [B, n_kv_heads]
   float* out;        // [B, n_heads*64]
   __nv_bfloat16* out_bf16;  // optional copy for the tensor-core o_proj
-  int max_splits;
+  // Placed after the outputs: with scale_log2 right behind n_rep, ptxas gives both attention kernels
+  // 5 / 12 more registers (sm_90a, CUDA 12.9).
+  float scale_log2;  // head_dim^-0.5 * log2(e)
   // Fused RoPE + KV append (tensor-core variant, batch > 4): when qkv != nullptr the kernel reads the projection output
   // itself ([B, qkv_n] fp32, bias already added, `qkv_parts` split-K slices `qkv_pstride` floats apart, summed in slice
   // order), rotates q / k at position seq_lens[b], appends the new K/V row to the cache and ignores `q`.
@@ -96,7 +89,7 @@ struct SamplerParams {
   int32_t* dbg_token;      // [B]
   const int32_t* n_generated_override;  // nt_op_topk_sample: read-only counters, no state update
   int32_t step_override;
-  int32_t slot_base;  // global slot index of local sequence 0 (keys the Philox counter; grouped megakernel launches)
+  int32_t slot_base;  // global slot index of local sequence 0 (keys the Philox counter)
 };
 int launch_sampler(const SamplerParams& p, int B, cudaStream_t stream);
 int launch_sampler_check(const SamplerParams& p);

@@ -3,8 +3,9 @@ oracle would take minutes per forward.  Parity there is checked through size-ind
 
   * prefill / decode consistency: the logits after prefill(P) + k teacher-forced decode steps equal the logits at
     the last position of prefill(P + k) — two different kernel families (tensor-core GEMMs + flash attention vs the
-    persistent GEMV megakernel with split-KV attention) over the same paged KV cache, RoPE positions and weights;
-  * batch invariance: a sequence decoded alone (megakernel) and inside a batch of 6 (per-op wgmma chain) agrees;
+    persistent wgmma decode kernel with split-KV attention) over the same paged KV cache, RoPE positions and weights;
+  * batch invariance: a sequence decoded alone and inside a batch of 6 agrees (both on the persistent wgmma kernel,
+    which folds the split-K slices in every CTA at batch 1 and in dedicated fold phases at batch 6);
   * reproducibility: the same seed gives the same sampled tokens twice.
 """
 import pytest
@@ -52,10 +53,10 @@ def test_full_size_batch_invariance_and_reproducibility(full_lm):
     forced = torch.randint(0, 217472, (6, 8), generator=torch.Generator().manual_seed(3))
     sp = lm.sampling(eos, min_new_tokens=0, max_new_tokens=8, forced=forced)
     lm.prefill(prompts, sp)
-    batch = lm.decode(4, sp, return_logits=True)[:, 1].float().cpu()          # slot 1, per-op chain (batch 6)
+    batch = lm.decode(4, sp, return_logits=True)[:, 1].float().cpu()          # slot 1, persistent kernel at batch 6
     sp1 = lm.sampling(eos, min_new_tokens=0, max_new_tokens=8, forced=forced[1:2])
     lm.prefill(prompts[1:2], sp1)
-    solo = lm.decode(4, sp1, return_logits=True)[:, 0].float().cpu()          # same sequence alone (megakernel)
+    solo = lm.decode(4, sp1, return_logits=True)[:, 0].float().cpu()          # same sequence alone (persistent kernel, batch 1)
     r = rel_err(batch, solo)
     print(f"FULL-SIZE batch invariance: relRMS {r:.2e}")
     assert r < 3e-2, r

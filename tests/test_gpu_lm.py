@@ -59,22 +59,22 @@ def test_lm_b1_logits_vs_oracle(cuda, cfgkw, P, n_new):
     got = _teacher_forced(cfg, w, lm, [prompt.tolist()], forced, n_new, eos)[0]
     _, mir = O.generate(cfg, w, prompt, eos, max_length=512, max_new_tokens=n_new, forced=forced[0], mirror=True)
     _, ref = O.generate(cfg, w, prompt, eos, max_length=512, max_new_tokens=n_new, forced=forced[0], mirror=False)
-    # step 0 comes out of the tensor-core prefill path, the rest out of the GEMV decode path
+    # step 0 comes out of the tensor-core prefill path, the rest out of the persistent decode kernel
     _check_logits(got, mir, ref, f"H{cfg.hidden_size} P{P}")
     # state machine: forced tokens were recorded, counters advanced
     assert lm.out_tokens[0, :n_new].cpu().tolist() == forced[0].tolist()
     assert int(lm.n_generated[0]) == n_new and int(lm.seq_lens[0]) == P + n_new - 1
 
 
-@pytest.mark.parametrize("mega", [True, False], ids=["megakernel", "per-op-kernels"])
+@pytest.mark.parametrize("persistent", [True, False], ids=["persistent-kernel", "per-op-chain"])
 @pytest.mark.parametrize("cfgkw", [SMALL, WIDE])
-def test_lm_decode_path_tight(cuda, cfgkw, mega, monkeypatch):
-    """Both decode implementations for batch <= 4: the persistent megakernel (default) and the per-op
-    kernel chain (NT_NO_MEGA=1).  A 1-token prompt followed by 70 teacher-forced steps exercises only the GEMV / split-KV decode
-    kernels (fp32 activations, bf16 KV; crosses the 64-token page boundary): against the mirrored
+def test_lm_decode_path_tight(cuda, cfgkw, persistent, monkeypatch):
+    """Both decode implementations for batch <= 4: the persistent wgmma kernel (default) and the per-op
+    CUDA-core chain (NT_DECODE_IMPL=perop).  A 1-token prompt followed by 70 teacher-forced steps exercises only the
+    decode kernels (fp32-grade activations, bf16 KV; crosses the 64-token page boundary): against the mirrored
     oracle the only noise left is the rare flip of a bf16 K/V rounding -> 1e-3 relative RMS."""
-    if not mega:
-        monkeypatch.setenv("NT_NO_MEGA", "1")
+    if not persistent:
+        monkeypatch.setenv("NT_DECODE_IMPL", "perop")
     cfg, w, lm = _setup(cfgkw, 13, max_batch=1, max_ctx=256, page_shuffle_seed=5)
     g = torch.Generator().manual_seed(6)
     n_new, eos = 71, cfg.vocab_size - 1
@@ -84,17 +84,18 @@ def test_lm_decode_path_tight(cuda, cfgkw, mega, monkeypatch):
     # the persistent wgmma kernel keeps fp32-grade activations (bf16 hi + lo pairs) but runs the attention products
     # on bf16 tensor-core operands like the prefill kernel: mirror "decode_tc"; the per-op chain is all fp32: "decode"
     _, mir = O.generate(cfg, w, prompt, eos, max_length=256, max_new_tokens=n_new, forced=forced[0], mirror=True,
-                        decode_mirror="decode_tc" if mega else None)
+                        decode_mirror="decode_tc" if persistent else None)
     r = rel_err(got, mir)
-    print(f"DECODE-PATH-PARITY H{cfg.hidden_size} mega={mega}: relRMS {r:.2e} max {max_err(got, mir):.2e}")
+    print(f"DECODE-PATH-PARITY H{cfg.hidden_size} persistent={persistent}: relRMS {r:.2e} max {max_err(got, mir):.2e}")
     assert r < 1e-3, r
 
 
-@pytest.mark.parametrize("mega", [True, False], ids=["megakernel", "per-op-kernels"])
-def test_lm_ragged_batch_prefill_and_decode(cuda, mega, monkeypatch):
-    """Ragged prompts packed back to back (no left padding); batch 3 uses the CUDA-core GEMV path."""
-    if not mega:
-        monkeypatch.setenv("NT_NO_MEGA", "1")
+@pytest.mark.parametrize("persistent", [True, False], ids=["persistent-kernel", "per-op-chain"])
+def test_lm_ragged_batch_prefill_and_decode(cuda, persistent, monkeypatch):
+    """Ragged prompts packed back to back (no left padding); batch 3 decodes on the persistent wgmma kernel
+    (default) or on the per-op CUDA-core chain (NT_DECODE_IMPL=perop)."""
+    if not persistent:
+        monkeypatch.setenv("NT_DECODE_IMPL", "perop")
     cfg, w, lm = _setup(SMALL, 21, max_batch=4, max_ctx=256)
     g = torch.Generator().manual_seed(9)
     lens, n_new, eos = [33, 64, 7], 5, cfg.vocab_size - 1
@@ -104,6 +105,16 @@ def test_lm_ragged_batch_prefill_and_decode(cuda, mega, monkeypatch):
     for b, p in enumerate(prompts):
         _, mir = O.generate(cfg, w, p, eos, max_length=256, max_new_tokens=n_new, forced=forced[b], mirror=True)
         assert rel_err(got[b], mir) < 6e-3 and max_err(got[b], mir) < 5e-2 * float(mir.std()), (b, rel_err(got[b], mir))
+
+
+def test_lm_decode_impl_rejects_unknown_value(cuda, monkeypatch):
+    """NT_DECODE_IMPL takes tc or perop; any other value, such as "mega", fails instead of silently picking a path."""
+    cfg, w, lm = _setup(SMALL, 23, max_batch=1, max_ctx=128)
+    sp = lm.sampling(cfg.vocab_size - 1, min_new_tokens=0, max_new_tokens=4)
+    lm.prefill([[1, 2, 3]], sp)
+    monkeypatch.setenv("NT_DECODE_IMPL", "mega")
+    with pytest.raises(ValueError, match="tc and perop"):
+        lm.decode(2, sp)
 
 
 @pytest.mark.parametrize("B,impl", [(6, None), (10, None), (18, None), (18, "tc"), (34, "tc"), (7, "perop")],
