@@ -150,6 +150,17 @@ int nt_lm_destroy(nt_lm* lm);
 int nt_lm_prefill(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu_seqlens_host, int B,
                   const nt_sampling* sp, float* logits_out, void* stream);
 
+/* Prefill B prompts into the listed slots (distinct, < max_batch) while every other slot keeps its KV pages,
+ * tokens and counters.  ids / cu_seqlens_host as in nt_lm_prefill; slots_host, stream_ids_host: host [B].
+ * Samples the first token of each listed slot.  Philox is keyed by stream_ids[i] (>= 0) instead of slot + slot_base
+ * for that slot until the next nt_lm_prefill (which restores slot + slot_base for all slots).  Afterwards
+ * nt_lm_decode(B_decode) continues every live slot < B_decode.  logits_out: optional [B][vocab] in call order.
+ * The caller writes the listed slots' page-table rows (and limits entries) before the call, on the same stream.
+ * Needs an earlier nt_lm_prefill; cur_token must hold a valid token id in every slot (a zeroed state does). */
+int nt_lm_prefill_slots(nt_lm* lm, const nt_lm_state* st, const int32_t* slots_host, const int32_t* stream_ids_host,
+                        const int32_t* ids, const int32_t* cu_seqlens_host, int B, const nt_sampling* sp,
+                        float* logits_out, void* stream);
+
 /* Run n_steps decode steps for slots 0..B-1 with no host synchronisation in between
  * (finished slots keep their state; their work is skipped on device).
  * logits_out: optional device f32 [n_steps][B][vocab] (tests only; forces logits to HBM). */

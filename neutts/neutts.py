@@ -186,6 +186,12 @@ class NeuTTS:
         Sampling parameters are the reference's (``neutts/neutts.py:338-347``)."""
         eos = self._tok_id("<|SPEECH_GENERATION_END|>")
         seed = self.seed if self.seed is not None else int(torch.randint(0, 2**31 - 1, (1,)).item())
+        if len(prompts) > self.max_batch and hasattr(self.backbone, "generate_queue"):
+            # more prompts than slots: refill each slot as soon as its utterance ends (prompt i keeps the Philox
+            # stream slot_base + i that the chunked loop gives it)
+            return self.backbone.generate_queue(list(prompts), eos, max_length=self.max_context, min_new_tokens=min_new_tokens,
+                                                temperature=1.0, top_k=50, max_new_tokens=max_new_tokens, seed=seed,
+                                                slot_base=slot_base)
         if hasattr(self.backbone, "generate_batch"):
             return self.backbone.generate_batch(list(prompts), eos, max_length=self.max_context, min_new_tokens=min_new_tokens,
                                                 temperature=1.0, top_k=50, max_new_tokens=max_new_tokens, seed=seed,
@@ -260,17 +266,27 @@ class NeuTTS:
     def infer_from_prompt_ids(self, prompts: Sequence[Sequence[int]], max_new_tokens: int | None = None,
                               min_new_tokens: int = 50, slot_base: int = 0) -> list:
         """Hot path only: prompt ids (host) -> waveforms (host).  Used by bench.py's end-to-end leg.
-        ``slot_base`` offsets the sampler's Philox slot index so chunks / ranks under one seed draw independently."""
+        ``slot_base`` offsets the sampler's Philox slot index so chunks / ranks under one seed draw independently.
+        More prompts than ``max_batch`` go through the backbone's ``generate_queue`` when it has one."""
         gen = self._generate_ids(prompts, max_new_tokens, min_new_tokens, slot_base)
         return [self._watermark(w) for w in self._decode_codes([self._ids_to_codes(g) for g in gen])]
 
     def infer_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], distributed: bool = False) -> list:
         """List in / list out.  With ``distributed=True`` (inside an initialised torch.distributed job) the
-        utterances are sharded over ranks and every rank returns all waveforms (one all-gather)."""
+        utterances are sharded over ranks and every rank returns all waveforms (one all-gather).
+
+        A list longer than ``max_batch`` (per rank when distributed) runs as one queue on a backbone that has
+        ``generate_queue``: a slot whose utterance ended takes the next one while the others keep decoding, so a
+        short utterance does not hold its slot until the longest of its chunk ends.  Utterance i keeps the random
+        stream it has in the chunked schedule.  Shorter lists, and backbones without ``generate_queue``, run in
+        chunks of ``max_batch``.  The codec then decodes the finished code lists either way."""
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
         prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(texts, ref_codes, ref_texts)]
+        queue = hasattr(self.backbone, "generate_queue")
         if not distributed:
+            if queue and len(prompts) > self.max_batch:
+                return self.infer_from_prompt_ids(prompts, slot_base=0)
             out = []
             for j in range(0, len(prompts), self.max_batch):
                 out += self.infer_from_prompt_ids(prompts[j: j + self.max_batch], slot_base=j)
@@ -280,6 +296,9 @@ class NeuTTS:
         mine = dist.shard_indices(len(prompts), [len(p) for p in prompts])
         local = []
         rank = dist.world()[0]
+        if queue and len(mine) > self.max_batch:
+            local = self.infer_from_prompt_ids([prompts[i] for i in mine], slot_base=rank << 20)
+            return dist.all_gather_waveforms(local, mine, len(prompts), device=self.codec.device)
         for j in range(0, len(mine), self.max_batch):
             local += self.infer_from_prompt_ids([prompts[i] for i in mine[j: j + self.max_batch]], slot_base=(rank << 20) + j)
         return dist.all_gather_waveforms(local, mine, len(prompts), device=self.codec.device)

@@ -88,7 +88,8 @@ class CodecWeights(C.Structure):
 # every symbol include/neutts_b200.h declares (tests check the library exports all of them)
 EXPORTS = [
     "nt_last_error", "nt_abi_version", "nt_launch_count", "nt_gemm",
-    "nt_lm_workspace_bytes", "nt_lm_create", "nt_lm_destroy", "nt_lm_prefill", "nt_lm_decode", "nt_lm_head_gemv",
+    "nt_lm_workspace_bytes", "nt_lm_create", "nt_lm_destroy", "nt_lm_prefill", "nt_lm_prefill_slots", "nt_lm_decode",
+    "nt_lm_head_gemv",
     "nt_lm_debug_set_layers", "nt_lm_debug_ptr", "nt_lm_debug_set_profile", "nt_debug_launch_chain",
     "nt_codec_workspace_bytes", "nt_codec_create", "nt_codec_destroy", "nt_codec_decode",
     "nt_op_rmsnorm", "nt_op_topk_sample",
@@ -120,6 +121,8 @@ def lib() -> C.CDLL:
     L.nt_lm_destroy.argtypes = [C.c_void_p]
     L.nt_lm_prefill.argtypes = [C.c_void_p, C.POINTER(LMState), C.c_void_p, C.POINTER(C.c_int32), C.c_int,
                                 C.POINTER(Sampling), C.c_void_p, C.c_void_p]
+    L.nt_lm_prefill_slots.argtypes = [C.c_void_p, C.POINTER(LMState), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p,
+                                      C.POINTER(C.c_int32), C.c_int, C.POINTER(Sampling), C.c_void_p, C.c_void_p]
     L.nt_lm_decode.argtypes = [C.c_void_p, C.POINTER(LMState), C.c_int, C.c_int, C.POINTER(Sampling), C.c_void_p, C.c_void_p]
     L.nt_lm_head_gemv.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     L.nt_lm_debug_set_layers.argtypes = [C.c_void_p, C.c_int]

@@ -113,6 +113,10 @@ struct nt_lm {
          *tc_h2 = nullptr;
   size_t tc_pair_bytes = 0;           // extent of the stamped buffers (contiguous, starting at tc_pq2)
   int tc_stamp = 0, tc_hstamp = 0;    // stamps handed out so far (see TcParams::stamp_base)
+  // prefill into chosen slots (nt_lm_prefill_slots)
+  int* slot_key = nullptr;            // [max_batch] Philox stream key per slot, -1: slot + slot_base
+  int* slot_args = nullptr;           // [3][max_batch] slots, stream keys, prompt lengths of the last call
+  int* slot_table = nullptr;          // [max_batch][max_pages] the listed slots' page-table rows, in call order
 };
 
 template <typename F>
@@ -166,6 +170,9 @@ static size_t lm_carve(const nt_lm_config& c, void* ws, size_t bytes, F&& assign
     (L)->tc_pg2 = a.take<float2>(size_t(kTcMaxGuSlices) * 4 * 2 * I);                          \
     (L)->tc_h2 = a.take<float2>(size_t(2) * 4 * H);                                            \
     (L)->tc_pair_bytes = size_t(reinterpret_cast<uint8_t*>((L)->tc_h2 + size_t(2) * 4 * H) - reinterpret_cast<uint8_t*>((L)->tc_pq2)); \
+    (L)->slot_key = a.take<int>(c.max_batch);                                                  \
+    (L)->slot_args = a.take<int>(size_t(3) * c.max_batch);                                     \
+    (L)->slot_table = a.take<int>(size_t(c.max_batch) * max_splits);                           \
   }
 
 static int lm_check_config(const nt_lm_config* c) {
@@ -246,7 +253,8 @@ extern "C" int nt_lm_create(const nt_lm_config* cfg, const nt_lm_weights* w, voi
   }
   if (cudaMemcpy(lm->inv_freq, invf, sizeof(invf), cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemcpy(lm->iota, iota.data(), iota.size() * sizeof(int), cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemcpy(lm->ptr_tab, pt.data(), pt.size() * sizeof(const float*), cudaMemcpyHostToDevice) != cudaSuccess) {
+      cudaMemcpy(lm->ptr_tab, pt.data(), pt.size() * sizeof(const float*), cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemset(lm->slot_key, 0xff, size_t(c.max_batch) * sizeof(int)) != cudaSuccess) {
     delete lm;
     return set_error(NT_ERR_CUDA, "workspace initialisation failed: %s", cudaGetErrorString(cudaGetLastError()));
   }
@@ -337,6 +345,7 @@ static SamplerParams make_sampler(const nt_lm* lm, const nt_lm_state* st, const 
   s.h = lm->h;
   s.hidden = lm->cfg.hidden;
   s.slot_base = sp->slot_base;
+  s.slot_key = lm->slot_key;
   return s;
 }
 
@@ -384,10 +393,12 @@ static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cud
 
 // Transformer layers over `rows` token rows held in lm->h, via tensor-core GEMMs.
 // mode 0: prefill (causal attention over the prompt);  mode 1: one new token per sequence.
+// table: page table to address the KV cache with, row b for sequence b of the call (default: the state's).
 static int layers_gemm(nt_lm* lm, const nt_lm_state* st, int rows, int B, int mode, int max_len, cudaStream_t stream,
-                       SplitK* tail = nullptr) {
+                       SplitK* tail = nullptr, const int32_t* table = nullptr) {
   const nt_lm_config& c = lm->cfg;
-  const KVLayout kv = make_kv(lm, st);
+  KVLayout kv = make_kv(lm, st);
+  if (table) kv.page_table = table;
   const int H = c.hidden, I = c.inter, QN = lm->qkv_n, HD = c.n_heads * 64;
   const float scale_log2 = (1.0f / 8.0f) * 1.4426950408889634f;
   int rc;
@@ -456,19 +467,16 @@ static int layers_gemm(nt_lm* lm, const nt_lm_state* st, int rows, int B, int mo
   return NT_OK;
 }
 
-extern "C" int nt_lm_prefill(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, int B,
-                             const nt_sampling* sp, float* logits_out, void* stream_) {
-  if (!lm || !st || !ids || !cu) return set_error(NT_ERR_INVALID, "nt_lm_prefill: null argument");
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+// Checks cu_seqlens [B+1] and stages the per-token tables of a prefill: the sequence and position of every token row,
+// the last row of every sequence.  lens / max_len: the prompt lengths.
+static int prefill_stage(nt_lm* lm, const int32_t* cu, int B, std::vector<int>& lens, int& max_len, cudaStream_t stream) {
   const nt_lm_config& c = lm->cfg;
-  if (B < 1 || B > c.max_batch) return set_error(NT_ERR_INVALID, "batch %d not in 1..%d", B, c.max_batch);
-  int rc = check_sampling(lm, st, sp);
-  if (rc) return rc;
   const int T = cu[B];
   if (cu[0] != 0 || T < B || T > c.max_prefill_tokens)
     return set_error(NT_ERR_INVALID, "prefill tokens %d not in %d..%d", T, B, c.max_prefill_tokens);
-  std::vector<int> tseq(T), tpos(T), last(B), lens(B);
-  int max_len = 0;
+  std::vector<int> tseq(T), tpos(T), last(B);
+  lens.assign(B, 0);
+  max_len = 0;
   for (int b = 0; b < B; ++b) {
     const int len = cu[b + 1] - cu[b];
     if (len < 1 || len >= c.max_ctx) return set_error(NT_ERR_INVALID, "prompt %d has length %d (must be 1..%d)", b, len, c.max_ctx - 1);
@@ -482,17 +490,83 @@ extern "C" int nt_lm_prefill(nt_lm* lm, const nt_lm_state* st, const int32_t* id
   NT_CUDA_CHECK(cudaMemcpyAsync(lm->cu_dev, cu, (B + 1) * sizeof(int), cudaMemcpyHostToDevice, stream));
   NT_CUDA_CHECK(cudaMemcpyAsync(lm->last_rows, last.data(), B * sizeof(int), cudaMemcpyHostToDevice, stream));
   // host vectors above are pageable: the runtime stages them before returning, so they may go out of scope
-  if ((rc = launch_embed_rows(lm->embed, ids, T, c.hidden, lm->h, stream))) return rc;
-  if ((rc = layers_gemm(lm, st, T, B, 0, max_len, stream))) return rc;
+  return NT_OK;
+}
+
+// Prompt rows -> KV cache + last-position logits in lm->logits (and logits_out).  table: see layers_gemm.
+static int prefill_forward(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, int B, int max_len,
+                           const int32_t* table, float* logits_out, cudaStream_t stream) {
+  const nt_lm_config& c = lm->cfg;
+  int rc;
+  if ((rc = launch_embed_rows(lm->embed, ids, cu[B], c.hidden, lm->h, stream))) return rc;
+  if ((rc = layers_gemm(lm, st, cu[B], B, 0, max_len, stream, nullptr, table))) return rc;
   if ((rc = launch_gather_rows(lm->h, lm->last_rows, B, c.hidden, lm->h_last, stream))) return rc;
   if ((rc = lm_head_rows(lm, lm->h_last, B, lm->logits, stream))) return rc;
   if (logits_out)
     NT_CUDA_CHECK(cudaMemcpyAsync(logits_out, lm->logits, size_t(B) * c.vocab_size * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+  return NT_OK;
+}
+
+extern "C" int nt_lm_prefill(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, int B,
+                             const nt_sampling* sp, float* logits_out, void* stream_) {
+  if (!lm || !st || !ids || !cu) return set_error(NT_ERR_INVALID, "nt_lm_prefill: null argument");
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  const nt_lm_config& c = lm->cfg;
+  if (B < 1 || B > c.max_batch) return set_error(NT_ERR_INVALID, "batch %d not in 1..%d", B, c.max_batch);
+  int rc = check_sampling(lm, st, sp);
+  if (rc) return rc;
+  std::vector<int> lens;
+  int max_len = 0;
+  if ((rc = prefill_stage(lm, cu, B, lens, max_len, stream))) return rc;
+  if ((rc = prefill_forward(lm, st, ids, cu, B, max_len, nullptr, logits_out, stream))) return rc;
   NT_CUDA_CHECK(cudaMemcpyAsync(st->seq_lens, lens.data(), B * sizeof(int), cudaMemcpyHostToDevice, stream));
+  NT_CUDA_CHECK(cudaMemsetAsync(lm->slot_key, 0xff, size_t(c.max_batch) * sizeof(int), stream));  // every slot: slot + slot_base
   SamplerParams s = make_sampler(lm, st, sp);
   if ((rc = run_sampler(lm, s, B, stream))) return rc;
   lm->prefilled = true;
   return NT_OK;
+}
+
+// Prefill into the listed slots while every other slot keeps its KV pages, tokens and counters.  The prefill chain
+// addresses KV by the sequence index of the call, so a small kernel first gathers the listed slots' page-table rows
+// into a compact table in call order (and resets those slots' length, counters and Philox key); the chain then runs
+// unchanged on that table.  The sampler maps logits row i to slot slots[i].  lm->h served as the prefill's token-row
+// scratch and row s of it is slot s's next decode input, so afterwards every slot's row is re-embedded from
+// cur_token: the survivors get back exactly what their last sampler step wrote there.
+extern "C" int nt_lm_prefill_slots(nt_lm* lm, const nt_lm_state* st, const int32_t* slots, const int32_t* stream_ids,
+                                   const int32_t* ids, const int32_t* cu, int B, const nt_sampling* sp, float* logits_out,
+                                   void* stream_) {
+  if (!lm || !st || !slots || !stream_ids || !ids || !cu) return set_error(NT_ERR_INVALID, "nt_lm_prefill_slots: null argument");
+  if (!lm->prefilled) return set_error(NT_ERR_STATE, "nt_lm_prefill_slots called before nt_lm_prefill");
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  const nt_lm_config& c = lm->cfg;
+  if (B < 1 || B > c.max_batch) return set_error(NT_ERR_INVALID, "batch %d not in 1..%d", B, c.max_batch);
+  int rc = check_sampling(lm, st, sp);
+  if (rc) return rc;
+  std::vector<int> args(size_t(3) * B);
+  std::vector<char> seen(c.max_batch, 0);
+  for (int i = 0; i < B; ++i) {
+    if (slots[i] < 0 || slots[i] >= c.max_batch || seen[slots[i]])
+      return set_error(NT_ERR_INVALID, "slot %d: slots must be distinct and in 0..%d", slots[i], c.max_batch - 1);
+    if (stream_ids[i] < 0) return set_error(NT_ERR_INVALID, "stream id %d must be >= 0", stream_ids[i]);
+    seen[slots[i]] = 1;
+    args[i] = slots[i], args[B + i] = stream_ids[i];
+  }
+  std::vector<int> lens;
+  int max_len = 0;
+  if ((rc = prefill_stage(lm, cu, B, lens, max_len, stream))) return rc;
+  for (int i = 0; i < B; ++i) args[2 * B + i] = lens[i];
+  NT_CUDA_CHECK(cudaMemcpyAsync(lm->slot_args, args.data(), args.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
+  const int max_pages = c.max_ctx / c.page_size;
+  if ((rc = launch_slots_setup(lm->slot_args, B, st->page_table, max_pages, lm->slot_table, st->seq_lens, st->n_generated, st->done,
+                               lm->slot_key, stream)))
+    return rc;
+  if ((rc = prefill_forward(lm, st, ids, cu, B, max_len, lm->slot_table, logits_out, stream))) return rc;
+  SamplerParams s = make_sampler(lm, st, sp);
+  s.row_slot = lm->slot_args;
+  s.h = nullptr;  // the residual rows are rebuilt below, for every slot
+  if ((rc = run_sampler(lm, s, B, stream))) return rc;
+  return launch_embed_rows(lm->embed, st->cur_token, c.max_batch, c.hidden, lm->h, stream);
 }
 
 // one decode step for slots 0..B-1 (all launches asynchronous, PDL-chained)

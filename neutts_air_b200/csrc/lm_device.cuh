@@ -252,9 +252,9 @@ NT_DEVINL uint32_t processed_key(float logit, int idx, bool mask_eos, int eos_id
 // Sampler stage 1 for one (sequence b, chunk): processors + exact top-64 of a 2048-logit chunk read
 // from global memory.  keys: [kTopChunk] uint32 shared; scratch: [kSelScratch] uint32 shared.
 template <typename Sync>
-NT_DEVINL void sample_stage1_chunk(const SamplerParams& p, int b, int chunk, uint32_t* keys, uint32_t* scratch, Sync sync) {
+NT_DEVINL void sample_stage1_chunk(const SamplerParams& p, int b, int chunk, uint32_t* keys, uint32_t* scratch, Sync sync, int slot = -1) {
   const int tid = threadIdx.x;
-  const int ngen = p.n_generated_override ? __ldcg(p.n_generated_override + b) : __ldcg(p.n_generated + b);
+  const int ngen = p.n_generated_override ? __ldcg(p.n_generated_override + b) : __ldcg(p.n_generated + (slot >= 0 ? slot : b));
   const bool mask_eos = ngen < p.sp.min_new_tokens;
   const float inv_t = 1.0f / p.sp.temperature;
   const float* lg = p.logits + static_cast<long long>(b) * p.V;
@@ -281,11 +281,13 @@ NT_DEVINL void sample_stage1_chunk(const SamplerParams& p, int b, int chunk, uin
 // Tail of the sampler for sequence b, given the k kept candidates sorted (score desc, index asc) in win[0..k):
 // softmax over them (TopK processor + softmax, utils.py:2789), Philox draw, state update, stop flags, and the next
 // token's embedding -> residual stream row (fp32; optionally also as (value, stamp) pairs for the polled hand-off).
-// Clobbers win[kTopKeep .. 2 kTopKeep) (exponentials).
+// Clobbers win[kTopKeep .. 2 kTopKeep) (exponentials).  b: logits row; slot >= 0: the slot whose state row b updates
+// (prefill into chosen slots), else slot b.
 template <typename Sync>
 NT_DEVINL void sample_finish(const SamplerParams& p, int b, int k, Cand* win, int* s_tok, bool stateless, int ngen, bool is_done, Sync sync,
-                             float2* h2dst = nullptr, float h2stamp = 0.f) {
+                             float2* h2dst = nullptr, float h2stamp = 0.f, int slot = -1) {
   const int tid = threadIdx.x;
+  const int s = slot >= 0 ? slot : b;
   float* ev = reinterpret_cast<float*>(win + kTopKeep);   // [kTopKeep] exp(score - max)
   if (tid < 32) {
     const float m = win[0].v;
@@ -303,11 +305,15 @@ NT_DEVINL void sample_finish(const SamplerParams& p, int b, int k, Cand* win, in
     if (tid == 0) {
       int tok;
       if (p.sp.forced && !stateless) {
-        tok = p.sp.forced[static_cast<long long>(b) * p.max_new + ngen];
+        tok = p.sp.forced[static_cast<long long>(s) * p.max_new + ngen];
       } else if (p.sp.greedy) {
         tok = win[0].i;
       } else {
-        uint32_t ctr[4] = {static_cast<uint32_t>(stateless ? p.step_override : ngen), static_cast<uint32_t>(b + p.slot_base), 0u, 0u};
+        // stream key: the slot's own key once a refill set one (-1 otherwise), so a refilled slot does not replay
+        // its previous occupant's draws
+        const int key = p.slot_key ? __ldg(p.slot_key + s) : -1;
+        uint32_t ctr[4] = {static_cast<uint32_t>(stateless ? p.step_override : ngen), static_cast<uint32_t>(key >= 0 ? key : s + p.slot_base),
+                           0u, 0u};
         philox4x32_10(ctr, static_cast<uint32_t>(p.sp.seed), static_cast<uint32_t>(p.sp.seed >> 32));
         const float u = (ctr[0] >> 8) * (1.0f / 16777216.0f);  // [0,1)
         const float target = u * sum;
@@ -324,14 +330,14 @@ NT_DEVINL void sample_finish(const SamplerParams& p, int b, int k, Cand* win, in
       *s_tok = tok;
       if (p.dbg_token) p.dbg_token[b] = tok;
       if (!stateless && !is_done) {
-        p.out_tokens[static_cast<long long>(b) * p.max_new + ngen] = tok;
-        p.n_generated[b] = ngen + 1;
-        p.cur_token[b] = tok;
-        const int cached = __ldcg(p.seq_lens + b) + p.advance;  // decode: this step's input token is now in the KV cache
-        if (p.advance) p.seq_lens[b] = cached;
+        p.out_tokens[static_cast<long long>(s) * p.max_new + ngen] = tok;
+        p.n_generated[s] = ngen + 1;
+        p.cur_token[s] = tok;
+        const int cached = __ldcg(p.seq_lens + s) + p.advance;  // decode: this step's input token is now in the KV cache
+        if (p.advance) p.seq_lens[s] = cached;
         const int total = cached + 1;  // tokens in context once `tok` is appended
-        const int lim = p.sp.limits ? min(p.sp.max_new_tokens, __ldg(p.sp.limits + b)) : p.sp.max_new_tokens;
-        if (tok == p.sp.eos_id || ngen + 1 >= lim || ngen + 1 >= p.max_new || total >= p.max_ctx) p.done[b] = 1;
+        const int lim = p.sp.limits ? min(p.sp.max_new_tokens, __ldg(p.sp.limits + s)) : p.sp.max_new_tokens;
+        if (tok == p.sp.eos_id || ngen + 1 >= lim || ngen + 1 >= p.max_new || total >= p.max_ctx) p.done[s] = 1;
       }
     }
   }
@@ -356,11 +362,12 @@ struct NoMark {
 };
 template <typename Sync, typename Mark = NoMark>
 NT_DEVINL void sample_stage2_seq(const SamplerParams& p, int b, int ncand, uint32_t* keys, uint32_t* scratch, Cand* win, int* s_tok,
-                                 Sync sync, Mark mark = Mark(), long long cand_stride = -1) {
+                                 Sync sync, Mark mark = Mark(), long long cand_stride = -1, int slot = -1) {
   const int tid = threadIdx.x;
   const bool stateless = p.n_generated_override != nullptr;
-  const int ngen = stateless ? __ldcg(p.n_generated_override + b) : __ldcg(p.n_generated + b);
-  const bool is_done = stateless ? false : (__ldcg(p.done + b) != 0);
+  const int s = slot >= 0 ? slot : b;
+  const int ngen = stateless ? __ldcg(p.n_generated_override + b) : __ldcg(p.n_generated + s);
+  const bool is_done = stateless ? false : (__ldcg(p.done + s) != 0);
   // candidate rows: [b * stride, b * stride + ncand); stride = ncand unless the caller's rows have their own pitch
   const long long cstride = cand_stride >= 0 ? cand_stride : static_cast<long long>(ncand);
   const float* cv = p.cand_val + static_cast<long long>(b) * cstride;
@@ -406,7 +413,7 @@ NT_DEVINL void sample_stage2_seq(const SamplerParams& p, int b, int ncand, uint3
   sync();
   mark();  // winners sorted
 
-  sample_finish(p, b, k, win, s_tok, stateless, ngen, is_done, sync);
+  sample_finish(p, b, k, win, s_tok, stateless, ngen, is_done, sync, nullptr, 0.f, slot);
 }
 
 // Sampler of the tile-max schemes, for sequence b, on 256 threads (0..255) of one CTA.  The lm_head epilogue left the
@@ -422,7 +429,7 @@ NT_DEVINL void sample_stage2_seq(const SamplerParams& p, int b, int ncand, uint3
 template <typename Sync, typename Mark>
 NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax, int nt, float tmax_scale, int fix_tile, float fix_val,
                                 const float* logits, int V, bool mask_eos, uint8_t* uni, unsigned uni_bytes, int* sel, Sync sync, Mark pm,
-                                float2* h2dst, float h2stamp) {
+                                float2* h2dst, float h2stamp, int slot = -1) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int H = p.hidden;
   uint32_t* scratch = reinterpret_cast<uint32_t*>(uni);
@@ -435,8 +442,8 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
   const float inv_t = 1.0f / p.sp.temperature;
   const int eos = p.sp.eos_id;
   const bool stateless = false;
-  const int ngen = __ldcg(p.n_generated + b);
-  const bool is_done = __ldcg(p.done + b) != 0;
+  const int ngen = __ldcg(p.n_generated + (slot >= 0 ? slot : b));
+  const bool is_done = __ldcg(p.done + (slot >= 0 ? slot : b)) != 0;
   const float* lg = logits + static_cast<long long>(b) * V;
   auto tile_max = [&](int i) -> float {
     const float v = __ldcg(tmax + static_cast<long long>(b) * nt + i) * tmax_scale;
@@ -552,7 +559,7 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
             }
             sync();
             pm(124);
-            sample_finish(p, b, k2, win, s_tok, stateless, ngen, is_done, sync, h2dst, h2stamp);
+            sample_finish(p, b, k2, win, s_tok, stateless, ngen, is_done, sync, h2dst, h2stamp, slot);
             pm(125);
             return;
           }
@@ -635,7 +642,7 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
       if (rank < k2) win[rank] = me;
     }
     sync();
-    sample_finish(p, b, k2, win, s_tok, stateless, ngen, is_done, sync, h2dst, h2stamp);
+    sample_finish(p, b, k2, win, s_tok, stateless, ngen, is_done, sync, h2dst, h2stamp, slot);
     return;
   }
   // ---- general path (thousands of candidates: tiny vocabularies, or exact ties at the threshold)
@@ -689,7 +696,7 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
     }
   }
   sync();
-  sample_stage2_seq(p, b, ncand, keys, scratch, win, s_tok, sync, NoMark(), kCandPitch);
+  sample_stage2_seq(p, b, ncand, keys, scratch, win, s_tok, sync, NoMark(), kCandPitch, slot);
   if (h2dst) {  // the next token's embedding becomes the residual stream of the next step's first fold
     sync();
     for (int i = tid; i < H; i += kConsumerThreads) h2dst[i] = make_float2(p.h[static_cast<long long>(b) * H + i], h2stamp);

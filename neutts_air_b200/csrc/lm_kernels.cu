@@ -756,7 +756,7 @@ __global__ void __launch_bounds__(kConsumerThreads) topk_stage1_kernel(const Sam
   __shared__ uint32_t scratch[kSelScratch];
   pdl_launch_dependents();
   pdl_wait();
-  sample_stage1_chunk(p, blockIdx.y, blockIdx.x, keys, scratch, SyncAll());
+  sample_stage1_chunk(p, blockIdx.y, blockIdx.x, keys, scratch, SyncAll(), p.row_slot ? __ldg(p.row_slot + blockIdx.y) : -1);
 }
 
 // stage 2: grid (B), 256 threads
@@ -767,7 +767,8 @@ __global__ void __launch_bounds__(kConsumerThreads) topk_stage2_kernel(const Sam
   __shared__ int s_tok;
   pdl_launch_dependents();
   pdl_wait();
-  sample_stage2_seq(p, blockIdx.x, ncand, reinterpret_cast<uint32_t*>(smem_raw), scratch, win, &s_tok, SyncAll());
+  sample_stage2_seq(p, blockIdx.x, ncand, reinterpret_cast<uint32_t*>(smem_raw), scratch, win, &s_tok, SyncAll(), NoMark(), -1,
+                    p.row_slot ? __ldg(p.row_slot + blockIdx.x) : -1);
 }
 
 int launch_sampler_check(const SamplerParams& p) {
@@ -802,7 +803,8 @@ __global__ void __launch_bounds__(kConsumerThreads) topk_tiles_kernel(const Samp
   pdl_launch_dependents();
   pdl_wait();
   const int b = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const bool mask_eos = __ldcg(p.n_generated + b) < p.sp.min_new_tokens;
+  const int slot = p.row_slot ? __ldg(p.row_slot + b) : b;
+  const bool mask_eos = __ldcg(p.n_generated + slot) < p.sp.min_new_tokens;
   const float inv_t = 1.0f / p.sp.temperature;
   int fix_tile = -1;
   float fix_val = 0.f;
@@ -821,7 +823,7 @@ __global__ void __launch_bounds__(kConsumerThreads) topk_tiles_kernel(const Samp
     fix_val = fix;
   }
   sample_tiles_seq(p, b, tmax, nt, inv_t, fix_tile, fix_val, p.logits, p.V, mask_eos, uni, kTilesScratch, sel, SyncAll(), NoMarkI(),
-                   static_cast<float2*>(nullptr), 0.f);
+                   static_cast<float2*>(nullptr), 0.f, slot);
 }
 
 int launch_sampler_tiles(const SamplerParams& p, int B, const float* tmax, int nt, cudaStream_t stream) {
@@ -1154,6 +1156,27 @@ __global__ void gather_rows_kernel(const float* src, const int32_t* rows, int co
 }
 int launch_gather_rows(const float* src, const int32_t* rows, int n, int cols, float* dst, cudaStream_t s) {
   return launch_kernel(gather_rows_kernel, dim3(n), dim3(256), 0, s, true, src, rows, cols, dst);
+}
+
+// one CTA per listed slot: compact page-table row + the slot's fresh length, counters and Philox key
+__global__ void slots_setup_kernel(const int32_t* args, int B, const int32_t* page_table, int max_pages, int32_t* table,
+                                   int32_t* seq_lens, int32_t* n_generated, int32_t* done, int32_t* slot_key) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int i = blockIdx.x, s = args[i];
+  for (int j = threadIdx.x; j < max_pages; j += blockDim.x)
+    table[static_cast<long long>(i) * max_pages + j] = page_table[static_cast<long long>(s) * max_pages + j];
+  if (threadIdx.x == 0) {
+    slot_key[s] = args[B + i];
+    seq_lens[s] = args[2 * B + i];
+    n_generated[s] = 0;
+    done[s] = 0;
+  }
+}
+int launch_slots_setup(const int32_t* args, int B, const int32_t* page_table, int max_pages, int32_t* table, int32_t* seq_lens,
+                       int32_t* n_generated, int32_t* done, int32_t* slot_key, cudaStream_t s) {
+  return launch_kernel(slots_setup_kernel, dim3(B), dim3(128), 0, s, true, args, B, page_table, max_pages, table, seq_lens, n_generated,
+                       done, slot_key);
 }
 
 }  // namespace nt

@@ -90,6 +90,10 @@ struct SamplerParams {
   const int32_t* n_generated_override;  // nt_op_topk_sample: read-only counters, no state update
   int32_t step_override;
   int32_t slot_base;  // global slot index of local sequence 0 (keys the Philox counter)
+  // Prefill into chosen slots: logits row i updates the state of slot row_slot[i] (nullptr: row i is slot i).  Read
+  // by the stand-alone sampler kernels only; the persistent decode kernel samples row b into slot b.
+  const int32_t* row_slot;
+  const int32_t* slot_key;  // optional [max_batch] Philox stream key per slot; -1: slot + slot_base
 };
 int launch_sampler(const SamplerParams& p, int B, cudaStream_t stream);
 int launch_sampler_check(const SamplerParams& p);
@@ -120,5 +124,9 @@ int launch_attn_prefill(const AttnPrefillParams& p, int B, int n_layers, cudaStr
 // one TMA descriptor (box 64 rows x 128 B, SWIZZLE_128B) over the whole paged KV pool viewed as rows of 64 bf16
 int kv_pool_tmap(const KVLayout& kv, int n_layers, ::CUtensorMap_st* out);
 int launch_gather_rows(const float* src, const int32_t* rows, int n, int cols, float* dst, cudaStream_t s);
+// Prefill into chosen slots.  args: device [3][B] = slots, Philox stream keys, prompt lengths.  Gathers the listed
+// slots' page-table rows into table [B][max_pages] and resets those slots' seq_lens / n_generated / done / slot_key.
+int launch_slots_setup(const int32_t* args, int B, const int32_t* page_table, int max_pages, int32_t* table, int32_t* seq_lens,
+                       int32_t* n_generated, int32_t* done, int32_t* slot_key, cudaStream_t s);
 
 }  // namespace nt

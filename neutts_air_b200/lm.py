@@ -210,10 +210,7 @@ class SpeechLM:
             raise ValueError(f"batch {B} not in 1..{self.max_batch}")
         if ids_host.dtype != torch.int32 or ids_host.numel() != sum(lens):
             raise ValueError("ids_host must be int32 with sum(lens) elements")
-        for b in range(self.max_batch):
-            if self._slot_pages[b]:
-                self.pool.release(self._slot_pages[b])
-                self._slot_pages[b] = []
+        self.release_pages()
         table = np.zeros((self.max_batch, self.max_pages), dtype=np.int32)
         for b, n in enumerate(lens):
             if not 1 <= n < self.max_ctx:
@@ -236,6 +233,72 @@ class SpeechLM:
                                             cu.ctypes.data_as(C.POINTER(C.c_int32)), B, C.byref(sp),
                                             logits.data_ptr() if return_logits else None, _lib.current_stream_ptr()))
         self._B = B
+        return logits
+
+    def release_pages(self, slots=None) -> None:
+        """Return the KV pages of ``slots`` (default: every slot) to the pool."""
+        for b in range(self.max_batch) if slots is None else slots:
+            if self._slot_pages[b]:
+                self.pool.release(self._slot_pages[b])
+                self._slot_pages[b] = []
+
+    def prefill_slots(self, slots, prompts, sp, stream_ids, return_logits: bool = False, limits=None):
+        """Prefill ``prompts`` into the listed ``slots`` while every other slot keeps its KV pages, tokens and counters
+        (so its decoding simply continues).  Needs an earlier ``prefill``.  Samples the first token of each listed slot.
+        ``stream_ids``: the Philox stream key of each prompt (>= 0), used for its slot instead of slot + slot_base
+        until the next ``prefill``.  ``limits``: optional cap on generated tokens per prompt, written into the slots'
+        entries of the per-slot limits (``sp`` must come from ``sampling(..., limits=...)``).  Afterwards ``decode``
+        continues every live slot below the widest batch prefilled so far.  Returns the [len(slots), vocab]
+        logits in call order when ``return_logits``."""
+        slots = [int(s) for s in slots]
+        B = len(slots)
+        if B == 0 or B != len(prompts) or B != len(stream_ids):
+            raise ValueError("slots, prompts and stream_ids must be non-empty and of equal length")
+        if len(set(slots)) != B or min(slots) < 0 or max(slots) >= self.max_batch:
+            raise ValueError(f"slots must be distinct and in 0..{self.max_batch - 1}")
+        if getattr(self, "_B", None) is None:
+            raise RuntimeError("prefill_slots needs an earlier prefill")
+        lens = [len(p) for p in prompts]
+        if min(lens) < 1 or max(lens) >= self.max_ctx:
+            raise ValueError(f"prompt lengths must be in 1..{self.max_ctx - 1}")
+        if min(int(s) for s in stream_ids) < 0:
+            raise ValueError("stream ids must be >= 0")
+        caps = [min(int(c), sp.max_new_tokens) for c in limits] if limits is not None else [sp.max_new_tokens] * B
+        if limits is not None and (getattr(self, "limits", None) is None or sp.limits != self.limits.data_ptr()):
+            raise ValueError("per-prompt limits need sampling params built with limits=")
+        flat = np.concatenate([np.asarray(p, dtype=np.int64) for p in prompts])
+        if flat.min() < 0 or flat.max() >= self.shape.vocab_size:
+            raise ValueError("token id out of range")
+        self.release_pages(slots)
+        table = self._table_host.copy()
+        for s, n, cap in zip(slots, lens, caps):
+            need = (min(n + cap, self.max_ctx) + self.PAGE - 1) // self.PAGE
+            pages = self.pool.alloc(need)
+            self._slot_pages[s] = pages
+            table[s] = 0
+            table[s, :need] = pages
+        if getattr(self, "_ids_pinned", None) is None or self._ids_pinned.numel() < flat.size:
+            self._ids_pinned = torch.empty(max(flat.size, self.max_prefill_tokens), dtype=torch.int32).pin_memory()
+        staged = self._ids_pinned[: flat.size]
+        staged.copy_(torch.from_numpy(flat.astype(np.int32)))
+        cu = np.zeros(B + 1, dtype=np.int32)
+        cu[1:] = np.cumsum(lens)
+        slots_h = np.asarray(slots, dtype=np.int32)
+        keys_h = np.asarray([int(k) for k in stream_ids], dtype=np.int32)
+        i32p = C.POINTER(C.c_int32)
+        with torch.cuda.device(self.device):
+            ids = staged.to(self.device, non_blocking=True)
+            self.page_table.copy_(torch.from_numpy(table))   # same stream as the prefill below
+            self._table_host = table
+            if limits is not None:
+                self.limits.index_copy_(0, torch.tensor(slots, device=self.device),
+                                        torch.tensor(caps, dtype=torch.int32, device=self.device))
+            logits = torch.empty(B, self.shape.vocab_size, dtype=torch.float32, device=self.device) if return_logits else None
+            _lib.check(self.L.nt_lm_prefill_slots(self.handle, C.byref(self.state), slots_h.ctypes.data_as(i32p),
+                                                  keys_h.ctypes.data_as(i32p), ids.data_ptr(), cu.ctypes.data_as(i32p), B,
+                                                  C.byref(sp), logits.data_ptr() if return_logits else None,
+                                                  _lib.current_stream_ptr()))
+        self._B = max(self._B, max(slots) + 1)
         return logits
 
     def decode(self, n_steps: int, sp, return_logits: bool = False):
@@ -268,12 +331,21 @@ class SpeechLM:
         return self.workspace[off: off + n].view(dtype).view(*shape)
 
     # ------------------------------------------------------------------ generation
+    def _caps(self, lens, max_length: int, max_new_tokens) -> list:
+        """Generated-token cap per prompt; ``max_new_tokens``: None, one int, or one int per prompt."""
+        if max_new_tokens is None or isinstance(max_new_tokens, int):
+            max_new_tokens = [max_new_tokens or max_length] * len(lens)
+        if len(max_new_tokens) != len(lens):
+            raise ValueError("max_new_tokens needs one entry per prompt")
+        return [min(max_length - n, int(m), self.max_new) for n, m in zip(lens, max_new_tokens)]
+
     def generate_batch(self, prompts, eos_token_id: int, max_length: int | None = None, min_new_tokens: int = 50,
                        temperature: float = 1.0, top_k: int = 50, max_new_tokens: int | None = None, seed: int = 0,
                        greedy: bool = False, forced: torch.Tensor | None = None, check_every: int = 64, slot_base: int = 0):
         """Returns a list of int64 CPU tensors with the generated ids of each prompt (EOS included
         when it was sampled), following transformers' stopping rules (stopping_criteria.py:73-84,
-        467-471): stop at EOS or when prompt + generated reaches max_length."""
+        467-471): stop at EOS or when prompt + generated reaches max_length.  ``max_new_tokens`` may also be a
+        list with one cap per prompt."""
         max_length = max_length or self.max_ctx
         if max_length > self.max_ctx:
             raise ValueError(f"max_length {max_length} exceeds the engine context {self.max_ctx}")
@@ -282,7 +354,7 @@ class SpeechLM:
             raise ValueError("prompt already at max_length")
         # max_length counts prompt + generated PER SEQUENCE (stopping_criteria.py:73-84): a long prompt in the batch
         # must not shorten its neighbours, so every slot gets its own cap and the loop runs to the largest one
-        caps = [min(max_length - n, max_new_tokens or max_length, self.max_new) for n in lens]
+        caps = self._caps(lens, max_length, max_new_tokens)
         limit = max(caps)
         sp = self.sampling(eos_token_id, min_new_tokens, limit, top_k, temperature, seed, greedy, forced,
                            limits=caps if min(caps) < limit else None, slot_base=slot_base)
@@ -298,6 +370,72 @@ class SpeechLM:
         ngen = self.n_generated[:B].cpu()
         toks = self.out_tokens[:B].cpu()
         return [toks[b, : int(ngen[b])].long() for b in range(B)]
+
+    def generate_queue(self, prompts, eos_token_id: int, max_length: int | None = None, min_new_tokens: int = 50,
+                       temperature: float = 1.0, top_k: int = 50, max_new_tokens: int | None = None, seed: int = 0,
+                       greedy: bool = False, check_every: int = 32, slot_base: int = 0):
+        """Continuous batching over any number of prompts: ``generate_batch``'s results and stopping rules, but a slot
+        whose sequence finished is refilled with the next waiting prompt while the other slots keep decoding.
+
+        Prompts are admitted FIFO into ``min(len(prompts), max_batch)`` slots; prompt i draws from Philox stream
+        ``slot_base + i``, the stream the chunked loop (``generate_batch`` per ``max_batch`` prompts with
+        ``slot_base`` = the chunk's first index) gives it.  Decoding runs in launches of at most ``check_every``
+        steps, each cut short so that it ends with the earliest cap-driven completion while prompts wait.  After each
+        launch one small read of (n_generated, done) finds the finished slots; their tokens are copied out and the next
+        prompts go into all freed slots with one ``prefill_slots`` call.  Returns the generated ids per prompt (int64
+        CPU tensors, EOS included when sampled) in input order; every KV page is back in the pool afterwards."""
+        max_length = max_length or self.max_ctx
+        if max_length > self.max_ctx:
+            raise ValueError(f"max_length {max_length} exceeds the engine context {self.max_ctx}")
+        n = len(prompts)
+        if n == 0:
+            return []
+        if check_every < 1:
+            raise ValueError("check_every must be >= 1")
+        lens = [len(p) for p in prompts]
+        if min(max_length - m for m in lens) < 1:
+            raise ValueError("prompt already at max_length")
+        caps = self._caps(lens, max_length, max_new_tokens)
+        S = min(n, self.max_batch)
+        sp = self.sampling(eos_token_id, min_new_tokens, max(caps), top_k, temperature, seed, greedy,
+                           limits=caps[:S], slot_base=slot_base)
+        self.prefill([prompts[i] for i in range(S)], sp)
+        occ = list(range(S))   # prompt held by each slot, None once harvested
+        ngen = [1] * S         # generated tokens per slot, as of the last read
+        nxt = S                # next prompt to admit
+        out = [None] * n
+        # a sequence can finish inside its prefill: a cap of 1, or EOS when it is not masked at step 0
+        at_prefill = lambda idx: min_new_tokens <= 0 or min(caps[i] for i in idx) <= 1
+        read = at_prefill(range(S))
+        while True:
+            if read:
+                st = torch.stack((self.n_generated[:S], self.done[:S])).cpu()   # the one small D2H read per launch
+                ngen = st[0].tolist()
+                fin = [s for s in range(S) if occ[s] is not None and int(st[1, s])]
+                if fin:
+                    rows = self.out_tokens[fin].cpu()
+                    for r, s in enumerate(fin):
+                        out[occ[s]] = rows[r, : ngen[s]].long()
+                        occ[s] = None
+                    take = fin[: n - nxt]
+                    if take:
+                        idx = list(range(nxt, nxt + len(take)))
+                        nxt += len(take)
+                        self.prefill_slots(take, [prompts[i] for i in idx], sp, [slot_base + i for i in idx],
+                                           limits=[caps[i] for i in idx])
+                        for s, i in zip(take, idx):
+                            occ[s], ngen[s] = i, 1
+                        if at_prefill(idx):
+                            continue   # read again before decoding: a newcomer may be done already
+            live = [s for s in range(S) if occ[s] is not None]
+            if not live:
+                break
+            left = [caps[occ[s]] - ngen[s] for s in live]
+            steps = max(1, min(check_every, min(left) if nxt < n else max(left)))
+            self.decode(steps, sp)
+            read = True
+        self.release_pages()
+        return out
 
     @torch.no_grad()
     def generate(self, input_ids: torch.Tensor, max_length: int = 2048, eos_token_id: int | None = None,
