@@ -173,7 +173,7 @@ int nt_lm_head_gemv(nt_lm* lm, const float* h, int B, float* logits, void* strea
 
 /* Per-stage parity hooks (tests): run only the first n_layers layers (-1 = all), and look up an
  * internal activation buffer by name ("h", "q", "qkv", "attn", "act", "logits", "xn", "attn_bf16",
- * "act_bf16", "h_last"); the pointer lies inside the caller's workspace. */
+ * "act_bf16", "h_last", "tmax"); the pointer lies inside the caller's workspace. */
 int nt_lm_debug_set_layers(nt_lm* lm, int n_layers);
 /* launch-latency probe: n dependent trivial kernels (grid x block) each incrementing *counter */
 int nt_debug_launch_chain(int n, int grid, int block, int* counter, void* stream);
@@ -181,6 +181,13 @@ void* nt_lm_debug_ptr(nt_lm* lm, const char* name);
 /* persistent decode kernel timeline: buf = device int64 [2][1024] receiving %globaltimer marks of decode
  * step `step` from CTAs 0 and 1 (NULL disables) */
 int nt_lm_debug_set_profile(nt_lm* lm, long long* buf, int step);
+/* sampler window capture (tests): caller-owned device buffers topk_val fp32 [max_batch][64], topk_idx int32
+ * [max_batch][64] and token int32 [max_batch] receive, per logits row, the kept probabilities, the kept ids (-1
+ * padded) and the selected token of every sampler launch (prefill, prefill into slots, decode chain, persistent
+ * decode kernel).  Row b is logits row b: call order in nt_lm_prefill_slots.  Each launch overwrites them, so a
+ * multi-step persistent decode launch leaves its last step.  NULL pointers switch the capture off.  Debug "tmax"
+ * (nt_lm_debug_ptr) holds the per-128-column tile maxima of the last tile-max sampler input. */
+int nt_lm_debug_capture_sampler(nt_lm* lm, float* topk_val, int32_t* topk_idx, int32_t* token);
 
 /* ------------------------------------------------------------------------------------------
  * NeuCodec decoder (seam 2)

@@ -90,7 +90,8 @@ EXPORTS = [
     "nt_last_error", "nt_abi_version", "nt_launch_count", "nt_gemm",
     "nt_lm_workspace_bytes", "nt_lm_create", "nt_lm_destroy", "nt_lm_prefill", "nt_lm_prefill_slots", "nt_lm_decode",
     "nt_lm_head_gemv",
-    "nt_lm_debug_set_layers", "nt_lm_debug_ptr", "nt_lm_debug_set_profile", "nt_debug_launch_chain",
+    "nt_lm_debug_set_layers", "nt_lm_debug_ptr", "nt_lm_debug_set_profile", "nt_lm_debug_capture_sampler",
+    "nt_debug_launch_chain",
     "nt_codec_workspace_bytes", "nt_codec_create", "nt_codec_destroy", "nt_codec_decode",
     "nt_op_rmsnorm", "nt_op_topk_sample",
 ]
@@ -129,6 +130,7 @@ def lib() -> C.CDLL:
     L.nt_lm_debug_ptr.restype = C.c_void_p
     L.nt_lm_debug_ptr.argtypes = [C.c_void_p, C.c_char_p]
     L.nt_lm_debug_set_profile.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+    L.nt_lm_debug_capture_sampler.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.nt_debug_launch_chain.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     L.nt_codec_workspace_bytes.restype = C.c_size_t
     L.nt_codec_workspace_bytes.argtypes = [C.POINTER(CodecConfig)]

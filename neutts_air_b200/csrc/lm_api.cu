@@ -100,6 +100,9 @@ struct nt_lm {
   int debug_layers = -1;              // >= 0: run only this many layers (per-stage parity tests)
   long long* prof = nullptr;          // persistent decode kernel timeline buffer
   int prof_step = 0;
+  // sampler window capture (nt_lm_debug_capture_sampler): copied into every SamplerParams, nullptr = off
+  float* dbg_topk_val = nullptr;
+  int32_t *dbg_topk_idx = nullptr, *dbg_token = nullptr;
   // persistent wgmma decode kernel (lm_decode_tc.cu): plan, tensor maps and buffers live in the workspace
   bool tc_ok = false, tc_flat_ok = false;
   TcPlanInfo tc_info[2] = {};         // [0]: whole-K gate/up plan (any batch), [1]: flat plan (batch <= 4)
@@ -346,6 +349,7 @@ static SamplerParams make_sampler(const nt_lm* lm, const nt_lm_state* st, const 
   s.hidden = lm->cfg.hidden;
   s.slot_base = sp->slot_base;
   s.slot_key = lm->slot_key;
+  s.dbg_topk_val = lm->dbg_topk_val, s.dbg_topk_idx = lm->dbg_topk_idx, s.dbg_token = lm->dbg_token;
   return s;
 }
 
@@ -750,11 +754,24 @@ extern "C" int nt_lm_debug_set_profile(nt_lm* lm, long long* buf, int step) {
   lm->prof_step = step;
   return NT_OK;
 }
+extern "C" int nt_lm_debug_capture_sampler(nt_lm* lm, float* topk_val, int32_t* topk_idx, int32_t* token) {
+  if (!lm) return set_error(NT_ERR_INVALID, "nt_lm_debug_capture_sampler: null handle");
+  if (!topk_val != !topk_idx || !topk_val != !token)
+    return set_error(NT_ERR_INVALID, "nt_lm_debug_capture_sampler: pass all three buffers or none");
+  lm->dbg_topk_val = topk_val, lm->dbg_topk_idx = topk_idx, lm->dbg_token = token;
+  // the cached decode graph baked the previous pointers into its sampler node (the graph key does not see them)
+  if (lm->graph) {
+    cudaGraphExecDestroy(lm->graph);
+    lm->graph = nullptr;
+  }
+  return NT_OK;
+}
 extern "C" void* nt_lm_debug_ptr(nt_lm* lm, const char* name) {
   if (!lm || !name) return nullptr;
   const struct { const char* n; void* p; } tab[] = {
       {"h", lm->h}, {"q", lm->q}, {"qkv", lm->qkv}, {"attn", lm->attn}, {"act", lm->act}, {"logits", lm->logits},
-      {"xn", lm->xn}, {"attn_bf16", lm->attn_bf16}, {"act_bf16", lm->act_bf16}, {"h_last", lm->h_last}};
+      {"xn", lm->xn}, {"attn_bf16", lm->attn_bf16}, {"act_bf16", lm->act_bf16}, {"h_last", lm->h_last},
+      {"tmax", lm->tc_tmax}};
   for (const auto& e : tab)
     if (!strcmp(e.n, name)) return e.p;
   return nullptr;

@@ -445,6 +445,8 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
   const int ngen = __ldcg(p.n_generated + (slot >= 0 ? slot : b));
   const bool is_done = __ldcg(p.done + (slot >= 0 ? slot : b)) != 0;
   const float* lg = logits + static_cast<long long>(b) * V;
+  // row b starts b * V floats in: with V % 4 != 0 only some rows are 16-byte aligned for the float4 loads (CTA-uniform)
+  const bool vec4 = (reinterpret_cast<uintptr_t>(lg) & 15) == 0;
   auto tile_max = [&](int i) -> float {
     const float v = __ldcg(tmax + static_cast<long long>(b) * nt + i) * tmax_scale;
     return i == fix_tile ? fix_val : v;
@@ -517,12 +519,13 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
               x[u] = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
               if (tile[u] >= 0) {
                 const int r0 = tile[u] * 128 + lane * 4;
-                if (r0 + 3 < V) {
+                if (vec4 && r0 + 3 < V) {
                   x[u] = __ldcg(reinterpret_cast<const float4*>(lg + r0));
                 } else {
                   if (r0 < V) x[u].x = __ldcg(lg + r0);
                   if (r0 + 1 < V) x[u].y = __ldcg(lg + r0 + 1);
                   if (r0 + 2 < V) x[u].z = __ldcg(lg + r0 + 2);
+                  if (r0 + 3 < V) x[u].w = __ldcg(lg + r0 + 3);
                 }
               }
             }
@@ -583,12 +586,13 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
   auto tile_keys = [&](int tile, uint32_t (&kk)[4]) {   // this lane's 4 logits of the tile -> processed keys
     const int r0 = tile * 128 + lane * 4;
     float4 x = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
-    if (r0 + 3 < V) {
+    if (vec4 && r0 + 3 < V) {
       x = __ldcg(reinterpret_cast<const float4*>(lg + r0));
     } else {
       if (r0 < V) x.x = __ldcg(lg + r0);
       if (r0 + 1 < V) x.y = __ldcg(lg + r0 + 1);
       if (r0 + 2 < V) x.z = __ldcg(lg + r0 + 2);
+      if (r0 + 3 < V) x.w = __ldcg(lg + r0 + 3);
     }
     kk[0] = (r0 < V) ? processed_key(x.x, r0, mask_eos, eos, inv_t) : 0u;
     kk[1] = (r0 + 1 < V) ? processed_key(x.y, r0 + 1, mask_eos, eos, inv_t) : 0u;
@@ -646,6 +650,18 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
     return;
   }
   // ---- general path (thousands of candidates: tiny vocabularies, or exact ties at the threshold)
+  // Stage 2 keeps the first of the candidates tied at its threshold by position, so the candidate arrays list them in
+  // id order (smaller id wins, as on every other path): chosen tiles by index, each tile's candidates in id order.
+  {
+    int me = -1, r = 0;
+    if (tid < k) {
+      me = tiles[tid];
+      for (int j = 0; j < k; ++j) r += tiles[j] < me ? 1 : 0;
+    }
+    sync();
+    if (tid < k) tiles[r] = me;
+    sync();
+  }
   // pass 1: candidates (key >= threshold) per chosen tile
   for (int j = warp; j < k; j += kConsumerWarps) {
     uint32_t kk[4];
@@ -680,19 +696,29 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
     uint32_t kk[4];
     const int tile = tiles[j];
     tile_keys(tile, kk);
-    int base = counts[j];
+    bool hit[4];
+    int c = 0;
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
-      const bool hit = kk[q] >= cthr && kk[q] != 0u;
-      const uint32_t m = __ballot_sync(0xffffffffu, hit);
-      if (hit) {
-        const int o = base + __popc(m & ((1u << lane) - 1u));
+      hit[q] = kk[q] >= cthr && kk[q] != 0u;
+      c += hit[q] ? 1 : 0;
+    }
+    int incl = c;   // lane prefix: lane l's candidates follow those of lanes < l (ids tile * 128 + 4 l + q)
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, incl, off);
+      if (lane >= off) incl += t;
+    }
+    int o = counts[j] + incl - c;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      if (hit[q]) {
         if (o < ncand) {
           cv[o] = key2f(kk[q]);
           ci[o] = tile * 128 + lane * 4 + q;
         }
+        ++o;
       }
-      base += __popc(m);
     }
   }
   sync();

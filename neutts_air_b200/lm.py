@@ -330,6 +330,21 @@ class SpeechLM:
         n = int(np.prod(shape)) * torch.empty(0, dtype=dtype).element_size()
         return self.workspace[off: off + n].view(dtype).view(*shape)
 
+    def debug_capture_sampler(self, on: bool = True):
+        """Every later sampler launch writes, per logits row, its kept window (probabilities [64] fp32, ids [64] int32,
+        -1 padded) and the token it selected into buffers owned here; returns them as (topk_val, topk_idx, token), or
+        None when ``on`` is False (capture off).  Each launch overwrites the rows it samples."""
+        if not on:
+            _lib.check(self.L.nt_lm_debug_capture_sampler(self.handle, None, None, None))
+            self._capture = None
+            return None
+        B = self.max_batch
+        self._capture = (torch.zeros(B, 64, dtype=torch.float32, device=self.device),
+                         torch.full((B, 64), -2, dtype=torch.int32, device=self.device),
+                         torch.full((B,), -2, dtype=torch.int32, device=self.device))
+        _lib.check(self.L.nt_lm_debug_capture_sampler(self.handle, *(t.data_ptr() for t in self._capture)))
+        return self._capture
+
     # ------------------------------------------------------------------ generation
     def _caps(self, lens, max_length: int, max_new_tokens) -> list:
         """Generated-token cap per prompt; ``max_new_tokens``: None, one int, or one int per prompt."""
