@@ -167,6 +167,27 @@ int nt_lm_prefill_slots(nt_lm* lm, const nt_lm_state* st, const int32_t* slots_h
 int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps, const nt_sampling* sp, float* logits_out,
                  void* stream);
 
+/* Per-slot sampling controls, applied in transformers' processor order (generation/utils.py, logits_process.py):
+ * EOS mask -> logit * (1.0f / temperature) -> top_k (exactly k, the smaller id wins ties) -> top_p -> min_p ->
+ * softmax over what is left -> one multinomial draw with the same Philox counter as without the controls.
+ * top_p and min_p act on the window sorted by (score desc, id asc) with its fp32 softmax q: entry j stays iff
+ * sum_{i<j} q_i < top_p (entry 0 always stays) and q_j >= min_p * q_0.  top_p = 1 and min_p = 0 cut nothing. */
+typedef struct {
+  float temperature;  /* finite, > 0 */
+  int32_t top_k;      /* 1..64 */
+  float top_p;        /* (0, 1] */
+  float min_p;        /* [0, 1) */
+} nt_slot_sampling;
+
+/* host_table: host array of max_batch entries, row s for slot s; NULL switches the table off, and then
+ * nt_sampling.temperature / top_k govern every slot with top-p and min-p off.  While the table is on, its
+ * temperature and top_k replace nt_sampling's for every sampler launch of nt_lm_prefill, nt_lm_prefill_slots and
+ * nt_lm_decode (nt_sampling's own values are still validated); greedy and teacher-forced runs ignore it.  The copy
+ * is enqueued on `stream`, so it is ordered before the next prefill or decode on that stream.  Every entry is
+ * validated first; a bad one returns NT_ERR_INVALID and leaves the previous table in force.
+ * nt_op_topk_sample does not read the table: it takes nt_sampling's scalars only. */
+int nt_lm_set_slot_sampling(nt_lm* lm, const nt_slot_sampling* host_table, void* stream);
+
 /* Timed single-kernel entry for the roofline measurement: the lm_head GEMV (+ final RMSNorm)
  * exactly as the decode step launches it.  h: f32 [B][hidden] -> logits f32 [B][vocab]. */
 int nt_lm_head_gemv(nt_lm* lm, const float* h, int B, float* logits, void* stream);
@@ -242,6 +263,7 @@ int nt_codec_decode(nt_codec* c, const int32_t* codes, int B, int N, float* pcm,
  * ------------------------------------------------------------------------------------------ */
 int nt_op_rmsnorm(const float* x, const float* w, float eps, int rows, int cols, float* out_f32, void* out_bf16,
                   void* stream);
+/* scalar controls only (nt_sampling's temperature and top_k for every row; no per-slot table, no top-p / min-p) */
 int nt_op_topk_sample(const float* logits, int B, int V, const nt_sampling* sp, const int32_t* n_generated,
                       int32_t step, int32_t* out_token, float* out_topk_val, int32_t* out_topk_idx, void* workspace,
                       size_t workspace_bytes, void* stream);

@@ -29,6 +29,32 @@ import torch
 
 SPEECH_RE = re.compile(r"<\|speech_(\d+)\|>")
 CHAT = "user: Convert the text to speech:<|TEXT_REPLACE|>\nassistant:<|SPEECH_REPLACE|>"
+CONTROL_DEFAULTS = dict(temperature=1.0, top_k=50, top_p=1.0, min_p=0.0)   # the reference's (neutts/neutts.py:338-347)
+
+
+def _controls(n: int, temperature, top_k, top_p, min_p) -> dict:
+    """Sampling controls of n utterances: each a scalar or one value per utterance (a list then)."""
+    ctl = {}
+    for name, v in (("temperature", temperature), ("top_k", top_k), ("top_p", top_p), ("min_p", min_p)):
+        if isinstance(v, (list, tuple, np.ndarray, torch.Tensor)):
+            v = [x.item() if hasattr(x, "item") else x for x in v]
+            if len(v) != n:
+                raise ValueError(f"{name} needs one value per utterance ({n}), got {len(v)}")
+        ctl[name] = v
+    return ctl
+
+
+def _pick(ctl: dict, idx) -> dict:
+    """The controls of the utterances ``idx`` (lists are indexed, scalars stay)."""
+    return {k: [v[i] for i in idx] if isinstance(v, list) else v for k, v in ctl.items()}
+
+
+def _backbone_kw(ctl: dict) -> dict:
+    """generate kwargs: temperature and top_k always (as the reference passes them), top_p / min_p only when they are
+    in use, so that backbones without them keep working."""
+    kw = dict(temperature=ctl["temperature"], top_k=ctl["top_k"])
+    kw.update({k: ctl[k] for k in ("top_p", "min_p") if isinstance(ctl[k], list) or ctl[k] != CONTROL_DEFAULTS[k]})
+    return kw
 
 
 class _CrossFade:
@@ -181,27 +207,28 @@ class NeuTTS:
 
     # ------------------------------------------------------------------ hot path A
     def _generate_ids(self, prompts: Sequence[Sequence[int]], max_new_tokens: int | None = None,
-                      min_new_tokens: int = 50, slot_base: int = 0) -> list:
+                      min_new_tokens: int = 50, slot_base: int = 0, ctl: dict | None = None) -> list:
         """Batched device-side generation; returns generated token ids per prompt (CPU int64 tensors).
-        Sampling parameters are the reference's (``neutts/neutts.py:338-347``)."""
+        Sampling parameters default to the reference's (``neutts/neutts.py:338-347``); ``ctl`` (see ``_controls``)
+        overrides them, per prompt where a control is a list."""
         eos = self._tok_id("<|SPEECH_GENERATION_END|>")
         seed = self.seed if self.seed is not None else int(torch.randint(0, 2**31 - 1, (1,)).item())
+        kw = _backbone_kw(ctl if ctl is not None else CONTROL_DEFAULTS)
         if len(prompts) > self.max_batch and hasattr(self.backbone, "generate_queue"):
             # more prompts than slots: refill each slot as soon as its utterance ends (prompt i keeps the Philox
             # stream slot_base + i that the chunked loop gives it)
             return self.backbone.generate_queue(list(prompts), eos, max_length=self.max_context, min_new_tokens=min_new_tokens,
-                                                temperature=1.0, top_k=50, max_new_tokens=max_new_tokens, seed=seed,
-                                                slot_base=slot_base)
+                                                max_new_tokens=max_new_tokens, seed=seed, slot_base=slot_base, **kw)
         if hasattr(self.backbone, "generate_batch"):
             return self.backbone.generate_batch(list(prompts), eos, max_length=self.max_context, min_new_tokens=min_new_tokens,
-                                                temperature=1.0, top_k=50, max_new_tokens=max_new_tokens, seed=seed,
-                                                slot_base=slot_base)
+                                                max_new_tokens=max_new_tokens, seed=seed, slot_base=slot_base, **kw)
         outs = []  # injected transformers-style backbone: one sequence at a time, as the reference does
-        for p in prompts:
+        for i, p in enumerate(prompts):
             t = torch.tensor(list(p)).unsqueeze(0).to(self.backbone.device)
+            one = {k: v[i] if isinstance(v, list) else v for k, v in kw.items()}
             with torch.no_grad():
-                o = self.backbone.generate(t, max_length=self.max_context, eos_token_id=eos, do_sample=True, temperature=1.0,
-                                           top_k=50, use_cache=True, min_new_tokens=min_new_tokens)
+                o = self.backbone.generate(t, max_length=self.max_context, eos_token_id=eos, do_sample=True, use_cache=True,
+                                           min_new_tokens=min_new_tokens, **one)
             outs.append(o[0, t.shape[-1]:].cpu().long())
         return outs
 
@@ -259,19 +286,26 @@ class NeuTTS:
         return wav if self.watermarker is None else self.watermarker.apply_watermark(wav, sample_rate=24_000)
 
     # ------------------------------------------------------------------ public API
-    def infer(self, text: str, ref_codes, ref_text: str) -> np.ndarray:
-        """Text + reference voice -> 24 kHz float32 waveform (``neutts/neutts.py:216-243``)."""
-        return self.infer_batch([text], [ref_codes], [ref_text])[0]
+    def infer(self, text: str, ref_codes, ref_text: str, *, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0,
+              min_p: float = 0.0) -> np.ndarray:
+        """Text + reference voice -> 24 kHz float32 waveform (``neutts/neutts.py:216-243``).  The sampling controls
+        default to the reference's values; see ``infer_batch``."""
+        return self.infer_batch([text], [ref_codes], [ref_text], temperature=temperature, top_k=top_k, top_p=top_p,
+                                min_p=min_p)[0]
 
     def infer_from_prompt_ids(self, prompts: Sequence[Sequence[int]], max_new_tokens: int | None = None,
-                              min_new_tokens: int = 50, slot_base: int = 0) -> list:
+                              min_new_tokens: int = 50, slot_base: int = 0, *, temperature=1.0, top_k=50, top_p=1.0,
+                              min_p=0.0) -> list:
         """Hot path only: prompt ids (host) -> waveforms (host).  Used by bench.py's end-to-end leg.
         ``slot_base`` offsets the sampler's Philox slot index so chunks / ranks under one seed draw independently.
-        More prompts than ``max_batch`` go through the backbone's ``generate_queue`` when it has one."""
-        gen = self._generate_ids(prompts, max_new_tokens, min_new_tokens, slot_base)
+        More prompts than ``max_batch`` go through the backbone's ``generate_queue`` when it has one.  Sampling
+        controls as in ``infer_batch``."""
+        ctl = _controls(len(prompts), temperature, top_k, top_p, min_p)
+        gen = self._generate_ids(prompts, max_new_tokens, min_new_tokens, slot_base, ctl)
         return [self._watermark(w) for w in self._decode_codes([self._ids_to_codes(g) for g in gen])]
 
-    def infer_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], distributed: bool = False) -> list:
+    def infer_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], distributed: bool = False, *,
+                    temperature=1.0, top_k=50, top_p=1.0, min_p=0.0) -> list:
         """List in / list out.  With ``distributed=True`` (inside an initialised torch.distributed job) the
         utterances are sharded over ranks and every rank returns all waveforms (one all-gather).
 
@@ -279,17 +313,27 @@ class NeuTTS:
         ``generate_queue``: a slot whose utterance ended takes the next one while the others keep decoding, so a
         short utterance does not hold its slot until the longest of its chunk ends.  Utterance i keeps the random
         stream it has in the chunked schedule.  Shorter lists, and backbones without ``generate_queue``, run in
-        chunks of ``max_batch``.  The codec then decodes the finished code lists either way."""
+        chunks of ``max_batch``.  The codec then decodes the finished code lists either way.
+
+        Sampling controls (keyword-only; the defaults are the reference's): ``temperature`` (logits times 1 / T),
+        ``top_k`` (1..64), ``top_p`` (nucleus, (0, 1]) and ``min_p`` ([0, 1)), applied in transformers' order.  Each
+        is a scalar or a list with one value per utterance; a list follows its utterances through chunking, the queue
+        and the sharding over ranks."""
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
+        ctl = _controls(len(texts), temperature, top_k, top_p, min_p)
         prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(texts, ref_codes, ref_texts)]
         queue = hasattr(self.backbone, "generate_queue")
+
+        def run(idx, slot_base):
+            return self.infer_from_prompt_ids([prompts[i] for i in idx], slot_base=slot_base, **_pick(ctl, idx))
+
         if not distributed:
             if queue and len(prompts) > self.max_batch:
-                return self.infer_from_prompt_ids(prompts, slot_base=0)
+                return run(range(len(prompts)), 0)
             out = []
             for j in range(0, len(prompts), self.max_batch):
-                out += self.infer_from_prompt_ids(prompts[j: j + self.max_batch], slot_base=j)
+                out += run(range(j, min(j + self.max_batch, len(prompts))), j)
             return out
         from neutts_air_b200 import dist
 
@@ -297,22 +341,26 @@ class NeuTTS:
         local = []
         rank = dist.world()[0]
         if queue and len(mine) > self.max_batch:
-            local = self.infer_from_prompt_ids([prompts[i] for i in mine], slot_base=rank << 20)
+            local = run(mine, rank << 20)
             return dist.all_gather_waveforms(local, mine, len(prompts), device=self.codec.device)
         for j in range(0, len(mine), self.max_batch):
-            local += self.infer_from_prompt_ids([prompts[i] for i in mine[j: j + self.max_batch]], slot_base=(rank << 20) + j)
+            local += run(mine[j: j + self.max_batch], (rank << 20) + j)
         return dist.all_gather_waveforms(local, mine, len(prompts), device=self.codec.device)
 
-    def infer_stream(self, text: str, ref_codes, ref_text: str) -> Generator[np.ndarray, None, None]:
+    def infer_stream(self, text: str, ref_codes, ref_text: str, *, temperature: float = 1.0, top_k: int = 50,
+                     top_p: float = 1.0, min_p: float = 0.0) -> Generator[np.ndarray, None, None]:
         """Streaming synthesis with the reference's window geometry (``neutts/neutts.py:373-465``):
         every 25 new frames (once 5 look-ahead frames exist) the codec re-decodes
-        [n - 50 - 1, n + 25 + 5 + 1) and the chunk is cross-faded with triangular weights."""
+        [n - 50 - 1, n + 25 + 5 + 1) and the chunk is cross-faded with triangular weights.  Sampling controls as in
+        ``infer_batch``."""
         if self._is_quantized_model:  # kept for signature parity; never true on this build
             raise NotImplementedError("GGUF streaming is not part of the H100 build")
+        ctl = _controls(1, temperature, top_k, top_p, min_p)
         prompt = self._apply_chat_template(ref_codes, ref_text, text)
-        return self._stream(prompt, [int(c) for c in (ref_codes.tolist() if hasattr(ref_codes, "tolist") else ref_codes)])
+        return self._stream(prompt, [int(c) for c in (ref_codes.tolist() if hasattr(ref_codes, "tolist") else ref_codes)], ctl)
 
-    def infer_stream_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str]) -> Generator[list, None, None]:
+    def infer_stream_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], *, temperature=1.0,
+                           top_k=50, top_p=1.0, min_p=0.0) -> Generator[list, None, None]:
         """Streaming synthesis of up to ``max_batch`` utterances at once (BASELINE.json configs[4]; the reference
         streams one utterance, ``neutts/neutts.py:373-465``).  Every yield is a list with one entry per utterance:
         the next audio chunk (float32, cross-faded exactly as in ``infer_stream``) or ``None`` when that utterance
@@ -320,16 +368,17 @@ class NeuTTS:
         that are due are gathered on the device from the code history and go through the codec as one batch."""
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
+        ctl = _controls(len(texts), temperature, top_k, top_p, min_p)
         prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(texts, ref_codes, ref_texts)]
         refs = [[int(c) for c in (rc.tolist() if hasattr(rc, "tolist") else rc)] for rc in ref_codes]
-        return self._stream_batch(prompts, refs)
+        return self._stream_batch(prompts, refs, ctl)
 
-    def _stream(self, prompt, ref_codes) -> Generator[np.ndarray, None, None]:
-        for out in self._stream_batch([prompt], [list(ref_codes)]):
+    def _stream(self, prompt, ref_codes, ctl: dict | None = None) -> Generator[np.ndarray, None, None]:
+        for out in self._stream_batch([prompt], [list(ref_codes)], ctl):
             if out[0] is not None:
                 yield out[0]
 
-    def _stream_batch(self, prompts, refs) -> Generator[list, None, None]:
+    def _stream_batch(self, prompts, refs, ctl: dict | None = None) -> Generator[list, None, None]:
         """Window geometry of the reference (``neutts/neutts.py:87-91,401-421,443-465``): once F + LA undecoded frames
         exist, the codec decodes [n_dec - LB - OV, n_dec + F + LA) and the slice [n_dec - OV, n_dec + F + OV) is
         cross-faded at stride F * hop; a ragged tail closes the stream.  ``streaming_frames_per_chunk`` may be set to
@@ -350,7 +399,14 @@ class NeuTTS:
         if min(limits) < 1:
             raise ValueError("prompt already at max_length")
         limit = max(limits)
-        sp = lm.sampling(eos, 50, limit, 50, 1.0, seed) if min(limits) == limit else lm.sampling(eos, 50, limit, 50, 1.0, seed, limits=limits)
+        from neutts_air_b200.lm import per_prompt_controls
+
+        ctl = ctl if ctl is not None else CONTROL_DEFAULTS
+        rows = per_prompt_controls(B, **ctl)   # None: scalar controls without top-p / min-p
+        top_k, temp = (ctl["top_k"], ctl["temperature"]) if rows is None else (rows[0][1], rows[0][0])
+        sp = lm.sampling(eos, 50, limit, top_k, temp, seed) if min(limits) == limit else lm.sampling(eos, 50, limit, top_k, temp, seed, limits=limits)
+        if rows is not None or getattr(lm, "_slot_sp_host", None) is not None:
+            lm.set_slot_sampling(rows)   # before the prefill, on the same stream
         dev = lm.out_tokens.device
         cap = max(len(r) for r in refs) + limit
         hist = torch.zeros(B, cap + 1, dtype=torch.long, device=dev)          # column `cap` is a scratch slot for masked writes

@@ -61,6 +61,10 @@ class Sampling(C.Structure):
     ]
 
 
+class SlotSampling(C.Structure):
+    _fields_ = [("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float), ("min_p", C.c_float)]
+
+
 class CodecConfig(C.Structure):
     _fields_ = [
         ("hidden", C.c_int), ("depth", C.c_int), ("heads", C.c_int), ("head_dim", C.c_int),
@@ -89,7 +93,7 @@ class CodecWeights(C.Structure):
 EXPORTS = [
     "nt_last_error", "nt_abi_version", "nt_launch_count", "nt_gemm",
     "nt_lm_workspace_bytes", "nt_lm_create", "nt_lm_destroy", "nt_lm_prefill", "nt_lm_prefill_slots", "nt_lm_decode",
-    "nt_lm_head_gemv",
+    "nt_lm_set_slot_sampling", "nt_lm_head_gemv",
     "nt_lm_debug_set_layers", "nt_lm_debug_ptr", "nt_lm_debug_set_profile", "nt_lm_debug_capture_sampler",
     "nt_debug_launch_chain",
     "nt_codec_workspace_bytes", "nt_codec_create", "nt_codec_destroy", "nt_codec_decode",
@@ -125,6 +129,7 @@ def lib() -> C.CDLL:
     L.nt_lm_prefill_slots.argtypes = [C.c_void_p, C.POINTER(LMState), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p,
                                       C.POINTER(C.c_int32), C.c_int, C.POINTER(Sampling), C.c_void_p, C.c_void_p]
     L.nt_lm_decode.argtypes = [C.c_void_p, C.POINTER(LMState), C.c_int, C.c_int, C.POINTER(Sampling), C.c_void_p, C.c_void_p]
+    L.nt_lm_set_slot_sampling.argtypes = [C.c_void_p, C.POINTER(SlotSampling), C.c_void_p]
     L.nt_lm_head_gemv.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     L.nt_lm_debug_set_layers.argtypes = [C.c_void_p, C.c_int]
     L.nt_lm_debug_ptr.restype = C.c_void_p

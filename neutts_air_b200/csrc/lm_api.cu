@@ -120,6 +120,9 @@ struct nt_lm {
   int* slot_key = nullptr;            // [max_batch] Philox stream key per slot, -1: slot + slot_base
   int* slot_args = nullptr;           // [3][max_batch] slots, stream keys, prompt lengths of the last call
   int* slot_table = nullptr;          // [max_batch][max_pages] the listed slots' page-table rows, in call order
+  // per-slot sampling controls (nt_lm_set_slot_sampling): copied into every SamplerParams while on
+  nt_slot_sampling* slot_sp = nullptr;  // [max_batch]
+  bool slot_sp_on = false;
 };
 
 template <typename F>
@@ -176,6 +179,7 @@ static size_t lm_carve(const nt_lm_config& c, void* ws, size_t bytes, F&& assign
     (L)->slot_key = a.take<int>(c.max_batch);                                                  \
     (L)->slot_args = a.take<int>(size_t(3) * c.max_batch);                                     \
     (L)->slot_table = a.take<int>(size_t(c.max_batch) * max_splits);                           \
+    (L)->slot_sp = a.take<nt_slot_sampling>(c.max_batch);                                     \
   }
 
 static int lm_check_config(const nt_lm_config* c) {
@@ -349,6 +353,7 @@ static SamplerParams make_sampler(const nt_lm* lm, const nt_lm_state* st, const 
   s.hidden = lm->cfg.hidden;
   s.slot_base = sp->slot_base;
   s.slot_key = lm->slot_key;
+  s.slot_sp = lm->slot_sp_on ? lm->slot_sp : nullptr;
   s.dbg_topk_val = lm->dbg_topk_val, s.dbg_topk_idx = lm->dbg_topk_idx, s.dbg_token = lm->dbg_token;
   return s;
 }
@@ -734,6 +739,32 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
     NT_CUDA_CHECK(cudaGraphLaunch(lm->graph, stream));
     g_launches.fetch_add(lm->graph_kernels, std::memory_order_relaxed);
   }
+  return NT_OK;
+}
+
+extern "C" int nt_lm_set_slot_sampling(nt_lm* lm, const nt_slot_sampling* table, void* stream_) {
+  if (!lm) return set_error(NT_ERR_INVALID, "nt_lm_set_slot_sampling: null handle");
+  const bool on = table != nullptr;
+  if (on) {
+    for (int s = 0; s < lm->cfg.max_batch; ++s) {
+      const nt_slot_sampling& e = table[s];
+      if (!(std::isfinite(e.temperature) && e.temperature > 0.f))
+        return set_error(NT_ERR_INVALID, "slot %d: temperature %g must be finite and > 0", s, e.temperature);
+      if (e.top_k < 1 || e.top_k > 64) return set_error(NT_ERR_INVALID, "slot %d: top_k=%d not in 1..64", s, e.top_k);
+      if (!(e.top_p > 0.f && e.top_p <= 1.f)) return set_error(NT_ERR_INVALID, "slot %d: top_p %g not in (0, 1]", s, e.top_p);
+      if (!(e.min_p >= 0.f && e.min_p < 1.f)) return set_error(NT_ERR_INVALID, "slot %d: min_p %g not in [0, 1)", s, e.min_p);
+    }
+    // pageable source: the runtime has staged it by the time the call returns
+    NT_CUDA_CHECK(cudaMemcpyAsync(lm->slot_sp, table, size_t(lm->cfg.max_batch) * sizeof(nt_slot_sampling), cudaMemcpyHostToDevice,
+                                  reinterpret_cast<cudaStream_t>(stream_)));
+  }
+  // the cached decode graph baked the table pointer (or its absence) into its sampler node; new values in a table
+  // that stays on are read at the next replay
+  if (on != lm->slot_sp_on && lm->graph) {
+    cudaGraphExecDestroy(lm->graph);
+    lm->graph = nullptr;
+  }
+  lm->slot_sp_on = on;
   return NT_OK;
 }
 

@@ -150,6 +150,7 @@ struct TcMisc {
   int pos[kTcMaxBatch];   // this step's seq_lens snapshot
   int apage[32];          // physical pages of this CTA's attention split (this step)
   int mask_eos[kTcMaxBatch];
+  float inv_t[kTcMaxBatch];   // 1 / temperature per sequence (the launch's sampling controls)
   float red[64];
   float tile_max[2][4][kTcMaxBatch];
   float rstd[8];
@@ -205,6 +206,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
   }
   for (int i = tid; i < static_cast<int>(sizeof(TcPlan) / 4); i += kTcThreads)
     reinterpret_cast<int*>(&ms->plan)[i] = reinterpret_cast<const int*>(P.plan + blockIdx.x)[i];
+  if (tid < B) ms->inv_t[tid] = row_sampling(P.samp, tid).inv_t;
   __syncthreads();
   const TcPlan& plan = ms->plan;
   if (tid < 4) {  // chunk tables of the split phases (items in plan order, k-blocks ascending)
@@ -926,7 +928,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     auto epi_head = [&] {
       if (warp >= 4) return;
       const int V = P.vocab;
-      const float inv_t = 1.0f / P.samp.sp.temperature;
       const int eos = P.samp.sp.eos_id;
       for (int t = 0; t < n_head_tiles; ++t) {
         const int tile = plan.head_t0 + t;
@@ -941,7 +942,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
           pv[n] = -INFINITY;
           if (n < B) {
             if (ok) P.logits[static_cast<long long>(n) * V + row] = v[n];
-            if (ok && !(ms->mask_eos[n] && row == eos)) pv[n] = v[n] * inv_t;
+            if (ok && !(ms->mask_eos[n] && row == eos)) pv[n] = v[n] * ms->inv_t[n];
           }
         }
 #pragma unroll

@@ -243,6 +243,25 @@ NT_DEVINL void emit_local_topk(const SamplerParams& p, const uint32_t* keys, int
   }
 }
 
+// Sampling controls of the row whose state lives in `slot`: its entry of the per-slot table when that is on, else the
+// launch scalars with top-p and min-p off.  Every sampler path reads temperature and top_k here, so all of them form
+// the same fp32 1 / T.
+struct RowSampling {
+  float inv_t;
+  int top_k;
+  float top_p, min_p;
+};
+NT_DEVINL RowSampling row_sampling(const SamplerParams& p, int slot) {
+  RowSampling r;
+  if (p.slot_sp) {
+    const nt_slot_sampling e = p.slot_sp[slot];
+    r.inv_t = 1.0f / e.temperature, r.top_k = e.top_k, r.top_p = e.top_p, r.min_p = e.min_p;
+  } else {
+    r.inv_t = 1.0f / p.sp.temperature, r.top_k = p.sp.top_k, r.top_p = 1.f, r.min_p = 0.f;
+  }
+  return r;
+}
+
 // logits processors (MinNewTokensLength -> Temperature), then the order-preserving key
 NT_DEVINL uint32_t processed_key(float logit, int idx, bool mask_eos, int eos_id, float inv_t) {
   if (mask_eos && idx == eos_id) logit = -INFINITY;
@@ -256,7 +275,7 @@ NT_DEVINL void sample_stage1_chunk(const SamplerParams& p, int b, int chunk, uin
   const int tid = threadIdx.x;
   const int ngen = p.n_generated_override ? __ldcg(p.n_generated_override + b) : __ldcg(p.n_generated + (slot >= 0 ? slot : b));
   const bool mask_eos = ngen < p.sp.min_new_tokens;
-  const float inv_t = 1.0f / p.sp.temperature;
+  const float inv_t = row_sampling(p, slot >= 0 ? slot : b).inv_t;
   const float* lg = p.logits + static_cast<long long>(b) * p.V;
   const int base = chunk * kTopChunk;
   const int n = min(kTopChunk, p.V - base);
@@ -279,7 +298,8 @@ NT_DEVINL void sample_stage1_chunk(const SamplerParams& p, int b, int chunk, uin
 }
 
 // Tail of the sampler for sequence b, given the k kept candidates sorted (score desc, index asc) in win[0..k):
-// softmax over them (TopK processor + softmax, utils.py:2789), Philox draw, state update, stop flags, and the next
+// softmax over them (TopK processor + softmax, utils.py:2789), the slot's top-p and min-p cuts (which keep a prefix
+// k' <= k of the window, renormalised), Philox draw over the prefix, state update, stop flags, and the next
 // token's embedding -> residual stream row (fp32; optionally also as (value, stamp) pairs for the polled hand-off).
 // Clobbers win[kTopKeep .. 2 kTopKeep) (exponentials).  b: logits row; slot >= 0: the slot whose state row b updates
 // (prefill into chosen slots), else slot b.
@@ -291,9 +311,32 @@ NT_DEVINL void sample_finish(const SamplerParams& p, int b, int k, Cand* win, in
   float* ev = reinterpret_cast<float*>(win + kTopKeep);   // [kTopKeep] exp(score - max)
   if (tid < 32) {
     const float m = win[0].v;
-    const float e0 = (tid < k) ? __expf(win[tid].v - m) : 0.f;
-    const float e1 = (tid + 32 < k) ? __expf(win[tid + 32].v - m) : 0.f;
-    const float sum = warp_sum(e0 + e1);
+    float e0 = (tid < k) ? __expf(win[tid].v - m) : 0.f;
+    float e1 = (tid + 32 < k) ? __expf(win[tid + 32].v - m) : 0.f;
+    float sum = warp_sum(e0 + e1);
+    const RowSampling rs = row_sampling(p, s);
+    if (rs.top_p < 1.f || rs.min_p > 0.f) {   // warp-uniform; top_p == 1 and min_p == 0 leave the window as it is
+      // lane l holds window entries l and 32 + l.  top-p (TopPLogitsWarper): entry j stays iff the probability mass
+      // before it, an exclusive prefix sum of q = e / sum in window order, is < top_p, so entry 0 always stays.
+      // min-p (MinPLogitsWarper): q_j >= min_p * q_0, i.e. e_j >= min_p since e_0 = exp(0) = 1.  Both keep a prefix.
+      const float q0 = e0 / sum, q1 = e1 / sum;
+      float c0 = q0, c1 = q1;   // inclusive scans of each half
+#pragma unroll
+      for (int off = 1; off < 32; off <<= 1) {
+        const float a = __shfl_up_sync(0xffffffffu, c0, off), bb = __shfl_up_sync(0xffffffffu, c1, off);
+        if (tid >= off) c0 += a, c1 += bb;
+      }
+      const float tot0 = __shfl_sync(0xffffffffu, c0, 31);
+      const float u0 = __shfl_up_sync(0xffffffffu, c0, 1), u1 = __shfl_up_sync(0xffffffffu, c1, 1);
+      const float x0 = tid == 0 ? 0.f : u0, x1 = tid == 0 ? tot0 : tot0 + u1;   // exclusive prefixes
+      const bool keep0 = tid < k && (rs.top_p >= 1.f || x0 < rs.top_p) && e0 >= rs.min_p;
+      const bool keep1 = tid + 32 < k && (rs.top_p >= 1.f || x1 < rs.top_p) && e1 >= rs.min_p;
+      const uint32_t f0 = __ballot_sync(0xffffffffu, !keep0), f1 = __ballot_sync(0xffffffffu, !keep1);
+      k = max(1, f0 ? __ffs(f0) - 1 : (f1 ? 31 + __ffs(f1) : 64));   // first entry cut
+      e0 = tid < k ? e0 : 0.f;
+      e1 = tid + 32 < k ? e1 : 0.f;
+      sum = warp_sum(e0 + e1);
+    }
     if (p.dbg_topk_val) {
       p.dbg_topk_val[b * kTopKeep + tid] = (tid < k) ? e0 / sum : 0.f;
       p.dbg_topk_val[b * kTopKeep + tid + 32] = (tid + 32 < k) ? e1 / sum : 0.f;
@@ -390,7 +433,7 @@ NT_DEVINL void sample_stage2_seq(const SamplerParams& p, int b, int ncand, uint3
   if (tid < kTopKeep) raw[tid].v = -INFINITY, raw[tid].i = 0x7fffffff;
   sync();
   mark();  // keys staged
-  const int k = min(min(p.sp.top_k, kTopKeep), ncand);
+  const int k = min(min(row_sampling(p, s).top_k, kTopKeep), ncand);
   uint32_t thr;
   int take_eq;
   radix_select_kth(keys, ncand, k, scratch, thr, take_eq, sync);
@@ -439,7 +482,9 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
   int* s_tok = reinterpret_cast<int*>(win + 2 * kTopKeep);
   uint32_t* keys = reinterpret_cast<uint32_t*>(s_tok + 4);       // the rest of the scratch region
   const int key_cap = static_cast<int>((uni_bytes - (kSelScratch + 128 + 4) * 4 - 2 * kTopKeep * sizeof(Cand)) / 4);
-  const float inv_t = 1.0f / p.sp.temperature;
+  const RowSampling rs = row_sampling(p, slot >= 0 ? slot : b);
+  const float inv_t = rs.inv_t;
+  const int top_k = rs.top_k;
   const int eos = p.sp.eos_id;
   const bool stateless = false;
   const int ngen = __ldcg(p.n_generated + (slot >= 0 ? slot : b));
@@ -459,7 +504,7 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
   //      shared memory by (score desc, index asc).  Two round trips to L2, six CTA barriers, no radix passes.
   {
     constexpr int kPer = 8, kTileCap = 256, kCandCap = 512;
-    const int ktop = min(p.sp.top_k, kTopKeep);
+    const int ktop = min(top_k, kTopKeep);
     float* gmax = reinterpret_cast<float*>(keys);                         // [256]
     int* tl = reinterpret_cast<int*>(keys + kConsumerThreads);            // [kTileCap]
     Cand* fc = reinterpret_cast<Cand*>(keys + kConsumerThreads + kTileCap);  // [kCandCap]
@@ -574,12 +619,12 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
   for (int i = tid; i < nt; i += kConsumerThreads) keys[i] = f2key(tile_max(i));
   if (tid < 64) tiles[tid] = -1, counts[tid] = 0;
   sync();
-  const int k = min(min(p.sp.top_k, kTopKeep), nt);
+  const int k = min(min(top_k, kTopKeep), nt);
   uint32_t thr;
   int take_eq;
   radix_select_kth(keys, nt, k, scratch, thr, take_eq, sync);
   // fewer tiles than top_k: the tile maxima bound nothing, every logit of every tile is a candidate
-  const uint32_t cthr = nt < p.sp.top_k ? 1u : thr;
+  const uint32_t cthr = nt < top_k ? 1u : thr;
   // the k tiles: maxima above the threshold, then the first take_eq tiles (index order) that equal it
   compact_topk(keys, nt, thr, take_eq, scratch, sync, [&](int slot, int i) { tiles[slot] = i; });
   sync();
@@ -638,7 +683,7 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
   sync();
   const int nc = fast_fits ? *fcnt : kFastCap + 1;
   if (nc <= kFastCap) {
-    const int k2 = min(min(p.sp.top_k, kTopKeep), nc);
+    const int k2 = min(min(top_k, kTopKeep), nc);
     for (int i = tid; i < nc; i += kConsumerThreads) {   // rank among the candidates: (score desc, index asc) is a total order
       const Cand me = fc[i];
       int rank = 0;

@@ -805,7 +805,7 @@ __global__ void __launch_bounds__(kConsumerThreads) topk_tiles_kernel(const Samp
   const int b = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int slot = p.row_slot ? __ldg(p.row_slot + b) : b;
   const bool mask_eos = __ldcg(p.n_generated + slot) < p.sp.min_new_tokens;
-  const float inv_t = 1.0f / p.sp.temperature;
+  const float inv_t = row_sampling(p, slot).inv_t;
   int fix_tile = -1;
   float fix_val = 0.f;
   if (mask_eos) {   // the raw maximum of the tile that holds EOS may be the (masked) EOS logit itself: redo that tile without it

@@ -94,6 +94,9 @@ struct SamplerParams {
   // by the stand-alone sampler kernels only; the persistent decode kernel samples row b into slot b.
   const int32_t* row_slot;
   const int32_t* slot_key;  // optional [max_batch] Philox stream key per slot; -1: slot + slot_base
+  // optional [max_batch] temperature / top_k / top_p / min_p per slot (nt_lm_set_slot_sampling), read through
+  // row_sampling() with the row's slot; nullptr: sp.temperature and sp.top_k for every row, no top-p / min-p cut
+  const nt_slot_sampling* slot_sp;
 };
 int launch_sampler(const SamplerParams& p, int B, cudaStream_t stream);
 int launch_sampler_check(const SamplerParams& p);

@@ -8,6 +8,7 @@ All arithmetic happens in ``libneutts_b200.so``; torch is used for device memory
 from __future__ import annotations
 
 import ctypes as C
+import math
 from dataclasses import dataclass
 
 import numpy as np
@@ -107,6 +108,46 @@ class PagePool:
         self.free.extend(reversed(list(pages)))
 
 
+DEFAULT_CONTROLS = (1.0, 50, 1.0, 0.0)   # temperature, top_k, top_p, min_p: the reference's (neutts/neutts.py:338-347)
+
+
+def _is_seq(v) -> bool:
+    return isinstance(v, (list, tuple, np.ndarray, torch.Tensor))
+
+
+def check_controls(temperature, top_k, top_p, min_p) -> tuple:
+    """One slot's sampling controls, validated as ``nt_lm_set_slot_sampling`` does -> (float, int, float, float)."""
+    t, p, m = float(temperature), float(top_p), float(min_p)
+    if not (math.isfinite(t) and t > 0):
+        raise ValueError(f"temperature {temperature} must be finite and > 0")
+    if int(top_k) != top_k or not 1 <= int(top_k) <= 64:
+        raise ValueError(f"top_k {top_k} must be an integer in 1..64")
+    if not 0 < p <= 1:
+        raise ValueError(f"top_p {top_p} must be in (0, 1]")
+    if not 0 <= m < 1:
+        raise ValueError(f"min_p {min_p} must be in [0, 1)")
+    return t, int(top_k), p, m
+
+
+def per_prompt_controls(n: int, temperature, top_k, top_p, min_p):
+    """Sampling controls of n prompts.  Each control is a scalar or a sequence with one value per prompt.  Returns None
+    when every control is a scalar and top-p / min-p are off (``sampling``'s scalars then govern, exactly as without
+    per-slot controls), else one validated (temperature, top_k, top_p, min_p) per prompt."""
+    cols = []
+    for name, v in (("temperature", temperature), ("top_k", top_k), ("top_p", top_p), ("min_p", min_p)):
+        if _is_seq(v):
+            v = [x.item() if hasattr(x, "item") else x for x in v]
+            if len(v) != n:
+                raise ValueError(f"{name} needs one value per prompt ({n}), got {len(v)}")
+            cols.append(v)
+        else:
+            cols.append(None)
+    if all(c is None for c in cols) and top_p == 1 and min_p == 0:
+        return None
+    vals = [c if c is not None else [v] * n for c, v in zip(cols, (temperature, top_k, top_p, min_p))]
+    return [check_controls(*row) for row in zip(*vals)]
+
+
 class SpeechLM:
     PAGE = 64
 
@@ -156,6 +197,7 @@ class SpeechLM:
         self.pool = PagePool(self.num_pages, page_shuffle_seed)
         self._table_host = None
         self._slot_pages = [[] for _ in range(max_batch)]
+        self._slot_sp_host = None   # host mirror of the per-slot sampling controls (None: off)
 
     def __del__(self):
         try:
@@ -186,6 +228,33 @@ class SpeechLM:
             fptr = f.data_ptr()
         return _lib.Sampling(int(eos_id), int(min_new_tokens), int(mnt), int(top_k), float(temperature), int(seed),
                              int(bool(greedy)), fptr, lptr, int(slot_base))
+
+    def set_slot_sampling(self, rows, slots=None) -> None:
+        """Per-slot sampling controls.  ``rows``: one (temperature, top_k, top_p, min_p) per slot of ``slots`` (default:
+        slots 0..len(rows) - 1); every other slot keeps its entry, or the reference defaults (1.0, 50, 1.0, 0.0) when
+        the table was off.  ``None`` switches the table off, and ``sampling``'s temperature and top_k govern every
+        slot again.  The table is copied on the current stream, so it is ordered before the next prefill or decode."""
+        if rows is None:
+            _lib.check(self.L.nt_lm_set_slot_sampling(self.handle, None, _lib.current_stream_ptr()))
+            self._slot_sp_host = None
+            return
+        rows = [check_controls(*r) for r in rows]
+        slots = list(range(len(rows))) if slots is None else [int(s) for s in slots]
+        if len(slots) != len(rows) or len(set(slots)) != len(slots) or any(not 0 <= s < self.max_batch for s in slots):
+            raise ValueError(f"slots must be distinct, in 0..{self.max_batch - 1} and one per row")
+        table = list(self._slot_sp_host or [DEFAULT_CONTROLS] * self.max_batch)
+        for s, r in zip(slots, rows):
+            table[s] = r
+        arr = (_lib.SlotSampling * self.max_batch)(*(_lib.SlotSampling(*r) for r in table))
+        with torch.cuda.device(self.device):
+            _lib.check(self.L.nt_lm_set_slot_sampling(self.handle, arr, _lib.current_stream_ptr()))
+        self._slot_sp_host = table
+
+    def _use_controls(self, rows) -> None:
+        """Slots 0..len(rows) - 1 take ``rows``; None leaves the table off (switching it off only if an earlier call
+        left it on)."""
+        if rows is not None or getattr(self, "_slot_sp_host", None) is not None:
+            self.set_slot_sampling(rows)
 
     def prefill(self, prompts, sp, return_logits: bool = False):
         """prompts: list of 1-D int sequences.  Fills the KV cache and samples the first token."""
@@ -356,11 +425,13 @@ class SpeechLM:
 
     def generate_batch(self, prompts, eos_token_id: int, max_length: int | None = None, min_new_tokens: int = 50,
                        temperature: float = 1.0, top_k: int = 50, max_new_tokens: int | None = None, seed: int = 0,
-                       greedy: bool = False, forced: torch.Tensor | None = None, check_every: int = 64, slot_base: int = 0):
+                       greedy: bool = False, forced: torch.Tensor | None = None, check_every: int = 64, slot_base: int = 0,
+                       top_p: float = 1.0, min_p: float = 0.0):
         """Returns a list of int64 CPU tensors with the generated ids of each prompt (EOS included
         when it was sampled), following transformers' stopping rules (stopping_criteria.py:73-84,
         467-471): stop at EOS or when prompt + generated reaches max_length.  ``max_new_tokens`` may also be a
-        list with one cap per prompt."""
+        list with one cap per prompt.  ``temperature``, ``top_k``, ``top_p`` and ``min_p`` are each a scalar or one
+        value per prompt (per-slot controls, ``set_slot_sampling``)."""
         max_length = max_length or self.max_ctx
         if max_length > self.max_ctx:
             raise ValueError(f"max_length {max_length} exceeds the engine context {self.max_ctx}")
@@ -371,8 +442,12 @@ class SpeechLM:
         # must not shorten its neighbours, so every slot gets its own cap and the loop runs to the largest one
         caps = self._caps(lens, max_length, max_new_tokens)
         limit = max(caps)
+        rows = per_prompt_controls(len(prompts), temperature, top_k, top_p, min_p)
+        if rows is not None:   # the launch scalars are validated but not used while the table is on
+            temperature, top_k = rows[0][0], rows[0][1]
         sp = self.sampling(eos_token_id, min_new_tokens, limit, top_k, temperature, seed, greedy, forced,
                            limits=caps if min(caps) < limit else None, slot_base=slot_base)
+        self._use_controls(rows)
         self.prefill(prompts, sp)
         remaining = limit - 1
         B = len(prompts)
@@ -388,7 +463,8 @@ class SpeechLM:
 
     def generate_queue(self, prompts, eos_token_id: int, max_length: int | None = None, min_new_tokens: int = 50,
                        temperature: float = 1.0, top_k: int = 50, max_new_tokens: int | None = None, seed: int = 0,
-                       greedy: bool = False, check_every: int = 32, slot_base: int = 0):
+                       greedy: bool = False, check_every: int = 32, slot_base: int = 0, top_p: float = 1.0,
+                       min_p: float = 0.0):
         """Continuous batching over any number of prompts: ``generate_batch``'s results and stopping rules, but a slot
         whose sequence finished is refilled with the next waiting prompt while the other slots keep decoding.
 
@@ -398,7 +474,9 @@ class SpeechLM:
         steps, each cut short so that it ends with the earliest cap-driven completion while prompts wait.  After each
         launch one small read of (n_generated, done) finds the finished slots; their tokens are copied out and the next
         prompts go into all freed slots with one ``prefill_slots`` call.  Returns the generated ids per prompt (int64
-        CPU tensors, EOS included when sampled) in input order; every KV page is back in the pool afterwards."""
+        CPU tensors, EOS included when sampled) in input order; every KV page is back in the pool afterwards.
+        ``temperature``, ``top_k``, ``top_p`` and ``min_p`` are each a scalar or one value per prompt; a newcomer's
+        controls are written into its slot before its prefill, and the other slots keep theirs."""
         max_length = max_length or self.max_ctx
         if max_length > self.max_ctx:
             raise ValueError(f"max_length {max_length} exceeds the engine context {self.max_ctx}")
@@ -412,8 +490,12 @@ class SpeechLM:
             raise ValueError("prompt already at max_length")
         caps = self._caps(lens, max_length, max_new_tokens)
         S = min(n, self.max_batch)
+        ctl_rows = per_prompt_controls(n, temperature, top_k, top_p, min_p)
+        if ctl_rows is not None:
+            temperature, top_k = ctl_rows[0][0], ctl_rows[0][1]
         sp = self.sampling(eos_token_id, min_new_tokens, max(caps), top_k, temperature, seed, greedy,
                            limits=caps[:S], slot_base=slot_base)
+        self._use_controls(ctl_rows[:S] if ctl_rows is not None else None)
         self.prefill([prompts[i] for i in range(S)], sp)
         occ = list(range(S))   # prompt held by each slot, None once harvested
         ngen = [1] * S         # generated tokens per slot, as of the last read
@@ -436,6 +518,8 @@ class SpeechLM:
                     if take:
                         idx = list(range(nxt, nxt + len(take)))
                         nxt += len(take)
+                        if ctl_rows is not None:   # the newcomers' controls, before their prefill on the same stream
+                            self.set_slot_sampling([ctl_rows[i] for i in idx], slots=take)
                         self.prefill_slots(take, [prompts[i] for i in idx], sp, [slot_base + i for i in idx],
                                            limits=[caps[i] for i in idx])
                         for s, i in zip(take, idx):
@@ -455,8 +539,10 @@ class SpeechLM:
     @torch.no_grad()
     def generate(self, input_ids: torch.Tensor, max_length: int = 2048, eos_token_id: int | None = None,
                  do_sample: bool = True, temperature: float = 1.0, top_k: int = 50, use_cache: bool = True,
-                 min_new_tokens: int = 0, max_new_tokens: int | None = None, seed: int | None = None, **_):
-        """transformers-compatible seam used by ``NeuTTS._infer_torch`` (neutts/neutts.py:338-347)."""
+                 min_new_tokens: int = 0, max_new_tokens: int | None = None, seed: int | None = None,
+                 top_p: float = 1.0, min_p: float = 0.0, **_):
+        """transformers-compatible seam used by ``NeuTTS._infer_torch`` (neutts/neutts.py:338-347).  ``top_p`` and
+        ``min_p`` act as transformers' TopPLogitsWarper / MinPLogitsWarper; other generation kwargs are ignored."""
         if eos_token_id is None:
             raise ValueError("eos_token_id is required")
         if input_ids.dim() != 2:
@@ -464,8 +550,9 @@ class SpeechLM:
         prompts = [row.tolist() for row in input_ids.cpu()]
         if seed is None:
             seed = int(torch.randint(0, 2**31 - 1, (1,)).item())  # reference sampling is unseeded
+        cuts = {} if top_p == 1.0 and min_p == 0.0 else dict(top_p=top_p, min_p=min_p)
         outs = self.generate_batch(prompts, eos_token_id, max_length, min_new_tokens, temperature, top_k,
-                                   max_new_tokens, seed, greedy=not do_sample)
+                                   max_new_tokens, seed, greedy=not do_sample, **cuts)
         n = max(len(o) for o in outs)
         res = torch.full((len(outs), input_ids.shape[1] + n), int(eos_token_id), dtype=torch.long)
         for b, o in enumerate(outs):
