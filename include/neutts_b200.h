@@ -188,6 +188,19 @@ typedef struct {
  * nt_op_topk_sample does not read the table: it takes nt_sampling's scalars only. */
 int nt_lm_set_slot_sampling(nt_lm* lm, const nt_slot_sampling* host_table, void* stream);
 
+/* Vocabulary range (speech-token-only decoding; transformers' suppress_tokens with every id outside the allowed set).
+ * Every later sampler launch of nt_lm_prefill, nt_lm_prefill_slots and nt_lm_decode may only draw an id in
+ * [lo, hi) or the launch's nt_sampling.eos_id (EOS stays masked while n_generated < min_new_tokens).  The lm_head
+ * then computes only the 128-row tiles of [lo, hi) and the tile that holds EOS; in every logits output each
+ * suppressed id reads -inf and each allowed id is bit-identical to the same call with the range off.  The range holds
+ * for every slot.  lo = 0, hi = vocab_size switches it off (the default).  Rules: 0 <= lo < hi <= vocab_size,
+ * hi - lo >= 64, lo % 128 == 0, and hi % 128 == 0 or hi == vocab_size; a bad range returns NT_ERR_INVALID and leaves
+ * the previous one in force.  Host state only: it applies to the launches enqueued on `stream` after the call, and
+ * each launch carries it in its kernel parameters (nothing is copied to the device), so a graph a caller captures
+ * keeps the range that was in force at capture.
+ * nt_op_topk_sample and nt_lm_head_gemv ignore the range. */
+int nt_lm_set_vocab_range(nt_lm* lm, int32_t lo, int32_t hi, void* stream);
+
 /* Timed single-kernel entry for the roofline measurement: the lm_head GEMV (+ final RMSNorm)
  * exactly as the decode step launches it.  h: f32 [B][hidden] -> logits f32 [B][vocab]. */
 int nt_lm_head_gemv(nt_lm* lm, const float* h, int B, float* logits, void* stream);

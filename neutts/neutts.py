@@ -86,12 +86,14 @@ class _CrossFade:
 class NeuTTS:
     def __init__(self, backbone_repo="neuphonic/neutts-nano", backbone_device="cpu", codec_repo="neuphonic/neucodec",
                  codec_device="cpu", *, tokenizer=None, phonemizer=None, backbone=None, codec=None,
-                 max_batch: int = 1, seed: int | None = None):
+                 max_batch: int = 1, seed: int | None = None, speech_tokens_only: bool = False):
         """Same positional signature and defaults as the reference (``neutts/neutts.py:75-81``), so
         ``examples/basic_example.py:12-17`` runs unmodified.  The device strings keep their reference
         meaning for the CALLER -- ``"cpu"`` = results come back as host arrays, which this facade always
         does -- but the engines themselves only exist for sm_90a: a ``"cpu"`` request runs on the current
-        CUDA device and says so once (there is no CPU fallback)."""
+        CUDA device and says so once (there is no CPU fallback).  ``speech_tokens_only``: generation may only draw
+        ``<|speech_N|>`` ids and ``<|SPEECH_GENERATION_END|>`` (every other id suppressed, as transformers'
+        ``suppress_tokens``); the engine then skips the lm_head rows of every other id."""
         # constants the reference exposes (neutts/neutts.py:84-91)
         self.sample_rate = 24_000
         self.max_context = 2048
@@ -106,6 +108,7 @@ class NeuTTS:
         self.tokenizer = tokenizer
         self.max_batch = max_batch
         self.seed = seed
+        self.speech_tokens_only = bool(speech_tokens_only)
         self.phonemizer = phonemizer if phonemizer is not None else self._load_phonemizer()
         self._load_backbone(backbone_repo, backbone_device, backbone)
         self._load_codec(codec_repo, codec_device, codec)
@@ -214,6 +217,9 @@ class NeuTTS:
         eos = self._tok_id("<|SPEECH_GENERATION_END|>")
         seed = self.seed if self.seed is not None else int(torch.randint(0, 2**31 - 1, (1,)).item())
         kw = _backbone_kw(ctl if ctl is not None else CONTROL_DEFAULTS)
+        rng = self._speech_range()
+        if rng is not None:
+            kw["vocab_range"] = rng
         if len(prompts) > self.max_batch and hasattr(self.backbone, "generate_queue"):
             # more prompts than slots: refill each slot as soon as its utterance ends (prompt i keeps the Philox
             # stream slot_base + i that the chunked loop gives it)
@@ -223,14 +229,28 @@ class NeuTTS:
             return self.backbone.generate_batch(list(prompts), eos, max_length=self.max_context, min_new_tokens=min_new_tokens,
                                                 max_new_tokens=max_new_tokens, seed=seed, slot_base=slot_base, **kw)
         outs = []  # injected transformers-style backbone: one sequence at a time, as the reference does
+        suppress = {}
+        if rng is not None:   # the same allowed set as transformers' suppress_tokens list
+            del kw["vocab_range"]
+            vocab = getattr(getattr(self.backbone, "config", None), "vocab_size", None) or len(self.tokenizer)
+            suppress["suppress_tokens"] = [i for i in range(vocab) if not (rng[0] <= i < rng[1] or i == eos)]
         for i, p in enumerate(prompts):
             t = torch.tensor(list(p)).unsqueeze(0).to(self.backbone.device)
             one = {k: v[i] if isinstance(v, list) else v for k, v in kw.items()}
+            one.update(suppress)
             with torch.no_grad():
                 o = self.backbone.generate(t, max_length=self.max_context, eos_token_id=eos, do_sample=True, use_cache=True,
                                            min_new_tokens=min_new_tokens, **one)
             outs.append(o[0, t.shape[-1]:].cpu().long())
         return outs
+
+    def _n_codes(self) -> int:
+        shape = getattr(self.codec, "shape", None)
+        return getattr(shape, "fsq_levels", 4) ** getattr(shape, "fsq_dims", 8)
+
+    def _speech_range(self):
+        """[speech_base, speech_base + n_codes) while ``speech_tokens_only`` is on, else None."""
+        return (self.speech_base, self.speech_base + self._n_codes()) if self.speech_tokens_only else None
 
     def _ids_to_codes(self, ids: torch.Tensor) -> torch.Tensor:
         """Drop every token that is not ``<|speech_N|>`` (the reference's regex does the same, ``:276``)."""
@@ -407,6 +427,9 @@ class NeuTTS:
         sp = lm.sampling(eos, 50, limit, top_k, temp, seed) if min(limits) == limit else lm.sampling(eos, 50, limit, top_k, temp, seed, limits=limits)
         if rows is not None or getattr(lm, "_slot_sp_host", None) is not None:
             lm.set_slot_sampling(rows)   # before the prefill, on the same stream
+        rng = self._speech_range()
+        if rng is not None or getattr(lm, "_vocab_range", None) is not None:
+            lm.set_vocab_range(*(rng if rng is not None else (None,)))
         dev = lm.out_tokens.device
         cap = max(len(r) for r in refs) + limit
         hist = torch.zeros(B, cap + 1, dtype=torch.long, device=dev)          # column `cap` is a scratch slot for masked writes

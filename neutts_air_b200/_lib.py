@@ -93,7 +93,7 @@ class CodecWeights(C.Structure):
 EXPORTS = [
     "nt_last_error", "nt_abi_version", "nt_launch_count", "nt_gemm",
     "nt_lm_workspace_bytes", "nt_lm_create", "nt_lm_destroy", "nt_lm_prefill", "nt_lm_prefill_slots", "nt_lm_decode",
-    "nt_lm_set_slot_sampling", "nt_lm_head_gemv",
+    "nt_lm_set_slot_sampling", "nt_lm_set_vocab_range", "nt_lm_head_gemv",
     "nt_lm_debug_set_layers", "nt_lm_debug_ptr", "nt_lm_debug_set_profile", "nt_lm_debug_capture_sampler",
     "nt_debug_launch_chain",
     "nt_codec_workspace_bytes", "nt_codec_create", "nt_codec_destroy", "nt_codec_decode",
@@ -130,6 +130,7 @@ def lib() -> C.CDLL:
                                       C.POINTER(C.c_int32), C.c_int, C.POINTER(Sampling), C.c_void_p, C.c_void_p]
     L.nt_lm_decode.argtypes = [C.c_void_p, C.POINTER(LMState), C.c_int, C.c_int, C.POINTER(Sampling), C.c_void_p, C.c_void_p]
     L.nt_lm_set_slot_sampling.argtypes = [C.c_void_p, C.POINTER(SlotSampling), C.c_void_p]
+    L.nt_lm_set_vocab_range.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
     L.nt_lm_head_gemv.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     L.nt_lm_debug_set_layers.argtypes = [C.c_void_p, C.c_int]
     L.nt_lm_debug_ptr.restype = C.c_void_p

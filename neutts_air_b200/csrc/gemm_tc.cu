@@ -34,8 +34,9 @@ struct GemmEpilogue {
   long long split_stride;  // (no residual / activation; bias rides on slice 0) -- the consumer adds them in z order
   int w_const;             // W is never written on the device: its first ring of tiles may load before the PDL wait
   int w_stream;            // W is read exactly once by this launch (one row tile): fetch it with the L2 evict_first policy
-  float* tile_max;         // optional [M][gridDim.x]: maximum of the row's stored values inside this CTA's BN columns (lm_head ->
+  float* tile_max;         // optional [M][tile_ld]: maximum of the row's stored values inside this CTA's BN columns (lm_head ->
                            //   tile-max sampler); plain fp32 epilogue only
+  long long tile_ld;
 };
 
 // kShallow: half-depth ring (<= 113 KB of shared memory) for grids of more than one wave of CTAs.
@@ -304,7 +305,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-    if (ep.tile_max && row_ok) ep.tile_max[static_cast<long long>(row) * gridDim.x + blockIdx.x] = tmx;
+    if (ep.tile_max && row_ok) ep.tile_max[static_cast<long long>(row) * ep.tile_ld + blockIdx.x] = tmx;
   }
 }
 
@@ -375,7 +376,8 @@ int gemm_tile_n(int M, int N, bool swiglu) {
   return bn;
 }
 
-int gemm_dispatch(const nt_gemm_args& a, cudaStream_t stream, SplitK* split, bool w_const, const Split3* s3, float* tile_max) {
+int gemm_dispatch(const nt_gemm_args& a, cudaStream_t stream, SplitK* split, bool w_const, const Split3* s3, float* tile_max, int bn_req,
+                  long long tile_ld) {
   if (a.M <= 0 || a.N <= 0 || a.K <= 0) return set_error(NT_ERR_INVALID, "gemm: empty problem");
   const int esz = a.dtype == NT_BF16 ? 2 : 4;
   const int bk = 128 / esz;
@@ -402,7 +404,8 @@ int gemm_dispatch(const nt_gemm_args& a, cudaStream_t stream, SplitK* split, boo
 
   // tile-N choice: keep >= ~1 wave of CTAs when the problem allows it
   const int mt = (a.M + 127) / 128;
-  const int bn = gemm_tile_n(a.M, a.N, a.act == NT_ACT_SWIGLU);
+  const int bn = bn_req > 0 ? bn_req : gemm_tile_n(a.M, a.N, a.act == NT_ACT_SWIGLU);
+  if (bn != 32 && bn != 64 && bn != 128) return set_error(NT_ERR_INVALID, "gemm: tile width %d not in {32, 64, 128}", bn);
   if (tile_max && (split || a.act != NT_ACT_NONE || a.out_bf16)) return set_error(NT_ERR_INVALID, "gemm: tile maxima need the plain fp32 epilogue");
 
   if (s3 && (a.dtype != NT_TF32 || split)) return set_error(NT_ERR_INVALID, "gemm: 3xTF32 needs tf32 operands and no split-K");
@@ -429,6 +432,7 @@ int gemm_dispatch(const nt_gemm_args& a, cudaStream_t stream, SplitK* split, boo
   ep.split_stride = 0;
   ep.w_const = w_const ? 1 : 0;
   ep.tile_max = tile_max;
+  ep.tile_ld = tile_ld > 0 ? tile_ld : (a.N + bn - 1) / bn;
   ep.w_stream = (w_const && mt == 1) ? 1 : 0;
   if (split) {
     split->used = 1;

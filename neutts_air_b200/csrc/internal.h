@@ -67,8 +67,10 @@ struct Split3 {
   int a_lo_rows, w_lo_rows;
 };
 // tile_max (optional, plain fp32 epilogue): [M][ceil(N / gemm_tile_n)] maximum of every row inside every column tile
+// (row pitch tile_ld when > 0).  bn > 0 forces the tile width (32 | 64 | 128): a GEMM over a column range of a wider
+// matrix then runs the instruction shape, and so the arithmetic, of the GEMM over the whole matrix.
 int gemm_dispatch(const nt_gemm_args& a, cudaStream_t stream, SplitK* split = nullptr, bool w_const = false,
-                  const Split3* s3 = nullptr, float* tile_max = nullptr);
+                  const Split3* s3 = nullptr, float* tile_max = nullptr, int bn = 0, long long tile_ld = 0);
 int gemm_tile_n(int M, int N, bool swiglu);
 
 // 2-D TMA descriptor over a row-major matrix (rows x cols elements, row stride ld elements); box = box_rows x 128

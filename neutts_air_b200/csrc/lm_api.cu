@@ -123,7 +123,37 @@ struct nt_lm {
   // per-slot sampling controls (nt_lm_set_slot_sampling): copied into every SamplerParams while on
   nt_slot_sampling* slot_sp = nullptr;  // [max_batch]
   bool slot_sp_on = false;
+  // vocabulary range (nt_lm_set_vocab_range): allowed ids [vr_lo, vr_hi) + EOS while vr_on
+  bool vr_on = false;
+  int vr_lo = 0, vr_hi = 0;
 };
+
+// The lm_head tiles a launch computes under the vocabulary range: [t_lo, t_hi), plus eos_tile when EOS lies outside
+// them (eos_tile = -1 otherwise).  off: every tile.
+struct VocabTiles {
+  bool on;
+  int t_lo, t_hi, eos_tile;
+  int count() const { return t_hi - t_lo + (eos_tile >= 0 ? 1 : 0); }
+};
+static VocabTiles vocab_tiles(const nt_lm* lm, int eos) {
+  VocabTiles v;
+  v.on = lm->vr_on;
+  v.t_lo = lm->vr_on ? lm->vr_lo / 128 : 0;
+  v.t_hi = ((lm->vr_on ? lm->vr_hi : lm->cfg.vocab_size) + 127) / 128;
+  const int et = eos / 128;
+  v.eos_tile = (lm->vr_on && (et < v.t_lo || et >= v.t_hi)) ? et : -1;
+  return v;
+}
+
+// Every launch under the range first sets its logits rows [0, B) and their tile maxima to -inf; the lm_head then
+// writes only the tiles it computes, so each suppressed id reads -inf on every sampler path.
+static int vocab_fill(nt_lm* lm, int B, cudaStream_t stream) {
+  if (!lm->vr_on) return NT_OK;
+  const int V = lm->cfg.vocab_size, nt = (V + 127) / 128;
+  int rc = launch_fill_neg_inf(lm->logits, static_cast<long long>(B) * V, stream);
+  if (!rc && lm->tc_tmax) rc = launch_fill_neg_inf(lm->tc_tmax, static_cast<long long>(B < lm->tc_rows ? B : lm->tc_rows) * nt, stream);
+  return rc;
+}
 
 template <typename F>
 static size_t lm_carve(const nt_lm_config& c, void* ws, size_t bytes, F&& assign) {
@@ -376,28 +406,57 @@ static int run_sampler(nt_lm* lm, const SamplerParams& s, int B, cudaStream_t st
   return launch_sampler(s, B, stream);
 }
 
-static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cudaStream_t stream, const SplitK* pend = nullptr) {
+// eos >= 0: apply the vocabulary range with this EOS id (every sampler launch); -1: every row (nt_lm_head_gemv).  Under
+// the range the lm_head runs once over the range's rows and once over the EOS tile (when EOS lies outside them), each
+// a row slice of the full-vocabulary launch with the same per-row arithmetic, so every computed logit is bit-identical
+// to the range off; the rows it does not compute keep the -inf of vocab_fill.
+static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cudaStream_t stream, const SplitK* pend = nullptr,
+                        int eos = -1) {
   const nt_lm_config& c = lm->cfg;
+  const int V = c.vocab_size, nt = (V + 127) / 128;
+  const VocabTiles vt = eos >= 0 ? vocab_tiles(lm, eos) : VocabTiles{false, 0, nt, -1};
+  // row slices [r0, r1): the range (or everything), then the EOS tile
+  const int r0[2] = {vt.t_lo * 128, vt.eos_tile * 128};
+  const int r1[2] = {vt.t_hi * 128 < V ? vt.t_hi * 128 : V, (vt.eos_tile + 1) * 128 < V ? (vt.eos_tile + 1) * 128 : V};
+  const int nslices = vt.eos_tile >= 0 ? 2 : 1;
+  int rc;
   if (B <= kGemvMaxBatch) {
-    GemvParams g;
-    memset(&g, 0, sizeof(g));
-    g.W = lm->lm_head, g.rows = c.vocab_size, g.K = c.hidden;
-    g.x = hrows, g.ldx = c.hidden;
-    g.norm_w = lm->final_norm, g.eps = c.rms_eps;
-    g.epi = GEMV_STORE, g.out = logits, g.ldo = c.vocab_size;
-    return launch_gemv(g, B, lm->num_sms, stream);
+    for (int i = 0; i < nslices; ++i) {
+      GemvParams g;
+      memset(&g, 0, sizeof(g));
+      g.W = lm->lm_head + static_cast<long long>(r0[i]) * c.hidden, g.rows = r1[i] - r0[i], g.K = c.hidden;
+      g.x = hrows, g.ldx = c.hidden;
+      g.norm_w = lm->final_norm, g.eps = c.rms_eps;
+      g.epi = GEMV_STORE, g.out = logits + r0[i], g.ldo = V;
+      if ((rc = launch_gemv(g, B, lm->num_sms, stream))) return rc;
+    }
+    return vt.eos_tile >= 0 ? launch_vocab_eos_tile(logits, B, V, eos, nullptr, nt, stream) : NT_OK;
   }
   // pend: the last down_proj left split-K slices that still have to be folded into hrows (batched decode only)
   const bool fold = pend && pend->used > 1;
-  int rc = launch_rmsnorm_rows(hrows, lm->final_norm, c.rms_eps, B, c.hidden, nullptr, lm->xn, stream, fold ? pend->ws : nullptr,
+  rc = launch_rmsnorm_rows(hrows, lm->final_norm, c.rms_eps, B, c.hidden, nullptr, lm->xn, stream, fold ? pend->ws : nullptr,
                                fold ? pend->used : 0, fold ? pend->slice_stride : 0);
   if (rc) return rc;
-  nt_gemm_args a;
-  memset(&a, 0, sizeof(a));
-  a.dtype = NT_BF16, a.M = B, a.N = c.vocab_size, a.K = c.hidden;
-  a.A = lm->xn, a.lda = c.hidden, a.W = lm->lm_head, a.ldw = c.hidden;
-  a.out_f32 = logits, a.ldc = c.vocab_size;
-  return gemm_dispatch(a, stream, nullptr, true, nullptr, (use_tile_sampler(lm, B) && logits == lm->logits) ? lm->tc_tmax : nullptr);
+  float* tmax = (use_tile_sampler(lm, B) && logits == lm->logits) ? lm->tc_tmax : nullptr;
+  if (!vt.on) {
+    nt_gemm_args a;
+    memset(&a, 0, sizeof(a));
+    a.dtype = NT_BF16, a.M = B, a.N = V, a.K = c.hidden;
+    a.A = lm->xn, a.lda = c.hidden, a.W = lm->lm_head, a.ldw = c.hidden;
+    a.out_f32 = logits, a.ldc = V;
+    return gemm_dispatch(a, stream, nullptr, true, nullptr, tmax);
+  }
+  // slices run at the full-vocabulary tile width; their tile maxima land at absolute tile indices (128-column tiles)
+  const int bn = gemm_tile_n(B, V, false);
+  for (int i = 0; i < nslices; ++i) {
+    nt_gemm_args a;
+    memset(&a, 0, sizeof(a));
+    a.dtype = NT_BF16, a.M = B, a.N = r1[i] - r0[i], a.K = c.hidden;
+    a.A = lm->xn, a.lda = c.hidden, a.W = lm->lm_head + static_cast<long long>(r0[i]) * c.hidden, a.ldw = c.hidden;
+    a.out_f32 = logits + r0[i], a.ldc = V;
+    if ((rc = gemm_dispatch(a, stream, nullptr, true, nullptr, tmax ? tmax + r0[i] / 128 : nullptr, bn, nt))) return rc;
+  }
+  return vt.eos_tile >= 0 ? launch_vocab_eos_tile(logits, B, V, eos, tmax, nt, stream) : NT_OK;
 }
 
 // Transformer layers over `rows` token rows held in lm->h, via tensor-core GEMMs.
@@ -504,13 +563,14 @@ static int prefill_stage(nt_lm* lm, const int32_t* cu, int B, std::vector<int>& 
 
 // Prompt rows -> KV cache + last-position logits in lm->logits (and logits_out).  table: see layers_gemm.
 static int prefill_forward(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, int B, int max_len,
-                           const int32_t* table, float* logits_out, cudaStream_t stream) {
+                           const int32_t* table, float* logits_out, int eos, cudaStream_t stream) {
   const nt_lm_config& c = lm->cfg;
   int rc;
+  if ((rc = vocab_fill(lm, B, stream))) return rc;
   if ((rc = launch_embed_rows(lm->embed, ids, cu[B], c.hidden, lm->h, stream))) return rc;
   if ((rc = layers_gemm(lm, st, cu[B], B, 0, max_len, stream, nullptr, table))) return rc;
   if ((rc = launch_gather_rows(lm->h, lm->last_rows, B, c.hidden, lm->h_last, stream))) return rc;
-  if ((rc = lm_head_rows(lm, lm->h_last, B, lm->logits, stream))) return rc;
+  if ((rc = lm_head_rows(lm, lm->h_last, B, lm->logits, stream, nullptr, eos))) return rc;
   if (logits_out)
     NT_CUDA_CHECK(cudaMemcpyAsync(logits_out, lm->logits, size_t(B) * c.vocab_size * sizeof(float), cudaMemcpyDeviceToDevice, stream));
   return NT_OK;
@@ -527,7 +587,7 @@ extern "C" int nt_lm_prefill(nt_lm* lm, const nt_lm_state* st, const int32_t* id
   std::vector<int> lens;
   int max_len = 0;
   if ((rc = prefill_stage(lm, cu, B, lens, max_len, stream))) return rc;
-  if ((rc = prefill_forward(lm, st, ids, cu, B, max_len, nullptr, logits_out, stream))) return rc;
+  if ((rc = prefill_forward(lm, st, ids, cu, B, max_len, nullptr, logits_out, sp->eos_id, stream))) return rc;
   NT_CUDA_CHECK(cudaMemcpyAsync(st->seq_lens, lens.data(), B * sizeof(int), cudaMemcpyHostToDevice, stream));
   NT_CUDA_CHECK(cudaMemsetAsync(lm->slot_key, 0xff, size_t(c.max_batch) * sizeof(int), stream));  // every slot: slot + slot_base
   SamplerParams s = make_sampler(lm, st, sp);
@@ -570,7 +630,7 @@ extern "C" int nt_lm_prefill_slots(nt_lm* lm, const nt_lm_state* st, const int32
   if ((rc = launch_slots_setup(lm->slot_args, B, st->page_table, max_pages, lm->slot_table, st->seq_lens, st->n_generated, st->done,
                                lm->slot_key, stream)))
     return rc;
-  if ((rc = prefill_forward(lm, st, ids, cu, B, max_len, lm->slot_table, logits_out, stream))) return rc;
+  if ((rc = prefill_forward(lm, st, ids, cu, B, max_len, lm->slot_table, logits_out, sp->eos_id, stream))) return rc;
   SamplerParams s = make_sampler(lm, st, sp);
   s.row_slot = lm->slot_args;
   s.h = nullptr;  // the residual rows are rebuilt below, for every slot
@@ -622,7 +682,7 @@ static int decode_step(nt_lm* lm, const nt_lm_state* st, int B, const nt_samplin
   } else {
     if ((rc = layers_gemm(lm, st, B, B, 1, 0, stream, &tail))) return rc;
   }
-  if ((rc = lm_head_rows(lm, lm->h, B, lm->logits, stream, &tail))) return rc;
+  if ((rc = lm_head_rows(lm, lm->h, B, lm->logits, stream, &tail, sp->eos_id))) return rc;
   SamplerParams s = make_sampler(lm, st, sp);
   s.advance = 1;
   return run_sampler(lm, s, B, stream);
@@ -650,6 +710,7 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
     want_tc = impl[0] == 't';
   }
   if (n_steps == 0) return NT_OK;
+  if ((rc = vocab_fill(lm, B, stream))) return rc;   // once per launch: no step writes a suppressed row or tile maximum
   const int tc_layers = lm->debug_layers >= 0 ? lm->debug_layers : c.n_layers;
   if (want_tc && lm->tc_ok && B <= lm->tc_rows && B * c.n_kv_heads <= lm->num_sms) {
     TcParams P;
@@ -682,6 +743,10 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
     P.kv = make_kv(lm, st);
     if ((rc = kv_pool_tmap(P.kv, c.n_layers, &P.kvmap))) return rc;
     P.logits = lm->logits, P.tmax = lm->tc_tmax, P.ntiles = info.ntiles;
+    // lm_head tile list under the vocabulary range: the EOS tile sits before or after the range's tiles, in tile order
+    const VocabTiles vt = vocab_tiles(lm, sp->eos_id);
+    P.head_n = vt.count(), P.head_lo = vt.t_lo, P.head_eos = vt.eos_tile;
+    P.head_eos_at = vt.eos_tile < 0 ? -1 : (vt.eos_tile < vt.t_lo ? 0 : vt.t_hi - vt.t_lo);
     P.samp = make_sampler(lm, st, sp);
     P.samp.advance = 1;
     P.gbar = lm->gbar;
@@ -765,6 +830,26 @@ extern "C" int nt_lm_set_slot_sampling(nt_lm* lm, const nt_slot_sampling* table,
     lm->graph = nullptr;
   }
   lm->slot_sp_on = on;
+  return NT_OK;
+}
+
+extern "C" int nt_lm_set_vocab_range(nt_lm* lm, int32_t lo, int32_t hi, void* stream) {
+  (void)stream;   // host state only: read by the launches enqueued after this call
+  if (!lm) return set_error(NT_ERR_INVALID, "nt_lm_set_vocab_range: null handle");
+  const int V = lm->cfg.vocab_size;
+  if (!(0 <= lo && lo < hi && hi <= V)) return set_error(NT_ERR_INVALID, "vocab range [%d, %d) not inside [0, %d)", lo, hi, V);
+  if (hi - lo < 64) return set_error(NT_ERR_INVALID, "vocab range [%d, %d) holds fewer than 64 ids", lo, hi);
+  if (lo % 128 || (hi % 128 && hi != V))
+    return set_error(NT_ERR_INVALID, "vocab range [%d, %d): lo must be a multiple of 128, hi too unless it is %d", lo, hi, V);
+  const bool on = !(lo == 0 && hi == V);
+  // the cached decode graph baked the lm_head launches of the previous range
+  if ((on != lm->vr_on || lo != lm->vr_lo || hi != lm->vr_hi) && lm->graph) {
+    cudaGraphExecDestroy(lm->graph);
+    lm->graph = nullptr;
+  }
+  lm->vr_on = on;
+  lm->vr_lo = on ? lo : 0;
+  lm->vr_hi = on ? hi : 0;
   return NT_OK;
 }
 

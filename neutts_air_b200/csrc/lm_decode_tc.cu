@@ -214,9 +214,16 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     for (int i = 0; i < plan.n[tid]; ++i)
       for (int kb = 0; kb < plan.it[tid][i].nkb && c < 16; ++kb, ++c) ms->ckb[tid][c] = plan.it[tid][i].kb0 + kb;
     ms->nchunks[tid] = c;
+  } else if (tid == 4) {   // this CTA's positions in the lm_head tile list
+    ms->plan.head_t0 = static_cast<int>((static_cast<long long>(P.head_n) * blockIdx.x) / gridDim.x);
+    ms->plan.head_t1 = static_cast<int>((static_cast<long long>(P.head_n) * (blockIdx.x + 1)) / gridDim.x);
   }
   __syncthreads();
   const int n_head_tiles = plan.head_t1 - plan.head_t0;
+  // position in the lm_head tile list -> row tile (the identity while the vocabulary range is off)
+  auto head_tile = [&](int v) -> int {
+    return v == P.head_eos_at ? P.head_eos : P.head_lo + v - (P.head_eos_at >= 0 && v > P.head_eos_at ? 1 : 0);
+  };
 
   // stream / MMA warps (whole warp): released one decode step at a time, so that an early exit (every sequence done)
   // never leaves bulk copies in flight.  An mbarrier phase per step; `stop` is written before the releasing arrive.
@@ -257,8 +264,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
         }
       const CUtensorMap* hm = wmaps + 4 * P.total_layers;
       const int t0 = uniform(plan.head_t0), t1 = uniform(plan.head_t1);
-      for (int t = t0; t < t1; ++t)
-        for (int kb = 0; kb < KBH; ++kb) push(hm, kb * 64, t * 128);
+      for (int t = t0; t < t1; ++t) {
+        const int row0 = uniform(head_tile(t)) * 128;
+        for (int kb = 0; kb < KBH; ++kb) push(hm, kb * 64, row0);
+      }
     }
   } else if (warp >= kTcMmaWarp0) {
     // ================================================================== MMA warpgroup (warps kTcMmaWarp0 .. + 3)
@@ -930,19 +939,20 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
       const int V = P.vocab;
       const int eos = P.samp.sp.eos_id;
       for (int t = 0; t < n_head_tiles; ++t) {
-        const int tile = plan.head_t0 + t;
+        const int tile = head_tile(plan.head_t0 + t);
         float v[NT];
         acc_take(v);
         const int row = tile * 128 + warp * 32 + lane;
         const bool ok = row < V;
+        const bool allowed = tile != P.head_eos || row == eos;   // the EOS tile outside the vocabulary range: EOS only
         float (*tm)[kTcMaxBatch] = ms->tile_max[t & 1];
         float pv[NTOK];
 #pragma unroll
         for (int n = 0; n < NTOK; ++n) {
           pv[n] = -INFINITY;
           if (n < B) {
-            if (ok) P.logits[static_cast<long long>(n) * V + row] = v[n];
-            if (ok && !(ms->mask_eos[n] && row == eos)) pv[n] = v[n] * ms->inv_t[n];
+            if (ok) P.logits[static_cast<long long>(n) * V + row] = allowed ? v[n] : -INFINITY;
+            if (ok && allowed && !(ms->mask_eos[n] && row == eos)) pv[n] = v[n] * ms->inv_t[n];
           }
         }
 #pragma unroll
@@ -1220,10 +1230,6 @@ int tc_build_plan(const TcShape& s, int G, bool flat, TcPlan* plan, unsigned cha
   info->gu_split = flat ? 1 : 0;
   const int nt = (s.vocab + 127) / 128;
   info->ntiles = nt;
-  for (int c = 0; c < G; ++c) {
-    plan[c].head_t0 = int((static_cast<long long>(nt) * c) / G);
-    plan[c].head_t1 = int((static_cast<long long>(nt) * (c + 1)) / G);
-  }
   return NT_OK;
 }
 

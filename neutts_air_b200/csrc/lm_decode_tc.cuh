@@ -24,11 +24,13 @@ struct TcItem {
 };
 
 // Per-CTA plan, identical for every layer (the four weight matrices of a layer have the same shape in every
-// layer) + this CTA's contiguous range of lm_head row tiles.  Built on the host (tc_build_plan), read once.
+// layer).  Built on the host (tc_build_plan), read once.  The lm_head split is not built on the host: the kernel
+// fills head_t0 / head_t1 in its shared copy, CTA c taking positions [n c / G, n (c + 1) / G) of TcParams' lm_head
+// tile list (n = head_n), so a launch's vocabulary range lives in the kernel parameters alone.
 struct TcPlan {
   int n[4];                       // items per phase: 0 = qkv, 1 = o_proj, 2 = gate/up, 3 = down
   TcItem it[4][kTcMaxItems];
-  int head_t0, head_t1;           // lm_head row tiles [t0, t1)
+  int head_t0, head_t1;           // positions [t0, t1) of the lm_head tile list (filled by the kernel)
   int fold_q, fold_g;             // batch <= 4: this CTA writes the folded residual stream back (one CTA per fold point)
   int gu_split;                   // 1: gate/up items carry their own K range and write raw partial sums (flat plan)
 };
@@ -73,6 +75,10 @@ struct TcParams {
   float* logits;                  // [B][vocab]
   float* tmax;                    // [B][ntiles] processed maximum of every 128-row lm_head tile
   int ntiles;
+  // lm_head tile list, head_n tiles spread evenly over the CTAs: tile head_eos at position head_eos_at, the others
+  // head_lo, head_lo + 1, ... in order.  Vocabulary range off: head_n = ntiles, head_lo = 0, head_eos_at = -1 (every
+  // tile).  Range on: the range's tiles, plus the EOS tile when it lies outside them (only EOS is allowed there).
+  int head_n, head_lo, head_eos, head_eos_at;
   SamplerParams samp;
   unsigned* gbar;
   int n_steps;

@@ -833,6 +833,32 @@ int launch_sampler_tiles(const SamplerParams& p, int B, const float* tmax, int n
   return launch_kernel(topk_tiles_kernel, dim3(B), dim3(kConsumerThreads), smem, stream, true, p, tmax, nt);
 }
 
+// =================================================================================== vocabulary range
+__global__ void fill_neg_inf_kernel(float* p, long long n) {
+  pdl_launch_dependents();
+  pdl_wait();
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x)
+    p[i] = -INFINITY;
+}
+int launch_fill_neg_inf(float* p, long long n, cudaStream_t s) {
+  if (n <= 0) return NT_OK;
+  const long long blocks = (n + 255) / 256;
+  return launch_kernel(fill_neg_inf_kernel, dim3(static_cast<unsigned>(blocks < 1024 ? blocks : 1024)), dim3(256), 0, s, true, p, n);
+}
+
+// grid B, 128 threads: thread r owns row tile * 128 + r of logits row blockIdx.x
+__global__ void vocab_eos_tile_kernel(float* logits, int V, int eos, float* tmax, int nt) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int tile = eos >> 7, row = tile * 128 + threadIdx.x;
+  float* lg = logits + static_cast<long long>(blockIdx.x) * V;
+  if (row < V && row != eos) lg[row] = -INFINITY;
+  if (tmax && threadIdx.x == 0) tmax[static_cast<long long>(blockIdx.x) * nt + tile] = lg[eos];
+}
+int launch_vocab_eos_tile(float* logits, int B, int V, int eos, float* tmax, int nt, cudaStream_t s) {
+  return launch_kernel(vocab_eos_tile_kernel, dim3(B), dim3(128), 0, s, true, logits, V, eos, tmax, nt);
+}
+
 // =================================================================================== prefill helpers
 __global__ void embed_rows_kernel(const __nv_bfloat16* embed, const int32_t* ids, int hidden, float* h) {
   pdl_launch_dependents();

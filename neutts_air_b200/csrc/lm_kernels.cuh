@@ -103,6 +103,12 @@ int launch_sampler_check(const SamplerParams& p);
 // tmax: [B][nt] RAW maxima of the 128-column tiles of p.logits (GEMM epilogue, gemm_dispatch(..., tile_max))
 int launch_sampler_tiles(const SamplerParams& p, int B, const float* tmax, int nt, cudaStream_t stream);
 size_t sampler_scratch_floats(int B, int V);  // per-array element count for cand_val / cand_idx
+// Vocabulary range (nt_lm_set_vocab_range).  launch_fill_neg_inf: p[0, n) = -inf (the logits rows and tile maxima of a
+// launch, before its lm_head writes the tiles it computes).  launch_vocab_eos_tile: after an lm_head that computed the
+// whole 128-row tile holding `eos` although only `eos` is allowed there, rows [0, B) of that tile read -inf except eos,
+// and tmax (optional, [B][nt] raw maxima) holds the eos logit as the tile's maximum.
+int launch_fill_neg_inf(float* p, long long n, cudaStream_t s);
+int launch_vocab_eos_tile(float* logits, int B, int V, int eos, float* tmax, int nt, cudaStream_t s);
 int sampler_nchunks(int V);
 
 int launch_embed_rows(const __nv_bfloat16* embed, const int32_t* ids, int T, int hidden, float* h, cudaStream_t s);

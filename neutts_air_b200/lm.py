@@ -148,6 +148,25 @@ def per_prompt_controls(n: int, temperature, top_k, top_p, min_p):
     return [check_controls(*row) for row in zip(*vals)]
 
 
+def check_vocab_range(vocab_range, vocab_size: int):
+    """A vocabulary range (lo, hi), validated as ``nt_lm_set_vocab_range`` does -> (int, int); None -> None (off).
+    Rules: 0 <= lo < hi <= vocab_size, hi - lo >= 64 (top_k <= 64 always finds k allowed ids), lo % 128 == 0 and
+    hi % 128 == 0 unless hi == vocab_size."""
+    if vocab_range is None:
+        return None
+    lo, hi = vocab_range
+    if not all(isinstance(v, (int, float, np.integer)) for v in (lo, hi)) or int(lo) != lo or int(hi) != hi:
+        raise ValueError(f"vocab range {vocab_range} must be two integers")
+    lo, hi = int(lo), int(hi)
+    if not 0 <= lo < hi <= vocab_size:
+        raise ValueError(f"vocab range [{lo}, {hi}) not inside [0, {vocab_size})")
+    if hi - lo < 64:
+        raise ValueError(f"vocab range [{lo}, {hi}) holds fewer than 64 ids")
+    if lo % 128 or (hi % 128 and hi != vocab_size):
+        raise ValueError(f"vocab range [{lo}, {hi}): lo must be a multiple of 128, hi too unless it is {vocab_size}")
+    return lo, hi
+
+
 class SpeechLM:
     PAGE = 64
 
@@ -198,6 +217,7 @@ class SpeechLM:
         self._table_host = None
         self._slot_pages = [[] for _ in range(max_batch)]
         self._slot_sp_host = None   # host mirror of the per-slot sampling controls (None: off)
+        self._vocab_range = None    # (lo, hi) while the vocabulary range is on
 
     def __del__(self):
         try:
@@ -255,6 +275,30 @@ class SpeechLM:
         left it on)."""
         if rows is not None or getattr(self, "_slot_sp_host", None) is not None:
             self.set_slot_sampling(rows)
+
+    def set_vocab_range(self, lo, hi=None) -> None:
+        """Restrict every later sampler launch to ids in [lo, hi) plus the launch's EOS id (transformers'
+        ``suppress_tokens`` with every other id suppressed; the min-new-tokens EOS mask still applies).  The lm_head
+        then computes only the range's 128-row tiles and the EOS tile, and every suppressed logit reads -inf.  The
+        range holds for every slot.  ``set_vocab_range(None)`` switches it off; a bad range raises ValueError and leaves
+        the previous one in force (rules: ``check_vocab_range``)."""
+        if lo is not None and hi is None:
+            raise ValueError("set_vocab_range needs both lo and hi (or None to switch the range off)")
+        rng = None if lo is None else check_vocab_range((lo, hi), self.shape.vocab_size)
+        if rng is not None and rng == (0, self.shape.vocab_size):
+            rng = None
+        lo_, hi_ = rng if rng is not None else (0, self.shape.vocab_size)
+        with torch.cuda.device(self.device):
+            _lib.check(self.L.nt_lm_set_vocab_range(self.handle, lo_, hi_, _lib.current_stream_ptr()))
+        self._vocab_range = rng
+
+    def _use_vocab_range(self, vocab_range) -> None:
+        """The engine takes ``vocab_range``; None leaves the range off (switching it off only if an earlier call left
+        it on), so a default call makes no engine call."""
+        if vocab_range is not None:
+            self.set_vocab_range(*vocab_range)
+        elif getattr(self, "_vocab_range", None) is not None:
+            self.set_vocab_range(None)
 
     def prefill(self, prompts, sp, return_logits: bool = False):
         """prompts: list of 1-D int sequences.  Fills the KV cache and samples the first token."""
@@ -426,12 +470,15 @@ class SpeechLM:
     def generate_batch(self, prompts, eos_token_id: int, max_length: int | None = None, min_new_tokens: int = 50,
                        temperature: float = 1.0, top_k: int = 50, max_new_tokens: int | None = None, seed: int = 0,
                        greedy: bool = False, forced: torch.Tensor | None = None, check_every: int = 64, slot_base: int = 0,
-                       top_p: float = 1.0, min_p: float = 0.0):
+                       top_p: float = 1.0, min_p: float = 0.0, vocab_range=None):
         """Returns a list of int64 CPU tensors with the generated ids of each prompt (EOS included
         when it was sampled), following transformers' stopping rules (stopping_criteria.py:73-84,
         467-471): stop at EOS or when prompt + generated reaches max_length.  ``max_new_tokens`` may also be a
         list with one cap per prompt.  ``temperature``, ``top_k``, ``top_p`` and ``min_p`` are each a scalar or one
-        value per prompt (per-slot controls, ``set_slot_sampling``)."""
+        value per prompt (per-slot controls, ``set_slot_sampling``).  ``vocab_range``: (lo, hi) restricts every draw to
+        [lo, hi) plus EOS (``set_vocab_range``); None leaves the range off."""
+        if vocab_range is not None:   # validated before any engine call
+            vocab_range = check_vocab_range(vocab_range, self.shape.vocab_size)
         max_length = max_length or self.max_ctx
         if max_length > self.max_ctx:
             raise ValueError(f"max_length {max_length} exceeds the engine context {self.max_ctx}")
@@ -448,6 +495,7 @@ class SpeechLM:
         sp = self.sampling(eos_token_id, min_new_tokens, limit, top_k, temperature, seed, greedy, forced,
                            limits=caps if min(caps) < limit else None, slot_base=slot_base)
         self._use_controls(rows)
+        self._use_vocab_range(vocab_range)
         self.prefill(prompts, sp)
         remaining = limit - 1
         B = len(prompts)
@@ -464,7 +512,7 @@ class SpeechLM:
     def generate_queue(self, prompts, eos_token_id: int, max_length: int | None = None, min_new_tokens: int = 50,
                        temperature: float = 1.0, top_k: int = 50, max_new_tokens: int | None = None, seed: int = 0,
                        greedy: bool = False, check_every: int = 32, slot_base: int = 0, top_p: float = 1.0,
-                       min_p: float = 0.0):
+                       min_p: float = 0.0, vocab_range=None):
         """Continuous batching over any number of prompts: ``generate_batch``'s results and stopping rules, but a slot
         whose sequence finished is refilled with the next waiting prompt while the other slots keep decoding.
 
@@ -476,7 +524,10 @@ class SpeechLM:
         prompts go into all freed slots with one ``prefill_slots`` call.  Returns the generated ids per prompt (int64
         CPU tensors, EOS included when sampled) in input order; every KV page is back in the pool afterwards.
         ``temperature``, ``top_k``, ``top_p`` and ``min_p`` are each a scalar or one value per prompt; a newcomer's
-        controls are written into its slot before its prefill, and the other slots keep theirs."""
+        controls are written into its slot before its prefill, and the other slots keep theirs.  ``vocab_range`` as in
+        ``generate_batch``: set once before the first prefill, it holds across every refill."""
+        if vocab_range is not None:   # validated before any engine call
+            vocab_range = check_vocab_range(vocab_range, self.shape.vocab_size)
         max_length = max_length or self.max_ctx
         if max_length > self.max_ctx:
             raise ValueError(f"max_length {max_length} exceeds the engine context {self.max_ctx}")
@@ -496,6 +547,7 @@ class SpeechLM:
         sp = self.sampling(eos_token_id, min_new_tokens, max(caps), top_k, temperature, seed, greedy,
                            limits=caps[:S], slot_base=slot_base)
         self._use_controls(ctl_rows[:S] if ctl_rows is not None else None)
+        self._use_vocab_range(vocab_range)
         self.prefill([prompts[i] for i in range(S)], sp)
         occ = list(range(S))   # prompt held by each slot, None once harvested
         ngen = [1] * S         # generated tokens per slot, as of the last read
@@ -540,9 +592,10 @@ class SpeechLM:
     def generate(self, input_ids: torch.Tensor, max_length: int = 2048, eos_token_id: int | None = None,
                  do_sample: bool = True, temperature: float = 1.0, top_k: int = 50, use_cache: bool = True,
                  min_new_tokens: int = 0, max_new_tokens: int | None = None, seed: int | None = None,
-                 top_p: float = 1.0, min_p: float = 0.0, **_):
+                 top_p: float = 1.0, min_p: float = 0.0, vocab_range=None, **_):
         """transformers-compatible seam used by ``NeuTTS._infer_torch`` (neutts/neutts.py:338-347).  ``top_p`` and
-        ``min_p`` act as transformers' TopPLogitsWarper / MinPLogitsWarper; other generation kwargs are ignored."""
+        ``min_p`` act as transformers' TopPLogitsWarper / MinPLogitsWarper; ``vocab_range`` (lo, hi) suppresses every
+        id outside [lo, hi) and EOS (``set_vocab_range``); other generation kwargs are ignored."""
         if eos_token_id is None:
             raise ValueError("eos_token_id is required")
         if input_ids.dim() != 2:
@@ -551,6 +604,8 @@ class SpeechLM:
         if seed is None:
             seed = int(torch.randint(0, 2**31 - 1, (1,)).item())  # reference sampling is unseeded
         cuts = {} if top_p == 1.0 and min_p == 0.0 else dict(top_p=top_p, min_p=min_p)
+        if vocab_range is not None:
+            cuts["vocab_range"] = vocab_range
         outs = self.generate_batch(prompts, eos_token_id, max_length, min_new_tokens, temperature, top_k,
                                    max_new_tokens, seed, greedy=not do_sample, **cuts)
         n = max(len(o) for o in outs)
