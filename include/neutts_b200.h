@@ -222,6 +222,15 @@ int nt_lm_debug_set_profile(nt_lm* lm, long long* buf, int step);
  * multi-step persistent decode launch leaves its last step.  NULL pointers switch the capture off.  Debug "tmax"
  * (nt_lm_debug_ptr) holds the per-128-column tile maxima of the last tile-max sampler input. */
 int nt_lm_debug_capture_sampler(nt_lm* lm, float* topk_val, int32_t* topk_idx, int32_t* token);
+/* work plan of the persistent decode kernel (tests): runs the host planner for a model shape on n_sms CTAs with
+ * whole-K (flat = 0) or flat (flat = 1) gate/up, and makes no CUDA call.  Outputs (each may be NULL):
+ * items int16 [n_sms][4][4][4]: per CTA, phase (0 qkv, 1 o_proj, 2 gate/up, 3 down_proj) and item (tile, first k-block,
+ * k-blocks, slice), a k-block being 64 elements of K; counts int32 [n_sms][4]: items per phase; flags int32 [n_sms][3]:
+ * fold_q, fold_g, gu_split; gu_nsl uint8 [gu_cap]: K slices of every gate/up tile (flat plan); info int32 [7]: K slices
+ * of the qkv, o_proj and down_proj phases, most slices of a gate/up tile, lm_head tiles, most k-blocks a CTA stages in
+ * one phase, gu_split.  NT_ERR_INVALID with a message when the plan does not fit the kernel. */
+int nt_debug_decode_plan(int hidden, int inter, int n_heads, int n_kv, int vocab, int n_sms, int flat, int16_t* items,
+                         int32_t* counts, int32_t* flags, uint8_t* gu_nsl, int gu_cap, int32_t* info);
 
 /* ------------------------------------------------------------------------------------------
  * NeuCodec decoder (seam 2)

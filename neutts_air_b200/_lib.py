@@ -95,7 +95,7 @@ EXPORTS = [
     "nt_lm_workspace_bytes", "nt_lm_create", "nt_lm_destroy", "nt_lm_prefill", "nt_lm_prefill_slots", "nt_lm_decode",
     "nt_lm_set_slot_sampling", "nt_lm_set_vocab_range", "nt_lm_head_gemv",
     "nt_lm_debug_set_layers", "nt_lm_debug_ptr", "nt_lm_debug_set_profile", "nt_lm_debug_capture_sampler",
-    "nt_debug_launch_chain",
+    "nt_debug_launch_chain", "nt_debug_decode_plan",
     "nt_codec_workspace_bytes", "nt_codec_create", "nt_codec_destroy", "nt_codec_decode",
     "nt_op_rmsnorm", "nt_op_topk_sample",
 ]
@@ -138,6 +138,7 @@ def lib() -> C.CDLL:
     L.nt_lm_debug_set_profile.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
     L.nt_lm_debug_capture_sampler.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.nt_debug_launch_chain.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    L.nt_debug_decode_plan.argtypes = [C.c_int] * 7 + [C.c_void_p] * 4 + [C.c_int, C.c_void_p]
     L.nt_codec_workspace_bytes.restype = C.c_size_t
     L.nt_codec_workspace_bytes.argtypes = [C.POINTER(CodecConfig)]
     L.nt_codec_create.argtypes = [C.POINTER(CodecConfig), C.POINTER(CodecWeights), C.c_void_p, C.c_size_t, C.POINTER(C.c_void_p)]

@@ -882,6 +882,39 @@ extern "C" int nt_lm_debug_capture_sampler(nt_lm* lm, float* topk_val, int32_t* 
   }
   return NT_OK;
 }
+extern "C" int nt_debug_decode_plan(int hidden, int inter, int n_heads, int n_kv, int vocab, int n_sms, int flat,
+                                    int16_t* items, int32_t* counts, int32_t* flags, uint8_t* gu_nsl, int gu_cap,
+                                    int32_t* info) {
+  if (hidden < 64 || inter < 64 || n_heads < 1 || n_kv < 1 || vocab < 1)
+    return set_error(NT_ERR_INVALID, "nt_debug_decode_plan: bad shape");
+  if (n_sms < 8 || n_sms > 256) return set_error(NT_ERR_INVALID, "decode_tc: %d SMs unsupported", n_sms);
+  const TcShape ts{hidden, inter, n_heads, n_kv, (n_heads + 2 * n_kv) * 64, vocab};
+  const int tg = (2 * inter + 127) / 128;
+  if (flat && gu_nsl && gu_cap < tg) return set_error(NT_ERR_INVALID, "nt_debug_decode_plan: gu_nsl holds %d < %d tiles", gu_cap, tg);
+  std::vector<TcPlan> plan(n_sms);
+  std::vector<unsigned char> nsl(flat ? tg : 0, 0);
+  TcPlanInfo pi = {};
+  const int rc = tc_build_plan(ts, n_sms, flat != 0, plan.data(), flat ? nsl.data() : nullptr, &pi);
+  if (rc) return rc;
+  for (int c = 0; c < n_sms; ++c) {
+    for (int ph = 0; ph < 4; ++ph) {
+      if (counts) counts[4 * c + ph] = plan[c].n[ph];
+      for (int i = 0; i < kTcMaxItems && items; ++i) {
+        const TcItem& it = plan[c].it[ph][i];
+        int16_t* o = items + ((size_t(c) * 4 + ph) * kTcMaxItems + i) * 4;
+        o[0] = it.tile, o[1] = it.kb0, o[2] = it.nkb, o[3] = it.slice;
+      }
+    }
+    if (flags) flags[3 * c] = plan[c].fold_q, flags[3 * c + 1] = plan[c].fold_g, flags[3 * c + 2] = plan[c].gu_split;
+  }
+  if (flat && gu_nsl) memcpy(gu_nsl, nsl.data(), nsl.size());
+  if (info) {
+    const int v[7] = {pi.sq, pi.so, pi.sd, pi.sg, pi.ntiles, pi.max_chunks, pi.gu_split};
+    memcpy(info, v, sizeof(v));
+  }
+  return NT_OK;
+}
+
 extern "C" void* nt_lm_debug_ptr(nt_lm* lm, const char* name) {
   if (!lm || !name) return nullptr;
   const struct { const char* n; void* p; } tab[] = {

@@ -167,6 +167,34 @@ def check_vocab_range(vocab_range, vocab_size: int):
     return lo, hi
 
 
+PLAN_PHASES = ("qkv", "o", "gu", "d")   # phase order of the persistent kernel's work plan
+
+
+def debug_decode_plan(hidden: int, inter: int, n_heads: int, n_kv: int, vocab: int, n_sms: int, flat: bool) -> dict:
+    """The persistent decode kernel's work plan for a model shape on ``n_sms`` CTAs, built by the library's host planner
+    (no GPU needed): ``items[c][phase]`` lists CTA c's (tile, first k-block, k-blocks, slice) items of each phase
+    (``PLAN_PHASES``), ``fold_q`` / ``fold_g`` / ``gu_split`` its flags, ``gu_nsl`` the K slices of every gate/up tile
+    (flat plan), and ``sq, so, sd, sg, ntiles, max_chunks`` the plan summary.  Raises ValueError when the kernel cannot
+    take the shape (the engine then decodes on the per-op chain)."""
+    L = _lib.lib()
+    items = np.zeros((n_sms, 4, 4, 4), dtype=np.int16)
+    counts = np.zeros((n_sms, 4), dtype=np.int32)
+    flags = np.zeros((n_sms, 3), dtype=np.int32)
+    tg = (2 * inter + 127) // 128
+    nsl = np.zeros(tg, dtype=np.uint8)
+    info = np.zeros(7, dtype=np.int32)
+    ptr = lambda a: a.ctypes.data_as(C.c_void_p)
+    _lib.check(L.nt_debug_decode_plan(hidden, inter, n_heads, n_kv, vocab, n_sms, int(bool(flat)), ptr(items),
+                                      ptr(counts), ptr(flags), ptr(nsl), tg, ptr(info)))
+    out = dict(zip(("sq", "so", "sd", "sg", "ntiles", "max_chunks", "gu_split"), info.tolist()))
+    out["items"] = [{ph: [tuple(int(v) for v in items[c, p, i]) for i in range(counts[c, p])]
+                     for p, ph in enumerate(PLAN_PHASES)} for c in range(n_sms)]
+    out["fold_q"], out["fold_g"] = flags[:, 0].tolist(), flags[:, 1].tolist()
+    out["gu_split_cta"] = flags[:, 2].tolist()
+    out["gu_nsl"] = nsl.tolist() if flat else None
+    return out
+
+
 class SpeechLM:
     PAGE = 64
 

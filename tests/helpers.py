@@ -1,6 +1,8 @@
 """Shared test plumbing: oracle weights -> HF-style state dicts -> CUDA engines."""
 from __future__ import annotations
 
+import math
+
 import torch
 
 from oracle import codec_oracle, lm_oracle
@@ -62,3 +64,23 @@ def rel_err(a: torch.Tensor, b: torch.Tensor) -> float:
 
 def max_err(a: torch.Tensor, b: torch.Tensor) -> float:
     return float((a.double().cpu() - b.double().cpu()).abs().max())
+
+
+def rel_rms(got, ref) -> float:
+    """Relative RMS error; inf when ``got`` holds a NaN or an inf (so that max() over errors cannot drop it)."""
+    if not torch.isfinite(got).all():
+        return math.inf
+    return float((got.double() - ref.double()).norm() / ref.double().norm().clamp_min(1e-300))
+
+
+def gather_kv(lm, layer: int, b: int, n: int):
+    """Rows 0..n-1 of slot ``b``'s K and V in layer ``layer``, read through ``lm.page_table`` from the paged pool
+    ``lm.kv[layer, 0|1, page, kv_head, row, :]`` (pages of 64 rows).  Returns two float64 CPU tensors [n, n_kv, 64]."""
+    page = lm.kv.shape[-2]
+    npg = (n + page - 1) // page
+    pages = lm.page_table[b, :npg].to(device=lm.kv.device, dtype=torch.long)
+    out = []
+    for which in (0, 1):
+        t = lm.kv[layer, which].index_select(0, pages)                     # [npg, n_kv, 64, 64]
+        out.append(t.permute(0, 2, 1, 3).reshape(npg * page, t.shape[1], 64)[:n].double().cpu())
+    return out[0], out[1]

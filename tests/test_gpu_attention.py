@@ -31,7 +31,7 @@ import pytest
 import torch
 
 from oracle import lm_oracle as O
-from tests.helpers import make_lm
+from tests.helpers import gather_kv, make_lm, rel_rms
 
 PAGE = 64
 LOG2E = 1.4426950408889634
@@ -50,18 +50,6 @@ BARS = {"prefill": 3e-3, "decode-fp32": 2e-6, "decode-mma": 5e-3, "decode-bf16":
 
 
 # ====================================================================================== float64 reference helpers
-def gather_kv(lm, layer: int, b: int, n: int):
-    """Rows 0..n-1 of slot ``b``'s K and V in layer ``layer``, read through ``lm.page_table`` from the paged pool
-    ``lm.kv[layer, 0|1, page, kv_head, row, :]``.  Returns two float64 CPU tensors [n, n_kv, 64]."""
-    npg = (n + PAGE - 1) // PAGE
-    pages = lm.page_table[b, :npg].to(device=lm.kv.device, dtype=torch.long)
-    out = []
-    for which in (0, 1):
-        t = lm.kv[layer, which].index_select(0, pages)                     # [npg, n_kv, 64, 64]
-        out.append(t.permute(0, 2, 1, 3).reshape(npg * PAGE, t.shape[1], 64)[:n].double().cpu())
-    return out[0], out[1]
-
-
 def ref_attention(q, k, v, n_rep: int, causal_offset: int | None = None, mirror: str | None = None):
     """Attention in float64.  q: [Tq, Hq, 64]; k, v: [Tk, Hkv, 64]; query head h reads KV head h // n_rep.
     ``causal_offset``: key position of q[0]; query i sees keys 0..causal_offset + i (None: every key).
@@ -106,13 +94,6 @@ def rope64(x, pos: int, theta: float):
 
 def rmsnorm64(x, eps: float):
     return x / torch.sqrt(x.pow(2).mean() + eps)
-
-
-def rel_rms(got, ref) -> float:
-    """Relative RMS error; inf when ``got`` holds a NaN or an inf (so that max() over errors cannot drop it)."""
-    if not torch.isfinite(got).all():
-        return math.inf
-    return float((got.double() - ref.double()).norm() / ref.double().norm().clamp_min(1e-300))
 
 
 def per_head_err(got, ref) -> float:
