@@ -201,6 +201,27 @@ int nt_lm_set_slot_sampling(nt_lm* lm, const nt_slot_sampling* host_table, void*
  * nt_op_topk_sample and nt_lm_head_gemv ignore the range. */
 int nt_lm_set_vocab_range(nt_lm* lm, int32_t lo, int32_t hi, void* stream);
 
+/* Per-slot repetition penalty (transformers' RepetitionPenaltyLogitsProcessor).  Each slot's history is the set of
+ * distinct ids of the prompt its last nt_lm_prefill / nt_lm_prefill_slots filled it with (include_prompt = 1), plus
+ * every token written to out_tokens for it since (teacher-forced runs: the forced token).  Every id in the history
+ * has its logit s replaced once by s < 0 ? s * penalty : s / penalty (IEEE fp32), before the EOS mask, the vocabulary
+ * range and the temperature; it applies to greedy and teacher-forced runs too.  Every logits output and tile maximum
+ * holds the penalised scores; every id outside the history is bit-identical to the table off.
+ * The history lives on the device: a bitmap of the vocabulary per slot, built by each prefill and updated by the
+ * sampler itself, so the token drawn at step t is penalised at step t + 1 inside one multi-step launch. */
+typedef struct {
+  float penalty;          /* finite, > 0; 1 = no penalty for this slot */
+  int32_t include_prompt; /* 1: prompt ids count (transformers' default), 0: only generated ids */
+} nt_slot_penalty;
+
+/* host_table: max_batch entries (row s = slot s), or NULL = off (the default: nothing recorded, nothing penalised).
+ * Every entry is validated first; a bad one returns NT_ERR_INVALID and leaves the previous table in force.  The copy is
+ * enqueued on `stream`.  Switching the table on marks every slot unrecorded: an unrecorded slot is not penalised until
+ * a prefill fills it again (tokens drawn while the table was off were never recorded).  New values in a table that
+ * stays on take effect at the next launch, and the histories are kept.
+ * nt_op_topk_sample and nt_lm_head_gemv ignore the penalty. */
+int nt_lm_set_repetition_penalty(nt_lm* lm, const nt_slot_penalty* host_table, void* stream);
+
 /* Timed single-kernel entry for the roofline measurement: the lm_head GEMV (+ final RMSNorm)
  * exactly as the decode step launches it.  h: f32 [B][hidden] -> logits f32 [B][vocab]. */
 int nt_lm_head_gemv(nt_lm* lm, const float* h, int B, float* logits, void* stream);

@@ -30,12 +30,14 @@ import torch
 SPEECH_RE = re.compile(r"<\|speech_(\d+)\|>")
 CHAT = "user: Convert the text to speech:<|TEXT_REPLACE|>\nassistant:<|SPEECH_REPLACE|>"
 CONTROL_DEFAULTS = dict(temperature=1.0, top_k=50, top_p=1.0, min_p=0.0)   # the reference's (neutts/neutts.py:338-347)
+PENALTY_DEFAULTS = dict(repetition_penalty=1.0, penalize_prompt=True)       # no repetition penalty, as the reference
 
 
-def _controls(n: int, temperature, top_k, top_p, min_p) -> dict:
+def _controls(n: int, temperature, top_k, top_p, min_p, repetition_penalty=1.0, penalize_prompt=True) -> dict:
     """Sampling controls of n utterances: each a scalar or one value per utterance (a list then)."""
     ctl = {}
-    for name, v in (("temperature", temperature), ("top_k", top_k), ("top_p", top_p), ("min_p", min_p)):
+    for name, v in (("temperature", temperature), ("top_k", top_k), ("top_p", top_p), ("min_p", min_p),
+                    ("repetition_penalty", repetition_penalty), ("penalize_prompt", penalize_prompt)):
         if isinstance(v, (list, tuple, np.ndarray, torch.Tensor)):
             v = [x.item() if hasattr(x, "item") else x for x in v]
             if len(v) != n:
@@ -51,9 +53,13 @@ def _pick(ctl: dict, idx) -> dict:
 
 def _backbone_kw(ctl: dict) -> dict:
     """generate kwargs: temperature and top_k always (as the reference passes them), top_p / min_p only when they are
-    in use, so that backbones without them keep working."""
+    in use, and the repetition penalty pair only when it differs from the defaults, so that backbones without them keep
+    working."""
     kw = dict(temperature=ctl["temperature"], top_k=ctl["top_k"])
     kw.update({k: ctl[k] for k in ("top_p", "min_p") if isinstance(ctl[k], list) or ctl[k] != CONTROL_DEFAULTS[k]})
+    pen = {k: ctl.get(k, v) for k, v in PENALTY_DEFAULTS.items()}
+    if any(isinstance(v, list) or v != PENALTY_DEFAULTS[k] for k, v in pen.items()):
+        kw.update(pen)
     return kw
 
 
@@ -307,25 +313,25 @@ class NeuTTS:
 
     # ------------------------------------------------------------------ public API
     def infer(self, text: str, ref_codes, ref_text: str, *, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0,
-              min_p: float = 0.0) -> np.ndarray:
+              min_p: float = 0.0, repetition_penalty: float = 1.0, penalize_prompt: bool = True) -> np.ndarray:
         """Text + reference voice -> 24 kHz float32 waveform (``neutts/neutts.py:216-243``).  The sampling controls
         default to the reference's values; see ``infer_batch``."""
         return self.infer_batch([text], [ref_codes], [ref_text], temperature=temperature, top_k=top_k, top_p=top_p,
-                                min_p=min_p)[0]
+                                min_p=min_p, repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt)[0]
 
     def infer_from_prompt_ids(self, prompts: Sequence[Sequence[int]], max_new_tokens: int | None = None,
                               min_new_tokens: int = 50, slot_base: int = 0, *, temperature=1.0, top_k=50, top_p=1.0,
-                              min_p=0.0) -> list:
+                              min_p=0.0, repetition_penalty=1.0, penalize_prompt=True) -> list:
         """Hot path only: prompt ids (host) -> waveforms (host).  Used by bench.py's end-to-end leg.
         ``slot_base`` offsets the sampler's Philox slot index so chunks / ranks under one seed draw independently.
         More prompts than ``max_batch`` go through the backbone's ``generate_queue`` when it has one.  Sampling
         controls as in ``infer_batch``."""
-        ctl = _controls(len(prompts), temperature, top_k, top_p, min_p)
+        ctl = _controls(len(prompts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)
         gen = self._generate_ids(prompts, max_new_tokens, min_new_tokens, slot_base, ctl)
         return [self._watermark(w) for w in self._decode_codes([self._ids_to_codes(g) for g in gen])]
 
     def infer_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], distributed: bool = False, *,
-                    temperature=1.0, top_k=50, top_p=1.0, min_p=0.0) -> list:
+                    temperature=1.0, top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0, penalize_prompt=True) -> list:
         """List in / list out.  With ``distributed=True`` (inside an initialised torch.distributed job) the
         utterances are sharded over ranks and every rank returns all waveforms (one all-gather).
 
@@ -338,10 +344,13 @@ class NeuTTS:
         Sampling controls (keyword-only; the defaults are the reference's): ``temperature`` (logits times 1 / T),
         ``top_k`` (1..64), ``top_p`` (nucleus, (0, 1]) and ``min_p`` ([0, 1)), applied in transformers' order.  Each
         is a scalar or a list with one value per utterance; a list follows its utterances through chunking, the queue
-        and the sharding over ranks."""
+        and the sharding over ranks.  ``repetition_penalty`` (transformers' RepetitionPenaltyLogitsProcessor: > 0, 1 =
+        off) divides the positive logits and multiplies the negative ones of every id already in the utterance, which
+        breaks loops of one repeated codec id; ``penalize_prompt=False`` leaves the prompt (the reference codes) out of
+        that history.  Both are scalars or one value per utterance too."""
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
-        ctl = _controls(len(texts), temperature, top_k, top_p, min_p)
+        ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)
         prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(texts, ref_codes, ref_texts)]
         queue = hasattr(self.backbone, "generate_queue")
 
@@ -368,19 +377,21 @@ class NeuTTS:
         return dist.all_gather_waveforms(local, mine, len(prompts), device=self.codec.device)
 
     def infer_stream(self, text: str, ref_codes, ref_text: str, *, temperature: float = 1.0, top_k: int = 50,
-                     top_p: float = 1.0, min_p: float = 0.0) -> Generator[np.ndarray, None, None]:
+                     top_p: float = 1.0, min_p: float = 0.0, repetition_penalty: float = 1.0,
+                     penalize_prompt: bool = True) -> Generator[np.ndarray, None, None]:
         """Streaming synthesis with the reference's window geometry (``neutts/neutts.py:373-465``):
         every 25 new frames (once 5 look-ahead frames exist) the codec re-decodes
         [n - 50 - 1, n + 25 + 5 + 1) and the chunk is cross-faded with triangular weights.  Sampling controls as in
         ``infer_batch``."""
         if self._is_quantized_model:  # kept for signature parity; never true on this build
             raise NotImplementedError("GGUF streaming is not part of the H100 build")
-        ctl = _controls(1, temperature, top_k, top_p, min_p)
+        ctl = _controls(1, temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)
         prompt = self._apply_chat_template(ref_codes, ref_text, text)
         return self._stream(prompt, [int(c) for c in (ref_codes.tolist() if hasattr(ref_codes, "tolist") else ref_codes)], ctl)
 
     def infer_stream_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], *, temperature=1.0,
-                           top_k=50, top_p=1.0, min_p=0.0) -> Generator[list, None, None]:
+                           top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0,
+                           penalize_prompt=True) -> Generator[list, None, None]:
         """Streaming synthesis of up to ``max_batch`` utterances at once (BASELINE.json configs[4]; the reference
         streams one utterance, ``neutts/neutts.py:373-465``).  Every yield is a list with one entry per utterance:
         the next audio chunk (float32, cross-faded exactly as in ``infer_stream``) or ``None`` when that utterance
@@ -388,7 +399,7 @@ class NeuTTS:
         that are due are gathered on the device from the code history and go through the codec as one batch."""
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
-        ctl = _controls(len(texts), temperature, top_k, top_p, min_p)
+        ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)
         prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(texts, ref_codes, ref_texts)]
         refs = [[int(c) for c in (rc.tolist() if hasattr(rc, "tolist") else rc)] for rc in ref_codes]
         return self._stream_batch(prompts, refs, ctl)
@@ -419,14 +430,17 @@ class NeuTTS:
         if min(limits) < 1:
             raise ValueError("prompt already at max_length")
         limit = max(limits)
-        from neutts_air_b200.lm import per_prompt_controls
+        from neutts_air_b200.lm import per_prompt_controls, per_prompt_penalty
 
         ctl = ctl if ctl is not None else CONTROL_DEFAULTS
-        rows = per_prompt_controls(B, **ctl)   # None: scalar controls without top-p / min-p
+        rows = per_prompt_controls(B, **{k: ctl[k] for k in CONTROL_DEFAULTS})   # None: scalar controls without top-p / min-p
+        pen_rows = per_prompt_penalty(B, *(ctl.get(k, v) for k, v in PENALTY_DEFAULTS.items()))   # None: no penalty
         top_k, temp = (ctl["top_k"], ctl["temperature"]) if rows is None else (rows[0][1], rows[0][0])
         sp = lm.sampling(eos, 50, limit, top_k, temp, seed) if min(limits) == limit else lm.sampling(eos, 50, limit, top_k, temp, seed, limits=limits)
         if rows is not None or getattr(lm, "_slot_sp_host", None) is not None:
             lm.set_slot_sampling(rows)   # before the prefill, on the same stream
+        if pen_rows is not None or getattr(lm, "_penalty_host", None) is not None:
+            lm.set_repetition_penalty(pen_rows)   # before the prefill that records the prompts
         rng = self._speech_range()
         if rng is not None or getattr(lm, "_vocab_range", None) is not None:
             lm.set_vocab_range(*(rng if rng is not None else (None,)))

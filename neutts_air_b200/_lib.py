@@ -65,6 +65,10 @@ class SlotSampling(C.Structure):
     _fields_ = [("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float), ("min_p", C.c_float)]
 
 
+class SlotPenalty(C.Structure):
+    _fields_ = [("penalty", C.c_float), ("include_prompt", C.c_int32)]
+
+
 class CodecConfig(C.Structure):
     _fields_ = [
         ("hidden", C.c_int), ("depth", C.c_int), ("heads", C.c_int), ("head_dim", C.c_int),
@@ -93,7 +97,8 @@ class CodecWeights(C.Structure):
 EXPORTS = [
     "nt_last_error", "nt_abi_version", "nt_launch_count", "nt_gemm",
     "nt_lm_workspace_bytes", "nt_lm_create", "nt_lm_destroy", "nt_lm_prefill", "nt_lm_prefill_slots", "nt_lm_decode",
-    "nt_lm_set_slot_sampling", "nt_lm_set_vocab_range", "nt_lm_head_gemv",
+    "nt_lm_set_slot_sampling", "nt_lm_set_vocab_range", "nt_lm_set_repetition_penalty",
+    "nt_lm_head_gemv",
     "nt_lm_debug_set_layers", "nt_lm_debug_ptr", "nt_lm_debug_set_profile", "nt_lm_debug_capture_sampler",
     "nt_debug_launch_chain", "nt_debug_decode_plan",
     "nt_codec_workspace_bytes", "nt_codec_create", "nt_codec_destroy", "nt_codec_decode",
@@ -131,6 +136,7 @@ def lib() -> C.CDLL:
     L.nt_lm_decode.argtypes = [C.c_void_p, C.POINTER(LMState), C.c_int, C.c_int, C.POINTER(Sampling), C.c_void_p, C.c_void_p]
     L.nt_lm_set_slot_sampling.argtypes = [C.c_void_p, C.POINTER(SlotSampling), C.c_void_p]
     L.nt_lm_set_vocab_range.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
+    L.nt_lm_set_repetition_penalty.argtypes = [C.c_void_p, C.POINTER(SlotPenalty), C.c_void_p]
     L.nt_lm_head_gemv.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     L.nt_lm_debug_set_layers.argtypes = [C.c_void_p, C.c_int]
     L.nt_lm_debug_ptr.restype = C.c_void_p

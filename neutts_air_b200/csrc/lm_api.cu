@@ -126,6 +126,12 @@ struct nt_lm {
   // vocabulary range (nt_lm_set_vocab_range): allowed ids [vr_lo, vr_hi) + EOS while vr_on
   bool vr_on = false;
   int vr_lo = 0, vr_hi = 0;
+  // repetition penalty (nt_lm_set_repetition_penalty): history bitmaps, the per-slot table and "recorded" flags
+  uint32_t* rep_hist = nullptr;       // [max_batch][rep_words]
+  nt_slot_penalty* rep_tab = nullptr; // [max_batch]
+  int* rep_rec = nullptr;             // [max_batch] 1: the slot's history was built by a prefill while the table was on
+  int rep_words = 0;                  // ceil(vocab_size / 32)
+  bool rep_on = false;
 };
 
 // The lm_head tiles a launch computes under the vocabulary range: [t_lo, t_hi), plus eos_tile when EOS lies outside
@@ -210,6 +216,10 @@ static size_t lm_carve(const nt_lm_config& c, void* ws, size_t bytes, F&& assign
     (L)->slot_args = a.take<int>(size_t(3) * c.max_batch);                                     \
     (L)->slot_table = a.take<int>(size_t(c.max_batch) * max_splits);                           \
     (L)->slot_sp = a.take<nt_slot_sampling>(c.max_batch);                                     \
+    (L)->rep_words = (V + 31) / 32;                                                            \
+    (L)->rep_hist = a.take<uint32_t>(size_t(c.max_batch) * ((V + 31) / 32));                   \
+    (L)->rep_tab = a.take<nt_slot_penalty>(c.max_batch);                                       \
+    (L)->rep_rec = a.take<int>(c.max_batch);                                                   \
   }
 
 static int lm_check_config(const nt_lm_config* c) {
@@ -384,6 +394,8 @@ static SamplerParams make_sampler(const nt_lm* lm, const nt_lm_state* st, const 
   s.slot_base = sp->slot_base;
   s.slot_key = lm->slot_key;
   s.slot_sp = lm->slot_sp_on ? lm->slot_sp : nullptr;
+  s.rep_hist = lm->rep_on ? lm->rep_hist : nullptr;
+  s.rep_words = lm->rep_words;
   s.dbg_topk_val = lm->dbg_topk_val, s.dbg_topk_idx = lm->dbg_topk_idx, s.dbg_token = lm->dbg_token;
   return s;
 }
@@ -406,12 +418,20 @@ static int run_sampler(nt_lm* lm, const SamplerParams& s, int B, cudaStream_t st
   return launch_sampler(s, B, stream);
 }
 
+// While the repetition penalty is on (and eos >= 0), one fix-up launch after the lm_head rewrites each history logit
+// of every row (row i holds slot row_slot[i], or slot i) and the raw tile maxima it changed.
+static int rep_fixup(nt_lm* lm, int B, float* logits, float* tmax, int eos, const int32_t* row_slot, cudaStream_t stream) {
+  if (eos < 0 || !lm->rep_on) return NT_OK;
+  const int V = lm->cfg.vocab_size;
+  return launch_rep_penalty(logits, B, V, lm->rep_hist, lm->rep_words, lm->rep_tab, lm->rep_rec, row_slot, tmax, (V + 127) / 128, stream);
+}
+
 // eos >= 0: apply the vocabulary range with this EOS id (every sampler launch); -1: every row (nt_lm_head_gemv).  Under
 // the range the lm_head runs once over the range's rows and once over the EOS tile (when EOS lies outside them), each
 // a row slice of the full-vocabulary launch with the same per-row arithmetic, so every computed logit is bit-identical
-// to the range off; the rows it does not compute keep the -inf of vocab_fill.
+// to the range off; the rows it does not compute keep the -inf of vocab_fill.  row_slot: see rep_fixup.
 static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cudaStream_t stream, const SplitK* pend = nullptr,
-                        int eos = -1) {
+                        int eos = -1, const int32_t* row_slot = nullptr) {
   const nt_lm_config& c = lm->cfg;
   const int V = c.vocab_size, nt = (V + 127) / 128;
   const VocabTiles vt = eos >= 0 ? vocab_tiles(lm, eos) : VocabTiles{false, 0, nt, -1};
@@ -430,7 +450,8 @@ static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cud
       g.epi = GEMV_STORE, g.out = logits + r0[i], g.ldo = V;
       if ((rc = launch_gemv(g, B, lm->num_sms, stream))) return rc;
     }
-    return vt.eos_tile >= 0 ? launch_vocab_eos_tile(logits, B, V, eos, nullptr, nt, stream) : NT_OK;
+    if (vt.eos_tile >= 0 && (rc = launch_vocab_eos_tile(logits, B, V, eos, nullptr, nt, stream))) return rc;
+    return rep_fixup(lm, B, logits, nullptr, eos, row_slot, stream);
   }
   // pend: the last down_proj left split-K slices that still have to be folded into hrows (batched decode only)
   const bool fold = pend && pend->used > 1;
@@ -444,7 +465,8 @@ static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cud
     a.dtype = NT_BF16, a.M = B, a.N = V, a.K = c.hidden;
     a.A = lm->xn, a.lda = c.hidden, a.W = lm->lm_head, a.ldw = c.hidden;
     a.out_f32 = logits, a.ldc = V;
-    return gemm_dispatch(a, stream, nullptr, true, nullptr, tmax);
+    if ((rc = gemm_dispatch(a, stream, nullptr, true, nullptr, tmax))) return rc;
+    return rep_fixup(lm, B, logits, tmax, eos, row_slot, stream);
   }
   // slices run at the full-vocabulary tile width; their tile maxima land at absolute tile indices (128-column tiles)
   const int bn = gemm_tile_n(B, V, false);
@@ -456,7 +478,8 @@ static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cud
     a.out_f32 = logits + r0[i], a.ldc = V;
     if ((rc = gemm_dispatch(a, stream, nullptr, true, nullptr, tmax ? tmax + r0[i] / 128 : nullptr, bn, nt))) return rc;
   }
-  return vt.eos_tile >= 0 ? launch_vocab_eos_tile(logits, B, V, eos, tmax, nt, stream) : NT_OK;
+  if (vt.eos_tile >= 0 && (rc = launch_vocab_eos_tile(logits, B, V, eos, tmax, nt, stream))) return rc;
+  return rep_fixup(lm, B, logits, tmax, eos, row_slot, stream);
 }
 
 // Transformer layers over `rows` token rows held in lm->h, via tensor-core GEMMs.
@@ -562,15 +585,19 @@ static int prefill_stage(nt_lm* lm, const int32_t* cu, int B, std::vector<int>& 
 }
 
 // Prompt rows -> KV cache + last-position logits in lm->logits (and logits_out).  table: see layers_gemm.
+// row_slot: the slot of every prompt row (nullptr: row b is slot b); it fills that slot's repetition-penalty history.
 static int prefill_forward(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, int B, int max_len,
-                           const int32_t* table, float* logits_out, int eos, cudaStream_t stream) {
+                           const int32_t* table, float* logits_out, int eos, cudaStream_t stream, const int32_t* row_slot = nullptr) {
   const nt_lm_config& c = lm->cfg;
   int rc;
   if ((rc = vocab_fill(lm, B, stream))) return rc;
+  if (lm->rep_on &&
+      (rc = launch_rep_history(lm->rep_hist, lm->rep_words, lm->rep_tab, lm->rep_rec, row_slot, ids, lm->cu_dev, B, c.vocab_size, stream)))
+    return rc;
   if ((rc = launch_embed_rows(lm->embed, ids, cu[B], c.hidden, lm->h, stream))) return rc;
   if ((rc = layers_gemm(lm, st, cu[B], B, 0, max_len, stream, nullptr, table))) return rc;
   if ((rc = launch_gather_rows(lm->h, lm->last_rows, B, c.hidden, lm->h_last, stream))) return rc;
-  if ((rc = lm_head_rows(lm, lm->h_last, B, lm->logits, stream, nullptr, eos))) return rc;
+  if ((rc = lm_head_rows(lm, lm->h_last, B, lm->logits, stream, nullptr, eos, row_slot))) return rc;
   if (logits_out)
     NT_CUDA_CHECK(cudaMemcpyAsync(logits_out, lm->logits, size_t(B) * c.vocab_size * sizeof(float), cudaMemcpyDeviceToDevice, stream));
   return NT_OK;
@@ -630,7 +657,7 @@ extern "C" int nt_lm_prefill_slots(nt_lm* lm, const nt_lm_state* st, const int32
   if ((rc = launch_slots_setup(lm->slot_args, B, st->page_table, max_pages, lm->slot_table, st->seq_lens, st->n_generated, st->done,
                                lm->slot_key, stream)))
     return rc;
-  if ((rc = prefill_forward(lm, st, ids, cu, B, max_len, lm->slot_table, logits_out, sp->eos_id, stream))) return rc;
+  if ((rc = prefill_forward(lm, st, ids, cu, B, max_len, lm->slot_table, logits_out, sp->eos_id, stream, lm->slot_args))) return rc;
   SamplerParams s = make_sampler(lm, st, sp);
   s.row_slot = lm->slot_args;
   s.h = nullptr;  // the residual rows are rebuilt below, for every slot
@@ -749,6 +776,7 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
     P.head_eos_at = vt.eos_tile < 0 ? -1 : (vt.eos_tile < vt.t_lo ? 0 : vt.t_hi - vt.t_lo);
     P.samp = make_sampler(lm, st, sp);
     P.samp.advance = 1;
+    P.rep_tab = lm->rep_on ? lm->rep_tab : nullptr, P.rep_rec = lm->rep_rec;
     P.gbar = lm->gbar;
     P.n_steps = n_steps;
     P.logits_out = logits_out;
@@ -850,6 +878,33 @@ extern "C" int nt_lm_set_vocab_range(nt_lm* lm, int32_t lo, int32_t hi, void* st
   lm->vr_on = on;
   lm->vr_lo = on ? lo : 0;
   lm->vr_hi = on ? hi : 0;
+  return NT_OK;
+}
+
+extern "C" int nt_lm_set_repetition_penalty(nt_lm* lm, const nt_slot_penalty* table, void* stream_) {
+  if (!lm) return set_error(NT_ERR_INVALID, "nt_lm_set_repetition_penalty: null handle");
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  const bool on = table != nullptr;
+  if (on) {
+    for (int s = 0; s < lm->cfg.max_batch; ++s) {
+      const nt_slot_penalty& e = table[s];
+      if (!(std::isfinite(e.penalty) && e.penalty > 0.f))
+        return set_error(NT_ERR_INVALID, "slot %d: repetition penalty %g must be finite and > 0", s, e.penalty);
+      if (e.include_prompt != 0 && e.include_prompt != 1)
+        return set_error(NT_ERR_INVALID, "slot %d: include_prompt=%d must be 0 or 1", s, e.include_prompt);
+    }
+    // switching on: no slot holds a history yet (tokens drawn while the table was off were never recorded)
+    if (!lm->rep_on) NT_CUDA_CHECK(cudaMemsetAsync(lm->rep_rec, 0, size_t(lm->cfg.max_batch) * sizeof(int), stream));
+    // pageable source: the runtime has staged it by the time the call returns
+    NT_CUDA_CHECK(cudaMemcpyAsync(lm->rep_tab, table, size_t(lm->cfg.max_batch) * sizeof(nt_slot_penalty), cudaMemcpyHostToDevice, stream));
+  }
+  // the cached decode graph holds the fix-up launch (or its absence) and the sampler's history pointer; new values in a
+  // table that stays on are read at the next replay
+  if (on != lm->rep_on && lm->graph) {
+    cudaGraphExecDestroy(lm->graph);
+    lm->graph = nullptr;
+  }
+  lm->rep_on = on;
   return NT_OK;
 }
 

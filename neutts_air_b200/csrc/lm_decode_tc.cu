@@ -151,6 +151,7 @@ struct TcMisc {
   int apage[32];          // physical pages of this CTA's attention split (this step)
   int mask_eos[kTcMaxBatch];
   float inv_t[kTcMaxBatch];   // 1 / temperature per sequence (the launch's sampling controls)
+  float rep_pen[kTcMaxBatch]; // repetition penalty per sequence (1: none, or the slot is unrecorded)
   float red[64];
   float tile_max[2][4][kTcMaxBatch];
   float rstd[8];
@@ -206,7 +207,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
   }
   for (int i = tid; i < static_cast<int>(sizeof(TcPlan) / 4); i += kTcThreads)
     reinterpret_cast<int*>(&ms->plan)[i] = reinterpret_cast<const int*>(P.plan + blockIdx.x)[i];
-  if (tid < B) ms->inv_t[tid] = row_sampling(P.samp, tid).inv_t;
+  if (tid < B) {
+    ms->inv_t[tid] = row_sampling(P.samp, tid).inv_t;
+    ms->rep_pen[tid] = (P.rep_tab && P.rep_rec[tid]) ? P.rep_tab[tid].penalty : 1.f;
+  }
   __syncthreads();
   const TcPlan& plan = ms->plan;
   if (tid < 4) {  // chunk tables of the split phases (items in plan order, k-blocks ascending)
@@ -946,6 +950,18 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
         const bool ok = row < V;
         const bool allowed = tile != P.head_eos || row == eos;   // the EOS tile outside the vocabulary range: EOS only
         float (*tm)[kTcMaxBatch] = ms->tile_max[t & 1];
+        // repetition penalty, before the store and the processed maximum: this warp's 32 rows are one bitmap word per
+        // column (a broadcast load); the bits were set by the sampler of the previous step, behind a grid barrier
+        const int wi = tile * 4 + warp;
+        if (P.rep_tab && wi < P.samp.rep_words) {   // warp-uniform
+#pragma unroll
+          for (int n = 0; n < NTOK; ++n) {
+            if (n < B && ms->rep_pen[n] != 1.f) {
+              const uint32_t word = __ldcg(P.samp.rep_hist + static_cast<long long>(n) * P.samp.rep_words + wi);
+              if ((word >> lane) & 1u) v[n] = rep_penalize(v[n], ms->rep_pen[n]);
+            }
+          }
+        }
         float pv[NTOK];
 #pragma unroll
         for (int n = 0; n < NTOK; ++n) {

@@ -80,6 +80,9 @@ struct TcParams {
   // tile).  Range on: the range's tiles, plus the EOS tile when it lies outside them (only EOS is allowed there).
   int head_n, head_lo, head_eos, head_eos_at;
   SamplerParams samp;
+  // repetition penalty: per-slot table and recorded flags (nullptr = off); the history bitmap is samp.rep_hist
+  const nt_slot_penalty* rep_tab;
+  const int32_t* rep_rec;
   unsigned* gbar;
   int n_steps;
   float* logits_out;

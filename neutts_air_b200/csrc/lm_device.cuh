@@ -262,6 +262,10 @@ NT_DEVINL RowSampling row_sampling(const SamplerParams& p, int slot) {
   return r;
 }
 
+// RepetitionPenaltyLogitsProcessor on one score of an id in the history: a true IEEE division (not a product with the
+// reciprocal), so the result is bit-identical to torch's fp32 `score / penalty`; -inf stays -inf
+NT_DEVINL float rep_penalize(float s, float penalty) { return s < 0.f ? __fmul_rn(s, penalty) : __fdiv_rn(s, penalty); }
+
 // logits processors (MinNewTokensLength -> Temperature), then the order-preserving key
 NT_DEVINL uint32_t processed_key(float logit, int idx, bool mask_eos, int eos_id, float inv_t) {
   if (mask_eos && idx == eos_id) logit = -INFINITY;
@@ -374,6 +378,9 @@ NT_DEVINL void sample_finish(const SamplerParams& p, int b, int k, Cand* win, in
       if (p.dbg_token) p.dbg_token[b] = tok;
       if (!stateless && !is_done) {
         p.out_tokens[static_cast<long long>(s) * p.max_new + ngen] = tok;
+        // the history bit of this token: the persistent kernel's epi_head reads it at the next step, behind the grid
+        // barrier this thread arrives at after the sampler (see DESIGN.md §4, repetition penalty)
+        if (p.rep_hist) atomicOr(p.rep_hist + static_cast<long long>(s) * p.rep_words + (tok >> 5), 1u << (tok & 31));
         p.n_generated[s] = ngen + 1;
         p.cur_token[s] = tok;
         const int cached = __ldcg(p.seq_lens + s) + p.advance;  // decode: this step's input token is now in the KV cache

@@ -859,6 +859,81 @@ int launch_vocab_eos_tile(float* logits, int B, int V, int eos, float* tmax, int
   return launch_kernel(vocab_eos_tile_kernel, dim3(B), dim3(128), 0, s, true, logits, V, eos, tmax, nt);
 }
 
+// =================================================================================== repetition penalty
+// grid B, 256 threads: the history row of one slot is built in shared memory (ceil(V / 32) words) and written once
+__global__ void __launch_bounds__(256) rep_history_kernel(uint32_t* hist, int words, const nt_slot_penalty* tab, int32_t* recorded,
+                                                          const int32_t* row_slot, const int32_t* ids, const int32_t* cu, int V) {
+  extern __shared__ uint32_t rep_row[];
+  pdl_launch_dependents();
+  pdl_wait();
+  const int i = blockIdx.x, s = row_slot ? row_slot[i] : i;
+  for (int w = threadIdx.x; w < words; w += blockDim.x) rep_row[w] = 0u;
+  __syncthreads();
+  if (tab[s].include_prompt) {
+    for (int t = cu[i] + threadIdx.x; t < cu[i + 1]; t += blockDim.x) {
+      const int id = ids[t];
+      if (id >= 0 && id < V) atomicOr(&rep_row[id >> 5], 1u << (id & 31));
+    }
+  }
+  __syncthreads();
+  uint32_t* dst = hist + static_cast<long long>(s) * words;
+  for (int w = threadIdx.x; w < words; w += blockDim.x) dst[w] = rep_row[w];
+  if (threadIdx.x == 0) recorded[s] = 1;
+}
+int launch_rep_history(uint32_t* hist, int words, const nt_slot_penalty* tab, int32_t* recorded, const int32_t* row_slot,
+                       const int32_t* ids, const int32_t* cu, int B, int V, cudaStream_t s) {
+  return launch_kernel(rep_history_kernel, dim3(B), dim3(256), size_t(words) * sizeof(uint32_t), s, true, hist, words, tab, recorded,
+                       row_slot, ids, cu, V);
+}
+
+// grid (B, kRepSplit), 256 threads: the kRepSplit CTAs of row i share its tiles.  A warp takes 8 tiles (32 bitmap
+// words, one per lane) at a time and skips the tiles with no id in the history (a 500-token prompt touches ~40 % of
+// the Air vocabulary's tiles, and one warp walking them in series is latency-bound); lane l owns rows tile * 128 + 4 l .. + 3, i.e. bits 4 (l % 8) .. + 3 of the tile's word l / 8.  The
+// history ids are distinct, so every logit is rewritten once and each tile belongs to one warp (no race).
+__global__ void __launch_bounds__(256) rep_penalty_kernel(float* logits, int V, const uint32_t* hist, int words, const nt_slot_penalty* tab,
+                                                          const int32_t* recorded, const int32_t* row_slot, float* tmax, int nt) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int i = blockIdx.x, s = row_slot ? row_slot[i] : i;
+  const float pen = tab[s].penalty;
+  if (!recorded[s] || pen == 1.f) return;
+  const uint32_t* hrow = hist + static_cast<long long>(s) * words;
+  float* lg = logits + static_cast<long long>(i) * V;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nw = (blockDim.x >> 5) * gridDim.y;
+  for (int g = blockIdx.y * (blockDim.x >> 5) + warp; g * 8 < nt; g += nw) {
+    const int w = g * 32 + lane;
+    const uint32_t word = w < words ? __ldcg(hrow + w) : 0u;
+    const uint32_t any = __ballot_sync(0xffffffffu, word != 0u);
+    for (int j = 0; j < 8; ++j) {
+      if (!((any >> (4 * j)) & 0xfu)) continue;   // warp-uniform
+      const int tile = g * 8 + j;
+      const uint32_t bits = (__shfl_sync(0xffffffffu, word, 4 * j + (lane >> 3)) >> (4 * (lane & 7))) & 0xfu;
+      float m = -INFINITY;
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int r = tile * 128 + 4 * lane + q;
+        if (r < V) {
+          float v = lg[r];
+          if ((bits >> q) & 1u) {
+            v = rep_penalize(v, pen);
+            lg[r] = v;
+          }
+          m = fmaxf(m, v);
+        }
+      }
+      m = warp_max(m);
+      if (tmax && lane == 0) tmax[static_cast<long long>(i) * nt + tile] = m;
+    }
+  }
+}
+int launch_rep_penalty(float* logits, int B, int V, const uint32_t* hist, int words, const nt_slot_penalty* tab,
+                       const int32_t* recorded, const int32_t* row_slot, float* tmax, int nt, cudaStream_t s) {
+  constexpr int kRepSplit = 16;
+  return launch_kernel(rep_penalty_kernel, dim3(B, kRepSplit), dim3(256), 0, s, true, logits, V, hist, words, tab, recorded, row_slot,
+                       tmax, nt);
+}
+
 // =================================================================================== prefill helpers
 __global__ void embed_rows_kernel(const __nv_bfloat16* embed, const int32_t* ids, int hidden, float* h) {
   pdl_launch_dependents();

@@ -97,6 +97,10 @@ struct SamplerParams {
   // optional [max_batch] temperature / top_k / top_p / min_p per slot (nt_lm_set_slot_sampling), read through
   // row_sampling() with the row's slot; nullptr: sp.temperature and sp.top_k for every row, no top-p / min-p cut
   const nt_slot_sampling* slot_sp;
+  // repetition penalty (nt_lm_set_repetition_penalty): [max_batch][rep_words] history bitmap of every slot, nullptr =
+  // off.  sample_finish sets the bit of every token it writes to out_tokens.
+  uint32_t* rep_hist;
+  int rep_words;
 };
 int launch_sampler(const SamplerParams& p, int B, cudaStream_t stream);
 int launch_sampler_check(const SamplerParams& p);
@@ -110,6 +114,15 @@ size_t sampler_scratch_floats(int B, int V);  // per-array element count for can
 int launch_fill_neg_inf(float* p, long long n, cudaStream_t s);
 int launch_vocab_eos_tile(float* logits, int B, int V, int eos, float* tmax, int nt, cudaStream_t s);
 int sampler_nchunks(int V);
+// Repetition penalty.  launch_rep_history: one CTA per prefill row i builds the history row of slot row_slot[i] (row i
+// when row_slot is nullptr): cleared, then the ids ids[cu[i] .. cu[i + 1]) when the slot's entry includes the prompt;
+// the slot becomes recorded.  launch_rep_penalty: the CTAs of logits row i of `logits` [B][V] rewrite the logit of
+// every id in slot row_slot[i]'s history (recorded slots with a penalty != 1 only) and recompute the raw maximum of
+// every 128-row tile it touched in tmax [B][nt] (optional).
+int launch_rep_history(uint32_t* hist, int words, const nt_slot_penalty* tab, int32_t* recorded, const int32_t* row_slot,
+                       const int32_t* ids, const int32_t* cu, int B, int V, cudaStream_t s);
+int launch_rep_penalty(float* logits, int B, int V, const uint32_t* hist, int words, const nt_slot_penalty* tab,
+                       const int32_t* recorded, const int32_t* row_slot, float* tmax, int nt, cudaStream_t s);
 
 int launch_embed_rows(const __nv_bfloat16* embed, const int32_t* ids, int T, int hidden, float* h, cudaStream_t s);
 // parts != nullptr: x is updated in place first (x += sum of nparts split-K slices, slice order) -- see SplitK

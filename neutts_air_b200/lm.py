@@ -167,6 +167,40 @@ def check_vocab_range(vocab_range, vocab_size: int):
     return lo, hi
 
 
+DEFAULT_PENALTY = (1.0, True)   # repetition penalty, prompt included: transformers' RepetitionPenaltyLogitsProcessor
+
+
+def check_penalty(penalty, include_prompt=True) -> tuple:
+    """One slot's repetition penalty, validated as ``nt_lm_set_repetition_penalty`` does -> (float, bool).  The penalty
+    must be finite and > 0 in fp32 (1 = none); ``include_prompt``: the prompt's ids count (transformers' default)."""
+    if isinstance(penalty, bool) or not isinstance(penalty, (int, float, np.integer, np.floating)):
+        raise ValueError(f"repetition penalty {penalty!r} must be a number")
+    p = float(penalty)
+    with np.errstate(over="ignore"):
+        f = float(np.float32(p)) if math.isfinite(p) else p   # the value the library stores
+    if not (math.isfinite(f) and f > 0):
+        raise ValueError(f"repetition penalty {penalty} must be finite and > 0")
+    if not isinstance(include_prompt, (bool, int, np.integer, np.bool_)) or int(include_prompt) not in (0, 1):
+        raise ValueError(f"penalize_prompt {include_prompt!r} must be a bool")
+    return p, bool(include_prompt)
+
+
+def per_prompt_penalty(n: int, penalty, include_prompt):
+    """Repetition penalties of n prompts, each argument a scalar or one value per prompt.  Returns None when every
+    penalty is 1 (nothing to penalise: no engine call), else one validated (penalty, include_prompt) per prompt."""
+    cols = []
+    for name, v in (("repetition_penalty", penalty), ("penalize_prompt", include_prompt)):
+        if _is_seq(v):
+            v = [x.item() if hasattr(x, "item") else x for x in v]
+            if len(v) != n:
+                raise ValueError(f"{name} needs one value per prompt ({n}), got {len(v)}")
+            cols.append(v)
+        else:
+            cols.append([v] * n)
+    rows = [check_penalty(p, i) for p, i in zip(*cols)]
+    return None if all(r[0] == 1.0 for r in rows) else rows
+
+
 PLAN_PHASES = ("qkv", "o", "gu", "d")   # phase order of the persistent kernel's work plan
 
 
@@ -246,6 +280,7 @@ class SpeechLM:
         self._slot_pages = [[] for _ in range(max_batch)]
         self._slot_sp_host = None   # host mirror of the per-slot sampling controls (None: off)
         self._vocab_range = None    # (lo, hi) while the vocabulary range is on
+        self._penalty_host = None   # host mirror of the per-slot repetition penalties (None: off)
 
     def __del__(self):
         try:
@@ -327,6 +362,35 @@ class SpeechLM:
             self.set_vocab_range(*vocab_range)
         elif getattr(self, "_vocab_range", None) is not None:
             self.set_vocab_range(None)
+
+    def set_repetition_penalty(self, rows, slots=None) -> None:
+        """Per-slot repetition penalty (transformers' ``RepetitionPenaltyLogitsProcessor``).  ``rows``: one
+        (penalty, include_prompt) per slot of ``slots`` (default: slots 0..len(rows) - 1); every other slot keeps its
+        entry, or (1.0, True) when the table was off.  A slot's history is its prompt (when include_prompt) plus every
+        token generated for it since; it is recorded from the slot's next prefill, so switch the table on before the
+        prefill whose tokens should count.  ``None`` switches the table off.  The table is copied on the current stream,
+        so it is ordered before the next prefill or decode."""
+        if rows is None:
+            _lib.check(self.L.nt_lm_set_repetition_penalty(self.handle, None, _lib.current_stream_ptr()))
+            self._penalty_host = None
+            return
+        rows = [check_penalty(*r) for r in rows]
+        slots = list(range(len(rows))) if slots is None else [int(s) for s in slots]
+        if len(slots) != len(rows) or len(set(slots)) != len(slots) or any(not 0 <= s < self.max_batch for s in slots):
+            raise ValueError(f"slots must be distinct, in 0..{self.max_batch - 1} and one per row")
+        table = list(self._penalty_host or [DEFAULT_PENALTY] * self.max_batch)
+        for s, r in zip(slots, rows):
+            table[s] = r
+        arr = (_lib.SlotPenalty * self.max_batch)(*(_lib.SlotPenalty(p, int(i)) for p, i in table))
+        with torch.cuda.device(self.device):
+            _lib.check(self.L.nt_lm_set_repetition_penalty(self.handle, arr, _lib.current_stream_ptr()))
+        self._penalty_host = table
+
+    def _use_penalty(self, rows) -> None:
+        """Slots 0..len(rows) - 1 take ``rows``; None leaves the table off (switching it off only if an earlier call
+        left it on), so a default call makes no engine call."""
+        if rows is not None or getattr(self, "_penalty_host", None) is not None:
+            self.set_repetition_penalty(rows)
 
     def prefill(self, prompts, sp, return_logits: bool = False):
         """prompts: list of 1-D int sequences.  Fills the KV cache and samples the first token."""
@@ -498,15 +562,19 @@ class SpeechLM:
     def generate_batch(self, prompts, eos_token_id: int, max_length: int | None = None, min_new_tokens: int = 50,
                        temperature: float = 1.0, top_k: int = 50, max_new_tokens: int | None = None, seed: int = 0,
                        greedy: bool = False, forced: torch.Tensor | None = None, check_every: int = 64, slot_base: int = 0,
-                       top_p: float = 1.0, min_p: float = 0.0, vocab_range=None):
+                       top_p: float = 1.0, min_p: float = 0.0, vocab_range=None, repetition_penalty=1.0,
+                       penalize_prompt=True):
         """Returns a list of int64 CPU tensors with the generated ids of each prompt (EOS included
         when it was sampled), following transformers' stopping rules (stopping_criteria.py:73-84,
         467-471): stop at EOS or when prompt + generated reaches max_length.  ``max_new_tokens`` may also be a
         list with one cap per prompt.  ``temperature``, ``top_k``, ``top_p`` and ``min_p`` are each a scalar or one
         value per prompt (per-slot controls, ``set_slot_sampling``).  ``vocab_range``: (lo, hi) restricts every draw to
-        [lo, hi) plus EOS (``set_vocab_range``); None leaves the range off."""
+        [lo, hi) plus EOS (``set_vocab_range``); None leaves the range off.  ``repetition_penalty`` (> 0, 1 = off) and
+        ``penalize_prompt`` (the prompt's ids count) are each a scalar or one value per prompt
+        (``set_repetition_penalty``); they apply to greedy and teacher-forced runs too."""
         if vocab_range is not None:   # validated before any engine call
             vocab_range = check_vocab_range(vocab_range, self.shape.vocab_size)
+        pen_rows = per_prompt_penalty(len(prompts), repetition_penalty, penalize_prompt)
         max_length = max_length or self.max_ctx
         if max_length > self.max_ctx:
             raise ValueError(f"max_length {max_length} exceeds the engine context {self.max_ctx}")
@@ -524,6 +592,7 @@ class SpeechLM:
                            limits=caps if min(caps) < limit else None, slot_base=slot_base)
         self._use_controls(rows)
         self._use_vocab_range(vocab_range)
+        self._use_penalty(pen_rows)
         self.prefill(prompts, sp)
         remaining = limit - 1
         B = len(prompts)
@@ -540,7 +609,7 @@ class SpeechLM:
     def generate_queue(self, prompts, eos_token_id: int, max_length: int | None = None, min_new_tokens: int = 50,
                        temperature: float = 1.0, top_k: int = 50, max_new_tokens: int | None = None, seed: int = 0,
                        greedy: bool = False, check_every: int = 32, slot_base: int = 0, top_p: float = 1.0,
-                       min_p: float = 0.0, vocab_range=None):
+                       min_p: float = 0.0, vocab_range=None, repetition_penalty=1.0, penalize_prompt=True):
         """Continuous batching over any number of prompts: ``generate_batch``'s results and stopping rules, but a slot
         whose sequence finished is refilled with the next waiting prompt while the other slots keep decoding.
 
@@ -553,9 +622,11 @@ class SpeechLM:
         CPU tensors, EOS included when sampled) in input order; every KV page is back in the pool afterwards.
         ``temperature``, ``top_k``, ``top_p`` and ``min_p`` are each a scalar or one value per prompt; a newcomer's
         controls are written into its slot before its prefill, and the other slots keep theirs.  ``vocab_range`` as in
-        ``generate_batch``: set once before the first prefill, it holds across every refill."""
+        ``generate_batch``: set once before the first prefill, it holds across every refill.  ``repetition_penalty`` and
+        ``penalize_prompt`` as in ``generate_batch``; a newcomer's entry is written before its prefill."""
         if vocab_range is not None:   # validated before any engine call
             vocab_range = check_vocab_range(vocab_range, self.shape.vocab_size)
+        pen_rows = per_prompt_penalty(len(prompts), repetition_penalty, penalize_prompt)
         max_length = max_length or self.max_ctx
         if max_length > self.max_ctx:
             raise ValueError(f"max_length {max_length} exceeds the engine context {self.max_ctx}")
@@ -576,6 +647,7 @@ class SpeechLM:
                            limits=caps[:S], slot_base=slot_base)
         self._use_controls(ctl_rows[:S] if ctl_rows is not None else None)
         self._use_vocab_range(vocab_range)
+        self._use_penalty(pen_rows[:S] if pen_rows is not None else None)
         self.prefill([prompts[i] for i in range(S)], sp)
         occ = list(range(S))   # prompt held by each slot, None once harvested
         ngen = [1] * S         # generated tokens per slot, as of the last read
@@ -600,6 +672,8 @@ class SpeechLM:
                         nxt += len(take)
                         if ctl_rows is not None:   # the newcomers' controls, before their prefill on the same stream
                             self.set_slot_sampling([ctl_rows[i] for i in idx], slots=take)
+                        if pen_rows is not None:
+                            self.set_repetition_penalty([pen_rows[i] for i in idx], slots=take)
                         self.prefill_slots(take, [prompts[i] for i in idx], sp, [slot_base + i for i in idx],
                                            limits=[caps[i] for i in idx])
                         for s, i in zip(take, idx):
@@ -620,10 +694,11 @@ class SpeechLM:
     def generate(self, input_ids: torch.Tensor, max_length: int = 2048, eos_token_id: int | None = None,
                  do_sample: bool = True, temperature: float = 1.0, top_k: int = 50, use_cache: bool = True,
                  min_new_tokens: int = 0, max_new_tokens: int | None = None, seed: int | None = None,
-                 top_p: float = 1.0, min_p: float = 0.0, vocab_range=None, **_):
+                 top_p: float = 1.0, min_p: float = 0.0, vocab_range=None, repetition_penalty: float = 1.0, **_):
         """transformers-compatible seam used by ``NeuTTS._infer_torch`` (neutts/neutts.py:338-347).  ``top_p`` and
         ``min_p`` act as transformers' TopPLogitsWarper / MinPLogitsWarper; ``vocab_range`` (lo, hi) suppresses every
-        id outside [lo, hi) and EOS (``set_vocab_range``); other generation kwargs are ignored."""
+        id outside [lo, hi) and EOS (``set_vocab_range``); ``repetition_penalty`` acts as transformers'
+        RepetitionPenaltyLogitsProcessor (prompt included); other generation kwargs are ignored."""
         if eos_token_id is None:
             raise ValueError("eos_token_id is required")
         if input_ids.dim() != 2:
@@ -634,6 +709,8 @@ class SpeechLM:
         cuts = {} if top_p == 1.0 and min_p == 0.0 else dict(top_p=top_p, min_p=min_p)
         if vocab_range is not None:
             cuts["vocab_range"] = vocab_range
+        if repetition_penalty is not None and repetition_penalty != 1.0:
+            cuts["repetition_penalty"] = repetition_penalty
         outs = self.generate_batch(prompts, eos_token_id, max_length, min_new_tokens, temperature, top_k,
                                    max_new_tokens, seed, greedy=not do_sample, **cuts)
         n = max(len(o) for o in outs)
