@@ -27,6 +27,8 @@ from typing import Generator, Sequence
 import numpy as np
 import torch
 
+from neutts_air_b200.lm import per_item, resolve_settings
+
 SPEECH_RE = re.compile(r"<\|speech_(\d+)\|>")
 CHAT = "user: Convert the text to speech:<|TEXT_REPLACE|>\nassistant:<|SPEECH_REPLACE|>"
 CONTROL_DEFAULTS = dict(temperature=1.0, top_k=50, top_p=1.0, min_p=0.0)   # the reference's (neutts/neutts.py:338-347)
@@ -35,15 +37,8 @@ PENALTY_DEFAULTS = dict(repetition_penalty=1.0, penalize_prompt=True)       # no
 
 def _controls(n: int, temperature, top_k, top_p, min_p, repetition_penalty=1.0, penalize_prompt=True) -> dict:
     """Sampling controls of n utterances: each a scalar or one value per utterance (a list then)."""
-    ctl = {}
-    for name, v in (("temperature", temperature), ("top_k", top_k), ("top_p", top_p), ("min_p", min_p),
-                    ("repetition_penalty", repetition_penalty), ("penalize_prompt", penalize_prompt)):
-        if isinstance(v, (list, tuple, np.ndarray, torch.Tensor)):
-            v = [x.item() if hasattr(x, "item") else x for x in v]
-            if len(v) != n:
-                raise ValueError(f"{name} needs one value per utterance ({n}), got {len(v)}")
-        ctl[name] = v
-    return ctl
+    return per_item(n, "utterance", temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p,
+                    repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt)
 
 
 def _pick(ctl: dict, idx) -> dict:
@@ -430,20 +425,10 @@ class NeuTTS:
         if min(limits) < 1:
             raise ValueError("prompt already at max_length")
         limit = max(limits)
-        from neutts_air_b200.lm import per_prompt_controls, per_prompt_penalty
-
-        ctl = ctl if ctl is not None else CONTROL_DEFAULTS
-        rows = per_prompt_controls(B, **{k: ctl[k] for k in CONTROL_DEFAULTS})   # None: scalar controls without top-p / min-p
-        pen_rows = per_prompt_penalty(B, *(ctl.get(k, v) for k, v in PENALTY_DEFAULTS.items()))   # None: no penalty
-        top_k, temp = (ctl["top_k"], ctl["temperature"]) if rows is None else (rows[0][1], rows[0][0])
+        st = resolve_settings(lm, B, vocab_range=self._speech_range(), **(ctl if ctl is not None else CONTROL_DEFAULTS))
+        top_k, temp = st.top_k, st.temperature
         sp = lm.sampling(eos, 50, limit, top_k, temp, seed) if min(limits) == limit else lm.sampling(eos, 50, limit, top_k, temp, seed, limits=limits)
-        if rows is not None or getattr(lm, "_slot_sp_host", None) is not None:
-            lm.set_slot_sampling(rows)   # before the prefill, on the same stream
-        if pen_rows is not None or getattr(lm, "_penalty_host", None) is not None:
-            lm.set_repetition_penalty(pen_rows)   # before the prefill that records the prompts
-        rng = self._speech_range()
-        if rng is not None or getattr(lm, "_vocab_range", None) is not None:
-            lm.set_vocab_range(*(rng if rng is not None else (None,)))
+        st.apply(lm, B)   # before the prefill, on the same stream
         dev = lm.out_tokens.device
         cap = max(len(r) for r in refs) + limit
         hist = torch.zeros(B, cap + 1, dtype=torch.long, device=dev)          # column `cap` is a scratch slot for masked writes

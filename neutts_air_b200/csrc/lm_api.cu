@@ -74,6 +74,18 @@ __global__ void noop_chain_kernel(int* p) {
 
 using namespace nt;
 
+// Host settings a decode step bakes into its launches, set by the nt_lm_set_* / nt_lm_debug_* calls.  The cached
+// decode graph is keyed by these bytes, so each setter only updates this struct.
+struct StepSettings {
+  float* dbg_topk_val = nullptr;      // sampler window capture (nt_lm_debug_capture_sampler): nullptr = off
+  int32_t *dbg_topk_idx = nullptr, *dbg_token = nullptr;
+  int debug_layers = -1;              // >= 0: run only this many layers (per-stage parity tests)
+  int vr_lo = 0, vr_hi = 0;           // vocabulary range (nt_lm_set_vocab_range): ids [vr_lo, vr_hi) + EOS; 0, 0 while off
+  bool vr_on = false;
+  bool slot_sp_on = false;            // per-slot sampling table (nt_lm_set_slot_sampling)
+  bool rep_on = false;                // repetition penalty table (nt_lm_set_repetition_penalty)
+};
+
 struct nt_lm {
   nt_lm_config cfg;
   int qkv_n, num_sms, max_splits, nchunks, max_rows;
@@ -97,12 +109,9 @@ struct nt_lm {
                                       // stream, which cannot be captured); replay on the caller's stream
   uint64_t graph_kernels = 0;         // kernel nodes in the captured step (for nt_launch_count)
   bool prefilled = false;
-  int debug_layers = -1;              // >= 0: run only this many layers (per-stage parity tests)
+  StepSettings step = StepSettings(); // value-initialised: its padding bytes, which the graph key compares, are zero
   long long* prof = nullptr;          // persistent decode kernel timeline buffer
   int prof_step = 0;
-  // sampler window capture (nt_lm_debug_capture_sampler): copied into every SamplerParams, nullptr = off
-  float* dbg_topk_val = nullptr;
-  int32_t *dbg_topk_idx = nullptr, *dbg_token = nullptr;
   // persistent wgmma decode kernel (lm_decode_tc.cu): plan, tensor maps and buffers live in the workspace
   bool tc_ok = false, tc_flat_ok = false;
   TcPlanInfo tc_info[2] = {};         // [0]: whole-K gate/up plan (any batch), [1]: flat plan (batch <= 4)
@@ -120,18 +129,13 @@ struct nt_lm {
   int* slot_key = nullptr;            // [max_batch] Philox stream key per slot, -1: slot + slot_base
   int* slot_args = nullptr;           // [3][max_batch] slots, stream keys, prompt lengths of the last call
   int* slot_table = nullptr;          // [max_batch][max_pages] the listed slots' page-table rows, in call order
-  // per-slot sampling controls (nt_lm_set_slot_sampling): copied into every SamplerParams while on
+  // per-slot sampling controls (nt_lm_set_slot_sampling): copied into every SamplerParams while step.slot_sp_on
   nt_slot_sampling* slot_sp = nullptr;  // [max_batch]
-  bool slot_sp_on = false;
-  // vocabulary range (nt_lm_set_vocab_range): allowed ids [vr_lo, vr_hi) + EOS while vr_on
-  bool vr_on = false;
-  int vr_lo = 0, vr_hi = 0;
   // repetition penalty (nt_lm_set_repetition_penalty): history bitmaps, the per-slot table and "recorded" flags
   uint32_t* rep_hist = nullptr;       // [max_batch][rep_words]
   nt_slot_penalty* rep_tab = nullptr; // [max_batch]
   int* rep_rec = nullptr;             // [max_batch] 1: the slot's history was built by a prefill while the table was on
   int rep_words = 0;                  // ceil(vocab_size / 32)
-  bool rep_on = false;
 };
 
 // The lm_head tiles a launch computes under the vocabulary range: [t_lo, t_hi), plus eos_tile when EOS lies outside
@@ -142,19 +146,20 @@ struct VocabTiles {
   int count() const { return t_hi - t_lo + (eos_tile >= 0 ? 1 : 0); }
 };
 static VocabTiles vocab_tiles(const nt_lm* lm, int eos) {
+  const StepSettings& ss = lm->step;
   VocabTiles v;
-  v.on = lm->vr_on;
-  v.t_lo = lm->vr_on ? lm->vr_lo / 128 : 0;
-  v.t_hi = ((lm->vr_on ? lm->vr_hi : lm->cfg.vocab_size) + 127) / 128;
+  v.on = ss.vr_on;
+  v.t_lo = ss.vr_on ? ss.vr_lo / 128 : 0;
+  v.t_hi = ((ss.vr_on ? ss.vr_hi : lm->cfg.vocab_size) + 127) / 128;
   const int et = eos / 128;
-  v.eos_tile = (lm->vr_on && (et < v.t_lo || et >= v.t_hi)) ? et : -1;
+  v.eos_tile = (ss.vr_on && (et < v.t_lo || et >= v.t_hi)) ? et : -1;
   return v;
 }
 
 // Every launch under the range first sets its logits rows [0, B) and their tile maxima to -inf; the lm_head then
 // writes only the tiles it computes, so each suppressed id reads -inf on every sampler path.
 static int vocab_fill(nt_lm* lm, int B, cudaStream_t stream) {
-  if (!lm->vr_on) return NT_OK;
+  if (!lm->step.vr_on) return NT_OK;
   const int V = lm->cfg.vocab_size, nt = (V + 127) / 128;
   int rc = launch_fill_neg_inf(lm->logits, static_cast<long long>(B) * V, stream);
   if (!rc && lm->tc_tmax) rc = launch_fill_neg_inf(lm->tc_tmax, static_cast<long long>(B < lm->tc_rows ? B : lm->tc_rows) * nt, stream);
@@ -393,10 +398,11 @@ static SamplerParams make_sampler(const nt_lm* lm, const nt_lm_state* st, const 
   s.hidden = lm->cfg.hidden;
   s.slot_base = sp->slot_base;
   s.slot_key = lm->slot_key;
-  s.slot_sp = lm->slot_sp_on ? lm->slot_sp : nullptr;
-  s.rep_hist = lm->rep_on ? lm->rep_hist : nullptr;
+  const StepSettings& ss = lm->step;
+  s.slot_sp = ss.slot_sp_on ? lm->slot_sp : nullptr;
+  s.rep_hist = ss.rep_on ? lm->rep_hist : nullptr;
   s.rep_words = lm->rep_words;
-  s.dbg_topk_val = lm->dbg_topk_val, s.dbg_topk_idx = lm->dbg_topk_idx, s.dbg_token = lm->dbg_token;
+  s.dbg_topk_val = ss.dbg_topk_val, s.dbg_topk_idx = ss.dbg_topk_idx, s.dbg_token = ss.dbg_token;
   return s;
 }
 
@@ -421,7 +427,7 @@ static int run_sampler(nt_lm* lm, const SamplerParams& s, int B, cudaStream_t st
 // While the repetition penalty is on (and eos >= 0), one fix-up launch after the lm_head rewrites each history logit
 // of every row (row i holds slot row_slot[i], or slot i) and the raw tile maxima it changed.
 static int rep_fixup(nt_lm* lm, int B, float* logits, float* tmax, int eos, const int32_t* row_slot, cudaStream_t stream) {
-  if (eos < 0 || !lm->rep_on) return NT_OK;
+  if (eos < 0 || !lm->step.rep_on) return NT_OK;
   const int V = lm->cfg.vocab_size;
   return launch_rep_penalty(logits, B, V, lm->rep_hist, lm->rep_words, lm->rep_tab, lm->rep_rec, row_slot, tmax, (V + 127) / 128, stream);
 }
@@ -493,7 +499,7 @@ static int layers_gemm(nt_lm* lm, const nt_lm_state* st, int rows, int B, int mo
   const int H = c.hidden, I = c.inter, QN = lm->qkv_n, HD = c.n_heads * 64;
   const float scale_log2 = (1.0f / 8.0f) * 1.4426950408889634f;
   int rc;
-  const int n_layers = lm->debug_layers >= 0 ? lm->debug_layers : c.n_layers;
+  const int n_layers = lm->step.debug_layers >= 0 ? lm->step.debug_layers : c.n_layers;
   // o_proj / down_proj accumulate into the residual stream; with few row tiles (batched decode, short prompts)
   // they split K over grid.z into lm->splitk_ws and the RMSNorm that follows folds the slices into lm->h.
   // The last layer's down_proj splits only when the caller takes over the fold (`tail`: decode, where the final
@@ -591,7 +597,7 @@ static int prefill_forward(nt_lm* lm, const nt_lm_state* st, const int32_t* ids,
   const nt_lm_config& c = lm->cfg;
   int rc;
   if ((rc = vocab_fill(lm, B, stream))) return rc;
-  if (lm->rep_on &&
+  if (lm->step.rep_on &&
       (rc = launch_rep_history(lm->rep_hist, lm->rep_words, lm->rep_tab, lm->rep_rec, row_slot, ids, lm->cu_dev, B, c.vocab_size, stream)))
     return rc;
   if ((rc = launch_embed_rows(lm->embed, ids, cu[B], c.hidden, lm->h, stream))) return rc;
@@ -675,7 +681,7 @@ static int decode_step(nt_lm* lm, const nt_lm_state* st, int B, const nt_samplin
     const KVLayout kv = make_kv(lm, st);
     const int H = c.hidden, I = c.inter, HD = c.n_heads * 64;
     const float scale_log2 = (1.0f / 8.0f) * 1.4426950408889634f;
-    const int n_layers = lm->debug_layers >= 0 ? lm->debug_layers : c.n_layers;
+    const int n_layers = lm->step.debug_layers >= 0 ? lm->step.debug_layers : c.n_layers;
     for (int l = 0; l < n_layers; ++l) {
       GemvParams g;
       memset(&g, 0, sizeof(g));
@@ -738,7 +744,7 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
   }
   if (n_steps == 0) return NT_OK;
   if ((rc = vocab_fill(lm, B, stream))) return rc;   // once per launch: no step writes a suppressed row or tile maximum
-  const int tc_layers = lm->debug_layers >= 0 ? lm->debug_layers : c.n_layers;
+  const int tc_layers = lm->step.debug_layers >= 0 ? lm->step.debug_layers : c.n_layers;
   if (want_tc && lm->tc_ok && B <= lm->tc_rows && B * c.n_kv_heads <= lm->num_sms) {
     TcParams P;
     memset(&P, 0, sizeof(P));
@@ -776,7 +782,7 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
     P.head_eos_at = vt.eos_tile < 0 ? -1 : (vt.eos_tile < vt.t_lo ? 0 : vt.t_hi - vt.t_lo);
     P.samp = make_sampler(lm, st, sp);
     P.samp.advance = 1;
-    P.rep_tab = lm->rep_on ? lm->rep_tab : nullptr, P.rep_rec = lm->rep_rec;
+    P.rep_tab = lm->step.rep_on ? lm->rep_tab : nullptr, P.rep_rec = lm->rep_rec;
     P.gbar = lm->gbar;
     P.n_steps = n_steps;
     P.logits_out = logits_out;
@@ -798,11 +804,15 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
     }
     return NT_OK;
   }
-  // graph keyed by everything baked into the kernel parameters
-  std::vector<uint8_t> key(sizeof(int) + sizeof(nt_lm_state) + sizeof(nt_sampling));
-  memcpy(key.data(), &B, sizeof(int));
-  memcpy(key.data() + sizeof(int), st, sizeof(nt_lm_state));
-  memcpy(key.data() + sizeof(int) + sizeof(nt_lm_state), sp, sizeof(nt_sampling));
+  // The graph is keyed by every input decode_step bakes into its launches: the batch, the state and sampling params,
+  // and the host settings in lm->step.  The slot_sp / rep_tab contents stay out: the graph reads them at replay.
+  // prof / prof_step stay out: only the persistent kernel reads them, and it never runs from the graph.
+  std::vector<uint8_t> key(sizeof(int) + sizeof(nt_lm_state) + sizeof(nt_sampling) + sizeof(StepSettings));
+  uint8_t* k = key.data();
+  memcpy(k, &B, sizeof(int)), k += sizeof(int);
+  memcpy(k, st, sizeof(nt_lm_state)), k += sizeof(nt_lm_state);
+  memcpy(k, sp, sizeof(nt_sampling)), k += sizeof(nt_sampling);
+  memcpy(k, &lm->step, sizeof(StepSettings));
   if (!lm->graph || key != lm->graph_key) {
     if (lm->graph) {
       cudaGraphExecDestroy(lm->graph);
@@ -851,13 +861,7 @@ extern "C" int nt_lm_set_slot_sampling(nt_lm* lm, const nt_slot_sampling* table,
     NT_CUDA_CHECK(cudaMemcpyAsync(lm->slot_sp, table, size_t(lm->cfg.max_batch) * sizeof(nt_slot_sampling), cudaMemcpyHostToDevice,
                                   reinterpret_cast<cudaStream_t>(stream_)));
   }
-  // the cached decode graph baked the table pointer (or its absence) into its sampler node; new values in a table
-  // that stays on are read at the next replay
-  if (on != lm->slot_sp_on && lm->graph) {
-    cudaGraphExecDestroy(lm->graph);
-    lm->graph = nullptr;
-  }
-  lm->slot_sp_on = on;
+  lm->step.slot_sp_on = on;
   return NT_OK;
 }
 
@@ -870,14 +874,9 @@ extern "C" int nt_lm_set_vocab_range(nt_lm* lm, int32_t lo, int32_t hi, void* st
   if (lo % 128 || (hi % 128 && hi != V))
     return set_error(NT_ERR_INVALID, "vocab range [%d, %d): lo must be a multiple of 128, hi too unless it is %d", lo, hi, V);
   const bool on = !(lo == 0 && hi == V);
-  // the cached decode graph baked the lm_head launches of the previous range
-  if ((on != lm->vr_on || lo != lm->vr_lo || hi != lm->vr_hi) && lm->graph) {
-    cudaGraphExecDestroy(lm->graph);
-    lm->graph = nullptr;
-  }
-  lm->vr_on = on;
-  lm->vr_lo = on ? lo : 0;
-  lm->vr_hi = on ? hi : 0;
+  lm->step.vr_on = on;
+  lm->step.vr_lo = on ? lo : 0;
+  lm->step.vr_hi = on ? hi : 0;
   return NT_OK;
 }
 
@@ -894,17 +893,11 @@ extern "C" int nt_lm_set_repetition_penalty(nt_lm* lm, const nt_slot_penalty* ta
         return set_error(NT_ERR_INVALID, "slot %d: include_prompt=%d must be 0 or 1", s, e.include_prompt);
     }
     // switching on: no slot holds a history yet (tokens drawn while the table was off were never recorded)
-    if (!lm->rep_on) NT_CUDA_CHECK(cudaMemsetAsync(lm->rep_rec, 0, size_t(lm->cfg.max_batch) * sizeof(int), stream));
+    if (!lm->step.rep_on) NT_CUDA_CHECK(cudaMemsetAsync(lm->rep_rec, 0, size_t(lm->cfg.max_batch) * sizeof(int), stream));
     // pageable source: the runtime has staged it by the time the call returns
     NT_CUDA_CHECK(cudaMemcpyAsync(lm->rep_tab, table, size_t(lm->cfg.max_batch) * sizeof(nt_slot_penalty), cudaMemcpyHostToDevice, stream));
   }
-  // the cached decode graph holds the fix-up launch (or its absence) and the sampler's history pointer; new values in a
-  // table that stays on are read at the next replay
-  if (on != lm->rep_on && lm->graph) {
-    cudaGraphExecDestroy(lm->graph);
-    lm->graph = nullptr;
-  }
-  lm->rep_on = on;
+  lm->step.rep_on = on;
   return NT_OK;
 }
 
@@ -912,11 +905,7 @@ extern "C" int nt_lm_set_repetition_penalty(nt_lm* lm, const nt_slot_penalty* ta
 // internal activation buffers (device pointers into the caller's workspace).
 extern "C" int nt_lm_debug_set_layers(nt_lm* lm, int n_layers) {
   if (!lm || n_layers > lm->cfg.n_layers) return set_error(NT_ERR_INVALID, "nt_lm_debug_set_layers: bad argument");
-  lm->debug_layers = n_layers;
-  if (lm->graph) {
-    cudaGraphExecDestroy(lm->graph);
-    lm->graph = nullptr;
-  }
+  lm->step.debug_layers = n_layers;
   return NT_OK;
 }
 extern "C" int nt_lm_debug_set_profile(nt_lm* lm, long long* buf, int step) {
@@ -929,12 +918,7 @@ extern "C" int nt_lm_debug_capture_sampler(nt_lm* lm, float* topk_val, int32_t* 
   if (!lm) return set_error(NT_ERR_INVALID, "nt_lm_debug_capture_sampler: null handle");
   if (!topk_val != !topk_idx || !topk_val != !token)
     return set_error(NT_ERR_INVALID, "nt_lm_debug_capture_sampler: pass all three buffers or none");
-  lm->dbg_topk_val = topk_val, lm->dbg_topk_idx = topk_idx, lm->dbg_token = token;
-  // the cached decode graph baked the previous pointers into its sampler node (the graph key does not see them)
-  if (lm->graph) {
-    cudaGraphExecDestroy(lm->graph);
-    lm->graph = nullptr;
-  }
+  lm->step.dbg_topk_val = topk_val, lm->step.dbg_topk_idx = topk_idx, lm->step.dbg_token = token;
   return NT_OK;
 }
 extern "C" int nt_debug_decode_plan(int hidden, int inter, int n_heads, int n_kv, int vocab, int n_sms, int flat,

@@ -111,8 +111,22 @@ class PagePool:
 DEFAULT_CONTROLS = (1.0, 50, 1.0, 0.0)   # temperature, top_k, top_p, min_p: the reference's (neutts/neutts.py:338-347)
 
 
-def _is_seq(v) -> bool:
-    return isinstance(v, (list, tuple, np.ndarray, torch.Tensor))
+def per_item(n: int, noun: str, **values) -> dict:
+    """Each keyword a scalar (kept as it is) or a sequence with one value per ``noun`` (made a list of Python
+    scalars); raises ValueError for a sequence of another length."""
+    out = {}
+    for name, v in values.items():
+        if isinstance(v, (list, tuple, np.ndarray, torch.Tensor)):
+            v = [x.item() if hasattr(x, "item") else x for x in v]
+            if len(v) != n:
+                raise ValueError(f"{name} needs one value per {noun} ({n}), got {len(v)}")
+        out[name] = v
+    return out
+
+
+def _rows(n: int, cols: dict):
+    """The n rows of ``per_item``'s columns (a scalar repeats in every row)."""
+    return zip(*(v if isinstance(v, list) else [v] * n for v in cols.values()))
 
 
 def check_controls(temperature, top_k, top_p, min_p) -> tuple:
@@ -133,19 +147,10 @@ def per_prompt_controls(n: int, temperature, top_k, top_p, min_p):
     """Sampling controls of n prompts.  Each control is a scalar or a sequence with one value per prompt.  Returns None
     when every control is a scalar and top-p / min-p are off (``sampling``'s scalars then govern, exactly as without
     per-slot controls), else one validated (temperature, top_k, top_p, min_p) per prompt."""
-    cols = []
-    for name, v in (("temperature", temperature), ("top_k", top_k), ("top_p", top_p), ("min_p", min_p)):
-        if _is_seq(v):
-            v = [x.item() if hasattr(x, "item") else x for x in v]
-            if len(v) != n:
-                raise ValueError(f"{name} needs one value per prompt ({n}), got {len(v)}")
-            cols.append(v)
-        else:
-            cols.append(None)
-    if all(c is None for c in cols) and top_p == 1 and min_p == 0:
+    cols = per_item(n, "prompt", temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p)
+    if not any(isinstance(v, list) for v in cols.values()) and top_p == 1 and min_p == 0:
         return None
-    vals = [c if c is not None else [v] * n for c, v in zip(cols, (temperature, top_k, top_p, min_p))]
-    return [check_controls(*row) for row in zip(*vals)]
+    return [check_controls(*row) for row in _rows(n, cols)]
 
 
 def check_vocab_range(vocab_range, vocab_size: int):
@@ -188,17 +193,55 @@ def check_penalty(penalty, include_prompt=True) -> tuple:
 def per_prompt_penalty(n: int, penalty, include_prompt):
     """Repetition penalties of n prompts, each argument a scalar or one value per prompt.  Returns None when every
     penalty is 1 (nothing to penalise: no engine call), else one validated (penalty, include_prompt) per prompt."""
-    cols = []
-    for name, v in (("repetition_penalty", penalty), ("penalize_prompt", include_prompt)):
-        if _is_seq(v):
-            v = [x.item() if hasattr(x, "item") else x for x in v]
-            if len(v) != n:
-                raise ValueError(f"{name} needs one value per prompt ({n}), got {len(v)}")
-            cols.append(v)
-        else:
-            cols.append([v] * n)
-    rows = [check_penalty(p, i) for p, i in zip(*cols)]
+    cols = per_item(n, "prompt", repetition_penalty=penalty, penalize_prompt=include_prompt)
+    rows = [check_penalty(p, i) for p, i in _rows(n, cols)]
     return None if all(r[0] == 1.0 for r in rows) else rows
+
+
+@dataclass
+class Settings:
+    """The per-prompt generation settings of one call, resolved and validated before any engine call
+    (``resolve_settings``)."""
+
+    controls: list | None      # one (temperature, top_k, top_p, min_p) per prompt; None: the launch scalars govern
+    penalty: list | None       # one (penalty, include_prompt) per prompt; None: no penalty
+    vocab_range: tuple | None  # (lo, hi); None: the whole vocabulary
+    temperature: float         # the launch scalars, taken from the first row while the controls table is on (the
+    top_k: int                 # sampler then reads every slot's own row)
+
+    def apply(self, lm, n: int) -> None:
+        """Before a prefill of prompts 0..n-1 into slots 0..n-1, on its stream: controls, then range, then penalty.
+        Each setting is applied, or switched off when an earlier call left it on, or makes no call when it is off and
+        stays off.  ``lm`` needs the ``set_*`` methods only when a call is due; a missing mirror counts as off."""
+        if self.controls is not None or getattr(lm, "_slot_sp_host", None) is not None:
+            lm.set_slot_sampling(None if self.controls is None else self.controls[:n])
+        if self.vocab_range is not None:
+            lm.set_vocab_range(*self.vocab_range)
+        elif getattr(lm, "_vocab_range", None) is not None:
+            lm.set_vocab_range(None)
+        if self.penalty is not None or getattr(lm, "_penalty_host", None) is not None:
+            lm.set_repetition_penalty(None if self.penalty is None else self.penalty[:n])
+
+    def admit(self, lm, slots, idx) -> None:
+        """Before a refill of prompts ``idx`` into ``slots``: writes their rows; every other slot keeps its own, and
+        the range holds."""
+        if self.controls is not None:
+            lm.set_slot_sampling([self.controls[i] for i in idx], slots=slots)
+        if self.penalty is not None:
+            lm.set_repetition_penalty([self.penalty[i] for i in idx], slots=slots)
+
+
+def resolve_settings(lm, n: int, temperature=1.0, top_k=50, top_p=1.0, min_p=0.0, vocab_range=None,
+                     repetition_penalty=1.0, penalize_prompt=True) -> Settings:
+    """The settings of n prompts on engine ``lm``, each control a scalar or one value per prompt
+    (``per_prompt_controls``, ``per_prompt_penalty``, ``check_vocab_range``; ``lm.shape`` is read only for a range)."""
+    if vocab_range is not None:
+        vocab_range = check_vocab_range(vocab_range, lm.shape.vocab_size)
+    penalty = per_prompt_penalty(n, repetition_penalty, penalize_prompt)
+    controls = per_prompt_controls(n, temperature, top_k, top_p, min_p)
+    if controls:
+        temperature, top_k = controls[0][0], controls[0][1]
+    return Settings(controls, penalty, vocab_range, temperature, top_k)
 
 
 PLAN_PHASES = ("qkv", "o", "gu", "d")   # phase order of the persistent kernel's work plan
@@ -317,27 +360,26 @@ class SpeechLM:
         slots 0..len(rows) - 1); every other slot keeps its entry, or the reference defaults (1.0, 50, 1.0, 0.0) when
         the table was off.  ``None`` switches the table off, and ``sampling``'s temperature and top_k govern every
         slot again.  The table is copied on the current stream, so it is ordered before the next prefill or decode."""
-        if rows is None:
-            _lib.check(self.L.nt_lm_set_slot_sampling(self.handle, None, _lib.current_stream_ptr()))
-            self._slot_sp_host = None
-            return
-        rows = [check_controls(*r) for r in rows]
-        slots = list(range(len(rows))) if slots is None else [int(s) for s in slots]
-        if len(slots) != len(rows) or len(set(slots)) != len(slots) or any(not 0 <= s < self.max_batch for s in slots):
-            raise ValueError(f"slots must be distinct, in 0..{self.max_batch - 1} and one per row")
-        table = list(self._slot_sp_host or [DEFAULT_CONTROLS] * self.max_batch)
-        for s, r in zip(slots, rows):
-            table[s] = r
-        arr = (_lib.SlotSampling * self.max_batch)(*(_lib.SlotSampling(*r) for r in table))
-        with torch.cuda.device(self.device):
-            _lib.check(self.L.nt_lm_set_slot_sampling(self.handle, arr, _lib.current_stream_ptr()))
-        self._slot_sp_host = table
+        self._write_slot_table("_slot_sp_host", self.L.nt_lm_set_slot_sampling, _lib.SlotSampling, check_controls,
+                               DEFAULT_CONTROLS, rows, slots)
 
-    def _use_controls(self, rows) -> None:
-        """Slots 0..len(rows) - 1 take ``rows``; None leaves the table off (switching it off only if an earlier call
-        left it on)."""
-        if rows is not None or getattr(self, "_slot_sp_host", None) is not None:
-            self.set_slot_sampling(rows)
+    def _write_slot_table(self, mirror: str, setter, entry, check, default, rows, slots) -> None:
+        """Behind ``set_slot_sampling`` / ``set_repetition_penalty``: validates ``rows`` (``check``) and ``slots``,
+        merges them into the host mirror (attribute ``mirror``; ``default`` fills a table that was off), and hands the
+        whole table of ``entry`` structs to the C ``setter`` on the current stream.  ``rows=None``: the table goes off."""
+        table = arr = None
+        if rows is not None:
+            rows = [check(*r) for r in rows]
+            slots = list(range(len(rows))) if slots is None else [int(s) for s in slots]
+            if len(slots) != len(rows) or len(set(slots)) != len(slots) or any(not 0 <= s < self.max_batch for s in slots):
+                raise ValueError(f"slots must be distinct, in 0..{self.max_batch - 1} and one per row")
+            table = list(getattr(self, mirror) or [default] * self.max_batch)
+            for s, r in zip(slots, rows):
+                table[s] = r
+            arr = (entry * self.max_batch)(*(entry(*r) for r in table))
+        with torch.cuda.device(self.device):
+            _lib.check(setter(self.handle, arr, _lib.current_stream_ptr()))
+        setattr(self, mirror, table)
 
     def set_vocab_range(self, lo, hi=None) -> None:
         """Restrict every later sampler launch to ids in [lo, hi) plus the launch's EOS id (transformers'
@@ -355,14 +397,6 @@ class SpeechLM:
             _lib.check(self.L.nt_lm_set_vocab_range(self.handle, lo_, hi_, _lib.current_stream_ptr()))
         self._vocab_range = rng
 
-    def _use_vocab_range(self, vocab_range) -> None:
-        """The engine takes ``vocab_range``; None leaves the range off (switching it off only if an earlier call left
-        it on), so a default call makes no engine call."""
-        if vocab_range is not None:
-            self.set_vocab_range(*vocab_range)
-        elif getattr(self, "_vocab_range", None) is not None:
-            self.set_vocab_range(None)
-
     def set_repetition_penalty(self, rows, slots=None) -> None:
         """Per-slot repetition penalty (transformers' ``RepetitionPenaltyLogitsProcessor``).  ``rows``: one
         (penalty, include_prompt) per slot of ``slots`` (default: slots 0..len(rows) - 1); every other slot keeps its
@@ -370,42 +404,36 @@ class SpeechLM:
         token generated for it since; it is recorded from the slot's next prefill, so switch the table on before the
         prefill whose tokens should count.  ``None`` switches the table off.  The table is copied on the current stream,
         so it is ordered before the next prefill or decode."""
-        if rows is None:
-            _lib.check(self.L.nt_lm_set_repetition_penalty(self.handle, None, _lib.current_stream_ptr()))
-            self._penalty_host = None
-            return
-        rows = [check_penalty(*r) for r in rows]
-        slots = list(range(len(rows))) if slots is None else [int(s) for s in slots]
-        if len(slots) != len(rows) or len(set(slots)) != len(slots) or any(not 0 <= s < self.max_batch for s in slots):
-            raise ValueError(f"slots must be distinct, in 0..{self.max_batch - 1} and one per row")
-        table = list(self._penalty_host or [DEFAULT_PENALTY] * self.max_batch)
-        for s, r in zip(slots, rows):
-            table[s] = r
-        arr = (_lib.SlotPenalty * self.max_batch)(*(_lib.SlotPenalty(p, int(i)) for p, i in table))
-        with torch.cuda.device(self.device):
-            _lib.check(self.L.nt_lm_set_repetition_penalty(self.handle, arr, _lib.current_stream_ptr()))
-        self._penalty_host = table
+        self._write_slot_table("_penalty_host", self.L.nt_lm_set_repetition_penalty, _lib.SlotPenalty, check_penalty,
+                               DEFAULT_PENALTY, rows, slots)
 
-    def _use_penalty(self, rows) -> None:
-        """Slots 0..len(rows) - 1 take ``rows``; None leaves the table off (switching it off only if an earlier call
-        left it on), so a default call makes no engine call."""
-        if rows is not None or getattr(self, "_penalty_host", None) is not None:
-            self.set_repetition_penalty(rows)
+    def _stage_ids(self, prompts) -> torch.Tensor:
+        """The prompts' ids, range-checked, back to back in a persistent pinned buffer (so their H2D copy is
+        asynchronous)."""
+        flat = np.concatenate([np.asarray(p, dtype=np.int64) for p in prompts])
+        if flat.min() < 0 or flat.max() >= self.shape.vocab_size:
+            raise ValueError("token id out of range")
+        if getattr(self, "_ids_pinned", None) is None or self._ids_pinned.numel() < flat.size:
+            self._ids_pinned = torch.empty(max(flat.size, self.max_prefill_tokens), dtype=torch.int32).pin_memory()
+        staged = self._ids_pinned[: flat.size]
+        staged.copy_(torch.from_numpy(flat.astype(np.int32)))
+        return staged
+
+    def _alloc_pages(self, table, slots, lens, caps) -> None:
+        """KV pages for prompt + cap tokens of every listed slot, written into its row of the page table ``table``."""
+        for s, n, cap in zip(slots, lens, caps):
+            need = (min(n + cap, self.max_ctx) + self.PAGE - 1) // self.PAGE
+            pages = self.pool.alloc(need)
+            self._slot_pages[s] = pages
+            table[s] = 0
+            table[s, :need] = pages
 
     def prefill(self, prompts, sp, return_logits: bool = False):
         """prompts: list of 1-D int sequences.  Fills the KV cache and samples the first token."""
         lens = [len(p) for p in prompts]
         if not lens or min(lens) < 1:
             raise ValueError("empty prompt")
-        flat = np.concatenate([np.asarray(p, dtype=np.int64) for p in prompts])
-        if flat.min() < 0 or flat.max() >= self.shape.vocab_size:
-            raise ValueError("token id out of range")
-        # stage through a persistent pinned buffer: the H2D copy of the prompt ids is asynchronous and DMA-able
-        if getattr(self, "_ids_pinned", None) is None or self._ids_pinned.numel() < flat.size:
-            self._ids_pinned = torch.empty(max(flat.size, self.max_prefill_tokens), dtype=torch.int32).pin_memory()
-        staged = self._ids_pinned[: flat.size]
-        staged.copy_(torch.from_numpy(flat.astype(np.int32)))
-        return self.prefill_packed(staged, lens, sp, return_logits)
+        return self.prefill_packed(self._stage_ids(prompts), lens, sp, return_logits)
 
     def prefill_packed(self, ids_host: torch.Tensor, lens, sp, return_logits: bool = False):
         """ids_host: int32 host tensor (pinned memory makes the H2D copy asynchronous) holding the
@@ -415,15 +443,12 @@ class SpeechLM:
             raise ValueError(f"batch {B} not in 1..{self.max_batch}")
         if ids_host.dtype != torch.int32 or ids_host.numel() != sum(lens):
             raise ValueError("ids_host must be int32 with sum(lens) elements")
-        self.release_pages()
-        table = np.zeros((self.max_batch, self.max_pages), dtype=np.int32)
         for b, n in enumerate(lens):
             if not 1 <= n < self.max_ctx:
                 raise ValueError(f"prompt {b} has length {n}; must be in 1..{self.max_ctx - 1}")
-            need = (min(n + sp.max_new_tokens, self.max_ctx) + self.PAGE - 1) // self.PAGE
-            pages = self.pool.alloc(need)
-            self._slot_pages[b] = pages
-            table[b, :need] = pages
+        self.release_pages()
+        table = np.zeros((self.max_batch, self.max_pages), dtype=np.int32)
+        self._alloc_pages(table, range(B), lens, [sp.max_new_tokens] * B)
         cu = np.zeros(B + 1, dtype=np.int32)
         cu[1:] = np.cumsum(lens)
         with torch.cuda.device(self.device):
@@ -471,21 +496,10 @@ class SpeechLM:
         caps = [min(int(c), sp.max_new_tokens) for c in limits] if limits is not None else [sp.max_new_tokens] * B
         if limits is not None and (getattr(self, "limits", None) is None or sp.limits != self.limits.data_ptr()):
             raise ValueError("per-prompt limits need sampling params built with limits=")
-        flat = np.concatenate([np.asarray(p, dtype=np.int64) for p in prompts])
-        if flat.min() < 0 or flat.max() >= self.shape.vocab_size:
-            raise ValueError("token id out of range")
+        staged = self._stage_ids(prompts)
         self.release_pages(slots)
         table = self._table_host.copy()
-        for s, n, cap in zip(slots, lens, caps):
-            need = (min(n + cap, self.max_ctx) + self.PAGE - 1) // self.PAGE
-            pages = self.pool.alloc(need)
-            self._slot_pages[s] = pages
-            table[s] = 0
-            table[s, :need] = pages
-        if getattr(self, "_ids_pinned", None) is None or self._ids_pinned.numel() < flat.size:
-            self._ids_pinned = torch.empty(max(flat.size, self.max_prefill_tokens), dtype=torch.int32).pin_memory()
-        staged = self._ids_pinned[: flat.size]
-        staged.copy_(torch.from_numpy(flat.astype(np.int32)))
+        self._alloc_pages(table, slots, lens, caps)
         cu = np.zeros(B + 1, dtype=np.int32)
         cu[1:] = np.cumsum(lens)
         slots_h = np.asarray(slots, dtype=np.int32)
@@ -559,6 +573,20 @@ class SpeechLM:
             raise ValueError("max_new_tokens needs one entry per prompt")
         return [min(max_length - n, int(m), self.max_new) for n, m in zip(lens, max_new_tokens)]
 
+    def _prepare(self, prompts, max_length, max_new_tokens, **settings) -> tuple:
+        """Shared preamble of ``generate_batch`` / ``generate_queue``, run before any engine call: the max_length
+        checks, the generated-token cap per prompt and the resolved ``settings`` -> (caps, Settings)."""
+        max_length = max_length or self.max_ctx
+        if max_length > self.max_ctx:
+            raise ValueError(f"max_length {max_length} exceeds the engine context {self.max_ctx}")
+        lens = [len(p) for p in prompts]
+        if any(max_length - n < 1 for n in lens):
+            raise ValueError("prompt already at max_length")
+        # max_length counts prompt + generated PER SEQUENCE (stopping_criteria.py:73-84): a long prompt in the batch
+        # must not shorten its neighbours, so every slot gets its own cap and the loop runs to the largest one
+        caps = self._caps(lens, max_length, max_new_tokens)
+        return caps, resolve_settings(self, len(prompts), **settings)
+
     def generate_batch(self, prompts, eos_token_id: int, max_length: int | None = None, min_new_tokens: int = 50,
                        temperature: float = 1.0, top_k: int = 50, max_new_tokens: int | None = None, seed: int = 0,
                        greedy: bool = False, forced: torch.Tensor | None = None, check_every: int = 64, slot_base: int = 0,
@@ -572,30 +600,16 @@ class SpeechLM:
         [lo, hi) plus EOS (``set_vocab_range``); None leaves the range off.  ``repetition_penalty`` (> 0, 1 = off) and
         ``penalize_prompt`` (the prompt's ids count) are each a scalar or one value per prompt
         (``set_repetition_penalty``); they apply to greedy and teacher-forced runs too."""
-        if vocab_range is not None:   # validated before any engine call
-            vocab_range = check_vocab_range(vocab_range, self.shape.vocab_size)
-        pen_rows = per_prompt_penalty(len(prompts), repetition_penalty, penalize_prompt)
-        max_length = max_length or self.max_ctx
-        if max_length > self.max_ctx:
-            raise ValueError(f"max_length {max_length} exceeds the engine context {self.max_ctx}")
-        lens = [len(p) for p in prompts]
-        if min(max_length - n for n in lens) < 1:
-            raise ValueError("prompt already at max_length")
-        # max_length counts prompt + generated PER SEQUENCE (stopping_criteria.py:73-84): a long prompt in the batch
-        # must not shorten its neighbours, so every slot gets its own cap and the loop runs to the largest one
-        caps = self._caps(lens, max_length, max_new_tokens)
+        caps, settings = self._prepare(prompts, max_length, max_new_tokens, temperature=temperature, top_k=top_k,
+                                       top_p=top_p, min_p=min_p, vocab_range=vocab_range,
+                                       repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt)
         limit = max(caps)
-        rows = per_prompt_controls(len(prompts), temperature, top_k, top_p, min_p)
-        if rows is not None:   # the launch scalars are validated but not used while the table is on
-            temperature, top_k = rows[0][0], rows[0][1]
-        sp = self.sampling(eos_token_id, min_new_tokens, limit, top_k, temperature, seed, greedy, forced,
-                           limits=caps if min(caps) < limit else None, slot_base=slot_base)
-        self._use_controls(rows)
-        self._use_vocab_range(vocab_range)
-        self._use_penalty(pen_rows)
+        sp = self.sampling(eos_token_id, min_new_tokens, limit, settings.top_k, settings.temperature, seed, greedy,
+                           forced, limits=caps if min(caps) < limit else None, slot_base=slot_base)
+        B = len(prompts)
+        settings.apply(self, B)
         self.prefill(prompts, sp)
         remaining = limit - 1
-        B = len(prompts)
         while remaining > 0:
             n = min(check_every, remaining)
             self.decode(n, sp)
@@ -624,30 +638,18 @@ class SpeechLM:
         controls are written into its slot before its prefill, and the other slots keep theirs.  ``vocab_range`` as in
         ``generate_batch``: set once before the first prefill, it holds across every refill.  ``repetition_penalty`` and
         ``penalize_prompt`` as in ``generate_batch``; a newcomer's entry is written before its prefill."""
-        if vocab_range is not None:   # validated before any engine call
-            vocab_range = check_vocab_range(vocab_range, self.shape.vocab_size)
-        pen_rows = per_prompt_penalty(len(prompts), repetition_penalty, penalize_prompt)
-        max_length = max_length or self.max_ctx
-        if max_length > self.max_ctx:
-            raise ValueError(f"max_length {max_length} exceeds the engine context {self.max_ctx}")
+        caps, settings = self._prepare(prompts, max_length, max_new_tokens, temperature=temperature, top_k=top_k,
+                                       top_p=top_p, min_p=min_p, vocab_range=vocab_range,
+                                       repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt)
         n = len(prompts)
         if n == 0:
             return []
         if check_every < 1:
             raise ValueError("check_every must be >= 1")
-        lens = [len(p) for p in prompts]
-        if min(max_length - m for m in lens) < 1:
-            raise ValueError("prompt already at max_length")
-        caps = self._caps(lens, max_length, max_new_tokens)
         S = min(n, self.max_batch)
-        ctl_rows = per_prompt_controls(n, temperature, top_k, top_p, min_p)
-        if ctl_rows is not None:
-            temperature, top_k = ctl_rows[0][0], ctl_rows[0][1]
-        sp = self.sampling(eos_token_id, min_new_tokens, max(caps), top_k, temperature, seed, greedy,
+        sp = self.sampling(eos_token_id, min_new_tokens, max(caps), settings.top_k, settings.temperature, seed, greedy,
                            limits=caps[:S], slot_base=slot_base)
-        self._use_controls(ctl_rows[:S] if ctl_rows is not None else None)
-        self._use_vocab_range(vocab_range)
-        self._use_penalty(pen_rows[:S] if pen_rows is not None else None)
+        settings.apply(self, S)
         self.prefill([prompts[i] for i in range(S)], sp)
         occ = list(range(S))   # prompt held by each slot, None once harvested
         ngen = [1] * S         # generated tokens per slot, as of the last read
@@ -670,10 +672,7 @@ class SpeechLM:
                     if take:
                         idx = list(range(nxt, nxt + len(take)))
                         nxt += len(take)
-                        if ctl_rows is not None:   # the newcomers' controls, before their prefill on the same stream
-                            self.set_slot_sampling([ctl_rows[i] for i in idx], slots=take)
-                        if pen_rows is not None:
-                            self.set_repetition_penalty([pen_rows[i] for i in idx], slots=take)
+                        settings.admit(self, take, idx)   # before their prefill, on the same stream
                         self.prefill_slots(take, [prompts[i] for i in idx], sp, [slot_base + i for i in idx],
                                            limits=[caps[i] for i in idx])
                         for s, i in zip(take, idx):
