@@ -222,6 +222,19 @@ typedef struct {
  * nt_op_topk_sample and nt_lm_head_gemv ignore the penalty. */
 int nt_lm_set_repetition_penalty(nt_lm* lm, const nt_slot_penalty* host_table, void* stream);
 
+/* Per-token log-probabilities.  out: caller-owned device fp32 [max_batch][max_new][2] (8-byte aligned); entry [s][n]
+ * belongs to out_tokens[s][n] and is written wherever that token is (every sampler launch of nt_lm_prefill,
+ * nt_lm_prefill_slots and nt_lm_decode); nothing else is written.  NULL switches it off (the default).
+ *   [0] sampled: log-probability of the token in the distribution the sampler drew from, the kept window after
+ *       penalty -> EOS mask -> vocabulary range -> 1 / T -> top_k -> top_p -> min_p, renormalised (transformers'
+ *       compute_transition_scores(normalize_logits=True) on output_scores).  Greedy runs: equal to [1], since
+ *       transformers applies no warpers there.  Teacher-forced runs: -inf when the forced id lies outside the window.
+ *   [1] model: log-softmax of the token over the whole vocabulary, on the scores after the repetition penalty, the
+ *       min-new-tokens EOS mask (EOS left out of the sum while masked) and the vocabulary range (suppressed ids add
+ *       nothing), before temperature and the warpers.
+ * Host state only, like nt_lm_set_vocab_range.  nt_op_topk_sample and nt_lm_head_gemv ignore it. */
+int nt_lm_set_logprobs(nt_lm* lm, float* out, void* stream);
+
 /* Timed single-kernel entry for the roofline measurement: the lm_head GEMV (+ final RMSNorm)
  * exactly as the decode step launches it.  h: f32 [B][hidden] -> logits f32 [B][vocab]. */
 int nt_lm_head_gemv(nt_lm* lm, const float* h, int B, float* logits, void* stream);

@@ -210,14 +210,25 @@ class NeuTTS:
         return ids[:s] + [self._tok_id("<|SPEECH_GENERATION_START|>")] + [base + c for c in codes]
 
     # ------------------------------------------------------------------ hot path A
+    def _check_logprobs(self, distributed: bool = False) -> None:
+        """``return_logprobs`` needs an engine that writes them (``SpeechLM.set_logprobs``) and a single process."""
+        if distributed:
+            raise ValueError("return_logprobs is not supported with distributed=True")
+        if not hasattr(self.backbone, "set_logprobs"):
+            raise ValueError("return_logprobs needs a backbone with set_logprobs (neutts_air_b200.SpeechLM)")
+
     def _generate_ids(self, prompts: Sequence[Sequence[int]], max_new_tokens: int | None = None,
-                      min_new_tokens: int = 50, slot_base: int = 0, ctl: dict | None = None) -> list:
-        """Batched device-side generation; returns generated token ids per prompt (CPU int64 tensors).
+                      min_new_tokens: int = 50, slot_base: int = 0, ctl: dict | None = None, logprobs: bool = False):
+        """Batched device-side generation; returns generated token ids per prompt (CPU int64 tensors), or with
+        ``logprobs`` (ids, per-prompt float32 CPU tensors [n, 2] of (sampled, model) log-probabilities).
         Sampling parameters default to the reference's (``neutts/neutts.py:338-347``); ``ctl`` (see ``_controls``)
         overrides them, per prompt where a control is a list."""
         eos = self._tok_id("<|SPEECH_GENERATION_END|>")
         seed = self.seed if self.seed is not None else int(torch.randint(0, 2**31 - 1, (1,)).item())
         kw = _backbone_kw(ctl if ctl is not None else CONTROL_DEFAULTS)
+        if logprobs:
+            self._check_logprobs()
+            kw["return_logprobs"] = True
         rng = self._speech_range()
         if rng is not None:
             kw["vocab_range"] = rng
@@ -308,25 +319,32 @@ class NeuTTS:
 
     # ------------------------------------------------------------------ public API
     def infer(self, text: str, ref_codes, ref_text: str, *, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0,
-              min_p: float = 0.0, repetition_penalty: float = 1.0, penalize_prompt: bool = True) -> np.ndarray:
+              min_p: float = 0.0, repetition_penalty: float = 1.0, penalize_prompt: bool = True,
+              return_logprobs: bool = False):
         """Text + reference voice -> 24 kHz float32 waveform (``neutts/neutts.py:216-243``).  The sampling controls
-        default to the reference's values; see ``infer_batch``."""
-        return self.infer_batch([text], [ref_codes], [ref_text], temperature=temperature, top_k=top_k, top_p=top_p,
-                                min_p=min_p, repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt)[0]
+        default to the reference's values; see ``infer_batch``.  ``return_logprobs``: returns (waveform, log-probs)."""
+        out = self.infer_batch([text], [ref_codes], [ref_text], temperature=temperature, top_k=top_k, top_p=top_p,
+                               min_p=min_p, repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt,
+                               return_logprobs=return_logprobs)
+        return (out[0][0], out[1][0]) if return_logprobs else out[0]
 
     def infer_from_prompt_ids(self, prompts: Sequence[Sequence[int]], max_new_tokens: int | None = None,
                               min_new_tokens: int = 50, slot_base: int = 0, *, temperature=1.0, top_k=50, top_p=1.0,
-                              min_p=0.0, repetition_penalty=1.0, penalize_prompt=True) -> list:
+                              min_p=0.0, repetition_penalty=1.0, penalize_prompt=True, return_logprobs: bool = False):
         """Hot path only: prompt ids (host) -> waveforms (host).  Used by bench.py's end-to-end leg.
         ``slot_base`` offsets the sampler's Philox slot index so chunks / ranks under one seed draw independently.
         More prompts than ``max_batch`` go through the backbone's ``generate_queue`` when it has one.  Sampling
-        controls as in ``infer_batch``."""
+        controls and ``return_logprobs`` as in ``infer_batch``."""
         ctl = _controls(len(prompts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)
-        gen = self._generate_ids(prompts, max_new_tokens, min_new_tokens, slot_base, ctl)
-        return [self._watermark(w) for w in self._decode_codes([self._ids_to_codes(g) for g in gen])]
+        gen = self._generate_ids(prompts, max_new_tokens, min_new_tokens, slot_base, ctl, logprobs=return_logprobs)
+        if return_logprobs:
+            gen, lps = gen
+        wavs = [self._watermark(w) for w in self._decode_codes([self._ids_to_codes(g) for g in gen])]
+        return (wavs, [lp.numpy() for lp in lps]) if return_logprobs else wavs
 
     def infer_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], distributed: bool = False, *,
-                    temperature=1.0, top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0, penalize_prompt=True) -> list:
+                    temperature=1.0, top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0, penalize_prompt=True,
+                    return_logprobs: bool = False):
         """List in / list out.  With ``distributed=True`` (inside an initialised torch.distributed job) the
         utterances are sharded over ranks and every rank returns all waveforms (one all-gather).
 
@@ -342,23 +360,36 @@ class NeuTTS:
         and the sharding over ranks.  ``repetition_penalty`` (transformers' RepetitionPenaltyLogitsProcessor: > 0, 1 =
         off) divides the positive logits and multiplies the negative ones of every id already in the utterance, which
         breaks loops of one repeated codec id; ``penalize_prompt=False`` leaves the prompt (the reference codes) out of
-        that history.  Both are scalars or one value per utterance too."""
+        that history.  Both are scalars or one value per utterance too.
+
+        ``return_logprobs=True`` (not with ``distributed``; needs a ``SpeechLM`` backbone) returns (waveforms,
+        log-probs): per utterance a float32 array [n_generated, 2] with the (sampled, model) log-probability of every
+        generated token, EOS included (``SpeechLM.set_logprobs``).  Its rows follow the generated ids, not the codec
+        frames: a non-speech id the codec never sees keeps its row.  ``sampled`` is the token's log-probability in the
+        distribution it was drawn from (after every control above), ``model`` its log-softmax over the whole
+        vocabulary after the repetition penalty and before temperature and the warpers; their mean or minimum over an
+        utterance flags a bad take, or picks the best of several.  Streaming does not return them."""
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
         ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)
+        if return_logprobs:
+            self._check_logprobs(distributed)
         prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(texts, ref_codes, ref_texts)]
         queue = hasattr(self.backbone, "generate_queue")
 
         def run(idx, slot_base):
-            return self.infer_from_prompt_ids([prompts[i] for i in idx], slot_base=slot_base, **_pick(ctl, idx))
+            return self.infer_from_prompt_ids([prompts[i] for i in idx], slot_base=slot_base, return_logprobs=return_logprobs,
+                                              **_pick(ctl, idx))
 
         if not distributed:
             if queue and len(prompts) > self.max_batch:
                 return run(range(len(prompts)), 0)
-            out = []
+            out, lps = [], []
             for j in range(0, len(prompts), self.max_batch):
-                out += run(range(j, min(j + self.max_batch, len(prompts))), j)
-            return out
+                r = run(range(j, min(j + self.max_batch, len(prompts))), j)
+                out += r[0] if return_logprobs else r
+                lps += r[1] if return_logprobs else []
+            return (out, lps) if return_logprobs else out
         from neutts_air_b200 import dist
 
         mine = dist.shard_indices(len(prompts), [len(p) for p in prompts])
@@ -377,7 +408,7 @@ class NeuTTS:
         """Streaming synthesis with the reference's window geometry (``neutts/neutts.py:373-465``):
         every 25 new frames (once 5 look-ahead frames exist) the codec re-decodes
         [n - 50 - 1, n + 25 + 5 + 1) and the chunk is cross-faded with triangular weights.  Sampling controls as in
-        ``infer_batch``."""
+        ``infer_batch``; streaming returns no per-token log-probabilities (``return_logprobs`` is not supported here)."""
         if self._is_quantized_model:  # kept for signature parity; never true on this build
             raise NotImplementedError("GGUF streaming is not part of the H100 build")
         ctl = _controls(1, temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)
@@ -391,7 +422,8 @@ class NeuTTS:
         streams one utterance, ``neutts/neutts.py:373-465``).  Every yield is a list with one entry per utterance:
         the next audio chunk (float32, cross-faded exactly as in ``infer_stream``) or ``None`` when that utterance
         has nothing new.  The sequences decode in lock-step in ONE persistent-kernel launch per round; the windows
-        that are due are gathered on the device from the code history and go through the codec as one batch."""
+        that are due are gathered on the device from the code history and go through the codec as one batch.  Streaming
+        returns no per-token log-probabilities (``infer_batch``'s ``return_logprobs``)."""
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
         ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)

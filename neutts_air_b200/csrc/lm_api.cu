@@ -84,6 +84,7 @@ struct StepSettings {
   bool vr_on = false;
   bool slot_sp_on = false;            // per-slot sampling table (nt_lm_set_slot_sampling)
   bool rep_on = false;                // repetition penalty table (nt_lm_set_repetition_penalty)
+  float* logprob_out = nullptr;       // per-token log-probabilities (nt_lm_set_logprobs): nullptr = off
 };
 
 struct nt_lm {
@@ -402,6 +403,7 @@ static SamplerParams make_sampler(const nt_lm* lm, const nt_lm_state* st, const 
   s.slot_sp = ss.slot_sp_on ? lm->slot_sp : nullptr;
   s.rep_hist = ss.rep_on ? lm->rep_hist : nullptr;
   s.rep_words = lm->rep_words;
+  s.logprob_out = ss.logprob_out;
   s.dbg_topk_val = ss.dbg_topk_val, s.dbg_topk_idx = ss.dbg_topk_idx, s.dbg_token = ss.dbg_token;
   return s;
 }
@@ -898,6 +900,14 @@ extern "C" int nt_lm_set_repetition_penalty(nt_lm* lm, const nt_slot_penalty* ta
     NT_CUDA_CHECK(cudaMemcpyAsync(lm->rep_tab, table, size_t(lm->cfg.max_batch) * sizeof(nt_slot_penalty), cudaMemcpyHostToDevice, stream));
   }
   lm->step.rep_on = on;
+  return NT_OK;
+}
+
+extern "C" int nt_lm_set_logprobs(nt_lm* lm, float* out, void* stream) {
+  (void)stream;   // host state only: read by the launches enqueued after this call
+  if (!lm) return set_error(NT_ERR_INVALID, "nt_lm_set_logprobs: null handle");
+  if (reinterpret_cast<uintptr_t>(out) & 7u) return set_error(NT_ERR_INVALID, "nt_lm_set_logprobs: out must be 8-byte aligned");
+  lm->step.logprob_out = out;
   return NT_OK;
 }
 

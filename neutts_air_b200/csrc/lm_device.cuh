@@ -272,6 +272,61 @@ NT_DEVINL uint32_t processed_key(float logit, int idx, bool mask_eos, int eos_id
   return f2key(logit * inv_t);
 }
 
+// log(sum_v exp(lg[v])) over one logits row of V scores on the 256 consumer threads, id `eos` left out while mask_eos
+// (ids the vocabulary range suppresses hold -inf and add nothing).  Each thread keeps an online (max, sum) in fp32 over
+// its float4 columns; the warps' pairs meet in red (8 float2 of shared memory, free until the caller's next barrier).
+// Every thread returns the result.
+template <typename Sync>
+NT_DEVINL float row_logsumexp(const float* lg, int V, int eos, bool mask_eos, float2* red, Sync sync) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int skip = mask_eos ? eos : -1;
+  float m = -INFINITY, s = 0.f;
+  auto add = [&](float x, float y, float z, float w) {
+    const float c = fmaxf(fmaxf(x, y), fmaxf(z, w));
+    if (c > m) s *= __expf(m - c), m = c;
+    if (m > -INFINITY) s += (__expf(x - m) + __expf(y - m)) + (__expf(z - m) + __expf(w - m));
+  };
+  auto combine = [](float& m0, float& s0, float m1, float s1) {
+    const float mm = fmaxf(m0, m1);
+    s0 = mm == -INFINITY ? 0.f : s0 * __expf(m0 - mm) + s1 * __expf(m1 - mm);
+    m0 = mm;
+  };
+  // ids [0, head) and [head + 4 n4, V) one by one (the row need not start 16-byte aligned), the rest as float4
+  const int head = min(V, static_cast<int>(((16u - (reinterpret_cast<uintptr_t>(lg) & 15u)) & 15u) >> 2));
+  const int n4 = (V - head) >> 2;
+  if (tid < 8) {
+    const int i = tid < 4 ? (tid < head ? tid : V) : head + 4 * n4 + tid - 4;
+    add((i < V && i != skip) ? __ldcg(lg + i) : -INFINITY, -INFINITY, -INFINITY, -INFINITY);
+  }
+  const float4* body = reinterpret_cast<const float4*>(lg + head);
+  constexpr int kU = 8;   // independent 16-byte loads in flight per thread: the pass is bound by L2 latency
+  for (int i = tid; i < n4; i += kU * kConsumerThreads) {
+    float4 x[kU];
+#pragma unroll
+    for (int u = 0; u < kU; ++u) {
+      const int j = i + u * kConsumerThreads;
+      x[u] = j < n4 ? __ldcg(body + j) : make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
+    }
+#pragma unroll
+    for (int u = 0; u < kU; ++u) {
+      const int q = skip - (head + 4 * (i + u * kConsumerThreads));
+      if (q == 0) x[u].x = -INFINITY;
+      if (q == 1) x[u].y = -INFINITY;
+      if (q == 2) x[u].z = -INFINITY;
+      if (q == 3) x[u].w = -INFINITY;
+      add(x[u].x, x[u].y, x[u].z, x[u].w);
+    }
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) combine(m, s, __shfl_xor_sync(0xffffffffu, m, off), __shfl_xor_sync(0xffffffffu, s, off));
+  if (lane == 0) red[warp] = make_float2(m, s);
+  sync();
+  m = -INFINITY, s = 0.f;
+#pragma unroll
+  for (int w = 0; w < kConsumerWarps; ++w) combine(m, s, red[w].x, red[w].y);
+  return m + logf(s);
+}
+
 // Sampler stage 1 for one (sequence b, chunk): processors + exact top-64 of a 2048-logit chunk read
 // from global memory.  keys: [kTopChunk] uint32 shared; scratch: [kSelScratch] uint32 shared.
 template <typename Sync>
@@ -305,6 +360,8 @@ NT_DEVINL void sample_stage1_chunk(const SamplerParams& p, int b, int chunk, uin
 // softmax over them (TopK processor + softmax, utils.py:2789), the slot's top-p and min-p cuts (which keep a prefix
 // k' <= k of the window, renormalised), Philox draw over the prefix, state update, stop flags, and the next
 // token's embedding -> residual stream row (fp32; optionally also as (value, stamp) pairs for the polled hand-off).
+// With p.logprob_out, the written token's (sampled, model) log-probabilities go next to it (DESIGN.md §4, per-token
+// log-probabilities); the model one takes one extra pass over logits row b.
 // Clobbers win[kTopKeep .. 2 kTopKeep) (exponentials).  b: logits row; slot >= 0: the slot whose state row b updates
 // (prefill into chosen slots), else slot b.
 template <typename Sync>
@@ -313,6 +370,11 @@ NT_DEVINL void sample_finish(const SamplerParams& p, int b, int k, Cand* win, in
   const int tid = threadIdx.x;
   const int s = slot >= 0 ? slot : b;
   float* ev = reinterpret_cast<float*>(win + kTopKeep);   // [kTopKeep] exp(score - max)
+  const bool logprobs = p.logprob_out && !stateless && !is_done;   // CTA-uniform
+  const bool mask_eos = ngen < p.sp.min_new_tokens;
+  const float* lg = p.logits + static_cast<long long>(b) * p.V;
+  float lse = 0.f;
+  if (logprobs) lse = row_logsumexp(lg, p.V, p.sp.eos_id, mask_eos, reinterpret_cast<float2*>(ev + kTopKeep), sync);
   if (tid < 32) {
     const float m = win[0].v;
     float e0 = (tid < k) ? __expf(win[tid].v - m) : 0.f;
@@ -376,6 +438,20 @@ NT_DEVINL void sample_finish(const SamplerParams& p, int b, int k, Cand* win, in
       }
       *s_tok = tok;
       if (p.dbg_token) p.dbg_token[b] = tok;
+      if (logprobs) {
+        // model: log-softmax over the processed logits row (penalty, EOS mask, range; no temperature or warpers)
+        const float st = (tok < 0 || tok >= p.V || (mask_eos && tok == p.sp.eos_id)) ? -INFINITY : __ldcg(lg + tok);
+        const float model = st - lse;
+        // sampled: the token's log-probability in the kept window the draw used (greedy: transformers applies no
+        // warpers, so it is the model value); -inf for a forced id outside the window
+        float sampled = model;
+        if (p.sp.forced || !p.sp.greedy) {
+          int j = 0;
+          while (j < k && win[j].i != tok) ++j;
+          sampled = j < k ? (win[j].v - win[0].v) - logf(sum) : -INFINITY;
+        }
+        reinterpret_cast<float2*>(p.logprob_out)[static_cast<long long>(s) * p.max_new + ngen] = make_float2(sampled, model);
+      }
       if (!stateless && !is_done) {
         p.out_tokens[static_cast<long long>(s) * p.max_new + ngen] = tok;
         // the history bit of this token: the persistent kernel's epi_head reads it at the next step, behind the grid

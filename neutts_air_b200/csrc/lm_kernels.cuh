@@ -101,6 +101,9 @@ struct SamplerParams {
   // off.  sample_finish sets the bit of every token it writes to out_tokens.
   uint32_t* rep_hist;
   int rep_words;
+  // per-token log-probabilities (nt_lm_set_logprobs): [max_batch][max_new][2] (sampled, model), nullptr = off.
+  // sample_finish writes the pair of every token it writes to out_tokens.
+  float* logprob_out;
 };
 int launch_sampler(const SamplerParams& p, int B, cudaStream_t stream);
 int launch_sampler_check(const SamplerParams& p);

@@ -208,10 +208,11 @@ class Settings:
     vocab_range: tuple | None  # (lo, hi); None: the whole vocabulary
     temperature: float         # the launch scalars, taken from the first row while the controls table is on (the
     top_k: int                 # sampler then reads every slot's own row)
+    logprobs: bool = False     # per-token log-probabilities on (``SpeechLM.set_logprobs``)
 
     def apply(self, lm, n: int) -> None:
-        """Before a prefill of prompts 0..n-1 into slots 0..n-1, on its stream: controls, then range, then penalty.
-        Each setting is applied, or switched off when an earlier call left it on, or makes no call when it is off and
+        """Before a prefill of prompts 0..n-1 into slots 0..n-1, on its stream: controls, then range, then penalty, then
+        log-probabilities.  Each setting is applied, or switched off when an earlier call left it on, or makes no call when it is off and
         stays off.  ``lm`` needs the ``set_*`` methods only when a call is due; a missing mirror counts as off."""
         if self.controls is not None or getattr(lm, "_slot_sp_host", None) is not None:
             lm.set_slot_sampling(None if self.controls is None else self.controls[:n])
@@ -221,6 +222,8 @@ class Settings:
             lm.set_vocab_range(None)
         if self.penalty is not None or getattr(lm, "_penalty_host", None) is not None:
             lm.set_repetition_penalty(None if self.penalty is None else self.penalty[:n])
+        if self.logprobs != (getattr(lm, "logprobs", None) is not None):
+            lm.set_logprobs(self.logprobs)
 
     def admit(self, lm, slots, idx) -> None:
         """Before a refill of prompts ``idx`` into ``slots``: writes their rows; every other slot keeps its own, and
@@ -232,7 +235,7 @@ class Settings:
 
 
 def resolve_settings(lm, n: int, temperature=1.0, top_k=50, top_p=1.0, min_p=0.0, vocab_range=None,
-                     repetition_penalty=1.0, penalize_prompt=True) -> Settings:
+                     repetition_penalty=1.0, penalize_prompt=True, logprobs=False) -> Settings:
     """The settings of n prompts on engine ``lm``, each control a scalar or one value per prompt
     (``per_prompt_controls``, ``per_prompt_penalty``, ``check_vocab_range``; ``lm.shape`` is read only for a range)."""
     if vocab_range is not None:
@@ -241,7 +244,7 @@ def resolve_settings(lm, n: int, temperature=1.0, top_k=50, top_p=1.0, min_p=0.0
     controls = per_prompt_controls(n, temperature, top_k, top_p, min_p)
     if controls:
         temperature, top_k = controls[0][0], controls[0][1]
-    return Settings(controls, penalty, vocab_range, temperature, top_k)
+    return Settings(controls, penalty, vocab_range, temperature, top_k, bool(logprobs))
 
 
 PLAN_PHASES = ("qkv", "o", "gu", "d")   # phase order of the persistent kernel's work plan
@@ -324,6 +327,7 @@ class SpeechLM:
         self._slot_sp_host = None   # host mirror of the per-slot sampling controls (None: off)
         self._vocab_range = None    # (lo, hi) while the vocabulary range is on
         self._penalty_host = None   # host mirror of the per-slot repetition penalties (None: off)
+        self.logprobs = None        # per-token log-probabilities, [max_batch][max_new][2] on the device (None: off)
 
     def __del__(self):
         try:
@@ -406,6 +410,22 @@ class SpeechLM:
         so it is ordered before the next prefill or decode."""
         self._write_slot_table("_penalty_host", self.L.nt_lm_set_repetition_penalty, _lib.SlotPenalty, check_penalty,
                                DEFAULT_PENALTY, rows, slots)
+
+    def set_logprobs(self, on: bool = True):
+        """Per-token log-probabilities.  While on, every later sampler launch writes, for each token it writes to
+        ``out_tokens[s][n]``, the pair ``logprobs[s][n] = (sampled, model)`` into ``self.logprobs`` (device float32
+        [max_batch][max_new][2], allocated here and kept while on): ``sampled`` is the token's log-probability in the
+        kept window the sampler drew from (transformers' ``compute_transition_scores(normalize_logits=True)``; greedy
+        runs: equal to ``model``; teacher-forced ids outside the window: -inf), ``model`` its log-softmax over the whole
+        vocabulary after the repetition penalty, the min-new-tokens EOS mask and the vocabulary range, before
+        temperature and the warpers.  ``on=False`` switches it off and frees the buffer.  Returns the buffer or None."""
+        buf = (self.logprobs if self.logprobs is not None else
+               torch.zeros(self.max_batch, self.max_new, 2, dtype=torch.float32, device=self.device)) if on else None
+        with torch.cuda.device(self.device):
+            _lib.check(self.L.nt_lm_set_logprobs(self.handle, None if buf is None else buf.data_ptr(),
+                                                 _lib.current_stream_ptr()))
+        self.logprobs = buf
+        return buf
 
     def _stage_ids(self, prompts) -> torch.Tensor:
         """The prompts' ids, range-checked, back to back in a persistent pinned buffer (so their H2D copy is
@@ -573,6 +593,16 @@ class SpeechLM:
             raise ValueError("max_new_tokens needs one entry per prompt")
         return [min(max_length - n, int(m), self.max_new) for n, m in zip(lens, max_new_tokens)]
 
+    def _results(self, rows, ngen, logprobs: bool):
+        """Generated ids of ``rows`` (slots) as int64 CPU tensors, cut at ``ngen`` per row; with ``logprobs`` also
+        each row's float32 CPU ``[n, 2]`` (sampled, model) log-probabilities, read before any refill overwrites them."""
+        toks = self.out_tokens[rows].cpu()
+        ids = [toks[r, : int(n)].long() for r, n in enumerate(ngen)]
+        if not logprobs:
+            return ids, None
+        lp = self.logprobs[rows].cpu()
+        return ids, [lp[r, : int(n)].clone() for r, n in enumerate(ngen)]
+
     def _prepare(self, prompts, max_length, max_new_tokens, **settings) -> tuple:
         """Shared preamble of ``generate_batch`` / ``generate_queue``, run before any engine call: the max_length
         checks, the generated-token cap per prompt and the resolved ``settings`` -> (caps, Settings)."""
@@ -591,7 +621,7 @@ class SpeechLM:
                        temperature: float = 1.0, top_k: int = 50, max_new_tokens: int | None = None, seed: int = 0,
                        greedy: bool = False, forced: torch.Tensor | None = None, check_every: int = 64, slot_base: int = 0,
                        top_p: float = 1.0, min_p: float = 0.0, vocab_range=None, repetition_penalty=1.0,
-                       penalize_prompt=True):
+                       penalize_prompt=True, return_logprobs: bool = False):
         """Returns a list of int64 CPU tensors with the generated ids of each prompt (EOS included
         when it was sampled), following transformers' stopping rules (stopping_criteria.py:73-84,
         467-471): stop at EOS or when prompt + generated reaches max_length.  ``max_new_tokens`` may also be a
@@ -599,10 +629,14 @@ class SpeechLM:
         value per prompt (per-slot controls, ``set_slot_sampling``).  ``vocab_range``: (lo, hi) restricts every draw to
         [lo, hi) plus EOS (``set_vocab_range``); None leaves the range off.  ``repetition_penalty`` (> 0, 1 = off) and
         ``penalize_prompt`` (the prompt's ids count) are each a scalar or one value per prompt
-        (``set_repetition_penalty``); they apply to greedy and teacher-forced runs too."""
+        (``set_repetition_penalty``); they apply to greedy and teacher-forced runs too.  ``return_logprobs``: returns
+        ``(ids, logprobs)`` instead, ``logprobs[i]`` a float32 CPU tensor [len(ids[i]), 2] of (sampled, model)
+        log-probabilities per generated token (``set_logprobs``, switched on for the call and off by a later call
+        without it)."""
         caps, settings = self._prepare(prompts, max_length, max_new_tokens, temperature=temperature, top_k=top_k,
                                        top_p=top_p, min_p=min_p, vocab_range=vocab_range,
-                                       repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt)
+                                       repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt,
+                                       logprobs=return_logprobs)
         limit = max(caps)
         sp = self.sampling(eos_token_id, min_new_tokens, limit, settings.top_k, settings.temperature, seed, greedy,
                            forced, limits=caps if min(caps) < limit else None, slot_base=slot_base)
@@ -616,14 +650,14 @@ class SpeechLM:
             remaining -= n
             if remaining > 0 and bool(self.done[:B].all()):  # one small D2H read per `check_every` steps
                 break
-        ngen = self.n_generated[:B].cpu()
-        toks = self.out_tokens[:B].cpu()
-        return [toks[b, : int(ngen[b])].long() for b in range(B)]
+        ids, lps = self._results(slice(0, B), self.n_generated[:B].cpu().tolist(), return_logprobs)
+        return (ids, lps) if return_logprobs else ids
 
     def generate_queue(self, prompts, eos_token_id: int, max_length: int | None = None, min_new_tokens: int = 50,
                        temperature: float = 1.0, top_k: int = 50, max_new_tokens: int | None = None, seed: int = 0,
                        greedy: bool = False, check_every: int = 32, slot_base: int = 0, top_p: float = 1.0,
-                       min_p: float = 0.0, vocab_range=None, repetition_penalty=1.0, penalize_prompt=True):
+                       min_p: float = 0.0, vocab_range=None, repetition_penalty=1.0, penalize_prompt=True,
+                       return_logprobs: bool = False):
         """Continuous batching over any number of prompts: ``generate_batch``'s results and stopping rules, but a slot
         whose sequence finished is refilled with the next waiting prompt while the other slots keep decoding.
 
@@ -637,13 +671,16 @@ class SpeechLM:
         ``temperature``, ``top_k``, ``top_p`` and ``min_p`` are each a scalar or one value per prompt; a newcomer's
         controls are written into its slot before its prefill, and the other slots keep theirs.  ``vocab_range`` as in
         ``generate_batch``: set once before the first prefill, it holds across every refill.  ``repetition_penalty`` and
-        ``penalize_prompt`` as in ``generate_batch``; a newcomer's entry is written before its prefill."""
+        ``penalize_prompt`` as in ``generate_batch``; a newcomer's entry is written before its prefill.
+        ``return_logprobs`` as in ``generate_batch``: a finished slot's rows are copied out with its tokens, before
+        the refill that reuses the slot."""
         caps, settings = self._prepare(prompts, max_length, max_new_tokens, temperature=temperature, top_k=top_k,
                                        top_p=top_p, min_p=min_p, vocab_range=vocab_range,
-                                       repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt)
+                                       repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt,
+                                       logprobs=return_logprobs)
         n = len(prompts)
         if n == 0:
-            return []
+            return ([], []) if return_logprobs else []
         if check_every < 1:
             raise ValueError("check_every must be >= 1")
         S = min(n, self.max_batch)
@@ -655,6 +692,7 @@ class SpeechLM:
         ngen = [1] * S         # generated tokens per slot, as of the last read
         nxt = S                # next prompt to admit
         out = [None] * n
+        out_lp = [None] * n
         # a sequence can finish inside its prefill: a cap of 1, or EOS when it is not masked at step 0
         at_prefill = lambda idx: min_new_tokens <= 0 or min(caps[i] for i in idx) <= 1
         read = at_prefill(range(S))
@@ -664,9 +702,11 @@ class SpeechLM:
                 ngen = st[0].tolist()
                 fin = [s for s in range(S) if occ[s] is not None and int(st[1, s])]
                 if fin:
-                    rows = self.out_tokens[fin].cpu()
+                    ids, lps = self._results(fin, [ngen[s] for s in fin], return_logprobs)
                     for r, s in enumerate(fin):
-                        out[occ[s]] = rows[r, : ngen[s]].long()
+                        out[occ[s]] = ids[r]
+                        if return_logprobs:
+                            out_lp[occ[s]] = lps[r]
                         occ[s] = None
                     take = fin[: n - nxt]
                     if take:
@@ -687,7 +727,7 @@ class SpeechLM:
             self.decode(steps, sp)
             read = True
         self.release_pages()
-        return out
+        return (out, out_lp) if return_logprobs else out
 
     @torch.no_grad()
     def generate(self, input_ids: torch.Tensor, max_length: int = 2048, eos_token_id: int | None = None,
