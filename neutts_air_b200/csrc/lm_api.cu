@@ -89,7 +89,7 @@ struct StepSettings {
 
 struct nt_lm {
   nt_lm_config cfg;
-  int qkv_n, num_sms, max_splits, nchunks, max_rows;
+  int qkv_n, num_sms, max_splits, max_rows;
   const __nv_bfloat16* embed;
   const __nv_bfloat16* lm_head;
   const float* final_norm;
@@ -121,7 +121,7 @@ struct nt_lm {
   uint8_t* tc_maps = nullptr;         // CUtensorMap[4 * n_layers + 1] weights, then xa x {16,32,64}, act x {16,32,64}
   TcPlan* tc_plan = nullptr;
   __nv_bfloat16 *tc_xa = nullptr, *tc_act = nullptr;
-  float *tc_tmax = nullptr;
+  float* tmax = nullptr;              // [max_batch][ceil(V / 128)] tile maxima of the logits rows (see lm_head_rows)
   float2 *tc_pq2 = nullptr, *tc_po2 = nullptr, *tc_pd2 = nullptr, *tc_ao2 = nullptr, *tc_aml2 = nullptr, *tc_act2 = nullptr, *tc_pg2 = nullptr,
          *tc_h2 = nullptr;
   size_t tc_pair_bytes = 0;           // extent of the stamped buffers (contiguous, starting at tc_pq2)
@@ -163,7 +163,7 @@ static int vocab_fill(nt_lm* lm, int B, cudaStream_t stream) {
   if (!lm->step.vr_on) return NT_OK;
   const int V = lm->cfg.vocab_size, nt = (V + 127) / 128;
   int rc = launch_fill_neg_inf(lm->logits, static_cast<long long>(B) * V, stream);
-  if (!rc && lm->tc_tmax) rc = launch_fill_neg_inf(lm->tc_tmax, static_cast<long long>(B < lm->tc_rows ? B : lm->tc_rows) * nt, stream);
+  if (!rc) rc = launch_fill_neg_inf(lm->tmax, static_cast<long long>(B) * nt, stream);
   return rc;
 }
 
@@ -185,8 +185,9 @@ static size_t lm_carve(const nt_lm_config& c, void* ws, size_t bytes, F&& assign
     (L)->attn = a.take<float>(size_t(c.max_batch) * c.n_heads * 64);                           \
     (L)->act = a.take<float>(size_t(c.max_batch) * I);                                         \
     (L)->logits = a.take<float>(size_t(c.max_batch) * V);                                      \
-    (L)->cand_val = a.take<float>(sampler_scratch_floats(c.max_batch, V));                     \
-    (L)->cand_idx = a.take<int>(sampler_scratch_floats(c.max_batch, V));                       \
+    (L)->cand_val = a.take<float>(sampler_scratch_floats(c.max_batch));                        \
+    (L)->cand_idx = a.take<int>(sampler_scratch_floats(c.max_batch));                          \
+    (L)->tmax = a.take<float>(size_t(c.max_batch) * ((V + 127) / 128));                        \
     (L)->inv_freq = a.take<float>(64);                                                         \
     (L)->qkv = a.take<float>(size_t(rows) * qkv_n);                                            \
     (L)->h_last = a.take<float>(size_t(c.max_batch) * H);                                      \
@@ -208,7 +209,6 @@ static size_t lm_carve(const nt_lm_config& c, void* ws, size_t bytes, F&& assign
     (L)->tc_gu_nsl = a.take<unsigned char>(4096);                                              \
     (L)->tc_xa = a.take<__nv_bfloat16>(size_t(kTcMaxBatch) * H);                               \
     (L)->tc_act = a.take<__nv_bfloat16>(size_t(kTcMaxBatch) * I);                              \
-    (L)->tc_tmax = a.take<float>(size_t((L)->tc_rows) * ((V + 127) / 128));                    \
     (L)->tc_pq2 = a.take<float2>(size_t(kTcMaxSlices) * (L)->tc_rows * qkv_n);                 \
     (L)->tc_po2 = a.take<float2>(size_t(kTcMaxSlices) * (L)->tc_rows * H);                     \
     (L)->tc_pd2 = a.take<float2>(size_t(kTcMaxSlices) * (L)->tc_rows * H);                     \
@@ -268,7 +268,6 @@ extern "C" int nt_lm_create(const nt_lm_config* cfg, const nt_lm_weights* w, voi
   }
   lm->qkv_n = (c.n_heads + 2 * c.n_kv_heads) * 64;
   lm->max_splits = c.max_ctx / c.page_size;
-  lm->nchunks = sampler_nchunks(c.vocab_size);
   lm->max_rows = c.max_prefill_tokens > c.max_batch ? c.max_prefill_tokens : c.max_batch;
   lm->embed = static_cast<const __nv_bfloat16*>(w->embed);
   lm->lm_head = static_cast<const __nv_bfloat16*>(w->lm_head);
@@ -393,7 +392,6 @@ static SamplerParams make_sampler(const nt_lm* lm, const nt_lm_state* st, const 
   s.max_ctx = lm->cfg.max_ctx;
   s.cand_val = lm->cand_val;
   s.cand_idx = lm->cand_idx;
-  s.nchunks = lm->nchunks;
   s.embed = lm->embed;
   s.h = lm->h;
   s.hidden = lm->cfg.hidden;
@@ -416,14 +414,9 @@ static int check_sampling(const nt_lm* lm, const nt_lm_state* st, const nt_sampl
   return NT_OK;
 }
 
-// lm_head on B hidden rows (fp32, un-normalised) -> lm->logits / `logits`
-// tile-max sampler after the tensor-core lm_head (batch > 4): the GEMM must tile the vocabulary by 128 columns
-static bool use_tile_sampler(const nt_lm* lm, int B) {
-  return B > kGemvMaxBatch && B <= lm->tc_rows && lm->tc_tmax && gemm_tile_n(B, lm->cfg.vocab_size, false) == 128;
-}
+// the tile-max sampler on lm->logits rows [0, B) and the maxima lm_head_rows left in lm->tmax
 static int run_sampler(nt_lm* lm, const SamplerParams& s, int B, cudaStream_t stream) {
-  if (use_tile_sampler(lm, B)) return launch_sampler_tiles(s, B, lm->tc_tmax, (lm->cfg.vocab_size + 127) / 128, stream);
-  return launch_sampler(s, B, stream);
+  return launch_sampler_tiles(s, B, lm->tmax, (lm->cfg.vocab_size + 127) / 128, stream);
 }
 
 // While the repetition penalty is on (and eos >= 0), one fix-up launch after the lm_head rewrites each history logit
@@ -434,7 +427,10 @@ static int rep_fixup(nt_lm* lm, int B, float* logits, float* tmax, int eos, cons
   return launch_rep_penalty(logits, B, V, lm->rep_hist, lm->rep_words, lm->rep_tab, lm->rep_rec, row_slot, tmax, (V + 127) / 128, stream);
 }
 
-// eos >= 0: apply the vocabulary range with this EOS id (every sampler launch); -1: every row (nt_lm_head_gemv).  Under
+// lm_head on B hidden rows (fp32, un-normalised) -> `logits`.
+// eos >= 0: a sampler launch follows (logits = lm->logits): apply the vocabulary range with this EOS id and leave the
+// raw maximum of every 128-row tile of every row in lm->tmax; the GEMM epilogue takes them when it tiles the vocabulary
+// by 128, one small kernel on the finished rows otherwise.  -1: logits only, every row (nt_lm_head_gemv).  Under
 // the range the lm_head runs once over the range's rows and once over the EOS tile (when EOS lies outside them), each
 // a row slice of the full-vocabulary launch with the same per-row arithmetic, so every computed logit is bit-identical
 // to the range off; the rows it does not compute keep the -inf of vocab_fill.  row_slot: see rep_fixup.
@@ -448,6 +444,7 @@ static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cud
   const int r1[2] = {vt.t_hi * 128 < V ? vt.t_hi * 128 : V, (vt.eos_tile + 1) * 128 < V ? (vt.eos_tile + 1) * 128 : V};
   const int nslices = vt.eos_tile >= 0 ? 2 : 1;
   int rc;
+  float* tmax = nullptr;   // set when the GEMM epilogue writes the tile maxima
   if (B <= kGemvMaxBatch) {
     for (int i = 0; i < nslices; ++i) {
       GemvParams g;
@@ -458,36 +455,29 @@ static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cud
       g.epi = GEMV_STORE, g.out = logits + r0[i], g.ldo = V;
       if ((rc = launch_gemv(g, B, lm->num_sms, stream))) return rc;
     }
-    if (vt.eos_tile >= 0 && (rc = launch_vocab_eos_tile(logits, B, V, eos, nullptr, nt, stream))) return rc;
-    return rep_fixup(lm, B, logits, nullptr, eos, row_slot, stream);
-  }
-  // pend: the last down_proj left split-K slices that still have to be folded into hrows (batched decode only)
-  const bool fold = pend && pend->used > 1;
-  rc = launch_rmsnorm_rows(hrows, lm->final_norm, c.rms_eps, B, c.hidden, nullptr, lm->xn, stream, fold ? pend->ws : nullptr,
-                               fold ? pend->used : 0, fold ? pend->slice_stride : 0);
-  if (rc) return rc;
-  float* tmax = (use_tile_sampler(lm, B) && logits == lm->logits) ? lm->tc_tmax : nullptr;
-  if (!vt.on) {
-    nt_gemm_args a;
-    memset(&a, 0, sizeof(a));
-    a.dtype = NT_BF16, a.M = B, a.N = V, a.K = c.hidden;
-    a.A = lm->xn, a.lda = c.hidden, a.W = lm->lm_head, a.ldw = c.hidden;
-    a.out_f32 = logits, a.ldc = V;
-    if ((rc = gemm_dispatch(a, stream, nullptr, true, nullptr, tmax))) return rc;
-    return rep_fixup(lm, B, logits, tmax, eos, row_slot, stream);
-  }
-  // slices run at the full-vocabulary tile width; their tile maxima land at absolute tile indices (128-column tiles)
-  const int bn = gemm_tile_n(B, V, false);
-  for (int i = 0; i < nslices; ++i) {
-    nt_gemm_args a;
-    memset(&a, 0, sizeof(a));
-    a.dtype = NT_BF16, a.M = B, a.N = r1[i] - r0[i], a.K = c.hidden;
-    a.A = lm->xn, a.lda = c.hidden, a.W = lm->lm_head + static_cast<long long>(r0[i]) * c.hidden, a.ldw = c.hidden;
-    a.out_f32 = logits + r0[i], a.ldc = V;
-    if ((rc = gemm_dispatch(a, stream, nullptr, true, nullptr, tmax ? tmax + r0[i] / 128 : nullptr, bn, nt))) return rc;
+  } else {
+    // pend: the last down_proj left split-K slices that still have to be folded into hrows (batched decode only)
+    const bool fold = pend && pend->used > 1;
+    rc = launch_rmsnorm_rows(hrows, lm->final_norm, c.rms_eps, B, c.hidden, nullptr, lm->xn, stream, fold ? pend->ws : nullptr,
+                             fold ? pend->used : 0, fold ? pend->slice_stride : 0);
+    if (rc) return rc;
+    // slices run at the full-vocabulary tile width; their tile maxima land at absolute tile indices (128-column tiles)
+    const int bn = gemm_tile_n(B, V, false);
+    if (eos >= 0 && bn == 128) tmax = lm->tmax;
+    for (int i = 0; i < nslices; ++i) {
+      nt_gemm_args a;
+      memset(&a, 0, sizeof(a));
+      a.dtype = NT_BF16, a.M = B, a.N = r1[i] - r0[i], a.K = c.hidden;
+      a.A = lm->xn, a.lda = c.hidden, a.W = lm->lm_head + static_cast<long long>(r0[i]) * c.hidden, a.ldw = c.hidden;
+      a.out_f32 = logits + r0[i], a.ldc = V;
+      if ((rc = gemm_dispatch(a, stream, nullptr, true, nullptr, tmax ? tmax + r0[i] / 128 : nullptr, bn, nt))) return rc;
+    }
   }
   if (vt.eos_tile >= 0 && (rc = launch_vocab_eos_tile(logits, B, V, eos, tmax, nt, stream))) return rc;
-  return rep_fixup(lm, B, logits, tmax, eos, row_slot, stream);
+  if ((rc = rep_fixup(lm, B, logits, tmax, eos, row_slot, stream))) return rc;
+  // no epilogue maxima: the raw maxima of the finished rows (after the EOS tile and the penalty), as the epilogue has them
+  if (eos >= 0 && !tmax) return launch_tile_max(logits, B, V, lm->tmax, stream);
+  return NT_OK;
 }
 
 // Transformer layers over `rows` token rows held in lm->h, via tensor-core GEMMs.
@@ -777,7 +767,7 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
     lm->tc_stamp += need_s, lm->tc_hstamp += need_h;
     P.kv = make_kv(lm, st);
     if ((rc = kv_pool_tmap(P.kv, c.n_layers, &P.kvmap))) return rc;
-    P.logits = lm->logits, P.tmax = lm->tc_tmax, P.ntiles = info.ntiles;
+    P.logits = lm->logits, P.tmax = lm->tmax, P.ntiles = info.ntiles;
     // lm_head tile list under the vocabulary range: the EOS tile sits before or after the range's tiles, in tile order
     const VocabTiles vt = vocab_tiles(lm, sp->eos_id);
     P.head_n = vt.count(), P.head_lo = vt.t_lo, P.head_eos = vt.eos_tile;
@@ -969,7 +959,7 @@ extern "C" void* nt_lm_debug_ptr(nt_lm* lm, const char* name) {
   const struct { const char* n; void* p; } tab[] = {
       {"h", lm->h}, {"q", lm->q}, {"qkv", lm->qkv}, {"attn", lm->attn}, {"act", lm->act}, {"logits", lm->logits},
       {"xn", lm->xn}, {"attn_bf16", lm->attn_bf16}, {"act_bf16", lm->act_bf16}, {"h_last", lm->h_last},
-      {"tmax", lm->tc_tmax}};
+      {"tmax", lm->tmax}};
   for (const auto& e : tab)
     if (!strcmp(e.n, name)) return e.p;
   return nullptr;
@@ -1004,13 +994,17 @@ extern "C" int nt_op_topk_sample(const float* logits, int B, int V, const nt_sam
   SamplerParams s;
   memset(&s, 0, sizeof(s));
   s.logits = logits, s.V = V, s.sp = *sp;
-  s.nchunks = sampler_nchunks(V);
-  s.cand_val = a.take<float>(sampler_scratch_floats(B, V));
-  s.cand_idx = a.take<int>(sampler_scratch_floats(B, V));
+  const int nt = (V + 127) / 128;
+  s.cand_val = a.take<float>(sampler_scratch_floats(B));
+  s.cand_idx = a.take<int>(sampler_scratch_floats(B));
+  float* tmax = a.take<float>(size_t(B) * nt);
   if (!a.ok()) return set_error(NT_ERR_NOMEM, "nt_op_topk_sample: workspace too small (need %zu)", a.off);
-  s.n_generated_override = n_generated;
+  s.n_generated_override = n_generated;   // stateless: read-only counters, no state update
   s.step_override = step;
   s.dbg_token = out_token, s.dbg_topk_val = out_topk_val, s.dbg_topk_idx = out_topk_idx;
   s.max_new = 1 << 30, s.max_ctx = 1 << 30;
-  return launch_sampler(s, B, reinterpret_cast<cudaStream_t>(stream));
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  int rc = launch_sampler_check(s);
+  if (!rc) rc = launch_tile_max(logits, B, V, tmax, st);
+  return rc ? rc : launch_sampler_tiles(s, B, tmax, nt, st);
 }

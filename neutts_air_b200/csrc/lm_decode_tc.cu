@@ -156,7 +156,7 @@ struct TcMisc {
   float tile_max[2][4][kTcMaxBatch];
   float rstd[8];
   int sel[8];
-  int nchunks[4];         // B-operand chunks of this CTA's items per split phase
+  int bchunks[4];         // B-operand chunks of this CTA's items per split phase
   int ckb[4][16];         // k-block staged in chunk c (qkv / down: k-block of the input; o_proj: head)
   TcPlan plan;
 };
@@ -217,7 +217,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     int c = 0;
     for (int i = 0; i < plan.n[tid]; ++i)
       for (int kb = 0; kb < plan.it[tid][i].nkb && c < 16; ++kb, ++c) ms->ckb[tid][c] = plan.it[tid][i].kb0 + kb;
-    ms->nchunks[tid] = c;
+    ms->bchunks[tid] = c;
   } else if (tid == 4) {   // this CTA's positions in the lm_head tile list
     ms->plan.head_t0 = static_cast<int>((static_cast<long long>(P.head_n) * blockIdx.x) / gridDim.x);
     ms->plan.head_t1 = static_cast<int>((static_cast<long long>(P.head_n) * (blockIdx.x + 1)) / gridDim.x);
@@ -399,7 +399,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     auto load_bop_split = [&](const CUtensorMap* m, int ph) {   // chunks of the items' own k ranges, item after item
       const int n = uniform(plan.n[ph]);
       if (n == 0) return;
-      const int nch = uniform(ms->nchunks[ph]);
+      const int nch = uniform(ms->bchunks[ph]);
       if (elect_one()) {   // no wait inside: one election covers the whole batch of copies
         fence_proxy_async_all();
         mbar_arrive_expect_tx(&ms->bop_bar, static_cast<uint32_t>(nch) * CHUNK);
@@ -539,7 +539,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
           rs[b] = rsqrtf(t / static_cast<float>(H) + P.eps);
         }
       }
-      const int nch = ph < 0 ? KBH : ms->nchunks[ph];
+      const int nch = ph < 0 ? KBH : ms->bchunks[ph];
       const int per = B * 64;
       for (int e = tid; e < nch * per; e += kConsumerThreads) {
         const int c = e / per, r = e - c * per, b = r >> 6, k = r & 63;
@@ -799,7 +799,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     // attention split skips the attention barriers), so the staging below starts with a consumer barrier.
     auto stage_attn = [&](int stamp) {
       csync();
-      const int nch = ms->nchunks[kPhO];
+      const int nch = ms->bchunks[kPhO];
       const int per = B * 64;
       for (int e = tid; e < nch * per; e += kConsumerThreads) {
         const int c = e / per, r = e - c * per, b = r >> 6, d = r & 63;
@@ -854,7 +854,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     // ---- batch <= 4: down_proj input from the (value, stamp) SwiGLU outputs, two elements per thread
     auto stage_act = [&](int stamp) {
       csync();   // the B chunks of the gate/up phase are free (see stage_attn)
-      const int nch = ms->nchunks[kPhD];
+      const int nch = ms->bchunks[kPhD];
       const int per = B * 32;
       for (int e = tid; e < nch * per; e += kConsumerThreads) {
         const int c = e / per, r = e - c * per, b = r >> 5, k = (r & 31) * 2;
@@ -995,7 +995,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
       const float h2stamp = __int_as_float(P.hstamp_base + fold_no);
       // the epilogue stored PROCESSED maxima (temperature, EOS mask): no scale, no tile to fix up
       sample_tiles_seq(P.samp, b, P.tmax, P.ntiles, 1.0f, -1, 0.f, P.logits, P.vocab, ms->mask_eos[b] != 0, uni, P.uni_bytes, ms->sel,
-                       csync, pm, h2dst, h2stamp);
+                       csync, pm, h2dst, h2stamp, false);
     };
 
     // =============================================================== the decode loop

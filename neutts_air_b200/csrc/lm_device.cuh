@@ -74,8 +74,8 @@ NT_DEVINL void philox4x32_10(uint32_t (&ctr)[4], uint32_t k0, uint32_t k1) {
   }
 }
 
-constexpr int kTopChunk = 2048;
 constexpr int kTopKeep = 64;
+constexpr int kCandPitch = 256 * kTopKeep;          // row pitch of the candidate arrays (sampler_scratch_floats)
 constexpr int kSelList = 512;                       // radix select switches to a compacted list below this size
 constexpr int kSelScratch = 264 + kSelList;         // uint32 words of scratch the selector needs
 
@@ -221,28 +221,6 @@ NT_DEVINL void compact_topk(const uint32_t* keys, int n, uint32_t thr, int take_
   }
 }
 
-// Top-kTopKeep of n processed scores already held as keys in shared memory -> candidate slots
-// [o, o + kTopKeep) of the global candidate arrays (processed score, global index = idx_base + i).
-template <typename Sync>
-NT_DEVINL void emit_local_topk(const SamplerParams& p, const uint32_t* keys, int n, int idx_base, long long o, uint32_t* scratch,
-                               Sync sync) {
-  const int tid = threadIdx.x;
-  const int k = min(kTopKeep, n);
-  if (k > 0) {
-    uint32_t thr;
-    int take_eq;
-    radix_select_kth(keys, n, k, scratch, thr, take_eq, sync);
-    compact_topk(keys, n, thr, take_eq, scratch, sync, [&](int slot, int i) {
-      p.cand_val[o + slot] = key2f(keys[i]);
-      p.cand_idx[o + slot] = idx_base + i;
-    });
-  }
-  for (int s = k + tid; s < kTopKeep; s += kConsumerThreads) {
-    p.cand_val[o + s] = -INFINITY;
-    p.cand_idx[o + s] = 0x7fffffff;
-  }
-}
-
 // Sampling controls of the row whose state lives in `slot`: its entry of the per-slot table when that is on, else the
 // launch scalars with top-p and min-p off.  Every sampler path reads temperature and top_k here, so all of them form
 // the same fp32 1 / T.
@@ -325,35 +303,6 @@ NT_DEVINL float row_logsumexp(const float* lg, int V, int eos, bool mask_eos, fl
 #pragma unroll
   for (int w = 0; w < kConsumerWarps; ++w) combine(m, s, red[w].x, red[w].y);
   return m + logf(s);
-}
-
-// Sampler stage 1 for one (sequence b, chunk): processors + exact top-64 of a 2048-logit chunk read
-// from global memory.  keys: [kTopChunk] uint32 shared; scratch: [kSelScratch] uint32 shared.
-template <typename Sync>
-NT_DEVINL void sample_stage1_chunk(const SamplerParams& p, int b, int chunk, uint32_t* keys, uint32_t* scratch, Sync sync, int slot = -1) {
-  const int tid = threadIdx.x;
-  const int ngen = p.n_generated_override ? __ldcg(p.n_generated_override + b) : __ldcg(p.n_generated + (slot >= 0 ? slot : b));
-  const bool mask_eos = ngen < p.sp.min_new_tokens;
-  const float inv_t = row_sampling(p, slot >= 0 ? slot : b).inv_t;
-  const float* lg = p.logits + static_cast<long long>(b) * p.V;
-  const int base = chunk * kTopChunk;
-  const int n = min(kTopChunk, p.V - base);
-  sync();  // keys/scratch may still be in use by the previous call of this CTA
-  {
-    float v[kTopChunk / kConsumerThreads];
-#pragma unroll
-    for (int j = 0; j < kTopChunk / kConsumerThreads; ++j) {
-      const int e = j * kConsumerThreads + tid;
-      v[j] = (e < n) ? __ldcg(lg + base + e) : 0.f;
-    }
-#pragma unroll
-    for (int j = 0; j < kTopChunk / kConsumerThreads; ++j) {
-      const int e = j * kConsumerThreads + tid;
-      if (e < n) keys[e] = processed_key(v[j], base + e, mask_eos, p.sp.eos_id, inv_t);
-    }
-  }
-  sync();
-  emit_local_topk(p, keys, n, base, (static_cast<long long>(b) * p.nchunks + chunk) * kTopKeep, scratch, sync);
 }
 
 // Tail of the sampler for sequence b, given the k kept candidates sorted (score desc, index asc) in win[0..k):
@@ -481,23 +430,20 @@ NT_DEVINL void sample_finish(const SamplerParams& p, int b, int k, Cand* win, in
   }
 }
 
-// Sampler stage 2 for sequence b: top-k of the candidate scores (already processed), softmax, draw,
-// state update, next embedding.  keys: [ncand] uint32 shared; scratch: [kSelScratch]; win: [2*kTopKeep].
-struct NoMark {
-  NT_DEVINL void operator()() const {}
-};
-template <typename Sync, typename Mark = NoMark>
+// General path of sample_tiles_seq, second half, for sequence b: top-k of the ncand candidate scores (already
+// processed) in row b of the candidate arrays, softmax, draw, state update, next embedding.  keys: [ncand] uint32
+// shared; scratch: [kSelScratch]; win: [2*kTopKeep].  Stateless (see sample_tiles_seq) when p.n_generated_override is
+// set: a run-time test here, where a caller's compile-time flag shifts ptxas's spills in the persistent kernel.
+template <typename Sync>
 NT_DEVINL void sample_stage2_seq(const SamplerParams& p, int b, int ncand, uint32_t* keys, uint32_t* scratch, Cand* win, int* s_tok,
-                                 Sync sync, Mark mark = Mark(), long long cand_stride = -1, int slot = -1) {
+                                 Sync sync, int slot = -1) {
   const int tid = threadIdx.x;
   const bool stateless = p.n_generated_override != nullptr;
   const int s = slot >= 0 ? slot : b;
   const int ngen = stateless ? __ldcg(p.n_generated_override + b) : __ldcg(p.n_generated + s);
   const bool is_done = stateless ? false : (__ldcg(p.done + s) != 0);
-  // candidate rows: [b * stride, b * stride + ncand); stride = ncand unless the caller's rows have their own pitch
-  const long long cstride = cand_stride >= 0 ? cand_stride : static_cast<long long>(ncand);
-  const float* cv = p.cand_val + static_cast<long long>(b) * cstride;
-  const int32_t* ci = p.cand_idx + static_cast<long long>(b) * cstride;
+  const float* cv = p.cand_val + static_cast<long long>(b) * kCandPitch;
+  const int32_t* ci = p.cand_idx + static_cast<long long>(b) * kCandPitch;
   Cand* raw = win + kTopKeep;  // unsorted winners
   sync();
   for (int e0 = 0; e0 < ncand; e0 += 8 * kConsumerThreads) {  // 8 independent loads in flight per thread
@@ -515,18 +461,15 @@ NT_DEVINL void sample_stage2_seq(const SamplerParams& p, int b, int ncand, uint3
   }
   if (tid < kTopKeep) raw[tid].v = -INFINITY, raw[tid].i = 0x7fffffff;
   sync();
-  mark();  // keys staged
   const int k = min(min(row_sampling(p, s).top_k, kTopKeep), ncand);
   uint32_t thr;
   int take_eq;
   radix_select_kth(keys, ncand, k, scratch, thr, take_eq, sync);
-  mark();  // threshold found
   compact_topk(keys, ncand, thr, take_eq, scratch, sync, [&](int slot, int i) {
     raw[slot].v = key2f(keys[i]);
     raw[slot].i = __ldcg(ci + i);
   });
   sync();
-  mark();  // winners gathered
   if (tid < kTopKeep) {  // rank sort of the 64 winners: (score desc, index asc), ties of padding by slot
     const Cand me = raw[tid];
     int rank = 0;
@@ -537,8 +480,6 @@ NT_DEVINL void sample_stage2_seq(const SamplerParams& p, int b, int ncand, uint3
     win[rank] = me;
   }
   sync();
-  mark();  // winners sorted
-
   sample_finish(p, b, k, win, s_tok, stateless, ngen, is_done, sync, nullptr, 0.f, slot);
 }
 
@@ -552,10 +493,11 @@ NT_DEVINL void sample_stage2_seq(const SamplerParams& p, int b, int ncand, uint3
 //   tmax: [*, nt] tile maxima (times tmax_scale = processed maxima); fix_tile >= 0: that tile's processed maximum is
 //   fix_val instead (the tile holding a masked EOS, when the maxima were taken on raw logits).
 //   uni / uni_bytes: >= 16 KB of shared scratch (1024-byte aligned); sel: >= 4 ints of shared memory.
+//   stateless (nt_op_topk_sample): n_generated_override[b] is the row's count, the row is live and no state is written.
 template <typename Sync, typename Mark>
 NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax, int nt, float tmax_scale, int fix_tile, float fix_val,
                                 const float* logits, int V, bool mask_eos, uint8_t* uni, unsigned uni_bytes, int* sel, Sync sync, Mark pm,
-                                float2* h2dst, float h2stamp, int slot = -1) {
+                                float2* h2dst, float h2stamp, bool stateless, int slot = -1) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int H = p.hidden;
   uint32_t* scratch = reinterpret_cast<uint32_t*>(uni);
@@ -569,9 +511,8 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
   const float inv_t = rs.inv_t;
   const int top_k = rs.top_k;
   const int eos = p.sp.eos_id;
-  const bool stateless = false;
-  const int ngen = __ldcg(p.n_generated + (slot >= 0 ? slot : b));
-  const bool is_done = __ldcg(p.done + (slot >= 0 ? slot : b)) != 0;
+  const int ngen = stateless ? __ldcg(p.n_generated_override + b) : __ldcg(p.n_generated + (slot >= 0 ? slot : b));
+  const bool is_done = stateless ? false : __ldcg(p.done + (slot >= 0 ? slot : b)) != 0;
   const float* lg = logits + static_cast<long long>(b) * V;
   // row b starts b * V floats in: with V % 4 != 0 only some rows are 16-byte aligned for the float4 loads (CTA-uniform)
   const bool vec4 = (reinterpret_cast<uintptr_t>(lg) & 15) == 0;
@@ -817,7 +758,6 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
   sync();
   const int ncand = min(min(sel[0], key_cap), 256 * kTopKeep);   // beyond: thousands of exact ties at the threshold
   // pass 2: write the candidates at their deterministic offsets
-  constexpr long long kCandPitch = 256 * kTopKeep;   // row pitch of the candidate arrays (sampler_scratch_floats)
   float* cv = p.cand_val + static_cast<long long>(b) * kCandPitch;
   int32_t* ci = p.cand_idx + static_cast<long long>(b) * kCandPitch;
   for (int j = warp; j < k; j += kConsumerWarps) {
@@ -850,7 +790,7 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
     }
   }
   sync();
-  sample_stage2_seq(p, b, ncand, keys, scratch, win, s_tok, sync, NoMark(), kCandPitch, slot);
+  sample_stage2_seq(p, b, ncand, keys, scratch, win, s_tok, sync, slot);
   if (h2dst) {  // the next token's embedding becomes the residual stream of the next step's first fold
     sync();
     for (int i = tid; i < H; i += kConsumerThreads) h2dst[i] = make_float2(p.h[static_cast<long long>(b) * H + i], h2stamp);

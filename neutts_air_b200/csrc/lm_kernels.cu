@@ -742,55 +742,51 @@ int launch_attn_decode(const AttnDecParams& p, int B, int n_layers, cudaStream_t
 }
 
 // =================================================================================== sampler
-int sampler_nchunks(int V) { return (V + kTopChunk - 1) / kTopChunk; }
-// candidate arrays: [sequence][chunk][64], indexed by 2048-logit chunk.  At least 256 chunks per sequence: the general
-// path of sample_tiles_seq writes up to 256 * kTopKeep candidates per sequence (row pitch kCandPitch).
-size_t sampler_scratch_floats(int B, int V) {
-  const int chunks = sampler_nchunks(V) > 256 ? sampler_nchunks(V) : 256;
-  return size_t(B) * chunks * kTopKeep;
-}
+// candidate arrays: [sequence][kCandPitch], the general path of sample_tiles_seq writes up to 256 * kTopKeep
+// candidates per sequence
+size_t sampler_scratch_floats(int B) { return size_t(B) * kCandPitch; }
 
-// stage 1: grid (nchunks, B), 256 threads
-__global__ void __launch_bounds__(kConsumerThreads) topk_stage1_kernel(const SamplerParams p) {
-  __shared__ uint32_t keys[kTopChunk];
-  __shared__ uint32_t scratch[kSelScratch];
-  pdl_launch_dependents();
-  pdl_wait();
-  sample_stage1_chunk(p, blockIdx.y, blockIdx.x, keys, scratch, SyncAll(), p.row_slot ? __ldg(p.row_slot + blockIdx.y) : -1);
-}
-
-// stage 2: grid (B), 256 threads
-__global__ void __launch_bounds__(kConsumerThreads) topk_stage2_kernel(const SamplerParams p, const int ncand) {
-  extern __shared__ uint8_t smem_raw[];
-  __shared__ uint32_t scratch[kSelScratch];
-  __shared__ Cand win[2 * kTopKeep];
-  __shared__ int s_tok;
-  pdl_launch_dependents();
-  pdl_wait();
-  sample_stage2_seq(p, blockIdx.x, ncand, reinterpret_cast<uint32_t*>(smem_raw), scratch, win, &s_tok, SyncAll(), NoMark(), -1,
-                    p.row_slot ? __ldg(p.row_slot + blockIdx.x) : -1);
-}
+// The general path of sample_tiles_seq stages one key per 128-id tile in shared memory: at most kMaxTiles tiles
+// (50 KB of keys), i.e. V <= 1 638 400.
+constexpr int kMaxTiles = 12800;
 
 int launch_sampler_check(const SamplerParams& p) {
   if (p.sp.top_k < 1 || p.sp.top_k > kTopKeep) return set_error(NT_ERR_INVALID, "sampler: top_k=%d not in 1..64", p.sp.top_k);
   if (!(p.sp.temperature > 0.f)) return set_error(NT_ERR_INVALID, "sampler: temperature must be > 0");
-  if (size_t(p.nchunks) * kTopKeep * sizeof(uint32_t) > 200 * 1024) return set_error(NT_ERR_INVALID, "sampler: vocabulary too large (%d)", p.V);
+  if ((p.V + 127) / 128 > kMaxTiles) return set_error(NT_ERR_INVALID, "sampler: vocabulary too large (%d)", p.V);
   return NT_OK;
 }
 
-int launch_sampler(const SamplerParams& p, int B, cudaStream_t stream) {
-  if (int rc0 = launch_sampler_check(p)) return rc0;
-  const int ncand = p.nchunks * kTopKeep;
-  const size_t smem = size_t(ncand) * sizeof(uint32_t);
-  int rc = launch_kernel(topk_stage1_kernel, dim3(p.nchunks, B), dim3(kConsumerThreads), 0, stream, true, p);
-  if (rc) return rc;
-  return launch_kernel(topk_stage2_kernel, dim3(B), dim3(kConsumerThreads), smem, stream, true, p, ncand);
+// Raw maximum of every 128-id tile of logits rows [0, B) -> tmax [B][nt] (the last tile may be partial): the maxima
+// the lm_head GEMM epilogue writes when it tiles the vocabulary by 128, for every other lm_head and for
+// nt_op_topk_sample.  grid (ceil(nt / 8), B), 256 threads: one warp per tile, one float4 per lane.
+__global__ void __launch_bounds__(256) tile_max_kernel(const float* logits, int V, float* tmax, int nt) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int tile = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (tile >= nt) return;
+  const float* lg = logits + static_cast<long long>(blockIdx.y) * V;
+  const int r0 = tile * 128 + lane * 4;
+  float m = -INFINITY;
+  // row b starts b * V floats in: with V % 4 != 0 only some rows are 16-byte aligned for the float4 load
+  if ((reinterpret_cast<uintptr_t>(lg) & 15) == 0 && r0 + 3 < V) {
+    const float4 x = __ldcg(reinterpret_cast<const float4*>(lg + r0));
+    m = fmaxf(fmaxf(x.x, x.y), fmaxf(x.z, x.w));
+  } else {
+    for (int q = 0; q < 4; ++q)
+      if (r0 + q < V) m = fmaxf(m, __ldcg(lg + r0 + q));
+  }
+  m = warp_max(m);
+  if (lane == 0) tmax[static_cast<long long>(blockIdx.y) * nt + tile] = m;
+}
+int launch_tile_max(const float* logits, int B, int V, float* tmax, cudaStream_t s) {
+  const int nt = (V + 127) / 128;
+  return launch_kernel(tile_max_kernel, dim3((nt + 7) / 8, B), dim3(256), 0, s, true, logits, V, tmax, nt);
 }
 
-// Tile-max sampler for the tensor-core lm_head GEMM (batch > 4): the GEMM epilogue left the RAW maximum of every
-// 128-column tile per sequence; one CTA per sequence picks the candidate tiles from those maxima and ranks the few
-// dozen candidate logits (sample_tiles_seq, the scheme of the persistent decode kernel).  Replaces topk_stage1 (a
-// radix select over every 2048-logit chunk: 98 us at batch 64) + topk_stage2 (29 us) by one ~20 us launch.
+// Tile-max sampler outside the persistent decode kernel: tmax holds the RAW maximum of every 128-column tile per
+// sequence (the lm_head GEMM epilogue's, or launch_tile_max's); one CTA per sequence picks the candidate tiles from
+// those maxima and ranks the few dozen candidate logits (sample_tiles_seq, the scheme of the persistent decode kernel).
 struct NoMarkI {
   NT_DEVINL void operator()(int) const {}
 };
@@ -804,7 +800,9 @@ __global__ void __launch_bounds__(kConsumerThreads) topk_tiles_kernel(const Samp
   pdl_wait();
   const int b = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int slot = p.row_slot ? __ldg(p.row_slot + b) : b;
-  const bool mask_eos = __ldcg(p.n_generated + slot) < p.sp.min_new_tokens;
+  const bool stateless = p.n_generated_override != nullptr;
+  const int ngen = stateless ? __ldcg(p.n_generated_override + b) : __ldcg(p.n_generated + slot);
+  const bool mask_eos = ngen < p.sp.min_new_tokens;
   const float inv_t = row_sampling(p, slot).inv_t;
   int fix_tile = -1;
   float fix_val = 0.f;
@@ -823,12 +821,11 @@ __global__ void __launch_bounds__(kConsumerThreads) topk_tiles_kernel(const Samp
     fix_val = fix;
   }
   sample_tiles_seq(p, b, tmax, nt, inv_t, fix_tile, fix_val, p.logits, p.V, mask_eos, uni, kTilesScratch, sel, SyncAll(), NoMarkI(),
-                   static_cast<float2*>(nullptr), 0.f, slot);
+                   static_cast<float2*>(nullptr), 0.f, stateless, slot);
 }
 
 int launch_sampler_tiles(const SamplerParams& p, int B, const float* tmax, int nt, cudaStream_t stream) {
   if (int rc0 = launch_sampler_check(p)) return rc0;
-  if (p.n_generated_override) return set_error(NT_ERR_INVALID, "tile-max sampler: stateless mode unsupported");
   const int smem = int(kTilesScratch) + 1024;
   return launch_kernel(topk_tiles_kernel, dim3(B), dim3(kConsumerThreads), smem, stream, true, p, tmax, nt);
 }

@@ -75,10 +75,9 @@ struct SamplerParams {
   int32_t* done;
   int max_new, max_ctx;
   int advance;  // 1 in a decode step (seq_lens += 1 for live slots), 0 after prefill
-  // candidates scratch: [B, nchunks, 64] (val, idx)
+  // candidates scratch: [B][kCandPitch] (val, idx), the general path of sample_tiles_seq
   float* cand_val;
   int32_t* cand_idx;
-  int nchunks;
   // next-step embedding
   const __nv_bfloat16* embed;
   float* h;  // [B, hidden]
@@ -105,18 +104,19 @@ struct SamplerParams {
   // sample_finish writes the pair of every token it writes to out_tokens.
   float* logprob_out;
 };
-int launch_sampler(const SamplerParams& p, int B, cudaStream_t stream);
 int launch_sampler_check(const SamplerParams& p);
-// tmax: [B][nt] RAW maxima of the 128-column tiles of p.logits (GEMM epilogue, gemm_dispatch(..., tile_max))
+// tmax: [B][nt] RAW maxima of the 128-column tiles of p.logits (GEMM epilogue, gemm_dispatch(..., tile_max), or
+// launch_tile_max).  p.n_generated_override set: stateless (nt_op_topk_sample).
 int launch_sampler_tiles(const SamplerParams& p, int B, const float* tmax, int nt, cudaStream_t stream);
-size_t sampler_scratch_floats(int B, int V);  // per-array element count for cand_val / cand_idx
+// tmax [B][ceil(V / 128)] = the raw maximum of every 128-column tile of logits rows [0, B)
+int launch_tile_max(const float* logits, int B, int V, float* tmax, cudaStream_t s);
+size_t sampler_scratch_floats(int B);  // per-array element count for cand_val / cand_idx
 // Vocabulary range (nt_lm_set_vocab_range).  launch_fill_neg_inf: p[0, n) = -inf (the logits rows and tile maxima of a
 // launch, before its lm_head writes the tiles it computes).  launch_vocab_eos_tile: after an lm_head that computed the
 // whole 128-row tile holding `eos` although only `eos` is allowed there, rows [0, B) of that tile read -inf except eos,
 // and tmax (optional, [B][nt] raw maxima) holds the eos logit as the tile's maximum.
 int launch_fill_neg_inf(float* p, long long n, cudaStream_t s);
 int launch_vocab_eos_tile(float* logits, int B, int V, int eos, float* tmax, int nt, cudaStream_t s);
-int sampler_nchunks(int V);
 // Repetition penalty.  launch_rep_history: one CTA per prefill row i builds the history row of slot row_slot[i] (row i
 // when row_slot is nullptr): cleared, then the ids ids[cu[i] .. cu[i + 1]) when the slot's entry includes the prompt;
 // the slot becomes recorded.  launch_rep_penalty: the CTAs of logits row i of `logits` [B][V] rewrite the logit of

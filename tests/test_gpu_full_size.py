@@ -68,12 +68,16 @@ def test_full_size_batch_invariance_and_reproducibility(full_lm):
                          ids=["persistent-b1", "persistent-b3", "persistent-b6", "chain-b6-tile-sampler"])
 def test_decode_kernel_sampler_matches_standalone_sampler(full_lm, B, impl, monkeypatch):
     """The persistent decode kernel samples inside the kernel (tile maxima -> candidate tiles -> exact top-k ->
-    Philox draw); the per-op chain runs the same scheme as a kernel of its own behind the lm_head GEMM.  Given the logits it returns for a step, the stand-alone sampler op (``nt_op_topk_sample``, pinned
-    to the HF processors + multinomial by tests/test_gpu_kernels.py) must pick the very same token: same top-50 set,
-    same probabilities, same Philox counter (seed, slot, n_generated).  Covers the EOS mask (min_new_tokens) too."""
+    Philox draw); the per-op chain runs the same scheme as a kernel of its own behind the lm_head GEMM.  Given the logits
+    it returns for a step, the stand-alone sampler op (``nt_op_topk_sample``, pinned to the HF processors +
+    multinomial by tests/test_gpu_kernels.py) must pick the very same token: same top-50 set, same probabilities, same
+    Philox counter (seed, slot, n_generated).  All three run ``sample_tiles_seq``, so the window and the token are also
+    held to the float64 sampler of test_gpu_sampler on the same logits and Philox draw.  Covers the EOS mask
+    (min_new_tokens) too."""
     import ctypes as C
 
     from neutts_air_b200 import _lib
+    from tests.test_gpu_sampler import BARS, draw_u, prob_err, ref_token, ref_window
 
     if impl:   # the per-op chain: tensor-core lm_head with tile maxima in its epilogue + topk_tiles_kernel
         monkeypatch.setenv("NT_DECODE_IMPL", impl)
@@ -100,3 +104,10 @@ def test_decode_kernel_sampler_matches_standalone_sampler(full_lm, B, impl, monk
         assert tok.cpu().tolist() == toks[:, ngen].tolist(), (s, tok.cpu().tolist(), toks[:, ngen].tolist())
         if ngen < 5:
             assert eos not in ti[:, :50].cpu().flatten().tolist()
+        rows, tvs, tis = row.cpu().numpy(), tv.cpu().numpy(), ti.cpu().numpy()
+        for b in range(B):
+            ids, p = ref_window(rows[b], ngen, eos, 5, 50, 0.8)
+            assert tis[b, :50].tolist() == ids.tolist() and (tis[b, 50:] == -1).all(), (s, b)
+            assert prob_err(tvs[b, :50], p) < BARS["prob"], (s, b)
+            _, ok = ref_token((ids, p), draw_u(sp.seed, ngen, b + sp.slot_base))
+            assert int(toks[b, ngen]) in ok, (s, b, int(toks[b, ngen]), ok)

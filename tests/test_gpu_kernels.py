@@ -169,14 +169,18 @@ def test_sampler_topk_set_eos_mask_and_distribution(cuda):
     logits = torch.randn(2, V, generator=g) * 2
     logits[:, eos] = 30.0                                   # EOS would dominate if not masked
     sp = _lib.Sampling(eos, 50, 1 << 20, 50, 0.7, 1234, 0, None)
-    tok, tv, ti = _sample(L, logits.to(cuda), sp, [10, 60], 0)
-    for b, ngen in enumerate([10, 60]):
-        idx, p = topk_probs(logits[b], ngen, eos, 50, 0.7, 50)
-        assert ti[b, :50].tolist() == idx.tolist()          # exact top-50 set and order
-        assert (ti[b, 50:] == -1).all()
-        assert max_err(tv[b, :50], p) < 1e-5
-        assert (eos in ti[b, :50].tolist()) == (ngen >= 50)
-        assert int(tok[b]) in idx.tolist()
+    # V = 4142: 33 tiles, fewer than top_k, so every logit is a candidate (the general path of sample_tiles_seq)
+    small = torch.randn(2, 4142, generator=g) * 2
+    small[:, 4100] = 30.0
+    for lg, e in ((logits, eos), (small, 4100)):
+        tok, tv, ti = _sample(L, lg.to(cuda), _lib.Sampling(e, 50, 1 << 20, 50, 0.7, 1234, 0, None), [10, 60], 0)
+        for b, ngen in enumerate([10, 60]):
+            idx, p = topk_probs(lg[b], ngen, e, 50, 0.7, 50)
+            assert ti[b, :50].tolist() == idx.tolist()          # exact top-50 set and order
+            assert (ti[b, 50:] == -1).all()
+            assert max_err(tv[b, :50], p) < 1e-5
+            assert (e in ti[b, :50].tolist()) == (ngen >= 50)
+            assert int(tok[b]) in idx.tolist()
     # chi-square of 20000 draws against the oracle distribution (RNG streams cannot match torch.multinomial)
     idx, p = topk_probs(logits[0], 10, eos, 50, 0.7, 50)
     counts = torch.zeros(50)

@@ -5,14 +5,14 @@ wrong threshold, tie order or EOS mask changes the audio without moving one logi
 sampler path kept and drew with a plain float64 reference that reads the operands the kernel read: its own logits
 (returned by the call), its own ``n_generated`` and its own Philox counter.
 
-Sampler paths (all end in ``sample_finish`` in lm_device.cuh):
-  * radix sampler (``topk_stage1_kernel`` + ``topk_stage2_kernel``): prefill and the per-op decode chain at batch <= 4,
-    ``prefill_slots`` with a ``row_slot`` map, and every batch whose lm_head GEMM does not tile the vocabulary by 128;
-  * tile-max sampler kernel (``topk_tiles_kernel``) behind the tensor-core lm_head (batch > 4): raw tile maxima, the
-    EOS tile patched through ``fix_tile`` while EOS is masked;
+Sampler paths (both run ``sample_tiles_seq`` and end in ``sample_finish`` in lm_device.cuh):
+  * tile-max sampler kernel (``topk_tiles_kernel``): prefill, ``prefill_slots`` with a ``row_slot`` map and the per-op
+    decode chain, on raw tile maxima -- from the tensor-core lm_head's epilogue where its GEMM tiles the vocabulary by
+    128, from ``tile_max_kernel`` behind the GEMV lm_head (batch <= 4) and narrower GEMM tiles -- with the EOS tile
+    patched through ``fix_tile`` while EOS is masked;
   * the persistent decode kernel's sampler (``sample_phase``): processed tile maxima written by ``epi_head``.
-Inside ``sample_tiles_seq`` (the last two) the *direct*, *fast* and *general* paths are chosen from the tile maxima;
-``tile_path`` restates that choice so that every case can assert which one its rows took.
+Inside ``sample_tiles_seq`` the *direct*, *fast* and *general* paths are chosen from the tile maxima; ``tile_path``
+restates that choice so that every case can assert which one its rows took.
 
 The model is programmable: one layer with wo = 0 and down_proj = 0 leaves the residual stream at exactly
 ``embed[tok]``, and ``embed[t]`` is a one-hot on the pattern that owns ``t mod P``.  Token t's logits are then one
@@ -519,12 +519,6 @@ class Checker:
         assert self.ambiguous <= max(1, BARS["ambiguous"] * self.draws), (self.ambiguous, self.draws)
 
 
-def _tile_sampler(V: int, B: int) -> bool:
-    """The per-op chain's lm_head tiles the vocabulary by 128 (so the tile-max sampler kernel runs) -- gemm_tile_n."""
-    sms = torch.cuda.get_device_properties(0).multi_processor_count
-    return B > 4 and -(-V // 128) >= sms * 13 // 16
-
-
 def _set_impl(monkeypatch, impl):
     if impl:
         monkeypatch.setenv("NT_DECODE_IMPL", impl)
@@ -537,7 +531,7 @@ def _prompts(m, pats):
 
 
 def run_decode_steps(ck: Checker, B: int, steps: int, persistent: bool, tag: str):
-    lm, m = ck.lm, ck.m
+    lm = ck.lm
     for step in range(steps):
         before = ck.snapshot()
         if before["done"][:B].all():
@@ -551,10 +545,7 @@ def run_decode_steps(ck: Checker, B: int, steps: int, persistent: bool, tag: str
         ck.check_handoff(logits, range(B), before["cur"], f"{tag} step {step}")
         ck.check_launch(logits, list(range(B)), [ck.sp.slot_base + b for b in range(B)], before, after, 1,
                         tag=f"{tag} step {step}")
-        if persistent:
-            ck.check_tmax(logits, before["ngen"][:B], True, f"{tag} step {step}")
-        elif _tile_sampler(m.V, B):
-            ck.check_tmax(logits, before["ngen"][:B], False, f"{tag} step {step}")
+        ck.check_tmax(logits, before["ngen"][:B], persistent, f"{tag} step {step}")
 
 
 # (id, vocabulary, batch, NT_DECODE_IMPL, top_k, temperature, greedy, patterns, per-row limits, expected decode paths)
@@ -582,8 +573,7 @@ MIN_NEW = 3
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
 def test_sampler_vs_float64(cuda, case, monkeypatch):
-    """Prefill (radix sampler at batch <= 4, tile-max kernel with the EOS fix_tile beyond) and STEPS single decode
-    steps on the given path.  At every launch: kept ids, kept probabilities, the drawn token, the state update, the
+    """Prefill (tile-max kernel with the EOS fix_tile) and STEPS single decode steps on the given path.  At every launch: kept ids, kept probabilities, the drawn token, the state update, the
     hand-off into the next step and (where readable) the tile maxima."""
     name, V, B, impl, top_k, T, greedy, pats, limits, want_paths = case
     m = programmable(V)
@@ -602,8 +592,7 @@ def test_sampler_vs_float64(cuda, case, monkeypatch):
     ck.check_handoff(logits, range(B), {b: p[-1] for b, p in enumerate(prompts)}, "prefill")
     ck.check_launch(logits, list(range(B)), list(range(B)), before, after, 0, tag="prefill")
     assert after["seq"][:B].tolist() == [len(p) for p in prompts]
-    if _tile_sampler(V, B):
-        ck.check_tmax(logits, [0] * B, False, "prefill")
+    ck.check_tmax(logits, [0] * B, False, "prefill")
     ck.paths.clear()
     _set_impl(monkeypatch, impl)
     persistent = impl == "tc" or (impl is None and B <= 16)
@@ -623,7 +612,7 @@ def test_sampler_vs_float64(cuda, case, monkeypatch):
         assert stopped and all(int(ngen[b]) == MIN_NEW + 1 for b in stopped), (eos_rows, stopped)
 
 
-SLOT_CASES = [   # (id, max_batch, first prefill batch, refilled slots, stream ids): radix (B = 2) / tile kernel (B = 6)
+SLOT_CASES = [   # (id, max_batch, first prefill batch, refilled slots, stream ids): GEMV (B = 2) / GEMM (B = 6) lm_head
     ("radix-b2-into-9", 9, 9, [7, 2], [100, 3]),
     ("tile-b6-into-12", 12, 12, [11, 0, 5, 3, 8, 1], [40, 41, 7, 43, 44, 45]),
 ]
@@ -659,8 +648,7 @@ def test_prefill_slots_sampler_vs_float64(cuda, case, monkeypatch):
         for f in ("ngen", "done", "seq", "cur"):
             assert after[f][s] == before[f][s], (s, f)
         assert (after["out"][s] == before["out"][s]).all(), s
-    if _tile_sampler(V, len(slots)):
-        ck.check_tmax(logits, [0] * len(slots), False, "prefill_slots")
+    ck.check_tmax(logits, [0] * len(slots), False, "prefill_slots")
     key_of = {s: k for s, k in zip(slots, keys)}
     for step in range(2):
         before = ck.snapshot()

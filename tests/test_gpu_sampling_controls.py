@@ -21,7 +21,7 @@ import pytest
 import torch
 
 from tests.helpers import make_lm
-from tests.test_gpu_sampler import (BARS, MIN_NEW, PATTERNS, PATTERNS_ALL, SEED, _prompts, _set_impl, _tile_sampler, draw_u,
+from tests.test_gpu_sampler import (BARS, MIN_NEW, PATTERNS, PATTERNS_ALL, SEED, _prompts, _set_impl, draw_u,
                                     fp32_logits, prob_err, processed_scores, programmable, ref_token, tile_maxima, tile_path)
 from tests.test_sampling_controls import chain64, ref_window_cut
 
@@ -64,7 +64,7 @@ def _windows(m, pat: str, ctl):
     return [ref_window_cut(lg, ngen, m.eos, MIN_NEW, *ctl) for ngen in (0, MIN_NEW)]
 
 
-SLOT_CASES = [   # (id, max_batch, refilled slots, stream ids): radix (B = 2) / tile kernel (B = 6)
+SLOT_CASES = [   # (id, max_batch, refilled slots, stream ids): GEMV (B = 2) / GEMM (B = 6) lm_head
     ("radix-b2-into-9", 9, [7, 2], [100, 3]),
     ("tile-b6-into-12", 12, [11, 0, 5, 3, 8, 1], [40, 41, 7, 43, 44, 45]),
 ]
@@ -203,12 +203,8 @@ def test_identity_and_mixed_controls(cuda, case, monkeypatch):
     persistent = impl is None and B <= 16
     stats = dict(prob=0.0, draws=0, ambiguous=0, cut=0, paths=set())
     for r in recs:
-        tm = None
-        if r["tag"] != "prefill" and persistent:
-            tm = True                                   # 3. processed maxima of the persistent epilogue, per-row T
-        elif _tile_sampler(V, B):
-            tm = False                                  # raw maxima of the chain's lm_head GEMM
-        check_launch(m, r, ctl, stats, tm)
+        # 3. processed maxima of the persistent epilogue (per-row T), else the raw maxima behind the lm_head
+        check_launch(m, r, ctl, stats, r["tag"] != "prefill" and persistent)
     if persistent:
         assert want_paths <= stats["paths"], (want_paths, stats["paths"])
     print(f"CONTROLS {name}: draws {stats['draws']} ambiguous {stats['ambiguous']} cut {stats['cut']} "
@@ -244,8 +240,7 @@ def test_refilled_slots_sample_with_their_own_controls(cuda, case, monkeypatch):
     prompts = [[m.token_for(p, 5), m.token_for(p, 9)] for p in pats]
     lg = lm.prefill_slots(slots, prompts, sp, keys, return_logits=True)
     stats = dict(prob=0.0, draws=0, ambiguous=0, cut=0, paths=set())
-    check_launch(m, _record(lm, cap, lg, before, slots, keys, m.nt, "prefill_slots"), ctl, stats,
-                 False if _tile_sampler(V, len(slots)) else None)
+    check_launch(m, _record(lm, cap, lg, before, slots, keys, m.nt, "prefill_slots"), ctl, stats, False)
     key_of = dict(zip(slots, keys))
     for step in range(2):
         before = _snap(lm)

@@ -19,8 +19,7 @@ import torch
 from neutts_air_b200 import synthetic
 from neutts_air_b200.lm import LMShape, SpeechLM
 from tests.helpers import make_lm
-from tests.test_gpu_sampler import (MIN_NEW, PATTERNS, SEED, Checker, _prompts, _set_impl, _tile_sampler,
-                                    programmable)
+from tests.test_gpu_sampler import MIN_NEW, PATTERNS, SEED, Checker, _prompts, _set_impl, programmable
 
 pytestmark = pytest.mark.gpu
 
@@ -100,8 +99,7 @@ def _run(m, B, impl, top_k, T, pats, rng, monkeypatch):
     before["ngen"][:] = 0
     before["done"][:] = 0
     ck.check_launch(launches[0], list(range(B)), list(range(B)), before, after, 0, tag="prefill")
-    if _tile_sampler(m.V, B):
-        ck.check_tmax(launches[0], [0] * B, False, "prefill")
+    ck.check_tmax(launches[0], [0] * B, False, "prefill")
     ck.paths.clear()
     _set_impl(monkeypatch, impl)
     persistent = impl == "tc" or (impl is None and B <= 16)
@@ -115,10 +113,7 @@ def _run(m, B, impl, top_k, T, pats, rng, monkeypatch):
         assert ((lm.L.nt_launch_count() - n0 - (2 if rng else 0)) == 1) == persistent
         after = ck.snapshot()
         ck.check_launch(lg, list(range(B)), [b for b in range(B)], before, after, 1, tag=f"step {step}")
-        if persistent:
-            ck.check_tmax(lg, before["ngen"][:B], True, f"step {step}")
-        elif _tile_sampler(m.V, B):
-            ck.check_tmax(lg, before["ngen"][:B], False, f"step {step}")
+        ck.check_tmax(lg, before["ngen"][:B], persistent, f"step {step}")
         launches.append(lg)
         curs.append(lm.cur_token[:B].cpu().numpy().copy())
     ck.report("vocab-range" if rng else "range-off")
@@ -289,12 +284,7 @@ def test_vocab_range_with_slot_controls(cuda, case, monkeypatch):
     stats = dict(prob=0.0, draws=0, ambiguous=0, cut=0, paths=set())
     for r in recs:
         assert np.isneginf(r["logits"][:, ~allowed]).all(), (name, r["tag"])
-        tm = None
-        if r["tag"] != "prefill" and persistent:
-            tm = True
-        elif _tile_sampler(V, B):
-            tm = False
-        check_launch(m, r, ctl, stats, tm)
+        check_launch(m, r, ctl, stats, r["tag"] != "prefill" and persistent)
         assert allowed[r["tt"]].all(), (name, r["tag"], r["tt"])
     print(f"CONTROLS+RANGE {name}: draws {stats['draws']} ambiguous {stats['ambiguous']} cut {stats['cut']} "
           f"worst prob err {stats['prob']:.2e} (margin bar {MARGIN}) paths {sorted(stats['paths'])}")
@@ -304,7 +294,7 @@ def test_vocab_range_with_slot_controls(cuda, case, monkeypatch):
 
 
 # ------------------------------------------------------------------------------------ prefill into chosen slots
-SLOT_CASES = [   # (id, max_batch, first prefill batch, refilled slots, stream ids): radix (B = 2) / tile kernel (B = 6)
+SLOT_CASES = [   # (id, max_batch, first prefill batch, refilled slots, stream ids): GEMV (B = 2) / GEMM (B = 6) lm_head
     ("radix-b2-into-9", 9, 9, [7, 2], [100, 3]),
     ("tile-b6-into-12", 12, 12, [11, 0, 5, 3, 8, 1], [40, 41, 7, 43, 44, 45]),
 ]
@@ -340,8 +330,7 @@ def test_vocab_range_prefill_slots(cuda, case, monkeypatch):
         for s in slots:
             before["ngen"][s], before["done"][s] = 0, 0
         ck.check_launch(logits, slots, keys, before, after, 0, tag=f"prefill_slots {rng}")
-        if _tile_sampler(V, len(slots)):
-            ck.check_tmax(logits, [0] * len(slots), False, f"prefill_slots {rng}")
+        ck.check_tmax(logits, [0] * len(slots), False, f"prefill_slots {rng}")
         got[rng is not None] = logits
         if rng:
             assert allowed[[int(after["out"][s, 0]) for s in slots]].all()
