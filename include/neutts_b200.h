@@ -161,6 +161,19 @@ int nt_lm_prefill_slots(nt_lm* lm, const nt_lm_state* st, const int32_t* slots_h
                         const int32_t* ids, const int32_t* cu_seqlens_host, int B, const nt_sampling* sp,
                         float* logits_out, void* stream);
 
+/* n takes of each of B prompts from one prefill (transformers' num_return_sequences).  A full prefill like
+ * nt_lm_prefill: it resets every slot.  Take j of prompt i lives in slot i*n + j (repeat_interleave order);
+ * 1 <= B*n <= max_batch.  The prompts are prefilled once, into the page-table rows of the parent slots i*n, so
+ * logits_out (optional, [B][vocab]) is bit-identical to nt_lm_prefill on the same B prompts.  Page sharing: the
+ * caller writes every take's page-table row before the call, naming the parent's pages for the P_i / 64 full prompt
+ * pages and the take's own pages from page P_i / 64 on; the call copies rows [0, P_i % 64) of the parent's page
+ * P_i / 64 into each other take's page P_i / 64 (every layer, K and V).  Afterwards every take has seq_lens = P_i,
+ * n_generated = done = 0, Philox stream i*n + j + slot_base, and a copy of its parent's repetition-penalty history;
+ * its first token is drawn from the parent's logits row.  Decoding never writes a shared page: every decode path
+ * writes K/V only at position seq_lens[s] of slot s, which lies in the take's own pages. */
+int nt_lm_prefill_fork(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu_seqlens_host, int B, int n,
+                       const nt_sampling* sp, float* logits_out, void* stream);
+
 /* Run n_steps decode steps for slots 0..B-1 with no host synchronisation in between
  * (finished slots keep their state; their work is skipped on device).
  * logits_out: optional device f32 [n_steps][B][vocab] (tests only; forces logits to HBM). */

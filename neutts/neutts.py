@@ -58,6 +58,17 @@ def _backbone_kw(ctl: dict) -> dict:
     return kw
 
 
+def best_takes(logprobs, n: int) -> list:
+    """Index of the kept take of every prompt, given its n takes' log-probability rows in slot order (take j of prompt i
+    at index i * n + j, rows [n_generated, 2] of (sampled, model)): the take with the highest mean ``model``
+    log-probability over its generated tokens, EOS included; ties go to the lowest take index."""
+    keep = []
+    for i in range(len(logprobs) // n):
+        means = [float(np.mean(np.asarray(logprobs[i * n + j], dtype=np.float64)[:, 1])) for j in range(n)]
+        keep.append(i * n + max(range(n), key=lambda j: (means[j], -j)))
+    return keep
+
+
 class _CrossFade:
     """Incremental equivalent of the reference's ``_linear_overlap_add`` (``neutts/neutts.py:46-70``):
     triangular weights over every chunk, weighted sum / weight sum, but only the samples a new chunk
@@ -217,12 +228,27 @@ class NeuTTS:
         if not hasattr(self.backbone, "set_logprobs"):
             raise ValueError("return_logprobs needs a backbone with set_logprobs (neutts_air_b200.SpeechLM)")
 
+    def _check_takes(self, takes, distributed: bool = False) -> int:
+        """``takes`` per utterance: an integer in 1..max_batch; more than one needs a single process and an engine that
+        writes log-probabilities (the best take is chosen by them) and forks a prefill (``generate_batch``'s
+        ``num_return_sequences``)."""
+        if isinstance(takes, bool) or not isinstance(takes, (int, np.integer)) or not 1 <= takes <= self.max_batch:
+            raise ValueError(f"takes {takes!r} must be an integer in 1..max_batch ({self.max_batch})")
+        if takes > 1:
+            if distributed:
+                raise ValueError("takes > 1 is not supported with distributed=True")
+            if not hasattr(self.backbone, "set_logprobs"):
+                raise ValueError("takes > 1 needs a backbone with set_logprobs (neutts_air_b200.SpeechLM)")
+        return int(takes)
+
     def _generate_ids(self, prompts: Sequence[Sequence[int]], max_new_tokens: int | None = None,
-                      min_new_tokens: int = 50, slot_base: int = 0, ctl: dict | None = None, logprobs: bool = False):
+                      min_new_tokens: int = 50, slot_base: int = 0, ctl: dict | None = None, logprobs: bool = False,
+                      takes: int = 1):
         """Batched device-side generation; returns generated token ids per prompt (CPU int64 tensors), or with
         ``logprobs`` (ids, per-prompt float32 CPU tensors [n, 2] of (sampled, model) log-probabilities).
         Sampling parameters default to the reference's (``neutts/neutts.py:338-347``); ``ctl`` (see ``_controls``)
-        overrides them, per prompt where a control is a list."""
+        overrides them, per prompt where a control is a list.  ``takes`` > 1: that many takes of every prompt from
+        one prefill (len(prompts) * takes <= max_batch), of which the one ``best_takes`` picks is returned."""
         eos = self._tok_id("<|SPEECH_GENERATION_END|>")
         seed = self.seed if self.seed is not None else int(torch.randint(0, 2**31 - 1, (1,)).item())
         kw = _backbone_kw(ctl if ctl is not None else CONTROL_DEFAULTS)
@@ -232,6 +258,14 @@ class NeuTTS:
         rng = self._speech_range()
         if rng is not None:
             kw["vocab_range"] = rng
+        if takes > 1:
+            kw["return_logprobs"] = True
+            ids, lps = self.backbone.generate_batch(list(prompts), eos, max_length=self.max_context, min_new_tokens=min_new_tokens,
+                                                    max_new_tokens=max_new_tokens, seed=seed, slot_base=slot_base,
+                                                    num_return_sequences=takes, **kw)
+            keep = best_takes(lps, takes)
+            ids, lps = [ids[k] for k in keep], [lps[k] for k in keep]
+            return (ids, lps) if logprobs else ids
         if len(prompts) > self.max_batch and hasattr(self.backbone, "generate_queue"):
             # more prompts than slots: refill each slot as soon as its utterance ends (prompt i keeps the Philox
             # stream slot_base + i that the chunked loop gives it)
@@ -320,23 +354,30 @@ class NeuTTS:
     # ------------------------------------------------------------------ public API
     def infer(self, text: str, ref_codes, ref_text: str, *, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0,
               min_p: float = 0.0, repetition_penalty: float = 1.0, penalize_prompt: bool = True,
-              return_logprobs: bool = False):
+              return_logprobs: bool = False, takes: int = 1):
         """Text + reference voice -> 24 kHz float32 waveform (``neutts/neutts.py:216-243``).  The sampling controls
-        default to the reference's values; see ``infer_batch``.  ``return_logprobs``: returns (waveform, log-probs)."""
+        default to the reference's values; see ``infer_batch``.  ``return_logprobs``: returns (waveform, log-probs).
+        ``takes``: generate that many takes and keep the most probable one (``infer_batch``)."""
         out = self.infer_batch([text], [ref_codes], [ref_text], temperature=temperature, top_k=top_k, top_p=top_p,
                                min_p=min_p, repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt,
-                               return_logprobs=return_logprobs)
+                               return_logprobs=return_logprobs, takes=takes)
         return (out[0][0], out[1][0]) if return_logprobs else out[0]
 
     def infer_from_prompt_ids(self, prompts: Sequence[Sequence[int]], max_new_tokens: int | None = None,
                               min_new_tokens: int = 50, slot_base: int = 0, *, temperature=1.0, top_k=50, top_p=1.0,
-                              min_p=0.0, repetition_penalty=1.0, penalize_prompt=True, return_logprobs: bool = False):
+                              min_p=0.0, repetition_penalty=1.0, penalize_prompt=True, return_logprobs: bool = False,
+                              takes: int = 1):
         """Hot path only: prompt ids (host) -> waveforms (host).  Used by bench.py's end-to-end leg.
         ``slot_base`` offsets the sampler's Philox slot index so chunks / ranks under one seed draw independently.
         More prompts than ``max_batch`` go through the backbone's ``generate_queue`` when it has one.  Sampling
-        controls and ``return_logprobs`` as in ``infer_batch``."""
+        controls, ``return_logprobs`` and ``takes`` as in ``infer_batch`` (here len(prompts) * takes <= max_batch,
+        and ``slot_base`` counts takes)."""
         ctl = _controls(len(prompts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)
-        gen = self._generate_ids(prompts, max_new_tokens, min_new_tokens, slot_base, ctl, logprobs=return_logprobs)
+        takes = self._check_takes(takes)
+        if takes > 1 and return_logprobs:
+            self._check_logprobs()
+        gen = self._generate_ids(prompts, max_new_tokens, min_new_tokens, slot_base, ctl, logprobs=return_logprobs,
+                                 takes=takes)
         if return_logprobs:
             gen, lps = gen
         wavs = [self._watermark(w) for w in self._decode_codes([self._ids_to_codes(g) for g in gen])]
@@ -344,7 +385,7 @@ class NeuTTS:
 
     def infer_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], distributed: bool = False, *,
                     temperature=1.0, top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0, penalize_prompt=True,
-                    return_logprobs: bool = False):
+                    return_logprobs: bool = False, takes: int = 1):
         """List in / list out.  With ``distributed=True`` (inside an initialised torch.distributed job) the
         utterances are sharded over ranks and every rank returns all waveforms (one all-gather).
 
@@ -368,13 +409,22 @@ class NeuTTS:
         frames: a non-speech id the codec never sees keeps its row.  ``sampled`` is the token's log-probability in the
         distribution it was drawn from (after every control above), ``model`` its log-softmax over the whole
         vocabulary after the repetition penalty and before temperature and the warpers; their mean or minimum over an
-        utterance flags a bad take, or picks the best of several.  Streaming does not return them."""
+        utterance flags a bad take, or picks the best of several.  Streaming does not return them.
+
+        ``takes`` > 1 (at most ``max_batch``; not with ``distributed``; needs a ``SpeechLM`` backbone): every utterance
+        is generated ``takes`` times from one prefill of its prompt (``generate_batch``'s ``num_return_sequences``:
+        the takes share the prompt's KV pages), and only the take with the highest mean ``model`` log-probability over
+        its generated tokens (EOS included; ties: the first take) goes through the codec.  Utterances run in chunks of
+        ``max_batch // takes``; ``return_logprobs`` returns the kept takes' rows."""
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
         ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)
+        takes = self._check_takes(takes, distributed)
         if return_logprobs:
             self._check_logprobs(distributed)
         prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(texts, ref_codes, ref_texts)]
+        if takes > 1:
+            return self._infer_takes(prompts, ctl, takes, return_logprobs)
         queue = hasattr(self.backbone, "generate_queue")
 
         def run(idx, slot_base):
@@ -402,13 +452,37 @@ class NeuTTS:
             local += run(mine[j: j + self.max_batch], (rank << 20) + j)
         return dist.all_gather_waveforms(local, mine, len(prompts), device=self.codec.device)
 
+    @staticmethod
+    def take_chunks(n_utterances: int, takes: int, max_batch: int) -> list:
+        """(utterance indices, slot_base) of every chunk ``infer_batch`` runs with ``takes`` > 1: ``max_batch // takes``
+        utterances per chunk, slot_base = the chunk's first utterance x takes, so that take j of utterance u draws from
+        the Philox stream u * takes + j under one seed whatever the chunking."""
+        per = max_batch // takes
+        return [(range(j, min(j + per, n_utterances)), j * takes) for j in range(0, n_utterances, per)]
+
+    def _infer_takes(self, prompts, ctl: dict, takes: int, return_logprobs: bool):
+        out, lps = [], []
+        for idx, slot_base in self.take_chunks(len(prompts), takes, self.max_batch):
+            r = self.infer_from_prompt_ids([prompts[i] for i in idx], slot_base=slot_base, return_logprobs=return_logprobs,
+                                           takes=takes, **_pick(ctl, idx))
+            out += r[0] if return_logprobs else r
+            lps += r[1] if return_logprobs else []
+        return (out, lps) if return_logprobs else out
+
+    @staticmethod
+    def _no_takes(takes) -> None:
+        if takes != 1:
+            raise ValueError("streaming synthesis generates one take per utterance (takes=1)")
+
     def infer_stream(self, text: str, ref_codes, ref_text: str, *, temperature: float = 1.0, top_k: int = 50,
                      top_p: float = 1.0, min_p: float = 0.0, repetition_penalty: float = 1.0,
-                     penalize_prompt: bool = True) -> Generator[np.ndarray, None, None]:
+                     penalize_prompt: bool = True, takes: int = 1) -> Generator[np.ndarray, None, None]:
         """Streaming synthesis with the reference's window geometry (``neutts/neutts.py:373-465``):
         every 25 new frames (once 5 look-ahead frames exist) the codec re-decodes
         [n - 50 - 1, n + 25 + 5 + 1) and the chunk is cross-faded with triangular weights.  Sampling controls as in
-        ``infer_batch``; streaming returns no per-token log-probabilities (``return_logprobs`` is not supported here)."""
+        ``infer_batch``; streaming returns no per-token log-probabilities (``return_logprobs`` is not supported here)
+        and generates one take per utterance (``takes`` other than 1 raises ValueError)."""
+        self._no_takes(takes)
         if self._is_quantized_model:  # kept for signature parity; never true on this build
             raise NotImplementedError("GGUF streaming is not part of the H100 build")
         ctl = _controls(1, temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)
@@ -417,13 +491,15 @@ class NeuTTS:
 
     def infer_stream_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], *, temperature=1.0,
                            top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0,
-                           penalize_prompt=True) -> Generator[list, None, None]:
+                           penalize_prompt=True, takes: int = 1) -> Generator[list, None, None]:
         """Streaming synthesis of up to ``max_batch`` utterances at once (BASELINE.json configs[4]; the reference
         streams one utterance, ``neutts/neutts.py:373-465``).  Every yield is a list with one entry per utterance:
         the next audio chunk (float32, cross-faded exactly as in ``infer_stream``) or ``None`` when that utterance
         has nothing new.  The sequences decode in lock-step in ONE persistent-kernel launch per round; the windows
         that are due are gathered on the device from the code history and go through the codec as one batch.  Streaming
-        returns no per-token log-probabilities (``infer_batch``'s ``return_logprobs``)."""
+        returns no per-token log-probabilities (``infer_batch``'s ``return_logprobs``) and generates one take per
+        utterance (``takes`` other than 1 raises ValueError)."""
+        self._no_takes(takes)
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
         ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)

@@ -130,6 +130,9 @@ struct nt_lm {
   int* slot_key = nullptr;            // [max_batch] Philox stream key per slot, -1: slot + slot_base
   int* slot_args = nullptr;           // [3][max_batch] slots, stream keys, prompt lengths of the last call
   int* slot_table = nullptr;          // [max_batch][max_pages] the listed slots' page-table rows, in call order
+  // several takes of one prompt (nt_lm_prefill_fork): [max_batch] logits row of every sample row, then
+  // [3][children] parent slot, child slot, prompt length of every child
+  int* fork_args = nullptr;
   // per-slot sampling controls (nt_lm_set_slot_sampling): copied into every SamplerParams while step.slot_sp_on
   nt_slot_sampling* slot_sp = nullptr;  // [max_batch]
   // repetition penalty (nt_lm_set_repetition_penalty): history bitmaps, the per-slot table and "recorded" flags
@@ -221,6 +224,7 @@ static size_t lm_carve(const nt_lm_config& c, void* ws, size_t bytes, F&& assign
     (L)->slot_key = a.take<int>(c.max_batch);                                                  \
     (L)->slot_args = a.take<int>(size_t(3) * c.max_batch);                                     \
     (L)->slot_table = a.take<int>(size_t(c.max_batch) * max_splits);                           \
+    (L)->fork_args = a.take<int>(size_t(4) * c.max_batch);                                     \
     (L)->slot_sp = a.take<nt_slot_sampling>(c.max_batch);                                     \
     (L)->rep_words = (V + 31) / 32;                                                            \
     (L)->rep_hist = a.take<uint32_t>(size_t(c.max_batch) * ((V + 31) / 32));                   \
@@ -661,6 +665,54 @@ extern "C" int nt_lm_prefill_slots(nt_lm* lm, const nt_lm_state* st, const int32
   s.h = nullptr;  // the residual rows are rebuilt below, for every slot
   if ((rc = run_sampler(lm, s, B, stream))) return rc;
   return launch_embed_rows(lm->embed, st->cur_token, c.max_batch, c.hidden, lm->h, stream);
+}
+
+// n takes of each of B prompts: take j of prompt i lives in slot i * n + j, and slot i * n is its prompt's parent.  The
+// prefill chain runs once over the B prompts on the parents' page-table rows (gathered into a compact table as in
+// nt_lm_prefill_slots); its KV and logits are those of nt_lm_prefill on the same prompts.  A child's page-table row
+// already names the parent's full prompt pages (the caller shares them), so only the partly filled last prompt page
+// is copied into the child's own page, together with the parent's repetition-penalty history.  The sampler then
+// draws every take from its parent's logits row (row_src), with the take's own slot state and Philox stream.
+extern "C" int nt_lm_prefill_fork(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, int B, int n,
+                                  const nt_sampling* sp, float* logits_out, void* stream_) {
+  if (!lm || !st || !ids || !cu) return set_error(NT_ERR_INVALID, "nt_lm_prefill_fork: null argument");
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  const nt_lm_config& c = lm->cfg;
+  if (B < 1 || n < 1 || static_cast<long long>(B) * n > c.max_batch)
+    return set_error(NT_ERR_INVALID, "%d prompts x %d takes not in 1..%d slots", B, n, c.max_batch);
+  int rc = check_sampling(lm, st, sp);
+  if (rc) return rc;
+  const int N = B * n, nc = N - B;
+  std::vector<int> lens;
+  int max_len = 0;
+  if ((rc = prefill_stage(lm, cu, B, lens, max_len, stream))) return rc;
+  std::vector<int> args(size_t(3) * B), fork(size_t(N) + size_t(3) * nc), seq(N);
+  for (int i = 0; i < B; ++i) args[i] = i * n, args[B + i] = -1, args[2 * B + i] = lens[i];
+  for (int r = 0, k = 0; r < N; ++r) {
+    const int i = r / n;
+    fork[r] = i, seq[r] = lens[i];
+    if (r % n) fork[N + k] = i * n, fork[N + nc + k] = r, fork[N + 2 * nc + k] = lens[i], ++k;
+  }
+  NT_CUDA_CHECK(cudaMemcpyAsync(lm->slot_args, args.data(), args.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
+  NT_CUDA_CHECK(cudaMemcpyAsync(lm->fork_args, fork.data(), fork.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
+  // every slot: slot + slot_base, no token yet; the takes start at their prompt's length
+  NT_CUDA_CHECK(cudaMemsetAsync(lm->slot_key, 0xff, size_t(c.max_batch) * sizeof(int), stream));
+  NT_CUDA_CHECK(cudaMemsetAsync(st->n_generated, 0, size_t(c.max_batch) * sizeof(int), stream));
+  NT_CUDA_CHECK(cudaMemsetAsync(st->done, 0, size_t(c.max_batch) * sizeof(int), stream));
+  NT_CUDA_CHECK(cudaMemcpyAsync(st->seq_lens, seq.data(), N * sizeof(int), cudaMemcpyHostToDevice, stream));
+  const int max_pages = c.max_ctx / c.page_size;
+  if ((rc = launch_slots_setup(lm->slot_args, B, st->page_table, max_pages, lm->slot_table, st->seq_lens, st->n_generated, st->done,
+                               lm->slot_key, stream)))
+    return rc;
+  if ((rc = prefill_forward(lm, st, ids, cu, B, max_len, lm->slot_table, logits_out, sp->eos_id, stream, lm->slot_args))) return rc;
+  if ((rc = launch_fork_tails(lm->fork_args + N, nc, make_kv(lm, st), c.n_layers, lm->step.rep_on ? lm->rep_hist : nullptr,
+                              lm->rep_words, lm->rep_rec, stream)))
+    return rc;
+  SamplerParams s = make_sampler(lm, st, sp);
+  s.row_src = n > 1 ? lm->fork_args : nullptr;
+  if ((rc = run_sampler(lm, s, N, stream))) return rc;
+  lm->prefilled = true;
+  return NT_OK;
 }
 
 // one decode step for slots 0..B-1 (all launches asynchronous, PDL-chained)

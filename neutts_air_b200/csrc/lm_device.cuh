@@ -311,17 +311,18 @@ NT_DEVINL float row_logsumexp(const float* lg, int V, int eos, bool mask_eos, fl
 // token's embedding -> residual stream row (fp32; optionally also as (value, stamp) pairs for the polled hand-off).
 // With p.logprob_out, the written token's (sampled, model) log-probabilities go next to it (DESIGN.md §4, per-token
 // log-probabilities); the model one takes one extra pass over logits row b.
-// Clobbers win[kTopKeep .. 2 kTopKeep) (exponentials).  b: logits row; slot >= 0: the slot whose state row b updates
-// (prefill into chosen slots), else slot b.
+// Clobbers win[kTopKeep .. 2 kTopKeep) (exponentials).  b: sample row; slot >= 0: the slot whose state row b updates
+// (prefill into chosen slots), else slot b; src >= 0: the logits row sample row b reads (several takes of one
+// prompt), else row b.
 template <typename Sync>
 NT_DEVINL void sample_finish(const SamplerParams& p, int b, int k, Cand* win, int* s_tok, bool stateless, int ngen, bool is_done, Sync sync,
-                             float2* h2dst = nullptr, float h2stamp = 0.f, int slot = -1) {
+                             float2* h2dst = nullptr, float h2stamp = 0.f, int slot = -1, int src = -1) {
   const int tid = threadIdx.x;
   const int s = slot >= 0 ? slot : b;
   float* ev = reinterpret_cast<float*>(win + kTopKeep);   // [kTopKeep] exp(score - max)
   const bool logprobs = p.logprob_out && !stateless && !is_done;   // CTA-uniform
   const bool mask_eos = ngen < p.sp.min_new_tokens;
-  const float* lg = p.logits + static_cast<long long>(b) * p.V;
+  const float* lg = p.logits + static_cast<long long>(src >= 0 ? src : b) * p.V;
   float lse = 0.f;
   if (logprobs) lse = row_logsumexp(lg, p.V, p.sp.eos_id, mask_eos, reinterpret_cast<float2*>(ev + kTopKeep), sync);
   if (tid < 32) {
@@ -436,7 +437,7 @@ NT_DEVINL void sample_finish(const SamplerParams& p, int b, int k, Cand* win, in
 // set: a run-time test here, where a caller's compile-time flag shifts ptxas's spills in the persistent kernel.
 template <typename Sync>
 NT_DEVINL void sample_stage2_seq(const SamplerParams& p, int b, int ncand, uint32_t* keys, uint32_t* scratch, Cand* win, int* s_tok,
-                                 Sync sync, int slot = -1) {
+                                 Sync sync, int slot = -1, int src = -1) {
   const int tid = threadIdx.x;
   const bool stateless = p.n_generated_override != nullptr;
   const int s = slot >= 0 ? slot : b;
@@ -480,7 +481,7 @@ NT_DEVINL void sample_stage2_seq(const SamplerParams& p, int b, int ncand, uint3
     win[rank] = me;
   }
   sync();
-  sample_finish(p, b, k, win, s_tok, stateless, ngen, is_done, sync, nullptr, 0.f, slot);
+  sample_finish(p, b, k, win, s_tok, stateless, ngen, is_done, sync, nullptr, 0.f, slot, src);
 }
 
 // Sampler of the tile-max schemes, for sequence b, on 256 threads (0..255) of one CTA.  The lm_head epilogue left the
@@ -494,10 +495,11 @@ NT_DEVINL void sample_stage2_seq(const SamplerParams& p, int b, int ncand, uint3
 //   fix_val instead (the tile holding a masked EOS, when the maxima were taken on raw logits).
 //   uni / uni_bytes: >= 16 KB of shared scratch (1024-byte aligned); sel: >= 4 ints of shared memory.
 //   stateless (nt_op_topk_sample): n_generated_override[b] is the row's count, the row is live and no state is written.
+//   src >= 0: the logits and tile-maxima row sample row b reads (see sample_finish), else row b.
 template <typename Sync, typename Mark>
 NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax, int nt, float tmax_scale, int fix_tile, float fix_val,
                                 const float* logits, int V, bool mask_eos, uint8_t* uni, unsigned uni_bytes, int* sel, Sync sync, Mark pm,
-                                float2* h2dst, float h2stamp, bool stateless, int slot = -1) {
+                                float2* h2dst, float h2stamp, bool stateless, int slot = -1, int src = -1) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int H = p.hidden;
   uint32_t* scratch = reinterpret_cast<uint32_t*>(uni);
@@ -513,11 +515,12 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
   const int eos = p.sp.eos_id;
   const int ngen = stateless ? __ldcg(p.n_generated_override + b) : __ldcg(p.n_generated + (slot >= 0 ? slot : b));
   const bool is_done = stateless ? false : __ldcg(p.done + (slot >= 0 ? slot : b)) != 0;
-  const float* lg = logits + static_cast<long long>(b) * V;
-  // row b starts b * V floats in: with V % 4 != 0 only some rows are 16-byte aligned for the float4 loads (CTA-uniform)
+  const int src_row = src >= 0 ? src : b;
+  const float* lg = logits + static_cast<long long>(src_row) * V;
+  // the row starts src_row * V floats in: with V % 4 != 0 only some rows are 16-byte aligned for the float4 loads (CTA-uniform)
   const bool vec4 = (reinterpret_cast<uintptr_t>(lg) & 15) == 0;
   auto tile_max = [&](int i) -> float {
-    const float v = __ldcg(tmax + static_cast<long long>(b) * nt + i) * tmax_scale;
+    const float v = __ldcg(tmax + static_cast<long long>(src_row) * nt + i) * tmax_scale;
     return i == fix_tile ? fix_val : v;
   };
   pm(120);
@@ -631,7 +634,7 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
             }
             sync();
             pm(124);
-            sample_finish(p, b, k2, win, s_tok, stateless, ngen, is_done, sync, h2dst, h2stamp, slot);
+            sample_finish(p, b, k2, win, s_tok, stateless, ngen, is_done, sync, h2dst, h2stamp, slot, src);
             pm(125);
             return;
           }
@@ -715,7 +718,7 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
       if (rank < k2) win[rank] = me;
     }
     sync();
-    sample_finish(p, b, k2, win, s_tok, stateless, ngen, is_done, sync, h2dst, h2stamp, slot);
+    sample_finish(p, b, k2, win, s_tok, stateless, ngen, is_done, sync, h2dst, h2stamp, slot, src);
     return;
   }
   // ---- general path (thousands of candidates: tiny vocabularies, or exact ties at the threshold)
@@ -790,7 +793,7 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
     }
   }
   sync();
-  sample_stage2_seq(p, b, ncand, keys, scratch, win, s_tok, sync, slot);
+  sample_stage2_seq(p, b, ncand, keys, scratch, win, s_tok, sync, slot, src);
   if (h2dst) {  // the next token's embedding becomes the residual stream of the next step's first fold
     sync();
     for (int i = tid; i < H; i += kConsumerThreads) h2dst[i] = make_float2(p.h[static_cast<long long>(b) * H + i], h2stamp);

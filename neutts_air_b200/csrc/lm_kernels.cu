@@ -800,6 +800,7 @@ __global__ void __launch_bounds__(kConsumerThreads) topk_tiles_kernel(const Samp
   pdl_wait();
   const int b = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int slot = p.row_slot ? __ldg(p.row_slot + b) : b;
+  const int src = p.row_src ? __ldg(p.row_src + b) : -1;   // logits / tile-maxima row (-1: row b)
   const bool stateless = p.n_generated_override != nullptr;
   const int ngen = stateless ? __ldcg(p.n_generated_override + b) : __ldcg(p.n_generated + slot);
   const bool mask_eos = ngen < p.sp.min_new_tokens;
@@ -812,7 +813,7 @@ __global__ void __launch_bounds__(kConsumerThreads) topk_tiles_kernel(const Samp
       float m = -INFINITY;
       for (int q = 0; q < 4; ++q) {
         const int r = fix_tile * 128 + lane * 4 + q;
-        if (r < p.V && r != p.sp.eos_id) m = fmaxf(m, __ldcg(p.logits + static_cast<long long>(b) * p.V + r));
+        if (r < p.V && r != p.sp.eos_id) m = fmaxf(m, __ldcg(p.logits + static_cast<long long>(src >= 0 ? src : b) * p.V + r));
       }
       m = warp_max(m);
       if (lane == 0) fix = m * inv_t;
@@ -821,7 +822,7 @@ __global__ void __launch_bounds__(kConsumerThreads) topk_tiles_kernel(const Samp
     fix_val = fix;
   }
   sample_tiles_seq(p, b, tmax, nt, inv_t, fix_tile, fix_val, p.logits, p.V, mask_eos, uni, kTilesScratch, sel, SyncAll(), NoMarkI(),
-                   static_cast<float2*>(nullptr), 0.f, stateless, slot);
+                   static_cast<float2*>(nullptr), 0.f, stateless, slot, src);
 }
 
 int launch_sampler_tiles(const SamplerParams& p, int B, const float* tmax, int nt, cudaStream_t stream) {
@@ -1275,6 +1276,40 @@ int launch_slots_setup(const int32_t* args, int B, const int32_t* page_table, in
                        int32_t* n_generated, int32_t* done, int32_t* slot_key, cudaStream_t s) {
   return launch_kernel(slots_setup_kernel, dim3(B), dim3(128), 0, s, true, args, B, page_table, max_pages, table, seq_lens, n_generated,
                        done, slot_key);
+}
+
+// grid (children, n_layers * 2 * n_kv [+ 1 with hist]), 128 threads.  CTA (c, y < n_layers * 2 * n_kv) copies the first
+// P % 64 rows (128 B each, 8 x 16 B) of one (layer, K|V, kv head) block of child c's last prompt page; CTA (c, last y)
+// copies the history row and the recorded flag.
+__global__ void __launch_bounds__(128) fork_tails_kernel(const int32_t* args, int nc, const KVLayout kv, int n_units, uint32_t* hist,
+                                                         int words, int32_t* recorded) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int c = blockIdx.x, y = blockIdx.y;
+  const int parent = args[c], child = args[nc + c], P = args[2 * nc + c];
+  if (y < n_units) {
+    const int rows = P & 63;
+    if (rows == 0) return;   // the prompt ends on a page boundary: every prompt page is full and shared
+    const int pg = P >> 6;
+    const int src = kv.page_table[static_cast<long long>(parent) * kv.max_pages_per_seq + pg];
+    const int dst = kv.page_table[static_cast<long long>(child) * kv.max_pages_per_seq + pg];
+    const int kvh = y % kv.n_kv_heads, is_v = (y / kv.n_kv_heads) & 1, layer = y / (2 * kv.n_kv_heads);
+    const uint4* s = reinterpret_cast<const uint4*>(kv.page_ptr(layer, is_v, src, kvh));
+    uint4* d = reinterpret_cast<uint4*>(kv.page_ptr(layer, is_v, dst, kvh));
+    for (int i = threadIdx.x; i < rows * 8; i += blockDim.x) d[i] = s[i];
+    return;
+  }
+  const uint32_t* hs = hist + static_cast<long long>(parent) * words;
+  uint32_t* hd = hist + static_cast<long long>(child) * words;
+  for (int w = threadIdx.x; w < words; w += blockDim.x) hd[w] = hs[w];
+  if (threadIdx.x == 0) recorded[child] = recorded[parent];
+}
+int launch_fork_tails(const int32_t* args, int nc, const KVLayout& kv, int n_layers, uint32_t* hist, int words, int32_t* recorded,
+                      cudaStream_t s) {
+  if (nc <= 0) return NT_OK;
+  const int n_units = n_layers * 2 * kv.n_kv_heads;
+  return launch_kernel(fork_tails_kernel, dim3(nc, n_units + (hist ? 1 : 0)), dim3(128), 0, s, true, args, nc, kv, n_units, hist, words,
+                       recorded);
 }
 
 }  // namespace nt

@@ -92,6 +92,10 @@ struct SamplerParams {
   // Prefill into chosen slots: logits row i updates the state of slot row_slot[i] (nullptr: row i is slot i).  Read
   // by the stand-alone sampler kernels only; the persistent decode kernel samples row b into slot b.
   const int32_t* row_slot;
+  // Several takes of one prompt (nt_lm_prefill_fork): sample row i reads logits row and tile-maxima row row_src[i]
+  // (nullptr: row i).  The capture, the residual row and the candidate scratch stay indexed by sample row i.  Read by
+  // the stand-alone sampler kernels only.
+  const int32_t* row_src;
   const int32_t* slot_key;  // optional [max_batch] Philox stream key per slot; -1: slot + slot_base
   // optional [max_batch] temperature / top_k / top_p / min_p per slot (nt_lm_set_slot_sampling), read through
   // row_sampling() with the row's slot; nullptr: sp.temperature and sp.top_k for every row, no top-p / min-p cut
@@ -153,5 +157,12 @@ int launch_gather_rows(const float* src, const int32_t* rows, int n, int cols, f
 // slots' page-table rows into table [B][max_pages] and resets those slots' seq_lens / n_generated / done / slot_key.
 int launch_slots_setup(const int32_t* args, int B, const int32_t* page_table, int max_pages, int32_t* table, int32_t* seq_lens,
                        int32_t* n_generated, int32_t* done, int32_t* slot_key, cudaStream_t s);
+// Several takes of one prompt.  args: device [3][nc] = parent slot, child slot, prompt length P of each child.  For
+// every child with P % 64 != 0, rows [0, P % 64) of the parent's page P / 64 (its partly filled last prompt page) are
+// copied into the child's page P / 64, in every layer, K and V, every KV head; full prompt pages are shared through
+// the page table and never copied.  hist != nullptr: the child's repetition-penalty history row and recorded flag
+// become copies of the parent's, in the same launch.
+int launch_fork_tails(const int32_t* args, int nc, const KVLayout& kv, int n_layers, uint32_t* hist, int words, int32_t* recorded,
+                      cudaStream_t s);
 
 }  // namespace nt

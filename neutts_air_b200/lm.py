@@ -8,7 +8,9 @@ All arithmetic happens in ``libneutts_b200.so``; torch is used for device memory
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
 import math
+from collections import Counter
 from dataclasses import dataclass
 
 import numpy as np
@@ -90,7 +92,9 @@ def pack_weights(shape: LMShape, sd: dict, device) -> dict:
 
 
 class PagePool:
-    """Free-list allocator over the KV page ids (host side; one id addresses every layer)."""
+    """Free-list allocator over the KV page ids (host side; one id addresses every layer).  Every allocated page has a
+    reference count: several slots may hold one page (the takes of one prompt share its full prompt pages), and a
+    page returns to the free list when its last holder releases it."""
 
     def __init__(self, num_pages: int, shuffle_seed: int | None = None):
         order = list(range(num_pages))
@@ -98,14 +102,42 @@ class PagePool:
             rng = np.random.default_rng(shuffle_seed)
             rng.shuffle(order)
         self.free = order[::-1]
+        self.refs = [0] * num_pages
+
+    @property
+    def num_free(self) -> int:
+        """Pages no slot holds."""
+        return len(self.free)
 
     def alloc(self, n: int) -> list:
         if n > len(self.free):
             raise RuntimeError(f"KV page pool exhausted: need {n}, have {len(self.free)}")
-        return [self.free.pop() for _ in range(n)]
+        pages = [self.free.pop() for _ in range(n)]
+        for p in pages:
+            self.refs[p] = 1
+        return pages
+
+    def _check_held(self, pages, verb: str) -> list:
+        pages = list(pages)
+        for p, k in Counter(pages).items():
+            if not 0 <= p < len(self.refs) or self.refs[p] < k:
+                raise ValueError(f"cannot {verb} page {p}: it is held {self.refs[p] if 0 <= p < len(self.refs) else 0} "
+                                 f"time(s), asked {k}")
+        return pages
+
+    def share(self, pages) -> None:
+        """One more reference to each of ``pages`` (allocated ones only)."""
+        for p in self._check_held(pages, "share"):
+            self.refs[p] += 1
 
     def release(self, pages) -> None:
-        self.free.extend(reversed(list(pages)))
+        """Drops one reference to each of ``pages``; a page whose count reaches zero is free again."""
+        freed = []
+        for p in self._check_held(pages, "release"):
+            self.refs[p] -= 1
+            if self.refs[p] == 0:
+                freed.append(p)
+        self.free.extend(reversed(freed))
 
 
 DEFAULT_CONTROLS = (1.0, 50, 1.0, 0.0)   # temperature, top_k, top_p, min_p: the reference's (neutts/neutts.py:338-347)
@@ -172,6 +204,21 @@ def check_vocab_range(vocab_range, vocab_size: int):
     return lo, hi
 
 
+def check_takes(n_prompts: int, n, max_batch: int) -> int:
+    """Takes per prompt (``num_return_sequences``), validated: an integer >= 1 with n_prompts * n <= max_batch."""
+    if isinstance(n, bool) or not isinstance(n, (int, np.integer)) or n < 1:
+        raise ValueError(f"num_return_sequences {n!r} must be an integer >= 1")
+    if n_prompts * int(n) > max_batch:
+        raise ValueError(f"{n_prompts} prompt(s) x {int(n)} takes need {n_prompts * int(n)} slots; the engine has {max_batch}")
+    return int(n)
+
+
+def fork_slots(n_prompts: int, n: int, slot_base: int = 0) -> list:
+    """(prompt, take, slot, Philox stream key) of every slot ``prefill_fork`` fills: take j of prompt i in slot i * n + j
+    (transformers' repeat_interleave order), drawing from stream slot + slot_base."""
+    return [(i, j, i * n + j, i * n + j + slot_base) for i in range(n_prompts) for j in range(n)]
+
+
 DEFAULT_PENALTY = (1.0, True)   # repetition penalty, prompt included: transformers' RepetitionPenaltyLogitsProcessor
 
 
@@ -224,6 +271,12 @@ class Settings:
             lm.set_repetition_penalty(None if self.penalty is None else self.penalty[:n])
         if self.logprobs != (getattr(lm, "logprobs", None) is not None):
             lm.set_logprobs(self.logprobs)
+
+    def repeat(self, n: int) -> "Settings":
+        """The settings of n takes of every prompt: each prompt's row repeated n times, in slot order (take j of prompt
+        i in slot i * n + j), so that ``apply`` writes it into all of the prompt's take slots."""
+        rows = lambda r: None if r is None else [x for x in r for _ in range(n)]
+        return dataclasses.replace(self, controls=rows(self.controls), penalty=rows(self.penalty))
 
     def admit(self, lm, slots, idx) -> None:
         """Before a refill of prompts ``idx`` into ``slots``: writes their rows; every other slot keeps its own, and
@@ -448,6 +501,24 @@ class SpeechLM:
             table[s] = 0
             table[s, :need] = pages
 
+    def _alloc_fork_pages(self, table, lens, n: int, cap: int) -> None:
+        """KV pages of n takes of every prompt, written into the page table ``table``: take j of prompt i (slot i * n + j)
+        holds the prompt's P // 64 full pages, shared by all n takes, then pages of its own from page P // 64 on (the
+        partly filled last prompt page, if any, and room for ``cap`` generated tokens)."""
+        need = [(min(P + cap, self.max_ctx) + self.PAGE - 1) // self.PAGE for P in lens]
+        total = sum(P // self.PAGE + n * (m - P // self.PAGE) for P, m in zip(lens, need))
+        if total > self.pool.num_free:
+            raise RuntimeError(f"KV page pool exhausted: need {total}, have {self.pool.num_free}")
+        for i, j, s, _ in fork_slots(len(lens), n):
+            if j == 0:
+                shared = self.pool.alloc(lens[i] // self.PAGE)
+            else:
+                self.pool.share(shared)
+            pages = shared + self.pool.alloc(need[i] - len(shared))
+            self._slot_pages[s] = pages
+            table[s] = 0
+            table[s, : need[i]] = pages
+
     def prefill(self, prompts, sp, return_logits: bool = False):
         """prompts: list of 1-D int sequences.  Fills the KV cache and samples the first token."""
         lens = [len(p) for p in prompts]
@@ -485,8 +556,40 @@ class SpeechLM:
         self._B = B
         return logits
 
+    def prefill_fork(self, prompts, n: int, sp, return_logits: bool = False):
+        """n takes of every prompt from one prefill (``nt_lm_prefill_fork``).  Take j of prompt i lives in slot i * n + j
+        and draws from Philox stream i * n + j + slot_base, as in ``prefill`` on the prompts each repeated n times; the
+        prompts are prefilled once, and all n takes read one copy of each full prompt page (``_alloc_fork_pages``).
+        Resets every slot; afterwards ``decode`` continues all len(prompts) * n takes.  Returns the [len(prompts), vocab]
+        last-position logits (identical to ``prefill``'s on the same prompts) when ``return_logits``."""
+        B = len(prompts)
+        n = check_takes(B, n, self.max_batch)
+        lens = [len(p) for p in prompts]
+        if not lens or min(lens) < 1:
+            raise ValueError("empty prompt")
+        if max(lens) >= self.max_ctx:
+            raise ValueError(f"prompt lengths must be in 1..{self.max_ctx - 1}")
+        staged = self._stage_ids(prompts)
+        self.release_pages()
+        table = np.zeros((self.max_batch, self.max_pages), dtype=np.int32)
+        self._alloc_fork_pages(table, lens, n, sp.max_new_tokens)
+        cu = np.zeros(B + 1, dtype=np.int32)
+        cu[1:] = np.cumsum(lens)
+        with torch.cuda.device(self.device):
+            ids = staged.to(self.device, non_blocking=True)
+            if self._table_host is None or not np.array_equal(self._table_host, table):
+                self.page_table.copy_(torch.from_numpy(table))
+                self._table_host = table
+            logits = torch.empty(B, self.shape.vocab_size, dtype=torch.float32, device=self.device) if return_logits else None
+            _lib.check(self.L.nt_lm_prefill_fork(self.handle, C.byref(self.state), ids.data_ptr(),
+                                                 cu.ctypes.data_as(C.POINTER(C.c_int32)), B, n, C.byref(sp),
+                                                 logits.data_ptr() if return_logits else None, _lib.current_stream_ptr()))
+        self._B = B * n
+        return logits
+
     def release_pages(self, slots=None) -> None:
-        """Return the KV pages of ``slots`` (default: every slot) to the pool."""
+        """Return the KV pages of ``slots`` (default: every slot) to the pool.  A page shared with another slot (the
+        full prompt pages of ``prefill_fork``'s takes) stays held until its last holder releases it."""
         for b in range(self.max_batch) if slots is None else slots:
             if self._slot_pages[b]:
                 self.pool.release(self._slot_pages[b])
@@ -621,7 +724,7 @@ class SpeechLM:
                        temperature: float = 1.0, top_k: int = 50, max_new_tokens: int | None = None, seed: int = 0,
                        greedy: bool = False, forced: torch.Tensor | None = None, check_every: int = 64, slot_base: int = 0,
                        top_p: float = 1.0, min_p: float = 0.0, vocab_range=None, repetition_penalty=1.0,
-                       penalize_prompt=True, return_logprobs: bool = False):
+                       penalize_prompt=True, return_logprobs: bool = False, num_return_sequences: int = 1):
         """Returns a list of int64 CPU tensors with the generated ids of each prompt (EOS included
         when it was sampled), following transformers' stopping rules (stopping_criteria.py:73-84,
         467-471): stop at EOS or when prompt + generated reaches max_length.  ``max_new_tokens`` may also be a
@@ -632,17 +735,27 @@ class SpeechLM:
         (``set_repetition_penalty``); they apply to greedy and teacher-forced runs too.  ``return_logprobs``: returns
         ``(ids, logprobs)`` instead, ``logprobs[i]`` a float32 CPU tensor [len(ids[i]), 2] of (sampled, model)
         log-probabilities per generated token (``set_logprobs``, switched on for the call and off by a later call
-        without it)."""
+        without it).  ``num_return_sequences`` n > 1: n takes of every prompt from one prefill (``prefill_fork``;
+        len(prompts) * n <= max_batch), returned in slot order, take j of prompt i at index i * n + j, each drawing
+        from the Philox stream the prompt repeated n times would give it; every per-prompt setting (and cap) applies
+        to all n takes of its prompt, while ``forced`` has one row per take."""
+        n_takes = check_takes(len(prompts), num_return_sequences, self.max_batch)
         caps, settings = self._prepare(prompts, max_length, max_new_tokens, temperature=temperature, top_k=top_k,
                                        top_p=top_p, min_p=min_p, vocab_range=vocab_range,
                                        repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt,
                                        logprobs=return_logprobs)
+        if n_takes > 1:
+            caps = [c for c in caps for _ in range(n_takes)]
+            settings = settings.repeat(n_takes)
         limit = max(caps)
         sp = self.sampling(eos_token_id, min_new_tokens, limit, settings.top_k, settings.temperature, seed, greedy,
                            forced, limits=caps if min(caps) < limit else None, slot_base=slot_base)
-        B = len(prompts)
+        B = len(prompts) * n_takes
         settings.apply(self, B)
-        self.prefill(prompts, sp)
+        if n_takes > 1:
+            self.prefill_fork(prompts, n_takes, sp)
+        else:
+            self.prefill(prompts, sp)
         remaining = limit - 1
         while remaining > 0:
             n = min(check_every, remaining)
@@ -657,7 +770,7 @@ class SpeechLM:
                        temperature: float = 1.0, top_k: int = 50, max_new_tokens: int | None = None, seed: int = 0,
                        greedy: bool = False, check_every: int = 32, slot_base: int = 0, top_p: float = 1.0,
                        min_p: float = 0.0, vocab_range=None, repetition_penalty=1.0, penalize_prompt=True,
-                       return_logprobs: bool = False):
+                       return_logprobs: bool = False, num_return_sequences: int = 1):
         """Continuous batching over any number of prompts: ``generate_batch``'s results and stopping rules, but a slot
         whose sequence finished is refilled with the next waiting prompt while the other slots keep decoding.
 
@@ -673,7 +786,11 @@ class SpeechLM:
         ``generate_batch``: set once before the first prefill, it holds across every refill.  ``repetition_penalty`` and
         ``penalize_prompt`` as in ``generate_batch``; a newcomer's entry is written before its prefill.
         ``return_logprobs`` as in ``generate_batch``: a finished slot's rows are copied out with its tokens, before
-        the refill that reuses the slot."""
+        the refill that reuses the slot.  One sequence per prompt: ``num_return_sequences`` > 1 raises ValueError
+        (``generate_batch`` takes several per prompt)."""
+        if num_return_sequences != 1:
+            raise ValueError("generate_queue returns one sequence per prompt; use generate_batch(num_return_sequences=n) "
+                             "for several takes of each prompt")
         caps, settings = self._prepare(prompts, max_length, max_new_tokens, temperature=temperature, top_k=top_k,
                                        top_p=top_p, min_p=min_p, vocab_range=vocab_range,
                                        repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt,
@@ -733,11 +850,14 @@ class SpeechLM:
     def generate(self, input_ids: torch.Tensor, max_length: int = 2048, eos_token_id: int | None = None,
                  do_sample: bool = True, temperature: float = 1.0, top_k: int = 50, use_cache: bool = True,
                  min_new_tokens: int = 0, max_new_tokens: int | None = None, seed: int | None = None,
-                 top_p: float = 1.0, min_p: float = 0.0, vocab_range=None, repetition_penalty: float = 1.0, **_):
+                 top_p: float = 1.0, min_p: float = 0.0, vocab_range=None, repetition_penalty: float = 1.0,
+                 num_return_sequences: int = 1, **_):
         """transformers-compatible seam used by ``NeuTTS._infer_torch`` (neutts/neutts.py:338-347).  ``top_p`` and
         ``min_p`` act as transformers' TopPLogitsWarper / MinPLogitsWarper; ``vocab_range`` (lo, hi) suppresses every
         id outside [lo, hi) and EOS (``set_vocab_range``); ``repetition_penalty`` acts as transformers'
-        RepetitionPenaltyLogitsProcessor (prompt included); other generation kwargs are ignored."""
+        RepetitionPenaltyLogitsProcessor (prompt included); ``num_return_sequences`` n returns n takes of every prompt
+        from one prefill, [B * n, P + gen] with take j of row b at row b * n + j, as transformers; other generation
+        kwargs are ignored."""
         if eos_token_id is None:
             raise ValueError("eos_token_id is required")
         if input_ids.dim() != 2:
@@ -750,11 +870,14 @@ class SpeechLM:
             cuts["vocab_range"] = vocab_range
         if repetition_penalty is not None and repetition_penalty != 1.0:
             cuts["repetition_penalty"] = repetition_penalty
+        if num_return_sequences != 1:
+            cuts["num_return_sequences"] = num_return_sequences
         outs = self.generate_batch(prompts, eos_token_id, max_length, min_new_tokens, temperature, top_k,
                                    max_new_tokens, seed, greedy=not do_sample, **cuts)
         n = max(len(o) for o in outs)
+        takes = len(outs) // len(prompts)
         res = torch.full((len(outs), input_ids.shape[1] + n), int(eos_token_id), dtype=torch.long)
         for b, o in enumerate(outs):
-            res[b, : input_ids.shape[1]] = input_ids[b].cpu()
+            res[b, : input_ids.shape[1]] = input_ids[b // takes].cpu()
             res[b, input_ids.shape[1]: input_ids.shape[1] + len(o)] = o
         return res.to(input_ids.device)
