@@ -174,6 +174,31 @@ int nt_lm_prefill_slots(nt_lm* lm, const nt_lm_state* st, const int32_t* slots_h
 int nt_lm_prefill_fork(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu_seqlens_host, int B, int n,
                        const nt_sampling* sp, float* logits_out, void* stream);
 
+/* Teacher-forced scoring: per-token log-probabilities of given sequences under the model alone, from one prefill pass.
+ * For sequence b with tokens x_0 .. x_{L-1} (L = L_b) and start s = start_host[b], the score of token t (s <= t < L) is
+ *   log_softmax(lm_head(final_norm(h_{t-1})))[x_t]
+ * under causal attention over x_0 .. x_{t-1}: transformers' -cross_entropy(logits[s-1:L-1], ids[s:L]).  No repetition
+ * penalty, EOS mask, vocabulary range, temperature or warper applies; the per-slot tables and the range are ignored
+ * and left as they are.
+ *   ids: device [total], the B sequences back to back; cu_seqlens_host: host [B+1]; start_host: host [B].
+ *   out: device fp32 [sum_b (L_b - s_b)], the scores of sequence 0, then sequence 1, ...
+ *   scratch: caller-owned device memory, 256-byte aligned, of at least nt_lm_score_scratch_bytes(cfg) bytes.
+ * Rules: 1 <= B <= max_batch, sum L_b <= max_prefill_tokens, 1 <= s_b < L_b <= max_ctx; a violation returns
+ * NT_ERR_INVALID.  The caller writes page-table rows 0..B-1 as for nt_lm_prefill; the prefill chain fills those pages.
+ * Afterwards slot b < B has seq_lens = L_b, every slot has n_generated = 0 and done = 1, and nt_lm_decode /
+ * nt_lm_prefill_slots return NT_ERR_STATE until the next nt_lm_prefill or nt_lm_prefill_fork.  Nothing is sampled:
+ * out_tokens, cur_token, the log-probability buffer, the repetition-penalty histories, the Philox keys and the
+ * settings tables are not written.
+ * The lm_head runs over the scored rows in blocks of R = min(1024, max_prefill_tokens) rows with the log-softmax fused
+ * into its epilogue: per row and 128-column vocabulary tile only the pair (max, sum exp) and the target logit leave
+ * the GEMM, and a combine kernel folds the pairs in a fixed order.  Every token row's arithmetic is independent of the
+ * other sequences in the call, so a sequence's scores are bit-identical however it is batched. */
+/* scratch bytes of nt_lm_score (0 for an invalid config; needs no GPU):
+ *   a(8 * R * ceil(vocab_size / 128)) + a(4 * R) + 2 * a(4 * max_prefill_tokens),  a(x) = x rounded up to 256 */
+size_t nt_lm_score_scratch_bytes(const nt_lm_config* cfg);
+int nt_lm_score(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu_seqlens_host, const int32_t* start_host,
+                int B, float* out, void* scratch, size_t scratch_bytes, void* stream);
+
 /* Run n_steps decode steps for slots 0..B-1 with no host synchronisation in between
  * (finished slots keep their state; their work is skipped on device).
  * logits_out: optional device f32 [n_steps][B][vocab] (tests only; forces logits to HBM). */

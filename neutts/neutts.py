@@ -469,6 +469,53 @@ class NeuTTS:
             lps += r[1] if return_logprobs else []
         return (out, lps) if return_logprobs else out
 
+    # ------------------------------------------------------------------ scoring
+    def score(self, text: str, ref_codes, ref_text: str, codes, *, include_eos: bool = True) -> np.ndarray:
+        """How likely the speech codes ``codes`` are as this model's rendering of ``text`` in the voice of
+        (``ref_codes``, ``ref_text``): float32 log-probabilities, one per code and one more for
+        ``<|SPEECH_GENERATION_END|>`` when ``include_eos``, each token's log-softmax over the whole vocabulary given
+        the prompt and every earlier code, from one prefill pass (``SpeechLM.score``).  No sampling control applies,
+        and ``speech_tokens_only`` does not change the scores.  Their negated mean is the finetuning recipe's loss over
+        the speech tokens; a low mean flags a transcript that does not match its audio, and ranks takes or clips."""
+        return self.score_batch([text], [ref_codes], [ref_text], [codes], include_eos=include_eos)[0]
+
+    def score_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], codes: Sequence, *,
+                    include_eos: bool = True) -> list:
+        """``score`` over lists, one entry per utterance; returns a list of float32 arrays."""
+        if not (len(texts) == len(ref_codes) == len(ref_texts) == len(codes)):
+            raise ValueError("texts, ref_codes, ref_texts and codes must have the same length")
+        self._check_score()
+        n_codes = self._n_codes()
+        conts = []
+        for c in codes:
+            c = [int(x) for x in (c.tolist() if hasattr(c, "tolist") else c)]
+            if not c:
+                raise ValueError("codes to score must not be empty")
+            if min(c) < 0 or max(c) >= n_codes:
+                raise ValueError(f"codes must lie in 0..{n_codes - 1}")
+            conts.append(c)
+        prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(texts, ref_codes, ref_texts)]
+        base = self.speech_base
+        eos = [self._tok_id("<|SPEECH_GENERATION_END|>")] if include_eos else []
+        return self.score_from_prompt_ids(prompts, [[base + x for x in c] + eos for c in conts])
+
+    def score_from_prompt_ids(self, prompts: Sequence[Sequence[int]], continuations: Sequence[Sequence[int]]) -> list:
+        """Hot path only: the log-probability of every id of each continuation after its prompt (host ids in, float32
+        arrays out, one value per continuation id)."""
+        if len(prompts) != len(continuations):
+            raise ValueError("prompts and continuations must have the same length")
+        self._check_score()
+        if any(len(c) == 0 for c in continuations) or any(len(p) == 0 for p in prompts):
+            raise ValueError("prompts and continuations must not be empty")
+        seqs = [list(p) + list(c) for p, c in zip(prompts, continuations)]
+        out = self.backbone.score(seqs, [len(p) for p in prompts])
+        return [np.asarray(o, dtype=np.float32) for o in out]
+
+    def _check_score(self) -> None:
+        """Scoring needs an engine that scores (``SpeechLM.score``)."""
+        if not hasattr(self.backbone, "score"):
+            raise ValueError("score needs a backbone with score (neutts_air_b200.SpeechLM)")
+
     @staticmethod
     def _no_takes(takes) -> None:
         if takes != 1:

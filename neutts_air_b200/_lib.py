@@ -97,7 +97,7 @@ class CodecWeights(C.Structure):
 EXPORTS = [
     "nt_last_error", "nt_abi_version", "nt_launch_count", "nt_gemm",
     "nt_lm_workspace_bytes", "nt_lm_create", "nt_lm_destroy", "nt_lm_prefill", "nt_lm_prefill_slots", "nt_lm_prefill_fork",
-    "nt_lm_decode",
+    "nt_lm_score_scratch_bytes", "nt_lm_score", "nt_lm_decode",
     "nt_lm_set_slot_sampling", "nt_lm_set_vocab_range", "nt_lm_set_repetition_penalty", "nt_lm_set_logprobs",
     "nt_lm_head_gemv",
     "nt_lm_debug_set_layers", "nt_lm_debug_ptr", "nt_lm_debug_set_profile", "nt_lm_debug_capture_sampler",
@@ -136,6 +136,10 @@ def lib() -> C.CDLL:
                                       C.POINTER(C.c_int32), C.c_int, C.POINTER(Sampling), C.c_void_p, C.c_void_p]
     L.nt_lm_prefill_fork.argtypes = [C.c_void_p, C.POINTER(LMState), C.c_void_p, C.POINTER(C.c_int32), C.c_int, C.c_int,
                                      C.POINTER(Sampling), C.c_void_p, C.c_void_p]
+    L.nt_lm_score_scratch_bytes.restype = C.c_size_t
+    L.nt_lm_score_scratch_bytes.argtypes = [C.POINTER(LMConfig)]
+    L.nt_lm_score.argtypes = [C.c_void_p, C.POINTER(LMState), C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int,
+                              C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.nt_lm_decode.argtypes = [C.c_void_p, C.POINTER(LMState), C.c_int, C.c_int, C.POINTER(Sampling), C.c_void_p, C.c_void_p]
     L.nt_lm_set_slot_sampling.argtypes = [C.c_void_p, C.POINTER(SlotSampling), C.c_void_p]
     L.nt_lm_set_vocab_range.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]

@@ -37,7 +37,16 @@ struct GemmEpilogue {
   float* tile_max;         // optional [M][tile_ld]: maximum of the row's stored values inside this CTA's BN columns (lm_head ->
                            //   tile-max sampler); plain fp32 epilogue only
   long long tile_ld;
+  // log-softmax epilogue (kEpi == kEpiLogSoftmax, teacher-forced scoring): no logits are stored; per row and column tile
+  // the pair (max, sum exp(v - max)) over the tile's columns < N goes to lse[row * tile_ld + blockIdx.x], and the CTA
+  // whose columns hold tgt[row] writes that logit to zt[row]
+  float2* lse;
+  const int32_t* tgt;
+  float* zt;
 };
+
+constexpr int kEpiStore = 0;       // bias / residual / activation, fp32 and/or bf16 rows (every GEMM of the library)
+constexpr int kEpiLogSoftmax = 1;  // per-tile log-sum-exp pairs + the target logit (gemm_logsoftmax)
 
 // kShallow: half-depth ring (<= 113 KB of shared memory) for grids of more than one wave of CTAs.
 // kS3 (tf32 only): 3xTF32 in ONE pass.  Both operands arrive as hi/lo halves (hi = the value rounded to TF32, lo = the
@@ -57,7 +66,7 @@ struct GemmCfg {
   static_assert(BM * OUT_LD * 4 <= STAGES * STAGE_BYTES, "accumulator staging must fit the ring");
 };
 
-template <int kFmt, int BN, bool kShallow, bool kS3 = false>
+template <int kFmt, int BN, bool kShallow, bool kS3 = false, int kEpi = kEpiStore>
 __global__ void __launch_bounds__(256, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmEpilogue ep, int M,
                int N, int num_kb, int kb_per_tap, int a_lo_rows, int w_lo_rows) {
@@ -197,6 +206,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int q = warp - 4;  // rows [32 q, 32 q + 32) of the tile, one per lane
     const float* srow = stage + (q * 32 + lane) * Cfg::OUT_LD;
     const int row = m0 + q * 32 + lane;
+    if constexpr (kEpi == kEpiLogSoftmax) {
+      // this lane's row over the tile's valid columns: max, then sum exp(v - max), both in column order
+      if (row >= M) return;
+      const int nv = min(BN, N - n0);
+      float m = -INFINITY;
+      for (int j = 0; j < nv; ++j) m = fmaxf(m, srow[j]);
+      float s = 0.f;
+      for (int j = 0; j < nv; ++j) s += expf(srow[j] - m);
+      ep.lse[static_cast<long long>(row) * ep.tile_ld + blockIdx.x] = make_float2(m, s);
+      const int t = __ldg(ep.tgt + row) - n0;
+      if (t >= 0 && t < nv) ep.zt[row] = srow[t];
+      return;
+    }
     bool row_ok = row < M;
     if (ep.valid_period > 0 && (row % ep.valid_period) >= ep.valid_len) row_ok = false;
     float tmx = -INFINITY;
@@ -345,12 +367,12 @@ int make_tmap(CUtensorMap* out, nt_dtype dt, const void* base, uint64_t rows, ui
   return NT_OK;
 }
 
-template <int kFmt, int BN, bool kShallow, bool kS3 = false>
+template <int kFmt, int BN, bool kShallow, bool kS3 = false, int kEpi = kEpiStore>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int M, int N, int num_kb,
                        int kb_per_tap, cudaStream_t stream, int a_lo_rows = 0, int w_lo_rows = 0) {
   const int splits = ep.split_k > 1 ? ep.split_k : 1;
   using Cfg = GemmCfg<BN, kShallow, kS3>;
-  auto kern = gemm_tc_kernel<kFmt, BN, kShallow, kS3>;   // launch_kernel opts in to the dynamic shared memory per device
+  auto kern = gemm_tc_kernel<kFmt, BN, kShallow, kS3, kEpi>;   // launch_kernel opts in to the dynamic shared memory per device
   dim3 grid((N + BN - 1) / BN, (M + Cfg::BM - 1) / Cfg::BM, splits);
   return launch_kernel(kern, grid, dim3(256), Cfg::SMEM_BYTES, stream, /*pdl=*/true, ta, tb, ep, M, N, num_kb,
                        kb_per_tap, a_lo_rows, w_lo_rows);
@@ -474,6 +496,28 @@ int gemm_dispatch(const nt_gemm_args& a, cudaStream_t stream, SplitK* split, boo
     NT_GEMM_CASE(2, 32);
   }
 #undef NT_GEMM_CASE
+}
+
+int gemm_logsoftmax(const void* A, int M, int K, const void* W, int N, const int32_t* tgt, float2* lse,
+                    long long lse_ld, float* zt, cudaStream_t stream) {
+  if (M <= 0 || N <= 0 || K <= 0 || K % 64) return set_error(NT_ERR_INVALID, "gemm_logsoftmax: bad shape %d x %d x %d", M, N, K);
+  if (lse_ld < (N + 127) / 128) return set_error(NT_ERR_INVALID, "gemm_logsoftmax: pair row pitch %lld < %d tiles", lse_ld, (N + 127) / 128);
+  CUtensorMap ta, tb;
+  int rc = make_tmap(&ta, NT_BF16, A, uint64_t(M), uint64_t(K), uint64_t(K), 128);
+  if (rc) return rc;
+  if ((rc = make_tmap(&tb, NT_BF16, W, uint64_t(N), uint64_t(K), uint64_t(K), 128))) return rc;
+  GemmEpilogue ep;
+  memset(&ep, 0, sizeof(ep));
+  ep.split_k = 1;
+  ep.w_const = 1;
+  ep.w_stream = M <= 128 ? 1 : 0;
+  ep.tile_ld = lse_ld;
+  ep.lse = lse, ep.tgt = tgt, ep.zt = zt;
+  const int num_kb = K / 64;
+  // the vocabulary tile is always 128 columns, so a row's pairs do not depend on M
+  const int ctas = ((M + 127) / 128) * ((N + 127) / 128);
+  return ctas > num_sms() ? launch_gemm<1, 128, true, false, kEpiLogSoftmax>(ta, tb, ep, M, N, num_kb, num_kb, stream)
+                          : launch_gemm<1, 128, false, false, kEpiLogSoftmax>(ta, tb, ep, M, N, num_kb, num_kb, stream);
 }
 
 }  // namespace nt

@@ -72,6 +72,11 @@ struct Split3 {
 int gemm_dispatch(const nt_gemm_args& a, cudaStream_t stream, SplitK* split = nullptr, bool w_const = false,
                   const Split3* s3 = nullptr, float* tile_max = nullptr, int bn = 0, long long tile_ld = 0);
 int gemm_tile_n(int M, int N, bool swiglu);
+// Teacher-forced scoring: logits = A[M,K] . W[N,K]^T (bf16, K-major, row stride K) at a fixed 128-column tile, never
+// stored.  Per row r and column tile t: lse[r * lse_ld + t] = (max, sum exp(v - max)) over the tile's columns < N; the
+// tile holding tgt[r] also writes that logit to zt[r].  Each row's arithmetic is independent of M.
+int gemm_logsoftmax(const void* A, int M, int K, const void* W, int N, const int32_t* tgt, float2* lse, long long lse_ld,
+                    float* zt, cudaStream_t stream);
 
 // 2-D TMA descriptor over a row-major matrix (rows x cols elements, row stride ld elements); box = box_rows x 128
 // bytes, SWIZZLE_128B (gemm_tc.cu)

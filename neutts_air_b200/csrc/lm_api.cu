@@ -487,8 +487,10 @@ static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cud
 // Transformer layers over `rows` token rows held in lm->h, via tensor-core GEMMs.
 // mode 0: prefill (causal attention over the prompt);  mode 1: one new token per sequence.
 // table: page table to address the KV cache with, row b for sequence b of the call (default: the state's).
+// row_local (nt_lm_score): no split-K, 128-column GEMM tiles and the one-warp-per-row RMSNorm for every row count, so that
+// each token row's arithmetic does not depend on how many rows the call holds.
 static int layers_gemm(nt_lm* lm, const nt_lm_state* st, int rows, int B, int mode, int max_len, cudaStream_t stream,
-                       SplitK* tail = nullptr, const int32_t* table = nullptr) {
+                       SplitK* tail = nullptr, const int32_t* table = nullptr, bool row_local = false) {
   const nt_lm_config& c = lm->cfg;
   KVLayout kv = make_kv(lm, st);
   if (table) kv.page_table = table;
@@ -502,9 +504,10 @@ static int layers_gemm(nt_lm* lm, const nt_lm_state* st, int rows, int B, int mo
   // norm of lm_head_rows reads lm->h next); in prefill a row gather comes first, so it stays whole.
   SplitK pend;
   pend.ws = lm->splitk_ws, pend.ws_floats = lm->splitk_floats, pend.used = 1, pend.slice_stride = 0;
+  const int bn = row_local ? 128 : 0;
   for (int l = 0; l < n_layers; ++l) {
     if ((rc = launch_rmsnorm_rows(lm->h, lm->ln1[l], c.rms_eps, rows, H, nullptr, lm->xn, stream,
-                                  pend.used > 1 ? pend.ws : nullptr, pend.used > 1 ? pend.used : 0, pend.slice_stride)))
+                                  pend.used > 1 ? pend.ws : nullptr, pend.used > 1 ? pend.used : 0, pend.slice_stride, row_local)))
       return rc;
     pend.used = 1;
     nt_gemm_args a;
@@ -514,7 +517,7 @@ static int layers_gemm(nt_lm* lm, const nt_lm_state* st, int rows, int B, int mo
     // few row tiles: the projection splits K into slices that rope_append sums (the bias rides on slice 0)
     SplitK qsplit;
     qsplit.ws = lm->splitk_ws, qsplit.ws_floats = lm->splitk_floats, qsplit.used = 1, qsplit.slice_stride = 0;
-    if ((rc = gemm_dispatch(a, stream, &qsplit, true))) return rc;
+    if ((rc = gemm_dispatch(a, stream, row_local ? nullptr : &qsplit, true, nullptr, nullptr, bn))) return rc;
     const int32_t* tseq = mode == 0 ? lm->tok_seq : lm->iota;
     const int32_t* tpos = mode == 0 ? lm->tok_pos : st->seq_lens;
     // decode on the tensor-core attention kernel (batch > 4): RoPE + KV append run in that kernel's prologue
@@ -542,37 +545,39 @@ static int layers_gemm(nt_lm* lm, const nt_lm_state* st, int rows, int B, int mo
     memset(&a, 0, sizeof(a));
     a.dtype = NT_BF16, a.M = rows, a.N = H, a.K = HD, a.A = lm->attn_bf16, a.lda = HD, a.W = lm->wo[l], a.ldw = HD;
     a.residual = lm->h, a.ldr = H, a.out_f32 = lm->h, a.ldc = H;
-    if ((rc = gemm_dispatch(a, stream, &pend, true))) return rc;
+    if ((rc = gemm_dispatch(a, stream, row_local ? nullptr : &pend, true, nullptr, nullptr, bn))) return rc;
     if ((rc = launch_rmsnorm_rows(lm->h, lm->ln2[l], c.rms_eps, rows, H, nullptr, lm->xn, stream,
-                                  pend.used > 1 ? pend.ws : nullptr, pend.used > 1 ? pend.used : 0, pend.slice_stride)))
+                                  pend.used > 1 ? pend.ws : nullptr, pend.used > 1 ? pend.used : 0, pend.slice_stride, row_local)))
       return rc;
     pend.used = 1;
     memset(&a, 0, sizeof(a));
     a.dtype = NT_BF16, a.M = rows, a.N = 2 * I, a.K = H, a.A = lm->xn, a.lda = H, a.W = lm->wgu[l], a.ldw = H;
     a.act = NT_ACT_SWIGLU, a.out_bf16 = lm->act_bf16, a.ldc = I;
-    if ((rc = gemm_dispatch(a, stream, nullptr, true))) return rc;
+    if ((rc = gemm_dispatch(a, stream, nullptr, true, nullptr, nullptr, bn))) return rc;
     memset(&a, 0, sizeof(a));
     a.dtype = NT_BF16, a.M = rows, a.N = H, a.K = I, a.A = lm->act_bf16, a.lda = I, a.W = lm->wd[l], a.ldw = I;
     a.residual = lm->h, a.ldr = H, a.out_f32 = lm->h, a.ldc = H;
-    if ((rc = gemm_dispatch(a, stream, (l + 1 < n_layers || tail) ? &pend : nullptr, true))) return rc;
+    if ((rc = gemm_dispatch(a, stream, (!row_local && (l + 1 < n_layers || tail)) ? &pend : nullptr, true, nullptr, nullptr, bn))) return rc;
   }
   if (tail) *tail = pend;
   return NT_OK;
 }
 
 // Checks cu_seqlens [B+1] and stages the per-token tables of a prefill: the sequence and position of every token row,
-// the last row of every sequence.  lens / max_len: the prompt lengths.
-static int prefill_stage(nt_lm* lm, const int32_t* cu, int B, std::vector<int>& lens, int& max_len, cudaStream_t stream) {
+// the last row of every sequence.  lens / max_len: the prompt lengths, each at most len_max (default max_ctx - 1).
+static int prefill_stage(nt_lm* lm, const int32_t* cu, int B, std::vector<int>& lens, int& max_len, cudaStream_t stream,
+                         int len_max = -1) {
   const nt_lm_config& c = lm->cfg;
   const int T = cu[B];
   if (cu[0] != 0 || T < B || T > c.max_prefill_tokens)
     return set_error(NT_ERR_INVALID, "prefill tokens %d not in %d..%d", T, B, c.max_prefill_tokens);
+  if (len_max < 0) len_max = c.max_ctx - 1;
   std::vector<int> tseq(T), tpos(T), last(B);
   lens.assign(B, 0);
   max_len = 0;
   for (int b = 0; b < B; ++b) {
     const int len = cu[b + 1] - cu[b];
-    if (len < 1 || len >= c.max_ctx) return set_error(NT_ERR_INVALID, "prompt %d has length %d (must be 1..%d)", b, len, c.max_ctx - 1);
+    if (len < 1 || len > len_max) return set_error(NT_ERR_INVALID, "prompt %d has length %d (must be 1..%d)", b, len, len_max);
     for (int t = 0; t < len; ++t) tseq[cu[b] + t] = b, tpos[cu[b] + t] = t;
     last[b] = cu[b + 1] - 1;
     lens[b] = len;
@@ -586,6 +591,14 @@ static int prefill_stage(nt_lm* lm, const int32_t* cu, int B, std::vector<int>& 
   return NT_OK;
 }
 
+// The prefill chain: prompt ids -> lm->h rows (every position, after the last layer) + KV cache.  table, row_local: see
+// layers_gemm.
+static int prefill_layers(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, int B, int max_len,
+                          const int32_t* table, cudaStream_t stream, bool row_local = false) {
+  int rc = launch_embed_rows(lm->embed, ids, cu[B], lm->cfg.hidden, lm->h, stream);
+  return rc ? rc : layers_gemm(lm, st, cu[B], B, 0, max_len, stream, nullptr, table, row_local);
+}
+
 // Prompt rows -> KV cache + last-position logits in lm->logits (and logits_out).  table: see layers_gemm.
 // row_slot: the slot of every prompt row (nullptr: row b is slot b); it fills that slot's repetition-penalty history.
 static int prefill_forward(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, int B, int max_len,
@@ -596,8 +609,7 @@ static int prefill_forward(nt_lm* lm, const nt_lm_state* st, const int32_t* ids,
   if (lm->step.rep_on &&
       (rc = launch_rep_history(lm->rep_hist, lm->rep_words, lm->rep_tab, lm->rep_rec, row_slot, ids, lm->cu_dev, B, c.vocab_size, stream)))
     return rc;
-  if ((rc = launch_embed_rows(lm->embed, ids, cu[B], c.hidden, lm->h, stream))) return rc;
-  if ((rc = layers_gemm(lm, st, cu[B], B, 0, max_len, stream, nullptr, table))) return rc;
+  if ((rc = prefill_layers(lm, st, ids, cu, B, max_len, table, stream))) return rc;
   if ((rc = launch_gather_rows(lm->h, lm->last_rows, B, c.hidden, lm->h_last, stream))) return rc;
   if ((rc = lm_head_rows(lm, lm->h_last, B, lm->logits, stream, nullptr, eos, row_slot))) return rc;
   if (logits_out)
@@ -712,6 +724,82 @@ extern "C" int nt_lm_prefill_fork(nt_lm* lm, const nt_lm_state* st, const int32_
   s.row_src = n > 1 ? lm->fork_args : nullptr;
   if ((rc = run_sampler(lm, s, N, stream))) return rc;
   lm->prefilled = true;
+  return NT_OK;
+}
+
+// Teacher-forced scoring.  The caller's scratch holds, for one block of R scored rows, the (max, sum exp) pair of every
+// 128-column vocabulary tile and the target logit, and for the whole call the source row and the target of every scored
+// row.  Each pointer is 256-byte aligned relative to the scratch base.
+constexpr int kScoreRows = 1024;
+struct ScoreScratch {
+  float2* lse;   // [R][nt]
+  float* zt;     // [R]
+  int32_t* src;  // [max_prefill_tokens] row of lm->h each scored row reads
+  int32_t* tgt;  // [max_prefill_tokens] token each scored row predicts
+  int R, nt;
+};
+static size_t score_carve(const nt_lm_config& c, void* base, ScoreScratch* s) {
+  Arena a(base, 0);
+  s->R = c.max_prefill_tokens < kScoreRows ? c.max_prefill_tokens : kScoreRows;
+  s->nt = (c.vocab_size + 127) / 128;
+  s->lse = a.take<float2>(size_t(s->R) * s->nt);
+  s->zt = a.take<float>(s->R);
+  s->src = a.take<int32_t>(c.max_prefill_tokens);
+  s->tgt = a.take<int32_t>(c.max_prefill_tokens);
+  return a.off;
+}
+
+extern "C" size_t nt_lm_score_scratch_bytes(const nt_lm_config* cfg) {
+  if (lm_check_config(cfg)) return 0;
+  ScoreScratch s;
+  return score_carve(*cfg, nullptr, &s);
+}
+
+// The prefill chain in its row-local form over every token, then the final norm of the scored rows, then per block of
+// R rows the lm_head GEMM with the log-softmax epilogue and the combine kernel.  No logits row is stored anywhere.
+extern "C" int nt_lm_score(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, const int32_t* start, int B,
+                           float* out, void* scratch, size_t scratch_bytes, void* stream_) {
+  if (!lm || !st || !ids || !cu || !start || !out || !scratch) return set_error(NT_ERR_INVALID, "nt_lm_score: null argument");
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  const nt_lm_config& c = lm->cfg;
+  if (B < 1 || B > c.max_batch) return set_error(NT_ERR_INVALID, "batch %d not in 1..%d", B, c.max_batch);
+  ScoreScratch ss;
+  const size_t need = score_carve(c, nullptr, &ss);
+  if (scratch_bytes < need) return set_error(NT_ERR_INVALID, "nt_lm_score: scratch holds %zu bytes, needs %zu", scratch_bytes, need);
+  if (reinterpret_cast<uintptr_t>(scratch) & 255) return set_error(NT_ERR_INVALID, "nt_lm_score: scratch must be 256-byte aligned");
+  score_carve(c, scratch, &ss);
+  if (cu[0] != 0) return set_error(NT_ERR_INVALID, "nt_lm_score: cu_seqlens[0] must be 0");
+  std::vector<int32_t> src;
+  for (int b = 0; b < B; ++b) {
+    const int L = cu[b + 1] - cu[b], s = start[b];
+    if (L < 2 || L > c.max_ctx) return set_error(NT_ERR_INVALID, "sequence %d has length %d (must be 2..%d)", b, L, c.max_ctx);
+    if (s < 1 || s >= L) return set_error(NT_ERR_INVALID, "sequence %d: start %d not in 1..%d", b, s, L - 1);
+    if (cu[b + 1] > c.max_prefill_tokens)
+      return set_error(NT_ERR_INVALID, "scoring %d+ tokens in one call; at most %d", cu[b + 1], c.max_prefill_tokens);
+    for (int p = s - 1; p < L - 1; ++p) src.push_back(cu[b] + p);   // row p predicts token p + 1
+  }
+  const int n = static_cast<int>(src.size());
+  std::vector<int> lens;
+  int max_len = 0;
+  int rc = prefill_stage(lm, cu, B, lens, max_len, stream, c.max_ctx);
+  if (rc) return rc;
+  NT_CUDA_CHECK(cudaMemcpyAsync(ss.src, src.data(), n * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+  if ((rc = prefill_layers(lm, st, ids, cu, B, max_len, nullptr, stream, /*row_local=*/true))) return rc;
+  if ((rc = launch_score_rows(lm->h, ss.src, ids, n, c.hidden, lm->final_norm, c.rms_eps, lm->xn, ss.tgt, stream))) return rc;
+  for (int i0 = 0; i0 < n; i0 += ss.R) {
+    const int m = n - i0 < ss.R ? n - i0 : ss.R;
+    if ((rc = gemm_logsoftmax(lm->xn + static_cast<long long>(i0) * c.hidden, m, c.hidden, lm->lm_head, c.vocab_size, ss.tgt + i0,
+                              ss.lse, ss.nt, ss.zt, stream)))
+      return rc;
+    if ((rc = launch_score_combine(ss.lse, ss.nt, ss.nt, ss.zt, m, out + i0, stream))) return rc;
+  }
+  // every slot: its sequence's length (0 beyond B), nothing generated, finished; decoding needs a new prefill
+  std::vector<int32_t> seq(c.max_batch, 0), ones(c.max_batch, 1);
+  for (int b = 0; b < B; ++b) seq[b] = lens[b];
+  NT_CUDA_CHECK(cudaMemcpyAsync(st->seq_lens, seq.data(), seq.size() * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+  NT_CUDA_CHECK(cudaMemsetAsync(st->n_generated, 0, size_t(c.max_batch) * sizeof(int32_t), stream));
+  NT_CUDA_CHECK(cudaMemcpyAsync(st->done, ones.data(), ones.size() * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+  lm->prefilled = false;
   return NT_OK;
 }
 

@@ -1038,9 +1038,10 @@ __global__ void __launch_bounds__(256) rmsnorm_rows_wide_kernel(float* x, const 
 }
 
 int launch_rmsnorm_rows(const float* x, const float* w, float eps, int rows, int cols, float* out_f32,
-                        __nv_bfloat16* out_bf16, cudaStream_t s, const float* parts, int nparts, long long pstride) {
+                        __nv_bfloat16* out_bf16, cudaStream_t s, const float* parts, int nparts, long long pstride,
+                        bool per_warp) {
   if (cols % 4) return set_error(NT_ERR_INVALID, "rmsnorm: cols must be a multiple of 4");
-  if (rows <= 256 && cols <= 1024 && nparts <= 8)
+  if (!per_warp && rows <= 256 && cols <= 1024 && nparts <= 8)
     return launch_kernel(rmsnorm_rows_wide_kernel, dim3(rows), dim3(256), 0, s, true, const_cast<float*>(x), w, eps, cols, out_f32,
                          out_bf16, parts, nparts, pstride);
   // few rows (batched decode): one warp per CTA so the rows spread over the SMs; many rows (prefill): 8 per CTA
@@ -1255,6 +1256,69 @@ __global__ void gather_rows_kernel(const float* src, const int32_t* rows, int co
 }
 int launch_gather_rows(const float* src, const int32_t* rows, int n, int cols, float* dst, cudaStream_t s) {
   return launch_kernel(gather_rows_kernel, dim3(n), dim3(256), 0, s, true, src, rows, cols, dst);
+}
+
+// =================================================================================== teacher-forced scoring
+// One warp per scored row i: the final RMSNorm of h[src[i]] as rmsnorm_rows_kernel computes it (the same per-lane
+// float4 sums and warp reduction), rounded to bf16 into xn[i] (the lm_head's A operand); tgt[i] = ids[src[i] + 1], the
+// token the row predicts.
+__global__ void __launch_bounds__(256) score_rows_kernel(const float* h, const int32_t* src, const int32_t* ids, int n, int cols,
+                                                         const float* w, float eps, __nv_bfloat16* xn, int32_t* tgt) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (i >= n) return;
+  const int r = src[i];
+  if (lane == 0) tgt[i] = ids[r + 1];
+  const float4* xr = reinterpret_cast<const float4*>(h + static_cast<long long>(r) * cols);
+  const float4* wr = reinterpret_cast<const float4*>(w);
+  const int nvec = cols >> 2;
+  float ss = 0.f;
+  for (int i0 = lane; i0 < nvec; i0 += 32 * 8) {
+    float4 v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = (i0 + 32 * j < nvec) ? xr[i0 + 32 * j] : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) ss += v[j].x * v[j].x + v[j].y * v[j].y + v[j].z * v[j].z + v[j].w * v[j].w;
+  }
+  ss = warp_sum(ss);
+  const float sc = rsqrtf(ss / static_cast<float>(cols) + eps);
+  uint2* out = reinterpret_cast<uint2*>(xn + static_cast<long long>(i) * cols);
+  for (int k = lane; k < nvec; k += 32) {
+    const float4 v = xr[k], g = wr[k];
+    out[k] = make_uint2(pack_bf16x2(g.x * (v.x * sc), g.y * (v.y * sc)), pack_bf16x2(g.z * (v.z * sc), g.w * (v.w * sc)));
+  }
+}
+int launch_score_rows(const float* h, const int32_t* src, const int32_t* ids, int n, int cols, const float* w, float eps,
+                      __nv_bfloat16* xn, int32_t* tgt, cudaStream_t s) {
+  if (cols % 4) return set_error(NT_ERR_INVALID, "score rows: cols must be a multiple of 4");
+  return launch_kernel(score_rows_kernel, dim3((n + 7) / 8), dim3(256), 0, s, true, h, src, ids, n, cols, w, eps, xn, tgt);
+}
+
+// One warp per row: M = max of the tile maxima, S = sum s_t exp(m_t - M), each lane over tiles lane, lane + 32, ...
+// in order and the lanes combined by a fixed butterfly, so a row's result depends on its pairs alone.
+__global__ void __launch_bounds__(256) score_combine_kernel(const float2* lse, long long ld, int nt, const float* zt, int n,
+                                                            float* out) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (r >= n) return;
+  const float2* p = lse + static_cast<long long>(r) * ld;
+  float m = -INFINITY;
+  for (int t = lane; t < nt; t += 32) m = fmaxf(m, p[t].x);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  float s = 0.f;
+  for (int t = lane; t < nt; t += 32) {
+    const float2 q = p[t];
+    s += q.y * expf(q.x - m);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) out[r] = zt[r] - (m + logf(s));
+}
+int launch_score_combine(const float2* lse, long long ld, int nt, const float* zt, int n, float* out, cudaStream_t s) {
+  return launch_kernel(score_combine_kernel, dim3((n + 7) / 8), dim3(256), 0, s, true, lse, ld, nt, zt, n, out);
 }
 
 // one CTA per listed slot: compact page-table row + the slot's fresh length, counters and Philox key

@@ -132,10 +132,17 @@ int launch_rep_penalty(float* logits, int B, int V, const uint32_t* hist, int wo
                        const int32_t* recorded, const int32_t* row_slot, float* tmax, int nt, cudaStream_t s);
 
 int launch_embed_rows(const __nv_bfloat16* embed, const int32_t* ids, int T, int hidden, float* h, cudaStream_t s);
-// parts != nullptr: x is updated in place first (x += sum of nparts split-K slices, slice order) -- see SplitK
+// parts != nullptr: x is updated in place first (x += sum of nparts split-K slices, slice order) -- see SplitK.
+// per_warp: always the one-warp-per-row kernel, whose per-row arithmetic does not depend on `rows`.
 int launch_rmsnorm_rows(const float* x, const float* w, float eps, int rows, int cols, float* out_f32,
                         __nv_bfloat16* out_bf16, cudaStream_t s, const float* parts = nullptr, int nparts = 0,
-                        long long pstride = 0);
+                        long long pstride = 0, bool per_warp = false);
+// Teacher-forced scoring (nt_lm_score).  launch_score_rows: for each of n scored rows, xn[i] = bf16(final RMSNorm of
+// h[src[i]]) and tgt[i] = ids[src[i] + 1].  launch_score_combine: out[r] = zt[r] - log-sum-exp of row r's nt tile pairs
+// (lse, row pitch ld; see gemm_logsoftmax), folded in a fixed order.
+int launch_score_rows(const float* h, const int32_t* src, const int32_t* ids, int n, int cols, const float* w, float eps,
+                      __nv_bfloat16* xn, int32_t* tgt, cudaStream_t s);
+int launch_score_combine(const float2* lse, long long ld, int nt, const float* zt, int n, float* out, cudaStream_t s);
 // qkv: [T, qkv_n] fp32 in packed (pair-interleaved) column order -> q natural order + K/V pages
 int launch_rope_append(const float* qkv, int T, int qkv_n, const int32_t* tok_seq, const int32_t* tok_pos, int n_heads,
                        const float* inv_freq, float* q_out, const KVLayout& kv, int layer, cudaStream_t s, int nparts = 1,

@@ -219,6 +219,36 @@ def fork_slots(n_prompts: int, n: int, slot_base: int = 0) -> list:
     return [(i, j, i * n + j, i * n + j + slot_base) for i in range(n_prompts) for j in range(n)]
 
 
+def score_starts(lens, start) -> list:
+    """The start of every sequence ``score`` takes: ``start`` is an int or one value per sequence, each in 1..L - 1."""
+    starts = per_item(len(lens), "sequence", start=start)["start"]
+    starts = starts if isinstance(starts, list) else [starts] * len(lens)
+    out = []
+    for b, (L, s) in enumerate(zip(lens, starts)):
+        if isinstance(s, bool) or int(s) != s or not 1 <= int(s) < L:
+            raise ValueError(f"sequence {b}: start {s!r} must be an integer in 1..{L - 1} (its length is {L})")
+        out.append(int(s))
+    return out
+
+
+def pack_score_calls(lens, max_batch: int, max_tokens: int, max_ctx: int) -> list:
+    """Sequences of lengths ``lens`` packed greedily, in input order, into ``nt_lm_score`` calls of at most
+    ``max_batch`` sequences and ``max_tokens`` tokens -> a list of index lists.  A sequence longer than ``max_ctx`` or
+    ``max_tokens`` fits no call and raises ValueError."""
+    calls, cur, tok = [], [], 0
+    for i, L in enumerate(lens):
+        if L > max_ctx or L > max_tokens:
+            raise ValueError(f"sequence {i} has {L} tokens; one scoring call takes at most {min(max_ctx, max_tokens)}")
+        if cur and (len(cur) == max_batch or tok + L > max_tokens):
+            calls.append(cur)
+            cur, tok = [], 0
+        cur.append(i)
+        tok += L
+    if cur:
+        calls.append(cur)
+    return calls
+
+
 DEFAULT_PENALTY = (1.0, True)   # repetition penalty, prompt included: transformers' RepetitionPenaltyLogitsProcessor
 
 
@@ -642,6 +672,61 @@ class SpeechLM:
                                                   _lib.current_stream_ptr()))
         self._B = max(self._B, max(slots) + 1)
         return logits
+
+    @torch.no_grad()
+    def score(self, sequences, start) -> list:
+        """Teacher-forced scoring (``nt_lm_score``): for every sequence x_0 .. x_{L-1} and its start s, the
+        log-probability of each token x_t (s <= t < L) under the model given x_0 .. x_{t-1}, from one prefill pass -- the
+        model alone, with no repetition penalty, EOS mask, vocabulary range, temperature or warper (the settings stay as
+        they are).  transformers' ``-cross_entropy(logits[s-1:L-1], ids[s:L], reduction="none")``.
+
+        ``sequences``: 1-D int sequences (at least 2 ids each); ``start``: an int or one per sequence.  Returns one
+        float32 CPU tensor [L - s] per sequence, in input order.  Sequences go into calls of at most ``max_batch``
+        sequences and ``max_prefill_tokens`` tokens (``pack_score_calls``); each call takes KV pages as ``prefill`` does
+        and gives them all back.  A sequence's scores do not depend on the others in its call.  Every slot is reset:
+        ``decode`` and ``prefill_slots`` need a new ``prefill`` afterwards."""
+        seqs = [np.asarray(s, dtype=np.int64).reshape(-1) for s in sequences]
+        lens = [len(s) for s in seqs]
+        starts = score_starts(lens, start)
+        calls = pack_score_calls(lens, self.max_batch, self.max_prefill_tokens, self.max_ctx)
+        if seqs:
+            self._stage_ids(seqs)   # range check of every id before any engine call
+        if getattr(self, "_score_scratch", None) is None:
+            n = self.L.nt_lm_score_scratch_bytes(C.byref(self.cfg))
+            if n == 0:
+                _lib.check(-1)
+            self._score_scratch = torch.empty(n, dtype=torch.uint8, device=self.device)
+        out = [None] * len(seqs)
+        i32p = C.POINTER(C.c_int32)
+        for idx in calls:
+            B = len(idx)
+            clens = [lens[i] for i in idx]
+            staged = self._stage_ids([seqs[i] for i in idx])
+            self.release_pages()
+            table = np.zeros((self.max_batch, self.max_pages), dtype=np.int32)
+            self._alloc_pages(table, range(B), clens, [0] * B)
+            cu = np.zeros(B + 1, dtype=np.int32)
+            cu[1:] = np.cumsum(clens)
+            st = np.asarray([starts[i] for i in idx], dtype=np.int32)
+            n = sum(L - s for L, s in zip(clens, st.tolist()))
+            try:
+                with torch.cuda.device(self.device):
+                    ids = staged.to(self.device, non_blocking=True)
+                    if self._table_host is None or not np.array_equal(self._table_host, table):
+                        self.page_table.copy_(torch.from_numpy(table))
+                        self._table_host = table
+                    res = torch.empty(n, dtype=torch.float32, device=self.device)
+                    _lib.check(self.L.nt_lm_score(self.handle, C.byref(self.state), ids.data_ptr(), cu.ctypes.data_as(i32p),
+                                                  st.ctypes.data_as(i32p), B, res.data_ptr(), self._score_scratch.data_ptr(),
+                                                  self._score_scratch.numel(), _lib.current_stream_ptr()))
+                    res = res.cpu()
+            finally:
+                self.release_pages()
+            o = 0
+            for i, L, s in zip(idx, clens, st.tolist()):
+                out[i] = res[o: o + L - s].clone()
+                o += L - s
+        return out
 
     def decode(self, n_steps: int, sp, return_logits: bool = False):
         B = self._B
