@@ -539,16 +539,26 @@ class NeuTTS:
     def infer_stream_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], *, temperature=1.0,
                            top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0,
                            penalize_prompt=True, takes: int = 1) -> Generator[list, None, None]:
-        """Streaming synthesis of up to ``max_batch`` utterances at once (BASELINE.json configs[4]; the reference
-        streams one utterance, ``neutts/neutts.py:373-465``).  Every yield is a list with one entry per utterance:
-        the next audio chunk (float32, cross-faded exactly as in ``infer_stream``) or ``None`` when that utterance
-        has nothing new.  The sequences decode in lock-step in ONE persistent-kernel launch per round; the windows
-        that are due are gathered on the device from the code history and go through the codec as one batch.  Streaming
-        returns no per-token log-probabilities (``infer_batch``'s ``return_logprobs``) and generates one take per
-        utterance (``takes`` other than 1 raises ValueError)."""
+        """Streaming synthesis of many utterances at once (BASELINE.json configs[4]; the reference streams one
+        utterance, ``neutts/neutts.py:373-465``).  Every yield is a list with one entry per utterance, as many entries
+        as ``texts``: the next audio chunk (float32, cross-faded exactly as in ``infer_stream``) or ``None`` when that
+        utterance has nothing new.  The sequences decode in lock-step in ONE persistent-kernel launch per round; the
+        windows that are due are gathered on the device from the code history and go through the codec as one batch.
+
+        A list longer than the engine's ``max_batch`` streams as a queue: utterances take the slots in list order, and
+        a slot whose utterance has sent its last chunk takes the next waiting one while the others keep decoding, so
+        a late utterance starts as soon as a slot frees up instead of after whole chunks of the list.  Utterance i
+        draws from random stream i, the stream it has when the list fits into the slots, and its sampling controls
+        (scalars or one value per utterance) follow it into whichever slot it takes.  The queue needs a backbone with
+        ``prefill_slots`` (ValueError otherwise), and every KV page is given back when the generator ends or is
+        closed early.
+
+        Streaming returns no per-token log-probabilities (``infer_batch``'s ``return_logprobs``) and generates one take
+        per utterance (``takes`` other than 1 raises ValueError)."""
         self._no_takes(takes)
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
+        self._stream_slots(len(texts))
         ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)
         prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(texts, ref_codes, ref_texts)]
         refs = [[int(c) for c in (rc.tolist() if hasattr(rc, "tolist") else rc)] for rc in ref_codes]
@@ -559,6 +569,15 @@ class NeuTTS:
             if out[0] is not None:
                 yield out[0]
 
+    def _stream_slots(self, n: int) -> int:
+        """Slots that stream n utterances: the engine's ``max_batch`` (n when it has none).  More utterances than slots
+        run as a queue, which needs an engine that refills single slots (``prefill_slots``)."""
+        slots = getattr(self.backbone, "max_batch", n)
+        if n > slots and not hasattr(self.backbone, "prefill_slots"):
+            raise ValueError(f"streaming {n} utterances through {slots} slots needs a backbone with prefill_slots "
+                             "(neutts_air_b200.SpeechLM)")
+        return min(n, slots)
+
     def _stream_batch(self, prompts, refs, ctl: dict | None = None) -> Generator[list, None, None]:
         """Window geometry of the reference (``neutts/neutts.py:87-91,401-421,443-465``): once F + LA undecoded frames
         exist, the codec decodes [n_dec - LB - OV, n_dec + F + LA) and the slice [n_dec - OV, n_dec + F + OV) is
@@ -566,8 +585,14 @@ class NeuTTS:
         50 for the "codec every 50 tokens" configuration BASELINE.json names.
 
         State per slot: the code history (reference codes, then generated ones) lives ON THE DEVICE next to the
-        engine's ``out_tokens``; a round is  decode(k steps, all slots) -> absorb the new tokens into the history
-        with device ops -> one small D2H read of (n_generated, done, history length) -> batched codec call."""
+        engine's ``out_tokens``; a round is  absorb the new tokens into the history with device ops -> one small D2H
+        read of (n_generated, done, history length) -> batched codec call -> yield -> refill -> decode(k steps, all
+        slots).  Cross-fade state and decode position belong to the utterance.
+
+        More utterances than the engine's ``max_batch`` run as a queue on its S slots: utterance i is admitted FIFO and
+        draws from Philox stream i (the first S through ``prefill``, later ones through ``prefill_slots``); a slot is
+        refilled once its utterance's tail has been decoded from its history row.  Every KV page is back in the pool
+        when the generator ends, closed early included."""
         hop, F, LA, LB, OV = self.hop_length, self.streaming_frames_per_chunk, self.streaming_lookforward, \
             self.streaming_lookback, self.streaming_overlap_frames
         eos = self._tok_id("<|SPEECH_GENERATION_END|>")
@@ -575,29 +600,44 @@ class NeuTTS:
         lm = self.backbone
         if not hasattr(lm, "prefill"):
             raise NotImplementedError("Streaming needs the neutts_air_b200.SpeechLM backbone")
-        B = len(prompts)
+        N = len(prompts)
+        B = self._stream_slots(N)
+        queue = N > B
         limits = [min(self.max_context - len(p), lm.max_new) for p in prompts]
         if min(limits) < 1:
             raise ValueError("prompt already at max_length")
         limit = max(limits)
-        st = resolve_settings(lm, B, vocab_range=self._speech_range(), **(ctl if ctl is not None else CONTROL_DEFAULTS))
+        st = resolve_settings(lm, N, vocab_range=self._speech_range(), **(ctl if ctl is not None else CONTROL_DEFAULTS))
         top_k, temp = st.top_k, st.temperature
-        sp = lm.sampling(eos, 50, limit, top_k, temp, seed) if min(limits) == limit else lm.sampling(eos, 50, limit, top_k, temp, seed, limits=limits)
+        if queue or min(limits) < limit:   # a refill writes its newcomer's cap into the per-slot limits
+            sp = lm.sampling(eos, 50, limit, top_k, temp, seed, limits=limits[:B])
+        else:
+            sp = lm.sampling(eos, 50, limit, top_k, temp, seed)
         st.apply(lm, B)   # before the prefill, on the same stream
         dev = lm.out_tokens.device
         cap = max(len(r) for r in refs) + limit
         hist = torch.zeros(B, cap + 1, dtype=torch.long, device=dev)          # column `cap` is a scratch slot for masked writes
-        for b, r in enumerate(refs):
-            hist[b, : len(r)] = torch.as_tensor(r, dtype=torch.long)
-        hlen = torch.tensor([len(r) for r in refs], dtype=torch.long, device=dev)
+        hlen = torch.zeros(B, dtype=torch.long, device=dev)
         absorbed = torch.zeros(B, dtype=torch.long, device=dev)                # generated tokens already looked at
         n_dec = [len(r) for r in refs]
-        fades = [_CrossFade(self.streaming_stride_samples) for _ in range(B)]
-        tail_done = [False] * B
-        lim_t = torch.tensor(limits, dtype=torch.long)
+        fades = [_CrossFade(self.streaming_stride_samples) for _ in range(N)]
+        tail_done = [False] * N
+        occ = list(range(B))   # utterance held by each slot; None once its tail is out and nobody waits
+        nxt = B                # next utterance to admit
+
+        def seat(slots, idx):
+            """history rows of ``slots`` := the reference codes of utterances ``idx``, nothing absorbed yet"""
+            rows = torch.zeros(len(slots), max(len(refs[i]) for i in idx), dtype=torch.long)
+            for r, i in enumerate(idx):
+                rows[r, : len(refs[i])] = torch.as_tensor(refs[i], dtype=torch.long)
+            sl = torch.tensor(slots, device=dev)
+            hist[sl, : rows.shape[1]] = rows.to(dev)
+            hlen[sl] = torch.tensor([len(refs[i]) for i in idx], device=dev)
+            absorbed[sl] = 0
 
         def absorb(lo: int, hi: int):
             """tokens [lo, hi) of every slot -> history (non-speech ids dropped, as the reference's regex does)"""
+            hi = min(hi, lm.out_tokens.shape[1])   # a slot that stopped at max_new may lead the round's bound
             if hi <= lo:
                 return
             ngen = lm.n_generated[:B].long()
@@ -630,60 +670,88 @@ class NeuTTS:
                         out.setdefault(b, []).append(wav[max(s0, 0):] if s1 is None else wav[s0:s1])
             return out
 
-        lm.prefill(prompts, sp)             # samples the first token of every slot
-        lo, hi = 0, 1
-        while True:
-            absorb(lo, hi)
-            st = torch.stack((lm.n_generated[:B].long(), lm.done[:B].long(), hlen)).cpu()   # the round's one D2H read
-            ngen_h, done_h, hlen_h = st[0], st[1], st[2]
-            finished = [bool(done_h[b]) or int(ngen_h[b]) >= limits[b] for b in range(B)]
-            jobs = []
-            for b in range(B):
-                while int(hlen_h[b]) - n_dec[b] >= F + LA:
-                    t0 = max(n_dec[b] - LB - OV, 0)
-                    # the reference slices up to n_dec + F + LA + OV, but tokens arrive one at a time there, so
-                    # its cache never holds more than n_dec + F + LA entries when a chunk fires (:401-415)
-                    t1 = n_dec[b] + F + LA
-                    s0 = (n_dec[b] - t0) * hop
-                    jobs.append((b, t0, t1, s0, s0 + (F + 2 * OV) * hop))
-                    n_dec[b] += F
-            out = [None] * B
-            if jobs:
-                for b, wavs in decode_windows(jobs).items():
-                    out[b] = np.concatenate([fades[b].push(w) for w in wavs])
-            # ragged tail of a slot that finished (neutts/neutts.py:443-465), once its regular chunks are out
-            tails = []
-            all_finished = all(finished)
-            for b in range(B):
-                if finished[b] and not tail_done[b] and (all_finished or out[b] is None):
-                    tail_done[b] = True
-                    n = int(hlen_h[b])
-                    if n > n_dec[b]:
-                        rem = n - n_dec[b]
-                        t0 = max(n - (LB + OV + rem), 0)
-                        tails.append((b, t0, n, (n - t0 - rem - OV) * hop, None))
-                    elif fades[b].acc.shape[0]:
-                        flush = fades[b].push(np.zeros(0, np.float32), final=True)
-                        out[b] = flush if out[b] is None else np.concatenate((out[b], flush))
-            if all_finished and any(o is not None for o in out) and tails:
-                yield out                    # regular chunks first: a tail is its own yield, as in the reference
-                out = [None] * B
-            if tails:
-                for b, wavs in decode_windows(tails).items():
-                    t = fades[b].push(wavs[0], final=True)
-                    out[b] = t if out[b] is None else np.concatenate((out[b], t))
-            if any(o is not None for o in out):
-                yield out
-            if all_finished:
-                break
-            # decode just enough steps for the next chunk of the most advanced unfinished slot to fire (non-speech
-            # ids may make it take another pass); finished slots idle inside the kernel
-            need = min(F + LA - (int(hlen_h[b]) - n_dec[b]) for b in range(B) if not finished[b])
-            room = min(limits[b] - int(ngen_h[b]) for b in range(B) if not finished[b])
-            steps = max(1, min(need, room))
-            lo = min(int(ngen_h[b]) for b in range(B) if not finished[b])   # finished slots were absorbed completely above
-            lm.decode(steps, sp)
-            hi = int(ngen_h.max()) + steps
+        seat(list(range(B)), list(range(B)))
+        try:
+            lm.prefill(prompts[:B], sp)             # samples the first token of every slot
+            lo, hi = 0, 1
+            while True:
+                absorb(lo, hi)
+                rd = torch.stack((lm.n_generated[:B].long(), lm.done[:B].long(), hlen)).cpu()   # the round's one D2H read
+                ngen_h, done_h, hlen_h = rd[0].tolist(), rd[1].tolist(), rd[2].tolist()
+                held = [b for b in range(B) if occ[b] is not None]
+                finished = {b: bool(done_h[b]) or ngen_h[b] >= limits[occ[b]] for b in held}
+                jobs = []
+                for b in held:
+                    u = occ[b]
+                    while hlen_h[b] - n_dec[u] >= F + LA:
+                        t0 = max(n_dec[u] - LB - OV, 0)
+                        # the reference slices up to n_dec + F + LA + OV, but tokens arrive one at a time there, so
+                        # its cache never holds more than n_dec + F + LA entries when a chunk fires (:401-415)
+                        t1 = n_dec[u] + F + LA
+                        s0 = (n_dec[u] - t0) * hop
+                        jobs.append((b, t0, t1, s0, s0 + (F + 2 * OV) * hop))
+                        n_dec[u] += F
+                out = [None] * N
+                if jobs:
+                    for b, wavs in decode_windows(jobs).items():
+                        out[occ[b]] = np.concatenate([fades[occ[b]].push(w) for w in wavs])
+                # ragged tail of an utterance that finished (neutts/neutts.py:443-465), once its regular chunks are out
+                tails = []
+                all_finished = nxt == N and all(finished.values())
+                for b in held:
+                    u = occ[b]
+                    if finished[b] and not tail_done[u] and (all_finished or out[u] is None):
+                        tail_done[u] = True
+                        n = hlen_h[b]
+                        if n > n_dec[u]:
+                            rem = n - n_dec[u]
+                            t0 = max(n - (LB + OV + rem), 0)
+                            tails.append((b, t0, n, (n - t0 - rem - OV) * hop, None))
+                        elif fades[u].acc.shape[0]:
+                            flush = fades[u].push(np.zeros(0, np.float32), final=True)
+                            out[u] = flush if out[u] is None else np.concatenate((out[u], flush))
+                if all_finished and any(o is not None for o in out) and tails:
+                    yield out                    # regular chunks first: a tail is its own yield, as in the reference
+                    out = [None] * N
+                if tails:
+                    for b, wavs in decode_windows(tails).items():
+                        t = fades[occ[b]].push(wavs[0], final=True)
+                        out[occ[b]] = t if out[occ[b]] is None else np.concatenate((out[occ[b]], t))
+                if any(o is not None for o in out):
+                    yield out
+                if all_finished:
+                    break
+                # refill every slot whose utterance's tail is out (its history row has been read), FIFO
+                new = []
+                for b in held:
+                    if tail_done[occ[b]]:
+                        occ[b] = None
+                        if nxt < N:
+                            occ[b], nxt = nxt, nxt + 1
+                            new.append(b)
+                if new:
+                    idx = [occ[b] for b in new]
+                    st.admit(lm, new, idx)   # before their prefill, on the same stream
+                    seat(new, idx)
+                    lm.prefill_slots(new, [prompts[i] for i in idx], sp, stream_ids=idx, limits=[limits[i] for i in idx])
+                    for b, i in zip(new, idx):
+                        ngen_h[b], hlen_h[b], finished[b] = 1, len(refs[i]), False
+                # decode just enough steps for the next chunk of the most advanced unfinished stream to fire (non-speech
+                # ids may make it take another pass), and no further than the earliest cap-driven completion; finished
+                # slots idle inside the kernel.  A newcomer's first token is not in its history yet.
+                live = [b for b in range(B) if occ[b] is not None and not finished[b]]
+                steps = 0
+                if live and not any(limits[occ[b]] <= 1 for b in new):   # a cap of 1 ends inside the prefill: read first
+                    need = min(F + LA - (hlen_h[b] + (b in new) - n_dec[occ[b]]) for b in live)
+                    room = min(limits[occ[b]] - ngen_h[b] for b in live)
+                    steps = max(1, min(need, room))
+                    lm.decode(steps, sp)
+                # every slot's tokens up to its last read count are in its history; a newcomer's start at 0
+                lo = min((0 if b in new else ngen_h[b] for b in live), default=0)
+                hi = max(ngen_h) + steps
+        finally:
+            if queue:
+                lm.release_pages()   # also when the consumer stops early (generator close)
 
     def encode_reference(self, ref_audio_path):
         """wav -> NeuCodec codes (``neutts/neutts.py:266-271``).  The encoder is outside the hot path; this
