@@ -358,8 +358,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     const int split_cap = P.split_cap;
     constexpr bool fold_cta = FOLD;   // batch <= 4: consumers fold the split-K slices themselves (no fold phases, no barriers)
     const int I = P.inter;
-    float* xf = reinterpret_cast<float*>(uni + 14 * CHUNK);   // fold_in_cta: fp32 folded rows [B][H] behind the B chunks
-    float* xw = xf + 4096;                                      // ... and the RMSNorm weight row [H] (H <= 1024)
     const int AW = P.att_warps;
     uint8_t* att = smem + P.att_off;
     auto att_k = [&](int w) { return reinterpret_cast<__nv_bfloat16*>(att + static_cast<size_t>(w) * 8192); };
@@ -498,72 +496,58 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
       }
     };
 
-    // ---- batch <= 4: fold ALL rows in this CTA (residual pairs + slices, slice order), normalise, stage the B chunks
-    //      of phase `ph` (-1: every k-block).  The designated CTA publishes the folded stream for the next fold.
+    // ---- batch 1: fold the row in this CTA (residual pairs + slices, slice order), normalise, stage the B chunks of
+    //      phase `ph` (-1: every k-block).  Thread q < H / 4 keeps elements 4q .. 4q + 3 in registers from the fold to
+    //      the staging and the write-back, so no fp32 copy of the row takes shared memory away from the weight ring.
+    //      The designated CTA publishes the folded stream for the next fold.
     auto fold_stage = [&](const float2* parts, int nparts, int pstamp, int rows, const float* norm_w, int ph, bool writer) {
-      const float2* hsrc = P.h2 + static_cast<long long>(fold_no & 1) * B * H;
+      const float2* hsrc = P.h2 + static_cast<long long>(fold_no & 1) * H;
       const int hstamp = P.hstamp_base + fold_no;
-      const int nq = H >> 2;
+      const int i4 = tid * 4;
+      const bool mine = i4 < H;   // H <= 4 * kConsumerThreads (tc_fold_in_cta)
       pm(1);
-      float ssb[4] = {0.f, 0.f, 0.f, 0.f};   // this thread's share of every row's sum of squares
-#pragma unroll
-      for (int b = 0; b < 4; ++b) {
-        if (b < B) {
-          for (int q = tid; q < nq; q += kConsumerThreads) {
-            const int i4 = q * 4;
-            float acc[4];
-            const float4 nw = __ldg(reinterpret_cast<const float4*>(norm_w + i4));   // in flight together with the slices
-            tc_fold4(hsrc, hstamp, parts, nparts, pstamp, rows, B, H, b, i4, acc);
-            *reinterpret_cast<float4*>(xf + b * H + i4) = make_float4(acc[0], acc[1], acc[2], acc[3]);
-            if (b == 0) *reinterpret_cast<float4*>(xw + i4) = nw;
-            ssb[b] += (acc[0] * acc[0] + acc[1] * acc[1]) + (acc[2] * acc[2] + acc[3] * acc[3]);
-          }
-        }
+      float acc[4] = {0.f, 0.f, 0.f, 0.f};
+      float4 nw = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (mine) {
+        nw = __ldg(reinterpret_cast<const float4*>(norm_w + i4));   // in flight together with the slices
+        tc_fold4(hsrc, hstamp, parts, nparts, pstamp, rows, B, H, 0, i4, acc);
       }
       pm(2);
+      const float ss = warp_sum((acc[0] * acc[0] + acc[1] * acc[1]) + (acc[2] * acc[2] + acc[3] * acc[3]));
+      if (lane == 0) ms->red[warp] = ss;
+      csync();   // also: the B chunks of the previous phase are free (see stage_attn)
+      float t = 0.f;
 #pragma unroll
-      for (int b = 0; b < 4; ++b) {
-        if (b < B) {
-          const float t = warp_sum(ssb[b]);
-          if (lane == 0) ms->red[b * kConsumerWarps + warp] = t;
+      for (int w = 0; w < kConsumerWarps; ++w) t += ms->red[w];   // fixed order: every CTA gets the same bits
+      const float rstd = rsqrtf(t / static_cast<float>(H) + P.eps);
+      if (mine) {
+        const float xn[4] = {nw.x * (acc[0] * rstd), nw.y * (acc[1] * rstd), nw.z * (acc[2] * rstd), nw.w * (acc[3] * rstd)};
+        __nv_bfloat16 hi[4], lo[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) split_hilo(xn[j], hi[j], lo[j]);
+        const uint2 vhi = make_uint2(pack2(hi[0], hi[1]), pack2(hi[2], hi[3])), vlo = make_uint2(pack2(lo[0], lo[1]), pack2(lo[2], lo[3]));
+        const int kb = i4 >> 6, k4 = i4 & 63;   // 4 consecutive k of one row: one 8-byte run of a 16-byte swizzle group
+        auto put = [&](int c) {
+          uint8_t* cb = uni + c * CHUNK;
+          *reinterpret_cast<uint2*>(chunk_elem(cb, 0, k4)) = vhi;
+          *reinterpret_cast<uint2*>(chunk_elem(cb, 8, k4)) = vlo;
+        };
+        if (ph < 0) {
+          put(kb);
+        } else {   // every chunk that holds k-block kb (two items of one K slice stage it twice)
+          const int nch = ms->bchunks[ph];
+          for (int c = 0; c < nch; ++c)
+            if (ms->ckb[ph][c] == kb) put(c);
         }
-      }
-      csync();
-      float rs[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-      for (int b = 0; b < 4; ++b) {
-        if (b < B) {
-          float t = 0.f;
-#pragma unroll
-          for (int w = 0; w < kConsumerWarps; ++w) t += ms->red[b * kConsumerWarps + w];   // fixed order: every CTA gets the same bits
-          rs[b] = rsqrtf(t / static_cast<float>(H) + P.eps);
-        }
-      }
-      const int nch = ph < 0 ? KBH : ms->bchunks[ph];
-      const int per = B * 64;
-      for (int e = tid; e < nch * per; e += kConsumerThreads) {
-        const int c = e / per, r = e - c * per, b = r >> 6, k = r & 63;
-        const int i = (ph < 0 ? c : ms->ckb[ph][c]) * 64 + k;
-        const float rstd = b == 0 ? rs[0] : (b == 1 ? rs[1] : (b == 2 ? rs[2] : rs[3]));
-        const float xn = xw[i] * (xf[b * H + i] * rstd);
-        __nv_bfloat16 hi, lo;
-        split_hilo(xn, hi, lo);
-        uint8_t* cb = uni + c * CHUNK;
-        *chunk_elem(cb, b, k) = hi;
-        *chunk_elem(cb, 8 + b, k) = lo;
       }
       pm(4);
       bop_ready();
       pm(5);
-      if (writer) {
-        float2* hdst = P.h2 + static_cast<long long>((fold_no + 1) & 1) * B * H;
+      if (writer && mine) {
+        float4* d = reinterpret_cast<float4*>(P.h2 + static_cast<long long>((fold_no + 1) & 1) * H + i4);
         const float sf = __int_as_float(hstamp + 1);
-        for (int q = tid; q < B * nq; q += kConsumerThreads) {
-          const float4 v = *reinterpret_cast<const float4*>(xf + q * 4);
-          float4* d = reinterpret_cast<float4*>(hdst + q * 4);
-          d[0] = make_float4(v.x, sf, v.y, sf);
-          d[1] = make_float4(v.z, sf, v.w, sf);
-        }
+        d[0] = make_float4(acc[0], sf, acc[1], sf);
+        d[1] = make_float4(acc[2], sf, acc[3], sf);
       }
       ++fold_no;
     };
@@ -1144,10 +1128,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
 }
 
 // ------------------------------------------------------------------------------------------ host side
-static size_t tc_chunk_bytes(int nt) {   // B chunks (+ fold_in_cta: fp32 rows and the norm weights), 1024-aligned
-  const size_t u = size_t(14) * nt * 128 + (nt == 16 ? 20 * 1024 : 0);
-  return (u + 1023) & ~size_t(1023);
-}
+static size_t tc_chunk_bytes(int nt) { return size_t(14) * nt * 128; }   // the B chunks (a multiple of 1024 bytes)
 static size_t tc_attn_bytes(int aw) { return (tc_attn_layout_bytes(aw) + 1023) & ~size_t(1023); }
 
 bool tc_fold_in_cta(int B, int hidden) {
