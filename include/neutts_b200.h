@@ -349,8 +349,24 @@ size_t nt_codec_workspace_bytes(const nt_codec_config* cfg);
 int nt_codec_create(const nt_codec_config* cfg, const nt_codec_weights* w, void* workspace, size_t workspace_bytes,
                     nt_codec** out);
 int nt_codec_destroy(nt_codec* c);
-/* codes: device int32 [B][N] (all items the same length N); pcm: device f32 [B][hop*N]. */
+/* codes: device int32 [B][N] (all items the same length N); pcm: device f32 [B][hop*N].  Every int32 id decodes as
+ * id mod fsq_levels**fsq_dims (floor modulo: -1 is the last code). */
 int nt_codec_decode(nt_codec* c, const int32_t* codes, int B, int N, float* pcm, void* stream);
+/* Per-stage parity hooks (tests).  Later nt_codec_decode calls run only stages first..last (last = -1: through the
+ * last stage; (0, -1), the default, runs them all).  Stages in launch order:
+ *   0 fsq (codes -> x0, after the memsets of x0, x1, x2)   1 embed (conv k7, x0 -> x1)
+ *   per resnet block (2 before the transformer blocks, 2 after), 4 each:
+ *     gn1 (x1 -> x2) | conv1 (x2 -> x3) | gn2 (x3 -> x2) | conv2 (x2 + x1 -> x1)
+ *   per transformer block, 8 each (7 when rope_time_axis = 0, which has no rope stage):
+ *     norm1 (x1 -> xn) | qkv (xn -> qkv) | rope (qkv in place) | attn (qkv -> att) | proj (att + x1 -> x1) |
+ *     norm2 (x1 -> xn) | fc1 + SiLU (xn -> hbuf) | fc2 (hbuf + x1 -> x1)
+ *   final LN (x1 -> xn) | head (xn -> sp) | spec (sp in place) | idft (sp -> fr) | ola (fr -> pcm)
+ * A 3xTF32 GEMM's operand split belongs to its stage.  A call that starts past stage 0 reads the buffers as the
+ * previous call (or the caller) left them.  A range outside 0..n_stages-1 returns NT_ERR_INVALID.  nt_codec_debug_ptr
+ * looks up a workspace buffer by name ("x0", "x1", "x2", "x3", "xn", "qkv", "hbuf", "att", "sp", "fr"; NULL for any
+ * other name).  Activations are channels-last fp32 rows; item b, frame t sits at row b*(N+6) + 3 + t. */
+int nt_codec_debug_set_stages(nt_codec* c, int first, int last);
+void* nt_codec_debug_ptr(nt_codec* c, const char* name);
 
 /* ------------------------------------------------------------------------------------------
  * Single-op entry points (unit tests; each mirrors one row of SURVEY.md §8a)

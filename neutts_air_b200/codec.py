@@ -140,7 +140,8 @@ class CodecDecoder:
 
         Range validation needs the values on the host: it runs for CPU inputs (free) and is skipped for CUDA
         inputs unless ``validate=True`` (a min/max read-back is a device synchronisation inside the hot path;
-        the kernel itself never reads out of bounds on a bad id, it decodes the id modulo the codebook)."""
+        the kernel itself never reads out of bounds on a bad id, it decodes the id modulo the codebook, with a floor
+        modulo: -1 is the last code)."""
         if codes.dim() != 3 or codes.shape[1] != 1:
             raise ValueError("codes must be [B, 1, N]")
         B, _, N = codes.shape
@@ -156,6 +157,20 @@ class CodecDecoder:
             pcm = torch.empty(B, 1, self.shape.hop * N, dtype=torch.float32, device=self.device)
             _lib.check(self.L.nt_codec_decode(self.handle, c32.data_ptr(), B, N, pcm.data_ptr(), _lib.current_stream_ptr()))
         return pcm
+
+    # ------------------------------------------------------------------ per-stage parity hooks (tests)
+    def debug_set_stages(self, first: int = 0, last: int = -1) -> None:
+        """Later decodes run only stages ``first..last`` (``-1``: through the last) of the list in
+        include/neutts_b200.h (``nt_codec_debug_set_stages``); ``(0, -1)`` runs them all."""
+        _lib.check(self.L.nt_codec_debug_set_stages(self.handle, first, last))
+
+    def debug_buffer(self, name: str, shape) -> torch.Tensor:
+        """fp32 view of a workspace buffer ("x0" .. "fr", see ``nt_codec_debug_ptr``; lives inside ``self.workspace``)."""
+        ptr = self.L.nt_codec_debug_ptr(self.handle, name.encode())
+        if not ptr:
+            raise KeyError(name)
+        off = ptr - self.workspace.data_ptr()
+        return self.workspace[off: off + 4 * math.prod(shape)].view(torch.float32).view(*shape)
 
     def encode_code(self, audio_or_path):
         """The encoder half (wav -> codes, ``neutts/neutts.py:266-271``) is outside the hot path (SURVEY.md §2:

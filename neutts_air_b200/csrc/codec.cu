@@ -30,9 +30,11 @@ __global__ void __launch_bounds__(256) fsq_embed_kernel(const int32_t* codes, in
   int code = codes[bt];
   float z[16];
   const float half = static_cast<float>(levels / 2);
-  for (int i = 0; i < dims; ++i) {
-    z[i] = (static_cast<float>(code % levels) - half) / half;
+  for (int i = 0; i < dims; ++i) {   // floor division and modulo: every int32 id decodes as id mod levels**dims
+    int d = code % levels;
     code /= levels;
+    if (d < 0) d += levels, code -= 1;
+    z[i] = (static_cast<float>(d) - half) / half;
   }
   float* o = out + (static_cast<long long>(b) * Tp + 3 + t) * C;
   for (int c = threadIdx.x; c < C; c += 256) {
@@ -287,7 +289,13 @@ struct nt_codec {
   SplitW s_head, s_idft, s_embed;
   std::vector<SplitW> s_rn[2], s_blk[4];   // resnet conv1 / conv2; wqkv, wproj, fc1, fc2
   float* a_split = nullptr;   // hi half, then the lo half a_rows rows further down (placed per GEMM)
+  int dbg_first = 0, dbg_last = -1;   // nt_codec_debug_set_stages: stages nt_codec_decode runs (-1 = through the last)
 };
+
+// Stages of nt_codec_decode in launch order (nt_codec_debug_set_stages): fsq (+ the memsets of x0, x1, x2), embed,
+// 4 per resnet block (gn1, conv1, gn2, conv2) for the 2 prior ones, 8 per transformer block (norm1, qkv, rope, attn,
+// proj, norm2, fc1, fc2; 7 without rope), 4 per post resnet block, then final LN, head, spec, idft, ola.
+static int codec_stage_count(const nt_codec_config& c) { return 2 + 4 * 4 + c.depth * (c.rope_time_axis ? 8 : 7) + 5; }
 
 static int codec_check(const nt_codec_config* c) {
   if (!c) return set_error(NT_ERR_INVALID, "null codec config");
@@ -421,6 +429,10 @@ struct CodecRun {
   nt_codec* k;
   int B, N, Tp, rows, C;
   cudaStream_t s;
+  int stage;               // index of the next stage
+  int first;               // first stage to run
+  unsigned span;           // stages first..first+span run
+  bool on() { return static_cast<unsigned>(stage++ - first) <= span; }
 
   // masked GEMM on the padded layout: out rows r+3 for r with (r % Tp) < N.
   // A points at the first row the tap window of output row 0 touches.
@@ -450,15 +462,19 @@ struct CodecRun {
     const nt_codec_config& c = k->cfg;
     const int cpg = C / c.groups;
     int rc;
-    if ((rc = launch_kernel(groupnorm_swish_kernel, dim3(c.groups, B), dim3(256), 0, s, true, (const float*)k->x1, N, Tp, C, cpg,
-                            c.norm_eps, k->rn[0][idx], k->rn[1][idx], k->x2)))
+    if (on() && (rc = launch_kernel(groupnorm_swish_kernel, dim3(c.groups, B), dim3(256), 0, s, true, (const float*)k->x1, N, Tp, C,
+                                    cpg, c.norm_eps, k->rn[0][idx], k->rn[1][idx], k->x2)))
       return rc;
-    if ((rc = gemm(k->x2 + 2 * C, 3 * C, C, k->rn[2][idx], k->rn[3][idx], nullptr, NT_ACT_NONE, k->x3 + 3 * C, C, C, true, sp(k->s_rn[0], idx))))
+    if (on() && (rc = gemm(k->x2 + 2 * C, 3 * C, C, k->rn[2][idx], k->rn[3][idx], nullptr, NT_ACT_NONE, k->x3 + 3 * C, C, C, true,
+                           sp(k->s_rn[0], idx))))
       return rc;
-    if ((rc = launch_kernel(groupnorm_swish_kernel, dim3(c.groups, B), dim3(256), 0, s, true, (const float*)k->x3, N, Tp, C, cpg,
-                            c.norm_eps, k->rn[4][idx], k->rn[5][idx], k->x2)))
+    if (on() && (rc = launch_kernel(groupnorm_swish_kernel, dim3(c.groups, B), dim3(256), 0, s, true, (const float*)k->x3, N, Tp, C,
+                                    cpg, c.norm_eps, k->rn[4][idx], k->rn[5][idx], k->x2)))
       return rc;
-    return gemm(k->x2 + 2 * C, 3 * C, C, k->rn[6][idx], k->rn[7][idx], k->x1 + 3 * C, NT_ACT_NONE, k->x1 + 3 * C, C, C, true, sp(k->s_rn[1], idx));
+    if (on() && (rc = gemm(k->x2 + 2 * C, 3 * C, C, k->rn[6][idx], k->rn[7][idx], k->x1 + 3 * C, NT_ACT_NONE, k->x1 + 3 * C, C, C,
+                           true, sp(k->s_rn[1], idx))))
+      return rc;
+    return NT_OK;
   }
 };
 }  // namespace
@@ -470,57 +486,86 @@ extern "C" int nt_codec_decode(nt_codec* k, const int32_t* codes, int B, int N, 
   if (N < 1 || N > c.max_frames) return set_error(NT_ERR_INVALID, "codec frames %d not in 1..%d", N, c.max_frames);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
   const int C = c.hidden, Tp = N + 6, rows = B * Tp;
-  CodecRun r{k, B, N, Tp, rows, C, s};
+  const int last = k->dbg_last >= 0 ? k->dbg_last : codec_stage_count(c) - 1;
+  CodecRun r{k, B, N, Tp, rows, C, s, 0, k->dbg_first, static_cast<unsigned>(last - k->dbg_first)};
   int rc;
-  const size_t act_bytes = size_t(rows + 8) * C * sizeof(float);
-  NT_CUDA_CHECK(cudaMemsetAsync(k->x0, 0, act_bytes, s));
-  NT_CUDA_CHECK(cudaMemsetAsync(k->x1, 0, act_bytes, s));
-  NT_CUDA_CHECK(cudaMemsetAsync(k->x2, 0, act_bytes, s));
 
-  // B1+B2
-  if ((rc = launch_kernel(fsq_embed_kernel, dim3(B * N), dim3(256), 0, s, true, codes, N, Tp, C, c.fsq_levels, c.fsq_dims,
-                          k->w.fsq_w, k->w.fsq_b, k->x0)))
-    return rc;
+  // B1+B2 (the memsets zero the pad rows every conv's "same" padding reads)
+  if (r.on()) {
+    const size_t act_bytes = size_t(rows + 8) * C * sizeof(float);
+    NT_CUDA_CHECK(cudaMemsetAsync(k->x0, 0, act_bytes, s));
+    NT_CUDA_CHECK(cudaMemsetAsync(k->x1, 0, act_bytes, s));
+    NT_CUDA_CHECK(cudaMemsetAsync(k->x2, 0, act_bytes, s));
+    if ((rc = launch_kernel(fsq_embed_kernel, dim3(B * N), dim3(256), 0, s, true, codes, N, Tp, C, c.fsq_levels, c.fsq_dims,
+                            k->w.fsq_w, k->w.fsq_b, k->x0)))
+      return rc;
+  }
   // B3: Conv1d k=7 pad=3
-  if ((rc = r.gemm(k->x0, 7 * C, C, k->w.embed_w, k->w.embed_b, nullptr, NT_ACT_NONE, k->x1 + 3 * C, C, C, true, &k->s_embed))) return rc;
+  if (r.on() && (rc = r.gemm(k->x0, 7 * C, C, k->w.embed_w, k->w.embed_b, nullptr, NT_ACT_NONE, k->x1 + 3 * C, C, C, true, &k->s_embed)))
+    return rc;
   // B4: prior_net
   for (int i = 0; i < 2; ++i)
     if ((rc = r.resnet(i))) return rc;
   // B5: transformer blocks
   const float scale_log2 = 0.125f * 1.4426950408889634f;
   for (int l = 0; l < c.depth; ++l) {
-    if ((rc = launch_kernel(rownorm_kernel, dim3((rows + 7) / 8), dim3(256), 0, s, true, (const float*)k->x1, rows, C, c.norm_eps,
-                            k->blk[0][l], (const float*)nullptr, 0, k->xn)))
+    if (r.on() && (rc = launch_kernel(rownorm_kernel, dim3((rows + 7) / 8), dim3(256), 0, s, true, (const float*)k->x1, rows, C,
+                                      c.norm_eps, k->blk[0][l], (const float*)nullptr, 0, k->xn)))
       return rc;
-    if ((rc = r.gemm(k->xn, C, C, k->blk[1][l], nullptr, nullptr, NT_ACT_NONE, k->qkv, 3 * C, 3 * C, false, r.sp(k->s_blk[0], l)))) return rc;
-    if (c.rope_time_axis)
-      if ((rc = launch_kernel(codec_rope_kernel, dim3(B * N), dim3(256), 0, s, true, k->qkv, N, Tp, C, c.heads, (const float*)k->inv_freq)))
-        return rc;
-    if ((rc = launch_kernel(codec_attn_kernel, dim3((N + 127) / 128, c.heads, B), dim3(128), 0, s, true, (const float*)k->qkv, N, Tp, C,
-                            scale_log2, k->att)))
+    if (r.on() && (rc = r.gemm(k->xn, C, C, k->blk[1][l], nullptr, nullptr, NT_ACT_NONE, k->qkv, 3 * C, 3 * C, false, r.sp(k->s_blk[0], l))))
       return rc;
-    if ((rc = r.gemm(k->att + 3 * C, C, C, k->blk[2][l], nullptr, k->x1 + 3 * C, NT_ACT_NONE, k->x1 + 3 * C, C, C, true, r.sp(k->s_blk[1], l))))
+    if (c.rope_time_axis && r.on() &&
+        (rc = launch_kernel(codec_rope_kernel, dim3(B * N), dim3(256), 0, s, true, k->qkv, N, Tp, C, c.heads, (const float*)k->inv_freq)))
       return rc;
-    if ((rc = launch_kernel(rownorm_kernel, dim3((rows + 7) / 8), dim3(256), 0, s, true, (const float*)k->x1, rows, C, c.norm_eps,
-                            k->blk[3][l], (const float*)nullptr, 0, k->xn)))
+    if (r.on() && (rc = launch_kernel(codec_attn_kernel, dim3((N + 127) / 128, c.heads, B), dim3(128), 0, s, true, (const float*)k->qkv,
+                                      N, Tp, C, scale_log2, k->att)))
       return rc;
-    if ((rc = r.gemm(k->xn, C, C, k->blk[4][l], nullptr, nullptr, NT_ACT_SILU, k->hbuf, c.mlp_hidden, c.mlp_hidden, false, r.sp(k->s_blk[2], l))))
+    if (r.on() && (rc = r.gemm(k->att + 3 * C, C, C, k->blk[2][l], nullptr, k->x1 + 3 * C, NT_ACT_NONE, k->x1 + 3 * C, C, C, true,
+                               r.sp(k->s_blk[1], l))))
       return rc;
-    if ((rc = r.gemm(k->hbuf + 3 * size_t(c.mlp_hidden), c.mlp_hidden, c.mlp_hidden, k->blk[5][l], nullptr, k->x1 + 3 * C, NT_ACT_NONE,
-                     k->x1 + 3 * C, C, C, true, r.sp(k->s_blk[3], l))))
+    if (r.on() && (rc = launch_kernel(rownorm_kernel, dim3((rows + 7) / 8), dim3(256), 0, s, true, (const float*)k->x1, rows, C,
+                                      c.norm_eps, k->blk[3][l], (const float*)nullptr, 0, k->xn)))
+      return rc;
+    if (r.on() && (rc = r.gemm(k->xn, C, C, k->blk[4][l], nullptr, nullptr, NT_ACT_SILU, k->hbuf, c.mlp_hidden, c.mlp_hidden, false,
+                               r.sp(k->s_blk[2], l))))
+      return rc;
+    if (r.on() && (rc = r.gemm(k->hbuf + 3 * size_t(c.mlp_hidden), c.mlp_hidden, c.mlp_hidden, k->blk[5][l], nullptr, k->x1 + 3 * C,
+                               NT_ACT_NONE, k->x1 + 3 * C, C, C, true, r.sp(k->s_blk[3], l))))
       return rc;
   }
   // post_net
   for (int i = 2; i < 4; ++i)
     if ((rc = r.resnet(i))) return rc;
   // B6: final LayerNorm, head, spectrum
-  if ((rc = launch_kernel(rownorm_kernel, dim3((rows + 7) / 8), dim3(256), 0, s, true, (const float*)k->x1, rows, C, c.norm_eps,
-                          k->w.final_ln_w, k->w.final_ln_b, 1, k->xn)))
+  if (r.on() && (rc = launch_kernel(rownorm_kernel, dim3((rows + 7) / 8), dim3(256), 0, s, true, (const float*)k->x1, rows, C, c.norm_eps,
+                                    k->w.final_ln_w, k->w.final_ln_b, 1, k->xn)))
     return rc;
   const int nb = c.n_fft / 2 + 1, kp = k->kpad;
-  if ((rc = r.gemm(k->xn, C, C, k->w.head_w, k->w.head_b, nullptr, NT_ACT_NONE, k->sp, kp, 2 * nb, false, &k->s_head))) return rc;
-  if ((rc = launch_kernel(spec_kernel, dim3(rows), dim3(256), 0, s, true, k->sp, (long long)kp, nb, c.mag_clip))) return rc;
+  if (r.on() && (rc = r.gemm(k->xn, C, C, k->w.head_w, k->w.head_b, nullptr, NT_ACT_NONE, k->sp, kp, 2 * nb, false, &k->s_head))) return rc;
+  if (r.on() && (rc = launch_kernel(spec_kernel, dim3(rows), dim3(256), 0, s, true, k->sp, (long long)kp, nb, c.mag_clip))) return rc;
   // B7: inverse rDFT (windowed basis) as a GEMM, then overlap-add
-  if ((rc = r.gemm(k->sp, 2 * nb, kp, k->w.idft_basis, nullptr, nullptr, NT_ACT_NONE, k->fr, c.n_fft, c.n_fft, false, &k->s_idft, kp))) return rc;
-  return launch_kernel(ola_kernel, dim3((c.hop * N + 255) / 256, B), dim3(256), 0, s, true, (const float*)k->fr, N, Tp, c.n_fft, c.hop, pcm);
+  if (r.on() && (rc = r.gemm(k->sp, 2 * nb, kp, k->w.idft_basis, nullptr, nullptr, NT_ACT_NONE, k->fr, c.n_fft, c.n_fft, false, &k->s_idft, kp)))
+    return rc;
+  if (r.on() && (rc = launch_kernel(ola_kernel, dim3((c.hop * N + 255) / 256, B), dim3(256), 0, s, true, (const float*)k->fr, N, Tp, c.n_fft,
+                                    c.hop, pcm)))
+    return rc;
+  return NT_OK;
+}
+
+extern "C" int nt_codec_debug_set_stages(nt_codec* k, int first, int last) {
+  if (!k) return set_error(NT_ERR_INVALID, "nt_codec_debug_set_stages: null handle");
+  const int n = codec_stage_count(k->cfg);
+  if (first < 0 || first >= n || last < -1 || last >= n || (last >= 0 && last < first))
+    return set_error(NT_ERR_INVALID, "nt_codec_debug_set_stages: range %d..%d not within the %d stages", first, last, n);
+  k->dbg_first = first, k->dbg_last = last;
+  return NT_OK;
+}
+
+extern "C" void* nt_codec_debug_ptr(nt_codec* k, const char* name) {
+  if (!k || !name) return nullptr;
+  const struct { const char* n; void* p; } tab[] = {{"x0", k->x0}, {"x1", k->x1},     {"x2", k->x2},   {"x3", k->x3}, {"xn", k->xn},
+                                                     {"qkv", k->qkv}, {"hbuf", k->hbuf}, {"att", k->att}, {"sp", k->sp}, {"fr", k->fr}};
+  for (const auto& e : tab)
+    if (!strcmp(e.n, name)) return e.p;
+  return nullptr;
 }

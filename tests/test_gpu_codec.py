@@ -2,7 +2,8 @@
 
 Bar (BASELINE.json north_star): PCM within 1e-3 RMS of the fp32 reference path.  The oracle is
 "parity unpinned" at the reference boundary (neucodec is not available offline) — these tests pin
-the CUDA path to the restatement, stage by stage and end to end."""
+the CUDA path to the restatement end to end.  tests/test_gpu_codec_stages.py checks every stage on its
+own inputs against float64, in every precision mode."""
 import pytest
 import torch
 
