@@ -37,6 +37,9 @@ class LMShape:
 
     @staticmethod
     def from_hf_config(cfg: dict) -> "LMShape":
+        """The shape a transformers config.json describes, read as transformers' Qwen2 / Llama / Mistral config classes
+        read it: ``rope_theta`` from ``rope_parameters`` (transformers 5) or the top level (transformers 4), else
+        10 000; ``tie_word_embeddings`` false when absent (the checkpoint's tensors may still tie: loader.py)."""
         rope = cfg.get("rope_theta")
         if rope is None and isinstance(cfg.get("rope_parameters"), dict):
             rope = cfg["rope_parameters"].get("rope_theta")
@@ -44,10 +47,10 @@ class LMShape:
         return LMShape(
             vocab_size=cfg["vocab_size"], hidden_size=cfg["hidden_size"], intermediate_size=cfg["intermediate_size"],
             num_layers=cfg["num_hidden_layers"], num_heads=heads,
-            num_kv_heads=cfg.get("num_key_value_heads", heads),
+            num_kv_heads=cfg.get("num_key_value_heads") or heads,
             head_dim=cfg.get("head_dim") or cfg["hidden_size"] // heads,
-            rms_eps=cfg.get("rms_norm_eps", 1e-6), rope_theta=float(rope if rope is not None else 1e6),
-            tie_embeddings=bool(cfg.get("tie_word_embeddings", True)))
+            rms_eps=cfg.get("rms_norm_eps", 1e-6), rope_theta=float(rope if rope is not None else 1e4),
+            tie_embeddings=bool(cfg.get("tie_word_embeddings", False)))
 
 
 def _rope_pair_perm(n_heads: int) -> torch.Tensor:
@@ -56,9 +59,31 @@ def _rope_pair_perm(n_heads: int) -> torch.Tensor:
     return (torch.arange(n_heads)[:, None] * 64 + one[None, :]).reshape(-1)
 
 
+_LAYER_TENSORS = ("input_layernorm.weight", "post_attention_layernorm.weight", "self_attn.q_proj.weight",
+                  "self_attn.q_proj.bias", "self_attn.k_proj.weight", "self_attn.k_proj.bias", "self_attn.v_proj.weight",
+                  "self_attn.v_proj.bias", "self_attn.o_proj.weight", "mlp.gate_proj.weight", "mlp.up_proj.weight",
+                  "mlp.down_proj.weight")
+
+
+def check_tensors(shape: LMShape, sd: dict) -> None:
+    """Raises ValueError listing the names under ``model.`` and ``lm_head.`` that ``pack_weights`` would not read: an
+    o_proj or MLP bias, per-head q/k norms, a layer beyond ``num_layers``.  The kernels have no place for them, so a
+    checkpoint holding one describes a different model.  ``rotary_emb.inv_freq`` buffers (older .bin files) are
+    derived from the config and ignored."""
+    known = {"model.embed_tokens.weight", "model.norm.weight", "lm_head.weight"}
+    known.update(f"model.layers.{i}.{n}" for i in range(shape.num_layers) for n in _LAYER_TENSORS)
+    extra = sorted(k for k in sd if k.startswith(("model.", "lm_head.")) and k not in known
+                   and not k.endswith("rotary_emb.inv_freq"))
+    if extra:
+        raise ValueError(f"checkpoint tensors the speech-LM kernels do not implement: {', '.join(extra[:8])}"
+                         + (f" (+{len(extra) - 8} more)" if len(extra) > 8 else ""))
+
+
 def pack_weights(shape: LMShape, sd: dict, device) -> dict:
-    """HF Qwen2 state_dict (``model.layers.N.self_attn.q_proj.weight`` ...) -> the packed bf16/fp32
-    device tensors the kernels stream (layouts documented in include/neutts_b200.h)."""
+    """HF Qwen2 / Llama / Mistral state_dict (``model.layers.N.self_attn.q_proj.weight`` ...) -> the packed bf16/fp32
+    device tensors the kernels stream (layouts documented in include/neutts_b200.h).  Raises ValueError when the
+    state_dict holds a tensor the kernels would not use (``check_tensors``)."""
+    check_tensors(shape, sd)
     dev = torch.device(device)
     bf = lambda t: t.to(device=dev, dtype=torch.bfloat16).contiguous()
     f32 = lambda t: t.to(device=dev, dtype=torch.float32).contiguous()

@@ -1,8 +1,11 @@
 """Checkpoint readers (SURVEY.md §8f N2): HF safetensors / .bin -> the packed device layouts.
 
-Nothing here is exercised against the real ``neuphonic/*`` checkpoints in this environment (offline,
-no cache); the Qwen2 reader is tested against checkpoints written by ``transformers.save_pretrained``
-and the codec reader against a state_dict laid out with the upstream ``neucodec`` names.
+The speech-LM reader takes Qwen2, Llama and Mistral checkpoints and refuses, before any CUDA work, every config or
+tensor the kernels would compute differently than transformers does (``check_lm_config``, ``lm.check_tensors``).
+It is tested end to end against checkpoints that transformers' own classes write (bf16 and sharded fp32 safetensors,
+fp16 ``pytorch_model.bin``; tests/test_loader_families.py on the CPU, tests/test_gpu_loader_families.py through the
+kernels); the real ``neuphonic/*`` checkpoints are not available offline.  The codec reader is tested against a
+state_dict laid out with the upstream ``neucodec`` names.
 """
 from __future__ import annotations
 
@@ -13,7 +16,7 @@ from pathlib import Path
 import torch
 
 from .codec import CodecDecoder, CodecShape
-from .lm import LMShape, SpeechLM
+from .lm import LMShape, SpeechLM, check_tensors
 
 
 def resolve_repo(repo: str) -> Path:
@@ -50,29 +53,80 @@ def load_tokenizer(repo: str):
     return AutoTokenizer.from_pretrained(str(resolve_repo(repo)))
 
 
-def load_speech_lm(repo: str, device="cuda", **kw) -> SpeechLM:
-    """``AutoModelForCausalLM.from_pretrained`` replacement (neutts/neutts.py:163-166): config.json decides
-    every dimension (NeuTTS-Nano and Air differ), weights are cast to bf16."""
+# the kernels implement the pre-norm RMSNorm / RoPE (half-split) / GQA / SwiGLU decoder that these three share; q/k/v
+# biases are optional (absent in Llama and Mistral checkpoints -> zeros)
+ARCHITECTURES = {"Qwen2ForCausalLM": "qwen2", "LlamaForCausalLM": "llama", "MistralForCausalLM": "mistral"}
+
+
+def _binding_window(cfg: dict) -> int | None:
+    """The attention window some layer of the transformers model attends within, or None when every layer attends to
+    its whole context.  ``layer_types`` (transformers 5) names the sliding layers; without it Qwen2 slides from layer
+    ``max_window_layers`` on when ``use_sliding_window`` is set, and Mistral slides in every layer."""
+    window = cfg.get("sliding_window")
+    if window is None:
+        return None
+    if cfg.get("layer_types") is not None:
+        return window if "sliding_attention" in cfg["layer_types"] else None
+    if cfg.get("model_type") == "qwen2":
+        slides = cfg.get("use_sliding_window", False) and cfg.get("max_window_layers", 28) < cfg["num_hidden_layers"]
+        return window if slides else None
+    return window
+
+
+def check_lm_config(cfg: dict, max_ctx: int) -> None:
+    """Raises ValueError, naming the key, for a config.json whose model the kernels would compute differently than
+    transformers does: another architecture, scaled or partial RoPE, an activation other than SiLU, or an attention
+    window shorter than the engine's context ``max_ctx``."""
+    archs = cfg.get("architectures") or []
+    mtype = cfg.get("model_type")
+    # one allowlisted family, named by the architecture, the model_type or both (and then the same one)
+    families = {ARCHITECTURES.get(a) for a in archs} | ({mtype} if mtype is not None else set())
+    if len(families) != 1 or not families <= set(ARCHITECTURES.values()):
+        raise ValueError(f"unsupported backbone (architectures={archs!r}, model_type={mtype!r}): the sm_90a kernels "
+                         f"implement {', '.join(ARCHITECTURES)} (RMSNorm, RoPE, GQA, SwiGLU)")
+    for key in ("rope_scaling", "rope_parameters"):
+        rope = cfg.get(key) or {}
+        kind = rope.get("rope_type", rope.get("type", "default"))
+        if kind != "default":
+            raise ValueError(f"{key}.rope_type = {kind!r}: scaled RoPE variants are not implemented")
+        if float(rope.get("partial_rotary_factor", 1.0)) != 1.0:
+            raise ValueError(f"{key}.partial_rotary_factor = {rope['partial_rotary_factor']}: partial RoPE is not implemented")
+    if float(cfg.get("partial_rotary_factor", 1.0)) != 1.0:
+        raise ValueError(f"partial_rotary_factor = {cfg['partial_rotary_factor']}: partial RoPE is not implemented")
+    act = cfg.get("hidden_act", "silu")
+    if act != "silu":
+        raise ValueError(f"hidden_act = {act!r}: the MLP kernels compute SwiGLU (silu)")
+    window = _binding_window(cfg)
+    if window is not None and window < max_ctx:
+        raise ValueError(f"sliding_window = {window} < max_ctx = {max_ctx}: the attention kernels attend to the whole "
+                         f"context; load with max_ctx <= {window}")
+
+
+def read_speech_lm(repo: str, max_ctx: int = 2048) -> tuple:
+    """Everything ``load_speech_lm`` does short of the device: (LMShape, state_dict) of a checked checkpoint.
+
+    The lm_head follows the tensors the way ``from_pretrained`` does: an ``lm_head.weight`` in the checkpoint is used
+    even under ``tie_word_embeddings = true`` (shared with the embedding only when equal to it); without one the head
+    is the embedding, and an untied config without one is refused (transformers would initialise a random head)."""
     root = resolve_repo(repo)
     cfg = json.loads((root / "config.json").read_text())
-    arch = (cfg.get("architectures") or ["Qwen2ForCausalLM"])[0]
-    # the kernels implement the pre-norm RMSNorm / RoPE (half-split) / GQA / SwiGLU decoder that Qwen2, Llama and
-    # Mistral share; q/k/v biases are optional (absent in Llama-style checkpoints -> zeros)
-    family = ("Qwen2", "Llama", "Mistral", "Qwen3")
-    if not any(f in arch for f in family) and cfg.get("model_type") not in ("qwen2", "llama", "mistral"):
-        raise ValueError(f"unsupported backbone architecture {arch!r}: the sm_90a kernels implement the "
-                         f"Qwen2/Llama-family decoder (RMSNorm, RoPE, GQA, SwiGLU)")
-    if cfg.get("rope_scaling") not in (None, {}) and (cfg["rope_scaling"] or {}).get("rope_type", "default") != "default":
-        raise ValueError("scaled RoPE variants are not implemented")
+    check_lm_config(cfg, max_ctx)
     sd = read_state_dict(root)
     shape = LMShape.from_hf_config(cfg)
-    # tied embeddings: trust the tensors, not a missing config key (a real lm_head must not be dropped silently)
-    if "lm_head.weight" in sd and "model.embed_tokens.weight" in sd:
-        same = sd["lm_head.weight"].shape == sd["model.embed_tokens.weight"].shape and bool(
+    check_tensors(shape, sd)
+    if "lm_head.weight" in sd:
+        shape.tie_embeddings = sd["lm_head.weight"].shape == sd["model.embed_tokens.weight"].shape and bool(
             torch.equal(sd["lm_head.weight"], sd["model.embed_tokens.weight"]))
-        shape.tie_embeddings = same
-    elif "lm_head.weight" not in sd:
-        shape.tie_embeddings = True
+    elif not shape.tie_embeddings:
+        raise ValueError("tie_word_embeddings is false (or absent) and the checkpoint has no lm_head.weight")
+    return shape, sd
+
+
+def load_speech_lm(repo: str, device="cuda", **kw) -> SpeechLM:
+    """``AutoModelForCausalLM.from_pretrained`` replacement (neutts/neutts.py:163-166) for Qwen2, Llama and Mistral
+    checkpoints: config.json decides every dimension (NeuTTS-Nano and Air differ), weights are cast to bf16.  Every
+    refusal of ``read_speech_lm`` happens before any CUDA work."""
+    shape, sd = read_speech_lm(repo, kw.get("max_ctx", 2048))
     return SpeechLM(shape, sd, device=device, **kw)
 
 

@@ -199,8 +199,9 @@ def test_page_pool_and_weight_packing():
     assert pk["lm_head"] is pk["embed"]
 
 
-def test_loader_reads_hf_checkpoint(tmp_path):
+def test_loader_reads_hf_checkpoint(tmp_path, monkeypatch):
     pytest.importorskip("transformers")
+    monkeypatch.setenv("HF_HUB_OFFLINE", "1")     # the missing repo below must not reach for the hub
     from neutts_air_b200 import loader
     from neutts_air_b200.lm import LMShape
     from oracle import lm_oracle as LO
