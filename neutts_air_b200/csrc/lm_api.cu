@@ -98,7 +98,7 @@ struct nt_lm {
   // workspace
   float *h, *q, *attn, *act, *logits, *cand_val, *inv_freq, *qkv, *h_last, *splitk_ws;
   size_t splitk_floats;
-  int *cand_idx, *tok_seq, *tok_pos, *cu_dev, *last_rows, *iota;
+  int *cand_idx, *tok_seq, *tok_pos, *cu_dev, *last_rows;
   __nv_bfloat16 *xn, *attn_bf16, *act_bf16;
   // persistent decode kernel tables (device)
   const float** ptr_tab;   // [3][n_layers]: ln1, bqkv, ln2
@@ -198,7 +198,6 @@ static size_t lm_carve(const nt_lm_config& c, void* ws, size_t bytes, F&& assign
     (L)->tok_pos = a.take<int>(rows);                                                          \
     (L)->cu_dev = a.take<int>(c.max_batch + 1);                                                \
     (L)->last_rows = a.take<int>(c.max_batch);                                                 \
-    (L)->iota = a.take<int>(c.max_batch);                                                      \
     (L)->xn = a.take<__nv_bfloat16>(size_t(rows) * H);                                         \
     (L)->attn_bf16 = a.take<__nv_bfloat16>(size_t(rows) * c.n_heads * 64);                     \
     (L)->act_bf16 = a.take<__nv_bfloat16>(size_t(rows) * I);                                   \
@@ -296,11 +295,9 @@ extern "C" int nt_lm_create(const nt_lm_config* cfg, const nt_lm_weights* w, voi
     return set_error(NT_ERR_CUDA, "device is sm_%d%d; this library is built for sm_90a only", prop.major, prop.minor);
   }
   lm->num_sms = prop.multiProcessorCount;
-  // rotary inverse frequencies (modeling_qwen2.py:95-100), iota, per-layer norm / bias pointers
+  // rotary inverse frequencies (modeling_qwen2.py:95-100), per-layer norm / bias pointers
   float invf[64] = {0};
   for (int i = 0; i < 32; ++i) invf[i] = static_cast<float>(1.0 / std::pow(static_cast<double>(c.rope_theta), (2.0 * i) / 64.0));
-  std::vector<int> iota(c.max_batch);
-  for (int i = 0; i < c.max_batch; ++i) iota[i] = i;
   std::vector<const float*> pt(size_t(3) * c.n_layers);
   for (int l = 0; l < c.n_layers; ++l) {
     pt[l] = lm->ln1[l];
@@ -308,7 +305,6 @@ extern "C" int nt_lm_create(const nt_lm_config* cfg, const nt_lm_weights* w, voi
     pt[2 * c.n_layers + l] = lm->ln2[l];
   }
   if (cudaMemcpy(lm->inv_freq, invf, sizeof(invf), cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemcpy(lm->iota, iota.data(), iota.size() * sizeof(int), cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemcpy(lm->ptr_tab, pt.data(), pt.size() * sizeof(const float*), cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemset(lm->slot_key, 0xff, size_t(c.max_batch) * sizeof(int)) != cudaSuccess) {
     delete lm;
@@ -485,7 +481,7 @@ static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cud
 }
 
 // Transformer layers over `rows` token rows held in lm->h, via tensor-core GEMMs.
-// mode 0: prefill (causal attention over the prompt);  mode 1: one new token per sequence.
+// mode 0: prefill (causal attention over the prompt);  mode 1: one new token per sequence (decode at batch > 4).
 // table: page table to address the KV cache with, row b for sequence b of the call (default: the state's).
 // row_local (nt_lm_score): no split-K, 128-column GEMM tiles and the one-warp-per-row RMSNorm for every row count, so that
 // each token row's arithmetic does not depend on how many rows the call holds.
@@ -514,32 +510,25 @@ static int layers_gemm(nt_lm* lm, const nt_lm_state* st, int rows, int B, int mo
     memset(&a, 0, sizeof(a));
     a.dtype = NT_BF16, a.M = rows, a.N = QN, a.K = H, a.A = lm->xn, a.lda = H, a.W = lm->wqkv[l], a.ldw = H;
     a.bias = lm->bqkv[l], a.out_f32 = lm->qkv, a.ldc = QN;
-    // few row tiles: the projection splits K into slices that rope_append sums (the bias rides on slice 0)
+    // few row tiles: the projection splits K into slices that the RoPE + KV append sums (the bias rides on slice 0)
     SplitK qsplit;
     qsplit.ws = lm->splitk_ws, qsplit.ws_floats = lm->splitk_floats, qsplit.used = 1, qsplit.slice_stride = 0;
     if ((rc = gemm_dispatch(a, stream, row_local ? nullptr : &qsplit, true, nullptr, nullptr, bn))) return rc;
-    const int32_t* tseq = mode == 0 ? lm->tok_seq : lm->iota;
-    const int32_t* tpos = mode == 0 ? lm->tok_pos : st->seq_lens;
-    // decode on the tensor-core attention kernel (batch > 4): RoPE + KV append run in that kernel's prologue
-    const bool fuse_rope = mode == 1 && B > 4;
-    if (!fuse_rope &&
-        (rc = launch_rope_append(qsplit.used > 1 ? qsplit.ws : lm->qkv, rows, QN, tseq, tpos, c.n_heads, lm->inv_freq, lm->q, kv, l, stream,
-                                 qsplit.used, qsplit.slice_stride)))
-      return rc;
     if (mode == 0) {
+      if ((rc = launch_rope_append(qsplit.used > 1 ? qsplit.ws : lm->qkv, rows, QN, lm->tok_seq, lm->tok_pos, c.n_heads, lm->inv_freq, lm->q, kv,
+                                   l, stream, qsplit.used, qsplit.slice_stride)))
+        return rc;
       AttnPrefillParams ap;
       ap.q = lm->q, ap.kv = kv, ap.layer = l, ap.n_heads = c.n_heads, ap.n_rep = c.n_heads / c.n_kv_heads;
       ap.scale_log2 = scale_log2, ap.cu_seqlens = lm->cu_dev, ap.out = lm->attn_bf16, ap.max_len = max_len;
       if ((rc = launch_attn_prefill(ap, B, c.n_layers, stream))) return rc;
-    } else {
+    } else {   // decode (batch > 4): RoPE + KV append run in the tensor-core attention kernel's prologue
       AttnDecParams ad;
       memset(&ad, 0, sizeof(ad));
-      ad.q = lm->q, ad.kv = kv, ad.layer = l, ad.n_heads = c.n_heads, ad.n_rep = c.n_heads / c.n_kv_heads;
+      ad.kv = kv, ad.layer = l, ad.n_heads = c.n_heads, ad.n_rep = c.n_heads / c.n_kv_heads;
       ad.scale_log2 = scale_log2, ad.out = lm->attn, ad.out_bf16 = lm->attn_bf16;
-      if (fuse_rope) {
-        ad.qkv = qsplit.used > 1 ? qsplit.ws : lm->qkv, ad.qkv_n = QN, ad.qkv_parts = qsplit.used;
-        ad.qkv_pstride = qsplit.slice_stride, ad.inv_freq = lm->inv_freq;
-      }
+      ad.qkv = qsplit.used > 1 ? qsplit.ws : lm->qkv, ad.qkv_n = QN, ad.qkv_parts = qsplit.used;
+      ad.qkv_pstride = qsplit.slice_stride, ad.inv_freq = lm->inv_freq;
       if ((rc = launch_attn_decode(ad, B, c.n_layers, stream))) return rc;
     }
     memset(&a, 0, sizeof(a));

@@ -81,10 +81,6 @@ NT_DEVINL void split_hilo(float x, __nv_bfloat16& hi, __nv_bfloat16& lo) {
   hi = __float2bfloat16(x);
   lo = __float2bfloat16(x - __bfloat162float(hi));
 }
-// element (row n, k) of a K-major SWIZZLE_128B chunk [rows][64 bf16]: 16-byte group g = k / 8 sits at g ^ (n & 7)
-NT_DEVINL __nv_bfloat16* chunk_elem(uint8_t* chunk, int n, int k) {
-  return reinterpret_cast<__nv_bfloat16*>(chunk + n * 128 + ((((k >> 3) ^ (n & 7)) << 4) | ((k & 7) << 1)));
-}
 
 
 NT_DEVINL void tc_spin_check(uint32_t& spins, const char* what) {
@@ -572,14 +568,12 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     // lane 0 of an attention warp: K and V page of (sequence, kv head) -> this warp's buffers
     //   (whole attention warp, converged; fence: see the proxy fence after the sampler's grid barrier)
     auto issue_page = [&](int l, int pg, int p0, bool fence) {
-      const int krow0 = l * 2 * P.kv.num_pages * P.kv.n_kv_heads * 64;
-      const int vrow0 = krow0 + P.kv.num_pages * P.kv.n_kv_heads * 64;
       const int page = uniform(page_of(pg, p0));
       if (elect_one()) {
         if (fence) fence_proxy_async_all();
         mbar_arrive_expect_tx(&ms->att_bar[warp], 2 * 8192);
-        tma_load_2d(att_k(warp), kvmap, 0, krow0 + (page * P.kv.n_kv_heads + my_kvh) * 64, &ms->att_bar[warp]);
-        tma_load_2d(att_v(warp), kvmap, 0, vrow0 + (page * P.kv.n_kv_heads + my_kvh) * 64, &ms->att_bar[warp]);
+        tma_load_2d(att_k(warp), kvmap, 0, P.kv.tmap_row(l, 0, page, my_kvh), &ms->att_bar[warp]);
+        tma_load_2d(att_v(warp), kvmap, 0, P.kv.tmap_row(l, 1, page, my_kvh), &ms->att_bar[warp]);
       }
     };
     // dedicated staging: the first round of pages of layer l is fetched before the layer's projections run (they do
@@ -621,8 +615,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
         else row0 = (P.n_heads + P.n_kv + kvh) * 64 + 2 * i;
         if (which != 0 && !appends) continue;
         const float2 bia = __ldg(reinterpret_cast<const float2*>(bias + row0));
-        float sn = 0.f, cs = 1.f;
-        if (which != 2) sincosf(static_cast<float>(pos) * __ldg(P.inv_freq + i), &sn, &cs);
+        // ahead of the wait for the slices, which hides its latency
+        const float2 sc = which != 2 ? rope_sincos(pos, __ldg(P.inv_freq + i)) : make_float2(0.f, 1.f);
         float2 a = make_float2(0.f, 0.f);
         for (int s0 = 0; s0 < P.sq; s0 += 8) {
           float4 t[8];
@@ -644,9 +638,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
         if (which == 2) {
           att_vnew[2 * i] = a.x, att_vnew[2 * i + 1] = a.y;
         } else {
-          const float lo = a.x * cs - a.y * sn, hi = a.y * cs + a.x * sn;   // rows (2i, 2i+1) = dims (i, i + 32)
-          if (which == 0) att_q[(idx >> 5) * 64 + i] = lo, att_q[(idx >> 5) * 64 + i + 32] = hi;
-          else att_knew[i] = lo, att_knew[i + 32] = hi;
+          // rope_pair's rotation, but dim i + 32 fuses x sin and rounds y cos where rope_pair does the opposite: the
+          // rounding this kernel has always had, which keeps its decode output bit-identical
+          const float2 r = make_float2(__fmaf_rn(a.x, sc.y, -__fmul_rn(a.y, sc.x)), __fmaf_rn(a.x, sc.x, __fmul_rn(a.y, sc.y)));
+          if (which == 0) att_q[(idx >> 5) * 64 + i] = r.x, att_q[(idx >> 5) * 64 + i + 32] = r.y;
+          else att_knew[i] = r.x, att_knew[i + 32] = r.y;
         }
       }
       pm(22);
@@ -658,120 +654,35 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
         P.kv.page_ptr(l, 1, page, kvh)[(pos & 63) * 64 + d] = __float2bfloat16(att_vnew[d]);
       }
       if (warp < AW) {
-        const int g = lane >> 2, t = lane & 3, lrow = lane & 7, lmat = lane >> 3;
-        // query fragments: row g = head g of the group (rows >= n_rep and rows 8..15 are zero); scale * log2(e) folded in
         uint32_t qa[4][4];
-        {
-          const float* qp = att_q + min(g, n_rep - 1) * 64;
-          const float sc = (g < n_rep) ? P.scale_log2 : 0.f;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float2 a0 = *reinterpret_cast<const float2*>(qp + 16 * j + 2 * t);
-            const float2 a2 = *reinterpret_cast<const float2*>(qp + 16 * j + 8 + 2 * t);
-            qa[j][0] = pack_bf16x2(a0.x * sc, a0.y * sc);
-            qa[j][1] = 0u;
-            qa[j][2] = pack_bf16x2(a2.x * sc, a2.y * sc);
-            qa[j][3] = 0u;
-          }
-        }
+        decode_query_frags(att_q, n_rep, P.scale_log2, qa);
         float o[8][4];
 #pragma unroll
         for (int n = 0; n < 8; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
-        float m0 = -INFINITY, l0 = 0.f;
+        float m[1] = {-INFINITY}, lsum[1] = {0.f};
         const uint32_t kbase = smem_u32(att_k(warp)), vbase = smem_u32(att_v(warp));
         for (int pg = p0 + warp; pg < p1; pg += AW) {
           mbar_wait(&ms->att_bar[warp], att_par);
           att_par ^= 1;
           if (warp == 0) pm(23);
-          if (appends && pg == (pos >> 6)) {  // patch the staged page with the new row (the copy may predate our store)
-            const int r = pos & 63;
-            uint8_t* kb8 = reinterpret_cast<uint8_t*>(att_k(warp));
-            uint8_t* vb8 = reinterpret_cast<uint8_t*>(att_v(warp));
-            *reinterpret_cast<uint32_t*>(chunk_elem(kb8, r, 2 * lane)) = pack_bf16x2(att_knew[2 * lane], att_knew[2 * lane + 1]);
-            *reinterpret_cast<uint32_t*>(chunk_elem(vb8, r, 2 * lane)) = pack_bf16x2(att_vnew[2 * lane], att_vnew[2 * lane + 1]);
-            __syncwarp();
-          }
-          float sc[8][4];
-#pragma unroll
-          for (int n = 0; n < 8; ++n) {
-            sc[n][0] = sc[n][1] = sc[n][2] = sc[n][3] = 0.f;
-            const int row = 8 * n + lrow;
-#pragma unroll
-            for (int half = 0; half < 2; ++half) {
-              uint32_t kb[4];
-              ldmatrix_x4(kb, kbase + row * 128 + (((4 * half + lmat) ^ lrow) << 4));
-              mma_bf16_16816(sc[n], qa[2 * half], kb[0], kb[1]);
-              mma_bf16_16816(sc[n], qa[2 * half + 1], kb[2], kb[3]);
-            }
-          }
+          if (appends && pg == (pos >> 6)) patch_staged_row(att_k(warp), att_v(warp), pos & 63, att_knew, att_vnew);
           const int k0 = pg * 64;
-          if (k0 + 64 > geo.n_ctx) {
-#pragma unroll
-            for (int n = 0; n < 8; ++n) {
-              const int kv0 = k0 + 8 * n + 2 * t;
-              if (kv0 >= geo.n_ctx) sc[n][0] = -INFINITY;
-              if (kv0 + 1 >= geo.n_ctx) sc[n][1] = -INFINITY;
-            }
-          }
-          float mx = -INFINITY;
-#pragma unroll
-          for (int n = 0; n < 8; ++n) mx = fmaxf(mx, fmaxf(sc[n][0], sc[n][1]));
-          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1)), mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-          const float mn = fmaxf(m0, mx);  // the first token of every page walked is valid -> finite
-          const float c = exp2f(m0 - mn);
-          m0 = mn;
-          l0 *= c;
-#pragma unroll
-          for (int n = 0; n < 8; ++n) o[n][0] *= c, o[n][1] *= c;
-          uint32_t pa[4][4];
-#pragma unroll
-          for (int n = 0; n < 8; ++n) {
-            const float p0v = exp2f(sc[n][0] - mn), p1v = exp2f(sc[n][1] - mn);
-            l0 += p0v + p1v;
-            pa[n >> 1][(n & 1) * 2 + 0] = pack_bf16x2(p0v, p1v);
-            pa[n >> 1][(n & 1) * 2 + 1] = 0u;
-          }
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int row = 16 * j + 8 * (lmat & 1) + lrow;
-#pragma unroll
-            for (int nd = 0; nd < 8; nd += 2) {
-              uint32_t vb[4];
-              ldmatrix_x4_trans(vb, vbase + row * 128 + (((nd + (lmat >> 1)) ^ lrow) << 4));
-              mma_bf16_16816(o[nd], pa[j], vb[0], vb[1]);
-              mma_bf16_16816(o[nd + 1], pa[j], vb[2], vb[3]);
-            }
-          }
+          attn_page_step<1>(kbase, vbase, qa, o, m, lsum, k0 + 64 > geo.n_ctx, [&](int, int key) { return k0 + key >= geo.n_ctx; });
           __syncwarp();  // all lanes are done with the buffers before they are refilled
           if (pg + AW < p1) issue_page(l, pg + AW, p0, !att_separate);
         }
-        l0 += __shfl_xor_sync(0xffffffffu, l0, 1), l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-        if (g < n_rep) {
-#pragma unroll
-          for (int n = 0; n < 8; ++n) *reinterpret_cast<float2*>(att_o + (warp * 8 + g) * 64 + 8 * n + 2 * t) = make_float2(o[n][0], o[n][1]);
-          if (t == 0) att_ml[(warp * 8 + g) * 2] = m0, att_ml[(warp * 8 + g) * 2 + 1] = l0;
-        }
+        decode_store_partial(o, m[0], lsum[0], n_rep, att_o + warp * 8 * 64, att_ml + warp * 8 * 2);
       }
       csync();
       const float sf = __int_as_float(stamp);
       for (int i = tid; i < n_rep * 64; i += kConsumerThreads) {
         const int h = i >> 6, d = i & 63;
-        float M = -INFINITY;
-#pragma unroll
-        for (int w = 0; w < kAttWarpsMax; ++w)
-          if (w < AW) M = fmaxf(M, att_ml[(w * 8 + h) * 2]);
-        float Ls = 0.f, O = 0.f;
-#pragma unroll
-        for (int w = 0; w < kAttWarpsMax; ++w) {
-          if (w < AW) {
-            const float wgt = exp2f(att_ml[(w * 8 + h) * 2] - M);   // 0 for a warp that walked no page (m = -inf, l = 0)
-            Ls += wgt * att_ml[(w * 8 + h) * 2 + 1];
-            O += wgt * att_o[(w * 8 + h) * 64 + d];
-          }
-        }
+        const SoftmaxPart r = merge_parts<kAttWarpsMax>(AW, [&](int w) {
+          return SoftmaxPart{att_ml[(w * 8 + h) * 2], att_ml[(w * 8 + h) * 2 + 1], att_o[(w * 8 + h) * 64 + d]};
+        });
         const long long hh = static_cast<long long>(b) * P.n_heads + kvh * n_rep + h;
-        P.ao2[(hh * P.max_splits + my_split) * 64 + d] = make_float2(O, sf);
-        if (d == 0) *reinterpret_cast<float4*>(P.aml2 + (hh * P.max_splits + my_split) * 2) = make_float4(M, sf, Ls, sf);
+        P.ao2[(hh * P.max_splits + my_split) * 64 + d] = make_float2(r.o, sf);
+        if (d == 0) *reinterpret_cast<float4*>(P.aml2 + (hh * P.max_splits + my_split) * 2) = make_float4(r.m, sf, r.l, sf);
       }
       pm(25);
       csync();   // the union region is free again
@@ -807,19 +718,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
           if (ok) break;
           tc_spin_check(spins, "attention partials");
         }
-        float M = -INFINITY;
-#pragma unroll
-        for (int s = 0; s < 8; ++s)
-          if (s < g.nsplit) M = fmaxf(M, mv[s].x);
-        float Ls = 0.f, O = 0.f;
-#pragma unroll
-        for (int s = 0; s < 8; ++s)
-          if (s < g.nsplit) {
-            const float wgt = exp2f(mv[s].x - M);
-            Ls += wgt * mv[s].z;
-            O += wgt * ov[s].x;
-          }
-        const float val = O / Ls;
+        const SoftmaxPart mp = merge_parts<8>(g.nsplit, [&](int s) { return SoftmaxPart{mv[s].x, mv[s].z, ov[s].x}; });
+        const float val = mp.o / mp.l;
         uint8_t* cb = uni + c * CHUNK;
         if constexpr (HILO) {
           __nv_bfloat16 hi, lo;

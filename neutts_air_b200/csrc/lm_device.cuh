@@ -1,5 +1,6 @@
 // Device-side building blocks shared by the per-op kernels (lm_kernels.cu) and the persistent wgmma decode kernel
-// (lm_decode_tc.cu): sync functors, ld_cg, the mma.sync helpers, the split-KV geometry and the sampler pieces.
+// (lm_decode_tc.cu): sync functors, ld_cg, the mma.sync helpers, RoPE, the tensor-core attention page step and the
+// merge of its partials, the split-KV geometry and the sampler pieces.
 // Every block-cooperative function takes a `Sync` functor: SyncAll (= __syncthreads, per-op kernels) or
 // SyncConsumers (named barrier over 256 consumer threads, for kernels whose other warps never join).
 // All functions assume the cooperating threads are threadIdx.x in [0, 256).
@@ -24,7 +25,7 @@ NT_DEVINL T ld_cg(const T* p) {
   return __ldcg(p);
 }
 
-// ---- legacy tensor-core path used by both attention kernels (wgmma needs 64 rows of M; these tiles have 7-16)
+// ---- legacy tensor-core path used by the attention kernels (wgmma needs 64 rows of M; these tiles have 7-16)
 NT_DEVINL void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile(
       "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
@@ -40,6 +41,169 @@ NT_DEVINL void ldmatrix_x4_trans(uint32_t (&r)[4], uint32_t addr) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
                : "r"(addr));
+}
+
+// element (row n, k) of a K-major SWIZZLE_128B chunk [rows][64 bf16]: 16-byte group g = k / 8 sits at g ^ (n & 7)
+NT_DEVINL __nv_bfloat16* chunk_elem(uint8_t* chunk, int n, int k) {
+  return reinterpret_cast<__nv_bfloat16*>(chunk + n * 128 + ((((k >> 3) ^ (n & 7)) << 4) | ((k & 7) << 1)));
+}
+
+// (sin, cos) of the RoPE angle pos * inv_freq_i (modeling_qwen2.py:116-146)
+NT_DEVINL float2 rope_sincos(int pos, float inv_freq_i) {
+  float s, c;
+  sincosf(static_cast<float>(pos) * inv_freq_i, &s, &c);
+  return make_float2(s, c);
+}
+// RoPE of one packed pair: projection rows (2i, 2i+1) hold dims (i, i + 32) of a q / k head (pair-interleaved at pack
+// time), rotated by half-split RoPE at position pos; returns dims (i, i + 32).  The fma and the rounded product are
+// spelled out so that the result does not depend on how ptxas contracts the expression at a call site.
+NT_DEVINL float2 rope_pair(float x, float y, int pos, float inv_freq_i) {
+  const float2 sc = rope_sincos(pos, inv_freq_i);
+  return make_float2(__fmaf_rn(x, sc.y, -__fmul_rn(y, sc.x)), __fmaf_rn(y, sc.y, __fmul_rn(x, sc.x)));
+}
+
+// ---- tensor-core attention over 64-token KV pages (attn_prefill_kernel, attn_decode_mma_kernel, decode_tc_kernel).
+// Fragment coordinates of m16n8k16: lane = 4 g + t; accumulator entry e of key group n is query row g + 8 (e >> 1),
+// key 8 n + 2 t + (e & 1) of the page.
+NT_DEVINL float quad_max(float x) {
+  x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
+  return fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 2));
+}
+NT_DEVINL float quad_sum(float x) {
+  x += __shfl_xor_sync(0xffffffffu, x, 1);
+  return x + __shfl_xor_sync(0xffffffffu, x, 2);
+}
+
+// One page step of one warp: S = Q K^T from the staged K page (SWIZZLE_128B, ldmatrix), masking, base-2 online softmax
+// on the accumulator fragments, P rounded to bf16, O += P V from the staged V page (ldmatrix .trans).  qa: A fragments
+// of the 16-row query tile, scale * log2(e) folded in.  H: live 8-row halves of the tile (1: rows 8..15 are zero and
+// their statistics are not kept; 2: both).  m / l: running maximum and this lane's partial sum of each live half.
+// masked: dead(half, key) is true for every (query row half, key of the page) the query must not see.  The first key
+// of every page must be visible to every live row (m stays finite).
+template <int H, typename Dead>
+NT_DEVINL void attn_page_step(uint32_t kbase, uint32_t vbase, const uint32_t (&qa)[4][4], float (&o)[8][4], float (&m)[H],
+                              float (&l)[H], bool masked, Dead dead) {
+  const int lane = threadIdx.x & 31, t = lane & 3, lrow = lane & 7, lmat = lane >> 3;
+  // S = Q K^T: 8 key groups of 8 tokens; ldmatrix: lane supplies row (lane & 7) of matrix (lane >> 3)
+  float sc[8][4];
+#pragma unroll
+  for (int n = 0; n < 8; ++n) {
+    sc[n][0] = sc[n][1] = sc[n][2] = sc[n][3] = 0.f;
+    const int row = 8 * n + lrow;  // key token within the page; row & 7 == lrow
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {  // dims 0..31 / 32..63: 4 chunks of 8 dims each
+      uint32_t kb[4];
+      ldmatrix_x4(kb, kbase + row * 128 + (((4 * half + lmat) ^ lrow) << 4));
+      mma_bf16_16816(sc[n], qa[2 * half], kb[0], kb[1]);
+      mma_bf16_16816(sc[n], qa[2 * half + 1], kb[2], kb[3]);
+    }
+  }
+  if (masked) {
+#pragma unroll
+    for (int n = 0; n < 8; ++n)
+#pragma unroll
+      for (int e = 0; e < 2 * H; ++e)
+        if (dead(e >> 1, 8 * n + 2 * t + (e & 1))) sc[n][e] = -INFINITY;
+  }
+#pragma unroll
+  for (int h = 0; h < H; ++h) {
+    float mx = -INFINITY;
+#pragma unroll
+    for (int n = 0; n < 8; ++n) mx = fmaxf(mx, fmaxf(sc[n][2 * h], sc[n][2 * h + 1]));
+    const float mn = fmaxf(m[h], quad_max(mx));
+    const float c = exp2f(m[h] - mn);   // 0 on the first page
+    m[h] = mn;
+    l[h] *= c;
+#pragma unroll
+    for (int n = 0; n < 8; ++n) o[n][2 * h] *= c, o[n][2 * h + 1] *= c;
+  }
+  uint32_t pa[4][4];  // P as A fragments: k-step j covers key groups 2j, 2j+1
+#pragma unroll
+  for (int n = 0; n < 8; ++n) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      uint32_t pk = 0u;
+      if (h < H) {
+        const float p0 = exp2f(sc[n][2 * h] - m[h]), p1 = exp2f(sc[n][2 * h + 1] - m[h]);
+        l[h] += p0 + p1;
+        pk = pack_bf16x2(p0, p1);
+      }
+      pa[n >> 1][(n & 1) * 2 + h] = pk;
+    }
+  }
+  // O += P V: k-steps of 16 keys, output dim groups of 8 (two per ldmatrix)
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int row = 16 * j + 8 * (lmat & 1) + lrow;  // key token; row & 7 == lrow
+#pragma unroll
+    for (int nd = 0; nd < 8; nd += 2) {
+      uint32_t vb[4];
+      ldmatrix_x4_trans(vb, vbase + row * 128 + (((nd + (lmat >> 1)) ^ lrow) << 4));
+      mma_bf16_16816(o[nd], pa[j], vb[0], vb[1]);
+      mma_bf16_16816(o[nd + 1], pa[j], vb[2], vb[3]);
+    }
+  }
+}
+
+// Decode query tile: row g = query head g of the KV head's group, from q [n_rep][64] fp32 (shared memory), times
+// scale_log2, as bf16 A fragments; rows >= n_rep and rows 8..15 are zero.
+NT_DEVINL void decode_query_frags(const float* q, int n_rep, float scale_log2, uint32_t (&qa)[4][4]) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const float* qp = q + min(g, n_rep - 1) * 64;
+  const float sc = (g < n_rep) ? scale_log2 : 0.f;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float2 a0 = *reinterpret_cast<const float2*>(qp + 16 * j + 2 * t);
+    const float2 a2 = *reinterpret_cast<const float2*>(qp + 16 * j + 8 + 2 * t);
+    qa[j][0] = pack_bf16x2(a0.x * sc, a0.y * sc);
+    qa[j][1] = 0u;
+    qa[j][2] = pack_bf16x2(a2.x * sc, a2.y * sc);
+    qa[j][3] = 0u;
+  }
+}
+
+// The new token's K and V rows (fp32 [64] each) -> row r of the staged K and V pages (bf16, SWIZZLE_128B), two dims per
+// lane: the page copy may predate the row's store to the cache.  Whole warp, before its ldmatrix reads of the page.
+NT_DEVINL void patch_staged_row(void* kstage, void* vstage, int r, const float* knew, const float* vnew) {
+  const int lane = threadIdx.x & 31;
+  *reinterpret_cast<uint32_t*>(chunk_elem(static_cast<uint8_t*>(kstage), r, 2 * lane)) = pack_bf16x2(knew[2 * lane], knew[2 * lane + 1]);
+  *reinterpret_cast<uint32_t*>(chunk_elem(static_cast<uint8_t*>(vstage), r, 2 * lane)) = pack_bf16x2(vnew[2 * lane], vnew[2 * lane + 1]);
+  __syncwarp();
+}
+
+// A decode warp's partial for the merge: rows g < n_rep store their unnormalised output to o_w [8][64] and (m, l) to
+// ml_w [8][2], l summed over the quad first.
+NT_DEVINL void decode_store_partial(const float (&o)[8][4], float m, float l, int n_rep, float* o_w, float* ml_w) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  l = quad_sum(l);
+  if (g < n_rep) {
+#pragma unroll
+    for (int n = 0; n < 8; ++n) *reinterpret_cast<float2*>(o_w + g * 64 + 8 * n + 2 * t) = make_float2(o[n][0], o[n][1]);
+    if (t == 0) ml_w[2 * g] = m, ml_w[2 * g + 1] = l;
+  }
+}
+
+// One base-2 online-softmax partial of one (head, dim): running maximum, sum of exponentials, unnormalised output.
+struct SoftmaxPart {
+  float m, l, o;
+};
+// Merge of the partials part(0) .. part(n - 1), n <= kMax, summed in index order (warp or split 0 first).
+template <int kMax, typename Part>
+NT_DEVINL SoftmaxPart merge_parts(int n, Part part) {
+  SoftmaxPart r{-INFINITY, 0.f, 0.f};
+#pragma unroll
+  for (int w = 0; w < kMax; ++w)
+    if (w < n) r.m = fmaxf(r.m, part(w).m);
+#pragma unroll
+  for (int w = 0; w < kMax; ++w) {
+    if (w < n) {
+      const SoftmaxPart e = part(w);
+      const float wgt = exp2f(e.m - r.m);  // 0 for a partial that saw no token (m = -inf, l = 0)
+      r.l += wgt * e.l;
+      r.o += wgt * e.o;
+    }
+  }
+  return r;
 }
 
 // split geometry shared by the producer of the partials and their consumer

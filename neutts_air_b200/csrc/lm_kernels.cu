@@ -161,20 +161,16 @@ NT_DEVINL void gemv_epilogue(const GemvParams& p, int u, float (&d0)[NB], float 
     const int pos = __ldcg(p.kv.seq_lens + b);
     const int n_kv = p.kv.n_kv_heads;
     if (head < p.n_heads + n_kv) {
-      // rows (i, i+32) of a q/k head: half-split rotation (modeling_qwen2.py:116-146)
-      float s, c;
-      sincosf(static_cast<float>(pos) * __ldg(p.inv_freq + i), &s, &c);
-      const float lo = a0 * c - a1 * s;
-      const float hi = a1 * c + a0 * s;
+      const float2 r = rope_pair(a0, a1, pos, __ldg(p.inv_freq + i));
       if (head < p.n_heads) {
         float* q = p.q_out + (static_cast<long long>(b) * p.n_heads + head) * 64;
-        q[i] = lo;
-        q[i + 32] = hi;
+        q[i] = r.x;
+        q[i + 32] = r.y;
       } else if (pos < p.kv.max_ctx) {
         const int page = __ldcg(p.kv.page_table + b * p.kv.max_pages_per_seq + (pos >> 6));
         __nv_bfloat16* kp = p.kv.page_ptr(p.layer, 0, page, head - p.n_heads) + (pos & 63) * 64;
-        kp[i] = __float2bfloat16(lo);
-        kp[i + 32] = __float2bfloat16(hi);
+        kp[i] = __float2bfloat16(r.x);
+        kp[i + 32] = __float2bfloat16(r.y);
       }
     } else if (pos < p.kv.max_ctx) {
       const int page = __ldcg(p.kv.page_table + b * p.kv.max_pages_per_seq + (pos >> 6));
@@ -453,13 +449,12 @@ __global__ void __launch_bounds__(32 * kAttnWarps) attn_decode_kernel(const Attn
   uint32_t parity = 0;
   const __nv_bfloat16* kb = sm->k[pair] + (sub * 32 + lane) * 64;  // this lane's token row of the page
   const __nv_bfloat16* vb = sm->v[pair] + sub * 32 * 64;           // this warp's 32 token rows
-  const int krow_layer = p.layer * 2 * p.kv.num_pages * p.kv.n_kv_heads * 64;  // K rows of this layer in the pool
   for (int pg = pair; pg < npages; pg += kAttnPairs) {
     if (sub == 0 && lane == 0) {
       const int page = __ldcg(p.kv.page_table + b * p.kv.max_pages_per_seq + pg);
       asm volatile("fence.proxy.async;" ::: "memory");
       mbar_arrive_expect_tx(&sm->bar[pair], 2 * 8192);
-      tma_load_2d(sm->k[pair], &kmap, 0, krow_layer + (page * p.kv.n_kv_heads + kvh) * 64, &sm->bar[pair]);
+      tma_load_2d(sm->k[pair], &kmap, 0, p.kv.tmap_row(p.layer, 0, page, kvh), &sm->bar[pair]);
       bulk_g2s(sm->v[pair], p.kv.page_ptr(p.layer, 1, page, kvh), 8192, &sm->bar[pair]);
     }
     mbar_wait(&sm->bar[pair], parity);
@@ -524,26 +519,18 @@ __global__ void __launch_bounds__(32 * kAttnWarps) attn_decode_kernel(const Attn
   __syncthreads();
   for (int i = tid; i < n_rep * 64; i += 32 * kAttnWarps) {
     const int h = i >> 6, d = i & 63;
-    float M = -INFINITY;
-#pragma unroll
-    for (int w = 0; w < kAttnWarps; ++w) M = fmaxf(M, sm->ml[w][h][0]);
-    float L = 0.f, O = 0.f;
-#pragma unroll
-    for (int w = 0; w < kAttnWarps; ++w) {
-      const float wgt = exp2f(sm->ml[w][h][0] - M);  // 0 for a warp that saw no token (m = -inf, l = 0)
-      L += wgt * sm->ml[w][h][1];
-      O += wgt * sm->o[w][h][d];
-    }
+    // captured by value: by reference, ptxas gives this kernel 2 more registers (CUDA 12.9)
+    const SoftmaxPart r = merge_parts<kAttnWarps>(kAttnWarps, [=](int w) { return SoftmaxPart{sm->ml[w][h][0], sm->ml[w][h][1], sm->o[w][h][d]}; });
     const long long hh = static_cast<long long>(b) * p.n_heads + kvh * n_rep + h;
-    if (p.out) p.out[hh * 64 + d] = O / L;
-    if (p.out_bf16) p.out_bf16[hh * 64 + d] = __float2bfloat16(O / L);
+    if (p.out) p.out[hh * 64 + d] = r.o / r.l;
+    if (p.out_bf16) p.out_bf16[hh * 64 + d] = __float2bfloat16(r.o / r.l);
   }
 }
 
 
 // Batched-decode variant on tensor cores (batch > 4, where GEMM inputs are bf16 anyway): same CTA shape -- one CTA
 // per (sequence, kv head), warps walk pages warp, warp+8, ... through private 16 KB K/V buffers (both pages by
-// swizzled TMA) -- but a page is two rounds of mma.sync: S[16 x 64] = Q K^T with the n_rep query heads in rows
+// swizzled TMA) -- but a page is one attn_page_step: S[16 x 64] = Q K^T with the n_rep query heads in rows
 // 0..n_rep-1 of the A tile (rows 8..15 are zero), online softmax on the accumulator fragments, O += P V with P
 // rounded to bf16.  ~150 instructions per page instead of ~2 200 on the fp32 path.
 struct AttnMmaSmem {
@@ -552,7 +539,7 @@ struct AttnMmaSmem {
   float o[8][8][64];   // per-warp unnormalised outputs [head][dim]
   float ml[8][8][2];
   uint64_t bar[8];
-  float q[8][64];      // fused prologue: this group's rotated queries, the new token's K / V row
+  float q[8][64];      // prologue: this group's rotated queries, the new token's K / V row
   float knew[64], vnew[64];
 };
 __global__ void __launch_bounds__(256) attn_decode_mma_kernel(const AttnDecParams p, const __grid_constant__ CUtensorMap kvmap) {
@@ -570,68 +557,40 @@ __global__ void __launch_bounds__(256) attn_decode_mma_kernel(const AttnDecParam
   const int pos = __ldcg(p.kv.seq_lens + b);   // position of the new token
   const int n_ctx = min(pos + 1, p.kv.max_ctx);
   const int npages = (n_ctx + 63) >> 6;
-  const int g = lane >> 2, t = lane & 3, lrow = lane & 7, lmat = lane >> 3;
-  const bool fused = p.qkv != nullptr;
-  const bool appends = fused && pos < p.kv.max_ctx;
-  if (fused) {
-    // RoPE + KV append of this (sequence, kv head) -- what rope_append_kernel did in a launch of its own: pair u of a
-    // head holds dims (i, i + 32) (rows are pair-interleaved at pack time), V is plain.  Slices summed in slice order.
-    const float* row = p.qkv + static_cast<long long>(b) * p.qkv_n;
-    const int n_kv = p.kv.n_kv_heads;
-    for (int idx = tid; idx < (n_rep + 2) * 32; idx += 256) {
-      const int which = idx < n_rep * 32 ? 0 : (idx < n_rep * 32 + 32 ? 1 : 2);
-      const int i = idx & 31;
-      const int col = (which == 0 ? (kvh * n_rep + (idx >> 5)) : (which == 1 ? p.n_heads + kvh : p.n_heads + n_kv + kvh)) * 64 + 2 * i;
-      float2 v = __ldcg(reinterpret_cast<const float2*>(row + col));
-      for (int z = 1; z < p.qkv_parts; ++z) {
-        const float2 w = __ldcg(reinterpret_cast<const float2*>(row + z * p.qkv_pstride + col));
-        v.x += w.x, v.y += w.y;
-      }
-      if (which == 2) {
-        sm->vnew[2 * i] = v.x, sm->vnew[2 * i + 1] = v.y;
-      } else {
-        float sn, cs;
-        sincosf(static_cast<float>(pos) * __ldg(p.inv_freq + i), &sn, &cs);
-        const float lo = v.x * cs - v.y * sn, hi = v.y * cs + v.x * sn;
-        if (which == 0) sm->q[idx >> 5][i] = lo, sm->q[idx >> 5][i + 32] = hi;
-        else sm->knew[i] = lo, sm->knew[i + 32] = hi;
-      }
+  const bool appends = pos < p.kv.max_ctx;
+  // RoPE + KV append of this (sequence, kv head) -- what rope_append_kernel did in a launch of its own: pair u of a
+  // head holds dims (i, i + 32) (rows are pair-interleaved at pack time), V is plain.  Slices summed in slice order.
+  const float* row = p.qkv + static_cast<long long>(b) * p.qkv_n;
+  const int n_kv = p.kv.n_kv_heads;
+  for (int idx = tid; idx < (n_rep + 2) * 32; idx += 256) {
+    const int which = idx < n_rep * 32 ? 0 : (idx < n_rep * 32 + 32 ? 1 : 2);
+    const int i = idx & 31;
+    const int col = (which == 0 ? (kvh * n_rep + (idx >> 5)) : (which == 1 ? p.n_heads + kvh : p.n_heads + n_kv + kvh)) * 64 + 2 * i;
+    float2 v = __ldcg(reinterpret_cast<const float2*>(row + col));
+    for (int z = 1; z < p.qkv_parts; ++z) {
+      const float2 w = __ldcg(reinterpret_cast<const float2*>(row + z * p.qkv_pstride + col));
+      v.x += w.x, v.y += w.y;
     }
-    __syncthreads();
-    if (appends && tid < 64) {   // the row joins the cache for the steps to come; this step patches it into the staged page
-      const int page = __ldcg(p.kv.page_table + b * p.kv.max_pages_per_seq + (pos >> 6));
-      p.kv.page_ptr(p.layer, 0, page, kvh)[(pos & 63) * 64 + tid] = __float2bfloat16(sm->knew[tid]);
-      p.kv.page_ptr(p.layer, 1, page, kvh)[(pos & 63) * 64 + tid] = __float2bfloat16(sm->vnew[tid]);
+    if (which == 2) {
+      sm->vnew[2 * i] = v.x, sm->vnew[2 * i + 1] = v.y;
+    } else {
+      const float2 r = rope_pair(v.x, v.y, pos, __ldg(p.inv_freq + i));
+      if (which == 0) sm->q[idx >> 5][i] = r.x, sm->q[idx >> 5][i + 32] = r.y;
+      else sm->knew[i] = r.x, sm->knew[i + 32] = r.y;
     }
   }
-  // query fragments: row g = head g of the group (rows >= n_rep and rows 8..15 are zero)
+  __syncthreads();
+  if (appends && tid < 64) {   // the row joins the cache for the steps to come; this step patches it into the staged page
+    const int page = __ldcg(p.kv.page_table + b * p.kv.max_pages_per_seq + (pos >> 6));
+    p.kv.page_ptr(p.layer, 0, page, kvh)[(pos & 63) * 64 + tid] = __float2bfloat16(sm->knew[tid]);
+    p.kv.page_ptr(p.layer, 1, page, kvh)[(pos & 63) * 64 + tid] = __float2bfloat16(sm->vnew[tid]);
+  }
   uint32_t qa[4][4];
-  {
-    const float* qp = fused ? sm->q[min(g, n_rep - 1)]
-                            : p.q + (static_cast<long long>(b) * p.n_heads + kvh * n_rep + min(g, n_rep - 1)) * 64;
-    const float sc = (g < n_rep) ? p.scale_log2 : 0.f;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float2 a0, a2;
-      if (fused) {   // shared memory
-        a0 = *reinterpret_cast<const float2*>(qp + 16 * j + 2 * t);
-        a2 = *reinterpret_cast<const float2*>(qp + 16 * j + 8 + 2 * t);
-      } else {
-        a0 = __ldcg(reinterpret_cast<const float2*>(qp + 16 * j + 2 * t));
-        a2 = __ldcg(reinterpret_cast<const float2*>(qp + 16 * j + 8 + 2 * t));
-      }
-      qa[j][0] = pack_bf16x2(a0.x * sc, a0.y * sc);
-      qa[j][1] = 0u;
-      qa[j][2] = pack_bf16x2(a2.x * sc, a2.y * sc);
-      qa[j][3] = 0u;
-    }
-  }
+  decode_query_frags(&sm->q[0][0], n_rep, p.scale_log2, qa);
   float o[8][4];
 #pragma unroll
   for (int n = 0; n < 8; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
-  float m0 = -INFINITY, l0 = 0.f;
-  const int krow0 = p.layer * 2 * p.kv.num_pages * p.kv.n_kv_heads * 64;
-  const int vrow0 = krow0 + p.kv.num_pages * p.kv.n_kv_heads * 64;
+  float m[1] = {-INFINITY}, l[1] = {0.f};
   const uint32_t kbase = smem_u32(sm->k[warp]), vbase = smem_u32(sm->v[warp]);
   uint32_t parity = 0;
   for (int pg = warp; pg < npages; pg += 8) {
@@ -639,93 +598,24 @@ __global__ void __launch_bounds__(256) attn_decode_mma_kernel(const AttnDecParam
       const int page = __ldcg(p.kv.page_table + b * p.kv.max_pages_per_seq + pg);
       asm volatile("fence.proxy.async;" ::: "memory");
       mbar_arrive_expect_tx(&sm->bar[warp], 2 * 8192);
-      tma_load_2d(sm->k[warp], &kvmap, 0, krow0 + (page * p.kv.n_kv_heads + kvh) * 64, &sm->bar[warp]);
-      tma_load_2d(sm->v[warp], &kvmap, 0, vrow0 + (page * p.kv.n_kv_heads + kvh) * 64, &sm->bar[warp]);
+      tma_load_2d(sm->k[warp], &kvmap, 0, p.kv.tmap_row(p.layer, 0, page, kvh), &sm->bar[warp]);
+      tma_load_2d(sm->v[warp], &kvmap, 0, p.kv.tmap_row(p.layer, 1, page, kvh), &sm->bar[warp]);
     }
     mbar_wait(&sm->bar[warp], parity);
     parity ^= 1;
-    if (appends && pg == (pos >> 6)) {   // patch the staged page with the new row (the copy may predate the store above)
-      const int r = pos & 63;
-      const int off = r * 128 + ((((2 * lane) >> 3) ^ (r & 7)) << 4) + ((2 * lane) & 7) * 2;
-      *reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(sm->k[warp]) + off) = pack_bf16x2(sm->knew[2 * lane], sm->knew[2 * lane + 1]);
-      *reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(sm->v[warp]) + off) = pack_bf16x2(sm->vnew[2 * lane], sm->vnew[2 * lane + 1]);
-      __syncwarp();
-    }
-    float sc[8][4];
-#pragma unroll
-    for (int n = 0; n < 8; ++n) {
-      sc[n][0] = sc[n][1] = sc[n][2] = sc[n][3] = 0.f;
-      const int row = 8 * n + lrow;
-#pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        uint32_t kb[4];
-        ldmatrix_x4(kb, kbase + row * 128 + (((4 * half + lmat) ^ lrow) << 4));
-        mma_bf16_16816(sc[n], qa[2 * half], kb[0], kb[1]);
-        mma_bf16_16816(sc[n], qa[2 * half + 1], kb[2], kb[3]);
-      }
-    }
+    if (appends && pg == (pos >> 6)) patch_staged_row(sm->k[warp], sm->v[warp], pos & 63, sm->knew, sm->vnew);
     const int k0 = pg * 64;
-    if (k0 + 64 > n_ctx) {
-#pragma unroll
-      for (int n = 0; n < 8; ++n) {
-        const int kv0 = k0 + 8 * n + 2 * t;
-        if (kv0 >= n_ctx) sc[n][0] = -INFINITY;
-        if (kv0 + 1 >= n_ctx) sc[n][1] = -INFINITY;
-      }
-    }
-    float mx = -INFINITY;
-#pragma unroll
-    for (int n = 0; n < 8; ++n) mx = fmaxf(mx, fmaxf(sc[n][0], sc[n][1]));
-    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1)), mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-    const float mn = fmaxf(m0, mx);  // the first token of every page walked is valid -> finite
-    const float c = exp2f(m0 - mn);
-    m0 = mn;
-    l0 *= c;
-#pragma unroll
-    for (int n = 0; n < 8; ++n) o[n][0] *= c, o[n][1] *= c;
-    uint32_t pa[4][4];
-#pragma unroll
-    for (int n = 0; n < 8; ++n) {
-      const float p0 = exp2f(sc[n][0] - mn), p1 = exp2f(sc[n][1] - mn);
-      l0 += p0 + p1;
-      pa[n >> 1][(n & 1) * 2 + 0] = pack_bf16x2(p0, p1);
-      pa[n >> 1][(n & 1) * 2 + 1] = 0u;
-    }
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int row = 16 * j + 8 * (lmat & 1) + lrow;
-#pragma unroll
-      for (int nd = 0; nd < 8; nd += 2) {
-        uint32_t vb[4];
-        ldmatrix_x4_trans(vb, vbase + row * 128 + (((nd + (lmat >> 1)) ^ lrow) << 4));
-        mma_bf16_16816(o[nd], pa[j], vb[0], vb[1]);
-        mma_bf16_16816(o[nd + 1], pa[j], vb[2], vb[3]);
-      }
-    }
+    attn_page_step<1>(kbase, vbase, qa, o, m, l, k0 + 64 > n_ctx, [&](int, int key) { return k0 + key >= n_ctx; });
     __syncwarp();  // all lanes are done with the buffers before lane 0 refills them
   }
-  l0 += __shfl_xor_sync(0xffffffffu, l0, 1), l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-  if (g < n_rep) {
-#pragma unroll
-    for (int n = 0; n < 8; ++n) *reinterpret_cast<float2*>(&sm->o[warp][g][8 * n + 2 * t]) = make_float2(o[n][0], o[n][1]);
-    if (t == 0) sm->ml[warp][g][0] = m0, sm->ml[warp][g][1] = l0;
-  }
+  decode_store_partial(o, m[0], l[0], n_rep, &sm->o[warp][0][0], &sm->ml[warp][0][0]);
   __syncthreads();
   for (int i = tid; i < n_rep * 64; i += 256) {
     const int h = i >> 6, d = i & 63;
-    float M = -INFINITY;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) M = fmaxf(M, sm->ml[w][h][0]);
-    float L = 0.f, O = 0.f;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) {
-      const float wgt = exp2f(sm->ml[w][h][0] - M);  // 0 for a warp that walked no page (m = -inf, l = 0)
-      L += wgt * sm->ml[w][h][1];
-      O += wgt * sm->o[w][h][d];
-    }
+    const SoftmaxPart r = merge_parts<8>(8, [=](int w) { return SoftmaxPart{sm->ml[w][h][0], sm->ml[w][h][1], sm->o[w][h][d]}; });
     const long long hh = static_cast<long long>(b) * p.n_heads + kvh * n_rep + h;
-    if (p.out) p.out[hh * 64 + d] = O / L;
-    if (p.out_bf16) p.out_bf16[hh * 64 + d] = __float2bfloat16(O / L);
+    if (p.out) p.out[hh * 64 + d] = r.o / r.l;
+    if (p.out_bf16) p.out_bf16[hh * 64 + d] = __float2bfloat16(r.o / r.l);
   }
 }
 
@@ -735,6 +625,7 @@ int launch_attn_decode(const AttnDecParams& p, int B, int n_layers, cudaStream_t
   CUtensorMap kmap;
   if (int rc = kv_pool_tmap(p.kv, n_layers, &kmap)) return rc;
   if (B > 4) {  // tensor-core variant: bf16 query / probabilities, like every other GEMM input of the batched path
+    if (!p.qkv) return set_error(NT_ERR_INVALID, "attention: batch %d > 4 needs the fused RoPE + KV append (qkv)", B);
     const int msmem = int(sizeof(AttnMmaSmem)) + 1024;
     return launch_kernel(attn_decode_mma_kernel, dim3(p.kv.n_kv_heads, B), dim3(256), msmem, stream, true, p, kmap);
   }
@@ -1069,16 +960,14 @@ __global__ void __launch_bounds__(256) rope_append_kernel(const float* qkv, int 
   const int b = tok_seq[t], pos = tok_pos[t];
   const int n_kv = kv.n_kv_heads;
   if (head < n_heads + n_kv) {
-    float s, c;
-    sincosf(static_cast<float>(pos) * inv_freq[i], &s, &c);
-    const float lo = v.x * c - v.y * s, hi = v.y * c + v.x * s;
+    const float2 r = rope_pair(v.x, v.y, pos, inv_freq[i]);
     if (head < n_heads) {
       float* q = q_out + (static_cast<long long>(t) * n_heads + head) * 64;
-      q[i] = lo, q[i + 32] = hi;
+      q[i] = r.x, q[i + 32] = r.y;
     } else {
       const int page = kv.page_table[b * kv.max_pages_per_seq + (pos >> 6)];
       __nv_bfloat16* kp = kv.page_ptr(layer, 0, page, head - n_heads) + (pos & 63) * 64;
-      kp[i] = __float2bfloat16(lo), kp[i + 32] = __float2bfloat16(hi);
+      kp[i] = __float2bfloat16(r.x), kp[i + 32] = __float2bfloat16(r.y);
     }
   } else {
     const int page = kv.page_table[b * kv.max_pages_per_seq + (pos >> 6)];
@@ -1097,9 +986,8 @@ int launch_rope_append(const float* qkv, int T, int qkv_n, const int32_t* tok_se
 // grid (ceil(max_len/16), n_kv_heads, B), n_rep warps: a CTA owns 16 query tokens of one sequence and one KV head;
 // warp h holds the 16 x 64 query tile of head kvh*n_rep + h as A fragments (bf16, softmax scale * log2e folded in)
 // and all warps share the K/V tiles.  A KV tile is one 64-token page: K and V land in shared memory through the
-// SWIZZLE_128B pool descriptor (double-buffered, one mbarrier per buffer), B fragments come from ldmatrix
-// (K: plain, V: .trans) with the swizzle applied to the row addresses.  Online softmax in the log2 domain on the
-// accumulator fragments (quad shuffles for row statistics); P is rounded to bf16 for the P.V MMA (as in
+// SWIZZLE_128B pool descriptor (double-buffered, one mbarrier per buffer); each warp runs attn_page_step on it with
+// both 8-row halves of its query tile live (log2-domain online softmax, P rounded to bf16 for the P.V MMA as in
 // FlashAttention-2).  Replaces a CUDA-core kernel that took 81 % of the prefill (451 us per layer at batch 1).
 constexpr int kPfQ = 16;
 __global__ void __launch_bounds__(256) attn_prefill_kernel(const AttnPrefillParams p, const __grid_constant__ CUtensorMap kvmap) {
@@ -1121,15 +1009,13 @@ __global__ void __launch_bounds__(256) attn_prefill_kernel(const AttnPrefillPara
   __syncthreads();
   const int kend = min(len, q0 + kPfQ);      // keys [0, kend) are visible to some query of this block
   const int ntiles = (kend + 63) >> 6;
-  const int krow0 = p.layer * 2 * p.kv.num_pages * p.kv.n_kv_heads * 64;
-  const int vrow0 = krow0 + p.kv.num_pages * p.kv.n_kv_heads * 64;
   auto issue = [&](int tile) {
     const int page = __ldg(p.kv.page_table + b * p.kv.max_pages_per_seq + tile);
     const int buf = tile & 1;
     asm volatile("fence.proxy.async;" ::: "memory");
     mbar_arrive_expect_tx(&full_bar[buf], 2 * 8192);
-    tma_load_2d(sK[buf], &kvmap, 0, krow0 + (page * p.kv.n_kv_heads + kvh) * 64, &full_bar[buf]);
-    tma_load_2d(sV[buf], &kvmap, 0, vrow0 + (page * p.kv.n_kv_heads + kvh) * 64, &full_bar[buf]);
+    tma_load_2d(sK[buf], &kvmap, 0, p.kv.tmap_row(p.layer, 0, page, kvh), &full_bar[buf]);
+    tma_load_2d(sV[buf], &kvmap, 0, p.kv.tmap_row(p.layer, 1, page, kvh), &full_bar[buf]);
   };
   if (tid == 0) issue(0);
 
@@ -1156,81 +1042,22 @@ __global__ void __launch_bounds__(256) attn_prefill_kernel(const AttnPrefillPara
   float o[8][4];
 #pragma unroll
   for (int n = 0; n < 8; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
-  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;  // rows g / g + 8 (l: this lane's partial sum)
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};  // rows g / g + 8 (l: this lane's partial sum)
   const int qi0 = q0 + g, qi1 = q0 + g + 8;
-  // ldmatrix row address pieces: lane supplies row (lane & 7) of matrix (lane >> 3)
-  const int lrow = lane & 7, lmat = lane >> 3;
 
   for (int tile = 0; tile < ntiles; ++tile) {
     const int buf = tile & 1;
     __syncthreads();  // every warp is done with the buffer the next copy overwrites
     if (tid == 0 && tile + 1 < ntiles) issue(tile + 1);
     mbar_wait(&full_bar[buf], (tile >> 1) & 1);
-    const uint32_t kbase = smem_u32(sK[buf]), vbase = smem_u32(sV[buf]);
-
-    // S = Q K^T : 8 key groups of 8 tokens
-    float sc[8][4];
-#pragma unroll
-    for (int n = 0; n < 8; ++n) {
-      sc[n][0] = sc[n][1] = sc[n][2] = sc[n][3] = 0.f;
-      const int row = 8 * n + lrow;  // key token within the tile; row & 7 == lrow
-#pragma unroll
-      for (int half = 0; half < 2; ++half) {  // dims 0..31 / 32..63: 4 chunks of 8 dims each
-        uint32_t kb[4];
-        ldmatrix_x4(kb, kbase + row * 128 + (((4 * half + lmat) ^ lrow) << 4));
-        mma_bf16_16816(sc[n], qa[2 * half], kb[0], kb[1]);
-        mma_bf16_16816(sc[n], qa[2 * half + 1], kb[2], kb[3]);
-      }
-    }
     // causal / length mask (only tiles that reach past the first query of the block need it)
     const int k0 = tile * 64;
-    if (k0 + 63 > q0 || k0 + 64 > len) {
-#pragma unroll
-      for (int n = 0; n < 8; ++n) {
-        const int kv0 = k0 + 8 * n + 2 * t;
-        if (kv0 > qi0 || kv0 >= len) sc[n][0] = -INFINITY;
-        if (kv0 + 1 > qi0 || kv0 + 1 >= len) sc[n][1] = -INFINITY;
-        if (kv0 > qi1 || kv0 >= len) sc[n][2] = -INFINITY;
-        if (kv0 + 1 > qi1 || kv0 + 1 >= len) sc[n][3] = -INFINITY;
-      }
-    }
-    // online softmax (base 2)
-    float mx0 = -INFINITY, mx1 = -INFINITY;
-#pragma unroll
-    for (int n = 0; n < 8; ++n) mx0 = fmaxf(mx0, fmaxf(sc[n][0], sc[n][1])), mx1 = fmaxf(mx1, fmaxf(sc[n][2], sc[n][3]));
-    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)), mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
-    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)), mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
-    const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);  // key 0 is visible to every query: finite from tile 0 on
-    const float c0 = exp2f(m0 - mn0), c1 = exp2f(m1 - mn1);
-    m0 = mn0, m1 = mn1;
-    l0 *= c0, l1 *= c1;
-#pragma unroll
-    for (int n = 0; n < 8; ++n) o[n][0] *= c0, o[n][1] *= c0, o[n][2] *= c1, o[n][3] *= c1;
-    uint32_t pa[4][4];  // P as A fragments: k-step j covers key groups 2j, 2j+1
-#pragma unroll
-    for (int n = 0; n < 8; ++n) {
-      const float p00 = exp2f(sc[n][0] - mn0), p01 = exp2f(sc[n][1] - mn0);
-      const float p10 = exp2f(sc[n][2] - mn1), p11 = exp2f(sc[n][3] - mn1);
-      l0 += p00 + p01, l1 += p10 + p11;
-      pa[n >> 1][(n & 1) * 2 + 0] = pack_bf16x2(p00, p01);
-      pa[n >> 1][(n & 1) * 2 + 1] = pack_bf16x2(p10, p11);
-    }
-    // O += P V : k-steps of 16 keys, output dim groups of 8 (two per ldmatrix)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int row = 16 * j + 8 * (lmat & 1) + lrow;  // key token; row & 7 == lrow
-#pragma unroll
-      for (int nd = 0; nd < 8; nd += 2) {
-        uint32_t vb[4];
-        ldmatrix_x4_trans(vb, vbase + row * 128 + (((nd + (lmat >> 1)) ^ lrow) << 4));
-        mma_bf16_16816(o[nd], pa[j], vb[0], vb[1]);
-        mma_bf16_16816(o[nd + 1], pa[j], vb[2], vb[3]);
-      }
-    }
+    attn_page_step<2>(smem_u32(sK[buf]), smem_u32(sV[buf]), qa, o, m, l, k0 + 63 > q0 || k0 + 64 > len, [&](int half, int key) {
+      const int kv = k0 + key;
+      return kv > (half ? qi1 : qi0) || kv >= len;
+    });
   }
-  l0 += __shfl_xor_sync(0xffffffffu, l0, 1), l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-  l1 += __shfl_xor_sync(0xffffffffu, l1, 1), l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-  const float i0 = 1.0f / l0, i1 = 1.0f / l1;
+  const float i0 = 1.0f / quad_sum(l[0]), i1 = 1.0f / quad_sum(l[1]);
   __nv_bfloat16* o0p = p.out + (static_cast<long long>(t0 + qi0) * p.n_heads + head) * 64 + 2 * t;
   __nv_bfloat16* o1p = p.out + (static_cast<long long>(t0 + qi1) * p.n_heads + head) * 64 + 2 * t;
 #pragma unroll

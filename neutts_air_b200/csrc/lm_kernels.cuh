@@ -16,6 +16,12 @@ struct KVLayout {
   NT_DEVINL __nv_bfloat16* page_ptr(int layer, int is_v, int page, int kvh) const {
     return pages + layer * layer_stride + is_v * kv_stride + (static_cast<long long>(page) * n_kv_heads + kvh) * 4096;
   }
+  // first row of the same page in the pool map of kv_pool_tmap (rows of 64 bf16; fits in int, kv_pool_tmap checks).
+  // The page-independent part stands apart: in this shape ptxas spills no more in decode_tc_kernel than with the row
+  // of the layer computed ahead of the page lookup.
+  NT_DEVINL int tmap_row(int layer, int is_v, int page, int kvh) const {
+    return (layer * 2 * num_pages * n_kv_heads + kvh) * 64 + (is_v * num_pages + page) * (n_kv_heads * 64);
+  }
 };
 
 enum GemvEpi { GEMV_STORE = 0, GEMV_SWIGLU = 1, GEMV_QKV_ROPE = 2 };
@@ -53,9 +59,9 @@ struct AttnDecParams {
   // Placed after the outputs: with scale_log2 right behind n_rep, ptxas gives both attention kernels
   // 5 / 12 more registers (sm_90a, CUDA 12.9).
   float scale_log2;  // head_dim^-0.5 * log2(e)
-  // Fused RoPE + KV append (tensor-core variant, batch > 4): when qkv != nullptr the kernel reads the projection output
-  // itself ([B, qkv_n] fp32, bias already added, `qkv_parts` split-K slices `qkv_pstride` floats apart, summed in slice
-  // order), rotates q / k at position seq_lens[b], appends the new K/V row to the cache and ignores `q`.
+  // Fused RoPE + KV append, required by the tensor-core variant (batch > 4), which ignores `q`: the kernel reads the
+  // projection output itself ([B, qkv_n] fp32, bias already added, `qkv_parts` split-K slices `qkv_pstride` floats
+  // apart, summed in slice order), rotates q / k at position seq_lens[b] and appends the new K/V row to the cache.
   const float* qkv;
   int qkv_n, qkv_parts;
   long long qkv_pstride;
