@@ -1,7 +1,9 @@
-"""Shared test plumbing: oracle weights -> HF-style state dicts -> CUDA engines."""
+"""Shared test plumbing: oracle weights -> HF-style state dicts -> CUDA engines, error measures, and the rule that picks
+the decode path."""
 from __future__ import annotations
 
 import math
+import warnings
 
 import torch
 
@@ -67,10 +69,12 @@ def max_err(a: torch.Tensor, b: torch.Tensor) -> float:
 
 
 def rel_rms(got, ref) -> float:
-    """Relative RMS error; inf when ``got`` holds a NaN or an inf (so that max() over errors cannot drop it)."""
+    """Relative RMS error of torch tensors, numpy arrays or lists; inf when ``got`` holds a NaN or an inf (so that max()
+    over errors cannot drop it)."""
+    got, ref = torch.as_tensor(got, dtype=torch.float64), torch.as_tensor(ref, dtype=torch.float64)
     if not torch.isfinite(got).all():
         return math.inf
-    return float((got.double() - ref.double()).norm() / ref.double().norm().clamp_min(1e-300))
+    return float((got - ref).norm() / ref.norm().clamp_min(1e-300))
 
 
 def gather_kv(lm, layer: int, b: int, n: int):
@@ -84,3 +88,57 @@ def gather_kv(lm, layer: int, b: int, n: int):
         t = lm.kv[layer, which].index_select(0, pages)                     # [npg, n_kv, 64, 64]
         out.append(t.permute(0, 2, 1, 3).reshape(npg * page, t.shape[1], 64)[:n].double().cpu())
     return out[0], out[1]
+
+
+# The decode path nt_lm_decode (lm_api.cu) takes: with NT_DECODE_IMPL unset, the persistent kernel up to
+# kTcDefaultMaxBatch sequences (lm_decode_tc.cuh) and the per-op chain above; "tc" or "perop" forces one.  The chain
+# runs its projections, and every lm_head its GEMV, up to kGemvMaxBatch rows (lm_kernels.cuh), wgmma GEMMs above.
+# test_decode_plan.py checks both constants against the headers.
+TC_DEFAULT_MAX_BATCH = 16
+GEMV_MAX_BATCH = 4
+
+
+def set_decode_impl(monkeypatch, impl):
+    """Force the decode path with NT_DECODE_IMPL = ``impl``, or leave the choice to the engine when ``impl`` is None."""
+    if impl:
+        monkeypatch.setenv("NT_DECODE_IMPL", impl)
+    else:
+        monkeypatch.delenv("NT_DECODE_IMPL", raising=False)
+
+
+def runs_persistent(impl, B: int) -> bool:
+    """Whether a decode at batch B runs the persistent kernel after ``set_decode_impl(monkeypatch, impl)``."""
+    return impl == "tc" or (impl is None and B <= TC_DEFAULT_MAX_BATCH)
+
+
+# ------------------------------------------------------------------------------- a small engine and its bar, a facade
+SMALL = dict(vocab_size=4096, hidden_size=256, intermediate_size=640, num_layers=3, num_heads=4, num_kv_heads=2)
+
+
+def _setup(max_batch, max_ctx=256, **kw):
+    cfg = lm_oracle.LMConfig.tiny(**SMALL)
+    w = lm_oracle.random_weights(cfg, 21, std=0.05, bf16_round=True)
+    return cfg, w, make_lm(cfg, w, max_batch=max_batch, max_ctx=max_ctx, **kw)
+
+
+def _bar(got, mir, tag):
+    r = rel_err(got, mir)
+    print(f"REFILL-PARITY {tag}: relRMS {r:.2e} max/std {max_err(got, mir) / float(mir.std()):.2e}")
+    assert r < 6e-3 and max_err(got, mir) < 5e-2 * float(mir.std()), (tag, r, max_err(got, mir))
+
+
+def _tts(max_batch=1, seed=7):
+    from neutts import NeuTTS
+    from tests.fakes import FakePhonemizer, SmallTok
+
+    cfg = lm_oracle.LMConfig.tiny(vocab_size=4096, hidden_size=256, intermediate_size=512, num_layers=2, num_heads=4,
+                                  num_kv_heads=2)
+    w = lm_oracle.random_weights(cfg, 3, std=0.05, bf16_round=True)
+    lm = make_lm(cfg, w, max_batch=max_batch, max_ctx=2048, max_new=512)
+    ccfg = codec_oracle.CodecConfig.tiny()
+    dec = make_codec(ccfg, codec_oracle.random_weights(ccfg, 2), max_batch=max_batch, max_frames=512)
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore")
+        tts = NeuTTS(tokenizer=SmallTok(), phonemizer=FakePhonemizer(), backbone=lm, codec=dec, max_batch=max_batch, seed=seed)
+    tts.max_context = 2048
+    return tts, ccfg

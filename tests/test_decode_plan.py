@@ -127,3 +127,17 @@ def test_bad_arguments_are_refused():
         debug_decode_plan(960, 4864, 15, 5, 20546, 132, False)     # hidden 960 > 896
     with pytest.raises(ValueError, match="multiples of 64"):
         debug_decode_plan(896, 4800 + 32, 14, 2, 20546, 132, False)
+
+
+def test_decode_path_constants_match_the_headers():
+    """The batch limits the GPU tests predict the decode path with (tests/helpers.py) are the library's own."""
+    import os
+    import re
+
+    from tests.helpers import GEMV_MAX_BATCH, TC_DEFAULT_MAX_BATCH
+
+    csrc = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "neutts_air_b200", "csrc")
+    for header, name, want in (("lm_decode_tc.cuh", "kTcDefaultMaxBatch", TC_DEFAULT_MAX_BATCH),
+                               ("lm_kernels.cuh", "kGemvMaxBatch", GEMV_MAX_BATCH)):
+        m = re.search(rf"constexpr\s+int\s+{name}\s*=\s*(\d+)\s*;", open(os.path.join(csrc, header)).read())
+        assert m and int(m.group(1)) == want, (header, name, m and m.group(1), want)

@@ -41,7 +41,7 @@ def _worker(rank, world, port, q):
         import warnings
 
         from neutts import NeuTTS
-        from tests.test_host_logic import FakeBackbone, FakeCodec, FakePhonemizer, FakeTokenizer
+        from tests.fakes import FakeBackbone, FakeCodec, FakePhonemizer, FakeTokenizer
 
         tok = FakeTokenizer()
         with warnings.catch_warnings():

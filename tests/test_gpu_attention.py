@@ -31,7 +31,7 @@ import pytest
 import torch
 
 from oracle import lm_oracle as O
-from tests.helpers import gather_kv, make_lm, rel_rms
+from tests.helpers import GEMV_MAX_BATCH, gather_kv, make_lm, rel_rms, runs_persistent, set_decode_impl
 
 PAGE = 64
 LOG2E = 1.4426950408889634
@@ -271,16 +271,13 @@ def run_crafted_decode(cfg, w, lens, steps, impl, max_ctx, monkeypatch, seed):
     sp = lm.sampling(eos, min_new_tokens=0, forced=forced)
     lm.prefill([[int(t)] for t in torch.randint(0, eos, (B,), generator=g)], sp)
     torch.cuda.synchronize()
-    persistent = impl == "tc" or (impl is None and B <= 16)
-    rb = B > 8 if persistent else B > 4
+    persistent = runs_persistent(impl, B)
+    rb = B > 8 if persistent else B > GEMV_MAX_BATCH
     n_rep = cfg.num_heads // cfg.num_kv_heads
     for b, L in enumerate(lens):
         craft_slot(lm, b, L, project(cfg, w, int(forced[b, 0]), L, rb)[0], n_rep, g)
     lm.seq_lens[:B] = torch.tensor(lens, dtype=torch.int32, device=lm.device)
-    if impl:
-        monkeypatch.setenv("NT_DECODE_IMPL", impl)
-    else:
-        monkeypatch.delenv("NT_DECODE_IMPL", raising=False)
+    set_decode_impl(monkeypatch, impl)
     n0 = lm.L.nt_launch_count()
     logits = lm.decode(steps, sp, return_logits=True)
     torch.cuda.synchronize()

@@ -14,7 +14,7 @@ import pytest
 import torch
 
 from oracle import lm_oracle as LO
-from tests.helpers import make_lm
+from tests.helpers import make_lm, set_decode_impl
 
 pytestmark = pytest.mark.gpu
 
@@ -81,10 +81,7 @@ def _same(a, b) -> bool:
 @pytest.mark.parametrize("B,impl", [(3, "perop"), (17, None)], ids=["chain-b3", "chain-b17"])
 @pytest.mark.parametrize("case", list(CASES))
 def test_decode_graph_follows_setting(cuda, case, B, impl, monkeypatch):
-    if impl:
-        monkeypatch.setenv("NT_DECODE_IMPL", impl)
-    else:
-        monkeypatch.delenv("NT_DECODE_IMPL", raising=False)   # batch 17 takes the chain by default
+    set_decode_impl(monkeypatch, impl)   # batch 17 takes the chain by default
     cfg = LO.LMConfig.tiny(vocab_size=V, hidden_size=256, intermediate_size=512, num_layers=2, num_heads=4, num_kv_heads=2)
     lm = make_lm(cfg, LO.random_weights(cfg, 5, bf16_round=True), max_batch=B, max_ctx=256, max_new=64)
     g = torch.Generator().manual_seed(B)

@@ -1,41 +1,15 @@
 """GPU: the drop-in facade end to end on the H100 engines (synthetic weights, injected tokenizer /
 phonemizer): the reference's own smoke assertions (tests/test_neutts.py:55-58), batched inference,
 and streaming with the reference's window geometry."""
-import warnings
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import codec_oracle as CO
-from oracle import lm_oracle as LO
 from oracle import stream_oracle as SO
-from tests.helpers import make_codec, make_lm
-from tests.test_host_logic import FakePhonemizer, FakeTokenizer
+from tests.helpers import _tts
 
 pytestmark = pytest.mark.gpu
-
-
-class SmallTok(FakeTokenizer):
-    """FakeTokenizer squeezed into a 4096-token vocabulary: 1024 speech codes from id 3000."""
-
-    def __init__(self):
-        super().__init__(n_speech=1024)
-
-
-def _tts(max_batch=1, seed=7):
-    from neutts import NeuTTS
-
-    cfg = LO.LMConfig.tiny(vocab_size=4096, hidden_size=256, intermediate_size=512, num_layers=2, num_heads=4, num_kv_heads=2)
-    w = LO.random_weights(cfg, 3, std=0.05, bf16_round=True)
-    lm = make_lm(cfg, w, max_batch=max_batch, max_ctx=2048, max_new=512)
-    ccfg = CO.CodecConfig.tiny()
-    dec = make_codec(ccfg, CO.random_weights(ccfg, 2), max_batch=max_batch, max_frames=512)
-    with warnings.catch_warnings():
-        warnings.simplefilter("ignore")
-        tts = NeuTTS(tokenizer=SmallTok(), phonemizer=FakePhonemizer(), backbone=lm, codec=dec, max_batch=max_batch, seed=seed)
-    tts.max_context = 2048
-    return tts, ccfg
 
 
 def test_facade_infer_on_gpu():

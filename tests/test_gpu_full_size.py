@@ -13,7 +13,7 @@ import torch
 
 from neutts_air_b200 import synthetic
 from neutts_air_b200.lm import LMShape, SpeechLM
-from tests.helpers import max_err, rel_err
+from tests.helpers import max_err, rel_err, set_decode_impl
 
 pytestmark = pytest.mark.gpu
 
@@ -72,15 +72,14 @@ def test_decode_kernel_sampler_matches_standalone_sampler(full_lm, B, impl, monk
     it returns for a step, the stand-alone sampler op (``nt_op_topk_sample``, pinned to the HF processors +
     multinomial by tests/test_gpu_kernels.py) must pick the very same token: same top-50 set, same probabilities, same
     Philox counter (seed, slot, n_generated).  All three run ``sample_tiles_seq``, so the window and the token are also
-    held to the float64 sampler of test_gpu_sampler on the same logits and Philox draw.  Covers the EOS mask
+    held to the float64 sampler of sampler_ref.py on the same logits and Philox draw.  Covers the EOS mask
     (min_new_tokens) too."""
     import ctypes as C
 
     from neutts_air_b200 import _lib
-    from tests.test_gpu_sampler import BARS, draw_u, prob_err, ref_token, ref_window
+    from tests.sampler_ref import BARS, draw_u, prob_err, ref_token, ref_window
 
-    if impl:   # the per-op chain: tensor-core lm_head with tile maxima in its epilogue + topk_tiles_kernel
-        monkeypatch.setenv("NT_DECODE_IMPL", impl)
+    set_decode_impl(monkeypatch, impl)   # perop: tensor-core lm_head, tile maxima in its epilogue, topk_tiles_kernel
     lm, eos, n_steps = full_lm, 151670, 9
     L = _lib.lib()
     prompts = [_prompt(40 + 17 * i, 30 + i) for i in range(B)]

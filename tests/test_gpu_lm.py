@@ -13,7 +13,7 @@ import pytest
 import torch
 
 from oracle import lm_oracle as O
-from tests.helpers import make_lm, max_err, rel_err
+from tests.helpers import make_lm, max_err, rel_err, set_decode_impl
 
 pytestmark = pytest.mark.gpu
 
@@ -73,8 +73,7 @@ def test_lm_decode_path_tight(cuda, cfgkw, persistent, monkeypatch):
     CUDA-core chain (NT_DECODE_IMPL=perop).  A 1-token prompt followed by 70 teacher-forced steps exercises only the
     decode kernels (fp32-grade activations, bf16 KV; crosses the 64-token page boundary): against the mirrored
     oracle the only noise left is the rare flip of a bf16 K/V rounding -> 1e-3 relative RMS."""
-    if not persistent:
-        monkeypatch.setenv("NT_DECODE_IMPL", "perop")
+    set_decode_impl(monkeypatch, None if persistent else "perop")
     cfg, w, lm = _setup(cfgkw, 13, max_batch=1, max_ctx=256, page_shuffle_seed=5)
     g = torch.Generator().manual_seed(6)
     n_new, eos = 71, cfg.vocab_size - 1
@@ -94,8 +93,7 @@ def test_lm_decode_path_tight(cuda, cfgkw, persistent, monkeypatch):
 def test_lm_ragged_batch_prefill_and_decode(cuda, persistent, monkeypatch):
     """Ragged prompts packed back to back (no left padding); batch 3 decodes on the persistent wgmma kernel
     (default) or on the per-op CUDA-core chain (NT_DECODE_IMPL=perop)."""
-    if not persistent:
-        monkeypatch.setenv("NT_DECODE_IMPL", "perop")
+    set_decode_impl(monkeypatch, None if persistent else "perop")
     cfg, w, lm = _setup(SMALL, 21, max_batch=4, max_ctx=256)
     g = torch.Generator().manual_seed(9)
     lens, n_new, eos = [33, 64, 7], 5, cfg.vocab_size - 1
@@ -112,7 +110,7 @@ def test_lm_decode_impl_rejects_unknown_value(cuda, monkeypatch):
     cfg, w, lm = _setup(SMALL, 23, max_batch=1, max_ctx=128)
     sp = lm.sampling(cfg.vocab_size - 1, min_new_tokens=0, max_new_tokens=4)
     lm.prefill([[1, 2, 3]], sp)
-    monkeypatch.setenv("NT_DECODE_IMPL", "mega")
+    set_decode_impl(monkeypatch, "mega")
     with pytest.raises(ValueError, match="tc and perop"):
         lm.decode(2, sp)
 
@@ -124,8 +122,7 @@ def test_lm_batched_decode(cuda, B, impl, monkeypatch):
     with plain bf16 activations on N = 16 / 32 / 64 token columns (the default up to batch 16; larger batches forced
     with NT_DECODE_IMPL=tc), and the per-op chain (default from batch 17; forced at batch 7).  Prefill is the
     tensor-core path in every case, so the bar is the pure-reference one."""
-    if impl:
-        monkeypatch.setenv("NT_DECODE_IMPL", impl)
+    set_decode_impl(monkeypatch, impl)
     cfg, w, lm = _setup(SMALL, 31, max_batch=36, max_ctx=256)
     g = torch.Generator().manual_seed(2)
     lens = ([20, 41, 64, 65, 9, 30, 17, 80, 33, 5, 12, 70, 3, 44, 27, 90, 61, 8] * 2)[:B]

@@ -1,8 +1,8 @@
 """Checkpoints that transformers' Qwen2, Llama and Mistral classes write, loaded through ``loader.load_speech_lm`` and run
 on the kernels: ragged prefill and teacher-forced decode on every decode path, against the oracle and transformers.
 
-The checkpoints (written at test time by tests/test_loader_families.py's ``write_checkpoint``; 3 layers, peaked
-attention, norm weights and biases away from 1 and 0, even vocabularies that are not multiples of 128):
+The checkpoints (written at test time by tests/checkpoints.py's ``write_checkpoint``; 3 layers, peaked attention, norm
+weights and biases away from 1 and 0, even vocabularies that are not multiples of 128):
 
     air-qwen2            hidden 896, 14/2 heads, inter 4864, q/k/v biases, theta 1e6, eps 1e-6, tied, bf16 safetensors
     nano-llama           hidden 576, 9/3 heads, inter 1536, no biases, theta 1e5, eps 1e-5, tied, fp32 in 3+ shards
@@ -18,8 +18,8 @@ launch count.  Each case compares
       on the bf16 paths), on weights read from transformers' model and rounded to bf16 as the engine streams them;
   (b) against transformers' float64 model on the same directory, its Linear and Embedding weights rounded to bf16.
 A 1-token prompt with 70 decode steps on the two batch-1 paths checks decode where it alone wrote the cache.  The bars
-and the measured errors are in test_loader_families.GPU_BARS; test_loader_faults_exceed_the_gpu_bars there shows that
-each loader fault moves these logits by 10x the decode-only bar and 4x the widest ragged bar.
+and the measured errors are in checkpoints.GPU_BARS; test_loader_faults_exceed_the_gpu_bars in test_loader_families.py
+shows that each loader fault moves these logits by 10x the decode-only bar and 4x the widest ragged bar.
 """
 from __future__ import annotations
 
@@ -29,8 +29,8 @@ import pytest
 import torch
 
 from oracle import lm_oracle as O
-from tests.helpers import max_err, rel_rms
-from tests.test_loader_families import GPU_BARS, Ckpt, hf_model64, oracle_of, write_checkpoint
+from tests.checkpoints import GPU_BARS, Ckpt, hf_model64, oracle_of, write_checkpoint
+from tests.helpers import GEMV_MAX_BATCH, max_err, rel_rms, runs_persistent, set_decode_impl
 
 pytestmark = pytest.mark.gpu
 
@@ -81,11 +81,12 @@ def _card() -> str:
 
 def _mirrors(B: int, impl):
     """(prefill mirror, decode mirror, decode bar key) of the path at batch B."""
-    persistent = impl is None and B <= 16
-    pm = "prefill" if B <= 4 else "batched"
+    persistent = runs_persistent(impl, B)
+    gemv = B <= GEMV_MAX_BATCH
+    pm = "prefill" if gemv else "batched"
     if persistent:
         return pm, ("decode_tc" if B <= 8 else "batched"), ("decode-exact" if B <= 8 else "decode-bf16")
-    return pm, ("decode" if B <= 4 else "batched"), ("decode-exact" if B <= 4 else "decode-bf16")
+    return pm, ("decode" if gemv else "batched"), ("decode-exact" if gemv else "decode-bf16")
 
 
 def _oracle(cfg, w, prompt, forced, pm, dm):
@@ -104,10 +105,7 @@ def test_loaded_checkpoint_vs_oracle_and_transformers(cuda, checkpoints, name, p
     pid, B, impl = path
     root, model, cfg, w = checkpoints(name)
     V = cfg.vocab_size
-    if impl:
-        monkeypatch.setenv("NT_DECODE_IMPL", impl)
-    else:
-        monkeypatch.delenv("NT_DECODE_IMPL", raising=False)
+    set_decode_impl(monkeypatch, impl)
     lm = loader.load_speech_lm(str(root), device="cuda:0", max_batch=B, max_ctx=MAX_CTX, page_shuffle_seed=B)
     assert lm.shape.tie_embeddings == (CHECKPOINTS[name].tied and not CHECKPOINTS[name].distinct_head)
     g = torch.Generator().manual_seed(100 + B)
@@ -121,7 +119,7 @@ def test_loaded_checkpoint_vs_oracle_and_transformers(cuda, checkpoints, name, p
     torch.cuda.synchronize()
     launches = lm.L.nt_launch_count() - n0
     got = torch.cat((l0[None], ls), 0).permute(1, 0, 2).double().cpu()          # [B, N_NEW, V]
-    if impl is None:
+    if runs_persistent(impl, B):
         assert launches == 1, launches                   # one launch: the persistent kernel
     else:
         assert launches > N_NEW - 1, launches            # the per-op chain: several kernels per step
@@ -158,10 +156,7 @@ def test_loaded_checkpoint_decode_only(cuda, checkpoints, name, path, monkeypatc
     pid, impl = path
     root, model, cfg, w = checkpoints(name)
     V, n_new = cfg.vocab_size, 71
-    if impl:
-        monkeypatch.setenv("NT_DECODE_IMPL", impl)
-    else:
-        monkeypatch.delenv("NT_DECODE_IMPL", raising=False)
+    set_decode_impl(monkeypatch, impl)
     lm = loader.load_speech_lm(str(root), device="cuda:0", max_batch=1, max_ctx=256, page_shuffle_seed=5)
     g = torch.Generator().manual_seed(6)
     prompt = torch.randint(0, V - 1, (1,), generator=g)

@@ -1,6 +1,6 @@
 """GPU: per-token log-probabilities (``SpeechLM.set_logprobs``) on every sampler path, against float64.
 
-Runs on the logit-programmable one-layer model of test_gpu_sampler.py (the lm_head writes chosen logits for every input
+Runs on the logit-programmable one-layer model of sampler_ref.py (the lm_head writes chosen logits for every input
 token), so each case reaches the sampler path it names.  Every case runs twice on one engine, with the feature off and
 on, from the same prefill and seed:
   1. tokens, returned logits, captured windows, tile maxima, state and ``nt_launch_count`` deltas are bit-identical;
@@ -21,8 +21,8 @@ import torch
 
 from neutts_air_b200 import synthetic
 from neutts_air_b200.lm import LMShape, SpeechLM
-from tests.helpers import make_lm
-from tests.test_gpu_sampler import PATTERNS, PATTERNS_ALL, SEED, _prompts, _set_impl, programmable
+from tests.helpers import _tts, make_lm, set_decode_impl
+from tests.sampler_ref import PATTERNS, PATTERNS_ALL, SEED, _prompts, programmable
 
 pytestmark = pytest.mark.gpu
 
@@ -167,7 +167,7 @@ def test_logprobs_every_path(cuda, case, monkeypatch):
     m = programmable(V)
     cfg, w = m.oracle()
     lm = make_lm(cfg, w, max_batch=B, max_ctx=256, max_new=64)
-    _set_impl(monkeypatch, impl)
+    set_decode_impl(monkeypatch, impl)
     if ctl is not None:
         lm.set_slot_sampling(ctl[:B])
     if rng is not None:
@@ -213,7 +213,7 @@ def test_prefill_slots_entries(cuda, slots, monkeypatch):
     m = programmable(V)
     cfg, w = m.oracle()
     lm = make_lm(cfg, w, max_batch=MB, max_ctx=256, max_new=64)
-    _set_impl(monkeypatch, None)
+    set_decode_impl(monkeypatch, None)
     sp = lm.sampling(m.eos, min_new_tokens=MIN_NEW, max_new_tokens=64, top_k=50, temperature=1.0, seed=SEED)
     buf = lm.set_logprobs(True)
     lm.prefill(_prompts(m, PATTERNS[:MB]), sp)
@@ -242,7 +242,7 @@ def test_decode_graph_recaptured_on_toggle(cuda, monkeypatch):
     m = programmable(V)
     cfg, w = m.oracle()
     lm = make_lm(cfg, w, max_batch=B, max_ctx=256, max_new=64)
-    _set_impl(monkeypatch, "perop")
+    set_decode_impl(monkeypatch, "perop")
     sp = lm.sampling(m.eos, min_new_tokens=64, max_new_tokens=64, top_k=50, temperature=1.0, seed=SEED)
     lm.prefill(_prompts(m, ["gauss", "ties", "flat"]), sp)
     lm.decode(3, sp)                                  # graph captured with the feature off
@@ -266,7 +266,7 @@ def test_queue_rows(cuda, monkeypatch):
     m = programmable(V)
     cfg, w = m.oracle()
     lm = make_lm(cfg, w, max_batch=3, max_ctx=256, max_new=64)
-    _set_impl(monkeypatch, None)
+    set_decode_impl(monkeypatch, None)
     pats = ["eos", "gauss", "ties", "eos", "flat", "partial", "eos"]
     prompts = _prompts(m, pats)
     lm.set_logprobs(True).fill_(float("nan"))
@@ -286,7 +286,7 @@ def test_queue_rows(cuda, monkeypatch):
 def test_full_size_model_logprobs(cuda, B, monkeypatch):
     """Air shape, synthetic weights: 500-token prompts and 249 decode steps with EOS masked, at batch 1 (persistent
     kernel) and 64 (chain); ``model`` against float64 log_softmax of the returned logits at several steps."""
-    _set_impl(monkeypatch, None)
+    set_decode_impl(monkeypatch, None)
     shape = LMShape()
     V, eos, steps = shape.vocab_size, 151670, 250
     lm = SpeechLM(shape, synthetic.lm_state_dict(shape, 0), device="cuda:0", max_batch=B, max_ctx=1024, max_new=256,
@@ -320,9 +320,7 @@ def test_full_size_model_logprobs(cuda, B, monkeypatch):
 def test_facade_returns_arrays(cuda, monkeypatch):
     """infer_batch(return_logprobs=True): one float32 [n_generated, 2] array per utterance, equal to the engine's rows
     for the same (seeded) generation."""
-    from tests.test_gpu_facade import _tts
-
-    _set_impl(monkeypatch, None)
+    set_decode_impl(monkeypatch, None)
     tts, _ = _tts(max_batch=3)
     texts, refs, rts = ["alpha", "beta gamma", "delta"], [torch.arange(10 + 5 * i) for i in range(3)], ["a", "b c", "d"]
     wavs, lps = tts.infer_batch(texts, refs, rts, return_logprobs=True)

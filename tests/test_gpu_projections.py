@@ -43,7 +43,7 @@ import pytest
 import torch
 
 from oracle import lm_oracle as O
-from tests.helpers import gather_kv, make_lm, rel_rms
+from tests.helpers import GEMV_MAX_BATCH, gather_kv, make_lm, rel_rms, runs_persistent, set_decode_impl
 
 # Worst errors measured on one H100 80GB HBM3 (132 SMs, 400 W power limit) over the whole case matrix, and the bars,
 # ~4x above.  Relative RMS of logits[:H] per (row, 128-element tile), of logits[H:] per row and of the prefill residual
@@ -280,13 +280,6 @@ def _card() -> str:
     return f"{name}, {_sms()} SMs, {pl}"
 
 
-def _set_impl(monkeypatch, impl):
-    if impl:
-        monkeypatch.setenv("NT_DECODE_IMPL", impl)
-    else:
-        monkeypatch.delenv("NT_DECODE_IMPL", raising=False)
-
-
 def _decode(lm, B: int, steps: int, sp):
     """One nt_lm_decode call over slots 0..B-1 (B may be below the batch the engine was prefilled with)."""
     from neutts_air_b200 import _lib
@@ -366,7 +359,7 @@ def _mean_v_from_cache(lm, shape, rows):
 def _path_key(kind: str, B: int) -> str:
     if kind == "tc":
         return "hilo" if B <= 8 else "bf16"
-    return "fp32" if B <= 4 else "bf16"
+    return "fp32" if B <= GEMV_MAX_BATCH else "bf16"
 
 
 @pytest.mark.gpu
@@ -389,10 +382,10 @@ def test_decode_projections_vs_float64(cuda, case, monkeypatch):
     sp = lm.sampling(EOS, min_new_tokens=0, max_new_tokens=STEPS + 4, forced=forced)
     lm.prefill(prompts, sp)
     torch.cuda.synchronize()
-    persistent = impl == "tc" or (impl is None and B <= 16)
-    _set_impl(monkeypatch, "tc" if persistent else "perop")
+    persistent = runs_persistent(impl, B)
+    set_decode_impl(monkeypatch, "tc" if persistent else "perop")
     _decode(lm, MB, 1, sp)                    # the earlier call: every slot, the loud ones included
-    _set_impl(monkeypatch, impl)
+    set_decode_impl(monkeypatch, impl)
     logits, launches = _decode(lm, B, STEPS, sp)
 
     # the branch
@@ -401,7 +394,7 @@ def test_decode_projections_vs_float64(cuda, case, monkeypatch):
         assert _tc_branch(shape, B) == branch
     else:
         assert launches > STEPS, launches
-        assert ("gemv" if B <= 4 else "gemm") == branch
+        assert ("gemv" if B <= GEMV_MAX_BATCH else "gemm") == branch
     kind = "tc" if persistent else "chain"
     key = _path_key(kind, B)
     rb = NONE if key in ("hilo", "fp32") else BF16
@@ -470,13 +463,14 @@ def test_prefill_projections_vs_float64(cuda, case):
     assert not lm.kv[:, 0].any(), "a K row is not 0"
     rows = [(b, p) for b, n in enumerate(lens) for p in range(n)]
     toks = [t for p in prompts for t in p]
-    rb = PREFILL_GEMV if B <= 4 else BF16
+    gemv = B <= GEMV_MAX_BATCH            # the prefill's lm_head runs as a GEMV
+    rb = PREFILL_GEMV if gemv else BF16
     ref = forward64(shape, toks, _mean_v_from_cache(lm, shape, rows), rb=rb)
     last = torch.tensor(lens).cumsum(0) - 1
     head, tail = logit_errors(logits.cpu(), ref["logits"][last], H)
     hres = row_errors(h_run[MB:], ref["h"][MB:])
     vrow = _check_rows(lm, rows, ref)
-    print(f"PROJ {name} [split-K {splits}, lm_head {'GEMV' if B <= 4 else 'wgmma'}, {_card()}]: logits[:H] tile "
+    print(f"PROJ {name} [split-K {splits}, lm_head {'GEMV' if gemv else 'wgmma'}, {_card()}]: logits[:H] tile "
           f"{head:.2e} logits[H:] {tail:.2e} residual rows >= {MB} {hres:.2e} V row {vrow:.2e}")
     assert max(head, tail, hres) < BARS["prefill"], (head, tail, hres)
     assert vrow < BARS["v-bf16"], vrow

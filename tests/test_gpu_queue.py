@@ -13,19 +13,12 @@ import torch
 
 from oracle import codec_oracle as CO
 from oracle import lm_oracle as O
-from tests.helpers import make_codec, make_lm, max_err, rel_err
-from tests.test_host_logic import FakePhonemizer, FakeTokenizer
+from tests.fakes import FakePhonemizer, SmallTok
+from tests.helpers import SMALL, _bar, _setup, make_codec, make_lm, max_err, rel_err, set_decode_impl
 
 pytestmark = pytest.mark.gpu
 
-SMALL = dict(vocab_size=4096, hidden_size=256, intermediate_size=640, num_layers=3, num_heads=4, num_kv_heads=2)
 N1, N2 = 6, 8   # decode steps before / after the refill
-
-
-def _setup(max_batch, max_ctx=256, **kw):
-    cfg = O.LMConfig.tiny(**SMALL)
-    w = O.random_weights(cfg, 21, std=0.05, bf16_round=True)
-    return cfg, w, make_lm(cfg, w, max_batch=max_batch, max_ctx=max_ctx, **kw)
 
 
 def _refill_run(cfg, lm, prompts, forced, slots, new_prompts, new_forced):
@@ -64,19 +57,13 @@ def _newcomers(new_lens, seed):
     return p, f
 
 
-def _bar(got, mir, tag):
-    r = rel_err(got, mir)
-    print(f"REFILL-PARITY {tag}: relRMS {r:.2e} max/std {max_err(got, mir) / float(mir.std()):.2e}")
-    assert r < 6e-3 and max_err(got, mir) < 5e-2 * float(mir.std()), (tag, r, max_err(got, mir))
-
-
 @pytest.mark.parametrize("impl", ["tc", "perop"], ids=["persistent-kernel", "per-op-chain"])
 @pytest.mark.parametrize("max_batch", [4, 10, 18])
 def test_refill_parity(cuda, max_batch, impl, monkeypatch):
     """Survivors decode across a refill of two other slots; newcomers (one longer than a 64-token page) start from
     their own prompts on a shuffled page pool.  Every sequence meets the oracle bar of its batch; the slot state
     (recorded tokens, counters, lengths) is each slot's own."""
-    monkeypatch.setenv("NT_DECODE_IMPL", impl)
+    set_decode_impl(monkeypatch, impl)
     cfg, w, lm = _setup(max_batch, page_shuffle_seed=7)
     prompts, forced, slots, new_lens = _case(max_batch, 3)
     new_prompts, new_forced = _newcomers(new_lens, 4)
@@ -112,7 +99,7 @@ def test_refill_parity(cuda, max_batch, impl, monkeypatch):
 def test_refill_leaves_survivors_bit_identical(cuda, max_batch, impl, monkeypatch):
     """Different newcomers (same lengths) in the refilled slots change nothing in any other slot, bit for bit; nor does
     the refill itself: the survivors' logits equal those of a run in which no slot was refilled."""
-    monkeypatch.setenv("NT_DECODE_IMPL", impl)
+    set_decode_impl(monkeypatch, impl)
     cfg, w, lm = _setup(max_batch, page_shuffle_seed=7)
     prompts, forced, slots, new_lens = _case(max_batch, 3)
     sp = lm.sampling(cfg.vocab_size - 1, min_new_tokens=0, max_new_tokens=1 + N1 + N2, forced=forced)
@@ -174,11 +161,6 @@ def test_queue_end_to_end(cuda):
         row = logits[-1]
         assert float(row.max() - row[t]) < 5e-2 * float(row.std()), (t, int(row.argmax()))
         logits, _ = O.forward(cfg, w, torch.tensor([t]), cache, mirror="decode")
-
-
-class SmallTok(FakeTokenizer):
-    def __init__(self):
-        super().__init__(n_speech=1024)
 
 
 def test_facade_infer_batch_queues_long_lists(cuda):

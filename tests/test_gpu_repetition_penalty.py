@@ -1,6 +1,6 @@
 """GPU: the repetition penalty on every lm_head and sampler path, against transformers' RepetitionPenaltyLogitsProcessor.
 
-The model is the logit-programmable one-layer model of ``test_gpu_sampler.py``: a token's logits are the pattern that
+The model is the logit-programmable one-layer model of ``sampler_ref.py``: a token's logits are the pattern that
 owns it, so teacher-forced runs with the table off give the exact fp32 logits every launch of a run with the table on
 starts from.  Each check applies transformers' processor (fp32 torch, CPU) to those logits with the history taken
 from the forced ids, and compares bit for bit:
@@ -14,7 +14,7 @@ from the forced ids, and compares bit for bit:
     token of step t in the bitmap that every CTA reads at step t + 1.
 
 The one bar that is not bit-exact, kept probabilities within 4e-7 of the float64 chain (BARS["prob"] of
-test_gpu_sampler.py), measured at most 1.8e-7 in the teacher-forced windows and 1.2e-7 in the sampled runs on one
+sampler_ref.py), measured at most 1.8e-7 in the teacher-forced windows and 1.2e-7 in the sampled runs on one
 H100 80GB HBM3 (400 W power limit), with no ambiguous draw.
 """
 from __future__ import annotations
@@ -25,12 +25,10 @@ import torch
 
 from neutts_air_b200 import synthetic
 from neutts_air_b200.lm import LMShape, SpeechLM
-from tests.helpers import make_lm
-from tests.test_gpu_sampler import (BARS, MIN_NEW, PATTERNS, SEED, Checker, _set_impl, fp32_logits, prob_err,
-                                    processed_scores, programmable, ref_window, tile_maxima)
-from tests.test_gpu_sampling_controls import MARGIN
-from tests.test_gpu_vocab_range import AlignedTok, _range
-from tests.test_sampling_controls import ref_window_cut
+from tests.fakes import AlignedTok
+from tests.helpers import make_lm, runs_persistent, set_decode_impl
+from tests.sampler_ref import (BARS, MARGIN, MIN_NEW, PATTERNS, SEED, Checker, _range, fp32_logits, prob_err,
+                               processed_scores, programmable, ref_window, ref_window_cut, tile_maxima)
 
 pytestmark = pytest.mark.gpu
 
@@ -112,8 +110,8 @@ def test_penalty_every_path(cuda, case, monkeypatch):
     m = programmable(V)
     cfg, w = m.oracle()
     lm = make_lm(cfg, w, max_batch=B, max_ctx=256, max_new=64)
-    _set_impl(monkeypatch, impl)
-    persistent = impl is None and B <= 16
+    set_decode_impl(monkeypatch, impl)
+    persistent = runs_persistent(impl, B)
     pats = (PATTERNS * 3)[:B]
     prompts, forced = _setup(m, B, pats, STEPS)
     rng = _range(m, rkind) if rkind else None
@@ -191,7 +189,7 @@ def test_penalty_sampled_vs_float64(cuda, impl, B, monkeypatch):
     m = programmable(V)
     cfg, w = m.oracle()
     lm = make_lm(cfg, w, max_batch=B, max_ctx=256, max_new=64)
-    _set_impl(monkeypatch, impl)
+    set_decode_impl(monkeypatch, impl)
     sp = lm.sampling(m.eos, min_new_tokens=MIN_NEW, max_new_tokens=64, top_k=50, temperature=1.0, seed=SEED)
     lm.set_repetition_penalty([(PENS[b], b % 2 == 1) for b in range(B)])
     ck = Checker(m, lm, sp, False)
@@ -223,7 +221,7 @@ def test_multistep_launch_breaks_a_greedy_loop(cuda, impl, B, monkeypatch):
     m = programmable(V)
     cfg, w = m.oracle()
     lm = make_lm(cfg, w, max_batch=B, max_ctx=256, max_new=64)
-    _set_impl(monkeypatch, impl)
+    set_decode_impl(monkeypatch, impl)
     # patterns with many strong ids: a set-based penalty walks through them (one dominant id and a cliff would not)
     pats = ["gauss", "ties", "stairs", "gauss", "ties", "stairs", "gauss", "ties"][:B]
     prompts, _ = _setup(m, B, pats, 0)
@@ -273,7 +271,7 @@ def test_prefill_slots_history_and_survivors(cuda, monkeypatch):
     newp = [int(ranked(m, "gauss")[3]), int(ranked(m, "gauss")[0]), m.token_for("gauss", 9)]
     rows = [(1.3, True), (0.8, True), (2.0, False), (1.2, True), (1.0, True), (1.5, True)]
     for impl in ("perop", None):
-        _set_impl(monkeypatch, impl)
+        set_decode_impl(monkeypatch, impl)
         res = {}
         for tag in ("refill", "plain", "off"):
             lm = make_lm(cfg, w, max_batch=MB, max_ctx=256, max_new=64)
@@ -310,7 +308,7 @@ def test_lifecycle(cuda, monkeypatch):
     prompts, forced = _setup(m, B, pats, 6)
     rows = [(1.3, True), (0.7, True), (2.0, True)]
     for impl in (None, "perop"):
-        _set_impl(monkeypatch, impl)
+        set_decode_impl(monkeypatch, impl)
         sp = lm.sampling(m.eos, min_new_tokens=0, max_new_tokens=64, forced=forced)
         lm.set_repetition_penalty(None)
         p_off = lm.prefill(prompts, sp, return_logits=True).cpu().numpy()
@@ -350,7 +348,7 @@ def test_full_size_teacher_forced(cuda, B, monkeypatch):
     """Air shape, synthetic weights: a 500-token prompt and 250 teacher-forced steps with penalty 1.3 (prompt included),
     at batch 1 (persistent kernel) and batch 64 (chain).  Every launch's logits are transformers' processor applied to
     the table-off logits of an identical engine run in lock-step, bit for bit."""
-    _set_impl(monkeypatch, None)
+    set_decode_impl(monkeypatch, None)
     shape = LMShape()
     V, eos, steps = shape.vocab_size, 151670, 250
     sd = synthetic.lm_state_dict(shape, 0)
@@ -397,10 +395,10 @@ def test_facade_per_utterance_penalty(cuda, mode, monkeypatch):
     from neutts import NeuTTS
     from oracle import codec_oracle as CO
     from oracle import lm_oracle as LO
+    from tests.fakes import FakePhonemizer
     from tests.helpers import make_codec
-    from tests.test_host_logic import FakePhonemizer
 
-    _set_impl(monkeypatch, None)
+    set_decode_impl(monkeypatch, None)
     tok = AlignedTok()
     V = tok.speech_base + 65536
     eos = tok.convert_tokens_to_ids("<|SPEECH_GENERATION_END|>")
@@ -447,7 +445,7 @@ def test_facade_per_utterance_penalty(cuda, mode, monkeypatch):
         assert [k["penalize_prompt"] for k, _ in seen] == ([incl] if mode == "queue" else [incl[0:2], incl[2:4]])
         got = [t for _, out in seen for t in out]
         monkeypatch.undo()
-        _set_impl(monkeypatch, None)
+        set_decode_impl(monkeypatch, None)
         gkw = dict(min_new_tokens=cap, max_new_tokens=cap) if mode == "queue" else dict(min_new_tokens=50)
         want = []
         for j in range(0, n, 2):

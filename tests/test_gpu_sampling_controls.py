@@ -1,7 +1,7 @@
-"""Per-slot sampling controls on every speech-LM sampler path, against the float64 chain of test_sampling_controls.
+"""Per-slot sampling controls on every speech-LM sampler path, against the float64 chain ``ref_window_cut``.
 
-The programmable one-layer model, the Philox restatement and the float64 top-k helpers come from test_gpu_sampler.py;
-every path that file covers is run here with the per-slot table on:
+The programmable one-layer model, the Philox restatement and the float64 top-k helpers come from sampler_ref.py; every
+path test_gpu_sampler.py covers is run here with the per-slot table on:
   * identity: a table whose entries equal the launch scalars (top_p = 1, min_p = 0) gives bit-identical tokens,
     captured windows and tile maxima to the table off;
   * mixed controls in one batch: every slot its own (temperature, top_k, top_p, min_p); kept ids exact, kept
@@ -20,30 +20,12 @@ import numpy as np
 import pytest
 import torch
 
-from tests.helpers import make_lm
-from tests.test_gpu_sampler import (BARS, MIN_NEW, PATTERNS, PATTERNS_ALL, SEED, _prompts, _set_impl, draw_u,
-                                    fp32_logits, prob_err, processed_scores, programmable, ref_token, tile_maxima, tile_path)
-from tests.test_sampling_controls import chain64, ref_window_cut
+from tests.helpers import make_lm, runs_persistent, set_decode_impl
+from tests.sampler_ref import (BARS, MARGIN, MIN_NEW, PATTERNS, PATTERNS_ALL, SEED, _prompts, _record, _snap, chain64,
+                               check_launch, controls_for, draw_u, drive, fp32_logits, processed_scores, programmable,
+                               ref_token, ref_window_cut, tile_path)
 
-MARGIN = 1e-4
 STEPS = 3
-
-# (temperature, top_k, top_p, min_p): k = 1 and 64, T < 1 and > 1, top-p cutting inside the window, min-p cutting
-# before top-p does, and a plain entry
-PALETTE = [
-    (0.7, 64, 0.5, 0.0),
-    (1.5, 1, 1.0, 0.0),
-    (1.0, 64, 1.0, 0.2),
-    (1.3, 50, 0.9, 0.3),
-    (0.5, 20, 0.3, 0.0),
-    (2.0, 64, 0.95, 0.01),
-    (1.0, 8, 0.6, 0.05),
-    (0.8, 33, 1.0, 0.0),
-]
-
-
-def controls_for(B: int, shift: int = 0):
-    return [PALETTE[(b + shift) % len(PALETTE)] for b in range(B)]
 
 
 # (id, vocabulary, batch, NT_DECODE_IMPL, patterns, palette shift, expected paths of sample_tiles_seq)
@@ -110,69 +92,6 @@ def test_cases_keep_clear_of_cut_thresholds():
 
 
 # ====================================================================================== GPU driver
-def _snap(lm):
-    return dict(ngen=lm.n_generated.cpu().numpy().copy(), done=lm.done.cpu().numpy().copy(),
-                seq=lm.seq_lens.cpu().numpy().copy(), out=lm.out_tokens.cpu().numpy().copy())
-
-
-def _record(lm, cap, logits, before, rows, keys, nt, tag):
-    torch.cuda.synchronize()
-    R = len(rows)
-    return dict(tag=tag, logits=logits.cpu().numpy(), before=before, after=_snap(lm), rows=list(rows), keys=list(keys),
-                tv=cap[0][:R].cpu().numpy().copy(), ti=cap[1][:R].cpu().numpy().copy(), tt=cap[2][:R].cpu().numpy().copy(),
-                tmax=lm.debug_buffer("tmax", (R, nt)).cpu().numpy().copy())
-
-
-def drive(lm, sp, prompts, steps, monkeypatch, impl, nt, table=None):
-    """prefill + `steps` single decode steps; per launch: logits, captured window, tile maxima, state before / after."""
-    cap = lm.debug_capture_sampler()
-    _set_impl(monkeypatch, None)
-    lm.set_slot_sampling(table)
-    B = len(prompts)
-    lm.out_tokens.zero_()                           # every run starts from the same buffers: a launch that does not
-    lm.debug_buffer("tmax", (B, nt)).zero_()        # write them leaves equal contents in both runs of a comparison
-    before = _snap(lm)
-    before["ngen"][:], before["done"][:] = 0, 0
-    recs = [_record(lm, cap, lm.prefill(prompts, sp, return_logits=True), before, range(B), range(B), nt, "prefill")]
-    _set_impl(monkeypatch, impl)
-    for step in range(steps):
-        before = _snap(lm)
-        if before["done"][:B].all():
-            break
-        lg = lm.decode(1, sp, return_logits=True)[0]
-        recs.append(_record(lm, cap, lg, before, range(B), range(B), nt, f"step {step}"))
-    return recs
-
-
-def check_launch(m, rec, ctl, stats, tmax_processed=None):
-    """One launch against the float64 chain with the per-slot controls ctl[slot]."""
-    tag = rec["tag"]
-    for i, (s, key) in enumerate(zip(rec["rows"], rec["keys"])):
-        T, k, p, mp = ctl[s]
-        lg = rec["logits"][i]
-        ngen = int(rec["before"]["ngen"][s])
-        ids, q, margin = ref_window_cut(lg, ngen, m.eos, MIN_NEW, T, k, p, mp)
-        assert margin >= MARGIN, (tag, i, ctl[s], margin)
-        n = len(ids)
-        assert rec["ti"][i, :n].tolist() == ids.tolist(), (tag, i, ctl[s], rec["ti"][i, :n].tolist(), ids.tolist())
-        assert (rec["ti"][i, n:] == -1).all() and (rec["tv"][i, n:] == 0).all(), (tag, i)
-        err = prob_err(rec["tv"][i, :n], q)
-        stats["prob"] = max(stats["prob"], err)
-        assert err < BARS["prob"], (tag, i, err)
-        tok, ok = ref_token((ids, q), draw_u(SEED, ngen, key))
-        stats["draws"] += 1
-        stats["ambiguous"] += len(ok) > 1
-        assert int(rec["tt"][i]) in ok, (tag, i, int(rec["tt"][i]), tok, ok)
-        if not rec["before"]["done"][s]:
-            assert int(rec["after"]["out"][s, ngen]) == int(rec["tt"][i]), (tag, s)
-        stats["cut"] += n < min(k, 64)
-        proc = processed_scores(lg, ngen, m.eos, MIN_NEW, T)
-        stats["paths"].add(tile_path(proc, k))
-        if tmax_processed is not None:
-            want = tile_maxima(proc) if tmax_processed else tile_maxima(lg)
-            assert np.array_equal(rec["tmax"][i], want), (tag, i, np.nonzero(rec["tmax"][i] != want)[0][:5])
-
-
 def _engine(V, B, max_batch=None):
     m = programmable(V)
     cfg, w = m.oracle()
@@ -200,7 +119,7 @@ def test_identity_and_mixed_controls(cuda, case, monkeypatch):
     # 2. mixed controls, one entry per slot
     ctl = controls_for(B, shift)
     recs = drive(lm, sp, prompts, STEPS, monkeypatch, impl, nt, table=ctl)
-    persistent = impl is None and B <= 16
+    persistent = runs_persistent(impl, B)
     stats = dict(prob=0.0, draws=0, ambiguous=0, cut=0, paths=set())
     for r in recs:
         # 3. processed maxima of the persistent epilogue (per-row T), else the raw maxima behind the lm_head
@@ -223,7 +142,7 @@ def test_refilled_slots_sample_with_their_own_controls(cuda, case, monkeypatch):
     m, lm = _engine(V, MB)
     sp = lm.sampling(m.eos, min_new_tokens=MIN_NEW, max_new_tokens=64, top_k=50, temperature=1.0, seed=SEED)
     cap = lm.debug_capture_sampler()
-    _set_impl(monkeypatch, None)
+    set_decode_impl(monkeypatch, None)
     ctl = controls_for(MB)
     lm.set_slot_sampling(ctl)
     lm.prefill(_prompts(m, (PATTERNS * 2)[:MB]), sp)
@@ -260,7 +179,7 @@ def test_multistep_launch_with_controls(cuda, impl, B, monkeypatch):
     m, lm = _engine(V, B)
     ctl = controls_for(B, shift=2)
     sp = lm.sampling(m.eos, min_new_tokens=MIN_NEW, max_new_tokens=64, top_k=50, temperature=1.0, seed=SEED)
-    _set_impl(monkeypatch, impl)
+    set_decode_impl(monkeypatch, impl)
     lm.set_slot_sampling(ctl)
     prompts = _prompts(m, PATTERNS[:B])
     lm.prefill(prompts, sp)
@@ -302,7 +221,7 @@ def test_validation_and_decode_graph(cuda, monkeypatch):
     V, B = 16462, 7
     m, lm = _engine(V, B)
     sp = lm.sampling(m.eos, min_new_tokens=MIN_NEW, max_new_tokens=64, top_k=50, temperature=1.0, seed=SEED)
-    _set_impl(monkeypatch, "perop")
+    set_decode_impl(monkeypatch, "perop")
     tv, ti, tt = lm.debug_capture_sampler()
     prompts = _prompts(m, PATTERNS)
     lm.prefill(prompts, sp)
@@ -347,9 +266,8 @@ def test_facade_lists_match_per_utterance_runs(cuda, monkeypatch):
     with every slot set to utterance i's controls (same seed, same stream ids).  Explicit defaults change nothing."""
     from oracle import codec_oracle as CO
     from oracle import lm_oracle as LO
+    from tests.fakes import FakePhonemizer, SmallTok
     from tests.helpers import make_codec
-    from tests.test_gpu_facade import SmallTok
-    from tests.test_host_logic import FakePhonemizer
     from neutts import NeuTTS
 
     cfg = LO.LMConfig.tiny(vocab_size=4096, hidden_size=256, intermediate_size=512, num_layers=2, num_heads=4, num_kv_heads=2)

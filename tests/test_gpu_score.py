@@ -1,6 +1,6 @@
 """GPU: teacher-forced scoring (``nt_lm_score`` / ``SpeechLM.score`` / ``NeuTTS.score``).
 
-  * exact logits: on the logit-programmable model of test_gpu_sampler.py the lm_head input of every scored row is one
+  * exact logits: on the logit-programmable model of sampler_ref.py the lm_head input of every scored row is one
     bf16 value on one pattern's column, so each row's logits are known exactly and the scores are checked against a
     float64 log-softmax of them, at a vocabulary with a partial last tile and at the Air vocabulary, across the row-block
     boundary of the lm_head;
@@ -21,8 +21,7 @@ import torch
 
 from oracle import lm_oracle as O
 from tests.helpers import make_lm
-from tests.test_gpu_sampler import PATTERNS_ALL, programmable
-from tests.test_score import score64
+from tests.sampler_ref import PATTERNS_ALL, programmable, score64
 
 pytestmark = pytest.mark.gpu
 
@@ -215,7 +214,7 @@ def test_score_facade_matches_engine(small):
     import warnings
 
     from neutts import NeuTTS
-    from tests.test_host_logic import FakeCodec, FakePhonemizer, FakeTokenizer
+    from tests.fakes import FakeCodec, FakePhonemizer, FakeTokenizer
 
     cfg, w, lm = small
     tok = FakeTokenizer()

@@ -14,9 +14,8 @@ import torch
 from oracle import codec_oracle as CO
 from oracle import lm_oracle as LO
 from oracle import stream_oracle as SO
+from tests.fakes import AlignedTok, FakePhonemizer
 from tests.helpers import make_codec, make_lm
-from tests.test_host_logic import FakePhonemizer
-from tests.test_gpu_vocab_range import AlignedTok
 
 pytestmark = pytest.mark.gpu
 

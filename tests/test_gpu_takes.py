@@ -18,10 +18,8 @@ import torch
 
 from neutts_air_b200.lm import fork_slots
 from oracle import lm_oracle as O
-from tests.helpers import gather_kv
-from tests.test_gpu_queue import _bar, _setup
-from tests.test_gpu_sampler import draw_u, ref_token
-from tests.test_sampling_controls import ref_window_cut
+from tests.helpers import _bar, _setup, _tts, gather_kv, set_decode_impl
+from tests.sampler_ref import draw_u, ref_token, ref_window_cut
 
 pytestmark = pytest.mark.gpu
 
@@ -63,7 +61,7 @@ def _privatise(lm, B, n, lens):
 @pytest.mark.parametrize("impl", ["tc", "perop"], ids=["persistent-kernel", "per-op-chain"])
 @pytest.mark.parametrize("B,n", CASES, ids=[f"{b}x{n}" for b, n in CASES])
 def test_fork_prefill_kv_and_decode(cuda, B, n, impl, monkeypatch):
-    monkeypatch.setenv("NT_DECODE_IMPL", impl)
+    set_decode_impl(monkeypatch, impl)
     N = B * n
     cfg, w, lm = _setup(N, page_shuffle_seed=7)
     _, _, plain = _setup(N, page_shuffle_seed=7)
@@ -162,7 +160,7 @@ def test_first_draws(cuda, B, n):
 def test_refill_one_take(cuda, impl, monkeypatch):
     """5. prefill_slots into one take's slot returns only that take's private pages and leaves its siblings' logits
     bit-identical; after generate_batch(num_return_sequences=n) every page goes back to the pool."""
-    monkeypatch.setenv("NT_DECODE_IMPL", impl)
+    set_decode_impl(monkeypatch, impl)
     B, n = 2, 3
     N = B * n
     cfg, w, lm = _setup(N, page_shuffle_seed=7)
@@ -209,7 +207,6 @@ def test_public_outputs(cuda):
 
 def test_facade_keeps_the_most_probable_take(cuda):
     from neutts.neutts import best_takes
-    from tests.test_gpu_facade import _tts
 
     takes = 2
     tts, _ = _tts(max_batch=4)

@@ -1,6 +1,6 @@
 """GPU: the vocabulary range (``nt_lm_set_vocab_range``, speech-token-only decoding) on every sampler path.
 
-Reuses the logit-programmable one-layer model and the float64 sampler of ``test_gpu_sampler.py``.  Every case runs the
+Reuses the logit-programmable one-layer model and the float64 sampler of ``sampler_ref.py``.  Every case runs the
 same prompts twice on one path, with the range off and on.  With the range on, at every launch:
   * every suppressed logit reads -inf, and every allowed logit equals the range-off launch bit for bit (a row keeps
     its pattern, and a pattern's logits depend on nothing else);
@@ -18,8 +18,10 @@ import torch
 
 from neutts_air_b200 import synthetic
 from neutts_air_b200.lm import LMShape, SpeechLM
-from tests.helpers import make_lm
-from tests.test_gpu_sampler import MIN_NEW, PATTERNS, SEED, Checker, _prompts, _set_impl, programmable
+from tests.fakes import AlignedTok
+from tests.helpers import make_lm, runs_persistent, set_decode_impl
+from tests.sampler_ref import (MARGIN, MIN_NEW, PATTERNS, SEED, Checker, _prompts, _range, check_launch, controls_for,
+                               drive, programmable)
 
 pytestmark = pytest.mark.gpu
 
@@ -62,27 +64,6 @@ CASES = [
 STEPS = 4
 
 
-def ties_ids(m):
-    """Ids of the "ties" pattern's 84 values tied at 10."""
-    j = PATTERNS.index("ties")
-    return np.nonzero(m.target[j] == 10.0)[0]
-
-
-def _range(m, kind):
-    if kind == "speech":   # the Air layout: [1187 * 128, V), EOS below it
-        lo = 1187 * 128 if m.V == 217472 else (m.nt - 3) * 128
-        return lo, m.V
-    t = m.eos // 128
-    if kind == "below-eos":   # [0, (t - 5) * 128): EOS lies above the range
-        return 0, (t - 5) * 128
-    if kind == "ties-lo":     # lo at the tile edge nearest the median tied id
-        ids = ties_ids(m)
-        lo = int(round(float(np.median(ids)) / 128)) * 128
-        assert (ids < lo).sum() >= 10 and (ids >= lo).sum() >= 10, lo
-        return lo, m.V
-    return (t - 20) * 128, (t + 20) * 128   # 40 tiles with EOS in the middle
-
-
 def _run(m, B, impl, top_k, T, pats, rng, monkeypatch):
     """Prefill + STEPS single decode steps; returns (logits per launch, tokens, checker paths, engine)."""
     cfg, w = m.oracle()
@@ -101,8 +82,8 @@ def _run(m, B, impl, top_k, T, pats, rng, monkeypatch):
     ck.check_launch(launches[0], list(range(B)), list(range(B)), before, after, 0, tag="prefill")
     ck.check_tmax(launches[0], [0] * B, False, "prefill")
     ck.paths.clear()
-    _set_impl(monkeypatch, impl)
-    persistent = impl == "tc" or (impl is None and B <= 16)
+    set_decode_impl(monkeypatch, impl)
+    persistent = runs_persistent(impl, B)
     curs = [lm.cur_token[:B].cpu().numpy().copy()]
     for step in range(STEPS):
         before = ck.snapshot()
@@ -150,7 +131,7 @@ def test_vocab_range_multistep_and_toggle(cuda, impl, B, monkeypatch):
     cfg, w = m.oracle()
     lm = make_lm(cfg, w, max_batch=B, max_ctx=256, max_new=64)
     sp = lm.sampling(m.eos, min_new_tokens=MIN_NEW, max_new_tokens=64, top_k=50, temperature=1.0, seed=SEED)
-    _set_impl(monkeypatch, impl)
+    set_decode_impl(monkeypatch, impl)
     lo, hi = 1187 * 128, V
     allowed = allowed_mask(V, lo, hi, m.eos)
     prompts = _prompts(m, PATTERNS[:B])
@@ -197,7 +178,7 @@ def air_lm(cuda):
 def test_full_size_speech_only_generation(air_lm, B, monkeypatch):
     """250 tokens per utterance at the Air shape with the range [speech_base, V): only speech ids or EOS.  Then
     teacher-forced logits with the range on equal the range-off logits on every allowed row, bit for bit."""
-    _set_impl(monkeypatch, None)
+    set_decode_impl(monkeypatch, None)
     lm, V, eos, base = air_lm, 217472, 151670, 151936
     allowed = allowed_mask(V, base, V, eos)
     g = torch.Generator().manual_seed(B)
@@ -225,7 +206,7 @@ def test_full_size_speech_only_generation(air_lm, B, monkeypatch):
 def test_full_size_queue_matches_chunked(cuda, rng, monkeypatch):
     """Equal caps (EOS masked) make the two schedules coincide (as in test_gpu_queue): generate_queue with the range,
     two slots refilled twice, gives exactly the tokens of generate_batch per chunk with the range."""
-    _set_impl(monkeypatch, None)
+    set_decode_impl(monkeypatch, None)
     shape = LMShape()
     lm = SpeechLM(shape, synthetic.lm_state_dict(shape, 0), device="cuda:0", max_batch=2, max_ctx=256, max_new=64)
     V, eos, base, cap = 217472, 151670, 151936, 20
@@ -243,8 +224,6 @@ def test_full_size_queue_matches_chunked(cuda, rng, monkeypatch):
 
 
 # ------------------------------------------------------------------------------------ per-slot controls on top
-from tests.test_gpu_sampling_controls import MARGIN, check_launch, controls_for, drive  # noqa: E402
-
 # Inside the speech range the "plateau" pattern keeps only its clipped background, dozens of values tied at 3.0: a
 # window of equal probabilities puts top-p's cumulative mass exactly on its threshold, which no reference can decide.
 NO_PLATEAU = [p for p in PATTERNS if p != "plateau"]
@@ -280,7 +259,7 @@ def test_vocab_range_with_slot_controls(cuda, case, monkeypatch):
             assert np.array_equal(a[f], b[f]), (name, a["tag"], f)
     ctl = controls_for(B, shift)
     recs = drive(lm, sp, prompts, 3, monkeypatch, impl, nt, table=ctl)
-    persistent = impl is None and B <= 16
+    persistent = runs_persistent(impl, B)
     stats = dict(prob=0.0, draws=0, ambiguous=0, cut=0, paths=set())
     for r in recs:
         assert np.isneginf(r["logits"][:, ~allowed]).all(), (name, r["tag"])
@@ -312,7 +291,7 @@ def test_vocab_range_prefill_slots(cuda, case, monkeypatch):
     pats = ["eos", "flat", "ties", "plateau", "partial", "gauss"][: len(slots)]
     prompts = [[m.token_for(p, 5), m.token_for(p, 9)] for p in pats]
     got = {}
-    _set_impl(monkeypatch, None)
+    set_decode_impl(monkeypatch, None)
     for rng in (None, (lo, hi)):
         cfg, w = m.oracle()
         lm = make_lm(cfg, w, max_batch=MB, max_ctx=256, max_new=64)
@@ -344,17 +323,6 @@ def test_vocab_range_prefill_slots(cuda, case, monkeypatch):
 
 
 # ------------------------------------------------------------------------------------ the facade end to end
-class AlignedTok:
-    """FakeTokenizer whose 65 536 speech ids start at a 128-aligned id (3072) and end at the vocabulary's end."""
-
-    def __new__(cls):
-        from tests.test_host_logic import FakeTokenizer
-
-        tok = FakeTokenizer(n_speech=65536)
-        tok.speech_base = 3072
-        return tok
-
-
 @pytest.mark.parametrize("stream", [False, True], ids=["infer_batch", "infer_stream_batch"])
 def test_facade_speech_tokens_only_end_to_end(cuda, stream, monkeypatch):
     """NeuTTS(speech_tokens_only=True) on a random-weight engine (which otherwise emits mostly non-speech ids): every
@@ -365,10 +333,10 @@ def test_facade_speech_tokens_only_end_to_end(cuda, stream, monkeypatch):
     from neutts import NeuTTS
     from oracle import codec_oracle as CO
     from oracle import lm_oracle as LO
+    from tests.fakes import FakePhonemizer
     from tests.helpers import make_codec
-    from tests.test_host_logic import FakePhonemizer
 
-    _set_impl(monkeypatch, None)
+    set_decode_impl(monkeypatch, None)
     tok = AlignedTok()
     V = tok.speech_base + 65536
     cfg = LO.LMConfig.tiny(vocab_size=V, hidden_size=256, intermediate_size=512, num_layers=2, num_heads=4, num_kv_heads=2)

@@ -1,6 +1,6 @@
 """CPU: host-side logic above the C-ABI — prompt construction, code<->token mapping, streaming
 cross-fade, KV page pool, weight packing, checkpoint reading, sharding plan.  A fake tokenizer /
-phonemizer stands in for the HF tokenizer and espeak (neither is available offline)."""
+phonemizer (fakes.py) stands in for the HF tokenizer and espeak (neither is available offline)."""
 import json
 import os
 
@@ -9,87 +9,8 @@ import pytest
 import torch
 
 from oracle import stream_oracle as SO
-
-
-class FakeTokenizer:
-    """Character-level tokenizer with the special tokens the reference adds (TRAINING.md:33-57)."""
-    SPECIALS = ["<|TEXT_REPLACE|>", "<|TEXT_PROMPT_START|>", "<|TEXT_PROMPT_END|>", "<|SPEECH_REPLACE|>",
-                "<|SPEECH_GENERATION_START|>", "<|SPEECH_GENERATION_END|>"]
-
-    def __init__(self, n_speech=65536):
-        self.chars = {chr(c): c for c in range(32, 1024)}
-        self.chars["\n"] = 10
-        self.special_base = 2000
-        self.speech_base = 3000
-        self.n_speech = n_speech
-
-    def convert_tokens_to_ids(self, tok):
-        if tok in self.SPECIALS:
-            return self.special_base + self.SPECIALS.index(tok)
-        if tok.startswith("<|speech_"):
-            return self.speech_base + int(tok[9:-2])
-        raise KeyError(tok)
-
-    def encode(self, text, add_special_tokens=True):
-        import re
-
-        out = []
-        for part in re.split(r"(<\|[A-Za-z_0-9]+\|>)", text):
-            if not part:
-                continue
-            if part.startswith("<|") and part.endswith("|>"):
-                out.append(self.convert_tokens_to_ids(part))
-            else:
-                out += [self.chars[c] for c in part]
-        return out
-
-    def decode(self, ids, add_special_tokens=False):
-        inv = {v: k for k, v in self.chars.items()}
-        s = ""
-        for i in ids:
-            if i >= self.speech_base:
-                s += f"<|speech_{i - self.speech_base}|>"
-            elif i >= self.special_base:
-                s += self.SPECIALS[i - self.special_base]
-            else:
-                s += inv[i]
-        return s
-
-
-class FakePhonemizer:
-    def phonemize(self, texts):
-        return [t.lower().replace(",", " ,") for t in texts]
-
-
-class FakeCodec:
-    device = torch.device("cpu")
-    max_batch = 4
-
-    def decode_code(self, codes):
-        return torch.zeros(codes.shape[0], 1, 480 * codes.shape[2]) + codes[:, :, :1].float() / 65536.0
-
-
-class FakeBackbone:
-    """transformers-style .generate(): appends fixed ids (some non-speech) and EOS."""
-    device = torch.device("cpu")
-
-    def __init__(self, tail):
-        self.tail = tail
-
-    def generate(self, ids, **kw):
-        self.kw = kw
-        return torch.cat((ids, torch.tensor([self.tail])), dim=1)
-
-
-def _tts(tail=None):
-    from neutts import NeuTTS
-
-    tok = FakeTokenizer()
-    tail = tail if tail is not None else [tok.speech_base + 5, 65, tok.speech_base + 70000, tok.speech_base + 9, tok.special_base + 5]
-    import warnings
-    with warnings.catch_warnings():
-        warnings.simplefilter("ignore")
-        return NeuTTS(tokenizer=tok, phonemizer=FakePhonemizer(), backbone=FakeBackbone(tail), codec=FakeCodec()), tok
+from tests.fakes import (BatchRampCodec, FakeBackbone, FakeBatchStreamLM, FakeCodec, FakePhonemizer, FakeTokenizer,
+                         RampCodec, _tts)
 
 
 def _reference_template(tok, phon, ref_codes, ref_text, input_text):
@@ -308,19 +229,6 @@ class FakeStreamLM:
             self._emit()
 
 
-class RampCodec:
-    """Deterministic 'codec': frame i of the window becomes hop samples of code/1000 + 0.01 * position-in-window,
-    so a wrong window start, slice or cross-fade weight changes the output."""
-    device = torch.device("cpu")
-    max_batch = 1
-    hop = 8
-
-    def decode_code(self, codes):
-        c = codes[0, 0].float()
-        frames = c[:, None] / 1000.0 + 0.01 * torch.arange(len(c))[:, None] + torch.zeros(1, self.hop)
-        return frames.reshape(1, 1, -1)
-
-
 @pytest.mark.parametrize("n_gen,junk_every,limit", [(143, 0, None), (90, 7, None), (30, 0, None), (12, 3, None), (400, 5, 301)])
 def test_stream_matches_reference_window_plan(n_gen, junk_every, limit):
     """infer_stream == the reference's window bookkeeping (neutts/neutts.py:373-465) restated in
@@ -462,53 +370,6 @@ def test_generate_batch_caps_are_per_sequence():
     assert list(kw["limits"]) == [548, 1748]  # ... and every slot carries its own cap (2048 - prompt length)
     lm.generate_batch([[1] * 300, [2] * 300], eos_token_id=9, max_length=2048, check_every=4096)
     assert calls["sampling"][1]["limits"] is None and calls["sampling"][0][2] == 1748
-
-
-class FakeBatchStreamLM:
-    """Batched prefill()/decode() surface of SpeechLM: one scripted token stream per slot, lock-step decoding,
-    finished slots idle (as inside the persistent kernel)."""
-    device = torch.device("cpu")
-
-    def __init__(self, scripts, max_new=4096):
-        self.scripts, self.max_new = [list(s) for s in scripts], max_new
-        B = len(scripts)
-        self.out_tokens = torch.zeros(B, max_new, dtype=torch.int32)
-        self.n_generated = torch.zeros(B, dtype=torch.int32)
-        self.done = torch.zeros(B, dtype=torch.int32)
-        self.decode_calls = []
-
-    def sampling(self, eos, min_new, max_new, top_k, temperature, seed, limits=None):
-        self.eos = eos
-        self.limits = list(limits) if limits is not None else [max_new] * len(self.scripts)
-        return None
-
-    def _emit(self):
-        for b, script in enumerate(self.scripts):
-            n = int(self.n_generated[b])
-            if int(self.done[b]) or n >= self.limits[b]:
-                continue
-            tok = script[n] if n < len(script) else self.eos
-            self.out_tokens[b, n] = tok
-            self.n_generated[b] = n + 1
-            if tok == self.eos or n + 1 >= self.limits[b]:
-                self.done[b] = 1
-
-    def prefill(self, prompts, sp):
-        self._emit()
-
-    def decode(self, steps, sp):
-        assert steps >= 1
-        self.decode_calls.append(steps)
-        for _ in range(steps):
-            self._emit()
-
-
-class BatchRampCodec(RampCodec):
-    max_batch = 2          # smaller than the batch: same-length windows are split over several codec calls
-
-    def decode_code(self, codes):
-        assert codes.shape[0] <= self.max_batch
-        return torch.cat([RampCodec.decode_code(self, codes[r: r + 1]) for r in range(codes.shape[0])])
 
 
 @pytest.mark.parametrize("frames_per_chunk", [25, 50])

@@ -11,8 +11,7 @@ from transformers import (LogitsProcessorList, MinNewTokensLengthLogitsProcessor
                           TopKLogitsWarper, TopPLogitsWarper)
 from transformers.generation.utils import GenerationMixin
 
-from tests.test_host_logic import FakeCodec, FakePhonemizer, FakeTokenizer
-from tests.test_queue_host import EOS, QueueStub, _prompts
+from tests.fakes import EOS, FakeCodec, FakePhonemizer, FakeTokenizer, QueueStub, _prompts
 
 
 # ----------------------------------------------------------------------------------------- float64 reference
@@ -229,7 +228,7 @@ def test_facade_returns_rows_aligned_with_ids():
 
 
 def test_facade_rejects_unsupported_logprobs():
-    from tests.test_host_logic import FakeBackbone
+    from tests.fakes import FakeBackbone
 
     tts = _facade(lambda tok: FakeBackbone([3005, 2005]))
     with pytest.raises(ValueError, match="set_logprobs"):

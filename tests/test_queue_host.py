@@ -1,84 +1,15 @@
 """Host logic of continuous batching (SpeechLM.generate_queue) and the facade's use of it, on a CPU stub engine.
 
-The stub keeps SpeechLM's host side (page pool, per-slot page lists, generate_queue, release_pages) and replaces the
-device calls: prompt i (every id of it is i + 1) emits the tokens 1000 * (i + 1) + step, or EOS at a chosen step.
+The stub (fakes.QueueStub) keeps SpeechLM's host side (page pool, per-slot page lists, generate_queue, release_pages)
+and replaces the device calls: prompt i (every id of it is i + 1) emits the tokens 1000 * (i + 1) + step, or EOS at a
+chosen step.
 """
-import types
 import warnings
 
 import numpy as np
 import torch
 
-from neutts_air_b200.lm import PagePool, SpeechLM
-from tests.test_host_logic import FakeCodec, FakePhonemizer, FakeTokenizer
-
-EOS = 9
-
-
-class QueueStub(SpeechLM):
-    def __init__(self, max_batch, eos_at=None):
-        self.max_ctx, self.max_new, self.max_batch, self.device = 2048, 2048, max_batch, torch.device("cpu")
-        self.max_pages = self.max_ctx // self.PAGE
-        self.num_pages = max_batch * self.max_pages
-        self.pool = PagePool(self.num_pages, shuffle_seed=1)
-        self._slot_pages = [[] for _ in range(max_batch)]
-        self.out_tokens = torch.zeros(max_batch, self.max_new, dtype=torch.int32)
-        self.n_generated = torch.zeros(max_batch, dtype=torch.int32)
-        self.done = torch.zeros(max_batch, dtype=torch.int32)
-        self.eos_at = eos_at or {}
-        self.who, self.cap = [None] * max_batch, [0] * max_batch
-        self.log, self.admitted = [], 0
-
-    def sampling(self, eos, min_new, max_new, top_k, temperature, seed, greedy, limits=None, slot_base=0):
-        self.limit_table = list(limits) + [max_new] * (self.max_batch - len(limits))
-        self.log.append(("sampling", list(limits), slot_base))
-        return types.SimpleNamespace(max_new_tokens=max_new, slot_base=slot_base)
-
-    def _start(self, s, prompt, key):
-        tag = prompt[0]
-        assert all(t == tag for t in prompt)
-        assert key == self.slot_base + tag - 1, (key, tag)   # Philox stream = slot_base + input index
-        self._slot_pages[s] = self.pool.alloc((len(prompt) + self.limit_table[s] + self.PAGE - 1) // self.PAGE)
-        self.who[s], self.cap[s] = tag, self.limit_table[s]
-        self.n_generated[s], self.done[s] = 0, 0
-        self.admitted += 1
-        self._emit(s)
-
-    def _emit(self, s):
-        g = int(self.n_generated[s])
-        tok = EOS if self.eos_at.get(self.who[s]) == g else 1000 * self.who[s] + g
-        self.out_tokens[s, g], self.n_generated[s] = tok, g + 1
-        if tok == EOS or g + 1 >= self.cap[s]:
-            self.done[s] = 1
-
-    def prefill(self, prompts, sp):
-        self.release_pages()
-        self.slot_base = sp.slot_base
-        self.log.append(("prefill", [p[0] for p in prompts]))
-        for s, p in enumerate(prompts):
-            self._start(s, p, sp.slot_base + s)
-        self._B = len(prompts)
-
-    def prefill_slots(self, slots, prompts, sp, stream_ids, return_logits=False, limits=None):
-        assert all(self.done[s] for s in slots)          # only finished slots are refilled
-        self.log.append(("refill", list(slots), [p[0] for p in prompts], list(stream_ids), list(limits)))
-        self.release_pages(slots)
-        for s, p, key, lim in zip(slots, prompts, stream_ids, limits):
-            self.limit_table[s] = lim
-            self._start(s, p, key)
-
-    def decode(self, n, sp):
-        live = [s for s in range(self._B) if not self.done[s]]
-        left = [self.cap[s] - int(self.n_generated[s]) for s in live]
-        self.log.append(("decode", n, min(left), max(left), self.admitted))
-        for _ in range(n):
-            for s in live:
-                if not self.done[s]:
-                    self._emit(s)
-
-
-def _prompts(lens):
-    return [[i + 1] * m for i, m in enumerate(lens)]
+from tests.fakes import EOS, FakeCodec, FakePhonemizer, FakeTokenizer, QueueStub, _prompts
 
 
 def test_queue_fifo_order_streams_limits_and_pages():

@@ -16,10 +16,8 @@ import pytest
 import torch
 
 from neutts_air_b200.lm import check_penalty, per_prompt_penalty
-from tests.test_host_logic import FakeTokenizer
-from tests.test_queue_host import EOS, QueueStub, _prompts
-from tests.test_sampling_controls import GenerateBackbone, KwBackbone, _facade, chain64
-from tests.test_vocab_range import suppressed_scores
+from tests.fakes import EOS, FakeTokenizer, GenerateBackbone, KwBackbone, QueueStub, _facade, _prompts
+from tests.sampler_ref import chain64, suppressed_scores
 
 
 def history(prompt, generated, include_prompt: bool = True):

@@ -1,51 +1,18 @@
 """Per-slot sampling controls (temperature, top_k, top_p, min_p) without a GPU: the float64 reference of the whole
 processor chain, pinned to transformers' own warpers, and the host plumbing of the engine and the facade on stubs.
 
-The reference here is what tests/test_gpu_sampling_controls.py compares every sampler path with.
+The reference (``chain64``, ``ref_window_cut`` in sampler_ref.py) is what tests/test_gpu_sampling_controls.py compares
+every sampler path with.
 """
 from __future__ import annotations
-
-import warnings
 
 import numpy as np
 import pytest
 import torch
 
 from neutts_air_b200.lm import per_prompt_controls
-from tests.test_gpu_sampler import processed_scores, ref_token
-from tests.test_host_logic import FakeCodec, FakePhonemizer, FakeTokenizer
-from tests.test_queue_host import EOS, QueueStub, _prompts
-
-
-# ====================================================================================== float64 reference chain
-def chain64(scores, top_k: int, top_p: float, min_p: float):
-    """Processed scores [V] -> kept window of the kernels: (score desc, id asc), the first min(top_k, 64); its float64
-    softmax q; top-p keeps entry j iff sum_{i<j} q_i < top_p (off at 1), min-p iff q_j >= min_p * q_0 (off at 0); the
-    kept prefix renormalised.  Returns (ids int64 [k'], probabilities float64 [k'], margin): margin is the distance of
-    the cut quantities (exclusive cumulative mass, q_j / q_0) to their thresholds over the window (inf: no cut)."""
-    s = np.asarray(scores, dtype=np.float64)
-    k = min(top_k, 64, s.size)
-    order = np.lexsort((np.arange(s.size), -s))[:k]
-    p = np.exp(s[order] - s[order[0]])
-    q = p / p.sum()
-    keep = np.ones(k, dtype=bool)
-    margin = np.inf
-    if top_p < 1:
-        excl = np.concatenate(([0.0], np.cumsum(q)[:-1]))
-        keep &= excl < top_p
-        margin = min(margin, float(np.abs(excl - top_p).min()))
-    if min_p > 0:
-        ratio = q / q[0]
-        keep &= ratio >= min_p
-        margin = min(margin, float(np.abs(ratio - min_p).min()))
-    kp = int(np.argmin(keep)) if not keep.all() else k
-    kp = max(kp, 1)
-    return order[:kp].astype(np.int64), q[:kp] / q[:kp].sum(), margin
-
-
-def ref_window_cut(logits, ngen: int, eos: int, min_new: int, temperature: float, top_k: int, top_p: float, min_p: float):
-    """The kernels' chain on logits: EOS mask and fp32(logit) * fp32(1 / T) (``processed_scores``), then ``chain64``."""
-    return chain64(processed_scores(logits, ngen, eos, min_new, temperature), top_k, top_p, min_p)
+from tests.fakes import EOS, FakeTokenizer, GenerateBackbone, KwBackbone, QueueStub, _facade, _prompts
+from tests.sampler_ref import chain64, ref_token, ref_window_cut
 
 
 def test_chain_matches_transformers_warpers():
@@ -204,42 +171,6 @@ def test_queue_writes_newcomers_controls_before_their_prefill():
 
 
 # ---------------------------------------------------------------------------------------- facade
-class KwBackbone:
-    device = torch.device("cpu")
-
-    def __init__(self, tok, queue=True):
-        self.tok, self.calls = tok, []
-        if queue:
-            self.generate_queue = lambda prompts, eos, **kw: self._call("queue", prompts, kw)
-
-    def _call(self, what, prompts, kw):
-        self.calls.append((what, len(prompts), kw))
-        return [torch.tensor([self.tok.speech_base + 1]) for _ in prompts]
-
-    def generate_batch(self, prompts, eos, **kw):
-        return self._call("batch", prompts, kw)
-
-
-class GenerateBackbone:
-    """transformers-style backbone: records the generate kwargs of every utterance."""
-    device = torch.device("cpu")
-
-    def __init__(self, tok):
-        self.tok, self.kws = tok, []
-
-    def generate(self, ids, **kw):
-        self.kws.append(kw)
-        return torch.cat((ids, torch.tensor([[self.tok.speech_base + 2]])), dim=1)
-
-
-def _facade(bb, max_batch):
-    from neutts import NeuTTS
-
-    with warnings.catch_warnings():
-        warnings.simplefilter("ignore")
-        return NeuTTS(tokenizer=bb.tok, phonemizer=FakePhonemizer(), backbone=bb, codec=FakeCodec(), max_batch=max_batch, seed=1)
-
-
 def _ctl(kw):
     return {k: kw[k] for k in ("temperature", "top_k", "top_p", "min_p") if k in kw}
 

@@ -8,46 +8,8 @@ import pytest
 import torch
 
 from oracle import lm_oracle as O
-from tests.test_host_logic import FakeCodec, FakePhonemizer, FakeTokenizer
-
-
-# ====================================================================================== float64 reference
-def forward64(cfg: O.LMConfig, w: O.LMWeights, ids) -> torch.Tensor:
-    """Qwen2 logits [T, V] in float64, causal attention; the rotary angles and the RMSNorm statistics in fp32, as
-    transformers forms them in a float64 model."""
-    d = lambda t: t.double()
-    ids = torch.as_tensor(ids, dtype=torch.long)
-    T = ids.shape[0]
-    cos, sin = O.rope_cos_sin(torch.arange(T), cfg.head_dim, cfg.rope_theta)
-    cos, sin = cos.double(), sin.double()
-
-    def norm(x, wt):
-        return O.rms_norm(x, d(wt), cfg.rms_eps)
-
-    n_rep = cfg.num_heads // cfg.num_kv_heads
-    mask = torch.triu(torch.ones(T, T, dtype=torch.bool), 1)
-    h = d(w.embed)[ids]
-    for L in w.layers:
-        x = norm(h, L["ln1"])
-        q = (x @ d(L["wq"]).T + d(L["bq"])).view(T, cfg.num_heads, cfg.head_dim)
-        k = (x @ d(L["wk"]).T + d(L["bk"])).view(T, cfg.num_kv_heads, cfg.head_dim)
-        v = (x @ d(L["wv"]).T + d(L["bv"])).view(T, cfg.num_kv_heads, cfg.head_dim)
-        q, k = O.apply_rope(q, cos, sin), O.apply_rope(k, cos, sin)
-        k, v = k.repeat_interleave(n_rep, 1), v.repeat_interleave(n_rep, 1)
-        s = torch.einsum("qhd,khd->hqk", q, k) * cfg.head_dim ** -0.5
-        p = torch.softmax(s.masked_fill(mask, float("-inf")), -1)
-        h = h + torch.einsum("hqk,khd->qhd", p, v).reshape(T, -1) @ d(L["wo"]).T
-        x = norm(h, L["ln2"])
-        h = h + (torch.nn.functional.silu(x @ d(L["wg"]).T) * (x @ d(L["wu"]).T)) @ d(L["wd"]).T
-    return norm(h, w.final_norm) @ d(w.lm_head).T
-
-
-def score64(cfg, w, ids, start: int) -> np.ndarray:
-    """score[t] = log_softmax(z_{t-1})[x_t] for start <= t < len(ids), float64."""
-    ids = torch.as_tensor(ids, dtype=torch.long)
-    lp = torch.log_softmax(forward64(cfg, w, ids), -1)
-    t = torch.arange(start, ids.shape[0])
-    return lp[t - 1, ids[t]].numpy()
+from tests.fakes import FakeCodec, FakePhonemizer, FakeTokenizer
+from tests.sampler_ref import score64
 
 
 def _tiny():
@@ -150,7 +112,7 @@ def test_facade_builds_prompt_codes_and_eos():
 
 
 def test_facade_score_errors():
-    from tests.test_host_logic import FakeBackbone
+    from tests.fakes import FakeBackbone
 
     tts = _facade()
     with pytest.raises(ValueError, match="empty"):

@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from oracle import stream_oracle as SO
-from tests.test_host_logic import BatchRampCodec, FakeBatchStreamLM, RampCodec, _tts
+from tests.fakes import BatchRampCodec, FakeBatchStreamLM, RampCodec, _tts
 
 
 class QueueStreamLM:

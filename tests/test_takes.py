@@ -11,7 +11,7 @@ import torch
 
 from neutts_air_b200 import _lib
 from neutts_air_b200.lm import PagePool, Settings, SpeechLM, check_takes, fork_slots, resolve_settings
-from tests.test_host_logic import FakeCodec, FakePhonemizer, FakeTokenizer
+from tests.fakes import FakeCodec, FakePhonemizer, FakeTokenizer
 
 EOS = 9
 

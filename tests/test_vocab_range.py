@@ -1,7 +1,7 @@
 """CPU: the vocabulary range (speech-token-only decoding) -- its float64 semantics, validation and host plumbing.
 
 * The float64 chain with suppression (every id outside [lo, hi) + EOS -> -inf, then the chain of
-  ``test_sampling_controls``) equals transformers' SuppressTokensLogitsProcessor, MinNewTokensLengthLogitsProcessor
+  ``sampler_ref.py``) equals transformers' SuppressTokensLogitsProcessor, MinNewTokensLengthLogitsProcessor
   and the four warpers applied in order.
 * ``check_vocab_range`` mirrors ``nt_lm_set_vocab_range``'s rules.
 * Stub engines: a default call never touches the range, a range is set before the first prefill, a range left on is
@@ -16,19 +16,8 @@ import pytest
 import torch
 
 from neutts_air_b200.lm import check_vocab_range
-from tests.test_gpu_sampler import processed_scores
-from tests.test_host_logic import FakeTokenizer
-from tests.test_queue_host import EOS, QueueStub, _prompts
-from tests.test_sampling_controls import GenerateBackbone, KwBackbone, _facade, chain64
-
-
-def suppressed_scores(logits, lo: int, hi: int, eos: int, ngen: int, min_new: int, temperature: float):
-    s = np.asarray(logits, dtype=np.float32).copy()
-    keep = np.zeros(s.size, dtype=bool)
-    keep[lo:hi] = True
-    keep[eos] = True
-    s[~keep] = -np.inf
-    return processed_scores(s, ngen, eos, min_new, temperature)
+from tests.fakes import EOS, FakeTokenizer, GenerateBackbone, KwBackbone, QueueStub, _facade, _prompts
+from tests.sampler_ref import chain64, suppressed_scores
 
 
 def test_suppression_chain_matches_transformers():
