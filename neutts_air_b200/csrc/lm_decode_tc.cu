@@ -65,6 +65,9 @@ NT_DEVINL uint32_t pack2(__nv_bfloat16 a, __nv_bfloat16 b) {
   return static_cast<uint32_t>(__bfloat16_as_ushort(a)) | (static_cast<uint32_t>(__bfloat16_as_ushort(b)) << 16);
 }
 NT_DEVINL void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
+// register budget of the calling warpgroup (every thread of it executes the same instruction)
+template <int R> NT_DEVINL void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> NT_DEVINL void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 NT_DEVINL void bar_epi() { asm volatile("bar.sync 2, 128;" ::: "memory"); }  // the four epilogue warps
 
 struct TcProf {   // timeline of one CTA: buf[n] = %globaltimer, buf[512 + n] = mark id
@@ -231,118 +234,15 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     mbar_wait(&ms->go_bar, static_cast<uint32_t>(step) & 1u);
     return *reinterpret_cast<volatile int*>(&ms->stop) == 0;
   };
-  if (warp == kTcStreamWarp) {
-    // ================================================================== weight stream
-    // The whole warp walks the plan (warp-uniform control flow); one elected lane issues the copies.  elect.sync is
-    // re-executed at every use: it is also the point where the lanes RECONVERGE after a data-dependent wait loop --
-    // the compiler emits the TMA / MMA instruction itself unpredicated (only its operand moves are predicated), so a
-    // lane group that reached it without the leader would issue it with stale operands.
-    // weights pass through L2 once per step: evict_first keeps KV pages, hand-off buffers and logits resident
-    const uint64_t wpolicy = P.weights_evict_first ? l2_policy_evict_first() : 0ull;
-    int slot = 0;
-    uint32_t par = 0;       // parity of the slot's NEXT completion of empty_bar that we must have seen
-    bool wrapped = false;   // ring used at least once
-    auto push = [&](const CUtensorMap* m, int kcol, int row) {
-      if (wrapped) mbar_wait(&ms->empty_bar[slot], par ^ 1);
-      if (elect_one()) {
-        mbar_arrive_expect_tx(&ms->full_bar[slot], 16384);
-        if (wpolicy) tma_load_2d_hint(ring + static_cast<size_t>(slot) * 16384, m, kcol, row, &ms->full_bar[slot], wpolicy);
-        else tma_load_2d(ring + static_cast<size_t>(slot) * 16384, m, kcol, row, &ms->full_bar[slot]);
-      }
-      if (++slot == NS) slot = 0, par ^= 1, wrapped = true;
-    };
-    for (int step = 0; step < P.n_steps; ++step) {
-      if (!wait_go(step)) break;
-      for (int l = 0; l < L; ++l)
-        for (int ph = 0; ph < 4; ++ph) {
-          const CUtensorMap* m = wmaps + 4 * l + ph;
-          const int n_it = uniform(plan.n[ph]);
-          for (int i = 0; i < n_it; ++i) {
-            const int tile = uniform(plan.it[ph][i].tile), kb0 = uniform(plan.it[ph][i].kb0), nkb = uniform(plan.it[ph][i].nkb);
-            for (int kb = 0; kb < nkb; ++kb) push(m, (kb0 + kb) * 64, tile * 128);
-          }
-        }
-      const CUtensorMap* hm = wmaps + 4 * P.total_layers;
-      const int t0 = uniform(plan.head_t0), t1 = uniform(plan.head_t1);
-      for (int t = t0; t < t1; ++t) {
-        const int row0 = uniform(head_tile(t)) * 128;
-        for (int kb = 0; kb < KBH; ++kb) push(hm, kb * 64, row0);
-      }
-    }
-  } else if (warp >= kTcMmaWarp0) {
-    // ================================================================== MMA warpgroup (warps kTcMmaWarp0 .. + 3)
-    // acc0 = weight rows [0, 64) of the tile, acc1 = rows [64, 128).  One k-block's MMAs form a commit group; a ring
-    // slot is released (one arrival per warp) once the next group has been issued and the older one retired.
-    int slot = 0;
-    uint32_t par = 0;
-    uint32_t bop_n = 0, acc_n = 0;
-    const uint32_t bop_addr = smem_u32(uni);
-    const uint32_t ring_addr = smem_u32(ring);
-    // one item: nkb ring tiles against B chunks chunk0, chunk0 + 1, ...
-    auto run_item = [&](int nkb, int chunk0) {
-      float acc0[NT / 2], acc1[NT / 2];
-#pragma unroll
-      for (int i = 0; i < NT / 2; ++i) acc0[i] = acc1[i] = 0.f;
-      int prev = -1;
-      for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait(&ms->full_bar[slot], par);
-        const uint64_t adesc = wgmma_desc_sw128(ring_addr + static_cast<uint32_t>(slot) * 16384u);
-        const uint64_t bdesc = wgmma_desc_sw128(bop_addr + static_cast<uint32_t>(chunk0 + kb) * CHUNK);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          wgmma_bf16<NT>(acc0, adesc + 2 * k, bdesc + 2 * k, 1u);
-          wgmma_bf16<NT>(acc1, adesc + 512 + 2 * k, bdesc + 2 * k, 1u);
-        }
-        wgmma_commit();
-        wgmma_wait<1>();
-        if (prev >= 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&ms->empty_bar[prev]);
-        }
-        prev = slot;
-        if (++slot == NS) slot = 0, par ^= 1;
-      }
-      wgmma_wait<0>();
-      wgmma_fence_regs(acc0);
-      wgmma_fence_regs(acc1);
-      __syncwarp();
-      if (prev >= 0 && lane == 0) mbar_arrive(&ms->empty_bar[prev]);
-      mbar_wait(&ms->acc_empty, (acc_n & 1) ^ 1);
-      wgmma_store_rows<NT>(acc0, accs, ACC_LD, 0);
-      wgmma_store_rows<NT>(acc1, accs, ACC_LD, 64);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&ms->acc_full);
-      ++acc_n;
-    };
-    const int gu_split = uniform(plan.gu_split);
-    const int n_head = uniform(n_head_tiles);
-    for (int step = 0; step < P.n_steps; ++step) {
-      if (!wait_go(step)) break;
-      for (int l = 0; l < L; ++l)
-        for (int ph = 0; ph < 4; ++ph) {
-          const int n_it = uniform(plan.n[ph]);
-          if (n_it == 0) continue;
-          mbar_wait(&ms->bop_bar, bop_n & 1);
-          ++bop_n;
-          int chunk = 0;
-          for (int i = 0; i < n_it; ++i) {
-            const int nkb = uniform(plan.it[ph][i].nkb);
-            if (ph == kPhG && !gu_split) {
-              run_item(nkb, 0);   // whole K, all items share the staged input
-            } else {
-              run_item(nkb, chunk);
-              chunk += nkb;
-            }
-          }
-        }
-      if (n_head > 0) {
-        mbar_wait(&ms->bop_bar, bop_n & 1);
-        ++bop_n;
-        for (int t = 0; t < n_head; ++t) run_item(KBH, 0);
-      }
-    }
-  } else {
+  // Register budgets per warpgroup (__launch_bounds__(512, 1) starts every thread at 128): WG3 keeps what the weight
+  // stream needs, WG2 the accumulators of two m64 x NT halves, and the worker warpgroups take the rest.
+  // 128 * (kRegStream + kRegMma) + 256 * kRegWork = 64 K registers.
+  constexpr int kRegStream = 24, kRegMma = NT == 64 ? 104 : (NT == 32 ? 72 : 56), kRegWork = (65536 / 128 - kRegStream - kRegMma) / 2;
+  static_assert(kRegWork % 8 == 0 && kRegWork <= 256, "setmaxnreg takes a multiple of 8 up to 256");
+  // Each setmaxnreg opens the branch of its role, so that ptxas allocates the role's code under that budget.  The
+  // worker branch comes first: laid out behind the other two, ptxas kept it at the entry budget of 128.
+  if (warp < kTcMmaWarp0) {
+    setmaxnreg_inc<kRegWork>();
     // ================================================================== worker warps 0..7
     const SyncConsumers csync;
     const unsigned G = gridDim.x;
@@ -1022,6 +922,121 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     if (tid == 0) {   // wake a warp that waits for a step that will not run
       *reinterpret_cast<volatile int*>(&ms->stop) = 1;
       mbar_arrive(&ms->go_bar);
+    }
+    } else if (warp < kTcStreamWarp) {
+    setmaxnreg_dec<kRegMma>();
+    // ================================================================== MMA warpgroup (warps kTcMmaWarp0 .. + 3)
+    // acc0 = weight rows [0, 64) of the tile, acc1 = rows [64, 128).  One k-block's MMAs form a commit group; a ring
+    // slot is released (one arrival per warp) once the next group has been issued and the older one retired.
+    int slot = 0;
+    uint32_t par = 0;
+    uint32_t bop_n = 0, acc_n = 0;
+    const uint32_t bop_addr = smem_u32(uni);
+    const uint32_t ring_addr = smem_u32(ring);
+    // one item: nkb ring tiles against B chunks chunk0, chunk0 + 1, ...
+    auto run_item = [&](int nkb, int chunk0) {
+      float acc0[NT / 2], acc1[NT / 2];
+#pragma unroll
+      for (int i = 0; i < NT / 2; ++i) acc0[i] = acc1[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(&ms->full_bar[slot], par);
+        const uint64_t adesc = wgmma_desc_sw128(ring_addr + static_cast<uint32_t>(slot) * 16384u);
+        const uint64_t bdesc = wgmma_desc_sw128(bop_addr + static_cast<uint32_t>(chunk0 + kb) * CHUNK);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          wgmma_bf16<NT>(acc0, adesc + 2 * k, bdesc + 2 * k, 1u);
+          wgmma_bf16<NT>(acc1, adesc + 512 + 2 * k, bdesc + 2 * k, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&ms->empty_bar[prev]);
+        }
+        prev = slot;
+        if (++slot == NS) slot = 0, par ^= 1;
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc0);
+      wgmma_fence_regs(acc1);
+      __syncwarp();
+      if (prev >= 0 && lane == 0) mbar_arrive(&ms->empty_bar[prev]);
+      mbar_wait(&ms->acc_empty, (acc_n & 1) ^ 1);
+      wgmma_store_rows<NT>(acc0, accs, ACC_LD, 0);
+      wgmma_store_rows<NT>(acc1, accs, ACC_LD, 64);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&ms->acc_full);
+      ++acc_n;
+    };
+    const int gu_split = uniform(plan.gu_split);
+    const int n_head = uniform(n_head_tiles);
+    for (int step = 0; step < P.n_steps; ++step) {
+      if (!wait_go(step)) break;
+      for (int l = 0; l < L; ++l)
+        for (int ph = 0; ph < 4; ++ph) {
+          const int n_it = uniform(plan.n[ph]);
+          if (n_it == 0) continue;
+          mbar_wait(&ms->bop_bar, bop_n & 1);
+          ++bop_n;
+          int chunk = 0;
+          for (int i = 0; i < n_it; ++i) {
+            const int nkb = uniform(plan.it[ph][i].nkb);
+            if (ph == kPhG && !gu_split) {
+              run_item(nkb, 0);   // whole K, all items share the staged input
+            } else {
+              run_item(nkb, chunk);
+              chunk += nkb;
+            }
+          }
+        }
+      if (n_head > 0) {
+        mbar_wait(&ms->bop_bar, bop_n & 1);
+        ++bop_n;
+        for (int t = 0; t < n_head; ++t) run_item(KBH, 0);
+      }
+    }
+  } else {
+    setmaxnreg_dec<kRegStream>();
+    // the parked warps 13..15 (they make WG3 a whole warpgroup) run no step and go on to the closing block barrier
+    const int n_steps = warp == kTcStreamWarp ? P.n_steps : 0;
+    // ================================================================== weight stream
+    // The whole warp walks the plan (warp-uniform control flow); one elected lane issues the copies.  elect.sync is
+    // re-executed at every use: it is also the point where the lanes RECONVERGE after a data-dependent wait loop --
+    // the compiler emits the TMA / MMA instruction itself unpredicated (only its operand moves are predicated), so a
+    // lane group that reached it without the leader would issue it with stale operands.
+    // weights pass through L2 once per step: evict_first keeps KV pages, hand-off buffers and logits resident
+    const uint64_t wpolicy = P.weights_evict_first ? l2_policy_evict_first() : 0ull;
+    int slot = 0;
+    uint32_t par = 0;       // parity of the slot's NEXT completion of empty_bar that we must have seen
+    bool wrapped = false;   // ring used at least once
+    auto push = [&](const CUtensorMap* m, int kcol, int row) {
+      if (wrapped) mbar_wait(&ms->empty_bar[slot], par ^ 1);
+      if (elect_one()) {
+        mbar_arrive_expect_tx(&ms->full_bar[slot], 16384);
+        if (wpolicy) tma_load_2d_hint(ring + static_cast<size_t>(slot) * 16384, m, kcol, row, &ms->full_bar[slot], wpolicy);
+        else tma_load_2d(ring + static_cast<size_t>(slot) * 16384, m, kcol, row, &ms->full_bar[slot]);
+      }
+      if (++slot == NS) slot = 0, par ^= 1, wrapped = true;
+    };
+    for (int step = 0; step < n_steps; ++step) {
+      if (!wait_go(step)) break;
+      for (int l = 0; l < L; ++l)
+        for (int ph = 0; ph < 4; ++ph) {
+          const CUtensorMap* m = wmaps + 4 * l + ph;
+          const int n_it = uniform(plan.n[ph]);
+          for (int i = 0; i < n_it; ++i) {
+            const int tile = uniform(plan.it[ph][i].tile), kb0 = uniform(plan.it[ph][i].kb0), nkb = uniform(plan.it[ph][i].nkb);
+            for (int kb = 0; kb < nkb; ++kb) push(m, (kb0 + kb) * 64, tile * 128);
+          }
+        }
+      const CUtensorMap* hm = wmaps + 4 * P.total_layers;
+      const int t0 = uniform(plan.head_t0), t1 = uniform(plan.head_t1);
+      for (int t = t0; t < t1; ++t) {
+        const int row0 = uniform(head_tile(t)) * 128;
+        for (int kb = 0; kb < KBH; ++kb) push(hm, kb * 64, row0);
+      }
     }
   }
   __syncthreads();

@@ -8,9 +8,11 @@
 namespace nt {
 
 constexpr int kTcMaxItems = 4;      // work items of one GEMM phase a CTA may own
-constexpr int kTcMmaWarp0 = 8;      // warps 8..11: the MMA warpgroup (warpgroup-aligned)
-constexpr int kTcStreamWarp = 12;   // the weight-stream warp
-constexpr int kTcThreads = 416;     // 8 worker warps + 1 MMA warpgroup + 1 weight-stream warp
+// Four whole warpgroups, so that each can set its own register budget (setmaxnreg acts on a warpgroup):
+// WG0-1 = worker warps 0..7, WG2 = the MMA warpgroup, WG3 = the weight-stream warp + 3 parked warps.
+constexpr int kTcMmaWarp0 = 8;      // warps 8..11: the MMA warpgroup
+constexpr int kTcStreamWarp = 12;   // the weight-stream warp (warps 13..15 only take part in the kernel's block barriers)
+constexpr int kTcThreads = 512;
 constexpr int kTcMaxBatch = 64;
 constexpr int kTcDefaultMaxBatch = 16;  // nt_lm_decode's default: larger batches take the per-op chain
 constexpr int kTcMaxSlices = 16;
