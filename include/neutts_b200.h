@@ -146,7 +146,8 @@ int nt_lm_destroy(nt_lm* lm);
 
 /* Prefill B prompts packed back to back: ids [total] (device), cu_seqlens [B+1] (host).
  * Fills the KV cache, samples the first token of every sequence (A2 + A10-A12 of SURVEY §8a).
- * logits_out: optional device f32 [B][vocab] receiving the last-position logits. */
+ * logits_out: optional device f32 [B][vocab] receiving the last-position logits.
+ * This is nt_lm_prefill_fork with n = 1: prompt b in slot b, every slot reset. */
 int nt_lm_prefill(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu_seqlens_host, int B,
                   const nt_sampling* sp, float* logits_out, void* stream);
 
@@ -161,10 +162,10 @@ int nt_lm_prefill_slots(nt_lm* lm, const nt_lm_state* st, const int32_t* slots_h
                         const int32_t* ids, const int32_t* cu_seqlens_host, int B, const nt_sampling* sp,
                         float* logits_out, void* stream);
 
-/* n takes of each of B prompts from one prefill (transformers' num_return_sequences).  A full prefill like
- * nt_lm_prefill: it resets every slot.  Take j of prompt i lives in slot i*n + j (repeat_interleave order);
+/* n takes of each of B prompts from one prefill (transformers' num_return_sequences).  A full prefill: it resets
+ * every slot.  Take j of prompt i lives in slot i*n + j (repeat_interleave order);
  * 1 <= B*n <= max_batch.  The prompts are prefilled once, into the page-table rows of the parent slots i*n, so
- * logits_out (optional, [B][vocab]) is bit-identical to nt_lm_prefill on the same B prompts.  Page sharing: the
+ * logits_out (optional, [B][vocab]) is bit-identical for every n on the same B prompts.  Page sharing: the
  * caller writes every take's page-table row before the call, naming the parent's pages for the P_i / 64 full prompt
  * pages and the take's own pages from page P_i / 64 on; the call copies rows [0, P_i % 64) of the parent's page
  * P_i / 64 into each other take's page P_i / 64 (every layer, K and V).  Afterwards every take has seq_lens = P_i,

@@ -589,9 +589,9 @@ static int prefill_layers(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, 
 }
 
 // Prompt rows -> KV cache + last-position logits in lm->logits (and logits_out).  table: see layers_gemm.
-// row_slot: the slot of every prompt row (nullptr: row b is slot b); it fills that slot's repetition-penalty history.
+// row_slot: the slot of every prompt row; it fills that slot's repetition-penalty history.
 static int prefill_forward(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, int B, int max_len,
-                           const int32_t* table, float* logits_out, int eos, cudaStream_t stream, const int32_t* row_slot = nullptr) {
+                           const int32_t* table, float* logits_out, int eos, cudaStream_t stream, const int32_t* row_slot) {
   const nt_lm_config& c = lm->cfg;
   int rc;
   if ((rc = vocab_fill(lm, B, stream))) return rc;
@@ -603,26 +603,6 @@ static int prefill_forward(nt_lm* lm, const nt_lm_state* st, const int32_t* ids,
   if ((rc = lm_head_rows(lm, lm->h_last, B, lm->logits, stream, nullptr, eos, row_slot))) return rc;
   if (logits_out)
     NT_CUDA_CHECK(cudaMemcpyAsync(logits_out, lm->logits, size_t(B) * c.vocab_size * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-  return NT_OK;
-}
-
-extern "C" int nt_lm_prefill(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, int B,
-                             const nt_sampling* sp, float* logits_out, void* stream_) {
-  if (!lm || !st || !ids || !cu) return set_error(NT_ERR_INVALID, "nt_lm_prefill: null argument");
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  const nt_lm_config& c = lm->cfg;
-  if (B < 1 || B > c.max_batch) return set_error(NT_ERR_INVALID, "batch %d not in 1..%d", B, c.max_batch);
-  int rc = check_sampling(lm, st, sp);
-  if (rc) return rc;
-  std::vector<int> lens;
-  int max_len = 0;
-  if ((rc = prefill_stage(lm, cu, B, lens, max_len, stream))) return rc;
-  if ((rc = prefill_forward(lm, st, ids, cu, B, max_len, nullptr, logits_out, sp->eos_id, stream))) return rc;
-  NT_CUDA_CHECK(cudaMemcpyAsync(st->seq_lens, lens.data(), B * sizeof(int), cudaMemcpyHostToDevice, stream));
-  NT_CUDA_CHECK(cudaMemsetAsync(lm->slot_key, 0xff, size_t(c.max_batch) * sizeof(int), stream));  // every slot: slot + slot_base
-  SamplerParams s = make_sampler(lm, st, sp);
-  if ((rc = run_sampler(lm, s, B, stream))) return rc;
-  lm->prefilled = true;
   return NT_OK;
 }
 
@@ -670,7 +650,7 @@ extern "C" int nt_lm_prefill_slots(nt_lm* lm, const nt_lm_state* st, const int32
 
 // n takes of each of B prompts: take j of prompt i lives in slot i * n + j, and slot i * n is its prompt's parent.  The
 // prefill chain runs once over the B prompts on the parents' page-table rows (gathered into a compact table as in
-// nt_lm_prefill_slots); its KV and logits are those of nt_lm_prefill on the same prompts.  A child's page-table row
+// nt_lm_prefill_slots); its KV and logits do not depend on n, and n = 1 is nt_lm_prefill.  A child's page-table row
 // already names the parent's full prompt pages (the caller shares them), so only the partly filled last prompt page
 // is copied into the child's own page, together with the parent's repetition-penalty history.  The sampler then
 // draws every take from its parent's logits row (row_src), with the take's own slot state and Philox stream.
@@ -714,6 +694,14 @@ extern "C" int nt_lm_prefill_fork(nt_lm* lm, const nt_lm_state* st, const int32_
   if ((rc = run_sampler(lm, s, N, stream))) return rc;
   lm->prefilled = true;
   return NT_OK;
+}
+
+// One take of each prompt: slot b holds prompt b, with no children to copy tails to and no row_src.
+extern "C" int nt_lm_prefill(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, int B,
+                             const nt_sampling* sp, float* logits_out, void* stream_) {
+  if (!lm || !st || !ids || !cu) return set_error(NT_ERR_INVALID, "nt_lm_prefill: null argument");
+  if (B < 1 || B > lm->cfg.max_batch) return set_error(NT_ERR_INVALID, "batch %d not in 1..%d", B, lm->cfg.max_batch);
+  return nt_lm_prefill_fork(lm, st, ids, cu, B, 1, sp, logits_out, stream_);
 }
 
 // Teacher-forced scoring.  The caller's scratch holds, for one block of R scored rows, the (max, sum exp) pair of every

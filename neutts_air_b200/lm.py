@@ -575,48 +575,16 @@ class SpeechLM:
             table[s, : need[i]] = pages
 
     def prefill(self, prompts, sp, return_logits: bool = False):
-        """prompts: list of 1-D int sequences.  Fills the KV cache and samples the first token."""
-        lens = [len(p) for p in prompts]
-        if not lens or min(lens) < 1:
-            raise ValueError("empty prompt")
-        return self.prefill_packed(self._stage_ids(prompts), lens, sp, return_logits)
-
-    def prefill_packed(self, ids_host: torch.Tensor, lens, sp, return_logits: bool = False):
-        """ids_host: int32 host tensor (pinned memory makes the H2D copy asynchronous) holding the
-        prompts back to back; lens: their lengths."""
-        B = len(lens)
-        if not 1 <= B <= self.max_batch:
-            raise ValueError(f"batch {B} not in 1..{self.max_batch}")
-        if ids_host.dtype != torch.int32 or ids_host.numel() != sum(lens):
-            raise ValueError("ids_host must be int32 with sum(lens) elements")
-        for b, n in enumerate(lens):
-            if not 1 <= n < self.max_ctx:
-                raise ValueError(f"prompt {b} has length {n}; must be in 1..{self.max_ctx - 1}")
-        self.release_pages()
-        table = np.zeros((self.max_batch, self.max_pages), dtype=np.int32)
-        self._alloc_pages(table, range(B), lens, [sp.max_new_tokens] * B)
-        cu = np.zeros(B + 1, dtype=np.int32)
-        cu[1:] = np.cumsum(lens)
-        with torch.cuda.device(self.device):
-            ids = ids_host.to(self.device, non_blocking=True)
-            if self._table_host is None or not np.array_equal(self._table_host, table):
-                self.page_table.copy_(torch.from_numpy(table))
-                self._table_host = table
-            self.n_generated.zero_()
-            self.done.zero_()
-            logits = torch.empty(B, self.shape.vocab_size, dtype=torch.float32, device=self.device) if return_logits else None
-            _lib.check(self.L.nt_lm_prefill(self.handle, C.byref(self.state), ids.data_ptr(),
-                                            cu.ctypes.data_as(C.POINTER(C.c_int32)), B, C.byref(sp),
-                                            logits.data_ptr() if return_logits else None, _lib.current_stream_ptr()))
-        self._B = B
-        return logits
+        """prompts: list of 1-D int sequences.  Fills the KV cache and samples the first token of every prompt, prompt b
+        in slot b: ``prefill_fork`` with one take per prompt."""
+        return self.prefill_fork(prompts, 1, sp, return_logits)
 
     def prefill_fork(self, prompts, n: int, sp, return_logits: bool = False):
         """n takes of every prompt from one prefill (``nt_lm_prefill_fork``).  Take j of prompt i lives in slot i * n + j
         and draws from Philox stream i * n + j + slot_base, as in ``prefill`` on the prompts each repeated n times; the
         prompts are prefilled once, and all n takes read one copy of each full prompt page (``_alloc_fork_pages``).
         Resets every slot; afterwards ``decode`` continues all len(prompts) * n takes.  Returns the [len(prompts), vocab]
-        last-position logits (identical to ``prefill``'s on the same prompts) when ``return_logits``."""
+        last-position logits (the same for every n) when ``return_logits``."""
         B = len(prompts)
         n = check_takes(B, n, self.max_batch)
         lens = [len(p) for p in prompts]

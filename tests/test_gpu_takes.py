@@ -2,13 +2,14 @@
 NeuTTS.infer_batch(takes=n)).
 
 The takes of a prompt share its full KV pages; each has a private copy of the partly filled last prompt page and pages
-of its own for generated tokens.  Checked here: the fork's prefill logits are those of a plain prefill, bit for bit; the
-page-table rows and the copied tail rows; decoding over shared pages gives exactly the logits of private copies and
-never writes a shared page; the first draw of every take is the float64 reference draw on its prompt's logits with its
+of its own for generated tokens.  Checked here: the fork's prefill logits are those of one take (a plain prefill), bit
+for bit, and the C entry nt_lm_prefill is that one take; the page-table rows and the copied tail rows; decoding over
+shared pages gives exactly the logits of private copies and never writes a shared page; the first draw of every take is the float64 reference draw on its prompt's logits with its
 own Philox stream; a refill of one take leaves its siblings alone; the public outputs keep transformers' layout.
 Prompt lengths cross page boundaries and include a multiple of 64; B * n covers the GEMV decode (<= 4), the persistent
 kernel (<= 16) and the per-op chain (> 16).
 """
+import ctypes as C
 import math
 import warnings
 
@@ -16,6 +17,7 @@ import numpy as np
 import pytest
 import torch
 
+from neutts_air_b200 import _lib
 from neutts_air_b200.lm import fork_slots
 from oracle import lm_oracle as O
 from tests.helpers import _bar, _setup, _tts, gather_kv, set_decode_impl
@@ -71,7 +73,7 @@ def test_fork_prefill_kv_and_decode(cuda, B, n, impl, monkeypatch):
     lens = [len(p) for p in prompts]
     sp = lm.sampling(eos, min_new_tokens=0, max_new_tokens=1 + STEPS, forced=forced)
     lf = lm.prefill_fork(prompts, n, sp, return_logits=True)
-    # 1. the prefill logits are those of a plain prefill of the same prompts, bit for bit
+    # 1. the prefill logits are those of a plain prefill (one take) of the same prompts, bit for bit
     lp = plain.prefill(prompts, plain.sampling(eos, min_new_tokens=0, max_new_tokens=1 + STEPS), return_logits=True)
     assert torch.equal(lf, lp)
     # 2. page-table rows: shared full pages, private tail page with the parent's rows, private pages after it
@@ -115,6 +117,33 @@ def test_fork_prefill_kv_and_decode(cuda, B, n, impl, monkeypatch):
     for i, j, s, _ in fork_slots(B, n):
         assert out[s, : 1 + STEPS].tolist() == forced[s].tolist()
         assert int(ngen[s]) == 1 + STEPS and int(seq[s]) == lens[i] + STEPS
+
+
+def test_c_prefill_is_one_take(cuda):
+    """The C entry nt_lm_prefill is nt_lm_prefill_fork with one take: on the pages SpeechLM.prefill laid out, it gives
+    the same logits, first tokens and slot state, resets every slot's counters itself, and refuses a batch outside
+    1..max_batch with its own message."""
+    B = 3
+    cfg, w, lm = _setup(B + 1, page_shuffle_seed=7)
+    prompts = _prompts(B)
+    sp = lm.sampling(cfg.vocab_size - 1, min_new_tokens=0, max_new_tokens=1 + STEPS, seed=4)
+    want = lm.prefill(prompts, sp, return_logits=True)
+    state = lambda: [t.clone() for t in (lm.out_tokens, lm.cur_token, lm.seq_lens, lm.n_generated, lm.done)]
+    before = state()
+    ids = torch.tensor([t for p in prompts for t in p], dtype=torch.int32, device=lm.device)
+    cu = np.cumsum([0] + [len(p) for p in prompts]).astype(np.int32)
+    got = torch.empty_like(want)
+    call = lambda b: lm.L.nt_lm_prefill(lm.handle, C.byref(lm.state), ids.data_ptr(), cu.ctypes.data_as(C.POINTER(C.c_int32)),
+                                        b, C.byref(sp), got.data_ptr(), _lib.current_stream_ptr())
+    lm.n_generated.fill_(7)
+    lm.done.fill_(1)
+    _lib.check(call(B))
+    torch.cuda.synchronize()
+    assert torch.equal(got, want)
+    assert all(torch.equal(a, b) for a, b in zip(state(), before))
+    for b in (0, B + 2):
+        with pytest.raises(ValueError, match=rf"batch {b} not in 1\.\.{B + 1}"):
+            _lib.check(call(b))
 
 
 PALETTE = [(0.8, 40, 0.9, 0.0), (1.3, 64, 1.0, 0.02), (1.0, 20, 0.7, 0.05)]

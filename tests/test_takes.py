@@ -170,6 +170,18 @@ def test_check_takes():
         check_takes(3, 3, 8)
 
 
+def test_prefill_argument_errors():
+    """SpeechLM.prefill (one take per prompt) raises ValueError for an empty call, an empty or over-long prompt, more
+    prompts than slots and an id outside the vocabulary, before it touches the page pool or the device."""
+    lm = object.__new__(SpeechLM)            # host fields only: a check that came later would hit a missing attribute
+    lm.max_batch, lm.max_ctx, lm.shape = 2, 128, types.SimpleNamespace(vocab_size=4096)
+    sp = types.SimpleNamespace(max_new_tokens=8)
+    for prompts, msg in (([], "empty prompt"), ([[1], []], "empty prompt"), ([[1] * 128], r"1\.\.127"),
+                         ([[1]] * 3, "slots"), ([[1, 4096]], "out of range"), ([[-1]], "out of range")):
+        with pytest.raises(ValueError, match=msg):
+            lm.prefill(prompts, sp)
+
+
 def test_generate_batch_validates_before_any_engine_call():
     lm = ForkStub(4)
     for n in (0, -2, 3):                                    # 3: 2 prompts x 3 takes > 4 slots
