@@ -261,6 +261,31 @@ typedef struct {
  * nt_op_topk_sample and nt_lm_head_gemv ignore the penalty. */
 int nt_lm_set_repetition_penalty(nt_lm* lm, const nt_slot_penalty* host_table, void* stream);
 
+/* Per-slot length control: transformers' MinNewTokensLengthLogitsProcessor and ExponentialDecayLengthPenalty, applied
+ * after the repetition penalty and before the vocabulary range, the temperature and the warpers.  With n the slot's
+ * n_generated when its next token is drawn (tokens generated since its prompt):
+ *   - EOS is masked (-inf) while n < min_new_tokens; the entry replaces nt_sampling.min_new_tokens for the slot;
+ *   - while n > decay_start, with k = n - decay_start, the EOS score s becomes s + |s| * c_k (fp32 product, then fp32
+ *     sum), where c_k = (float)(pow(decay_factor, k) - 1) is computed in double on the host, as transformers does.
+ * Both act on the EOS logit alone and apply to greedy and teacher-forced runs too: every logits output and tile maximum
+ * holds the decayed EOS score, and every other id is bit-identical to the table off.  An entry with decay_factor == 1
+ * never touches the score.  A prefill draws token 0 of the slots it fills, where only the mask can apply. */
+typedef struct {
+  int32_t min_new_tokens;  /* >= 0 */
+  int32_t decay_start;     /* >= 0 and >= min_new_tokens - 1 (the decay never meets the -inf of the mask) */
+  double decay_factor;     /* finite, > 0; 1 = no decay */
+} nt_slot_length;
+
+/* host_table: max_batch entries (row s = slot s), or NULL = off (the default: nt_sampling.min_new_tokens for every slot,
+ * no decay).  Every entry is validated first; a bad one returns NT_ERR_INVALID and leaves the previous table in force.
+ * The table and each slot's c_k for k = 1 .. max_ctx are copied on `stream`; new values take effect at the next launch.
+ * A c_k that is not finite in fp32 is refused by the launch that could reach it: nt_lm_prefill_slots,
+ * nt_lm_prefill_fork and nt_lm_decode return NT_ERR_INVALID while some slot the call samples (the listed slots, the
+ * B * n takes, or slots 0 .. B - 1) has a non-finite c_k with k <= nt_sampling.max_new_tokens - decay_start.  Other
+ * slots may keep entries of an earlier call with a shorter cap.
+ * nt_op_topk_sample, nt_lm_head_gemv and nt_lm_score ignore the table. */
+int nt_lm_set_length_control(nt_lm* lm, const nt_slot_length* host_table, void* stream);
+
 /* Per-token log-probabilities.  out: caller-owned device fp32 [max_batch][max_new][2] (8-byte aligned); entry [s][n]
  * belongs to out_tokens[s][n] and is written wherever that token is (every sampler launch of nt_lm_prefill,
  * nt_lm_prefill_slots and nt_lm_decode); nothing else is written.  NULL switches it off (the default).

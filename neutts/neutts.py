@@ -27,7 +27,7 @@ from typing import Generator, Sequence
 import numpy as np
 import torch
 
-from neutts_air_b200.lm import per_item, resolve_settings
+from neutts_air_b200.lm import per_item, per_prompt_decay, resolve_settings
 
 SPEECH_RE = re.compile(r"<\|speech_(\d+)\|>")
 CHAT = "user: Convert the text to speech:<|TEXT_REPLACE|>\nassistant:<|SPEECH_REPLACE|>"
@@ -35,10 +35,21 @@ CONTROL_DEFAULTS = dict(temperature=1.0, top_k=50, top_p=1.0, min_p=0.0)   # the
 PENALTY_DEFAULTS = dict(repetition_penalty=1.0, penalize_prompt=True)       # no repetition penalty, as the reference
 
 
-def _controls(n: int, temperature, top_k, top_p, min_p, repetition_penalty=1.0, penalize_prompt=True) -> dict:
-    """Sampling controls of n utterances: each a scalar or one value per utterance (a list then)."""
-    return per_item(n, "utterance", temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p,
-                    repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt)
+def _controls(n: int, temperature, top_k, top_p, min_p, repetition_penalty=1.0, penalize_prompt=True, min_new_tokens=50,
+              exponential_decay_length_penalty=None) -> dict:
+    """Sampling controls of n utterances: each a scalar or one value per utterance (a list then).  The length decay is
+    None, one (start, factor) tuple, or a list with one None / pair per utterance."""
+    ctl = per_item(n, "utterance", temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p,
+                   repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt, min_new_tokens=min_new_tokens)
+    decay = exponential_decay_length_penalty
+    if decay is not None:
+        per = per_prompt_decay(n, decay)
+        if all(d is None for d in per):   # a list with no pair asks for no decay: forward nothing
+            decay = None
+        else:
+            decay = tuple(decay) if per[0] is decay else [None if d is None else tuple(d) for d in per]
+    ctl["exponential_decay_length_penalty"] = decay
+    return ctl
 
 
 def _pick(ctl: dict, idx) -> dict:
@@ -55,6 +66,8 @@ def _backbone_kw(ctl: dict) -> dict:
     pen = {k: ctl.get(k, v) for k, v in PENALTY_DEFAULTS.items()}
     if any(isinstance(v, list) or v != PENALTY_DEFAULTS[k] for k, v in pen.items()):
         kw.update(pen)
+    if ctl.get("exponential_decay_length_penalty") is not None:
+        kw["exponential_decay_length_penalty"] = ctl["exponential_decay_length_penalty"]
     return kw
 
 
@@ -247,7 +260,7 @@ class NeuTTS:
         """Batched device-side generation; returns generated token ids per prompt (CPU int64 tensors), or with
         ``logprobs`` (ids, per-prompt float32 CPU tensors [n, 2] of (sampled, model) log-probabilities).
         Sampling parameters default to the reference's (``neutts/neutts.py:338-347``); ``ctl`` (see ``_controls``)
-        overrides them, per prompt where a control is a list.  ``takes`` > 1: that many takes of every prompt from
+        overrides them, per prompt where a control is a list; ``min_new_tokens`` is an int or one per prompt.  ``takes`` > 1: that many takes of every prompt from
         one prefill (len(prompts) * takes <= max_batch), of which the one ``best_takes`` picks is returned."""
         eos = self._tok_id("<|SPEECH_GENERATION_END|>")
         seed = self.seed if self.seed is not None else int(torch.randint(0, 2**31 - 1, (1,)).item())
@@ -283,10 +296,13 @@ class NeuTTS:
         for i, p in enumerate(prompts):
             t = torch.tensor(list(p)).unsqueeze(0).to(self.backbone.device)
             one = {k: v[i] if isinstance(v, list) else v for k, v in kw.items()}
+            if one.get("exponential_decay_length_penalty", ()) is None:   # this utterance has no decay: pass nothing
+                del one["exponential_decay_length_penalty"]
             one.update(suppress)
             with torch.no_grad():
                 o = self.backbone.generate(t, max_length=self.max_context, eos_token_id=eos, do_sample=True, use_cache=True,
-                                           min_new_tokens=min_new_tokens, **one)
+                                           min_new_tokens=min_new_tokens[i] if isinstance(min_new_tokens, list) else min_new_tokens,
+                                           **one)
             outs.append(o[0, t.shape[-1]:].cpu().long())
         return outs
 
@@ -354,25 +370,29 @@ class NeuTTS:
     # ------------------------------------------------------------------ public API
     def infer(self, text: str, ref_codes, ref_text: str, *, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0,
               min_p: float = 0.0, repetition_penalty: float = 1.0, penalize_prompt: bool = True,
-              return_logprobs: bool = False, takes: int = 1):
+              return_logprobs: bool = False, takes: int = 1, min_new_tokens: int = 50,
+              exponential_decay_length_penalty=None):
         """Text + reference voice -> 24 kHz float32 waveform (``neutts/neutts.py:216-243``).  The sampling controls
         default to the reference's values; see ``infer_batch``.  ``return_logprobs``: returns (waveform, log-probs).
         ``takes``: generate that many takes and keep the most probable one (``infer_batch``)."""
         out = self.infer_batch([text], [ref_codes], [ref_text], temperature=temperature, top_k=top_k, top_p=top_p,
                                min_p=min_p, repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt,
-                               return_logprobs=return_logprobs, takes=takes)
+                               return_logprobs=return_logprobs, takes=takes, min_new_tokens=min_new_tokens,
+                               exponential_decay_length_penalty=exponential_decay_length_penalty)
         return (out[0][0], out[1][0]) if return_logprobs else out[0]
 
     def infer_from_prompt_ids(self, prompts: Sequence[Sequence[int]], max_new_tokens: int | None = None,
                               min_new_tokens: int = 50, slot_base: int = 0, *, temperature=1.0, top_k=50, top_p=1.0,
                               min_p=0.0, repetition_penalty=1.0, penalize_prompt=True, return_logprobs: bool = False,
-                              takes: int = 1):
+                              takes: int = 1, exponential_decay_length_penalty=None):
         """Hot path only: prompt ids (host) -> waveforms (host).  Used by bench.py's end-to-end leg.
         ``slot_base`` offsets the sampler's Philox slot index so chunks / ranks under one seed draw independently.
         More prompts than ``max_batch`` go through the backbone's ``generate_queue`` when it has one.  Sampling
-        controls, ``return_logprobs`` and ``takes`` as in ``infer_batch`` (here len(prompts) * takes <= max_batch,
-        and ``slot_base`` counts takes)."""
-        ctl = _controls(len(prompts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)
+        controls, length controls, ``return_logprobs`` and ``takes`` as in ``infer_batch`` (here len(prompts) * takes <=
+        max_batch, and ``slot_base`` counts takes)."""
+        ctl = _controls(len(prompts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
+                        exponential_decay_length_penalty)
+        min_new_tokens = ctl.pop("min_new_tokens")
         takes = self._check_takes(takes)
         if takes > 1 and return_logprobs:
             self._check_logprobs()
@@ -385,7 +405,7 @@ class NeuTTS:
 
     def infer_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], distributed: bool = False, *,
                     temperature=1.0, top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0, penalize_prompt=True,
-                    return_logprobs: bool = False, takes: int = 1):
+                    return_logprobs: bool = False, takes: int = 1, min_new_tokens=50, exponential_decay_length_penalty=None):
         """List in / list out.  With ``distributed=True`` (inside an initialised torch.distributed job) the
         utterances are sharded over ranks and every rank returns all waveforms (one all-gather).
 
@@ -403,6 +423,14 @@ class NeuTTS:
         breaks loops of one repeated codec id; ``penalize_prompt=False`` leaves the prompt (the reference codes) out of
         that history.  Both are scalars or one value per utterance too.
 
+        Length controls (transformers' processors, acting on the end-of-speech score alone): ``min_new_tokens``
+        (default 50, the reference's one second of audio) masks the end of speech until that many tokens exist, an int
+        or one per utterance, so a short line need not run a whole second.  ``exponential_decay_length_penalty``
+        (start, factor), factor > 0 (ExponentialDecayLengthPenalty), is a soft cap: after ``start`` generated tokens the
+        end-of-speech score s becomes s + |s| * (factor ** k - 1) at step k past it, so an utterance that runs on ends
+        at a point the model picks near the length the caller expects, instead of being cut at the hard cap.  None, one
+        pair, or one None / pair per utterance; start must be >= min_new_tokens - 1.
+
         ``return_logprobs=True`` (not with ``distributed``; needs a ``SpeechLM`` backbone) returns (waveforms,
         log-probs): per utterance a float32 array [n_generated, 2] with the (sampled, model) log-probability of every
         generated token, EOS included (``SpeechLM.set_logprobs``).  Its rows follow the generated ids, not the codec
@@ -418,7 +446,8 @@ class NeuTTS:
         ``max_batch // takes``; ``return_logprobs`` returns the kept takes' rows."""
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
-        ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)
+        ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
+                        exponential_decay_length_penalty)
         takes = self._check_takes(takes, distributed)
         if return_logprobs:
             self._check_logprobs(distributed)
@@ -523,7 +552,8 @@ class NeuTTS:
 
     def infer_stream(self, text: str, ref_codes, ref_text: str, *, temperature: float = 1.0, top_k: int = 50,
                      top_p: float = 1.0, min_p: float = 0.0, repetition_penalty: float = 1.0,
-                     penalize_prompt: bool = True, takes: int = 1) -> Generator[np.ndarray, None, None]:
+                     penalize_prompt: bool = True, takes: int = 1, min_new_tokens: int = 50,
+                     exponential_decay_length_penalty=None) -> Generator[np.ndarray, None, None]:
         """Streaming synthesis with the reference's window geometry (``neutts/neutts.py:373-465``):
         every 25 new frames (once 5 look-ahead frames exist) the codec re-decodes
         [n - 50 - 1, n + 25 + 5 + 1) and the chunk is cross-faded with triangular weights.  Sampling controls as in
@@ -532,13 +562,15 @@ class NeuTTS:
         self._no_takes(takes)
         if self._is_quantized_model:  # kept for signature parity; never true on this build
             raise NotImplementedError("GGUF streaming is not part of the H100 build")
-        ctl = _controls(1, temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)
+        ctl = _controls(1, temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
+                        exponential_decay_length_penalty)
         prompt = self._apply_chat_template(ref_codes, ref_text, text)
         return self._stream(prompt, [int(c) for c in (ref_codes.tolist() if hasattr(ref_codes, "tolist") else ref_codes)], ctl)
 
     def infer_stream_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], *, temperature=1.0,
                            top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0,
-                           penalize_prompt=True, takes: int = 1) -> Generator[list, None, None]:
+                           penalize_prompt=True, takes: int = 1, min_new_tokens=50,
+                           exponential_decay_length_penalty=None) -> Generator[list, None, None]:
         """Streaming synthesis of many utterances at once (BASELINE.json configs[4]; the reference streams one
         utterance, ``neutts/neutts.py:373-465``).  Every yield is a list with one entry per utterance, as many entries
         as ``texts``: the next audio chunk (float32, cross-faded exactly as in ``infer_stream``) or ``None`` when that
@@ -559,7 +591,8 @@ class NeuTTS:
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
         self._stream_slots(len(texts))
-        ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt)
+        ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
+                        exponential_decay_length_penalty)
         prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(texts, ref_codes, ref_texts)]
         refs = [[int(c) for c in (rc.tolist() if hasattr(rc, "tolist") else rc)] for rc in ref_codes]
         return self._stream_batch(prompts, refs, ctl)
@@ -607,12 +640,13 @@ class NeuTTS:
         if min(limits) < 1:
             raise ValueError("prompt already at max_length")
         limit = max(limits)
-        st = resolve_settings(lm, N, vocab_range=self._speech_range(), **(ctl if ctl is not None else CONTROL_DEFAULTS))
-        top_k, temp = st.top_k, st.temperature
+        st = resolve_settings(lm, N, vocab_range=self._speech_range(), max_new=limit,
+                              **(ctl if ctl is not None else CONTROL_DEFAULTS))
+        top_k, temp, floor = st.top_k, st.temperature, st.min_new_tokens
         if queue or min(limits) < limit:   # a refill writes its newcomer's cap into the per-slot limits
-            sp = lm.sampling(eos, 50, limit, top_k, temp, seed, limits=limits[:B])
+            sp = lm.sampling(eos, floor, limit, top_k, temp, seed, limits=limits[:B])
         else:
-            sp = lm.sampling(eos, 50, limit, top_k, temp, seed)
+            sp = lm.sampling(eos, floor, limit, top_k, temp, seed)
         st.apply(lm, B)   # before the prefill, on the same stream
         dev = lm.out_tokens.device
         cap = max(len(r) for r in refs) + limit

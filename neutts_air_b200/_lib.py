@@ -69,6 +69,10 @@ class SlotPenalty(C.Structure):
     _fields_ = [("penalty", C.c_float), ("include_prompt", C.c_int32)]
 
 
+class SlotLength(C.Structure):
+    _fields_ = [("min_new_tokens", C.c_int32), ("decay_start", C.c_int32), ("decay_factor", C.c_double)]
+
+
 class CodecConfig(C.Structure):
     _fields_ = [
         ("hidden", C.c_int), ("depth", C.c_int), ("heads", C.c_int), ("head_dim", C.c_int),
@@ -98,7 +102,8 @@ EXPORTS = [
     "nt_last_error", "nt_abi_version", "nt_launch_count", "nt_gemm",
     "nt_lm_workspace_bytes", "nt_lm_create", "nt_lm_destroy", "nt_lm_prefill", "nt_lm_prefill_slots", "nt_lm_prefill_fork",
     "nt_lm_score_scratch_bytes", "nt_lm_score", "nt_lm_decode",
-    "nt_lm_set_slot_sampling", "nt_lm_set_vocab_range", "nt_lm_set_repetition_penalty", "nt_lm_set_logprobs",
+    "nt_lm_set_slot_sampling", "nt_lm_set_vocab_range", "nt_lm_set_repetition_penalty", "nt_lm_set_length_control",
+    "nt_lm_set_logprobs",
     "nt_lm_head_gemv",
     "nt_lm_debug_set_layers", "nt_lm_debug_ptr", "nt_lm_debug_set_profile", "nt_lm_debug_capture_sampler",
     "nt_debug_launch_chain", "nt_debug_decode_plan",
@@ -145,6 +150,7 @@ def lib() -> C.CDLL:
     L.nt_lm_set_slot_sampling.argtypes = [C.c_void_p, C.POINTER(SlotSampling), C.c_void_p]
     L.nt_lm_set_vocab_range.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
     L.nt_lm_set_repetition_penalty.argtypes = [C.c_void_p, C.POINTER(SlotPenalty), C.c_void_p]
+    L.nt_lm_set_length_control.argtypes = [C.c_void_p, C.POINTER(SlotLength), C.c_void_p]
     L.nt_lm_set_logprobs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     L.nt_lm_head_gemv.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     L.nt_lm_debug_set_layers.argtypes = [C.c_void_p, C.c_int]

@@ -84,6 +84,8 @@ struct StepSettings {
   bool vr_on = false;
   bool slot_sp_on = false;            // per-slot sampling table (nt_lm_set_slot_sampling)
   bool rep_on = false;                // repetition penalty table (nt_lm_set_repetition_penalty)
+  bool len_on = false;                // length-control table (nt_lm_set_length_control)
+  bool len_decay = false;             // ... and some entry decays (decay_factor != 1): the chain's fix-up launch
   float* logprob_out = nullptr;       // per-token log-probabilities (nt_lm_set_logprobs): nullptr = off
 };
 
@@ -140,6 +142,11 @@ struct nt_lm {
   nt_slot_penalty* rep_tab = nullptr; // [max_batch]
   int* rep_rec = nullptr;             // [max_batch] 1: the slot's history was built by a prefill while the table was on
   int rep_words = 0;                  // ceil(vocab_size / 32)
+  // length control (nt_lm_set_length_control): the per-slot table and every slot's c_k, k = 1 .. max_ctx
+  nt_slot_length* len_tab = nullptr;  // [max_batch]
+  float* len_c = nullptr;             // [max_batch][max_ctx]
+  // host: per slot, the decay start and the largest k with c_1 .. c_k finite in fp32 (checked at every launch)
+  std::vector<int> len_start, len_finite;
 };
 
 // The lm_head tiles a launch computes under the vocabulary range: [t_lo, t_hi), plus eos_tile when EOS lies outside
@@ -229,6 +236,8 @@ static size_t lm_carve(const nt_lm_config& c, void* ws, size_t bytes, F&& assign
     (L)->rep_hist = a.take<uint32_t>(size_t(c.max_batch) * ((V + 31) / 32));                   \
     (L)->rep_tab = a.take<nt_slot_penalty>(c.max_batch);                                       \
     (L)->rep_rec = a.take<int>(c.max_batch);                                                   \
+    (L)->len_tab = a.take<nt_slot_length>(c.max_batch);                                        \
+    (L)->len_c = a.take<float>(size_t(c.max_batch) * c.max_ctx);                               \
   }
 
 static int lm_check_config(const nt_lm_config* c) {
@@ -401,6 +410,9 @@ static SamplerParams make_sampler(const nt_lm* lm, const nt_lm_state* st, const 
   s.slot_sp = ss.slot_sp_on ? lm->slot_sp : nullptr;
   s.rep_hist = ss.rep_on ? lm->rep_hist : nullptr;
   s.rep_words = lm->rep_words;
+  s.len_tab = ss.len_on ? lm->len_tab : nullptr;
+  s.len_c = lm->len_c;
+  s.len_pitch = lm->cfg.max_ctx;
   s.logprob_out = ss.logprob_out;
   s.dbg_topk_val = ss.dbg_topk_val, s.dbg_topk_idx = ss.dbg_topk_idx, s.dbg_token = ss.dbg_token;
   return s;
@@ -411,6 +423,20 @@ static int check_sampling(const nt_lm* lm, const nt_lm_state* st, const nt_sampl
   if (sp->eos_id < 0 || sp->eos_id >= lm->cfg.vocab_size) return set_error(NT_ERR_INVALID, "eos_id out of range");
   if (sp->max_new_tokens < 1 || sp->max_new_tokens > st->max_new)
     return set_error(NT_ERR_INVALID, "max_new_tokens %d not in 1..%d", sp->max_new_tokens, st->max_new);
+  return NT_OK;
+}
+
+// While the length-control table is on: every slot a launch samples (slots[0 .. n), or 0 .. n - 1 when slots is
+// nullptr) must have a finite c_k for every k <= max_new_tokens - decay_start.  Slots the launch never reads may keep
+// entries of an earlier call with a shorter cap.
+static int check_length(const nt_lm* lm, const nt_sampling* sp, const int32_t* slots, int n) {
+  if (!lm->step.len_on) return NT_OK;
+  for (int i = 0; i < n; ++i) {
+    const int s = slots ? slots[i] : i;
+    if (sp->max_new_tokens - lm->len_start[s] > lm->len_finite[s])
+      return set_error(NT_ERR_INVALID, "slot %d: the length decay constant c_%d is not finite in fp32 (max_new_tokens %d, decay start %d)",
+                       s, lm->len_finite[s] + 1, sp->max_new_tokens, lm->len_start[s]);
+  }
   return NT_OK;
 }
 
@@ -428,6 +454,7 @@ static int rep_fixup(nt_lm* lm, int B, float* logits, float* tmax, int eos, cons
 }
 
 // lm_head on B hidden rows (fp32, un-normalised) -> `logits`.
+// decay (decode steps, row b = slot b): the length-control fix-up follows the penalty's while some entry decays.
 // eos >= 0: a sampler launch follows (logits = lm->logits): apply the vocabulary range with this EOS id and leave the
 // raw maximum of every 128-row tile of every row in lm->tmax; the GEMM epilogue takes them when it tiles the vocabulary
 // by 128, one small kernel on the finished rows otherwise.  -1: logits only, every row (nt_lm_head_gemv).  Under
@@ -435,7 +462,7 @@ static int rep_fixup(nt_lm* lm, int B, float* logits, float* tmax, int eos, cons
 // a row slice of the full-vocabulary launch with the same per-row arithmetic, so every computed logit is bit-identical
 // to the range off; the rows it does not compute keep the -inf of vocab_fill.  row_slot: see rep_fixup.
 static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cudaStream_t stream, const SplitK* pend = nullptr,
-                        int eos = -1, const int32_t* row_slot = nullptr) {
+                        int eos = -1, const int32_t* row_slot = nullptr, const SamplerParams* decay = nullptr) {
   const nt_lm_config& c = lm->cfg;
   const int V = c.vocab_size, nt = (V + 127) / 128;
   const VocabTiles vt = eos >= 0 ? vocab_tiles(lm, eos) : VocabTiles{false, 0, nt, -1};
@@ -475,7 +502,9 @@ static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cud
   }
   if (vt.eos_tile >= 0 && (rc = launch_vocab_eos_tile(logits, B, V, eos, tmax, nt, stream))) return rc;
   if ((rc = rep_fixup(lm, B, logits, tmax, eos, row_slot, stream))) return rc;
-  // no epilogue maxima: the raw maxima of the finished rows (after the EOS tile and the penalty), as the epilogue has them
+  if (decay && eos >= 0 && lm->step.len_decay && (rc = launch_len_decay(*decay, B, logits, tmax, nt, stream))) return rc;
+  // no epilogue maxima: the raw maxima of the finished rows (after the EOS tile, the penalty and the decay), as the
+  // epilogue has them
   if (eos >= 0 && !tmax) return launch_tile_max(logits, B, V, lm->tmax, stream);
   return NT_OK;
 }
@@ -631,6 +660,7 @@ extern "C" int nt_lm_prefill_slots(nt_lm* lm, const nt_lm_state* st, const int32
     seen[slots[i]] = 1;
     args[i] = slots[i], args[B + i] = stream_ids[i];
   }
+  if ((rc = check_length(lm, sp, slots, B))) return rc;
   std::vector<int> lens;
   int max_len = 0;
   if ((rc = prefill_stage(lm, cu, B, lens, max_len, stream))) return rc;
@@ -664,6 +694,7 @@ extern "C" int nt_lm_prefill_fork(nt_lm* lm, const nt_lm_state* st, const int32_
   int rc = check_sampling(lm, st, sp);
   if (rc) return rc;
   const int N = B * n, nc = N - B;
+  if ((rc = check_length(lm, sp, nullptr, N))) return rc;
   std::vector<int> lens;
   int max_len = 0;
   if ((rc = prefill_stage(lm, cu, B, lens, max_len, stream))) return rc;
@@ -824,9 +855,9 @@ static int decode_step(nt_lm* lm, const nt_lm_state* st, int B, const nt_samplin
   } else {
     if ((rc = layers_gemm(lm, st, B, B, 1, 0, stream, &tail))) return rc;
   }
-  if ((rc = lm_head_rows(lm, lm->h, B, lm->logits, stream, &tail, sp->eos_id))) return rc;
   SamplerParams s = make_sampler(lm, st, sp);
   s.advance = 1;
+  if ((rc = lm_head_rows(lm, lm->h, B, lm->logits, stream, &tail, sp->eos_id, nullptr, &s))) return rc;
   return run_sampler(lm, s, B, stream);
 }
 
@@ -839,6 +870,7 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
   if (B < 1 || B > c.max_batch) return set_error(NT_ERR_INVALID, "batch %d not in 1..%d", B, c.max_batch);
   int rc = check_sampling(lm, st, sp);
   if (rc) return rc;
+  if ((rc = check_length(lm, sp, nullptr, B))) return rc;
   if (n_steps < 0) return set_error(NT_ERR_INVALID, "negative step count");
 
   // NT_DECODE_IMPL = tc (persistent wgmma kernel) | perop (per-op kernel chain).  Unset: the persistent kernel up to
@@ -914,7 +946,8 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
     return NT_OK;
   }
   // The graph is keyed by every input decode_step bakes into its launches: the batch, the state and sampling params,
-  // and the host settings in lm->step.  The slot_sp / rep_tab contents stay out: the graph reads them at replay.
+  // and the host settings in lm->step.  The slot_sp / rep_tab / len_tab contents stay out: the graph reads them at
+  // replay.
   // prof / prof_step stay out: only the persistent kernel reads them, and it never runs from the graph.
   std::vector<uint8_t> key(sizeof(int) + sizeof(nt_lm_state) + sizeof(nt_sampling) + sizeof(StepSettings));
   uint8_t* k = key.data();
@@ -1007,6 +1040,49 @@ extern "C" int nt_lm_set_repetition_penalty(nt_lm* lm, const nt_slot_penalty* ta
     NT_CUDA_CHECK(cudaMemcpyAsync(lm->rep_tab, table, size_t(lm->cfg.max_batch) * sizeof(nt_slot_penalty), cudaMemcpyHostToDevice, stream));
   }
   lm->step.rep_on = on;
+  return NT_OK;
+}
+
+extern "C" int nt_lm_set_length_control(nt_lm* lm, const nt_slot_length* table, void* stream_) {
+  if (!lm) return set_error(NT_ERR_INVALID, "nt_lm_set_length_control: null handle");
+  const int S = lm->cfg.max_batch, K = lm->cfg.max_ctx;
+  const bool on = table != nullptr;
+  bool decays = false;
+  if (on) {
+    for (int s = 0; s < S; ++s) {
+      const nt_slot_length& e = table[s];
+      if (e.min_new_tokens < 0) return set_error(NT_ERR_INVALID, "slot %d: min_new_tokens %d must be >= 0", s, e.min_new_tokens);
+      if (!(std::isfinite(e.decay_factor) && e.decay_factor > 0.0))
+        return set_error(NT_ERR_INVALID, "slot %d: decay factor %g must be finite and > 0", s, e.decay_factor);
+      if (e.decay_start < 0) return set_error(NT_ERR_INVALID, "slot %d: decay start %d must be >= 0", s, e.decay_start);
+      // below min_new_tokens - 1 the decay would meet the mask's -inf, and -inf + inf is NaN
+      if (e.decay_start < e.min_new_tokens - 1)
+        return set_error(NT_ERR_INVALID, "slot %d: decay start %d must be >= min_new_tokens - 1 = %d", s, e.decay_start, e.min_new_tokens - 1);
+      decays = decays || e.decay_factor != 1.0;
+    }
+    // c_k as transformers computes it: pow(factor, k) - 1 in double, used as an fp32 scalar
+    std::vector<float> c(size_t(S) * K, 0.f);
+    std::vector<int> start(S), finite(S, K);
+    for (int s = 0; s < S; ++s) {
+      start[s] = table[s].decay_start;
+      if (table[s].decay_factor == 1.0) continue;
+      for (int k = 1; k <= K; ++k) {
+        const float v = static_cast<float>(std::pow(table[s].decay_factor, static_cast<double>(k)) - 1.0);
+        if (!std::isfinite(v)) {
+          finite[s] = k - 1;
+          break;
+        }
+        c[size_t(s) * K + k - 1] = v;
+      }
+    }
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    // pageable sources: the runtime has staged them by the time the calls return
+    NT_CUDA_CHECK(cudaMemcpyAsync(lm->len_tab, table, size_t(S) * sizeof(nt_slot_length), cudaMemcpyHostToDevice, stream));
+    NT_CUDA_CHECK(cudaMemcpyAsync(lm->len_c, c.data(), c.size() * sizeof(float), cudaMemcpyHostToDevice, stream));
+    lm->len_start = start, lm->len_finite = finite;
+  }
+  lm->step.len_on = on;
+  lm->step.len_decay = decays;
   return NT_OK;
 }
 

@@ -151,6 +151,7 @@ struct TcMisc {
   int mask_eos[kTcMaxBatch];
   float inv_t[kTcMaxBatch];   // 1 / temperature per sequence (the launch's sampling controls)
   float rep_pen[kTcMaxBatch]; // repetition penalty per sequence (1: none, or the slot is unrecorded)
+  float len_c[kTcMaxBatch];   // this step's EOS decay constant per sequence (0: none; length control)
   float red[64];
   float tile_max[2][4][kTcMaxBatch];
   float rstd[8];
@@ -746,6 +747,12 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
             }
           }
         }
+        // length control: the EOS decay after the penalty, before the store, the mask and 1 / T (one lane of one warp)
+        if (P.samp.len_tab && row == eos) {
+#pragma unroll
+          for (int n = 0; n < NTOK; ++n)
+            if (n < B && ms->len_c[n] != 0.f) v[n] = len_decay(v[n], ms->len_c[n]);
+        }
         float pv[NTOK];
 #pragma unroll
         for (int n = 0; n < NTOK; ++n) {
@@ -802,7 +809,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
       }
       if (tid < B) {
         ms->pos[tid] = __ldcg(P.kv.seq_lens + tid);
-        ms->mask_eos[tid] = __ldcg(P.samp.n_generated + tid) < P.samp.sp.min_new_tokens ? 1 : 0;
+        // n_generated was written by the previous step's sampler, before the grid barrier that follows it
+        const int ngen = __ldcg(P.samp.n_generated + tid);
+        ms->mask_eos[tid] = ngen < row_min_new(P.samp, tid) ? 1 : 0;
+        ms->len_c[tid] = len_decay_c(P.samp, tid, ngen);
       }
       csync();
       cache_pages();

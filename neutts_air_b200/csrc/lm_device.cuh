@@ -408,6 +408,19 @@ NT_DEVINL RowSampling row_sampling(const SamplerParams& p, int slot) {
 // reciprocal), so the result is bit-identical to torch's fp32 `score / penalty`; -inf stays -inf
 NT_DEVINL float rep_penalize(float s, float penalty) { return s < 0.f ? __fmul_rn(s, penalty) : __fdiv_rn(s, penalty); }
 
+// MinNewTokensLengthLogitsProcessor: EOS stays masked while the slot's n_generated is below this floor
+NT_DEVINL int row_min_new(const SamplerParams& p, int slot) { return p.len_tab ? p.len_tab[slot].min_new_tokens : p.sp.min_new_tokens; }
+
+// ExponentialDecayLengthPenalty: the constant c_k of the slot with n tokens generated (k = n - decay_start) while
+// n > decay_start, else 0 (the table holds 0 for every k of an entry without decay)
+NT_DEVINL float len_decay_c(const SamplerParams& p, int slot, int n) {
+  if (!p.len_tab) return 0.f;
+  const int k = n - p.len_tab[slot].decay_start;
+  return k > 0 && k <= p.len_pitch ? __ldg(p.len_c + static_cast<long long>(slot) * p.len_pitch + k - 1) : 0.f;
+}
+// transformers' `scores + |scores| * c` on the EOS score: the fp32 product, then the fp32 sum (no fused multiply-add)
+NT_DEVINL float len_decay(float s, float c) { return __fadd_rn(s, __fmul_rn(fabsf(s), c)); }
+
 // logits processors (MinNewTokensLength -> Temperature), then the order-preserving key
 NT_DEVINL uint32_t processed_key(float logit, int idx, bool mask_eos, int eos_id, float inv_t) {
   if (mask_eos && idx == eos_id) logit = -INFINITY;
@@ -485,7 +498,7 @@ NT_DEVINL void sample_finish(const SamplerParams& p, int b, int k, Cand* win, in
   const int s = slot >= 0 ? slot : b;
   float* ev = reinterpret_cast<float*>(win + kTopKeep);   // [kTopKeep] exp(score - max)
   const bool logprobs = p.logprob_out && !stateless && !is_done;   // CTA-uniform
-  const bool mask_eos = ngen < p.sp.min_new_tokens;
+  const bool mask_eos = ngen < row_min_new(p, s);
   const float* lg = p.logits + static_cast<long long>(src >= 0 ? src : b) * p.V;
   float lse = 0.f;
   if (logprobs) lse = row_logsumexp(lg, p.V, p.sp.eos_id, mask_eos, reinterpret_cast<float2*>(ev + kTopKeep), sync);

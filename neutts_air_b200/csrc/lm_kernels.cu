@@ -694,7 +694,7 @@ __global__ void __launch_bounds__(kConsumerThreads) topk_tiles_kernel(const Samp
   const int src = p.row_src ? __ldg(p.row_src + b) : -1;   // logits / tile-maxima row (-1: row b)
   const bool stateless = p.n_generated_override != nullptr;
   const int ngen = stateless ? __ldcg(p.n_generated_override + b) : __ldcg(p.n_generated + slot);
-  const bool mask_eos = ngen < p.sp.min_new_tokens;
+  const bool mask_eos = ngen < row_min_new(p, slot);
   const float inv_t = row_sampling(p, slot).inv_t;
   int fix_tile = -1;
   float fix_val = 0.f;
@@ -821,6 +821,29 @@ int launch_rep_penalty(float* logits, int B, int V, const uint32_t* hist, int wo
   constexpr int kRepSplit = 16;
   return launch_kernel(rep_penalty_kernel, dim3(B, kRepSplit), dim3(256), 0, s, true, logits, V, hist, words, tab, recorded, row_slot,
                        tmax, nt);
+}
+
+// =================================================================================== length control
+// grid B, 128 threads: thread r owns row (eos tile) * 128 + r of logits row b, which holds slot b.  The decay is read
+// from n_generated before this step's sampler advances it, so it is the n the sampler draws at.
+__global__ void len_decay_kernel(const SamplerParams p, float* logits, float* tmax, int nt) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x, eos = p.sp.eos_id, tile = eos >> 7, row = tile * 128 + threadIdx.x;
+  const float c = len_decay_c(p, b, __ldcg(p.n_generated + b));
+  if (c == 0.f) return;   // CTA-uniform: no decay for this slot at this step
+  float* lg = logits + static_cast<long long>(b) * p.V;
+  float v = row < p.V ? lg[row] : -INFINITY;
+  if (row == eos) lg[row] = v = len_decay(v, c);
+  if (!tmax) return;
+  __shared__ float red[4];
+  v = warp_max(v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x == 0) tmax[static_cast<long long>(b) * nt + tile] = fmaxf(fmaxf(red[0], red[1]), fmaxf(red[2], red[3]));
+}
+int launch_len_decay(const SamplerParams& p, int B, float* logits, float* tmax, int nt, cudaStream_t s) {
+  return launch_kernel(len_decay_kernel, dim3(B), dim3(128), 0, s, true, p, logits, tmax, nt);
 }
 
 // =================================================================================== prefill helpers

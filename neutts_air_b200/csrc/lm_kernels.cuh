@@ -110,6 +110,11 @@ struct SamplerParams {
   // off.  sample_finish sets the bit of every token it writes to out_tokens.
   uint32_t* rep_hist;
   int rep_words;
+  // length control (nt_lm_set_length_control): per-slot entries, nullptr = off (sp.min_new_tokens for every slot), and
+  // [max_batch][len_pitch] decay constants, entry k - 1 = c_k (all zero for an entry without decay)
+  const nt_slot_length* len_tab;
+  const float* len_c;
+  int len_pitch;
   // per-token log-probabilities (nt_lm_set_logprobs): [max_batch][max_new][2] (sampled, model), nullptr = off.
   // sample_finish writes the pair of every token it writes to out_tokens.
   float* logprob_out;
@@ -136,6 +141,10 @@ int launch_rep_history(uint32_t* hist, int words, const nt_slot_penalty* tab, in
                        const int32_t* ids, const int32_t* cu, int B, int V, cudaStream_t s);
 int launch_rep_penalty(float* logits, int B, int V, const uint32_t* hist, int words, const nt_slot_penalty* tab,
                        const int32_t* recorded, const int32_t* row_slot, float* tmax, int nt, cudaStream_t s);
+// Length control, decode steps only: logits row b [B][V] holds slot b; where the slot's decay is active at its
+// n_generated, the EOS logit becomes s + |s| c_k and the raw maximum of the EOS tile in tmax [B][nt] (optional) is
+// recomputed.  p supplies V, eos_id, n_generated and the length-control pointers.
+int launch_len_decay(const SamplerParams& p, int B, float* logits, float* tmax, int nt, cudaStream_t s);
 
 int launch_embed_rows(const __nv_bfloat16* embed, const int32_t* ids, int T, int hidden, float* h, cudaStream_t s);
 // parts != nullptr: x is updated in place first (x += sum of nparts split-K slices, slice order) -- see SplitK.

@@ -300,6 +300,73 @@ def per_prompt_penalty(n: int, penalty, include_prompt):
     return None if all(r[0] == 1.0 for r in rows) else rows
 
 
+DEFAULT_LENGTH = (50, 49, 1.0)   # min_new_tokens, decay start, decay factor: the reference's floor, no decay
+
+
+def _is_int(v) -> bool:
+    return not isinstance(v, (bool, np.bool_)) and isinstance(v, (int, np.integer))
+
+
+def check_length(min_new_tokens, decay_start, decay_factor, max_new: int | None = None) -> tuple:
+    """One slot's length control, validated as ``nt_lm_set_length_control`` does -> (int, int, float):
+    ``min_new_tokens`` >= 0 (transformers' MinNewTokensLengthLogitsProcessor), ``decay_start`` >= 0 and >=
+    min_new_tokens - 1 (the decay never meets the mask's -inf, which transformers would turn into NaN) and
+    ``decay_factor`` finite and > 0, 1 = no decay (ExponentialDecayLengthPenalty).  ``max_new``: also refuse a decay
+    whose c_k = pow(factor, k) - 1 is not finite in fp32 for some k <= max_new - decay_start, as every launch does."""
+    if not _is_int(min_new_tokens) or min_new_tokens < 0:
+        raise ValueError(f"min_new_tokens {min_new_tokens!r} must be an integer >= 0")
+    if not _is_int(decay_start) or decay_start < 0:
+        raise ValueError(f"exponential_decay_length_penalty start {decay_start!r} must be an integer >= 0")
+    if isinstance(decay_factor, bool) or not isinstance(decay_factor, (int, float, np.integer, np.floating)):
+        raise ValueError(f"exponential_decay_length_penalty factor {decay_factor!r} must be a number")
+    f = float(decay_factor)
+    if not (math.isfinite(f) and f > 0):
+        raise ValueError(f"exponential_decay_length_penalty factor {decay_factor} must be finite and > 0")
+    if decay_start < min_new_tokens - 1:
+        raise ValueError(f"exponential_decay_length_penalty start {decay_start} must be >= min_new_tokens - 1 = "
+                         f"{min_new_tokens - 1}: the decay would meet the -inf of the min_new_tokens mask")
+    k = (max_new or 0) - int(decay_start)
+    if f > 1 and k >= 1:   # c_k grows with k: the largest reachable one decides
+        try:
+            c = pow(f, k) - 1
+        except OverflowError:
+            c = math.inf
+        with np.errstate(over="ignore"):
+            if not math.isfinite(float(np.float32(c))):
+                raise ValueError(f"exponential_decay_length_penalty factor {f} overflows fp32 within {k} steps "
+                                 f"after its start (pow({f}, {k}) - 1)")
+    return int(min_new_tokens), int(decay_start), f
+
+
+def per_prompt_decay(n: int, decay) -> list:
+    """``exponential_decay_length_penalty`` of n prompts: None, one (start, factor) pair, or one None / pair per
+    prompt -> a list of n entries."""
+    pair = lambda d: isinstance(d, (list, tuple)) and len(d) == 2 and all(
+        isinstance(x, (int, float, np.integer, np.floating)) and not isinstance(x, bool) for x in d)
+    if decay is None or pair(decay):
+        return [decay] * n
+    if isinstance(decay, (list, tuple)) and len(decay) == n and all(d is None or pair(d) for d in decay):
+        return list(decay)
+    raise ValueError(f"exponential_decay_length_penalty must be None, one (start, factor) pair, or one of those per "
+                     f"prompt ({n}); got {decay!r}")
+
+
+def per_prompt_length(n: int, min_new_tokens, decay, max_new: int | None = None):
+    """Length control of n prompts: ``min_new_tokens`` an int or one per prompt, ``decay`` as ``per_prompt_decay``.
+    Returns None when ``min_new_tokens`` is one int and no prompt decays (the launch scalar then governs, exactly as without
+    the table), else one validated (min_new_tokens, decay_start, decay_factor) per prompt (``check_length``; a prompt
+    without decay gets factor 1 and start max(min_new_tokens - 1, 0))."""
+    floors = per_item(n, "prompt", min_new_tokens=min_new_tokens)["min_new_tokens"]
+    decays = per_prompt_decay(n, decay)
+    if not isinstance(floors, list):
+        check_length(floors, max(floors - 1, 0) if _is_int(floors) else 0, 1.0)
+        if all(d is None for d in decays):
+            return None
+        floors = [floors] * n
+    return [check_length(m, *(d if d is not None else (max(m - 1, 0) if _is_int(m) else 0, 1.0)), max_new=max_new)
+            for m, d in zip(floors, decays)]
+
+
 @dataclass
 class Settings:
     """The per-prompt generation settings of one call, resolved and validated before any engine call
@@ -311,10 +378,16 @@ class Settings:
     temperature: float         # the launch scalars, taken from the first row while the controls table is on (the
     top_k: int                 # sampler then reads every slot's own row)
     logprobs: bool = False     # per-token log-probabilities on (``SpeechLM.set_logprobs``)
+    length: list | None = None # one (min_new_tokens, decay_start, decay_factor) per prompt; None: the launch scalar
+    min_new_tokens: int = 50   # the launch scalar, row 0's while the length table is on
+
+    def floors(self, n: int) -> list:
+        """The min_new_tokens of each of the n prompts."""
+        return [r[0] for r in self.length] if self.length is not None else [self.min_new_tokens] * n
 
     def apply(self, lm, n: int) -> None:
         """Before a prefill of prompts 0..n-1 into slots 0..n-1, on its stream: controls, then range, then penalty, then
-        log-probabilities.  Each setting is applied, or switched off when an earlier call left it on, or makes no call when it is off and
+        length control, then log-probabilities.  Each setting is applied, or switched off when an earlier call left it on, or makes no call when it is off and
         stays off.  ``lm`` needs the ``set_*`` methods only when a call is due; a missing mirror counts as off."""
         if self.controls is not None or getattr(lm, "_slot_sp_host", None) is not None:
             lm.set_slot_sampling(None if self.controls is None else self.controls[:n])
@@ -324,6 +397,8 @@ class Settings:
             lm.set_vocab_range(None)
         if self.penalty is not None or getattr(lm, "_penalty_host", None) is not None:
             lm.set_repetition_penalty(None if self.penalty is None else self.penalty[:n])
+        if self.length is not None or getattr(lm, "_length_host", None) is not None:
+            lm.set_length_control(None if self.length is None else self.length[:n])
         if self.logprobs != (getattr(lm, "logprobs", None) is not None):
             lm.set_logprobs(self.logprobs)
 
@@ -331,7 +406,7 @@ class Settings:
         """The settings of n takes of every prompt: each prompt's row repeated n times, in slot order (take j of prompt
         i in slot i * n + j), so that ``apply`` writes it into all of the prompt's take slots."""
         rows = lambda r: None if r is None else [x for x in r for _ in range(n)]
-        return dataclasses.replace(self, controls=rows(self.controls), penalty=rows(self.penalty))
+        return dataclasses.replace(self, controls=rows(self.controls), penalty=rows(self.penalty), length=rows(self.length))
 
     def admit(self, lm, slots, idx) -> None:
         """Before a refill of prompts ``idx`` into ``slots``: writes their rows; every other slot keeps its own, and
@@ -340,19 +415,25 @@ class Settings:
             lm.set_slot_sampling([self.controls[i] for i in idx], slots=slots)
         if self.penalty is not None:
             lm.set_repetition_penalty([self.penalty[i] for i in idx], slots=slots)
+        if self.length is not None:
+            lm.set_length_control([self.length[i] for i in idx], slots=slots)
 
 
 def resolve_settings(lm, n: int, temperature=1.0, top_k=50, top_p=1.0, min_p=0.0, vocab_range=None,
-                     repetition_penalty=1.0, penalize_prompt=True, logprobs=False) -> Settings:
+                     repetition_penalty=1.0, penalize_prompt=True, logprobs=False, min_new_tokens=50,
+                     exponential_decay_length_penalty=None, max_new: int | None = None) -> Settings:
     """The settings of n prompts on engine ``lm``, each control a scalar or one value per prompt
-    (``per_prompt_controls``, ``per_prompt_penalty``, ``check_vocab_range``; ``lm.shape`` is read only for a range)."""
+    (``per_prompt_controls``, ``per_prompt_penalty``, ``per_prompt_length``, ``check_vocab_range``; ``lm.shape`` is
+    read only for a range).  ``max_new``: the call's largest generated-token cap, against which a decay is checked."""
     if vocab_range is not None:
         vocab_range = check_vocab_range(vocab_range, lm.shape.vocab_size)
     penalty = per_prompt_penalty(n, repetition_penalty, penalize_prompt)
+    length = per_prompt_length(n, min_new_tokens, exponential_decay_length_penalty, max_new)
     controls = per_prompt_controls(n, temperature, top_k, top_p, min_p)
     if controls:
         temperature, top_k = controls[0][0], controls[0][1]
-    return Settings(controls, penalty, vocab_range, temperature, top_k, bool(logprobs))
+    floor = length[0][0] if length else int(min_new_tokens)
+    return Settings(controls, penalty, vocab_range, temperature, top_k, bool(logprobs), length, floor)
 
 
 PLAN_PHASES = ("qkv", "o", "gu", "d")   # phase order of the persistent kernel's work plan
@@ -435,6 +516,7 @@ class SpeechLM:
         self._slot_sp_host = None   # host mirror of the per-slot sampling controls (None: off)
         self._vocab_range = None    # (lo, hi) while the vocabulary range is on
         self._penalty_host = None   # host mirror of the per-slot repetition penalties (None: off)
+        self._length_host = None    # host mirror of the per-slot length control (None: off)
         self.logprobs = None        # per-token log-probabilities, [max_batch][max_new][2] on the device (None: off)
 
     def __del__(self):
@@ -476,7 +558,7 @@ class SpeechLM:
                                DEFAULT_CONTROLS, rows, slots)
 
     def _write_slot_table(self, mirror: str, setter, entry, check, default, rows, slots) -> None:
-        """Behind ``set_slot_sampling`` / ``set_repetition_penalty``: validates ``rows`` (``check``) and ``slots``,
+        """Behind ``set_slot_sampling`` / ``set_repetition_penalty`` / ``set_length_control``: validates ``rows`` (``check``) and ``slots``,
         merges them into the host mirror (attribute ``mirror``; ``default`` fills a table that was off), and hands the
         whole table of ``entry`` structs to the C ``setter`` on the current stream.  ``rows=None``: the table goes off."""
         table = arr = None
@@ -518,6 +600,18 @@ class SpeechLM:
         so it is ordered before the next prefill or decode."""
         self._write_slot_table("_penalty_host", self.L.nt_lm_set_repetition_penalty, _lib.SlotPenalty, check_penalty,
                                DEFAULT_PENALTY, rows, slots)
+
+    def set_length_control(self, rows, slots=None) -> None:
+        """Per-slot length control (transformers' ``MinNewTokensLengthLogitsProcessor`` and
+        ``ExponentialDecayLengthPenalty``).  ``rows``: one (min_new_tokens, decay_start, decay_factor) per slot of
+        ``slots`` (default: slots 0..len(rows) - 1); every other slot keeps its entry, or (50, 49, 1.0) when the table
+        was off.  While on, a slot's min_new_tokens replaces ``sampling``'s, and once it has generated n > decay_start
+        tokens its EOS score s becomes s + |s| * (decay_factor ** (n - decay_start) - 1) before the vocabulary range,
+        the temperature and the warpers; greedy and teacher-forced runs see it too.  ``None`` switches the table off.
+        Rules: ``check_length``.  The table is copied on the current stream, so it is ordered before the next prefill
+        or decode."""
+        self._write_slot_table("_length_host", self.L.nt_lm_set_length_control, _lib.SlotLength, check_length,
+                               DEFAULT_LENGTH, rows, slots)
 
     def set_logprobs(self, on: bool = True):
         """Per-token log-probabilities.  While on, every later sampler launch writes, for each token it writes to
@@ -796,13 +890,14 @@ class SpeechLM:
         # max_length counts prompt + generated PER SEQUENCE (stopping_criteria.py:73-84): a long prompt in the batch
         # must not shorten its neighbours, so every slot gets its own cap and the loop runs to the largest one
         caps = self._caps(lens, max_length, max_new_tokens)
-        return caps, resolve_settings(self, len(prompts), **settings)
+        return caps, resolve_settings(self, len(prompts), max_new=max(caps, default=0), **settings)
 
     def generate_batch(self, prompts, eos_token_id: int, max_length: int | None = None, min_new_tokens: int = 50,
                        temperature: float = 1.0, top_k: int = 50, max_new_tokens: int | None = None, seed: int = 0,
                        greedy: bool = False, forced: torch.Tensor | None = None, check_every: int = 64, slot_base: int = 0,
                        top_p: float = 1.0, min_p: float = 0.0, vocab_range=None, repetition_penalty=1.0,
-                       penalize_prompt=True, return_logprobs: bool = False, num_return_sequences: int = 1):
+                       penalize_prompt=True, return_logprobs: bool = False, num_return_sequences: int = 1,
+                       exponential_decay_length_penalty=None):
         """Returns a list of int64 CPU tensors with the generated ids of each prompt (EOS included
         when it was sampled), following transformers' stopping rules (stopping_criteria.py:73-84,
         467-471): stop at EOS or when prompt + generated reaches max_length.  ``max_new_tokens`` may also be a
@@ -813,7 +908,9 @@ class SpeechLM:
         (``set_repetition_penalty``); they apply to greedy and teacher-forced runs too.  ``return_logprobs``: returns
         ``(ids, logprobs)`` instead, ``logprobs[i]`` a float32 CPU tensor [len(ids[i]), 2] of (sampled, model)
         log-probabilities per generated token (``set_logprobs``, switched on for the call and off by a later call
-        without it).  ``num_return_sequences`` n > 1: n takes of every prompt from one prefill (``prefill_fork``;
+        without it).  ``min_new_tokens`` is an int or one per prompt, and ``exponential_decay_length_penalty`` None,
+        transformers' (start, factor) or one None / pair per prompt (``set_length_control``): per-prompt floors or any
+        decay switch the per-slot table on for the call.  ``num_return_sequences`` n > 1: n takes of every prompt from one prefill (``prefill_fork``;
         len(prompts) * n <= max_batch), returned in slot order, take j of prompt i at index i * n + j, each drawing
         from the Philox stream the prompt repeated n times would give it; every per-prompt setting (and cap) applies
         to all n takes of its prompt, while ``forced`` has one row per take."""
@@ -821,12 +918,13 @@ class SpeechLM:
         caps, settings = self._prepare(prompts, max_length, max_new_tokens, temperature=temperature, top_k=top_k,
                                        top_p=top_p, min_p=min_p, vocab_range=vocab_range,
                                        repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt,
-                                       logprobs=return_logprobs)
+                                       logprobs=return_logprobs, min_new_tokens=min_new_tokens,
+                                       exponential_decay_length_penalty=exponential_decay_length_penalty)
         if n_takes > 1:
             caps = [c for c in caps for _ in range(n_takes)]
             settings = settings.repeat(n_takes)
         limit = max(caps)
-        sp = self.sampling(eos_token_id, min_new_tokens, limit, settings.top_k, settings.temperature, seed, greedy,
+        sp = self.sampling(eos_token_id, settings.min_new_tokens, limit, settings.top_k, settings.temperature, seed, greedy,
                            forced, limits=caps if min(caps) < limit else None, slot_base=slot_base)
         B = len(prompts) * n_takes
         settings.apply(self, B)
@@ -848,7 +946,8 @@ class SpeechLM:
                        temperature: float = 1.0, top_k: int = 50, max_new_tokens: int | None = None, seed: int = 0,
                        greedy: bool = False, check_every: int = 32, slot_base: int = 0, top_p: float = 1.0,
                        min_p: float = 0.0, vocab_range=None, repetition_penalty=1.0, penalize_prompt=True,
-                       return_logprobs: bool = False, num_return_sequences: int = 1):
+                       return_logprobs: bool = False, num_return_sequences: int = 1,
+                       exponential_decay_length_penalty=None):
         """Continuous batching over any number of prompts: ``generate_batch``'s results and stopping rules, but a slot
         whose sequence finished is refilled with the next waiting prompt while the other slots keep decoding.
 
@@ -864,7 +963,8 @@ class SpeechLM:
         ``generate_batch``: set once before the first prefill, it holds across every refill.  ``repetition_penalty`` and
         ``penalize_prompt`` as in ``generate_batch``; a newcomer's entry is written before its prefill.
         ``return_logprobs`` as in ``generate_batch``: a finished slot's rows are copied out with its tokens, before
-        the refill that reuses the slot.  One sequence per prompt: ``num_return_sequences`` > 1 raises ValueError
+        the refill that reuses the slot.  ``min_new_tokens`` and ``exponential_decay_length_penalty`` as in
+        ``generate_batch``; a newcomer's entry is written before its prefill.  One sequence per prompt: ``num_return_sequences`` > 1 raises ValueError
         (``generate_batch`` takes several per prompt)."""
         if num_return_sequences != 1:
             raise ValueError("generate_queue returns one sequence per prompt; use generate_batch(num_return_sequences=n) "
@@ -872,15 +972,16 @@ class SpeechLM:
         caps, settings = self._prepare(prompts, max_length, max_new_tokens, temperature=temperature, top_k=top_k,
                                        top_p=top_p, min_p=min_p, vocab_range=vocab_range,
                                        repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt,
-                                       logprobs=return_logprobs)
+                                       logprobs=return_logprobs, min_new_tokens=min_new_tokens,
+                                       exponential_decay_length_penalty=exponential_decay_length_penalty)
         n = len(prompts)
         if n == 0:
             return ([], []) if return_logprobs else []
         if check_every < 1:
             raise ValueError("check_every must be >= 1")
         S = min(n, self.max_batch)
-        sp = self.sampling(eos_token_id, min_new_tokens, max(caps), settings.top_k, settings.temperature, seed, greedy,
-                           limits=caps[:S], slot_base=slot_base)
+        sp = self.sampling(eos_token_id, settings.min_new_tokens, max(caps), settings.top_k, settings.temperature, seed,
+                           greedy, limits=caps[:S], slot_base=slot_base)
         settings.apply(self, S)
         self.prefill([prompts[i] for i in range(S)], sp)
         occ = list(range(S))   # prompt held by each slot, None once harvested
@@ -889,7 +990,8 @@ class SpeechLM:
         out = [None] * n
         out_lp = [None] * n
         # a sequence can finish inside its prefill: a cap of 1, or EOS when it is not masked at step 0
-        at_prefill = lambda idx: min_new_tokens <= 0 or min(caps[i] for i in idx) <= 1
+        floors = settings.floors(n)
+        at_prefill = lambda idx: min(floors[i] for i in idx) <= 0 or min(caps[i] for i in idx) <= 1
         read = at_prefill(range(S))
         while True:
             if read:
@@ -929,11 +1031,12 @@ class SpeechLM:
                  do_sample: bool = True, temperature: float = 1.0, top_k: int = 50, use_cache: bool = True,
                  min_new_tokens: int = 0, max_new_tokens: int | None = None, seed: int | None = None,
                  top_p: float = 1.0, min_p: float = 0.0, vocab_range=None, repetition_penalty: float = 1.0,
-                 num_return_sequences: int = 1, **_):
+                 num_return_sequences: int = 1, exponential_decay_length_penalty=None, **_):
         """transformers-compatible seam used by ``NeuTTS._infer_torch`` (neutts/neutts.py:338-347).  ``top_p`` and
         ``min_p`` act as transformers' TopPLogitsWarper / MinPLogitsWarper; ``vocab_range`` (lo, hi) suppresses every
         id outside [lo, hi) and EOS (``set_vocab_range``); ``repetition_penalty`` acts as transformers'
-        RepetitionPenaltyLogitsProcessor (prompt included); ``num_return_sequences`` n returns n takes of every prompt
+        RepetitionPenaltyLogitsProcessor (prompt included); ``exponential_decay_length_penalty`` (start, factor) acts as
+        transformers' ExponentialDecayLengthPenalty (``set_length_control``); ``num_return_sequences`` n returns n takes of every prompt
         from one prefill, [B * n, P + gen] with take j of row b at row b * n + j, as transformers; other generation
         kwargs are ignored."""
         if eos_token_id is None:
@@ -950,6 +1053,8 @@ class SpeechLM:
             cuts["repetition_penalty"] = repetition_penalty
         if num_return_sequences != 1:
             cuts["num_return_sequences"] = num_return_sequences
+        if exponential_decay_length_penalty is not None:
+            cuts["exponential_decay_length_penalty"] = tuple(exponential_decay_length_penalty)
         outs = self.generate_batch(prompts, eos_token_id, max_length, min_new_tokens, temperature, top_k,
                                    max_new_tokens, seed, greedy=not do_sample, **cuts)
         n = max(len(o) for o in outs)
