@@ -324,7 +324,8 @@ int nt_lm_debug_capture_sampler(nt_lm* lm, float* topk_val, int32_t* topk_idx, i
  * whole-K (flat = 0) or flat (flat = 1) gate/up, and makes no CUDA call.  Outputs (each may be NULL):
  * items int16 [n_sms][4][4][4]: per CTA, phase (0 qkv, 1 o_proj, 2 gate/up, 3 down_proj) and item (tile, first k-block,
  * k-blocks, slice), a k-block being 64 elements of K; counts int32 [n_sms][4]: items per phase; flags int32 [n_sms][3]:
- * fold_q, fold_g, gu_split; gu_nsl uint8 [gu_cap]: K slices of every gate/up tile (flat plan); info int32 [7]: K slices
+ * fold_q, fold_g (1 on the first CTA that consumes the ln1 / ln2 fold, i.e. has qkv / gate-up items), gu_split;
+ * gu_nsl uint8 [gu_cap]: K slices of every gate/up tile (flat plan); info int32 [7]: K slices
  * of the qkv, o_proj and down_proj phases, most slices of a gate/up tile, lm_head tiles, most k-blocks a CTA stages in
  * one phase, gu_split.  NT_ERR_INVALID with a message when the plan does not fit the kernel. */
 int nt_debug_decode_plan(int hidden, int inter, int n_heads, int n_kv, int vocab, int n_sms, int flat, int16_t* items,

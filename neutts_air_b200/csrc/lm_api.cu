@@ -104,7 +104,7 @@ struct nt_lm {
   __nv_bfloat16 *xn, *attn_bf16, *act_bf16;
   // persistent decode kernel tables (device)
   const float** ptr_tab;   // [3][n_layers]: ln1, bqkv, ln2
-  unsigned* gbar;          // grid barrier counters
+  unsigned* gbar;          // grid barrier counter (word 0) and the batch-1 tile arrival counters (words kTcCntOff..)
   // cached decode-step graph
   cudaGraphExec_t graph = nullptr;
   std::vector<uint8_t> graph_key;
@@ -925,6 +925,7 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
     P.samp.advance = 1;
     P.rep_tab = lm->step.rep_on ? lm->rep_tab : nullptr, P.rep_rec = lm->rep_rec;
     P.gbar = lm->gbar;
+    P.tile_cnt = lm->gbar + kTcCntOff;
     P.n_steps = n_steps;
     P.logits_out = logits_out;
     P.logits_step_stride = static_cast<long long>(B) * c.vocab_size;
@@ -1128,6 +1129,12 @@ extern "C" int nt_debug_decode_plan(int hidden, int inter, int n_heads, int n_kv
   TcPlanInfo pi = {};
   const int rc = tc_build_plan(ts, n_sms, flat != 0, plan.data(), flat ? nsl.data() : nullptr, &pi);
   if (rc) return rc;
+  // the first CTA that consumes the ln1 fold (has qkv items) and the ln2 fold (has gate/up items)
+  int first_q = -1, first_g = -1;
+  for (int c = n_sms - 1; c >= 0; --c) {
+    if (plan[c].n[0] > 0) first_q = c;   // phase 0: qkv
+    if (plan[c].n[2] > 0) first_g = c;   // phase 2: gate/up
+  }
   for (int c = 0; c < n_sms; ++c) {
     for (int ph = 0; ph < 4; ++ph) {
       if (counts) counts[4 * c + ph] = plan[c].n[ph];
@@ -1137,7 +1144,7 @@ extern "C" int nt_debug_decode_plan(int hidden, int inter, int n_heads, int n_kv
         o[0] = it.tile, o[1] = it.kb0, o[2] = it.nkb, o[3] = it.slice;
       }
     }
-    if (flags) flags[3 * c] = plan[c].fold_q, flags[3 * c + 1] = plan[c].fold_g, flags[3 * c + 2] = plan[c].gu_split;
+    if (flags) flags[3 * c] = c == first_q, flags[3 * c + 1] = c == first_g, flags[3 * c + 2] = plan[c].gu_split;
   }
   if (flat && gu_nsl) memcpy(gu_nsl, nsl.data(), nsl.size());
   if (info) {

@@ -18,9 +18,10 @@
 //   Phases of a layer (grid barrier between them):
 //       [fold+RMSNorm] qkv -> RoPE/KV-append + split-KV attention -> merge + o_proj -> [fold+RMSNorm] gate/up+SwiGLU
 //       -> down
-//     batch <= 4: the consumers fold the split-K slices and normalise while staging their B operand (5 barriers per
-//     layer); larger batches: token-owner CTAs fold + normalise into bf16 rows that the consumers fetch by TMA
-//     (7 barriers per layer, no per-CTA re-reading of the whole batch).
+//     batch 1: no grid barrier inside a layer; the last producer of each o_proj / down_proj row tile folds it into the
+//     residual stream, and the consumers normalise that row while staging their B operand; larger batches:
+//     token-owner CTAs fold + normalise into bf16 rows that the consumers fetch by TMA (3 barriers per layer, no
+//     per-CTA re-reading of the whole batch).
 //   lm_head epilogue: logits -> HBM once, plus the processed maximum of every 128-row tile; the sampler then needs
 //   only the top_k tiles with the largest maxima (provably a superset of the top-k logits), so selection costs
 //   ~10 us on one CTA per sequence instead of a pass over the vocabulary.
@@ -44,6 +45,13 @@ NT_DEVINL unsigned tc_ld_acquire(const unsigned* p) {
   unsigned v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
+}
+// arrival at a self-resetting counter: returns the old value, stores old + 1, or 0 when old == last.  Relaxed: it
+// only elects a CTA, the data it then reads carry their own stamps.
+NT_DEVINL unsigned tc_arrive_inc(unsigned* p, unsigned last) {
+  unsigned old;
+  asm volatile("atom.relaxed.gpu.global.inc.u32 %0, [%1], %2;" : "=r"(old) : "l"(p), "r"(last) : "memory");
+  return old;
 }
 NT_DEVINL long long tc_ns() {
   long long t;
@@ -156,6 +164,7 @@ struct TcMisc {
   float tile_max[2][4][kTcMaxBatch];
   float rstd[8];
   int sel[8];
+  int tile_last[2];       // batch 1: this CTA arrived last at the split-K tile it just stored (epilogue warps)
   int bchunks[4];         // B-operand chunks of this CTA's items per split phase
   int ckb[4][16];         // k-block staged in chunk c (qkv / down: k-block of the input; o_proj: head)
   TcPlan plan;
@@ -253,7 +262,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     auto pm = [&](int id) { if (tid == 0 && prof.fine) prof.mark(id); };
     const int n_rep = P.n_heads / P.n_kv;
     const int split_cap = P.split_cap;
-    constexpr bool fold_cta = FOLD;   // batch <= 4: consumers fold the split-K slices themselves (no fold phases, no barriers)
+    constexpr bool fold_cta = FOLD;   // batch 1: split-K tiles folded by their last producer (no fold phases, no barriers)
     const int I = P.inter;
     const int AW = P.att_warps;
     uint8_t* att = smem + P.att_off;
@@ -265,7 +274,22 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     float* att_knew = att_q + 8 * 64;
     float* att_vnew = att_knew + 64;
     const bool att_separate = P.att_off != P.uni_off;   // dedicated staging: KV pages are fetched ahead of the phase
-    int fold_no = 0;   // fold_in_cta: folds done in this launch (ping-pong parity + stamp of the residual stream)
+    // fold_in_cta: folds done in this launch.  Residual version n (stamp hstamp_base + n, buffer n & 1 of the h2
+    // ping-pong) is what fold n normalises: the sampler's row (or the prefill's, n = 0; copy 0 only, read behind a grid
+    // barrier) for the first fold of a step, else the previous one plus the o_proj or down_proj slices, written tile by
+    // tile by their last producers into all kTcH2Copies copies.
+    // Why two buffers suffice: writing version n over version n - 2 (rows of one tile t) needs every reader of
+    // version n - 2 to be done with it.  They are
+    //   * the last producer of tile t for version n - 1: it read those rows into the value it wrote for n - 1, and the
+    //     writer of n polls version n - 1 of tile t before it writes;
+    //   * the consumers of fold n - 2, which read the whole row.  A consumer has items in the GEMM that follows its
+    //     fold and runs them after the read.  Version n - 1 of tile t needs the slices of every item of that GEMM:
+    //     gate/up items feed down_proj k-blocks, and every down tile's slices cover all of them; qkv items feed the
+    //     attention of every split (q rows) or of the appending split (k/v rows; split 0 reads them when no split
+    //     appends), and every o_proj tile's slices cover all heads and merge all their splits.  The writer of n polls
+    //     version n - 1 of tile t, so it comes after every such read.
+    //   After the final norm the sampler writes the next version behind a grid barrier.
+    int fold_no = 0;
 
     // ---- grid barrier; `post` runs on thread 0 between the release and the trailing CTA barrier
     auto grid_sync = [&](auto post) {   // post runs on the whole of warp 0 (it issues TMA under elect_one())
@@ -334,6 +358,66 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
       }
     };
 
+    // ---- batch 1, o_proj and down_proj: the CTA that stores the last of a row tile's S slices folds the tile into
+    //      the residual stream (epilogue warps; lane = row of the tile).  It reads residual version fold_no - 1 and the
+    //      S slices and adds them in the order every consumer used to: acc = residual, then slice 0 .. S - 1, plus the
+    //      zero padding of tc_fold4's batches of eight -- the same fp32 additions, so the same bits.  The result is
+    //      residual version fold_no, which the consumers of fold fold_no poll (one pair per element, tc_fold4 with no
+    //      slices).  It is stored kTcH2Copies times: with one copy every CTA of the grid polled the same 7 KB, and on
+    //      H100 that hot spot cost more than the L2 traffic the fold saves (bench.py measured 885-895 us per step with
+    //      one copy, 825-836 us with four).
+    //      The counter only elects the last arriver (S arrivals per tile and layer; it wraps to 0 on the last one, and
+    //      the next layer's arrivals all depend on this fold).  Every value read is a (value, stamp) pair polled until
+    //      its stamp matches, so the arrival needs no release/acquire: a slice whose store is not yet visible to the
+    //      elected CTA is simply polled again.  Each lane issues its loads before the election returns, so the
+    //      arrival's round trip and the reads overlap; the other S - 1 producers drop what they loaded.
+    uint32_t tf_n = 0;   // tile_fold calls (parity of ms->tile_last)
+    auto tile_fold = [&](const float2* part, int S, int stamp, unsigned* cnt, int tile) {
+      int* last = &ms->tile_last[tf_n++ & 1];   // two slots: a lane still reading one never sees the next election
+      if (tid == 0) *last = tc_arrive_inc(cnt, static_cast<unsigned>(S - 1)) == static_cast<unsigned>(S - 1);
+      const int row = tile * 128 + warp * 32 + lane;
+      const bool in = row < H;
+      const int hstamp = P.hstamp_base + fold_no;
+      const float2* hsrc = P.h2 + static_cast<long long>((fold_no - 1) & 1) * kTcH2Copies * H + row;
+      const float2* psrc = part + row;
+      const float pad = __int_as_float(stamp);
+      float2 r = in ? ldp1(hsrc) : make_float2(0.f, __int_as_float(hstamp - 1));
+      float2 t[kTcMaxSlices];
+#pragma unroll
+      for (int j = 0; j < kTcMaxSlices; ++j) t[j] = in && j < S ? ldp1(psrc + static_cast<long long>(j) * H) : make_float2(0.f, pad);
+      bar_epi();
+      if (!*last) return;
+      pm(11);
+      uint32_t spins = 0;
+      while (__float_as_int(r.y) != hstamp - 1) {
+        tc_spin_check(spins, "the residual stream");
+        r = ldp1(hsrc);
+      }
+      spins = 0;
+      for (;;) {
+        bool ok = true;
+#pragma unroll
+        for (int j = 0; j < kTcMaxSlices; ++j) ok = ok && __float_as_int(t[j].y) == stamp;
+        if (ok) break;
+        tc_spin_check(spins, "split-K slices");
+#pragma unroll
+        for (int j = 0; j < kTcMaxSlices; ++j)
+          if (in && j < S && __float_as_int(t[j].y) != stamp) t[j] = ldp1(psrc + static_cast<long long>(j) * H);
+      }
+      // tc_fold4's order: slices in batches of eight, the last batch padded with zeros
+      const int nadd = (S + 7) & ~7;
+      float acc = r.x;
+#pragma unroll
+      for (int j = 0; j < kTcMaxSlices; ++j)
+        if (j < nadd) acc += t[j].x;
+      if (in) {
+        float2* dst = P.h2 + static_cast<long long>(fold_no & 1) * kTcH2Copies * H + row;
+#pragma unroll
+        for (int c = 0; c < kTcH2Copies; ++c) dst[static_cast<long long>(c) * H] = make_float2(acc, __int_as_float(hstamp));
+      }
+      pm(12);
+    };
+
     // ---- epilogue of the split-K phases: raw partial sums as (value, stamp) pairs, one row per lane
     auto epi_partials = [&](int ph, float2* part, int rows, int stamp) {
       if (warp >= 4) return;
@@ -349,6 +433,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
 #pragma unroll
           for (int n = 0; n < NTOK; ++n)
             if (n < B) dst[static_cast<long long>(n) * rows] = make_float2(v[n], sf);
+        }
+        if constexpr (FOLD) {
+          if (ph == kPhO || ph == kPhD)
+            tile_fold(part, ph == kPhO ? P.so : P.sd, stamp, P.tile_cnt + (ph == kPhD ? kTcMaxTiles : 0) + it.tile, it.tile);
         }
       }
     };
@@ -393,12 +481,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
       }
     };
 
-    // ---- batch 1: fold the row in this CTA (residual pairs + slices, slice order), normalise, stage the B chunks of
-    //      phase `ph` (-1: every k-block).  Thread q < H / 4 keeps elements 4q .. 4q + 3 in registers from the fold to
-    //      the staging and the write-back, so no fp32 copy of the row takes shared memory away from the weight ring.
-    //      The designated CTA publishes the folded stream for the next fold.
-    auto fold_stage = [&](const float2* parts, int nparts, int pstamp, int rows, const float* norm_w, int ph, bool writer) {
-      const float2* hsrc = P.h2 + static_cast<long long>(fold_no & 1) * H;
+    // ---- batch 1: read residual version fold_no (folded by the last producers of its row tiles, see tile_fold),
+    //      normalise, stage the B chunks of phase `ph` (-1: every k-block).  Thread q < H / 4 keeps elements
+    //      4q .. 4q + 3 in registers from the read to the staging, so no fp32 copy of the row takes shared memory away
+    //      from the weight ring.
+    auto fold_stage = [&](const float* norm_w, int ph, bool copies) {
+      // copy blockIdx % kTcH2Copies of a tile-folded version: the grid's polls spread over four times the L2 lines
+      const float2* hsrc = P.h2 + (static_cast<long long>(fold_no & 1) * kTcH2Copies + (copies ? blockIdx.x % kTcH2Copies : 0)) * H;
       const int hstamp = P.hstamp_base + fold_no;
       const int i4 = tid * 4;
       const bool mine = i4 < H;   // H <= 4 * kConsumerThreads (tc_fold_in_cta)
@@ -407,7 +496,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
       float4 nw = make_float4(0.f, 0.f, 0.f, 0.f);
       if (mine) {
         nw = __ldg(reinterpret_cast<const float4*>(norm_w + i4));   // in flight together with the slices
-        tc_fold4(hsrc, hstamp, parts, nparts, pstamp, rows, B, H, 0, i4, acc);
+        tc_fold4(hsrc, hstamp, nullptr, 0, 0, H, B, H, 0, i4, acc);
       }
       pm(2);
       const float ss = warp_sum((acc[0] * acc[0] + acc[1] * acc[1]) + (acc[2] * acc[2] + acc[3] * acc[3]));
@@ -440,12 +529,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
       pm(4);
       bop_ready();
       pm(5);
-      if (writer && mine) {
-        float4* d = reinterpret_cast<float4*>(P.h2 + static_cast<long long>((fold_no + 1) & 1) * H + i4);
-        const float sf = __int_as_float(hstamp + 1);
-        d[0] = make_float4(acc[0], sf, acc[1], sf);
-        d[1] = make_float4(acc[2], sf, acc[3], sf);
-      }
       ++fold_no;
     };
 
@@ -496,6 +579,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
       const int b = my_b, kvh = my_kvh;
       const int p0 = my_split * geo.pps, p1 = min(p0 + geo.pps, geo.npages);
       const bool appends = pos < P.kv.max_ctx && (pos >> 6) >= p0 && (pos >> 6) < p1;
+      // in-CTA fold: every qkv slice must be read by some split, or the h2 ping-pong loses its ordering (see fold_no)
+      const bool kv_rows = appends || (FOLD && pos >= P.kv.max_ctx && my_split == 0);
       if (!att_separate) {
         // the pages do not depend on this layer's projections (the new row is patched in below): fetch the first round now
         csync();   // the union region is ours (previous phase of this CTA is through with it)
@@ -514,7 +599,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
         if (which == 0) row0 = (kvh * n_rep + (idx >> 5)) * 64 + 2 * i;
         else if (which == 1) row0 = (P.n_heads + kvh) * 64 + 2 * i;
         else row0 = (P.n_heads + P.n_kv + kvh) * 64 + 2 * i;
-        if (which != 0 && !appends) continue;
+        if (which != 0 && !kv_rows) continue;
         const float2 bia = __ldg(reinterpret_cast<const float2*>(bias + row0));
         // ahead of the wait for the slices, which hides its latency
         const float2 sc = which != 2 ? rope_sincos(pos, __ldg(P.inv_freq + i)) : make_float2(0.f, 1.f);
@@ -782,7 +867,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     auto sample_phase = [&] {
       const int b = blockIdx.x;
       if (b >= B) return;
-      float2* h2dst = fold_cta ? P.h2 + (static_cast<long long>(fold_no & 1) * B + b) * H : nullptr;
+      float2* h2dst = fold_cta ? P.h2 + static_cast<long long>(fold_no & 1) * kTcH2Copies * H : nullptr;   // copy 0 (B = 1)
       const float h2stamp = __int_as_float(P.hstamp_base + fold_no);
       // the epilogue stored PROCESSED maxima (temperature, EOS mask): no scale, no tile to fix up
       sample_tiles_seq(P.samp, b, P.tmax, P.ntiles, 1.0f, -1, 0.f, P.logits, P.vocab, ms->mask_eos[b] != 0, uni, P.uni_bytes, ms->sel,
@@ -828,26 +913,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
           const bool second = (hl & 1) != 0, head = hl == 2 * L;
           const int st = stamp_of(step, l);
           prof.fine = prof.buf != nullptr && l == 2;
-          // fold (residual + split-K slices of the previous GEMM) + RMSNorm + B-operand staging
-          const float2* parts = second ? P.po2 : P.pd2;
-          const int nparts = second ? P.so : (l > 0 ? P.sd : 0);
-          const int pstamp = second ? st : stamp_of(step, l - 1);
+          // RMSNorm of the residual stream (already folded by the previous GEMM's last producers) + B-operand staging
           const float* norm_w = head ? P.final_norm : (second ? P.ln2[l] : P.ln1[l]);
           const int sph = head ? -1 : (second ? (plan.gu_split ? kPhG : -1) : kPhQ);
-          const bool writer = !head && (second ? plan.fold_g != 0 : plan.fold_q != 0);
           const bool need = head ? n_head_tiles > 0 : plan.n[second ? kPhG : kPhQ] > 0;
           if (!second && !head) attn_prefetch(l);
-          if (need) fold_stage(parts, nparts, pstamp, H, norm_w, sph, writer);
+          if (need) fold_stage(norm_w, sph, hl > 0);
           else ++fold_no;
           if (head) break;
-          if (second && !plan.gu_split) {
-            epi_swiglu(st);
-            if (tid == 0) prof.mark(103);
-            if (plan.n[kPhD] > 0) stage_act(st);
-            epi_partials(kPhD, P.pd2, H, st);
-            if (tid == 0) prof.mark(104);
-            continue;
-          }
           for (int e = 0; e < 2; ++e) {   // the two GEMMs of the half-layer: qkv | o_proj, or gate/up | down
             if (e == 1) {
               if (!second) {
@@ -861,7 +934,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
             const int ph = (second ? kPhG : kPhQ) + e;   // kPhQ, kPhO | kPhG, kPhD
             float2* part = ph == kPhQ ? P.pq2 : (ph == kPhO ? P.po2 : (ph == kPhG ? P.pg2 : P.pd2));
             const int rows = ph == kPhQ ? P.qkv_n : (ph == kPhG ? 2 * I : H);
-            epi_partials(ph, part, rows, st);
+            // one call site each: the down epilogue (with its tile fold) is inlined once
+            if (ph == kPhG && !plan.gu_split) epi_swiglu(st);   // whole-K gate/up: SwiGLU in the epilogue
+            else epi_partials(ph, part, rows, st);
             if (tid == 0) prof.mark(100 + ph + (ph > 0 ? 1 : 0));   // 100 qkv, 102 o_proj, 103 gate/up, 104 down
           }
         }
@@ -1057,8 +1132,8 @@ static size_t tc_chunk_bytes(int nt) { return size_t(14) * nt * 128; }   // the 
 static size_t tc_attn_bytes(int aw) { return (tc_attn_layout_bytes(aw) + 1023) & ~size_t(1023); }
 
 bool tc_fold_in_cta(int B, int hidden) {
-  // Every consumer re-folds ALL rows in the in-CTA fold, so its cost grows with the batch while the fold phases' is
-  // flat: the in-CTA fold runs at batch 1 only.
+  // The in-CTA fold (tile_fold, fold_stage) handles one token row: every consumer reads the whole row, a cost that
+  // would grow with the batch while the fold phases' is flat.  It runs at batch 1 only.
   return B == 1 && size_t(hidden) * 4 <= 16 * 1024 && hidden <= 1024;
 }
 
@@ -1135,7 +1210,6 @@ int tc_build_plan(const TcShape& s, int G, bool flat, TcPlan* plan, unsigned cha
   if (!split_phase(kPhQ, Tq, KBh, &info->sq) || !split_phase(kPhO, To, KBo, &info->so) || !split_phase(kPhD, To, KBi, &info->sd))
     return set_error(NT_ERR_INVALID, "decode_tc: too many split-K items per CTA");
   int worst = 0;
-  bool fq = false, fg = false;
   for (int c = 0; c < G; ++c) {
     for (int ph = 0; ph < 4; ++ph) {
       if (ph == kPhG && !flat) continue;
@@ -1143,8 +1217,6 @@ int tc_build_plan(const TcShape& s, int G, bool flat, TcPlan* plan, unsigned cha
       for (int i = 0; i < plan[c].n[ph]; ++i) chunks += plan[c].it[ph][i].nkb;
       if (chunks > worst) worst = chunks;
     }
-    if (!fq && plan[c].n[kPhQ] > 0) plan[c].fold_q = 1, fq = true;
-    if (!fg && plan[c].n[kPhG] > 0) plan[c].fold_g = 1, fg = true;
   }
   if (worst > 14) return set_error(NT_ERR_INVALID, "decode_tc: %d k-blocks per CTA exceed the staging area", worst);
   info->max_chunks = worst;

@@ -17,6 +17,9 @@ constexpr int kTcMaxBatch = 64;
 constexpr int kTcDefaultMaxBatch = 16;  // nt_lm_decode's default: larger batches take the per-op chain
 constexpr int kTcMaxSlices = 16;
 constexpr int kTcMaxGuSlices = 4;   // K slices of one gate/up tile in the flat plan (batch <= 4)
+constexpr int kTcMaxTiles = 8;      // row tiles of a hidden-sized output (hidden <= 1024)
+constexpr int kTcCntOff = 32;
+constexpr int kTcH2Copies = 4;      // batch 1: copies of each tile-folded residual version in the h2 buffers       // the tile counters sit at words [32, 32 + 2 kTcMaxTiles) of the grid barrier block
 
 // One GEMM work item: rows [tile*128, tile*128+128) of a weight matrix times k-blocks [kb0, kb0+nkb) of the
 // activations (a k-block = 64 elements = one 128-byte swizzle row).  Items of the split-K phases (qkv, o, down)
@@ -33,7 +36,6 @@ struct TcPlan {
   int n[4];                       // items per phase: 0 = qkv, 1 = o_proj, 2 = gate/up, 3 = down
   TcItem it[4][kTcMaxItems];
   int head_t0, head_t1;           // positions [t0, t1) of the lm_head tile list (filled by the kernel)
-  int fold_q, fold_g;             // batch <= 4: this CTA writes the folded residual stream back (one CTA per fold point)
   int gu_split;                   // 1: gate/up items carry their own K range and write raw partial sums (flat plan)
 };
 
@@ -70,7 +72,8 @@ struct TcParams {
   float2* act2;                   // batch <= 4, whole-K gate/up: SwiGLU output [B][inter] (fp32 value, stamp)
   float2* pg2;                    // batch <= 4, flat plan: gate/up partial sums [slice][B][2 * inter]
   const unsigned char* gu_nsl;    // flat plan: K slices of every gate/up tile (device, [tiles])
-  float2* h2;                     // batch <= 4: residual stream, ping-pong [2][B][hidden]
+  float2* h2;                     // batch 1: residual stream, ping-pong [2][kTcH2Copies][hidden]
+  unsigned* tile_cnt;             // batch 1: arrival counters of the o_proj [0, kTcMaxTiles) and down_proj row tiles
   int stamp_base, hstamp_base;    // stamps of this launch lie above these (host counters)
   int max_splits, split_cap;
   KVLayout kv;
