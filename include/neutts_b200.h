@@ -396,6 +396,52 @@ int nt_codec_debug_set_stages(nt_codec* c, int first, int last);
 void* nt_codec_debug_ptr(nt_codec* c, const char* name);
 
 /* ------------------------------------------------------------------------------------------
+ * Output resampler: 24 kHz PCM -> sample_rate, optionally as 16-bit PCM, for whole rows and for streams
+ * ------------------------------------------------------------------------------------------
+ * Semantics of torchaudio.functional.resample(x, 24000, sample_rate) with its defaults (sinc_interp_hann,
+ * lowpass_filter_width 6, rolloff 0.99).  With g = gcd(24000, sample_rate), orig = 24000 / g, target = sample_rate / g:
+ * width = ceil(6 * orig / (0.99 * min(orig, target))), taps = 2 * width + orig, and output sample k * target + p is
+ * the dot product of phase p of the filter table with x_pad[k * orig .. k * orig + taps), x_pad being x with `width`
+ * zeros in front and width + orig zeros behind; a row of L samples gives ceil(target * L / orig) samples.  At 24000 there
+ * is no filter (width 0, one tap of 1.0).  The table is computed in float64 and rounded once to fp32; outputs accumulate
+ * in fp32 over the taps in ascending order.  Rates whose fp32 table (target x taps) exceeds 227 KB, the shared memory
+ * an sm_90 block can opt into, are rejected.
+ * Streams: after L samples of a row have arrived, output frame k (samples k * target .. k * target + target - 1) is final
+ * once k * orig + width + orig <= L.  A push emits exactly the frames that became final and keeps the samples the first
+ * frame not yet final reads (fewer than taps); a final push pads with zeros, emits the rest, so a row's total is
+ * ceil(target * L / orig), and leaves the row reset.  Every output is bit-identical however its row was split into pushes.
+ * 16-bit PCM (NT_PCM_S16): each output y becomes __float2int_rn(fminf(fmaxf(y, -1), 1) * 32767) in fp32: clipped to
+ * [-32767, 32767], rounded half to even. */
+typedef enum { NT_PCM_F32 = 0, NT_PCM_S16 = 1 } nt_pcm_format;
+
+typedef struct {
+  int32_t orig, target;     /* 24000 / g, sample_rate / g */
+  int32_t width, taps;
+  size_t table_bytes;       /* device bytes of the filter table (16-byte aligned) */
+  size_t row_bytes;         /* device bytes of one row's stream state (16-byte aligned) */
+} nt_resampler_info;
+
+typedef struct nt_resampler nt_resampler;
+
+/* Geometry and sizes for a rate (needs no GPU); NT_ERR_INVALID, with the limit in the message, for a rejected rate. */
+int nt_resampler_query(int sample_rate, nt_resampler_info* info);
+/* table: caller-owned device memory of info.table_bytes, filled here (synchronously); state: device memory of
+ * max_rows * info.row_bytes (NULL when max_rows is 0), read and written by nt_resampler_push on the rows it names.
+ * Every row starts reset.  Needs an sm_90 device. */
+int nt_resampler_create(int sample_rate, int pcm_format, int max_rows, void* table, void* state, nt_resampler** out);
+int nt_resampler_destroy(nt_resampler* rs);
+/* Rows [n] (host) start a new stream: their held samples are dropped.  Host state only. */
+int nt_resampler_reset(nt_resampler* rs, const int32_t* rows, int n);
+/* Resample n items in one launch per 128 items.  in: device fp32, item i at in[in_offsets[i] .. in_offsets[i + 1]);
+ * out: device fp32 or int16 (the pcm_format of create), item i at out[out_offsets[i] .. out_offsets[i + 1]).  Offsets
+ * are host arrays of n + 1 non-decreasing entries.  rows: host [n] distinct rows < max_rows, whose streams continue;
+ * final_flags: host [n] (NULL: none final), nonzero ends that row's stream.  rows = NULL resamples each item whole as
+ * a one-shot row (no state is read or written; final_flags is ignored).  Each item's output span must be exactly the
+ * number of samples the contract above makes final, else NT_ERR_INVALID and nothing is launched. */
+int nt_resampler_push(nt_resampler* rs, int n, const int32_t* rows, const int32_t* final_flags, const float* in,
+                      const int64_t* in_offsets, void* out, const int64_t* out_offsets, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Single-op entry points (unit tests; each mirrors one row of SURVEY.md §8a)
  * ------------------------------------------------------------------------------------------ */
 int nt_op_rmsnorm(const float* x, const float* w, float eps, int rows, int cols, float* out_f32, void* out_bf16,

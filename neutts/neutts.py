@@ -111,16 +111,29 @@ class _CrossFade:
 class NeuTTS:
     def __init__(self, backbone_repo="neuphonic/neutts-nano", backbone_device="cpu", codec_repo="neuphonic/neucodec",
                  codec_device="cpu", *, tokenizer=None, phonemizer=None, backbone=None, codec=None,
-                 max_batch: int = 1, seed: int | None = None, speech_tokens_only: bool = False):
+                 max_batch: int = 1, seed: int | None = None, speech_tokens_only: bool = False,
+                 sample_rate: int = 24_000, pcm_format: str = "float32"):
         """Same positional signature and defaults as the reference (``neutts/neutts.py:75-81``), so
         ``examples/basic_example.py:12-17`` runs unmodified.  The device strings keep their reference
         meaning for the CALLER -- ``"cpu"`` = results come back as host arrays, which this facade always
         does -- but the engines themselves only exist for sm_90a: a ``"cpu"`` request runs on the current
         CUDA device and says so once (there is no CPU fallback).  ``speech_tokens_only``: generation may only draw
         ``<|speech_N|>`` ids and ``<|SPEECH_GENERATION_END|>`` (every other id suppressed, as transformers'
-        ``suppress_tokens``); the engine then skips the lm_head rows of every other id."""
+        ``suppress_tokens``); the engine then skips the lm_head rows of every other id.
+
+        ``sample_rate`` and ``pcm_format`` ("float32" or "int16") choose what every waveform comes back as.  NeuCodec
+        synthesises 24 kHz float32; any other setting resamples on the GPU before the copy to the host, with
+        torchaudio's ``resample`` semantics (``neutts_air_b200.resample.Resampler``), streams included.  "int16" is
+        ``rint(clip(y, -1, 1) * 32767)`` (clipped, rounded half to even), not the truncating ``astype`` that wraps
+        samples beyond +-1.  The watermark, when there is one, is applied at 24 kHz first, as the reference does."""
+        if not (type(sample_rate) is int and sample_rate == 24_000 and pcm_format == "float32"):
+            from neutts_air_b200.resample import check_args
+
+            check_args(sample_rate, pcm_format)   # ValueError for a rate or format the resampler cannot serve
+        self.sample_rate = int(sample_rate)       # the rate of every waveform returned (the codec's is 24 kHz)
+        self.pcm_format = pcm_format
+        self._resampler = None
         # constants the reference exposes (neutts/neutts.py:84-91)
-        self.sample_rate = 24_000
         self.max_context = 2048
         self.hop_length = 480
         self.streaming_overlap_frames = 1
@@ -334,8 +347,19 @@ class NeuTTS:
         return self.tokenizer.decode(out.numpy().tolist(), add_special_tokens=False)
 
     # ------------------------------------------------------------------ hot path B
-    def _decode_codes(self, codes: Sequence[torch.Tensor]) -> list:
-        """codes: list of 1-D int tensors -> list of float32 numpy waveforms (batched by equal length)."""
+    def _output_resampler(self):
+        """The GPU resampler to ``sample_rate`` / ``pcm_format`` (one row per slot), or None for 24 kHz float32."""
+        if self._resampler is None and (self.sample_rate, self.pcm_format) != (24_000, "float32"):
+            from neutts_air_b200.resample import Resampler
+
+            rows = max(self.max_batch, getattr(self.backbone, "max_batch", 1))
+            self._resampler = Resampler(self.sample_rate, self.pcm_format, device=self.codec.device, max_rows=rows)
+        return self._resampler
+
+    def _decode_codes(self, codes: Sequence[torch.Tensor], watermark: bool = False) -> list:
+        """codes: list of 1-D int tensors -> list of numpy waveforms at ``sample_rate`` in ``pcm_format`` (batched by
+        equal length).  ``watermark``: each waveform is watermarked at 24 kHz, before any resampling."""
+        rs = self._output_resampler()
         out = [None] * len(codes)
         by_len: dict = {}
         for i, c in enumerate(codes):
@@ -347,10 +371,22 @@ class NeuTTS:
             for j in range(0, len(idxs), cap):
                 grp = idxs[j: j + cap]
                 batch = torch.stack([codes[i].long() for i in grp])[:, None, :].to(self.codec.device)
+                if rs is None:
+                    with torch.no_grad():
+                        pcm = self.codec.decode_code(batch).cpu().numpy()
+                    for r, i in enumerate(grp):
+                        out[i] = pcm[r, 0, :]
+                    continue
                 with torch.no_grad():
-                    pcm = self.codec.decode_code(batch).cpu().numpy()
+                    pcm = self.codec.decode_code(batch)[:, 0, :]
+                if watermark and self.watermarker is not None:
+                    wm = np.stack([self._watermark(w) for w in pcm.cpu().numpy()]).astype(np.float32)
+                    pcm = torch.from_numpy(wm).to(rs.device)
+                pcm = rs.resample(pcm).cpu().numpy()
                 for r, i in enumerate(grp):
-                    out[i] = pcm[r, 0, :]
+                    out[i] = pcm[r]
+        if watermark and rs is None:
+            out = [self._watermark(w) for w in out]
         return out
 
     def _decode(self, codes) -> np.ndarray:
@@ -400,7 +436,7 @@ class NeuTTS:
                                  takes=takes)
         if return_logprobs:
             gen, lps = gen
-        wavs = [self._watermark(w) for w in self._decode_codes([self._ids_to_codes(g) for g in gen])]
+        wavs = self._decode_codes([self._ids_to_codes(g) for g in gen], watermark=True)
         return (wavs, [lp.numpy() for lp in lps]) if return_logprobs else wavs
 
     def infer_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], distributed: bool = False, *,
@@ -476,10 +512,12 @@ class NeuTTS:
         rank = dist.world()[0]
         if queue and len(mine) > self.max_batch:
             local = run(mine, rank << 20)
-            return dist.all_gather_waveforms(local, mine, len(prompts), device=self.codec.device)
-        for j in range(0, len(mine), self.max_batch):
-            local += run(mine[j: j + self.max_batch], (rank << 20) + j)
-        return dist.all_gather_waveforms(local, mine, len(prompts), device=self.codec.device)
+        else:
+            for j in range(0, len(mine), self.max_batch):
+                local += run(mine[j: j + self.max_batch], (rank << 20) + j)
+        out = dist.all_gather_waveforms(local, mine, len(prompts), device=self.codec.device)
+        # 16-bit samples are exact in the float32 gather buffer
+        return [w.astype(np.int16) for w in out] if self.pcm_format == "int16" else out
 
     @staticmethod
     def take_chunks(n_utterances: int, takes: int, max_batch: int) -> list:
@@ -658,6 +696,21 @@ class NeuTTS:
         tail_done = [False] * N
         occ = list(range(B))   # utterance held by each slot; None once its tail is out and nobody waits
         nxt = B                # next utterance to admit
+        rs = self._output_resampler()
+
+        def at_rate(out, ends=()):
+            """the round's 24 kHz chunks at ``sample_rate``: one push over the slots with new audio or an ending stream
+            (utterances ``ends``); a chunk whose samples are all still held becomes None"""
+            if rs is None:
+                return out
+            us = [u for u in range(N) if out[u] is not None or u in ends]
+            slot = {occ[b]: b for b in range(B) if occ[b] is not None}
+            got = rs.push([slot[u] for u in us], [np.zeros(0, np.float32) if out[u] is None else out[u] for u in us],
+                          [u in ends for u in us])
+            res = [None] * N
+            for u, y in zip(us, got):
+                res[u] = y if y.size else None
+            return res
 
         def seat(slots, idx):
             """history rows of ``slots`` := the reference codes of utterances ``idx``, nothing absorbed yet"""
@@ -668,6 +721,8 @@ class NeuTTS:
             hist[sl, : rows.shape[1]] = rows.to(dev)
             hlen[sl] = torch.tensor([len(refs[i]) for i in idx], device=dev)
             absorbed[sl] = 0
+            if rs is not None:
+                rs.reset(slots)
 
         def absorb(lo: int, hi: int):
             """tokens [lo, hi) of every slot -> history (non-speech ids dropped, as the reference's regex does)"""
@@ -730,12 +785,13 @@ class NeuTTS:
                     for b, wavs in decode_windows(jobs).items():
                         out[occ[b]] = np.concatenate([fades[occ[b]].push(w) for w in wavs])
                 # ragged tail of an utterance that finished (neutts/neutts.py:443-465), once its regular chunks are out
-                tails = []
+                tails, ending = [], []
                 all_finished = nxt == N and all(finished.values())
                 for b in held:
                     u = occ[b]
                     if finished[b] and not tail_done[u] and (all_finished or out[u] is None):
                         tail_done[u] = True
+                        ending.append(u)
                         n = hlen_h[b]
                         if n > n_dec[u]:
                             rem = n - n_dec[u]
@@ -745,12 +801,15 @@ class NeuTTS:
                             flush = fades[u].push(np.zeros(0, np.float32), final=True)
                             out[u] = flush if out[u] is None else np.concatenate((out[u], flush))
                 if all_finished and any(o is not None for o in out) and tails:
-                    yield out                    # regular chunks first: a tail is its own yield, as in the reference
+                    first = at_rate(out)         # regular chunks first: a tail is its own yield, as in the reference
+                    if any(o is not None for o in first):
+                        yield first
                     out = [None] * N
                 if tails:
                     for b, wavs in decode_windows(tails).items():
                         t = fades[occ[b]].push(wavs[0], final=True)
                         out[occ[b]] = t if out[occ[b]] is None else np.concatenate((out[occ[b]], t))
+                out = at_rate(out, ending)
                 if any(o is not None for o in out):
                     yield out
                 if all_finished:

@@ -86,6 +86,11 @@ class CodecConfig(C.Structure):
 _PP = C.POINTER(C.c_void_p)
 
 
+class ResamplerInfo(C.Structure):
+    _fields_ = [("orig", C.c_int32), ("target", C.c_int32), ("width", C.c_int32), ("taps", C.c_int32),
+                ("table_bytes", C.c_size_t), ("row_bytes", C.c_size_t)]
+
+
 class CodecWeights(C.Structure):
     _fields_ = [
         ("fsq_w", C.c_void_p), ("fsq_b", C.c_void_p), ("embed_w", C.c_void_p), ("embed_b", C.c_void_p),
@@ -109,6 +114,7 @@ EXPORTS = [
     "nt_debug_launch_chain", "nt_debug_decode_plan",
     "nt_codec_workspace_bytes", "nt_codec_create", "nt_codec_destroy", "nt_codec_decode",
     "nt_codec_debug_set_stages", "nt_codec_debug_ptr",
+    "nt_resampler_query", "nt_resampler_create", "nt_resampler_destroy", "nt_resampler_reset", "nt_resampler_push",
     "nt_op_rmsnorm", "nt_op_topk_sample",
 ]
 
@@ -168,6 +174,12 @@ def lib() -> C.CDLL:
     L.nt_codec_debug_set_stages.argtypes = [C.c_void_p, C.c_int, C.c_int]
     L.nt_codec_debug_ptr.restype = C.c_void_p
     L.nt_codec_debug_ptr.argtypes = [C.c_void_p, C.c_char_p]
+    L.nt_resampler_query.argtypes = [C.c_int, C.POINTER(ResamplerInfo)]
+    L.nt_resampler_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]
+    L.nt_resampler_destroy.argtypes = [C.c_void_p]
+    L.nt_resampler_reset.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int]
+    L.nt_resampler_push.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p,
+                                    C.POINTER(C.c_int64), C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]
     L.nt_op_rmsnorm.argtypes = [C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     L.nt_op_topk_sample.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(Sampling), C.c_void_p, C.c_int32,
                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
