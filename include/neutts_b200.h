@@ -76,6 +76,18 @@ typedef struct {
 
 int nt_gemm(const nt_gemm_args* args, void* stream);
 
+/* GEMM conformance hook (tests): nt_gemm with the dispatcher's internal choices exposed.
+ * bn: 0 = dispatcher's choice, else 32 | 64 | 128.  ring: -1 = dispatcher's choice, 0 = deep, 1 = shallow (half-depth).
+ * w_const: W may be fetched before the PDL wait.  split_ws / split_floats: lend a split-K workspace; split_info int64[2]
+ * receives (used, slice_stride).  a_lo_rows / w_lo_rows > 0: 3xTF32 (tf32 only, lo halves that many rows below).
+ * tile_max / tile_ld: per-row maxima of every column tile (plain fp32 epilogue). */
+int nt_debug_gemm(const nt_gemm_args* a, int bn, int ring, int w_const, float* split_ws, int64_t split_floats,
+                  int64_t* split_info, int a_lo_rows, int w_lo_rows, float* tile_max, int64_t tile_ld, void* stream);
+/* Teacher-forced scoring's lm_head epilogue alone (tests): bf16 A [M][K], W [N][K] (row stride K, K % 64 == 0);
+ * per row r and 128-column tile t, lse float2 [r * lse_ld + t] = (max, sum exp(v - max)); zt[r] = logit tgt[r]. */
+int nt_debug_gemm_logsoftmax(const void* A, int M, int K, const void* W, int N, const int32_t* tgt, void* lse,
+                             int64_t lse_ld, float* zt, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Speech LM (seam 1)
  * ------------------------------------------------------------------------------------------ */

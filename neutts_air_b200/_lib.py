@@ -104,7 +104,7 @@ class CodecWeights(C.Structure):
 
 # every symbol include/neutts_b200.h declares (tests check the library exports all of them)
 EXPORTS = [
-    "nt_last_error", "nt_abi_version", "nt_launch_count", "nt_gemm",
+    "nt_last_error", "nt_abi_version", "nt_launch_count", "nt_gemm", "nt_debug_gemm", "nt_debug_gemm_logsoftmax",
     "nt_lm_workspace_bytes", "nt_lm_create", "nt_lm_destroy", "nt_lm_prefill", "nt_lm_prefill_slots", "nt_lm_prefill_fork",
     "nt_lm_score_scratch_bytes", "nt_lm_score", "nt_lm_decode",
     "nt_lm_set_slot_sampling", "nt_lm_set_vocab_range", "nt_lm_set_repetition_penalty", "nt_lm_set_length_control",
@@ -138,6 +138,10 @@ def lib() -> C.CDLL:
     L.nt_abi_version.restype = C.c_int
     L.nt_launch_count.restype = C.c_uint64
     L.nt_gemm.argtypes = [C.POINTER(GemmArgs), C.c_void_p]
+    L.nt_debug_gemm.argtypes = [C.POINTER(GemmArgs), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_void_p,
+                                C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]
+    L.nt_debug_gemm_logsoftmax.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                           C.c_int64, C.c_void_p, C.c_void_p]
     L.nt_lm_workspace_bytes.restype = C.c_size_t
     L.nt_lm_workspace_bytes.argtypes = [C.POINTER(LMConfig)]
     L.nt_lm_create.argtypes = [C.POINTER(LMConfig), C.POINTER(LMWeights), C.c_void_p, C.c_size_t, C.POINTER(C.c_void_p)]

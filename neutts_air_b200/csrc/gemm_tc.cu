@@ -399,7 +399,7 @@ int gemm_tile_n(int M, int N, bool swiglu) {
 }
 
 int gemm_dispatch(const nt_gemm_args& a, cudaStream_t stream, SplitK* split, bool w_const, const Split3* s3, float* tile_max, int bn_req,
-                  long long tile_ld) {
+                  long long tile_ld, int ring) {
   if (a.M <= 0 || a.N <= 0 || a.K <= 0) return set_error(NT_ERR_INVALID, "gemm: empty problem");
   const int esz = a.dtype == NT_BF16 ? 2 : 4;
   const int bk = 128 / esz;
@@ -477,7 +477,7 @@ int gemm_dispatch(const nt_gemm_args& a, cudaStream_t stream, SplitK* split, boo
   const int ctas = mt * ((a.N + bn - 1) / bn) * (ep.split_k > 1 ? ep.split_k : 1);
   // Two CTAs per SM (half-depth ring) for every grid of more than one wave: one CTA's prologue / epilogue overlaps
   // the other's main loop, and grids just over a multiple of the SM count lose their short last wave.
-  const bool shallow = ctas > num_sms();
+  const bool shallow = ring >= 0 ? ring != 0 : ctas > num_sms();
 #define NT_GEMM_CASE(FMT, BNV)                                                                           \
   return shallow ? launch_gemm<FMT, BNV, true>(ta, tb, ep, a.M, a.N, num_kb, kb_per_tap, stream)         \
                  : launch_gemm<FMT, BNV, false>(ta, tb, ep, a.M, a.N, num_kb, kb_per_tap, stream)
@@ -525,4 +525,28 @@ int gemm_logsoftmax(const void* A, int M, int K, const void* W, int N, const int
 extern "C" int nt_gemm(const nt_gemm_args* args, void* stream) {
   if (!args) return nt::set_error(NT_ERR_INVALID, "nt_gemm: null args");
   return nt::gemm_dispatch(*args, reinterpret_cast<cudaStream_t>(stream), nullptr, /*w_const=*/false);
+}
+
+// Conformance hooks (tests): the production dispatcher with its internal choices exposed, nothing re-implemented.
+extern "C" int nt_debug_gemm(const nt_gemm_args* args, int bn, int ring, int w_const, float* split_ws, int64_t split_floats,
+                             int64_t* split_info, int a_lo_rows, int w_lo_rows, float* tile_max, int64_t tile_ld,
+                             void* stream) {
+  if (!args) return nt::set_error(NT_ERR_INVALID, "nt_debug_gemm: null args");
+  if (ring < -1 || ring > 1) return nt::set_error(NT_ERR_INVALID, "nt_debug_gemm: ring %d not in {-1, 0, 1}", ring);
+  const bool s3 = a_lo_rows > 0 || w_lo_rows > 0;
+  if (s3 && (a_lo_rows <= 0 || w_lo_rows <= 0))
+    return nt::set_error(NT_ERR_INVALID, "nt_debug_gemm: 3xTF32 needs both a_lo_rows and w_lo_rows > 0");
+  if (s3 && ring == 1) return nt::set_error(NT_ERR_INVALID, "nt_debug_gemm: 3xTF32 has no shallow ring");
+  if (split_ws && !split_info) return nt::set_error(NT_ERR_INVALID, "nt_debug_gemm: a split-K workspace needs split_info");
+  nt::SplitK sk{split_ws, static_cast<size_t>(split_floats > 0 ? split_floats : 0), 1, 0};
+  const nt::Split3 s3v{a_lo_rows, w_lo_rows};
+  const int rc = nt::gemm_dispatch(*args, reinterpret_cast<cudaStream_t>(stream), split_ws ? &sk : nullptr, w_const != 0,
+                                   s3 ? &s3v : nullptr, tile_max, bn, tile_ld, ring);
+  if (split_info) split_info[0] = sk.used, split_info[1] = sk.slice_stride;
+  return rc;
+}
+
+extern "C" int nt_debug_gemm_logsoftmax(const void* A, int M, int K, const void* W, int N, const int32_t* tgt, void* lse,
+                                        int64_t lse_ld, float* zt, void* stream) {
+  return nt::gemm_logsoftmax(A, M, K, W, N, tgt, static_cast<float2*>(lse), lse_ld, zt, reinterpret_cast<cudaStream_t>(stream));
 }

@@ -69,8 +69,11 @@ struct Split3 {
 // tile_max (optional, plain fp32 epilogue): [M][ceil(N / gemm_tile_n)] maximum of every row inside every column tile
 // (row pitch tile_ld when > 0).  bn > 0 forces the tile width (32 | 64 | 128): a GEMM over a column range of a wider
 // matrix then runs the instruction shape, and so the arithmetic, of the GEMM over the whole matrix.
+// ring >= 0 forces the shared-memory ring (0 deep, 1 shallow) instead of the choice by grid size (tests); the ring
+// depth changes the pipelining only, never the arithmetic.  3xTF32 always runs the deep ring.
 int gemm_dispatch(const nt_gemm_args& a, cudaStream_t stream, SplitK* split = nullptr, bool w_const = false,
-                  const Split3* s3 = nullptr, float* tile_max = nullptr, int bn = 0, long long tile_ld = 0);
+                  const Split3* s3 = nullptr, float* tile_max = nullptr, int bn = 0, long long tile_ld = 0,
+                  int ring = -1);
 int gemm_tile_n(int M, int N, bool swiglu);
 // Teacher-forced scoring: logits = A[M,K] . W[N,K]^T (bf16, K-major, row stride K) at a fixed 128-column tile, never
 // stored.  Per row r and column tile t: lse[r * lse_ld + t] = (max, sum exp(v - max)) over the tile's columns < N; the

@@ -77,6 +77,13 @@ def rel_rms(got, ref) -> float:
     return float((got - ref).norm() / ref.norm().clamp_min(1e-300))
 
 
+def tf32_truncate(x):
+    """fp32 -> TF32 (10-bit mantissa) by truncation, as the tensor core reads an fp32 operand in a plain TF32 MMA (this
+    model gives the 7.4e-4 .. 8.0e-4 per row that plain TF32 GEMMs measure on the H100; round to nearest gives 3e-4)."""
+    i = x.float().contiguous().view(torch.int32)
+    return (i & ~0x1FFF).view(torch.float32)
+
+
 def gather_kv(lm, layer: int, b: int, n: int):
     """Rows 0..n-1 of slot ``b``'s K and V in layer ``layer``, read through ``lm.page_table`` from the paged pool
     ``lm.kv[layer, 0|1, page, kv_head, row, :]`` (pages of 64 rows).  Returns two float64 CPU tensors [n, n_kv, 64]."""

@@ -40,7 +40,7 @@ import pytest
 import torch
 
 from oracle import codec_oracle as CO
-from tests.helpers import codec_shape, codec_weight_dict
+from tests.helpers import codec_shape, codec_weight_dict, tf32_truncate
 
 # Worst errors measured on one H100 80GB HBM3 (700 W power limit) over the whole GPU matrix, and the bars, ~4x above:
 #   fsq affine 7.8e-8; RMSNorm / LayerNorm rows 1.5e-7; GroupNorm + swish per group 4.0e-7; RoPE 4.0e-8;
@@ -98,13 +98,6 @@ def gemm_bar(op: str, mode: str) -> str:
     if op in ("head", "idft"):
         return "tf32" if mode == "tf32" else "3xtf32"
     return "3xtf32" if mode == "3xtf32" else "tf32"
-
-
-def tf32_truncate(x):
-    """fp32 -> TF32 (10-bit mantissa) by truncation, as the tensor core reads an fp32 operand in a plain TF32 MMA (this
-    model gives the 7.4e-4 .. 8.0e-4 per row that plain TF32 GEMMs measure on the H100; round to nearest gives 3e-4)."""
-    i = x.float().contiguous().view(torch.int32)
-    return (i & ~0x1FFF).view(torch.float32)
 
 
 # ====================================================================================== float64 stages

@@ -1,4 +1,5 @@
-"""GPU parity tests of single kernels through the C-ABI (wgmma GEMM, RMSNorm, sampler).
+"""GPU parity tests of single kernels through the C-ABI (RMSNorm, sampler); the wgmma GEMM has its own float64
+conformance matrix in test_gpu_gemm.py.
 
 The comparison target for these float kernels is a plain PyTorch fp32 evaluation of the same
 op on the same (rounded) operands; tolerances are stated next to each assertion."""
@@ -7,119 +8,9 @@ import ctypes as C
 import pytest
 import torch
 
-from tests.helpers import max_err, rel_err
+from tests.helpers import max_err
 
 pytestmark = pytest.mark.gpu
-
-
-def _gemm(L, dtype, A, W, M=None, N=None, K=None, lda=None, bias=None, residual=None, act=0, out_f32=None, out_bf16=None,
-          ldc=None, valid=(0, 0)):
-    from neutts_air_b200 import _lib
-
-    M = M if M is not None else A.shape[0]
-    N = N if N is not None else W.shape[0]
-    K = K if K is not None else W.shape[1]
-    a = _lib.GemmArgs()
-    a.dtype, a.M, a.N, a.K = dtype, M, N, K
-    a.A, a.lda = A.data_ptr(), lda if lda is not None else A.stride(0)
-    a.W, a.ldw = W.data_ptr(), W.stride(0)
-    a.bias = bias.data_ptr() if bias is not None else None
-    a.residual = residual.data_ptr() if residual is not None else None
-    a.ldr = residual.stride(0) if residual is not None else 0
-    a.act = act
-    a.out_f32 = out_f32.data_ptr() if out_f32 is not None else None
-    a.out_bf16 = out_bf16.data_ptr() if out_bf16 is not None else None
-    a.ldc = ldc if ldc is not None else (out_f32 if out_f32 is not None else out_bf16).stride(0)
-    a.valid_period, a.valid_len = valid
-    _lib.check(L.nt_gemm(C.byref(a), _lib.current_stream_ptr()))
-    torch.cuda.synchronize()
-
-
-@pytest.mark.parametrize("M,N,K", [(128, 128, 64), (500, 896, 896), (500, 1152, 896), (7, 896, 4864), (300, 1922, 1024),
-                                   (1000, 9728, 896), (64, 2048, 896)])
-def test_gemm_bf16_plain(cuda, M, N, K):
-    from neutts_air_b200 import _lib
-
-    L = _lib.lib()
-    g = torch.Generator(device="cpu").manual_seed(M * 7 + N)
-    A = torch.randn(M, K, generator=g).bfloat16().to(cuda)
-    W = (torch.randn(N, K, generator=g) / K ** 0.5).bfloat16().to(cuda)
-    out = torch.full((M, N), float("nan"), device=cuda)
-    _gemm(L, _lib.NT_BF16, A, W, out_f32=out)
-    ref = A.float() @ W.float().T
-    # same bf16 operands, fp32 accumulation on both sides: only summation order differs
-    assert rel_err(out, ref) < 1e-5, (rel_err(out, ref), max_err(out, ref))
-
-
-def test_gemm_bf16_epilogues(cuda):
-    from neutts_air_b200 import _lib
-
-    L = _lib.lib()
-    g = torch.Generator().manual_seed(3)
-    M, N, K = 333, 896, 896
-    A = torch.randn(M, K, generator=g).bfloat16().to(cuda)
-    W = (torch.randn(N, K, generator=g) / K ** 0.5).bfloat16().to(cuda)
-    bias = torch.randn(N, generator=g).to(cuda)
-    res = torch.randn(M, N, generator=g).to(cuda)
-    ref = A.float() @ W.float().T
-    # bias + residual, fp32 out aliasing the residual (the prefill o_proj/down_proj pattern)
-    out = res.clone()
-    _gemm(L, _lib.NT_BF16, A, W, bias=bias, residual=out, out_f32=out)
-    assert rel_err(out, ref + bias + res) < 1e-5
-    # SiLU + bf16 output
-    ob = torch.zeros(M, N, dtype=torch.bfloat16, device=cuda)
-    _gemm(L, _lib.NT_BF16, A, W, act=_lib.NT_ACT_SILU, out_bf16=ob)
-    assert rel_err(ob.float(), torch.nn.functional.silu(ref)) < 4e-3      # bf16 output rounding
-    # SwiGLU over interleaved (gate, up) columns -> N/2 bf16 outputs
-    og = torch.zeros(M, N // 2, dtype=torch.bfloat16, device=cuda)
-    _gemm(L, _lib.NT_BF16, A, W, act=_lib.NT_ACT_SWIGLU, out_bf16=og, ldc=N // 2)
-    want = torch.nn.functional.silu(ref[:, 0::2]) * ref[:, 1::2]
-    assert rel_err(og.float(), want) < 4e-3
-
-
-@pytest.mark.parametrize("M,N,K", [(256, 1024, 1024), (256, 1922, 1024), (250, 1920, 1922), (77, 3072, 1024)])
-def test_gemm_tf32(cuda, M, N, K):
-    from neutts_air_b200 import _lib
-
-    L = _lib.lib()
-    g = torch.Generator().manual_seed(N)
-    ld = (K + 31) // 32 * 32
-    A = torch.zeros(M, ld)
-    W = torch.zeros(N, ld)
-    A[:, :K] = torch.randn(M, K, generator=g)
-    W[:, :K] = torch.randn(N, K, generator=g) / K ** 0.5
-    A, W = A.to(cuda), W.to(cuda)
-    out = torch.full((M, N), float("nan"), device=cuda)
-    _gemm(L, _lib.NT_TF32, A, W, K=K, out_f32=out)
-    ref = (A[:, :K].double() @ W[:, :K].double().T).float()
-    # tf32 operands (10-bit mantissa), fp32 accumulation: ~1e-3 relative
-    assert rel_err(out, ref) < 2e-3, rel_err(out, ref)
-
-
-def test_gemm_conv_taps_and_row_mask(cuda):
-    """Conv1d(k=3, pad=1) over a padded-batch layout expressed as one GEMM (codec path)."""
-    from neutts_air_b200 import _lib
-
-    L = _lib.lib()
-    g = torch.Generator().manual_seed(5)
-    B, T, Cc, Co = 3, 50, 128, 96
-    Tp = T + 6
-    x = torch.randn(B, Cc, T, generator=g)
-    w = torch.randn(Co, Cc, 3, generator=g) / (3 * Cc) ** 0.5
-    b = torch.randn(Co, generator=g)
-    ref = torch.nn.functional.conv1d(x, w, b, padding=1)                      # [B, Co, T]
-    buf = torch.zeros(B * Tp + 8, Cc)
-    for i in range(B):
-        buf[i * Tp + 3: i * Tp + 3 + T] = x[i].T
-    buf = buf.to(cuda)
-    w2 = w.permute(0, 2, 1).reshape(Co, 3 * Cc).contiguous().to(cuda)
-    out = torch.zeros(B * Tp + 8, Co, device=cuda)
-    a_view = buf[2:]                                                           # first row the tap window of output row 0 touches
-    _gemm(L, _lib.NT_TF32, a_view, w2, M=B * Tp - 6, K=3 * Cc, lda=Cc, bias=b.to(cuda), out_f32=out[3:], valid=(Tp, T))
-    got = torch.stack([out[i * Tp + 3: i * Tp + 3 + T].T for i in range(B)]).cpu()
-    assert rel_err(got, ref) < 2e-3
-    pad_rows = torch.cat([out[i * Tp: i * Tp + 3] for i in range(B)] + [out[i * Tp + 3 + T: (i + 1) * Tp] for i in range(B)])
-    assert float(pad_rows.abs().max()) == 0.0                                  # masked rows were never written
 
 
 def test_rmsnorm_rows(cuda):
