@@ -319,6 +319,12 @@ int nt_lm_head_gemv(nt_lm* lm, const float* h, int B, float* logits, void* strea
  * internal activation buffer by name ("h", "q", "qkv", "attn", "act", "logits", "xn", "attn_bf16",
  * "act_bf16", "h_last", "tmax"); the pointer lies inside the caller's workspace. */
 int nt_lm_debug_set_layers(nt_lm* lm, int n_layers);
+/* Decode on n_ctas CTAs as if the device had that many SMs (tests): the persistent kernel's grid and work plans, its
+ * "batch x kv heads <= CTAs" gate and the GEMV grids all take n_ctas, and both plans are rebuilt for it (a whole-K
+ * plan the planner rejects there sends every decode to the per-op chain).  0 restores the default, the device's SM
+ * count capped at 256; otherwise 8 <= n_ctas <= min(device SMs, 256), else NT_ERR_INVALID.  Synchronises the device
+ * and drops the cached decode graph when the count changes.  The wgmma GEMMs keep sizing from the device. */
+int nt_lm_debug_set_sms(nt_lm* lm, int n_ctas);
 /* launch-latency probe: n dependent trivial kernels (grid x block) each incrementing *counter */
 int nt_debug_launch_chain(int n, int grid, int block, int* counter, void* stream);
 void* nt_lm_debug_ptr(nt_lm* lm, const char* name);

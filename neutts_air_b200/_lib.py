@@ -110,7 +110,7 @@ EXPORTS = [
     "nt_lm_set_slot_sampling", "nt_lm_set_vocab_range", "nt_lm_set_repetition_penalty", "nt_lm_set_length_control",
     "nt_lm_set_logprobs",
     "nt_lm_head_gemv",
-    "nt_lm_debug_set_layers", "nt_lm_debug_ptr", "nt_lm_debug_set_profile", "nt_lm_debug_capture_sampler",
+    "nt_lm_debug_set_layers", "nt_lm_debug_set_sms", "nt_lm_debug_ptr", "nt_lm_debug_set_profile", "nt_lm_debug_capture_sampler",
     "nt_debug_launch_chain", "nt_debug_decode_plan",
     "nt_codec_workspace_bytes", "nt_codec_create", "nt_codec_destroy", "nt_codec_decode",
     "nt_codec_debug_set_stages", "nt_codec_debug_ptr",
@@ -164,6 +164,7 @@ def lib() -> C.CDLL:
     L.nt_lm_set_logprobs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     L.nt_lm_head_gemv.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     L.nt_lm_debug_set_layers.argtypes = [C.c_void_p, C.c_int]
+    L.nt_lm_debug_set_sms.argtypes = [C.c_void_p, C.c_int]
     L.nt_lm_debug_ptr.restype = C.c_void_p
     L.nt_lm_debug_ptr.argtypes = [C.c_void_p, C.c_char_p]
     L.nt_lm_debug_set_profile.argtypes = [C.c_void_p, C.c_void_p, C.c_int]

@@ -91,7 +91,10 @@ struct StepSettings {
 
 struct nt_lm {
   nt_lm_config cfg;
-  int qkv_n, num_sms, max_splits, max_rows;
+  int qkv_n, max_splits, max_rows;
+  int dev_sms;   // the device's SM count
+  int num_sms;   // CTAs of the persistent kernel's grid and plans, and the GEMV grid cap: min(dev_sms, 256) unless
+                 // nt_lm_debug_set_sms overrides it
   const __nv_bfloat16* embed;
   const __nv_bfloat16* lm_head;
   const float* final_norm;
@@ -122,6 +125,7 @@ struct nt_lm {
   unsigned char* tc_gu_nsl = nullptr; // flat plan: K slices per gate/up tile
   uint8_t* tc_maps = nullptr;         // CUtensorMap[4 * n_layers + 1] weights, then xa x {16,32,64}, act x {16,32,64}
   TcPlan* tc_plan = nullptr;
+  bool tc_maps_ok = false;            // tc_maps built and the persistent kernel's buffers zeroed (done once)
   __nv_bfloat16 *tc_xa = nullptr, *tc_act = nullptr;
   float* tmax = nullptr;              // [max_batch][ceil(V / 128)] tile maxima of the logits rows (see lm_head_rows)
   float2 *tc_pq2 = nullptr, *tc_po2 = nullptr, *tc_pd2 = nullptr, *tc_ao2 = nullptr, *tc_aml2 = nullptr, *tc_act2 = nullptr, *tc_pg2 = nullptr,
@@ -253,6 +257,50 @@ static int lm_check_config(const nt_lm_config* c) {
   return NT_OK;
 }
 
+// Persistent wgmma decode kernel: both work plans for lm->num_sms CTAs, and every tensor map, built once (re-encoding
+// the maps on every GEMM call costs host time on each step; they do not depend on the CTA count).  A whole-K plan the
+// planner rejects leaves tc_ok false -> the per-op chain.  Synchronous: no launch may still read the plan buffers.
+static int tc_setup(nt_lm* lm) {
+  const nt_lm_config& c = lm->cfg;
+  lm->tc_ok = false;
+  std::vector<TcPlan> plan(512);
+  std::vector<unsigned char> nsl(4096, 0);
+  TcShape ts{c.hidden, c.inter, c.n_heads, c.n_kv_heads, lm->qkv_n, c.vocab_size};
+  const int G = lm->num_sms;
+  lm->tc_flat_ok = (2 * c.inter + 127) / 128 <= 4096 &&
+                   tc_build_plan(ts, G, true, plan.data() + 256, nsl.data(), &lm->tc_info[1]) == NT_OK;
+  if (tc_build_plan(ts, G, false, plan.data(), nullptr, &lm->tc_info[0]) != NT_OK) return NT_OK;
+  if (!lm->tc_maps_ok) {
+    const size_t nmaps = size_t(4) * c.n_layers + 1 + 6;
+    std::vector<CUtensorMap> maps(nmaps);
+    const int HD = c.n_heads * 64;
+    int rc = NT_OK;
+    for (int l = 0; l < c.n_layers && !rc; ++l) {
+      rc = make_tmap(&maps[4 * l + 0], NT_BF16, lm->wqkv[l], lm->qkv_n, c.hidden, c.hidden, 128);
+      if (!rc) rc = make_tmap(&maps[4 * l + 1], NT_BF16, lm->wo[l], c.hidden, HD, HD, 128);
+      if (!rc) rc = make_tmap(&maps[4 * l + 2], NT_BF16, lm->wgu[l], 2 * c.inter, c.hidden, c.hidden, 128);
+      if (!rc) rc = make_tmap(&maps[4 * l + 3], NT_BF16, lm->wd[l], c.hidden, c.inter, c.inter, 128);
+    }
+    if (!rc) rc = make_tmap(&maps[4 * c.n_layers], NT_BF16, lm->lm_head, c.vocab_size, c.hidden, c.hidden, 128);
+    const int nts[3] = {16, 32, 64};
+    for (int i = 0; i < 3 && !rc; ++i) {
+      rc = make_tmap(&maps[4 * c.n_layers + 1 + i], NT_BF16, lm->tc_xa, kTcMaxBatch, c.hidden, c.hidden, nts[i]);
+      if (!rc) rc = make_tmap(&maps[4 * c.n_layers + 4 + i], NT_BF16, lm->tc_act, kTcMaxBatch, c.inter, c.inter, nts[i]);
+    }
+    static_assert(sizeof(CUtensorMap) == 128, "CUtensorMap size");
+    if (rc) return rc;
+    NT_CUDA_CHECK(cudaMemcpy(lm->tc_maps, maps.data(), nmaps * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
+    NT_CUDA_CHECK(cudaMemset(lm->tc_xa, 0, size_t(kTcMaxBatch) * c.hidden * 2));
+    NT_CUDA_CHECK(cudaMemset(lm->tc_act, 0, size_t(kTcMaxBatch) * c.inter * 2));
+    NT_CUDA_CHECK(cudaMemset(lm->tc_pq2, 0, lm->tc_pair_bytes));   // stamp 0 = "never written"
+    lm->tc_maps_ok = true;
+  }
+  NT_CUDA_CHECK(cudaMemcpy(lm->tc_plan, plan.data(), 512 * sizeof(TcPlan), cudaMemcpyHostToDevice));
+  NT_CUDA_CHECK(cudaMemcpy(lm->tc_gu_nsl, nsl.data(), nsl.size(), cudaMemcpyHostToDevice));
+  lm->tc_ok = true;
+  return NT_OK;
+}
+
 extern "C" const char* nt_last_error(void) { return g_err; }
 extern "C" int nt_abi_version(void) { return 3; }
 extern "C" uint64_t nt_launch_count(void) { return g_launches.load(); }
@@ -303,7 +351,8 @@ extern "C" int nt_lm_create(const nt_lm_config* cfg, const nt_lm_weights* w, voi
     delete lm;
     return set_error(NT_ERR_CUDA, "device is sm_%d%d; this library is built for sm_90a only", prop.major, prop.minor);
   }
-  lm->num_sms = prop.multiProcessorCount;
+  lm->dev_sms = prop.multiProcessorCount;
+  lm->num_sms = lm->dev_sms > 256 ? 256 : lm->dev_sms;
   // rotary inverse frequencies (modeling_qwen2.py:95-100), per-layer norm / bias pointers
   float invf[64] = {0};
   for (int i = 0; i < 32; ++i) invf[i] = static_cast<float>(1.0 / std::pow(static_cast<double>(c.rope_theta), (2.0 * i) / 64.0));
@@ -319,42 +368,7 @@ extern "C" int nt_lm_create(const nt_lm_config* cfg, const nt_lm_weights* w, voi
     delete lm;
     return set_error(NT_ERR_CUDA, "workspace initialisation failed: %s", cudaGetErrorString(cudaGetLastError()));
   }
-  {
-    // persistent wgmma decode kernel: work plan + every tensor map, built once (re-encoding the maps on every GEMM
-    // call costs host time on each step).  A shape the plan cannot take leaves tc_ok false -> the per-op chain.
-    std::vector<TcPlan> plan(512);
-    std::vector<unsigned char> nsl(4096, 0);
-    TcShape ts{c.hidden, c.inter, c.n_heads, c.n_kv_heads, lm->qkv_n, c.vocab_size};
-    const int G = lm->num_sms > 256 ? 256 : lm->num_sms;
-    lm->tc_flat_ok = (2 * c.inter + 127) / 128 <= 4096 &&
-                     tc_build_plan(ts, G, true, plan.data() + 256, nsl.data(), &lm->tc_info[1]) == NT_OK;
-    if (tc_build_plan(ts, G, false, plan.data(), nullptr, &lm->tc_info[0]) == NT_OK) {
-      const size_t nmaps = size_t(4) * c.n_layers + 1 + 6;
-      std::vector<CUtensorMap> maps(nmaps);
-      const int HD = c.n_heads * 64;
-      int mrc = NT_OK;
-      for (int l = 0; l < c.n_layers && !mrc; ++l) {
-        mrc = make_tmap(&maps[4 * l + 0], NT_BF16, lm->wqkv[l], lm->qkv_n, c.hidden, c.hidden, 128);
-        if (!mrc) mrc = make_tmap(&maps[4 * l + 1], NT_BF16, lm->wo[l], c.hidden, HD, HD, 128);
-        if (!mrc) mrc = make_tmap(&maps[4 * l + 2], NT_BF16, lm->wgu[l], 2 * c.inter, c.hidden, c.hidden, 128);
-        if (!mrc) mrc = make_tmap(&maps[4 * l + 3], NT_BF16, lm->wd[l], c.hidden, c.inter, c.inter, 128);
-      }
-      if (!mrc) mrc = make_tmap(&maps[4 * c.n_layers], NT_BF16, lm->lm_head, c.vocab_size, c.hidden, c.hidden, 128);
-      const int nts[3] = {16, 32, 64};
-      for (int i = 0; i < 3 && !mrc; ++i) {
-        mrc = make_tmap(&maps[4 * c.n_layers + 1 + i], NT_BF16, lm->tc_xa, kTcMaxBatch, c.hidden, c.hidden, nts[i]);
-        if (!mrc) mrc = make_tmap(&maps[4 * c.n_layers + 4 + i], NT_BF16, lm->tc_act, kTcMaxBatch, c.inter, c.inter, nts[i]);
-      }
-      static_assert(sizeof(CUtensorMap) == 128, "CUtensorMap size");
-      if (!mrc && cudaMemcpy(lm->tc_maps, maps.data(), nmaps * sizeof(CUtensorMap), cudaMemcpyHostToDevice) == cudaSuccess &&
-          cudaMemcpy(lm->tc_plan, plan.data(), 512 * sizeof(TcPlan), cudaMemcpyHostToDevice) == cudaSuccess &&
-          cudaMemcpy(lm->tc_gu_nsl, nsl.data(), nsl.size(), cudaMemcpyHostToDevice) == cudaSuccess &&
-          cudaMemset(lm->tc_xa, 0, size_t(kTcMaxBatch) * c.hidden * 2) == cudaSuccess &&
-          cudaMemset(lm->tc_act, 0, size_t(kTcMaxBatch) * c.inter * 2) == cudaSuccess &&
-          cudaMemset(lm->tc_pq2, 0, lm->tc_pair_bytes) == cudaSuccess)   // stamp 0 = "never written"
-        lm->tc_ok = true;
-    }
-  }
+  tc_setup(lm);   // a failure leaves tc_ok false: every decode takes the per-op chain
   if (cudaStreamCreateWithFlags(&lm->cap_stream, cudaStreamNonBlocking) != cudaSuccess) {
     delete lm;
     return set_error(NT_ERR_CUDA, "stream creation failed");
@@ -931,7 +945,7 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
     P.logits_step_stride = static_cast<long long>(B) * c.vocab_size;
     P.prof = lm->prof, P.prof_step = lm->prof_step;
     if ((rc = launch_sampler_check(P.samp))) return rc;
-    return launch_decode_tc(P, B, lm->num_sms > 256 ? 256 : lm->num_sms, info, stream);
+    return launch_decode_tc(P, B, lm->num_sms, info, stream);
   }
 
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
@@ -1101,6 +1115,21 @@ extern "C" int nt_lm_debug_set_layers(nt_lm* lm, int n_layers) {
   if (!lm || n_layers > lm->cfg.n_layers) return set_error(NT_ERR_INVALID, "nt_lm_debug_set_layers: bad argument");
   lm->step.debug_layers = n_layers;
   return NT_OK;
+}
+extern "C" int nt_lm_debug_set_sms(nt_lm* lm, int n_ctas) {
+  if (!lm) return set_error(NT_ERR_INVALID, "nt_lm_debug_set_sms: null handle");
+  const int max = lm->dev_sms > 256 ? 256 : lm->dev_sms;
+  if (n_ctas != 0 && (n_ctas < 8 || n_ctas > max))   // a cooperative grid larger than the device cannot be launched
+    return set_error(NT_ERR_INVALID, "nt_lm_debug_set_sms: %d CTAs not in 8..%d (0: the device's count)", n_ctas, max);
+  const int G = n_ctas ? n_ctas : max;
+  NT_CUDA_CHECK(cudaDeviceSynchronize());   // no launch may still read the plan buffers tc_setup overwrites
+  if (G != lm->num_sms && lm->graph) {       // the chain's graph bakes in the GEMV grid
+    cudaGraphExecDestroy(lm->graph);
+    lm->graph = nullptr;
+    lm->graph_key.clear();
+  }
+  lm->num_sms = G;
+  return tc_setup(lm);
 }
 extern "C" int nt_lm_debug_set_profile(nt_lm* lm, long long* buf, int step) {
   if (!lm) return set_error(NT_ERR_INVALID, "nt_lm_debug_set_profile: null handle");

@@ -835,6 +835,11 @@ class SpeechLM:
     def debug_set_layers(self, n: int) -> None:
         _lib.check(self.L.nt_lm_debug_set_layers(self.handle, n))
 
+    def debug_set_sms(self, n: int) -> None:
+        """Decode on ``n`` CTAs (8 .. min(device SMs, 256)) as if the device had that many SMs: the persistent kernel's
+        grid and work plans, its batch gate and the GEMV grids; 0 restores the device's count."""
+        _lib.check(self.L.nt_lm_debug_set_sms(self.handle, n))
+
     def debug_buffer(self, name: str, shape, dtype=torch.float32) -> torch.Tensor:
         """View of an internal activation buffer (lives inside ``self.workspace``)."""
         ptr = self.L.nt_lm_debug_ptr(self.handle, name.encode())

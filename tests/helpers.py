@@ -2,6 +2,7 @@
 the decode path."""
 from __future__ import annotations
 
+import functools
 import math
 import warnings
 
@@ -116,6 +117,55 @@ def set_decode_impl(monkeypatch, impl):
 def runs_persistent(impl, B: int) -> bool:
     """Whether a decode at batch B runs the persistent kernel after ``set_decode_impl(monkeypatch, impl)``."""
     return impl == "tc" or (impl is None and B <= TC_DEFAULT_MAX_BATCH)
+
+
+# ------------------------------------------------------------------------------- the persistent kernel's work plans
+@functools.lru_cache(maxsize=None)
+def plan_summary(shape: tuple, G: int, flat: bool):
+    """The persistent decode kernel's plan for ``shape`` = (hidden, inter, n_heads, n_kv, vocab) on G CTAs, as (sq, so,
+    sd, sg, max_chunks, everybody), or None where the planner rejects it.  ``everybody``: the whole-K plan's gate/up
+    layout when fewer than 16 CTAs would be left for the split phases, so that every CTA takes gate/up tiles and split
+    items alike (restated from tc_build_plan, lm_decode_tc.cu); False for the flat plan."""
+    from neutts_air_b200.lm import debug_decode_plan
+
+    try:
+        p = debug_decode_plan(*shape, G, flat)
+    except ValueError:
+        return None
+    Tg = -(-2 * shape[1] // 128)
+    return p["sq"], p["so"], p["sd"], p["sg"], p["max_chunks"], not flat and G - min(Tg, G) < 16
+
+
+def plan_regime(shape: tuple, G: int):
+    """(whole-K plan, flat plan) summaries at G CTAs: what a decode of ``shape`` can run there."""
+    return plan_summary(shape, G, False), plan_summary(shape, G, True)
+
+
+@functools.lru_cache(maxsize=None)
+def regime_representatives(shape: tuple, max_G: int) -> dict:
+    """{regime: the smallest G in 8..max_G that has it}.  A regime recurring at separate counts counts once."""
+    reps = {}
+    for G in range(8, max_G + 1):
+        reps.setdefault(plan_regime(shape, G), G)
+    return reps
+
+
+def decode_branch(shape: tuple, B: int, G: int, max_ctx: int, impl=None) -> dict:
+    """The path nt_lm_decode (lm_api.cu) takes after ``set_decode_impl(monkeypatch, impl)``, for B <= max_batch
+    sequences of ``shape`` on G CTAs, restated from nt_lm_decode and launch_decode_tc: the persistent kernel when
+    ``runs_persistent(impl, B)``, its whole-K plan is accepted at G and B * n_kv <= G, else the per-op chain.  On the
+    persistent kernel: the flat plan when it is accepted and the slices are folded in the consumer CTAs (batch 1), bf16
+    hi + lo activation pairs up to batch 8, the tile width N and the attention splits per (sequence, kv head)."""
+    H, n_kv = shape[0], shape[3]
+    whole, flat = plan_regime(shape, G)
+    if not runs_persistent(impl, B) or whole is None or B * n_kv > G:
+        return dict(kind="chain", name="gemv" if B <= GEMV_MAX_BATCH else "gemm", split_cap=None)
+    fold = B == 1 and H * 4 <= 16 * 1024 and H <= 1024          # tc_fold_in_cta
+    plan = "flat" if flat is not None and fold else "wholeK"
+    nt = 16 if B <= 16 else (32 if B <= 32 else 64)
+    act = "hilo" if B <= 8 else "bf16"
+    return dict(kind="tc", plan=plan, fold=fold, act=act, nt=nt, split_cap=min(8, G // (B * n_kv), max_ctx // 64),
+                name=f"tc-{act}-n{nt}-{plan}-{'fold' if fold else 'phases'}")
 
 
 # ------------------------------------------------------------------------------- a small engine and its bar, a facade

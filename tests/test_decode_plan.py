@@ -3,8 +3,10 @@
 ``tc_build_plan`` (lm_decode_tc.cu) cuts the qkv, o_proj, gate/up and down_proj GEMMs of a layer into (tile, k-block
 range, slice) items and hands each CTA at most ``kTcMaxItems`` of them per phase.  The kernel trusts the plan: a tile
 slice listed twice is summed twice, one left out is never computed, and neither faults.  The plan depends on the shape
-and on the SM count, and a GPU run only ever sees one SM count, so these tests read the plan through
-``nt_debug_decode_plan`` (host code, no CUDA call) and check it for every count from 8 to 256.
+and on the CTA count, the device's SM count unless ``nt_lm_debug_set_sms`` sets a smaller one.  These tests read the
+plan through ``nt_debug_decode_plan`` (host code, no CUDA call) and check it for every count from 8 to 256.  They also
+pin the list of plan regimes (``tests.helpers.regime_representatives``): one CTA count per distinct plan, at which
+test_gpu_projections.py runs the kernel against float64.
 """
 from __future__ import annotations
 
@@ -115,6 +117,38 @@ def test_nano_batch1_plan_at_132_sms():
     assert plan_or_none(SHAPES["nano"], 132, True) is None
     p = plan_or_none(SHAPES["nano"], 132, False)
     assert p is not None and p["gu_split"] == 0 and p["sg"] == 1
+
+
+def test_plan_regimes_up_to_132_ctas():
+    """The regimes a 132-SM H100 can be made to run, one representative CTA count each (the smallest): a regime is the
+    (whole-K plan, flat plan) pair of (sq, so, sd, sg, max_chunks, gate/up layout) summaries, None where rejected."""
+    from tests.helpers import decode_branch, plan_regime, regime_representatives
+
+    reps = {name: regime_representatives(shape, 132) for name, shape in SHAPES.items()}
+    print("REGIMES " + "; ".join(f"{n} {len(r)}: {sorted(r.values())}" for n, r in reps.items()))
+    assert {n: len(r) for n, r in reps.items()} == {"air": 33, "nano": 52, "small": 14}
+    for name, r in reps.items():
+        assert len(set(r.values())) == len(r)
+        for regime, G in r.items():
+            assert plan_regime(SHAPES[name], G) == regime
+            assert all(plan_regime(SHAPES[name], g) != regime for g in range(8, G)), (name, G)
+        assert min(r.values()) == 8
+    air, nano, small = (regime_representatives(SHAPES[n], 132) for n in ("air", "nano", "small"))
+    everybody = lambda r: [G for (whole, _), G in r.items() if whole is not None and whole[5]]
+    # Air: the whole-K plan in the "everybody does everything" branch (42..91), also with no flat plan, where batch 1
+    # folds in the CTAs on the whole-K plan; o_proj in 13 slices (91); no whole-K plan at 92..117 (114: H100 PCIe)
+    assert everybody(air) and all(42 <= G <= 91 for G in everybody(air))
+    assert any(w is not None and w[5] and f is None for w, f in air)
+    assert any(w is not None and w[1] == 13 for w, _ in air)
+    assert sum(w is None and 92 <= G <= 117 for (w, _), G in air.items()) >= 2
+    assert all(decode_branch(SHAPES["air"], B, G, 512)["kind"] == "chain" for G in range(92, 118) for B in (1, 3, 12))
+    # Nano: the flat gate/up plan with the in-CTA fold, and the everybody branch
+    assert any(w is not None and f is not None for w, f in nano)
+    assert decode_branch(SHAPES["nano"], 1, 16, 512)["plan"] == "flat"
+    assert everybody(nano) and all(10 <= G <= 39 for G in everybody(nano))
+    # hidden 256: the everybody branch (8..25), attention in one split at batch 3
+    assert everybody(small) and all(8 <= G <= 25 for G in everybody(small))
+    assert any(decode_branch(SHAPES["small"], 3, G, 512)["split_cap"] == 1 for G in small.values())
 
 
 def test_bad_arguments_are_refused():

@@ -31,6 +31,11 @@ of every token row at index >= max_batch (lower rows are re-embedded by the samp
 steps in one call and checks every step.  Slots above the batch hold "loud" tokens (embedding rows scaled by 256), and
 a decode call at a larger batch (prefill: a prefill of every slot) runs first, so a leaked idle row moves the error by
 orders of magnitude.
+
+The persistent kernel runs the work plan its planner makes for its grid, the device's SM count unless
+``debug_set_sms`` sets a smaller one.  ``test_decode_projections_at_every_plan`` runs the decode checks at one CTA
+count per plan regime up to the device's count (tests.helpers.regime_representatives), at batches 1, 3 and 12, and
+also checks each row's kept sampler window against the float64 sampler.
 """
 from __future__ import annotations
 
@@ -43,7 +48,9 @@ import pytest
 import torch
 
 from oracle import lm_oracle as O
-from tests.helpers import GEMV_MAX_BATCH, gather_kv, make_lm, rel_rms, runs_persistent, set_decode_impl
+from tests.helpers import (GEMV_MAX_BATCH, decode_branch, gather_kv, make_lm, plan_regime, plan_summary,
+                           regime_representatives, rel_rms, set_decode_impl)
+from tests.sampler_ref import prob_err, ref_window
 
 # Worst errors measured on one H100 80GB HBM3 (132 SMs, 400 W power limit) over the whole case matrix, and the bars,
 # ~4x above.  Relative RMS of logits[:H] per (row, 128-element tile), of logits[H:] per row and of the prefill residual
@@ -220,24 +227,25 @@ def test_forward64_matches_the_oracle(shape):
     assert ((rms > 1.5) & (rms < 6)).sum() == len(toks) - 1 and rms[3] > 100
 
 
-def _fault_plan(shape: str, B: int):
-    """The plan the persistent kernel runs at batch B on 132 SMs, read from the library (no GPU needed)."""
-    from neutts_air_b200.lm import debug_decode_plan
+def _plan_shape(shape: str) -> tuple:
+    """(hidden, inter, n_heads, n_kv, vocab): the key of the tests.helpers plan functions."""
+    return SHAPES[shape] + (VOCAB,)
 
-    H, I, nh, nkv = SHAPES[shape]
-    flat = H <= 1024 and B == 1
-    try:
-        return debug_decode_plan(H, I, nh, nkv, VOCAB, 132, flat)
-    except ValueError:
-        return debug_decode_plan(H, I, nh, nkv, VOCAB, 132, False)
+
+def _most_slices(shape: str):
+    """(o_proj, down_proj) K slices of the plans that cut them finest, over every plan the planner accepts on 8..256
+    CTAs (read from the library, no GPU needed): the smallest slice any decode can run."""
+    plans = [p for G in range(8, 257) for flat in (False, True)
+             if (p := plan_summary(_plan_shape(shape), G, flat)) is not None]
+    return max(p[1] for p in plans), max(p[2] for p in plans)
 
 
 @pytest.mark.parametrize("shape", list(SHAPES))
 def test_fault_models_exceed_the_bars(shape):
     """float64, CPU: the faults these tests exist to catch move the error past the bar of every path that could commit
     them.  Activations rounded to bf16 instead of hi + lo: at least 10x past the hi + lo and fp32 bars.  One K slice of
-    one o_proj / down_proj tile dropped, or counted twice, with the slice bounds of the plan the persistent kernel runs
-    on 132 SMs (the most slices of any batch: the smallest slice): at least 10x past the hi + lo and fp32 bars, and at
+    one o_proj / down_proj tile dropped, or counted twice, with the slice bounds of the plan that cuts that GEMM finest
+    at any CTA count from 8 to 256 (the smallest slice): at least 10x past the hi + lo and fp32 bars, and at
     least 5x past the bf16 and prefill bars.  Those two sit on the noise floor of bf16 activations themselves: a
     rounding flip of one SwiGLU output moves the residual, which flips more roundings in the next layer, so even an fp32
     implementation with the same rounding points is ~4e-3 from the float64 mirror after three layers."""
@@ -253,9 +261,7 @@ def test_fault_models_exceed_the_bars(shape):
     bf16 = worst(forward64(shape, toks, attn_of, rb=BF16))
     lines = [f"bf16 activations {bf16:.2e}"]
     assert bf16 > 10 * max(BARS["hilo"], BARS["fp32"]), bf16
-    plans = [_fault_plan(shape, B) for B in (1, 3)]
-    for ph, KB, key in (("o", cfg.num_heads, "so"), ("d", cfg.intermediate_size // 64, "sd")):
-        S = max(p[key] for p in plans)
+    for ph, KB, S in zip(("o", "d"), (cfg.num_heads, cfg.intermediate_size // 64), _most_slices(shape)):
         for z, t, f in ((S - 1, 0, 0), (S // 2, (H - 1) // 128, 2)):   # the last slice of tile 0; a middle one, last tile
             k0, k1 = 64 * (KB * z // S), 64 * (KB * (z + 1) // S)
             e = worst(forward64(shape, toks, attn_of, fault=(1, ph, t, k0, k1, f)))
@@ -292,23 +298,6 @@ def _decode(lm, B: int, steps: int, sp):
     return logits.cpu(), lm.L.nt_launch_count() - n0
 
 
-def _tc_branch(shape: str, B: int) -> str:
-    """The persistent kernel's branch at batch B, restated from nt_lm_decode / launch_decode_tc: activations (hi + lo
-    up to batch 8), the tile width N, which plan and whether the split-K slices are folded in the consumer CTAs."""
-    from neutts_air_b200.lm import debug_decode_plan
-
-    H, I, nh, nkv = SHAPES[shape]
-    fold = B == 1 and H <= 1024
-    try:
-        debug_decode_plan(H, I, nh, nkv, VOCAB, _sms(), True)
-        flat_ok = True
-    except ValueError:
-        flat_ok = False
-    plan = "flat" if flat_ok and fold else "wholeK"
-    nt = 16 if B <= 16 else (32 if B <= 32 else 64)
-    return f"tc-{'hilo' if B <= 8 else 'bf16'}-n{nt}-{plan}-{'fold' if fold else 'phases'}"
-
-
 # (id, shape, batch, NT_DECODE_IMPL, branch)
 DECODE_CASES = [
     ("air-tc-b1", "air", 1, None, "tc-hilo-n16-flat-fold"),
@@ -332,11 +321,14 @@ DECODE_CASES = [
 def _check_rows(lm, rows, ref):
     """Worst error of the V rows the run appended, over layers and rows = [(slot, position)] in the order of ref's
     rows, against float64 v rounded to bf16."""
-    worst = 0.0
-    for l in range(N_LAYERS):
-        got = torch.stack([gather_kv(lm, l, b, p + 1)[1][p] for b, p in rows])
-        worst = max(worst, row_errors(got.reshape(len(rows), -1), _bf(ref["v"][l])))
-    return worst
+    got = _v_rows(lm, rows)
+    return max(row_errors(got[l], _bf(ref["v"][l])) for l in range(N_LAYERS))
+
+
+def _v_rows(lm, rows):
+    """The V rows [layers, len(rows), n_kv * 64] at rows = [(slot, position)] of the run's cache."""
+    return torch.stack([torch.stack([gather_kv(lm, l, b, p + 1)[1][p] for b, p in rows]).reshape(len(rows), -1)
+                        for l in range(N_LAYERS)])
 
 
 def _mean_v_from_cache(lm, shape, rows):
@@ -382,20 +374,17 @@ def test_decode_projections_vs_float64(cuda, case, monkeypatch):
     sp = lm.sampling(EOS, min_new_tokens=0, max_new_tokens=STEPS + 4, forced=forced)
     lm.prefill(prompts, sp)
     torch.cuda.synchronize()
-    persistent = runs_persistent(impl, B)
+    br = decode_branch(_plan_shape(shape), B, _sms(), MAX_CTX, impl)
+    persistent = br["kind"] == "tc"
     set_decode_impl(monkeypatch, "tc" if persistent else "perop")
     _decode(lm, MB, 1, sp)                    # the earlier call: every slot, the loud ones included
     set_decode_impl(monkeypatch, impl)
     logits, launches = _decode(lm, B, STEPS, sp)
 
     # the branch
-    if persistent:
-        assert launches == 1, launches
-        assert _tc_branch(shape, B) == branch
-    else:
-        assert launches > STEPS, launches
-        assert ("gemv" if B <= GEMV_MAX_BATCH else "gemm") == branch
-    kind = "tc" if persistent else "chain"
+    assert br["name"] == branch
+    assert launches == 1 if persistent else launches > STEPS, launches
+    kind = br["kind"]
     key = _path_key(kind, B)
     rb = NONE if key in ("hilo", "fp32") else BF16
 
@@ -416,6 +405,120 @@ def test_decode_projections_vs_float64(cuda, case, monkeypatch):
     print(msg)
     assert head < BARS[key] and tail < BARS[key], (head, tail)
     assert vrow < BARS["v-bf16" if key == "bf16" else "v-exact"], vrow
+
+
+# The CTA-count sweep: one engine per shape, batches run at every count
+SWEEP_BATCHES = (1, 3, 12)
+SWEEP_MAX_BATCH = 14
+# test_gpu_sampler.py's bar on the kept probabilities, max |p - p64| (tests/sampler_ref.py: BARS["prob"])
+PROB_BAR = 4e-7
+
+
+def _sweep_case(lm, shape: str, G: int, B: int, cap, monkeypatch):
+    """One case of the sweep at G CTAs and batch B, checked as in test_decode_projections_vs_float64, with the 4
+    teacher-forced steps in launches of 1 + 3 at batch 1 (fold counters and ping-pong parity carry across a launch),
+    and the last launch's kept sampler windows against the float64 sampler on the returned logits.  Returns the
+    logits, the appended V rows and the line to print."""
+    cfg, _ = avg_model(shape)
+    H = cfg.hidden_size
+    MB = B + 2
+    g = torch.Generator().manual_seed(3000 + B)
+    lens = [int(n) for n in torch.randint(1, 300, (MB,), generator=g)]
+    lens[0] = 299   # one slot past 4 pages
+    loud = lambda n: torch.randint(LOUD0, EOS, (n,), generator=g)
+    normal = lambda n: torch.randint(0, LOUD0, (n,), generator=g)
+    prompts = [(normal(n) if b < B else loud(n)).tolist() for b, n in enumerate(lens)]
+    forced = torch.stack([normal(STEPS + 2) if b < B else loud(STEPS + 2) for b in range(MB)])
+    sp = lm.sampling(EOS, min_new_tokens=0, max_new_tokens=STEPS + 4, forced=forced)
+    lm.prefill(prompts, sp)
+    torch.cuda.synchronize()
+    br = decode_branch(_plan_shape(shape), B, G, MAX_CTX)
+    persistent = br["kind"] == "tc"
+    set_decode_impl(monkeypatch, "tc" if persistent else "perop")
+    _decode(lm, MB, 1, sp)                    # the earlier call: every slot, the loud ones included
+    set_decode_impl(monkeypatch, None)
+    runs = [_decode(lm, B, n, sp) for n in ((1, STEPS - 1) if B == 1 else (STEPS,))]
+    logits, launches = torch.cat([r[0] for r in runs]), sum(r[1] for r in runs)
+    assert launches == len(runs) if persistent else launches > STEPS, (shape, G, B, br["name"], launches)
+
+    key = _path_key(br["kind"], B)
+    assert not lm.kv[:, 0].any(), "a K row is not 0"
+    rows = [(b, lens[b] + 1 + s) for s in range(STEPS) for b in range(B)]
+    toks = [int(forced[b, 1 + s]) for s in range(STEPS) for b in range(B)]
+    ref = forward64(shape, toks, _mean_v_from_cache(lm, shape, rows), rb=NONE if key in ("hilo", "fp32") else BF16)
+    head, tail = logit_errors(logits.reshape(STEPS * B, VOCAB), ref["logits"], H)
+    v = _v_rows(lm, rows)
+    vrow = max(row_errors(v[l], _bf(ref["v"][l])) for l in range(N_LAYERS))
+    vbar = BARS["v-bf16" if key == "bf16" else "v-exact"]
+
+    tv, ti, tt = (t.cpu().numpy() for t in cap)
+    perr = 0.0
+    for b in range(B):
+        ids, p = ref_window(logits[-1, b].numpy(), 0, EOS, 0, 50, 1.0)
+        assert ti[b, : len(ids)].tolist() == ids.tolist() and (ti[b, len(ids):] == -1).all(), (shape, G, B, b)
+        assert tt[b] == forced[b, STEPS + 1], (shape, G, B, b)
+        perr = max(perr, prob_err(tv[b, : len(ids)], p))
+
+    line = (f"PROJ-SMS {shape} G={G} B={B} [{br['name']}, split_cap {br['split_cap']}, {launches} launches]: "
+            f"logits[:H] tile {head:.2e} logits[H:] {tail:.2e} (bar {BARS[key]:.1e}) V row {vrow:.2e} (bar {vbar:.1e}) "
+            f"kept p {perr:.1e} (bar {PROB_BAR:.0e})")
+    assert head < BARS[key] and tail < BARS[key], line
+    assert vrow < vbar, line
+    assert perr < PROB_BAR, line
+    return logits, v, br, line
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("shape", list(SHAPES))
+def test_decode_projections_at_every_plan(cuda, shape, monkeypatch):
+    """The decode cases of test_decode_projections_vs_float64 at one CTA count per plan regime the planner makes up to
+    the device's SM count (tests.helpers.regime_representatives), set with ``debug_set_sms``, at batches 1, 3 and 12.
+    The engine takes the branch decode_branch predicts, the per-op chain where the persistent kernel has no plan or
+    too few CTAs.  The sweep starts and ends at the device's count, and those two runs must agree bit for bit: a change
+    of count leaves nothing stale in the plan, the fold counters or the stamps."""
+    cfg, w = avg_model(shape)
+    dev = _sms()
+    card = _card()
+    lm = make_lm(cfg, w, max_batch=SWEEP_MAX_BATCH, max_ctx=MAX_CTX, page_shuffle_seed=7)
+    cap = lm.debug_capture_sampler()
+    reps = sorted(regime_representatives(_plan_shape(shape), dev).values())
+    counts = [None] + reps + [0]      # None: the engine as created; 0: the device's count restored
+    first, caps, plans, seen = {}, set(), set(), []
+    for G in counts:
+        if G is not None:
+            lm.debug_set_sms(G)
+        g_eff = G or dev
+        for B in SWEEP_BATCHES:
+            logits, v, br, line = _sweep_case(lm, shape, g_eff, B, cap, monkeypatch)
+            print(f"{line} [{card}]")
+            if br["kind"] == "tc":
+                caps.add(br["split_cap"])
+                plans.add(br["plan"])
+            if G is None:
+                first[B] = (logits, v)
+            elif G == 0:
+                assert torch.equal(logits, first[B][0]) and torch.equal(v, first[B][1]), (shape, B)
+        seen.append(g_eff)
+    print(f"PROJ-SMS {shape}: {len(reps)} regimes at CTA counts {seen}; split_cap {sorted(caps)}; plans {sorted(plans)}")
+    assert {1, 8} <= caps, caps
+    regimes = [plan_regime(_plan_shape(shape), G) for G in reps]
+    want = {"wholeK"} if any(wk for wk, _ in regimes) else set()
+    if any(wk and fl for wk, fl in regimes):
+        want.add("flat")
+    assert plans == want, (plans, want)
+
+
+@pytest.mark.gpu
+def test_debug_set_sms_refuses_counts_the_device_cannot_run(cuda):
+    cfg, w = avg_model("small")
+    lm = make_lm(cfg, w, max_batch=1, max_ctx=MAX_CTX)
+    top = min(torch.cuda.get_device_properties(0).multi_processor_count, 256)
+    for n in (-1, 7, top + 1):
+        with pytest.raises(ValueError, match=f"not in 8..{top}"):
+            lm.debug_set_sms(n)
+    lm.debug_set_sms(8)
+    lm.debug_set_sms(top)
+    lm.debug_set_sms(0)
 
 
 def _gemm_splits(M: int, N: int, K: int, ws_floats: int) -> int:
