@@ -311,6 +311,32 @@ int nt_lm_set_length_control(nt_lm* lm, const nt_slot_length* host_table, void* 
  * Host state only, like nt_lm_set_vocab_range.  nt_op_topk_sample and nt_lm_head_gemv ignore it. */
 int nt_lm_set_logprobs(nt_lm* lm, float* out, void* stream);
 
+/* Classifier-free guidance (transformers' guidance_scale with negative_prompt_ids,
+ * UnbatchedClassifierFreeGuidanceLogitsProcessor).  A guided pair is two slots: c (conditional: its prompt, its tokens
+ * are the ones returned) and u = table[c].partner (unconditional: the negative prompt, then every token c draws).  At
+ * every sampler launch, right after the lm_head (and the vocabulary range's EOS tile), c's logits row becomes
+ *   g * (ls_c - ls_u) + ls_u      (fp32, in that order; g = table[c].scale)
+ * with ls the log-softmax of the row over the ids the lm_head computes; an id that reads -inf in either row stays -inf.
+ * The repetition penalty, EOS mask, length decay, temperature, warpers, Philox draw and log-probabilities then act on
+ * that row as usual, with c's settings.  u is never sampled: after each sampler launch its out_tokens, cur_token and
+ * n_generated mirror c's, its seq_lens advances, its done is c's, and its next input is c's token.  If u's context
+ * would reach max_ctx, both slots finish (cap c through nt_sampling.limits so that u fits).  The combine reads u's raw
+ * logits; u's own table entries only shape u's logits outputs.  Slots outside a pair are bit-identical to the table off.
+ * Rules (NT_ERR_INVALID, previous table kept): partner in -1 .. max_batch - 1 and not the slot itself; a partner serves
+ * one c and has no partner of its own; scale finite, > 0 and != 1 wherever partner >= 0 (ignored elsewhere).
+ * While the table is on: nt_lm_decode runs the per-op chain at every batch (NT_DECODE_IMPL=tc returns NT_ERR_INVALID),
+ * and every pair with a slot below the call's batch must lie wholly below it; nt_lm_prefill and nt_lm_prefill_slots
+ * need both slots of every pair they touch in the same call; nt_lm_prefill_fork returns NT_ERR_INVALID.  Switching the
+ * table on or off rebuilds the cached decode graph; new contents of a table that stays on reach it at replay.
+ * nt_op_topk_sample, nt_lm_head_gemv and nt_lm_score ignore the table. */
+typedef struct {
+  int32_t partner;   /* u slot of this c slot, or -1 */
+  float scale;       /* guidance scale g */
+} nt_slot_guidance;
+
+/* table: host array of max_batch entries (row s = slot s), or NULL = off (the default).  Copied on `stream`. */
+int nt_lm_set_guidance(nt_lm* lm, const nt_slot_guidance* table, void* stream);
+
 /* Timed single-kernel entry for the roofline measurement: the lm_head GEMV (+ final RMSNorm)
  * exactly as the decode step launches it.  h: f32 [B][hidden] -> logits f32 [B][vocab]. */
 int nt_lm_head_gemv(nt_lm* lm, const float* h, int B, float* logits, void* stream);

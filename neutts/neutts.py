@@ -27,7 +27,7 @@ from typing import Generator, Sequence
 import numpy as np
 import torch
 
-from neutts_air_b200.lm import per_item, per_prompt_decay, resolve_settings
+from neutts_air_b200.lm import check_guidance_scale, per_item, per_prompt_decay, resolve_settings
 
 SPEECH_RE = re.compile(r"<\|speech_(\d+)\|>")
 CHAT = "user: Convert the text to speech:<|TEXT_REPLACE|>\nassistant:<|SPEECH_REPLACE|>"
@@ -52,6 +52,26 @@ def _controls(n: int, temperature, top_k, top_p, min_p, repetition_penalty=1.0, 
     return ctl
 
 
+def _guided(n: int, guidance_scale) -> bool:
+    """Whether any of n utterances is guided: ``guidance_scale`` a number or one per utterance, each finite and > 0
+    (1 = off; ValueError otherwise)."""
+    g = per_item(n, "utterance", guidance_scale=guidance_scale)["guidance_scale"]
+    return any(check_guidance_scale(x) != 1.0 for x in (g if isinstance(g, list) else [g]))
+
+
+def _add_guidance(ctl: dict, n: int, guidance_scale, negatives) -> dict:
+    """The controls of n utterances with classifier-free guidance: ``negatives`` None or one negative prompt (id list,
+    or None for the prompt's last token) per utterance.  Nothing is added when no utterance is guided, so the engine
+    calls stay exactly those of a run without guidance."""
+    if _guided(n, guidance_scale):
+        g = per_item(n, "utterance", guidance_scale=guidance_scale)["guidance_scale"]
+        if negatives is not None and len(negatives) != n:
+            raise ValueError(f"negative prompts need one entry per utterance ({n}), got {len(negatives)}")
+        ctl["guidance_scale"] = g
+        ctl["negative_prompt_ids"] = None if negatives is None else [None if q is None else list(q) for q in negatives]
+    return ctl
+
+
 def _pick(ctl: dict, idx) -> dict:
     """The controls of the utterances ``idx`` (lists are indexed, scalars stay)."""
     return {k: [v[i] for i in idx] if isinstance(v, list) else v for k, v in ctl.items()}
@@ -68,6 +88,9 @@ def _backbone_kw(ctl: dict) -> dict:
         kw.update(pen)
     if ctl.get("exponential_decay_length_penalty") is not None:
         kw["exponential_decay_length_penalty"] = ctl["exponential_decay_length_penalty"]
+    if "guidance_scale" in ctl:
+        kw["guidance_scale"] = ctl["guidance_scale"]
+        kw["negative_prompt_ids"] = ctl["negative_prompt_ids"]
     return kw
 
 
@@ -284,6 +307,8 @@ class NeuTTS:
         rng = self._speech_range()
         if rng is not None:
             kw["vocab_range"] = rng
+        if takes > 1 and "guidance_scale" in kw:
+            raise ValueError("classifier-free guidance generates one take per utterance (takes=1)")
         if takes > 1:
             kw["return_logprobs"] = True
             ids, lps = self.backbone.generate_batch(list(prompts), eos, max_length=self.max_context, min_new_tokens=min_new_tokens,
@@ -292,7 +317,7 @@ class NeuTTS:
             keep = best_takes(lps, takes)
             ids, lps = [ids[k] for k in keep], [lps[k] for k in keep]
             return (ids, lps) if logprobs else ids
-        if len(prompts) > self.max_batch and hasattr(self.backbone, "generate_queue"):
+        if self._slots(len(prompts), kw) > self.max_batch and hasattr(self.backbone, "generate_queue"):
             # more prompts than slots: refill each slot as soon as its utterance ends (prompt i keeps the Philox
             # stream slot_base + i that the chunked loop gives it)
             return self.backbone.generate_queue(list(prompts), eos, max_length=self.max_context, min_new_tokens=min_new_tokens,
@@ -312,12 +337,38 @@ class NeuTTS:
             if one.get("exponential_decay_length_penalty", ()) is None:   # this utterance has no decay: pass nothing
                 del one["exponential_decay_length_penalty"]
             one.update(suppress)
+            g, neg = one.pop("guidance_scale", 1.0), one.pop("negative_prompt_ids", None)
+            if g != 1.0:   # transformers' UnbatchedClassifierFreeGuidanceLogitsProcessor; None: the prompt's last token
+                one["guidance_scale"] = g
+                if neg is not None:
+                    one["negative_prompt_ids"] = torch.tensor([list(neg)]).to(self.backbone.device)
             with torch.no_grad():
                 o = self.backbone.generate(t, max_length=self.max_context, eos_token_id=eos, do_sample=True, use_cache=True,
                                            min_new_tokens=min_new_tokens[i] if isinstance(min_new_tokens, list) else min_new_tokens,
                                            **one)
             outs.append(o[0, t.shape[-1]:].cpu().long())
         return outs
+
+    @staticmethod
+    def _slots(n: int, ctl: dict) -> int:
+        """Engine slots n prompts take at once: one each, and one more for every guided prompt's negative prompt."""
+        g = ctl.get("guidance_scale", 1.0)
+        return n + (sum(x != 1.0 for x in g) if isinstance(g, list) else (n if g != 1.0 else 0))
+
+    def _negatives(self, n: int, guidance_scale, negative_text, ref_codes, ref_texts):
+        """The negative prompts of n utterances: the chat template with the utterance's reference codes and text and
+        ``negative_text`` (a string or one per utterance; None is "", the voice without the words) as the input text.
+        None when no utterance is guided."""
+        if not _guided(n, guidance_scale):
+            return None
+        neg = per_item(n, "utterance", negative_text=negative_text)["negative_text"]
+        neg = neg if isinstance(neg, list) else [neg] * n
+        return [self._apply_chat_template(c, rt, t if t is not None else "") for c, rt, t in zip(ref_codes, ref_texts, neg)]
+
+    @staticmethod
+    def _no_guidance(guidance_scale, what: str) -> None:
+        if _guided(len(guidance_scale) if isinstance(guidance_scale, (list, tuple)) else 1, guidance_scale):
+            raise ValueError(f"classifier-free guidance is not supported by {what} (guidance_scale must be 1)")
 
     def _n_codes(self) -> int:
         shape = getattr(self.codec, "shape", None)
@@ -407,27 +458,34 @@ class NeuTTS:
     def infer(self, text: str, ref_codes, ref_text: str, *, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0,
               min_p: float = 0.0, repetition_penalty: float = 1.0, penalize_prompt: bool = True,
               return_logprobs: bool = False, takes: int = 1, min_new_tokens: int = 50,
-              exponential_decay_length_penalty=None):
+              exponential_decay_length_penalty=None, guidance_scale: float = 1.0, negative_text: str | None = None):
         """Text + reference voice -> 24 kHz float32 waveform (``neutts/neutts.py:216-243``).  The sampling controls
         default to the reference's values; see ``infer_batch``.  ``return_logprobs``: returns (waveform, log-probs).
-        ``takes``: generate that many takes and keep the most probable one (``infer_batch``)."""
+        ``takes``: generate that many takes and keep the most probable one (``infer_batch``).  ``guidance_scale`` and
+        ``negative_text``: classifier-free guidance (``infer_batch``)."""
         out = self.infer_batch([text], [ref_codes], [ref_text], temperature=temperature, top_k=top_k, top_p=top_p,
                                min_p=min_p, repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt,
                                return_logprobs=return_logprobs, takes=takes, min_new_tokens=min_new_tokens,
-                               exponential_decay_length_penalty=exponential_decay_length_penalty)
+                               exponential_decay_length_penalty=exponential_decay_length_penalty,
+                               guidance_scale=guidance_scale, negative_text=negative_text)
         return (out[0][0], out[1][0]) if return_logprobs else out[0]
 
     def infer_from_prompt_ids(self, prompts: Sequence[Sequence[int]], max_new_tokens: int | None = None,
                               min_new_tokens: int = 50, slot_base: int = 0, *, temperature=1.0, top_k=50, top_p=1.0,
                               min_p=0.0, repetition_penalty=1.0, penalize_prompt=True, return_logprobs: bool = False,
-                              takes: int = 1, exponential_decay_length_penalty=None):
+                              takes: int = 1, exponential_decay_length_penalty=None, guidance_scale=1.0,
+                              negative_prompt_ids=None):
         """Hot path only: prompt ids (host) -> waveforms (host).  Used by bench.py's end-to-end leg.
         ``slot_base`` offsets the sampler's Philox slot index so chunks / ranks under one seed draw independently.
         More prompts than ``max_batch`` go through the backbone's ``generate_queue`` when it has one.  Sampling
         controls, length controls, ``return_logprobs`` and ``takes`` as in ``infer_batch`` (here len(prompts) * takes <=
-        max_batch, and ``slot_base`` counts takes)."""
+        max_batch, and ``slot_base`` counts takes).  ``guidance_scale`` (a number or one per prompt, 1 = off) and
+        ``negative_prompt_ids`` (None, or one id list or None per prompt; None: the prompt's last token) add
+        classifier-free guidance (``SpeechLM.generate_batch``; transformers' ``guidance_scale`` and
+        ``negative_prompt_ids`` on an injected transformers backbone)."""
         ctl = _controls(len(prompts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
                         exponential_decay_length_penalty)
+        ctl = _add_guidance(ctl, len(prompts), guidance_scale, negative_prompt_ids)
         min_new_tokens = ctl.pop("min_new_tokens")
         takes = self._check_takes(takes)
         if takes > 1 and return_logprobs:
@@ -441,7 +499,8 @@ class NeuTTS:
 
     def infer_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], distributed: bool = False, *,
                     temperature=1.0, top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0, penalize_prompt=True,
-                    return_logprobs: bool = False, takes: int = 1, min_new_tokens=50, exponential_decay_length_penalty=None):
+                    return_logprobs: bool = False, takes: int = 1, min_new_tokens=50, exponential_decay_length_penalty=None,
+                    guidance_scale=1.0, negative_text=None):
         """List in / list out.  With ``distributed=True`` (inside an initialised torch.distributed job) the
         utterances are sharded over ranks and every rank returns all waveforms (one all-gather).
 
@@ -479,11 +538,22 @@ class NeuTTS:
         is generated ``takes`` times from one prefill of its prompt (``generate_batch``'s ``num_return_sequences``:
         the takes share the prompt's KV pages), and only the take with the highest mean ``model`` log-probability over
         its generated tokens (EOS included; ties: the first take) goes through the codec.  Utterances run in chunks of
-        ``max_batch // takes``; ``return_logprobs`` returns the kept takes' rows."""
+        ``max_batch // takes``; ``return_logprobs`` returns the kept takes' rows.
+
+        Classifier-free guidance (transformers' ``guidance_scale`` with a negative prompt): ``guidance_scale`` (a number
+        or one per utterance, > 0; 1 = off) and ``negative_text`` (a string or one per utterance).  The negative prompt
+        is the chat template with the utterance's own reference codes and reference text and ``negative_text`` as the
+        input text; None means "", the voice without the words, which steers the draws toward the text.  Each guided
+        utterance decodes its negative prompt in a second engine slot, so a chunk or the queue holds fewer of them at
+        once.  Not with ``takes`` > 1 (ValueError); ``distributed`` works, every rank guiding its own utterances."""
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
         ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
                         exponential_decay_length_penalty)
+        ctl = _add_guidance(ctl, len(texts), guidance_scale,
+                            self._negatives(len(texts), guidance_scale, negative_text, ref_codes, ref_texts))
+        if takes != 1 and "guidance_scale" in ctl:
+            raise ValueError("classifier-free guidance generates one take per utterance (takes=1)")
         takes = self._check_takes(takes, distributed)
         if return_logprobs:
             self._check_logprobs(distributed)
@@ -493,15 +563,25 @@ class NeuTTS:
         queue = hasattr(self.backbone, "generate_queue")
 
         def run(idx, slot_base):
+            c = _pick(ctl, idx)
+            g, neg = c.pop("guidance_scale", 1.0), c.pop("negative_prompt_ids", None)
             return self.infer_from_prompt_ids([prompts[i] for i in idx], slot_base=slot_base, return_logprobs=return_logprobs,
-                                              **_pick(ctl, idx))
+                                              guidance_scale=g, negative_prompt_ids=neg, **c)
 
+        # chunks of prompts whose slots (two for a guided one) fit the engine; prompt i keeps Philox stream i
+        chunks, j = [], 0
+        while j < len(prompts):
+            k = j + 1
+            while k < len(prompts) and self._slots(k + 1 - j, _pick(ctl, range(j, k + 1))) <= self.max_batch:
+                k += 1
+            chunks.append(range(j, k))
+            j = k
         if not distributed:
-            if queue and len(prompts) > self.max_batch:
+            if queue and len(chunks) > 1:
                 return run(range(len(prompts)), 0)
             out, lps = [], []
-            for j in range(0, len(prompts), self.max_batch):
-                r = run(range(j, min(j + self.max_batch, len(prompts))), j)
+            for idx in chunks:
+                r = run(idx, idx[0])
                 out += r[0] if return_logprobs else r
                 lps += r[1] if return_logprobs else []
             return (out, lps) if return_logprobs else out
@@ -510,7 +590,7 @@ class NeuTTS:
         mine = dist.shard_indices(len(prompts), [len(p) for p in prompts])
         local = []
         rank = dist.world()[0]
-        if queue and len(mine) > self.max_batch:
+        if queue and self._slots(len(mine), _pick(ctl, mine)) > self.max_batch:
             local = run(mine, rank << 20)
         else:
             for j in range(0, len(mine), self.max_batch):
@@ -591,13 +671,15 @@ class NeuTTS:
     def infer_stream(self, text: str, ref_codes, ref_text: str, *, temperature: float = 1.0, top_k: int = 50,
                      top_p: float = 1.0, min_p: float = 0.0, repetition_penalty: float = 1.0,
                      penalize_prompt: bool = True, takes: int = 1, min_new_tokens: int = 50,
-                     exponential_decay_length_penalty=None) -> Generator[np.ndarray, None, None]:
+                     exponential_decay_length_penalty=None, guidance_scale=1.0) -> Generator[np.ndarray, None, None]:
         """Streaming synthesis with the reference's window geometry (``neutts/neutts.py:373-465``):
         every 25 new frames (once 5 look-ahead frames exist) the codec re-decodes
         [n - 50 - 1, n + 25 + 5 + 1) and the chunk is cross-faded with triangular weights.  Sampling controls as in
         ``infer_batch``; streaming returns no per-token log-probabilities (``return_logprobs`` is not supported here)
-        and generates one take per utterance (``takes`` other than 1 raises ValueError)."""
+        and generates one take per utterance (``takes`` other than 1 raises ValueError); classifier-free guidance is not
+        supported (``guidance_scale`` other than 1 raises ValueError)."""
         self._no_takes(takes)
+        self._no_guidance(guidance_scale, "streaming synthesis")
         if self._is_quantized_model:  # kept for signature parity; never true on this build
             raise NotImplementedError("GGUF streaming is not part of the H100 build")
         ctl = _controls(1, temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
@@ -608,7 +690,7 @@ class NeuTTS:
     def infer_stream_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], *, temperature=1.0,
                            top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0,
                            penalize_prompt=True, takes: int = 1, min_new_tokens=50,
-                           exponential_decay_length_penalty=None) -> Generator[list, None, None]:
+                           exponential_decay_length_penalty=None, guidance_scale=1.0) -> Generator[list, None, None]:
         """Streaming synthesis of many utterances at once (BASELINE.json configs[4]; the reference streams one
         utterance, ``neutts/neutts.py:373-465``).  Every yield is a list with one entry per utterance, as many entries
         as ``texts``: the next audio chunk (float32, cross-faded exactly as in ``infer_stream``) or ``None`` when that
@@ -624,8 +706,9 @@ class NeuTTS:
         closed early.
 
         Streaming returns no per-token log-probabilities (``infer_batch``'s ``return_logprobs``) and generates one take
-        per utterance (``takes`` other than 1 raises ValueError)."""
+        per utterance (``takes`` other than 1 raises ValueError); ``guidance_scale`` other than 1 raises ValueError."""
         self._no_takes(takes)
+        self._no_guidance(guidance_scale, "streaming synthesis")
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
         self._stream_slots(len(texts))

@@ -87,6 +87,7 @@ struct StepSettings {
   bool len_on = false;                // length-control table (nt_lm_set_length_control)
   bool len_decay = false;             // ... and some entry decays (decay_factor != 1): the chain's fix-up launch
   float* logprob_out = nullptr;       // per-token log-probabilities (nt_lm_set_logprobs): nullptr = off
+  bool guide_on = false;              // classifier-free guidance table (nt_lm_set_guidance): per-op chain, combine + follow
 };
 
 struct nt_lm {
@@ -151,6 +152,14 @@ struct nt_lm {
   float* len_c = nullptr;             // [max_batch][max_ctx]
   // host: per slot, the decay start and the largest k with c_1 .. c_k finite in fp32 (checked at every launch)
   std::vector<int> len_start, len_finite;
+  // classifier-free guidance (nt_lm_set_guidance): the slot table, the same table in logits-row order for
+  // nt_lm_prefill_slots, each slot's c (-1 unless it is the u of a pair), and the combine's (max, sum) partials
+  nt_slot_guidance* guide_tab = nullptr;   // [max_batch]
+  nt_slot_guidance* guide_rows = nullptr;  // [max_batch]
+  int* guide_of = nullptr;                 // [max_batch]
+  float2* guide_part = nullptr;            // [max_batch][2][kGuideSplit]
+  std::vector<nt_slot_guidance> guide_host;   // host copies of guide_tab and guide_of while the table is on
+  std::vector<int> guide_of_host;
 };
 
 // The lm_head tiles a launch computes under the vocabulary range: [t_lo, t_hi), plus eos_tile when EOS lies outside
@@ -242,6 +251,10 @@ static size_t lm_carve(const nt_lm_config& c, void* ws, size_t bytes, F&& assign
     (L)->rep_rec = a.take<int>(c.max_batch);                                                   \
     (L)->len_tab = a.take<nt_slot_length>(c.max_batch);                                        \
     (L)->len_c = a.take<float>(size_t(c.max_batch) * c.max_ctx);                               \
+    (L)->guide_tab = a.take<nt_slot_guidance>(c.max_batch);                                    \
+    (L)->guide_rows = a.take<nt_slot_guidance>(c.max_batch);                                   \
+    (L)->guide_of = a.take<int>(c.max_batch);                                                  \
+    (L)->guide_part = a.take<float2>(size_t(c.max_batch) * 2 * kGuideSplit);                   \
   }
 
 static int lm_check_config(const nt_lm_config* c) {
@@ -454,9 +467,28 @@ static int check_length(const nt_lm* lm, const nt_sampling* sp, const int32_t* s
   return NT_OK;
 }
 
-// the tile-max sampler on lm->logits rows [0, B) and the maxima lm_head_rows left in lm->tmax
+// While guidance is on: every pair with a slot among the n rows of a launch (row i holds slot slots[i], or slot i when
+// slots is nullptr) has both slots there.  rows (optional, [n]) receives the table in row order: partner row and scale.
+static int check_guidance(const nt_lm* lm, const int32_t* slots, int n, std::vector<nt_slot_guidance>* rows = nullptr) {
+  if (!lm->step.guide_on) return NT_OK;
+  std::vector<int> row_of(lm->cfg.max_batch, -1);
+  for (int i = 0; i < n; ++i) row_of[slots ? slots[i] : i] = i;
+  if (rows) rows->assign(n, nt_slot_guidance{-1, 0.f});
+  for (int i = 0; i < n; ++i) {
+    const int s = slots ? slots[i] : i, p = lm->guide_host[s].partner, c = lm->guide_of_host[s];
+    if ((p >= 0 && row_of[p] < 0) || (c >= 0 && row_of[c] < 0))
+      return set_error(NT_ERR_INVALID, "slot %d is guided with slot %d, which this call does not include", s, p >= 0 ? p : c);
+    if (rows && p >= 0) (*rows)[i] = nt_slot_guidance{row_of[p], lm->guide_host[s].scale};
+  }
+  return NT_OK;
+}
+
+// the tile-max sampler on lm->logits rows [0, B) and the maxima lm_head_rows left in lm->tmax; while guidance is on,
+// the u slots are skipped and then take their c's token
 static int run_sampler(nt_lm* lm, const SamplerParams& s, int B, cudaStream_t stream) {
-  return launch_sampler_tiles(s, B, lm->tmax, (lm->cfg.vocab_size + 127) / 128, stream);
+  const bool guide = lm->step.guide_on;
+  int rc = launch_sampler_tiles(s, B, lm->tmax, (lm->cfg.vocab_size + 127) / 128, stream, guide ? lm->guide_of : nullptr);
+  return rc || !guide ? rc : launch_guidance_follow(s, B, lm->guide_tab, stream);
 }
 
 // While the repetition penalty is on (and eos >= 0), one fix-up launch after the lm_head rewrites each history logit
@@ -475,8 +507,11 @@ static int rep_fixup(nt_lm* lm, int B, float* logits, float* tmax, int eos, cons
 // the range the lm_head runs once over the range's rows and once over the EOS tile (when EOS lies outside them), each
 // a row slice of the full-vocabulary launch with the same per-row arithmetic, so every computed logit is bit-identical
 // to the range off; the rows it does not compute keep the -inf of vocab_fill.  row_slot: see rep_fixup.
+// guide (eos >= 0, guidance on): the guidance table in row order; the combine rewrites every guided c row (and its tile
+// maxima) before the penalty and the decay see it.
 static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cudaStream_t stream, const SplitK* pend = nullptr,
-                        int eos = -1, const int32_t* row_slot = nullptr, const SamplerParams* decay = nullptr) {
+                        int eos = -1, const int32_t* row_slot = nullptr, const SamplerParams* decay = nullptr,
+                        const nt_slot_guidance* guide = nullptr) {
   const nt_lm_config& c = lm->cfg;
   const int V = c.vocab_size, nt = (V + 127) / 128;
   const VocabTiles vt = eos >= 0 ? vocab_tiles(lm, eos) : VocabTiles{false, 0, nt, -1};
@@ -515,6 +550,7 @@ static int lm_head_rows(nt_lm* lm, const float* hrows, int B, float* logits, cud
     }
   }
   if (vt.eos_tile >= 0 && (rc = launch_vocab_eos_tile(logits, B, V, eos, tmax, nt, stream))) return rc;
+  if (guide && eos >= 0 && (rc = launch_guidance_combine(logits, B, V, guide, lm->guide_part, tmax, nt, stream))) return rc;
   if ((rc = rep_fixup(lm, B, logits, tmax, eos, row_slot, stream))) return rc;
   if (decay && eos >= 0 && lm->step.len_decay && (rc = launch_len_decay(*decay, B, logits, tmax, nt, stream))) return rc;
   // no epilogue maxima: the raw maxima of the finished rows (after the EOS tile, the penalty and the decay), as the
@@ -632,9 +668,10 @@ static int prefill_layers(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, 
 }
 
 // Prompt rows -> KV cache + last-position logits in lm->logits (and logits_out).  table: see layers_gemm.
-// row_slot: the slot of every prompt row; it fills that slot's repetition-penalty history.
+// row_slot: the slot of every prompt row; it fills that slot's repetition-penalty history.  guide: see lm_head_rows.
 static int prefill_forward(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, int B, int max_len,
-                           const int32_t* table, float* logits_out, int eos, cudaStream_t stream, const int32_t* row_slot) {
+                           const int32_t* table, float* logits_out, int eos, cudaStream_t stream, const int32_t* row_slot,
+                           const nt_slot_guidance* guide) {
   const nt_lm_config& c = lm->cfg;
   int rc;
   if ((rc = vocab_fill(lm, B, stream))) return rc;
@@ -643,7 +680,7 @@ static int prefill_forward(nt_lm* lm, const nt_lm_state* st, const int32_t* ids,
     return rc;
   if ((rc = prefill_layers(lm, st, ids, cu, B, max_len, table, stream))) return rc;
   if ((rc = launch_gather_rows(lm->h, lm->last_rows, B, c.hidden, lm->h_last, stream))) return rc;
-  if ((rc = lm_head_rows(lm, lm->h_last, B, lm->logits, stream, nullptr, eos, row_slot))) return rc;
+  if ((rc = lm_head_rows(lm, lm->h_last, B, lm->logits, stream, nullptr, eos, row_slot, nullptr, guide))) return rc;
   if (logits_out)
     NT_CUDA_CHECK(cudaMemcpyAsync(logits_out, lm->logits, size_t(B) * c.vocab_size * sizeof(float), cudaMemcpyDeviceToDevice, stream));
   return NT_OK;
@@ -675,16 +712,22 @@ extern "C" int nt_lm_prefill_slots(nt_lm* lm, const nt_lm_state* st, const int32
     args[i] = slots[i], args[B + i] = stream_ids[i];
   }
   if ((rc = check_length(lm, sp, slots, B))) return rc;
+  std::vector<nt_slot_guidance> grows;
+  if ((rc = check_guidance(lm, slots, B, &grows))) return rc;
   std::vector<int> lens;
   int max_len = 0;
   if ((rc = prefill_stage(lm, cu, B, lens, max_len, stream))) return rc;
   for (int i = 0; i < B; ++i) args[2 * B + i] = lens[i];
+  if (lm->step.guide_on)   // pageable source: the runtime has staged it by the time the call returns
+    NT_CUDA_CHECK(cudaMemcpyAsync(lm->guide_rows, grows.data(), B * sizeof(nt_slot_guidance), cudaMemcpyHostToDevice, stream));
   NT_CUDA_CHECK(cudaMemcpyAsync(lm->slot_args, args.data(), args.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
   const int max_pages = c.max_ctx / c.page_size;
   if ((rc = launch_slots_setup(lm->slot_args, B, st->page_table, max_pages, lm->slot_table, st->seq_lens, st->n_generated, st->done,
                                lm->slot_key, stream)))
     return rc;
-  if ((rc = prefill_forward(lm, st, ids, cu, B, max_len, lm->slot_table, logits_out, sp->eos_id, stream, lm->slot_args))) return rc;
+  if ((rc = prefill_forward(lm, st, ids, cu, B, max_len, lm->slot_table, logits_out, sp->eos_id, stream, lm->slot_args,
+                             lm->step.guide_on ? lm->guide_rows : nullptr)))
+    return rc;
   SamplerParams s = make_sampler(lm, st, sp);
   s.row_slot = lm->slot_args;
   s.h = nullptr;  // the residual rows are rebuilt below, for every slot
@@ -698,8 +741,9 @@ extern "C" int nt_lm_prefill_slots(nt_lm* lm, const nt_lm_state* st, const int32
 // already names the parent's full prompt pages (the caller shares them), so only the partly filled last prompt page
 // is copied into the child's own page, together with the parent's repetition-penalty history.  The sampler then
 // draws every take from its parent's logits row (row_src), with the take's own slot state and Philox stream.
-extern "C" int nt_lm_prefill_fork(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, int B, int n,
-                                  const nt_sampling* sp, float* logits_out, void* stream_) {
+// While guidance is on this serves nt_lm_prefill only (n = 1, row b = slot b), and the pairs are checked there.
+static int prefill_fork(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, int B, int n,
+                        const nt_sampling* sp, float* logits_out, void* stream_) {
   if (!lm || !st || !ids || !cu) return set_error(NT_ERR_INVALID, "nt_lm_prefill_fork: null argument");
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const nt_lm_config& c = lm->cfg;
@@ -730,7 +774,9 @@ extern "C" int nt_lm_prefill_fork(nt_lm* lm, const nt_lm_state* st, const int32_
   if ((rc = launch_slots_setup(lm->slot_args, B, st->page_table, max_pages, lm->slot_table, st->seq_lens, st->n_generated, st->done,
                                lm->slot_key, stream)))
     return rc;
-  if ((rc = prefill_forward(lm, st, ids, cu, B, max_len, lm->slot_table, logits_out, sp->eos_id, stream, lm->slot_args))) return rc;
+  if ((rc = prefill_forward(lm, st, ids, cu, B, max_len, lm->slot_table, logits_out, sp->eos_id, stream, lm->slot_args,
+                             lm->step.guide_on ? lm->guide_tab : nullptr)))
+    return rc;
   if ((rc = launch_fork_tails(lm->fork_args + N, nc, make_kv(lm, st), c.n_layers, lm->step.rep_on ? lm->rep_hist : nullptr,
                               lm->rep_words, lm->rep_rec, stream)))
     return rc;
@@ -741,12 +787,19 @@ extern "C" int nt_lm_prefill_fork(nt_lm* lm, const nt_lm_state* st, const int32_
   return NT_OK;
 }
 
+extern "C" int nt_lm_prefill_fork(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, int B, int n,
+                                  const nt_sampling* sp, float* logits_out, void* stream_) {
+  if (lm && lm->step.guide_on) return set_error(NT_ERR_INVALID, "nt_lm_prefill_fork: not available while guidance is on");
+  return prefill_fork(lm, st, ids, cu, B, n, sp, logits_out, stream_);
+}
+
 // One take of each prompt: slot b holds prompt b, with no children to copy tails to and no row_src.
 extern "C" int nt_lm_prefill(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, const int32_t* cu, int B,
                              const nt_sampling* sp, float* logits_out, void* stream_) {
   if (!lm || !st || !ids || !cu) return set_error(NT_ERR_INVALID, "nt_lm_prefill: null argument");
   if (B < 1 || B > lm->cfg.max_batch) return set_error(NT_ERR_INVALID, "batch %d not in 1..%d", B, lm->cfg.max_batch);
-  return nt_lm_prefill_fork(lm, st, ids, cu, B, 1, sp, logits_out, stream_);
+  if (int rc = check_guidance(lm, nullptr, B)) return rc;
+  return prefill_fork(lm, st, ids, cu, B, 1, sp, logits_out, stream_);
 }
 
 // Teacher-forced scoring.  The caller's scratch holds, for one block of R scored rows, the (max, sum exp) pair of every
@@ -871,7 +924,8 @@ static int decode_step(nt_lm* lm, const nt_lm_state* st, int B, const nt_samplin
   }
   SamplerParams s = make_sampler(lm, st, sp);
   s.advance = 1;
-  if ((rc = lm_head_rows(lm, lm->h, B, lm->logits, stream, &tail, sp->eos_id, nullptr, &s))) return rc;
+  if ((rc = lm_head_rows(lm, lm->h, B, lm->logits, stream, &tail, sp->eos_id, nullptr, &s, lm->step.guide_on ? lm->guide_tab : nullptr)))
+    return rc;
   return run_sampler(lm, s, B, stream);
 }
 
@@ -885,6 +939,7 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
   int rc = check_sampling(lm, st, sp);
   if (rc) return rc;
   if ((rc = check_length(lm, sp, nullptr, B))) return rc;
+  if ((rc = check_guidance(lm, nullptr, B))) return rc;
   if (n_steps < 0) return set_error(NT_ERR_INVALID, "negative step count");
 
   // NT_DECODE_IMPL = tc (persistent wgmma kernel) | perop (per-op kernel chain).  Unset: the persistent kernel up to
@@ -896,7 +951,10 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
     if (strcmp(impl, "tc") && strcmp(impl, "perop"))
       return set_error(NT_ERR_INVALID, "NT_DECODE_IMPL=%s: valid values are tc and perop", impl);
     want_tc = impl[0] == 't';
+    if (want_tc && lm->step.guide_on)
+      return set_error(NT_ERR_INVALID, "NT_DECODE_IMPL=tc: the persistent decode kernel does not run classifier-free guidance");
   }
+  if (lm->step.guide_on) want_tc = false;   // guidance runs on the per-op chain at every batch
   if (n_steps == 0) return NT_OK;
   if ((rc = vocab_fill(lm, B, stream))) return rc;   // once per launch: no step writes a suppressed row or tile maximum
   const int tc_layers = lm->step.debug_layers >= 0 ? lm->step.debug_layers : c.n_layers;
@@ -961,8 +1019,8 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
     return NT_OK;
   }
   // The graph is keyed by every input decode_step bakes into its launches: the batch, the state and sampling params,
-  // and the host settings in lm->step.  The slot_sp / rep_tab / len_tab contents stay out: the graph reads them at
-  // replay.
+  // and the host settings in lm->step.  The slot_sp / rep_tab / len_tab / guide_tab contents stay out: the graph reads
+  // them at replay.
   // prof / prof_step stay out: only the persistent kernel reads them, and it never runs from the graph.
   std::vector<uint8_t> key(sizeof(int) + sizeof(nt_lm_state) + sizeof(nt_sampling) + sizeof(StepSettings));
   uint8_t* k = key.data();
@@ -1098,6 +1156,36 @@ extern "C" int nt_lm_set_length_control(nt_lm* lm, const nt_slot_length* table, 
   }
   lm->step.len_on = on;
   lm->step.len_decay = decays;
+  return NT_OK;
+}
+
+extern "C" int nt_lm_set_guidance(nt_lm* lm, const nt_slot_guidance* table, void* stream_) {
+  if (!lm) return set_error(NT_ERR_INVALID, "nt_lm_set_guidance: null handle");
+  const int S = lm->cfg.max_batch;
+  const bool on = table != nullptr;
+  if (on) {
+    std::vector<int> of(S, -1);
+    for (int s = 0; s < S; ++s) {
+      const nt_slot_guidance& e = table[s];
+      if (e.partner < -1 || e.partner >= S || e.partner == s)
+        return set_error(NT_ERR_INVALID, "slot %d: partner %d must be -1 or another slot in 0..%d", s, e.partner, S - 1);
+      if (e.partner < 0) continue;
+      if (!(std::isfinite(e.scale) && e.scale > 0.f && e.scale != 1.f))
+        return set_error(NT_ERR_INVALID, "slot %d: guidance scale %g must be finite, > 0 and != 1", s, e.scale);
+      if (of[e.partner] >= 0)
+        return set_error(NT_ERR_INVALID, "slot %d is the partner of both slot %d and slot %d", e.partner, of[e.partner], s);
+      if (table[e.partner].partner >= 0)
+        return set_error(NT_ERR_INVALID, "slot %d: its partner %d has a partner of its own", s, e.partner);
+      of[e.partner] = s;
+    }
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    // pageable sources: the runtime has staged them by the time the calls return
+    NT_CUDA_CHECK(cudaMemcpyAsync(lm->guide_tab, table, size_t(S) * sizeof(nt_slot_guidance), cudaMemcpyHostToDevice, stream));
+    NT_CUDA_CHECK(cudaMemcpyAsync(lm->guide_of, of.data(), size_t(S) * sizeof(int), cudaMemcpyHostToDevice, stream));
+    lm->guide_host.assign(table, table + S);
+    lm->guide_of_host = of;
+  }
+  lm->step.guide_on = on;
   return NT_OK;
 }
 

@@ -682,7 +682,8 @@ struct NoMarkI {
   NT_DEVINL void operator()(int) const {}
 };
 constexpr unsigned kTilesScratch = 96 * 1024;
-__global__ void __launch_bounds__(kConsumerThreads) topk_tiles_kernel(const SamplerParams p, const float* tmax, const int nt) {
+__global__ void __launch_bounds__(kConsumerThreads) topk_tiles_kernel(const SamplerParams p, const float* tmax, const int nt,
+                                                                      const int32_t* skip) {
   extern __shared__ uint8_t tiles_raw[];
   uint8_t* uni = tiles_raw + ((1024u - (smem_u32(tiles_raw) & 1023u)) & 1023u);
   __shared__ int sel[8];
@@ -691,6 +692,7 @@ __global__ void __launch_bounds__(kConsumerThreads) topk_tiles_kernel(const Samp
   pdl_wait();
   const int b = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int slot = p.row_slot ? __ldg(p.row_slot + b) : b;
+  if (skip && __ldg(skip + slot) >= 0) return;   // CTA-uniform: an unconditional slot of a guided pair
   const int src = p.row_src ? __ldg(p.row_src + b) : -1;   // logits / tile-maxima row (-1: row b)
   const bool stateless = p.n_generated_override != nullptr;
   const int ngen = stateless ? __ldcg(p.n_generated_override + b) : __ldcg(p.n_generated + slot);
@@ -716,10 +718,10 @@ __global__ void __launch_bounds__(kConsumerThreads) topk_tiles_kernel(const Samp
                    static_cast<float2*>(nullptr), 0.f, stateless, slot, src);
 }
 
-int launch_sampler_tiles(const SamplerParams& p, int B, const float* tmax, int nt, cudaStream_t stream) {
+int launch_sampler_tiles(const SamplerParams& p, int B, const float* tmax, int nt, cudaStream_t stream, const int32_t* skip) {
   if (int rc0 = launch_sampler_check(p)) return rc0;
   const int smem = int(kTilesScratch) + 1024;
-  return launch_kernel(topk_tiles_kernel, dim3(B), dim3(kConsumerThreads), smem, stream, true, p, tmax, nt);
+  return launch_kernel(topk_tiles_kernel, dim3(B), dim3(kConsumerThreads), smem, stream, true, p, tmax, nt, skip);
 }
 
 // =================================================================================== vocabulary range
@@ -844,6 +846,152 @@ __global__ void len_decay_kernel(const SamplerParams p, float* logits, float* tm
 }
 int launch_len_decay(const SamplerParams& p, int B, float* logits, float* tmax, int nt, cudaStream_t s) {
   return launch_kernel(len_decay_kernel, dim3(B), dim3(128), 0, s, true, p, logits, tmax, nt);
+}
+
+// =================================================================================== classifier-free guidance
+// Online log-sum-exp in fp32 with the accurate expf: a (max, sum exp(x - max)) pair per thread, merged in a fixed order.
+NT_DEVINL void lse_add(float& m, float& s, float x) {
+  if (x > m) {
+    s = s * expf(m - x) + 1.f;
+    m = x;
+  } else if (x > -INFINITY) {
+    s += expf(x - m);
+  }
+}
+NT_DEVINL void lse_merge(float& m, float& s, float m1, float s1) {
+  const float mm = fmaxf(m, m1);
+  s = mm == -INFINITY ? 0.f : s * expf(m - mm) + s1 * expf(m1 - mm);
+  m = mm;
+}
+// the 4 ids r0 .. r0 + 3 of one row (a float4 where the row is 16-byte aligned there; ids >= V read -inf)
+NT_DEVINL float4 load4(const float* lg, int r0, int V) {
+  if ((reinterpret_cast<uintptr_t>(lg + r0) & 15) == 0 && r0 + 3 < V) return __ldcg(reinterpret_cast<const float4*>(lg + r0));
+  float v[4];
+  for (int q = 0; q < 4; ++q) v[q] = r0 + q < V ? __ldcg(lg + r0 + q) : -INFINITY;
+  return make_float4(v[0], v[1], v[2], v[3]);
+}
+// the tiles [t0, t1) of CTA x when nt tiles are shared by kGuideSplit CTAs
+NT_DEVINL void guide_chunk(int nt, int x, int& t0, int& t1) {
+  const int per = (nt + kGuideSplit - 1) / kGuideSplit;
+  t0 = min(nt, x * per), t1 = min(nt, t0 + per);
+}
+
+// grid (kGuideSplit, B, 2), 256 threads: CTA (x, r, z) folds its share of the tiles of row r (z = 0) or of r's partner
+// (z = 1) into part[r][z][x]; a warp takes one 128-id tile at a time, a lane 4 ids.
+__global__ void __launch_bounds__(256) guidance_lse_kernel(const float* logits, int V, const nt_slot_guidance* tab, float2* part, int nt) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int r = blockIdx.y, u = __ldg(&tab[r].partner);
+  if (u < 0) return;
+  const float* lg = logits + static_cast<long long>(blockIdx.z ? u : r) * V;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  int t0, t1;
+  guide_chunk(nt, blockIdx.x, t0, t1);
+  float m = -INFINITY, s = 0.f;
+  for (int t = t0 + warp; t < t1; t += 8) {
+    const float4 v = load4(lg, t * 128 + 4 * lane, V);
+    lse_add(m, s, v.x), lse_add(m, s, v.y), lse_add(m, s, v.z), lse_add(m, s, v.w);
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) lse_merge(m, s, __shfl_xor_sync(0xffffffffu, m, off), __shfl_xor_sync(0xffffffffu, s, off));
+  __shared__ float2 red[8];
+  if (lane == 0) red[warp] = make_float2(m, s);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    m = -INFINITY, s = 0.f;
+    for (int w = 0; w < 8; ++w) lse_merge(m, s, red[w].x, red[w].y);
+    part[(static_cast<long long>(r) * 2 + blockIdx.z) * kGuideSplit + blockIdx.x] = make_float2(m, s);
+  }
+}
+
+// grid (kGuideSplit, B), 256 threads: CTA (x, r) folds both rows' partials in index order (every CTA of the row gets
+// the same log-sum-exps), then rewrites its share of c row r and the tile maxima.
+__global__ void __launch_bounds__(256) guidance_mix_kernel(float* logits, int V, const nt_slot_guidance* tab, const float2* part,
+                                                           float* tmax, int nt) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int r = blockIdx.y, u = __ldg(&tab[r].partner);
+  if (u < 0) return;
+  __shared__ float lse[2];
+  if (threadIdx.x < 2) {
+    const float2* pr = part + (static_cast<long long>(r) * 2 + threadIdx.x) * kGuideSplit;
+    float m = -INFINITY, s = 0.f;
+    for (int x = 0; x < kGuideSplit; ++x) {
+      const float2 v = __ldcg(pr + x);
+      lse_merge(m, s, v.x, v.y);
+    }
+    lse[threadIdx.x] = m + logf(s);
+  }
+  __syncthreads();
+  const float lse_c = lse[0], lse_u = lse[1], g = __ldg(&tab[r].scale);
+  float* lc = logits + static_cast<long long>(r) * V;
+  const float* lu = logits + static_cast<long long>(u) * V;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  int t0, t1;
+  guide_chunk(nt, blockIdx.x, t0, t1);
+  for (int t = t0 + warp; t < t1; t += 8) {
+    const int r0 = t * 128 + 4 * lane;
+    const float4 c4 = load4(lc, r0, V), u4 = load4(lu, r0, V);
+    const float xc[4] = {c4.x, c4.y, c4.z, c4.w}, xu[4] = {u4.x, u4.y, u4.z, u4.w};
+    float y[4], mx = -INFINITY;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      // transformers' `g * (scores - uncond) + uncond` on the log-softmaxes, unfused; a suppressed id stays -inf
+      // (g * (-inf - -inf) would be NaN)
+      const float ls_u = __fsub_rn(xu[q], lse_u);
+      y[q] = (xc[q] == -INFINITY || xu[q] == -INFINITY) ? -INFINITY
+                                                        : __fadd_rn(__fmul_rn(g, __fsub_rn(__fsub_rn(xc[q], lse_c), ls_u)), ls_u);
+      mx = fmaxf(mx, y[q]);
+    }
+    if ((reinterpret_cast<uintptr_t>(lc + r0) & 15) == 0 && r0 + 3 < V) {
+      *reinterpret_cast<float4*>(lc + r0) = make_float4(y[0], y[1], y[2], y[3]);
+    } else {
+      for (int q = 0; q < 4; ++q)
+        if (r0 + q < V) lc[r0 + q] = y[q];
+    }
+    mx = warp_max(mx);
+    if (tmax && lane == 0) tmax[static_cast<long long>(r) * nt + t] = mx;
+  }
+}
+
+int launch_guidance_combine(float* logits, int B, int V, const nt_slot_guidance* tab, float2* part, float* tmax, int nt,
+                            cudaStream_t s) {
+  int rc = launch_kernel(guidance_lse_kernel, dim3(kGuideSplit, B, 2), dim3(256), 0, s, true, static_cast<const float*>(logits), V, tab,
+                         part, nt);
+  return rc ? rc : launch_kernel(guidance_mix_kernel, dim3(kGuideSplit, B), dim3(256), 0, s, true, logits, V, tab,
+                                 static_cast<const float2*>(part), tmax, nt);
+}
+
+// grid B, 256 threads: CTA i mirrors the sampler's state update of row i's slot onto its partner
+__global__ void __launch_bounds__(256) guidance_follow_kernel(const SamplerParams p, const nt_slot_guidance* tab) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int c = p.row_slot ? __ldg(p.row_slot + blockIdx.x) : static_cast<int>(blockIdx.x);
+  const int u = __ldg(&tab[c].partner);
+  if (u < 0) return;
+  __shared__ int s_tok;
+  if (threadIdx.x == 0) {
+    s_tok = -1;
+    if (!__ldcg(p.done + u)) {
+      const int n = __ldcg(p.n_generated + c), tok = __ldcg(p.cur_token + c);
+      p.out_tokens[static_cast<long long>(u) * p.max_new + n - 1] = tok;
+      p.n_generated[u] = n;
+      p.cur_token[u] = tok;
+      const int cached = __ldcg(p.seq_lens + u) + p.advance;
+      p.seq_lens[u] = cached;
+      int d = __ldcg(p.done + c);
+      if (cached + 1 >= p.max_ctx) p.done[c] = d = 1;
+      p.done[u] = d;
+      s_tok = tok;
+    }
+  }
+  __syncthreads();
+  if (s_tok < 0 || !p.h) return;
+  const __nv_bfloat16* e = p.embed + static_cast<long long>(s_tok) * p.hidden;
+  for (int i = threadIdx.x; i < p.hidden; i += blockDim.x) p.h[static_cast<long long>(u) * p.hidden + i] = __bfloat162float(e[i]);
+}
+int launch_guidance_follow(const SamplerParams& p, int B, const nt_slot_guidance* tab, cudaStream_t s) {
+  return launch_kernel(guidance_follow_kernel, dim3(B), dim3(256), 0, s, true, p, tab);
 }
 
 // =================================================================================== prefill helpers

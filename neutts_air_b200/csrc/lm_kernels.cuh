@@ -121,8 +121,11 @@ struct SamplerParams {
 };
 int launch_sampler_check(const SamplerParams& p);
 // tmax: [B][nt] RAW maxima of the 128-column tiles of p.logits (GEMM epilogue, gemm_dispatch(..., tile_max), or
-// launch_tile_max).  p.n_generated_override set: stateless (nt_op_topk_sample).
-int launch_sampler_tiles(const SamplerParams& p, int B, const float* tmax, int nt, cudaStream_t stream);
+// launch_tile_max).  p.n_generated_override set: stateless (nt_op_topk_sample).  skip (optional, [max_batch]): rows
+// whose slot s has skip[s] >= 0 are not sampled (the unconditional slots of guided pairs; launch_guidance_follow
+// writes their state).
+int launch_sampler_tiles(const SamplerParams& p, int B, const float* tmax, int nt, cudaStream_t stream,
+                         const int32_t* skip = nullptr);
 // tmax [B][ceil(V / 128)] = the raw maximum of every 128-column tile of logits rows [0, B)
 int launch_tile_max(const float* logits, int B, int V, float* tmax, cudaStream_t s);
 size_t sampler_scratch_floats(int B);  // per-array element count for cand_val / cand_idx
@@ -145,6 +148,21 @@ int launch_rep_penalty(float* logits, int B, int V, const uint32_t* hist, int wo
 // n_generated, the EOS logit becomes s + |s| c_k and the raw maximum of the EOS tile in tmax [B][nt] (optional) is
 // recomputed.  p supplies V, eos_id, n_generated and the length-control pointers.
 int launch_len_decay(const SamplerParams& p, int B, float* logits, float* tmax, int nt, cudaStream_t s);
+// Classifier-free guidance (nt_lm_set_guidance).  launch_guidance_combine: tab holds one entry per logits row r < B of
+// `logits` [B][V]; where tab[r].partner = u >= 0 (row r is a guided c row, row u its unconditional partner), row r
+// becomes g * (ls_c - ls_u) + ls_u in fp32, in that order (g = tab[r].scale, ls = x - log-sum-exp of the row), and -inf
+// where either logit is -inf; tmax (optional, [B][nt]) receives the raw maximum of every tile of the new row.  Two
+// launches: kGuideSplit CTAs per row fold (max, sum exp) partials into part [B][2][kGuideSplit], then kGuideSplit CTAs
+// per c row fold those in index order and rewrite their share of the tiles.  No float atomics: reruns are
+// bit-identical.
+constexpr int kGuideSplit = 32;
+int launch_guidance_combine(float* logits, int B, int V, const nt_slot_guidance* tab, float2* part, float* tmax, int nt,
+                            cudaStream_t s);
+// launch_guidance_follow, after the sampler: for each sample row i < B whose slot c (p.row_slot[i], or i) has a partner
+// slot u in the slot table tab, u takes c's new token unless it is finished already: out_tokens, cur_token and
+// n_generated mirror c's, seq_lens[u] += p.advance, done[u] = done[c], and (p.h set) residual row u = embed[token].  If
+// u's context would reach max_ctx, both slots finish, the rule the sampler applies to c's own context.
+int launch_guidance_follow(const SamplerParams& p, int B, const nt_slot_guidance* tab, cudaStream_t s);
 
 int launch_embed_rows(const __nv_bfloat16* embed, const int32_t* ids, int T, int hidden, float* h, cudaStream_t s);
 // parts != nullptr: x is updated in place first (x += sum of nparts split-K slices, slice order) -- see SplitK.

@@ -367,6 +367,95 @@ def per_prompt_length(n: int, min_new_tokens, decay, max_new: int | None = None)
             for m, d in zip(floors, decays)]
 
 
+NO_GUIDANCE = (-1, 1.0)   # (partner, scale) of a slot outside every guided pair
+
+
+def check_guidance_scale(scale) -> float:
+    """One prompt's ``guidance_scale``: a number, finite and > 0 in fp32 (the value the library stores) -> float.
+    1 means no guidance, as in transformers, which adds no processor then."""
+    if isinstance(scale, bool) or not isinstance(scale, (int, float, np.integer, np.floating)):
+        raise ValueError(f"guidance_scale {scale!r} must be a number")
+    g = float(scale)
+    with np.errstate(over="ignore"):
+        f = float(np.float32(g)) if math.isfinite(g) else g
+    if not (math.isfinite(f) and f > 0):
+        raise ValueError(f"guidance_scale {scale} must be finite and > 0")
+    return g if f != 1.0 else 1.0
+
+
+def check_guidance_table(table, max_batch: int) -> list:
+    """A whole slot table of (partner, scale) entries, validated as ``nt_lm_set_guidance`` does -> a list of
+    (int, float): partner -1 or another slot in 0..max_batch - 1; a partner serves one slot and has no partner of its
+    own; scale finite, > 0 and != 1 (in fp32) wherever partner >= 0."""
+    table = [(int(p), float(g)) for p, g in table]
+    if len(table) != max_batch:
+        raise ValueError(f"the guidance table needs {max_batch} entries, got {len(table)}")
+    served = {}
+    for s, (p, g) in enumerate(table):
+        if not (p == -1 or (0 <= p < max_batch and p != s)):
+            raise ValueError(f"slot {s}: partner {p} must be -1 or another slot in 0..{max_batch - 1}")
+        if p < 0:
+            continue
+        if check_guidance_scale(g) == 1.0:
+            raise ValueError(f"slot {s}: guidance scale {g} must be != 1")
+        if p in served:
+            raise ValueError(f"slot {p} is the partner of both slot {served[p]} and slot {s}")
+        if table[p][0] >= 0:
+            raise ValueError(f"slot {s}: its partner {p} has a partner of its own")
+        served[p] = s
+    return table
+
+
+def per_prompt_guidance(prompts, guidance_scale, negative_prompt_ids):
+    """Guidance of the prompts: ``guidance_scale`` a number or one per prompt, ``negative_prompt_ids`` None or one id
+    list per prompt (None entries: transformers' default, the prompt's last token).  Returns None when no prompt is
+    guided (scale 1), else one (scale, negative prompt) per prompt, (1.0, None) for an unguided one."""
+    n = len(prompts)
+    scales = per_item(n, "prompt", guidance_scale=guidance_scale)["guidance_scale"]
+    scales = [check_guidance_scale(g) for g in (scales if isinstance(scales, list) else [scales] * n)]
+    if negative_prompt_ids is None:
+        negs = [None] * n
+    elif isinstance(negative_prompt_ids, (list, tuple)) and len(negative_prompt_ids) == n:
+        negs = [None if q is None else [int(t) for t in (q.tolist() if hasattr(q, "tolist") else q)]
+                for q in negative_prompt_ids]
+    else:
+        raise ValueError(f"negative_prompt_ids must be None or one id list per prompt ({n})")
+    if all(g == 1.0 for g in scales):
+        return None
+    out = []
+    for p, g, q in zip(prompts, scales, negs):
+        if g == 1.0:
+            out.append((1.0, None))
+            continue
+        if q is not None and len(q) == 0:
+            raise ValueError("an empty negative prompt gives the unconditional sequence nothing to start from")
+        out.append((g, list(q) if q is not None else [int(p[-1])]))
+    return out
+
+
+def guided_layout(n: int, guidance) -> list:
+    """(c slot, u slot, scale) of every guided prompt of a batch: prompt i in slot i, the unconditional sequences in
+    slots n, n + 1, ... in prompt order, so that unguided prompts keep their slots and Philox streams."""
+    if guidance is None:
+        return []
+    pairs = [(i, g) for i, (g, _) in enumerate(guidance) if g != 1.0]
+    return [(i, n + k, g) for k, (i, g) in enumerate(pairs)]
+
+
+def guided_caps(caps, guidance, max_ctx: int) -> list:
+    """The generated-token cap of every prompt with guidance: a guided pair stops together, so its cap is
+    min(c's cap, max_ctx - len(negative prompt)).  A negative prompt that leaves no room raises ValueError."""
+    out = list(caps)
+    for i, (g, neg) in enumerate(guidance or []):
+        if g == 1.0:
+            continue
+        room = max_ctx - len(neg)
+        if room < 1:
+            raise ValueError(f"prompt {i}: its negative prompt of {len(neg)} tokens leaves no room in the context of {max_ctx}")
+        out[i] = min(out[i], room)
+    return out
+
+
 @dataclass
 class Settings:
     """The per-prompt generation settings of one call, resolved and validated before any engine call
@@ -380,6 +469,8 @@ class Settings:
     logprobs: bool = False     # per-token log-probabilities on (``SpeechLM.set_logprobs``)
     length: list | None = None # one (min_new_tokens, decay_start, decay_factor) per prompt; None: the launch scalar
     min_new_tokens: int = 50   # the launch scalar, row 0's while the length table is on
+    guidance: list | None = None  # one (partner slot, scale) per slot of the prefill (NO_GUIDANCE outside a pair);
+                                  # None: guidance off
 
     def floors(self, n: int) -> list:
         """The min_new_tokens of each of the n prompts."""
@@ -401,6 +492,24 @@ class Settings:
             lm.set_length_control(None if self.length is None else self.length[:n])
         if self.logprobs != (getattr(lm, "logprobs", None) is not None):
             lm.set_logprobs(self.logprobs)
+        if self.guidance is not None:   # the whole table: no pair of an earlier call survives
+            lm.set_guidance(self.guidance[:n] + [NO_GUIDANCE] * (lm.max_batch - n))
+        elif getattr(lm, "_guidance_host", None) is not None:
+            lm.set_guidance(None)
+
+    def pair(self, pairs) -> "Settings":
+        """The settings of a batch with guided pairs ((c, u, scale) from ``guided_layout``): the u slots, above the
+        prompts in pair order, repeat their c's rows (they are never sampled, but every launch checks their entries),
+        and ``guidance`` holds the table of every slot."""
+        if not pairs:
+            return self
+        n = pairs[0][1]
+        rows = lambda r: None if r is None else list(r) + [r[c] for c, _, _ in pairs]
+        table = [NO_GUIDANCE] * (n + len(pairs))
+        for c, u, g in pairs:
+            table[c] = (u, g)
+        return dataclasses.replace(self, controls=rows(self.controls), penalty=rows(self.penalty), length=rows(self.length),
+                                   guidance=table)
 
     def repeat(self, n: int) -> "Settings":
         """The settings of n takes of every prompt: each prompt's row repeated n times, in slot order (take j of prompt
@@ -408,15 +517,18 @@ class Settings:
         rows = lambda r: None if r is None else [x for x in r for _ in range(n)]
         return dataclasses.replace(self, controls=rows(self.controls), penalty=rows(self.penalty), length=rows(self.length))
 
-    def admit(self, lm, slots, idx) -> None:
+    def admit(self, lm, slots, idx, guide=None) -> None:
         """Before a refill of prompts ``idx`` into ``slots``: writes their rows; every other slot keeps its own, and
-        the range holds."""
+        the range holds.  ``guide`` (queue with guidance): {slot: (partner, scale)} for the refilled slots (a pair's u
+        slot is in ``slots`` with its prompt's index repeated in ``idx``) and every slot freed since the last refill."""
         if self.controls is not None:
             lm.set_slot_sampling([self.controls[i] for i in idx], slots=slots)
         if self.penalty is not None:
             lm.set_repetition_penalty([self.penalty[i] for i in idx], slots=slots)
         if self.length is not None:
             lm.set_length_control([self.length[i] for i in idx], slots=slots)
+        if guide is not None:
+            lm.set_guidance(list(guide.values()), slots=list(guide))
 
 
 def resolve_settings(lm, n: int, temperature=1.0, top_k=50, top_p=1.0, min_p=0.0, vocab_range=None,
@@ -518,6 +630,7 @@ class SpeechLM:
         self._penalty_host = None   # host mirror of the per-slot repetition penalties (None: off)
         self._length_host = None    # host mirror of the per-slot length control (None: off)
         self.logprobs = None        # per-token log-probabilities, [max_batch][max_new][2] on the device (None: off)
+        self._guidance_host = None  # host mirror of the guidance table (None: off)
 
     def __del__(self):
         try:
@@ -629,6 +742,31 @@ class SpeechLM:
         self.logprobs = buf
         return buf
 
+    def set_guidance(self, rows, slots=None) -> None:
+        """Classifier-free guidance (transformers' ``guidance_scale`` with ``negative_prompt_ids``).  ``rows``: one
+        (partner, scale) per slot of ``slots`` (default: slots 0..len(rows) - 1); every other slot keeps its entry, or
+        (-1, 1.0) (no partner) when the table was off.  Slot c with partner u >= 0 is guided: at every sampler launch
+        its logits row becomes ``scale * (ls_c - ls_u) + ls_u`` (log-softmaxes) before the penalty, the length control
+        and the warpers, and u, which holds the negative prompt, takes every token c draws and is never sampled.
+        ``None`` switches guidance off.  ``generate_batch`` / ``generate_queue`` leave their table on when they return
+        (the next call's settings replace it); a caller that then prefills or decodes directly switches it off first,
+        or its launches must include both slots of every pair still in the table.  The merged table is validated first (``check_guidance_table``); a bad one
+        raises ValueError and leaves the previous table in force.  Copied on the current stream."""
+        table = arr = None
+        if rows is not None:
+            rows = [(int(p), float(g)) for p, g in rows]
+            slots = list(range(len(rows))) if slots is None else [int(s) for s in slots]
+            if len(slots) != len(rows) or len(set(slots)) != len(slots) or any(not 0 <= s < self.max_batch for s in slots):
+                raise ValueError(f"slots must be distinct, in 0..{self.max_batch - 1} and one per row")
+            table = list(getattr(self, "_guidance_host", None) or [NO_GUIDANCE] * self.max_batch)
+            for s, r in zip(slots, rows):
+                table[s] = r
+            table = check_guidance_table(table, self.max_batch)
+            arr = (_lib.SlotGuidance * self.max_batch)(*(_lib.SlotGuidance(*r) for r in table))
+        with torch.cuda.device(self.device):
+            _lib.check(self.L.nt_lm_set_guidance(self.handle, arr, _lib.current_stream_ptr()))
+        self._guidance_host = table
+
     def _stage_ids(self, prompts) -> torch.Tensor:
         """The prompts' ids, range-checked, back to back in a persistent pinned buffer (so their H2D copy is
         asynchronous)."""
@@ -698,9 +836,13 @@ class SpeechLM:
                 self.page_table.copy_(torch.from_numpy(table))
                 self._table_host = table
             logits = torch.empty(B, self.shape.vocab_size, dtype=torch.float32, device=self.device) if return_logits else None
-            _lib.check(self.L.nt_lm_prefill_fork(self.handle, C.byref(self.state), ids.data_ptr(),
-                                                 cu.ctypes.data_as(C.POINTER(C.c_int32)), B, n, C.byref(sp),
-                                                 logits.data_ptr() if return_logits else None, _lib.current_stream_ptr()))
+            cu_p, lg_p = cu.ctypes.data_as(C.POINTER(C.c_int32)), logits.data_ptr() if return_logits else None
+            if n == 1 and self._guidance_host is not None:   # the fork entry is refused while guidance is on
+                _lib.check(self.L.nt_lm_prefill(self.handle, C.byref(self.state), ids.data_ptr(), cu_p, B, C.byref(sp), lg_p,
+                                                _lib.current_stream_ptr()))
+            else:
+                _lib.check(self.L.nt_lm_prefill_fork(self.handle, C.byref(self.state), ids.data_ptr(), cu_p, B, n,
+                                                     C.byref(sp), lg_p, _lib.current_stream_ptr()))
         self._B = B * n
         return logits
 
@@ -883,9 +1025,15 @@ class SpeechLM:
         lp = self.logprobs[rows].cpu()
         return ids, [lp[r, : int(n)].clone() for r, n in enumerate(ngen)]
 
-    def _prepare(self, prompts, max_length, max_new_tokens, **settings) -> tuple:
+    def _prepare(self, prompts, max_length, max_new_tokens, guidance_scale=1.0, negative_prompt_ids=None, **settings) -> tuple:
         """Shared preamble of ``generate_batch`` / ``generate_queue``, run before any engine call: the max_length
-        checks, the generated-token cap per prompt and the resolved ``settings`` -> (caps, Settings)."""
+        checks, the generated-token cap per prompt and the resolved ``settings`` -> (caps, Settings, guidance), with
+        guidance as ``per_prompt_guidance`` and every guided prompt's cap shortened so its negative prompt fits."""
+        guidance = per_prompt_guidance(prompts, guidance_scale, negative_prompt_ids)
+        caps, st = self._prepare_caps(prompts, max_length, max_new_tokens, **settings)
+        return guided_caps(caps, guidance, self.max_ctx), st, guidance
+
+    def _prepare_caps(self, prompts, max_length, max_new_tokens, **settings) -> tuple:
         max_length = max_length or self.max_ctx
         if max_length > self.max_ctx:
             raise ValueError(f"max_length {max_length} exceeds the engine context {self.max_ctx}")
@@ -902,7 +1050,7 @@ class SpeechLM:
                        greedy: bool = False, forced: torch.Tensor | None = None, check_every: int = 64, slot_base: int = 0,
                        top_p: float = 1.0, min_p: float = 0.0, vocab_range=None, repetition_penalty=1.0,
                        penalize_prompt=True, return_logprobs: bool = False, num_return_sequences: int = 1,
-                       exponential_decay_length_penalty=None):
+                       exponential_decay_length_penalty=None, guidance_scale=1.0, negative_prompt_ids=None):
         """Returns a list of int64 CPU tensors with the generated ids of each prompt (EOS included
         when it was sampled), following transformers' stopping rules (stopping_criteria.py:73-84,
         467-471): stop at EOS or when prompt + generated reaches max_length.  ``max_new_tokens`` may also be a
@@ -918,25 +1066,40 @@ class SpeechLM:
         decay switch the per-slot table on for the call.  ``num_return_sequences`` n > 1: n takes of every prompt from one prefill (``prefill_fork``;
         len(prompts) * n <= max_batch), returned in slot order, take j of prompt i at index i * n + j, each drawing
         from the Philox stream the prompt repeated n times would give it; every per-prompt setting (and cap) applies
-        to all n takes of its prompt, while ``forced`` has one row per take."""
+        to all n takes of its prompt, while ``forced`` has one row per take.
+
+        ``guidance_scale`` (a number or one per prompt; 1 = off) and ``negative_prompt_ids`` (None, or one id list or
+        None per prompt) add classifier-free guidance as transformers' ``UnbatchedClassifierFreeGuidanceLogitsProcessor``
+        (``set_guidance``): prompt i stays in slot i and the unconditional sequence of each guided prompt, its negative
+        prompt (default: the prompt's last token) followed by its draws, takes a slot above the prompts, so
+        len(prompts) + guided prompts <= max_batch.  A guided prompt's cap is at most max_ctx - len(negative prompt).
+        Guidance with ``num_return_sequences`` > 1 raises ValueError."""
         n_takes = check_takes(len(prompts), num_return_sequences, self.max_batch)
-        caps, settings = self._prepare(prompts, max_length, max_new_tokens, temperature=temperature, top_k=top_k,
-                                       top_p=top_p, min_p=min_p, vocab_range=vocab_range,
-                                       repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt,
-                                       logprobs=return_logprobs, min_new_tokens=min_new_tokens,
-                                       exponential_decay_length_penalty=exponential_decay_length_penalty)
+        caps, settings, guidance = self._prepare(
+            prompts, max_length, max_new_tokens, guidance_scale, negative_prompt_ids, temperature=temperature, top_k=top_k,
+            top_p=top_p, min_p=min_p, vocab_range=vocab_range, repetition_penalty=repetition_penalty,
+            penalize_prompt=penalize_prompt, logprobs=return_logprobs, min_new_tokens=min_new_tokens,
+            exponential_decay_length_penalty=exponential_decay_length_penalty)
+        pairs = guided_layout(len(prompts), guidance)
+        if pairs and n_takes > 1:
+            raise ValueError("classifier-free guidance takes one sequence per prompt (num_return_sequences=1)")
+        if len(prompts) + len(pairs) > self.max_batch:
+            raise ValueError(f"{len(prompts)} prompt(s) with {len(pairs)} guided need {len(prompts) + len(pairs)} slots; "
+                             f"the engine has {self.max_batch}")
         if n_takes > 1:
             caps = [c for c in caps for _ in range(n_takes)]
             settings = settings.repeat(n_takes)
+        caps = caps + [caps[c] for c, _, _ in pairs]
+        settings = settings.pair(pairs)
         limit = max(caps)
         sp = self.sampling(eos_token_id, settings.min_new_tokens, limit, settings.top_k, settings.temperature, seed, greedy,
                            forced, limits=caps if min(caps) < limit else None, slot_base=slot_base)
         B = len(prompts) * n_takes
-        settings.apply(self, B)
+        settings.apply(self, B + len(pairs))
         if n_takes > 1:
             self.prefill_fork(prompts, n_takes, sp)
         else:
-            self.prefill(prompts, sp)
+            self.prefill(list(prompts) + [guidance[c][1] for c, _, _ in pairs], sp)
         remaining = limit - 1
         while remaining > 0:
             n = min(check_every, remaining)
@@ -952,7 +1115,7 @@ class SpeechLM:
                        greedy: bool = False, check_every: int = 32, slot_base: int = 0, top_p: float = 1.0,
                        min_p: float = 0.0, vocab_range=None, repetition_penalty=1.0, penalize_prompt=True,
                        return_logprobs: bool = False, num_return_sequences: int = 1,
-                       exponential_decay_length_penalty=None):
+                       exponential_decay_length_penalty=None, guidance_scale=1.0, negative_prompt_ids=None):
         """Continuous batching over any number of prompts: ``generate_batch``'s results and stopping rules, but a slot
         whose sequence finished is refilled with the next waiting prompt while the other slots keep decoding.
 
@@ -970,20 +1133,27 @@ class SpeechLM:
         ``return_logprobs`` as in ``generate_batch``: a finished slot's rows are copied out with its tokens, before
         the refill that reuses the slot.  ``min_new_tokens`` and ``exponential_decay_length_penalty`` as in
         ``generate_batch``; a newcomer's entry is written before its prefill.  One sequence per prompt: ``num_return_sequences`` > 1 raises ValueError
-        (``generate_batch`` takes several per prompt)."""
+        (``generate_batch`` takes several per prompt).
+
+        ``guidance_scale`` and ``negative_prompt_ids`` as in ``generate_batch``.  A guided prompt needs two free slots,
+        filled by one ``prefill_slots`` call with the others admitted at that read; admission stays FIFO (the head of
+        the queue waits for room), and the pair's slots free together."""
         if num_return_sequences != 1:
             raise ValueError("generate_queue returns one sequence per prompt; use generate_batch(num_return_sequences=n) "
                              "for several takes of each prompt")
-        caps, settings = self._prepare(prompts, max_length, max_new_tokens, temperature=temperature, top_k=top_k,
-                                       top_p=top_p, min_p=min_p, vocab_range=vocab_range,
-                                       repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt,
-                                       logprobs=return_logprobs, min_new_tokens=min_new_tokens,
-                                       exponential_decay_length_penalty=exponential_decay_length_penalty)
+        caps, settings, guidance = self._prepare(
+            prompts, max_length, max_new_tokens, guidance_scale, negative_prompt_ids, temperature=temperature, top_k=top_k,
+            top_p=top_p, min_p=min_p, vocab_range=vocab_range, repetition_penalty=repetition_penalty,
+            penalize_prompt=penalize_prompt, logprobs=return_logprobs, min_new_tokens=min_new_tokens,
+            exponential_decay_length_penalty=exponential_decay_length_penalty)
         n = len(prompts)
         if n == 0:
             return ([], []) if return_logprobs else []
         if check_every < 1:
             raise ValueError("check_every must be >= 1")
+        if guidance is not None:
+            return self._generate_queue_guided(prompts, eos_token_id, caps, settings, guidance, seed, greedy, check_every,
+                                               slot_base, return_logprobs)
         S = min(n, self.max_batch)
         sp = self.sampling(eos_token_id, settings.min_new_tokens, max(caps), settings.top_k, settings.temperature, seed,
                            greedy, limits=caps[:S], slot_base=slot_base)
@@ -1031,24 +1201,125 @@ class SpeechLM:
         self.release_pages()
         return (out, out_lp) if return_logprobs else out
 
+    def _generate_queue_guided(self, prompts, eos_token_id, caps, settings, guidance, seed, greedy, check_every, slot_base,
+                               return_logprobs):
+        """``generate_queue`` with some prompts guided: the first prompts that fit go in by one ``prefill`` in the
+        ``generate_batch`` layout (prompt i in slot i, u slots above), later ones by ``prefill_slots`` into free slots."""
+        n, M = len(prompts), self.max_batch
+        need = [1 + (g != 1.0) for g, _ in guidance]
+        if max(need) > M:
+            raise ValueError(f"a guided prompt needs 2 slots; the engine has {M}")
+        k = 0
+        while k < n and sum(need[: k + 1]) <= M:   # prompts 0..k-1 and their u slots fit
+            k += 1
+        pairs = guided_layout(k, guidance[:k])
+        slot_caps = caps[:k] + [caps[c] for c, _, _ in pairs]
+        sp = self.sampling(eos_token_id, settings.min_new_tokens, max(caps), settings.top_k, settings.temperature, seed,
+                           greedy, limits=slot_caps, slot_base=slot_base)
+        first = dataclasses.replace(settings, controls=None if settings.controls is None else settings.controls[:k],
+                                    penalty=None if settings.penalty is None else settings.penalty[:k],
+                                    length=None if settings.length is None else settings.length[:k]).pair(pairs)
+        if first.guidance is None:
+            first = dataclasses.replace(first, guidance=[NO_GUIDANCE] * k)
+        first.apply(self, len(slot_caps))
+        self.prefill(list(prompts[:k]) + [guidance[c][1] for c, _, _ in pairs], sp)
+        occ = [None] * M           # prompt held by each c slot
+        for i in range(k):
+            occ[i] = i
+        partner = {c: u for c, u, _ in pairs}   # c slot -> u slot
+        busy = set(range(k)) | set(partner.values())
+        ngen = [1] * M
+        nxt = k
+        out, out_lp = [None] * n, [None] * n
+        floors = settings.floors(n)
+        at_prefill = lambda idx: min(floors[i] for i in idx) <= 0 or min(caps[i] for i in idx) <= 1
+        read = at_prefill(range(k))
+        while True:
+            if read:
+                st = torch.stack((self.n_generated, self.done)).cpu()
+                ngen = st[0].tolist()
+                fin = [s for s in range(M) if occ[s] is not None and int(st[1, s])]
+                freed = []
+                if fin:
+                    ids, lps = self._results(fin, [ngen[s] for s in fin], return_logprobs)
+                    for r, s in enumerate(fin):
+                        out[occ[s]] = ids[r]
+                        if return_logprobs:
+                            out_lp[occ[s]] = lps[r]
+                        occ[s] = None
+                        freed += [s] + ([partner.pop(s)] if s in partner else [])
+                    busy -= set(freed)
+                free = [s for s in range(M) if s not in busy]
+                slots, idx, neg_rows, take_u = [], [], [], []
+                while nxt < n and need[nxt] <= len(free) - len(slots) - len(take_u):
+                    rest = [s for s in free if s not in slots and s not in take_u]
+                    slots.append(rest[0])
+                    idx.append(nxt)
+                    if need[nxt] == 2:
+                        take_u.append(rest[1])
+                        neg_rows.append((len(slots) - 1, rest[1]))
+                    nxt += 1
+                if slots:
+                    all_slots = slots + take_u
+                    all_idx = idx + [idx[j] for j, _ in neg_rows]
+                    # every freed slot's entry is rewritten in the same call, so no finished pair survives
+                    guide = {s: NO_GUIDANCE for s in freed + all_slots}
+                    for j, u in neg_rows:
+                        guide[slots[j]] = (u, guidance[idx[j]][0])
+                    settings.admit(self, all_slots, all_idx, guide=guide)
+                    prompts_in = [prompts[i] for i in idx] + [guidance[idx[j]][1] for j, _ in neg_rows]
+                    self.prefill_slots(all_slots, prompts_in, sp, [slot_base + i for i in all_idx],
+                                       limits=[caps[i] for i in all_idx])
+                    for s, i in zip(slots, idx):
+                        occ[s], ngen[s] = i, 1
+                    for j, u in neg_rows:
+                        partner[slots[j]] = u
+                    busy |= set(all_slots)
+                    if at_prefill(idx):
+                        continue
+            live = [s for s in range(M) if occ[s] is not None]
+            if not live:
+                break
+            left = [caps[occ[s]] - ngen[s] for s in live]
+            steps = max(1, min(check_every, min(left) if nxt < n else max(left)))
+            self.decode(steps, sp)
+            read = True
+        self.release_pages()
+        return (out, out_lp) if return_logprobs else out
+
     @torch.no_grad()
     def generate(self, input_ids: torch.Tensor, max_length: int = 2048, eos_token_id: int | None = None,
                  do_sample: bool = True, temperature: float = 1.0, top_k: int = 50, use_cache: bool = True,
                  min_new_tokens: int = 0, max_new_tokens: int | None = None, seed: int | None = None,
                  top_p: float = 1.0, min_p: float = 0.0, vocab_range=None, repetition_penalty: float = 1.0,
-                 num_return_sequences: int = 1, exponential_decay_length_penalty=None, **_):
+                 num_return_sequences: int = 1, exponential_decay_length_penalty=None, guidance_scale=None,
+                 negative_prompt_ids=None, negative_prompt_attention_mask=None, **_):
         """transformers-compatible seam used by ``NeuTTS._infer_torch`` (neutts/neutts.py:338-347).  ``top_p`` and
         ``min_p`` act as transformers' TopPLogitsWarper / MinPLogitsWarper; ``vocab_range`` (lo, hi) suppresses every
         id outside [lo, hi) and EOS (``set_vocab_range``); ``repetition_penalty`` acts as transformers'
         RepetitionPenaltyLogitsProcessor (prompt included); ``exponential_decay_length_penalty`` (start, factor) acts as
         transformers' ExponentialDecayLengthPenalty (``set_length_control``); ``num_return_sequences`` n returns n takes of every prompt
-        from one prefill, [B * n, P + gen] with take j of row b at row b * n + j, as transformers; other generation
-        kwargs are ignored."""
+        from one prefill, [B * n, P + gen] with take j of row b at row b * n + j, as transformers; ``guidance_scale``
+        with ``negative_prompt_ids`` ([1 or B, L]; default: each prompt's last token) acts as transformers'
+        UnbatchedClassifierFreeGuidanceLogitsProcessor (``generate_batch``), and ``negative_prompt_attention_mask`` must
+        be None or all ones; other generation kwargs are ignored."""
         if eos_token_id is None:
             raise ValueError("eos_token_id is required")
         if input_ids.dim() != 2:
             raise ValueError("input_ids must be [B, P]")
         prompts = [row.tolist() for row in input_ids.cpu()]
+        guided = {}
+        if guidance_scale is not None and guidance_scale != 1:
+            if negative_prompt_attention_mask is not None and not bool(torch.as_tensor(negative_prompt_attention_mask).eq(1).all()):
+                raise ValueError("negative_prompt_attention_mask must be all ones: padded negative prompts are not supported")
+            negs = None
+            if negative_prompt_ids is not None:
+                q = torch.as_tensor(negative_prompt_ids)
+                q = q[None] if q.dim() == 1 else q
+                if q.shape[0] not in (1, len(prompts)):
+                    raise ValueError(f"negative_prompt_ids has {q.shape[0]} rows for {len(prompts)} prompts")
+                negs = [q[min(b, q.shape[0] - 1)].tolist() for b in range(len(prompts))]
+            guided = dict(guidance_scale=guidance_scale, negative_prompt_ids=negs)
         if seed is None:
             seed = int(torch.randint(0, 2**31 - 1, (1,)).item())  # reference sampling is unseeded
         cuts = {} if top_p == 1.0 and min_p == 0.0 else dict(top_p=top_p, min_p=min_p)
@@ -1061,7 +1332,7 @@ class SpeechLM:
         if exponential_decay_length_penalty is not None:
             cuts["exponential_decay_length_penalty"] = tuple(exponential_decay_length_penalty)
         outs = self.generate_batch(prompts, eos_token_id, max_length, min_new_tokens, temperature, top_k,
-                                   max_new_tokens, seed, greedy=not do_sample, **cuts)
+                                   max_new_tokens, seed, greedy=not do_sample, **cuts, **guided)
         n = max(len(o) for o in outs)
         takes = len(outs) // len(prompts)
         res = torch.full((len(outs), input_ids.shape[1] + n), int(eos_token_id), dtype=torch.long)
