@@ -486,6 +486,73 @@ int nt_resampler_push(nt_resampler* rs, int n, const int32_t* rows, const int32_
                       const int64_t* in_offsets, void* out, const int64_t* out_offsets, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Speaking rate: a phase-vocoder time stretch of 24 kHz PCM, for whole rows and for streams
+ * ------------------------------------------------------------------------------------------
+ * Semantics of librosa.effects.time_stretch(x, rate=r), 0.5 <= r <= 2.0 (r > 1 is faster speech; pitch is kept), as
+ * torch / torchaudio compute it in float64 for a row x of L samples:
+ *   S  = stft(x, n_fft 1024, hop 256, periodic Hann window, center, zero padding)       T = 1 + L / 256 frames
+ *   S2 = torchaudio.functional.phase_vocoder(S, r, linspace(0, pi * 256, 513))         K = ceil(T / r) frames
+ *   y  = istft(S2, same window, center, length = round(L / r))
+ * Output frame j sits at tau_j = j * r (fp64 product, never accumulated) and reads analysis frames a0_j = floor(tau_j)
+ * and a1_j = floor(tau_j + 1) (the fp64 sum, as torchaudio's (time_steps + 1).long()), frames at or past T being zero;
+ * K is torch.arange's count, ceil(T / r) in fp64; round is half to even.  (torch.arange's own values can differ from
+ * j * r by an ulp, depending on the CPU's vector width; where that crosses an integer torchaudio interpolates another
+ * frame pair.  The product is the contract here, the same on every machine.)
+ * The analysis and synthesis DFTs are wgmma GEMMs in 3xTF32 against windowed bases computed in float64; the vocoder
+ * runs in fp64 on the fp32 spectra with an fp64 phase accumulator wrapped to [-pi, pi] at every frame; the overlap-add
+ * sums frames in ascending order in fp32 and divides by the fp32 window-square envelope.
+ * Streams: with n input samples of a row received,
+ *   - analysis frame a is complete once n >= 256 a + 512 (its last input sample is x[256 a + 511]);
+ *   - output frame j is ready once frames a0_j and a1_j are complete: J(n) = the number of j with 256 a1_j + 512 <= n
+ *     (a prefix, since a1_j grows with j);
+ *   - output sample e reads output frames floor((e + 512 - 1023) / 256) .. floor((e + 512) / 256), so it is final once
+ *     e < 256 J(n) - 512.  That bound is always below round(n / r) - 511 <= round(L / r) - 511 for r <= 2, so a later
+ *     length = round(L / r) can never trim a sample a push has emitted.
+ * A push emits exactly the samples that became final: max(0, 256 J(n) - 512) in total after a non-final push.  A final
+ * push pads with zeros, emits the rest, so a row's total is round(L / r), and leaves the row reset.  Every output is
+ * bit-identical however its row was split into pushes and whichever other rows share a push. */
+typedef struct {
+  int32_t n_fft, hop;          /* 1024, 256 */
+  int32_t max_items;           /* rows per round of launches */
+  int32_t chunk;               /* input samples per row per round: a push walks longer inputs in rounds */
+  int32_t spec_ld;             /* debug "spec": fp32 rows of spec_ld floats, Re of bins 0..512 then Im of bins 0..512 */
+  int32_t stretch_ld;          /* debug "stretch": 3xTF32 hi rows of stretch_ld floats (Re | Im as above), the lo
+                                  halves stretch_lo_rows rows further down; a value is hi + lo */
+  int32_t stretch_lo_rows;
+  size_t table_bytes;          /* device bytes of the bases (filled by create) */
+  size_t row_bytes;            /* device bytes of one row's stream state */
+  size_t scratch_bytes;        /* device bytes of the scratch one push uses (independent of the input length) */
+} nt_stretch_info;
+
+typedef struct nt_stretch nt_stretch;
+
+/* Sizes (needs no GPU). */
+int nt_stretch_query(nt_stretch_info* info);
+/* table, state (max_rows * row_bytes; NULL when max_rows is 0) and scratch: caller-owned device memory, 256-byte aligned.
+ * The table is filled here (synchronously).  Every row starts reset.  Needs an sm_90 device. */
+int nt_stretch_create(int max_rows, void* table, void* state, void* scratch, nt_stretch** out);
+int nt_stretch_destroy(nt_stretch* st);
+/* Rows [n] (host) start a new stream: their held samples, phases and speed are dropped.  Host state only. */
+int nt_stretch_reset(nt_stretch* st, const int32_t* rows, int n);
+/* Stretch n items.  in: device fp32, item i at in[in_offsets[i] .. in_offsets[i + 1]); out: device fp32, item i at
+ * out[out_offsets[i] .. out_offsets[i + 1]); offsets are host arrays of n + 1 non-decreasing entries.  speeds: host [n]
+ * fp64, each in [0.5, 2.0].  rows: host [n] distinct rows < max_rows, whose streams continue; final_flags: host [n]
+ * (NULL: none final), nonzero ends that row's stream.  A row keeps the speed of its first push after a reset until its
+ * stream ends; a push that names another speed for it returns NT_ERR_INVALID.  rows = NULL stretches each item whole
+ * (one final push per item through the same path, on state rows inside the scratch; final_flags is ignored).  Each
+ * item's output span must be exactly the number of samples the contract above makes final, else NT_ERR_INVALID and
+ * nothing is launched.  Inputs longer than info.chunk are walked in rounds of that many samples per row, at most
+ * info.max_items rows per round; each round is five launches on `stream` (pack, analysis GEMM, vocoder, synthesis
+ * GEMM, overlap-add), the GEMMs skipped when no frame is due. */
+int nt_stretch_push(nt_stretch* st, int n, const int32_t* rows, const int32_t* final_flags, const double* speeds,
+                    const float* in, const int64_t* in_offsets, float* out, const int64_t* out_offsets, void* stream);
+/* Stage hooks (tests): the scratch buffers of the last round, by name: "spec" (analysis spectra: row rb + a - a0 is
+ * frame a of the round's row whose A rows start at rb; a lone row's first round starts at row 0 with frame 0),
+ * "stretch" (stretched spectra, hi / lo halves; a lone one-shot row of at most info.chunk samples holds its frames
+ * 0 .. K-1 at rows 0 .. K-1), "frames" (windowed time frames, 1024 floats per stretched row); NULL for other names. */
+void* nt_stretch_debug_ptr(nt_stretch* st, const char* name);
+
+/* ------------------------------------------------------------------------------------------
  * Single-op entry points (unit tests; each mirrors one row of SURVEY.md §8a)
  * ------------------------------------------------------------------------------------------ */
 int nt_op_rmsnorm(const float* x, const float* w, float eps, int rows, int cols, float* out_f32, void* out_bf16,

@@ -72,6 +72,16 @@ def _add_guidance(ctl: dict, n: int, guidance_scale, negatives) -> dict:
     return ctl
 
 
+def _speeds(n: int, speed):
+    """One speaking rate per utterance (``speed`` a number or one per utterance, each in [0.5, 2.0]; ValueError
+    otherwise), or None when every one is 1.0: then nothing is stretched and no stretcher is built."""
+    from neutts_air_b200.stretch import check_speed
+
+    s = per_item(n, "utterance", speed=speed)["speed"]
+    s = [check_speed(x) for x in s] if isinstance(s, list) else [check_speed(s)] * n
+    return s if any(x != 1.0 for x in s) else None
+
+
 def _pick(ctl: dict, idx) -> dict:
     """The controls of the utterances ``idx`` (lists are indexed, scalars stay)."""
     return {k: [v[i] for i in idx] if isinstance(v, list) else v for k, v in ctl.items()}
@@ -156,6 +166,7 @@ class NeuTTS:
         self.sample_rate = int(sample_rate)       # the rate of every waveform returned (the codec's is 24 kHz)
         self.pcm_format = pcm_format
         self._resampler = None
+        self._stretcher = None
         # constants the reference exposes (neutts/neutts.py:84-91)
         self.max_context = 2048
         self.hop_length = 480
@@ -407,9 +418,22 @@ class NeuTTS:
             self._resampler = Resampler(self.sample_rate, self.pcm_format, device=self.codec.device, max_rows=rows)
         return self._resampler
 
-    def _decode_codes(self, codes: Sequence[torch.Tensor], watermark: bool = False) -> list:
+    def _time_stretch(self):
+        """The GPU speaking-rate stretcher (one stream row per slot), built on first use."""
+        if self._stretcher is None:
+            from neutts_air_b200.stretch import TimeStretch
+
+            rows = max(self.max_batch, getattr(self.backbone, "max_batch", 1))
+            self._stretcher = TimeStretch(device=self.codec.device, max_rows=rows)
+        return self._stretcher
+
+    def _decode_codes(self, codes: Sequence[torch.Tensor], watermark: bool = False, speeds=None) -> list:
         """codes: list of 1-D int tensors -> list of numpy waveforms at ``sample_rate`` in ``pcm_format`` (batched by
-        equal length).  ``watermark``: each waveform is watermarked at 24 kHz, before any resampling."""
+        equal length).  ``watermark``: each waveform is watermarked at 24 kHz, before any resampling.  ``speeds``: None
+        or one speaking rate per waveform; a waveform whose rate is not 1.0 is stretched at 24 kHz right after the
+        codec, before the watermark and the resampler."""
+        if speeds is not None:
+            return self._decode_stretched(codes, watermark, speeds)
         rs = self._output_resampler()
         out = [None] * len(codes)
         by_len: dict = {}
@@ -440,6 +464,37 @@ class NeuTTS:
             out = [self._watermark(w) for w in out]
         return out
 
+    def _decode_stretched(self, codes, watermark: bool, speeds) -> list:
+        """``_decode_codes`` with speaking rates: per waveform codec -> stretch (rate != 1.0) -> watermark -> resample,
+        the stretch and the resampler on the device; a waveform at 1.0 gets the bytes it gets without rates."""
+        rs, ts = self._output_resampler(), self._time_stretch()
+        out = [None] * len(codes)
+        by_len: dict = {}
+        for i, c in enumerate(codes):
+            if len(c) == 0:
+                raise ValueError("No valid speech tokens found in the output.")
+            by_len.setdefault(len(c), []).append(i)
+        cap = getattr(self.codec, "max_batch", 1)
+        for n, idxs in by_len.items():
+            for j in range(0, len(idxs), cap):
+                grp = idxs[j: j + cap]
+                batch = torch.stack([codes[i].long() for i in grp])[:, None, :].to(self.codec.device)
+                with torch.no_grad():
+                    pcm = self.codec.decode_code(batch)[:, 0, :]
+                rows = list(pcm)
+                fast = [r for r, i in enumerate(grp) if speeds[i] != 1.0]
+                for r, y in zip(fast, ts.stretch([rows[r] for r in fast], [speeds[grp[r]] for r in fast])):
+                    rows[r] = y
+                for r, i in enumerate(grp):
+                    w = rows[r]
+                    if watermark and self.watermarker is not None:
+                        w = self._watermark(w.cpu().numpy())
+                        w = torch.from_numpy(np.asarray(w, dtype=np.float32)).to(pcm.device) if rs is not None else w
+                    if rs is not None:
+                        w = rs.resample(w)
+                    out[i] = w.cpu().numpy() if isinstance(w, torch.Tensor) else w
+        return out
+
     def _decode(self, codes) -> np.ndarray:
         """``codes``: the ``<|speech_N|>`` string of the reference seam (``neutts/neutts.py:273-295``) or a 1-D int sequence."""
         if isinstance(codes, str):
@@ -458,23 +513,24 @@ class NeuTTS:
     def infer(self, text: str, ref_codes, ref_text: str, *, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0,
               min_p: float = 0.0, repetition_penalty: float = 1.0, penalize_prompt: bool = True,
               return_logprobs: bool = False, takes: int = 1, min_new_tokens: int = 50,
-              exponential_decay_length_penalty=None, guidance_scale: float = 1.0, negative_text: str | None = None):
+              exponential_decay_length_penalty=None, guidance_scale: float = 1.0, negative_text: str | None = None,
+              speed: float = 1.0):
         """Text + reference voice -> 24 kHz float32 waveform (``neutts/neutts.py:216-243``).  The sampling controls
         default to the reference's values; see ``infer_batch``.  ``return_logprobs``: returns (waveform, log-probs).
         ``takes``: generate that many takes and keep the most probable one (``infer_batch``).  ``guidance_scale`` and
-        ``negative_text``: classifier-free guidance (``infer_batch``)."""
+        ``negative_text``: classifier-free guidance (``infer_batch``).  ``speed``: speaking rate (``infer_batch``)."""
         out = self.infer_batch([text], [ref_codes], [ref_text], temperature=temperature, top_k=top_k, top_p=top_p,
                                min_p=min_p, repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt,
                                return_logprobs=return_logprobs, takes=takes, min_new_tokens=min_new_tokens,
                                exponential_decay_length_penalty=exponential_decay_length_penalty,
-                               guidance_scale=guidance_scale, negative_text=negative_text)
+                               guidance_scale=guidance_scale, negative_text=negative_text, speed=speed)
         return (out[0][0], out[1][0]) if return_logprobs else out[0]
 
     def infer_from_prompt_ids(self, prompts: Sequence[Sequence[int]], max_new_tokens: int | None = None,
                               min_new_tokens: int = 50, slot_base: int = 0, *, temperature=1.0, top_k=50, top_p=1.0,
                               min_p=0.0, repetition_penalty=1.0, penalize_prompt=True, return_logprobs: bool = False,
                               takes: int = 1, exponential_decay_length_penalty=None, guidance_scale=1.0,
-                              negative_prompt_ids=None):
+                              negative_prompt_ids=None, speed=1.0):
         """Hot path only: prompt ids (host) -> waveforms (host).  Used by bench.py's end-to-end leg.
         ``slot_base`` offsets the sampler's Philox slot index so chunks / ranks under one seed draw independently.
         More prompts than ``max_batch`` go through the backbone's ``generate_queue`` when it has one.  Sampling
@@ -482,7 +538,9 @@ class NeuTTS:
         max_batch, and ``slot_base`` counts takes).  ``guidance_scale`` (a number or one per prompt, 1 = off) and
         ``negative_prompt_ids`` (None, or one id list or None per prompt; None: the prompt's last token) add
         classifier-free guidance (``SpeechLM.generate_batch``; transformers' ``guidance_scale`` and
-        ``negative_prompt_ids`` on an injected transformers backbone)."""
+        ``negative_prompt_ids`` on an injected transformers backbone).  ``speed``: speaking rate of each waveform (a
+        number or one per prompt, ``infer_batch``); it acts on the PCM alone and never reaches the backbone."""
+        speeds = _speeds(len(prompts), speed)
         ctl = _controls(len(prompts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
                         exponential_decay_length_penalty)
         ctl = _add_guidance(ctl, len(prompts), guidance_scale, negative_prompt_ids)
@@ -494,13 +552,13 @@ class NeuTTS:
                                  takes=takes)
         if return_logprobs:
             gen, lps = gen
-        wavs = self._decode_codes([self._ids_to_codes(g) for g in gen], watermark=True)
+        wavs = self._decode_codes([self._ids_to_codes(g) for g in gen], watermark=True, speeds=speeds)
         return (wavs, [lp.numpy() for lp in lps]) if return_logprobs else wavs
 
     def infer_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], distributed: bool = False, *,
                     temperature=1.0, top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0, penalize_prompt=True,
                     return_logprobs: bool = False, takes: int = 1, min_new_tokens=50, exponential_decay_length_penalty=None,
-                    guidance_scale=1.0, negative_text=None):
+                    guidance_scale=1.0, negative_text=None, speed=1.0):
         """List in / list out.  With ``distributed=True`` (inside an initialised torch.distributed job) the
         utterances are sharded over ranks and every rank returns all waveforms (one all-gather).
 
@@ -545,9 +603,16 @@ class NeuTTS:
         is the chat template with the utterance's own reference codes and reference text and ``negative_text`` as the
         input text; None means "", the voice without the words, which steers the draws toward the text.  Each guided
         utterance decodes its negative prompt in a second engine slot, so a chunk or the queue holds fewer of them at
-        once.  Not with ``takes`` > 1 (ValueError); ``distributed`` works, every rank guiding its own utterances."""
+        once.  Not with ``takes`` > 1 (ValueError); ``distributed`` works, every rank guiding its own utterances.
+
+        ``speed`` (a number or one per utterance, in [0.5, 2.0]; > 1 is faster) is the speaking rate: each waveform is
+        time-stretched at 24 kHz on the GPU right after the codec (librosa's ``time_stretch``, a phase vocoder: the
+        pitch is kept, a waveform of L samples becomes round(L / speed)), before the watermark and any resampling.  A
+        list follows its utterances through chunking, the queue, takes (the kept take is stretched) and the sharding
+        over ranks.  An utterance at exactly 1.0 is not stretched; with every speed at 1.0 nothing changes."""
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
+        speeds = _speeds(len(texts), speed)
         ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
                         exponential_decay_length_penalty)
         ctl = _add_guidance(ctl, len(texts), guidance_scale,
@@ -559,14 +624,15 @@ class NeuTTS:
             self._check_logprobs(distributed)
         prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(texts, ref_codes, ref_texts)]
         if takes > 1:
-            return self._infer_takes(prompts, ctl, takes, return_logprobs)
+            return self._infer_takes(prompts, ctl, takes, return_logprobs, speeds)
         queue = hasattr(self.backbone, "generate_queue")
 
         def run(idx, slot_base):
             c = _pick(ctl, idx)
             g, neg = c.pop("guidance_scale", 1.0), c.pop("negative_prompt_ids", None)
             return self.infer_from_prompt_ids([prompts[i] for i in idx], slot_base=slot_base, return_logprobs=return_logprobs,
-                                              guidance_scale=g, negative_prompt_ids=neg, **c)
+                                              guidance_scale=g, negative_prompt_ids=neg,
+                                              speed=1.0 if speeds is None else [speeds[i] for i in idx], **c)
 
         # chunks of prompts whose slots (two for a guided one) fit the engine; prompt i keeps Philox stream i
         chunks, j = [], 0
@@ -607,11 +673,12 @@ class NeuTTS:
         per = max_batch // takes
         return [(range(j, min(j + per, n_utterances)), j * takes) for j in range(0, n_utterances, per)]
 
-    def _infer_takes(self, prompts, ctl: dict, takes: int, return_logprobs: bool):
+    def _infer_takes(self, prompts, ctl: dict, takes: int, return_logprobs: bool, speeds=None):
         out, lps = [], []
         for idx, slot_base in self.take_chunks(len(prompts), takes, self.max_batch):
             r = self.infer_from_prompt_ids([prompts[i] for i in idx], slot_base=slot_base, return_logprobs=return_logprobs,
-                                           takes=takes, **_pick(ctl, idx))
+                                           takes=takes, speed=1.0 if speeds is None else [speeds[i] for i in idx],
+                                           **_pick(ctl, idx))
             out += r[0] if return_logprobs else r
             lps += r[1] if return_logprobs else []
         return (out, lps) if return_logprobs else out
@@ -671,26 +738,30 @@ class NeuTTS:
     def infer_stream(self, text: str, ref_codes, ref_text: str, *, temperature: float = 1.0, top_k: int = 50,
                      top_p: float = 1.0, min_p: float = 0.0, repetition_penalty: float = 1.0,
                      penalize_prompt: bool = True, takes: int = 1, min_new_tokens: int = 50,
-                     exponential_decay_length_penalty=None, guidance_scale=1.0) -> Generator[np.ndarray, None, None]:
+                     exponential_decay_length_penalty=None, guidance_scale=1.0,
+                     speed: float = 1.0) -> Generator[np.ndarray, None, None]:
         """Streaming synthesis with the reference's window geometry (``neutts/neutts.py:373-465``):
         every 25 new frames (once 5 look-ahead frames exist) the codec re-decodes
         [n - 50 - 1, n + 25 + 5 + 1) and the chunk is cross-faded with triangular weights.  Sampling controls as in
         ``infer_batch``; streaming returns no per-token log-probabilities (``return_logprobs`` is not supported here)
         and generates one take per utterance (``takes`` other than 1 raises ValueError); classifier-free guidance is not
-        supported (``guidance_scale`` other than 1 raises ValueError)."""
+        supported (``guidance_scale`` other than 1 raises ValueError).  ``speed``: speaking rate (``infer_batch``); each
+        cross-faded chunk goes through the stretcher's stream, so the chunks concatenate to the stretched stream."""
         self._no_takes(takes)
         self._no_guidance(guidance_scale, "streaming synthesis")
         if self._is_quantized_model:  # kept for signature parity; never true on this build
             raise NotImplementedError("GGUF streaming is not part of the H100 build")
         ctl = _controls(1, temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
                         exponential_decay_length_penalty)
+        speeds = _speeds(1, speed)
         prompt = self._apply_chat_template(ref_codes, ref_text, text)
-        return self._stream(prompt, [int(c) for c in (ref_codes.tolist() if hasattr(ref_codes, "tolist") else ref_codes)], ctl)
+        return self._stream(prompt, [int(c) for c in (ref_codes.tolist() if hasattr(ref_codes, "tolist") else ref_codes)], ctl,
+                            speeds)
 
     def infer_stream_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], *, temperature=1.0,
                            top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0,
                            penalize_prompt=True, takes: int = 1, min_new_tokens=50,
-                           exponential_decay_length_penalty=None, guidance_scale=1.0) -> Generator[list, None, None]:
+                           exponential_decay_length_penalty=None, guidance_scale=1.0, speed=1.0) -> Generator[list, None, None]:
         """Streaming synthesis of many utterances at once (BASELINE.json configs[4]; the reference streams one
         utterance, ``neutts/neutts.py:373-465``).  Every yield is a list with one entry per utterance, as many entries
         as ``texts``: the next audio chunk (float32, cross-faded exactly as in ``infer_stream``) or ``None`` when that
@@ -706,7 +777,10 @@ class NeuTTS:
         closed early.
 
         Streaming returns no per-token log-probabilities (``infer_batch``'s ``return_logprobs``) and generates one take
-        per utterance (``takes`` other than 1 raises ValueError); ``guidance_scale`` other than 1 raises ValueError."""
+        per utterance (``takes`` other than 1 raises ValueError); ``guidance_scale`` other than 1 raises ValueError.
+        ``speed`` (a number or one per utterance): speaking rate, as in ``infer_batch``; it follows its utterance into
+        whichever slot it takes.  Chunks go codec -> cross-fade -> stretch -> resample, and concatenate to the stretched
+        stream."""
         self._no_takes(takes)
         self._no_guidance(guidance_scale, "streaming synthesis")
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
@@ -716,10 +790,10 @@ class NeuTTS:
                         exponential_decay_length_penalty)
         prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(texts, ref_codes, ref_texts)]
         refs = [[int(c) for c in (rc.tolist() if hasattr(rc, "tolist") else rc)] for rc in ref_codes]
-        return self._stream_batch(prompts, refs, ctl)
+        return self._stream_batch(prompts, refs, ctl, _speeds(len(texts), speed))
 
-    def _stream(self, prompt, ref_codes, ctl: dict | None = None) -> Generator[np.ndarray, None, None]:
-        for out in self._stream_batch([prompt], [list(ref_codes)], ctl):
+    def _stream(self, prompt, ref_codes, ctl: dict | None = None, speeds=None) -> Generator[np.ndarray, None, None]:
+        for out in self._stream_batch([prompt], [list(ref_codes)], ctl, speeds):
             if out[0] is not None:
                 yield out[0]
 
@@ -732,7 +806,7 @@ class NeuTTS:
                              "(neutts_air_b200.SpeechLM)")
         return min(n, slots)
 
-    def _stream_batch(self, prompts, refs, ctl: dict | None = None) -> Generator[list, None, None]:
+    def _stream_batch(self, prompts, refs, ctl: dict | None = None, speeds=None) -> Generator[list, None, None]:
         """Window geometry of the reference (``neutts/neutts.py:87-91,401-421,443-465``): once F + LA undecoded frames
         exist, the codec decodes [n_dec - LB - OV, n_dec + F + LA) and the slice [n_dec - OV, n_dec + F + OV) is
         cross-faded at stride F * hop; a ragged tail closes the stream.  ``streaming_frames_per_chunk`` may be set to
@@ -780,6 +854,23 @@ class NeuTTS:
         occ = list(range(B))   # utterance held by each slot; None once its tail is out and nobody waits
         nxt = B                # next utterance to admit
         rs = self._output_resampler()
+        ts = self._time_stretch() if speeds is not None else None
+
+        def at_speed(out, ends=()):
+            """the round's cross-faded chunks at each utterance's speaking rate: one push over the slots whose utterance
+            is not at 1.0 and has new audio or ends; a chunk whose samples are all still held becomes None"""
+            if ts is None:
+                return out
+            us = [u for u in range(N) if speeds[u] != 1.0 and (out[u] is not None or u in ends)]
+            if not us:
+                return out
+            slot = {occ[b]: b for b in range(B) if occ[b] is not None}
+            got = ts.push([slot[u] for u in us], [np.zeros(0, np.float32) if out[u] is None else out[u] for u in us],
+                          [speeds[u] for u in us], [u in ends for u in us])
+            res = list(out)
+            for u, y in zip(us, got):
+                res[u] = y if y.size else None
+            return res
 
         def at_rate(out, ends=()):
             """the round's 24 kHz chunks at ``sample_rate``: one push over the slots with new audio or an ending stream
@@ -806,6 +897,8 @@ class NeuTTS:
             absorbed[sl] = 0
             if rs is not None:
                 rs.reset(slots)
+            if ts is not None:
+                ts.reset(slots)
 
         def absorb(lo: int, hi: int):
             """tokens [lo, hi) of every slot -> history (non-speech ids dropped, as the reference's regex does)"""
@@ -884,7 +977,7 @@ class NeuTTS:
                             flush = fades[u].push(np.zeros(0, np.float32), final=True)
                             out[u] = flush if out[u] is None else np.concatenate((out[u], flush))
                 if all_finished and any(o is not None for o in out) and tails:
-                    first = at_rate(out)         # regular chunks first: a tail is its own yield, as in the reference
+                    first = at_rate(at_speed(out))   # regular chunks first: a tail is its own yield, as in the reference
                     if any(o is not None for o in first):
                         yield first
                     out = [None] * N
@@ -892,7 +985,7 @@ class NeuTTS:
                     for b, wavs in decode_windows(tails).items():
                         t = fades[occ[b]].push(wavs[0], final=True)
                         out[occ[b]] = t if out[occ[b]] is None else np.concatenate((out[occ[b]], t))
-                out = at_rate(out, ending)
+                out = at_rate(at_speed(out, ending), ending)
                 if any(o is not None for o in out):
                     yield out
                 if all_finished:
@@ -928,6 +1021,8 @@ class NeuTTS:
         finally:
             if queue:
                 lm.release_pages()   # also when the consumer stops early (generator close)
+            if ts is not None:
+                ts.reset(range(B))
 
     def encode_reference(self, ref_audio_path):
         """wav -> NeuCodec codes (``neutts/neutts.py:266-271``).  The encoder is outside the hot path; this

@@ -95,6 +95,12 @@ class ResamplerInfo(C.Structure):
                 ("table_bytes", C.c_size_t), ("row_bytes", C.c_size_t)]
 
 
+class StretchInfo(C.Structure):
+    _fields_ = [("n_fft", C.c_int32), ("hop", C.c_int32), ("max_items", C.c_int32), ("chunk", C.c_int32),
+                ("spec_ld", C.c_int32), ("stretch_ld", C.c_int32), ("stretch_lo_rows", C.c_int32),
+                ("table_bytes", C.c_size_t), ("row_bytes", C.c_size_t), ("scratch_bytes", C.c_size_t)]
+
+
 class CodecWeights(C.Structure):
     _fields_ = [
         ("fsq_w", C.c_void_p), ("fsq_b", C.c_void_p), ("embed_w", C.c_void_p), ("embed_b", C.c_void_p),
@@ -119,6 +125,8 @@ EXPORTS = [
     "nt_codec_workspace_bytes", "nt_codec_create", "nt_codec_destroy", "nt_codec_decode",
     "nt_codec_debug_set_stages", "nt_codec_debug_ptr",
     "nt_resampler_query", "nt_resampler_create", "nt_resampler_destroy", "nt_resampler_reset", "nt_resampler_push",
+    "nt_stretch_query", "nt_stretch_create", "nt_stretch_destroy", "nt_stretch_reset", "nt_stretch_push",
+    "nt_stretch_debug_ptr",
     "nt_op_rmsnorm", "nt_op_topk_sample",
 ]
 
@@ -190,6 +198,14 @@ def lib() -> C.CDLL:
     L.nt_resampler_reset.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int]
     L.nt_resampler_push.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p,
                                     C.POINTER(C.c_int64), C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]
+    L.nt_stretch_query.argtypes = [C.POINTER(StretchInfo)]
+    L.nt_stretch_create.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]
+    L.nt_stretch_destroy.argtypes = [C.c_void_p]
+    L.nt_stretch_reset.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int]
+    L.nt_stretch_push.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_double),
+                                  C.c_void_p, C.POINTER(C.c_int64), C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]
+    L.nt_stretch_debug_ptr.restype = C.c_void_p
+    L.nt_stretch_debug_ptr.argtypes = [C.c_void_p, C.c_char_p]
     L.nt_op_rmsnorm.argtypes = [C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     L.nt_op_topk_sample.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(Sampling), C.c_void_p, C.c_int32,
                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
