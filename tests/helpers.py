@@ -168,6 +168,23 @@ def decode_branch(shape: tuple, B: int, G: int, max_ctx: int, impl=None) -> dict
                 name=f"tc-{act}-n{nt}-{plan}-{'fold' if fold else 'phases'}")
 
 
+def gemm_splits(M: int, N: int, K: int, ws_floats: int) -> int:
+    """Split-K slices gemm_dispatch (gemm_tc.cu) picks for an M x N x K bf16 GEMM with a split workspace of
+    ``ws_floats`` floats, on the device's SM count (restated)."""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    mt = -(-M // 128)
+    bn = 128
+    if mt * -(-N // 128) < sms * 13 // 16:
+        bn = 64
+    if mt * -(-N // 64) < sms * 11 // 16:
+        bn = 32
+    tiles, nkb = mt * -(-N // bn), -(-K // 64)
+    if tiles > 48 or nkb < 8:
+        return 1
+    sk = min((sms - 4) // tiles, nkb // 4, 8)
+    return sk if sk > 1 and M * N * sk <= ws_floats else 1
+
+
 # ------------------------------------------------------------------------------- a small engine and its bar, a facade
 SMALL = dict(vocab_size=4096, hidden_size=256, intermediate_size=640, num_layers=3, num_heads=4, num_kv_heads=2)
 

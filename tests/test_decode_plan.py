@@ -14,13 +14,27 @@ import pytest
 
 MAX_ITEMS, MAX_GU_SLICES, MAX_CHUNKS = 4, 4, 14   # kTcMaxItems, kTcMaxGuSlices, the staging area's k-blocks
 
-# (hidden, inter, n_heads, n_kv, vocab): NeuTTS-Air and NeuTTS-Nano widths, and a small model
-SHAPES = {"air": (896, 4864, 14, 2, 20546), "nano": (576, 1536, 9, 3, 20546), "small": (256, 640, 4, 2, 20546)}
-# which plans the planner accepts on an H100 SXM (132 SMs): (whole-K, flat)
-ACCEPTED_AT_132 = {"air": (True, True), "nano": (True, False), "small": (True, True)}
+# (hidden, inter, n_heads, n_kv, vocab): NeuTTS-Air and NeuTTS-Nano widths, a small model, the Nano-like model bench.py
+# measures in its streaming line (8 query / 2 KV heads, GQA ratio 4), Air widths over 16 / 4 heads, and the
+# attention-transparent models of test_gpu_attention.py at every GQA ratio (hidden = 64 * query heads, inter 256)
+SHAPES = {"air": (896, 4864, 14, 2, 20546), "nano": (576, 1536, 9, 3, 20546), "small": (256, 640, 4, 2, 20546),
+          "bench": (512, 2048, 8, 2, 217472), "air16x4": (896, 4864, 16, 4, 20546)}
+RATIO_HEADS = {"gqa1": (8, 8), "gqa2": (4, 2), "gqa3": (9, 3), "gqa4": (8, 2), "gqa4kv3": (12, 3), "gqa5": (10, 2),
+               "gqa6": (12, 2), "gqa7": (14, 2), "gqa8": (8, 1)}
+SHAPES.update({f"attn-{k}": (64 * nh, 256, nh, nkv, 2048) for k, (nh, nkv) in RATIO_HEADS.items()})
+# which plans the planner accepts on an H100 SXM (132 SMs): (whole-K, flat).  Of the transparent models only the
+# hidden-256 one has a flat plan there.
+ACCEPTED_AT_132 = {"air": (True, True), "nano": (True, False), "small": (True, True), "bench": (True, False),
+                   "air16x4": (True, True), **{f"attn-{k}": (True, k == "gqa2") for k in RATIO_HEADS}}
 # SM counts at which the Air shape has no whole-K plan (so no persistent-kernel plan at all: every decode takes the
 # per-op chain).  114 is the H100 PCIe.  DESIGN.md §2 records this performance cliff.
 AIR_WHOLE_K_REJECTED = set(range(8, 42)) | set(range(92, 118))
+# The bench shape has a whole-K plan from 12 CTAs up, and no flat plan at 132.
+BENCH_WHOLE_K_REJECTED = set(range(8, 12))
+# Plan regimes up to 132 CTAs (see test_plan_regimes_up_to_132_ctas)
+REGIMES_AT_132 = {"air": 33, "nano": 52, "small": 14, "bench": 47, "air16x4": 30, "attn-gqa1": 17, "attn-gqa2": 6,
+                  "attn-gqa3": 20, "attn-gqa4": 19, "attn-gqa4kv3": 25, "attn-gqa5": 22, "attn-gqa6": 27,
+                  "attn-gqa7": 31, "attn-gqa8": 18}
 
 
 def plan_or_none(shape, n_sms, flat):
@@ -98,6 +112,8 @@ def test_every_accepted_plan_is_a_partition(name, flat):
     assert (132 in accepted) == ACCEPTED_AT_132[name][flat]
     if name == "air" and not flat:
         assert set(rejected) == AIR_WHOLE_K_REJECTED, _ranges(rejected)
+    if name == "bench" and not flat:
+        assert set(rejected) == BENCH_WHOLE_K_REJECTED, _ranges(rejected)
 
 
 def _ranges(xs):
@@ -126,7 +142,7 @@ def test_plan_regimes_up_to_132_ctas():
 
     reps = {name: regime_representatives(shape, 132) for name, shape in SHAPES.items()}
     print("REGIMES " + "; ".join(f"{n} {len(r)}: {sorted(r.values())}" for n, r in reps.items()))
-    assert {n: len(r) for n, r in reps.items()} == {"air": 33, "nano": 52, "small": 14}
+    assert {n: len(r) for n, r in reps.items()} == REGIMES_AT_132
     for name, r in reps.items():
         assert len(set(r.values())) == len(r)
         for regime, G in r.items():
@@ -149,6 +165,25 @@ def test_plan_regimes_up_to_132_ctas():
     # hidden 256: the everybody branch (8..25), attention in one split at batch 3
     assert everybody(small) and all(8 <= G <= 25 for G in everybody(small))
     assert any(decode_branch(SHAPES["small"], 3, G, 512)["split_cap"] == 1 for G in small.values())
+
+
+def test_bench_and_ratio_shapes_at_132_sms():
+    """The paths the GPU tests expect at 132 CTAs.  The bench shape: batch 1 folds in the CTAs on the whole-K plan (no
+    flat plan), batch 8, the streaming line's batch, runs the phases on hi + lo activations.  Air widths over 16 / 4
+    heads: batch 1 takes the flat plan.  8 / 8 heads at batch 9..16: one attention split per (sequence, KV head)."""
+    from tests.helpers import decode_branch
+
+    bench = lambda B: decode_branch(SHAPES["bench"], B, 132, 2048)
+    assert [bench(B)["name"] for B in (1, 3, 8, 9, 16)] == [
+        "tc-hilo-n16-wholeK-fold", "tc-hilo-n16-wholeK-phases", "tc-hilo-n16-wholeK-phases",
+        "tc-bf16-n16-wholeK-phases", "tc-bf16-n16-wholeK-phases"]
+    assert decode_branch(SHAPES["air16x4"], 1, 132, 512)["name"] == "tc-hilo-n16-flat-fold"
+    assert decode_branch(SHAPES["air16x4"], 8, 132, 512)["name"] == "tc-hilo-n16-wholeK-phases"
+    gqa1 = SHAPES["attn-gqa1"]
+    assert all(decode_branch(gqa1, B, 132, 2048)["split_cap"] == 1 for B in range(9, 17))
+    assert decode_branch(gqa1, 8, 132, 2048)["split_cap"] == 2
+    for k in RATIO_HEADS:   # every transparent model runs the persistent kernel at batch 1, 8 and 16
+        assert all(decode_branch(SHAPES[f"attn-{k}"], B, 132, 2048)["kind"] == "tc" for B in (1, 8, 16)), k
 
 
 def test_bad_arguments_are_refused():

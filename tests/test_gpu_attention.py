@@ -10,14 +10,18 @@ a kernel must not read.
 
 Kernels and how each is observed:
   * prefill (``attn_prefill_kernel``): the ``attn_bf16`` buffer against ``ref_attention(mirror="mma")`` on the
-    ``q`` buffer and the cached K/V, per sequence and head, for GQA ratios 1, 2, 3, 7, 8;
+    ``q`` buffer and the cached K/V, per sequence and head, for GQA ratios 1 to 8;
+  * prefill RoPE + KV append (``rope_append_kernel``): the ``q`` buffer and every cached K and V row against the
+    float64 projection of the embedding, RoPE'd, with and without split-K slices of the qkv GEMM to sum;
   * per-op decode chain, fp32 (``attn_decode_kernel``, batch <= 4) and tensor-core (``attn_decode_mma_kernel``,
     batch > 4, RoPE + KV append fused), and the persistent kernel's split-KV attention and merge
     (``decode_tc_kernel``): through an attention-transparent model.  One layer with ``wo = I``, a zero MLP,
     ``final_norm = 1`` and an lm_head whose first ``hidden`` rows are ``I`` makes ``logits[:hidden]`` equal to
     ``rmsnorm(e + attn)`` (bf16-rounded on the paths whose GEMM inputs are bf16), so every decode path, the persistent
     kernel included, exposes its attention output.  The decode context is crafted in place: the test writes the
-    cache rows and ``seq_lens`` itself, so contexts up to 4095 tokens need no long prefill.
+    cache rows and ``seq_lens`` itself, so contexts up to 4095 tokens need no long prefill.  Every path runs at every
+    GQA ratio from 1 to 8 (``RATIO_MODELS``): the kernels' query tile, head-to-group mapping, prologue loops and the
+    persistent kernel's split count all depend on the ratio and the KV-head count.
 
 Errors are relative RMS per (sequence, head); the tests print them.  BARS lists the worst values measured on the
 H100 and the bars, about 4x above them.
@@ -31,7 +35,8 @@ import pytest
 import torch
 
 from oracle import lm_oracle as O
-from tests.helpers import GEMV_MAX_BATCH, gather_kv, make_lm, rel_rms, runs_persistent, set_decode_impl
+from tests.helpers import (GEMV_MAX_BATCH, decode_branch, gather_kv, gemm_splits, make_lm, rel_rms, runs_persistent,
+                           set_decode_impl)
 
 PAGE = 64
 LOG2E = 1.4426950408889634
@@ -44,9 +49,16 @@ KV_POISON_K, KV_POISON_V = 64.0, 8192.0   # prefill_slots: every stale row of th
 #   persistent kernel, batch <= 8 (bf16 hi + lo activations), "mma" mirror     1.3e-3  -> 5e-3
 #   bf16 activations (mma chain kernel, persistent kernel batch > 8)           3.2e-3  -> 1.2e-2
 #   appended K / V row against float64 RoPE'd k / v rounded to bf16           6.5e-4  -> 3e-3
+#   prefill q buffer per (row, head) against float64 (rope_append_kernel)                     9.1e-4  -> 4e-3
+#   prefill K / V rows per (row, head) against float64 rounded to bf16                        3.0e-3  -> 1.2e-2
 # The tensor-core kernels round each probability against the running maximum of its page, the mirror against the
-# global one; that and the odd flipped bf16 rounding of the query are what the mirror leaves.
-BARS = {"prefill": 3e-3, "decode-fp32": 2e-6, "decode-mma": 5e-3, "decode-bf16": 1.2e-2, "row": 3e-3}
+# global one; that and the odd flipped bf16 rounding of the query are what the mirror leaves.  The decode cases at GQA
+# ratios 1..8 and the prefill rows were measured on one H100 80GB HBM3 (132 SMs, 700 W power limit): fp32 chain 6.6e-7,
+# hi + lo 1.6e-3, bf16 activations 3.2e-3, appended rows 1.3e-3, all under the bars above.  The prefill rows' floor is
+# the bf16 rounding of the normalised input: an element whose fp32 and float64 values round to neighbouring bf16 values
+# moves its row's q by ~1e-4 .. 1e-3; rows without such a flip sit at 3e-7 (q).
+BARS = {"prefill": 3e-3, "decode-fp32": 2e-6, "decode-mma": 5e-3, "decode-bf16": 1.2e-2, "row": 3e-3,
+        "prefill-q": 4e-3, "row-head": 1.2e-2}
 
 
 # ====================================================================================== float64 reference helpers
@@ -82,11 +94,15 @@ def ref_attention(q, k, v, n_rep: int, causal_offset: int | None = None, mirror:
     return out
 
 
-def rope64(x, pos: int, theta: float):
-    """Half-split RoPE of x [heads, 64] (float64) at position ``pos``.  The angle pos * inv_freq is formed in fp32, as
-    the reference (modeling_qwen2.py rotary embedding) and the kernels form it; cos / sin are taken in float64."""
+def rope64(x, pos, theta: float):
+    """Half-split RoPE of x [heads, 64] (float64) at position ``pos``, or of x [T, heads, 64] at positions ``pos`` [T].
+    The angle pos * inv_freq is formed in fp32, as the reference (modeling_qwen2.py rotary embedding) and the kernels
+    form it; cos / sin are taken in float64."""
     inv = (1.0 / theta ** (torch.arange(32, dtype=torch.float64) * 2 / 64)).float()
-    ang = (torch.tensor(float(pos), dtype=torch.float32) * inv).double()
+    if torch.is_tensor(pos):
+        ang = (pos.to(torch.float32)[:, None, None] * inv).double()
+    else:
+        ang = (torch.tensor(float(pos), dtype=torch.float32) * inv).double()
     c, s = ang.cos(), ang.sin()
     x1, x2 = x[..., :32], x[..., 32:]
     return torch.cat((x1 * c - x2 * s, x2 * c + x1 * s), dim=-1)
@@ -167,6 +183,15 @@ def test_gather_kv_follows_a_shuffled_page_table():
     assert not K0.any()
 
 
+def test_project_rows_matches_project():
+    cfg, w = transparent_model(12, 3, seed=4)
+    toks, pos = [5, 900, 5, 2047], [0, 3, 700, 2046]
+    q, k, v = project_rows(cfg, w, toks, pos)
+    for i, (t, p) in enumerate(zip(toks, pos)):
+        q1, k1, v1 = project(cfg, w, t, p, rb=True)
+        assert rel_rms(q[i], q1) < 1e-14 and rel_rms(k[i], k1) < 1e-14 and rel_rms(v[i], v1) < 1e-14, i
+
+
 def test_rope64_matches_oracle_rope():
     g = torch.Generator().manual_seed(3)
     x = torch.randn(3, 64, generator=g, dtype=torch.float64)
@@ -176,6 +201,9 @@ def test_rope64_matches_oracle_rope():
         # the oracle computes inv_freq in fp32 arithmetic, the library (and rope64) rounds the float64 value to fp32:
         # at position 4095 the angles differ by a few 1e-6
         assert rel_rms(rope64(x, pos, 1e6), want) < 2e-5
+    pos = torch.tensor([0, 1, 700, 4095])
+    xs = torch.randn(4, 3, 64, generator=g, dtype=torch.float64)
+    assert torch.equal(rope64(xs, pos, 1e6), torch.stack([rope64(xs[i], int(p), 1e6) for i, p in enumerate(pos)]))
 
 
 # ====================================================================================== attention-transparent model
@@ -213,6 +241,18 @@ def project(cfg, w, tok: int, pos: int, rb: bool):
     q = rope64(lin("q").view(cfg.num_heads, 64), pos, cfg.rope_theta)
     k = rope64(lin("k").view(cfg.num_kv_heads, 64), pos, cfg.rope_theta)
     return q, k, lin("v").view(cfg.num_kv_heads, 64)
+
+
+def project_rows(cfg, w, toks, pos):
+    """``project(..., rb=True)`` of token rows ``toks`` [T] at positions ``pos`` [T] at once: float64 q [T, n_heads,
+    64], k, v [T, n_kv, 64] from the bf16-rounded normalised input, as the prefill's wgmma GEMM reads it."""
+    L0 = w.layers[0]
+    e = w.embed[torch.as_tensor(toks, dtype=torch.long)].double()
+    x = (e / torch.sqrt(e.pow(2).mean(-1, keepdim=True) + cfg.rms_eps) * L0["ln1"].double()).bfloat16().double()
+    lin = lambda n, heads: (x @ L0["w" + n].double().T + L0["b" + n].double()).view(len(toks), heads, 64)
+    pos = torch.as_tensor(pos)
+    return (rope64(lin("q", cfg.num_heads), pos, cfg.rope_theta), rope64(lin("k", cfg.num_kv_heads), pos, cfg.rope_theta),
+            lin("v", cfg.num_kv_heads))
 
 
 def transparent_logits(cfg, w, tok: int, attn, rb: bool):
@@ -325,8 +365,8 @@ def _prefill_errors(lm, cfg, slots, lens):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("n_heads,n_kv", [(4, 4), (4, 2), (9, 3), (14, 2), (8, 1)],
-                         ids=["gqa1", "gqa2", "gqa3", "gqa7", "gqa8"])
+@pytest.mark.parametrize("n_heads,n_kv", [(4, 4), (4, 2), (9, 3), (8, 2), (10, 2), (12, 2), (14, 2), (8, 1)],
+                         ids=["gqa1", "gqa2", "gqa3", "gqa4", "gqa5", "gqa6", "gqa7", "gqa8"])
 def test_prefill_attention_vs_float64(cuda, n_heads, n_kv):
     """attn_prefill_kernel on its own operands: one ragged prefill, lengths on the 16-query / 64-key tile edges up to
     the context limit, shuffled pages, q / k scaled so the softmax is peaked.  Worst per-(sequence, head) error
@@ -340,6 +380,50 @@ def test_prefill_attention_vs_float64(cuda, n_heads, n_kv):
     errs = _prefill_errors(lm, cfg, range(len(PREFILL_LENS)), PREFILL_LENS)
     print(f"PREFILL-ATTN gqa{n_heads // n_kv} ({n_heads}/{n_kv}): " + " ".join(f"{n}:{e:.2e}" for n, e in zip(PREFILL_LENS, errs)))
     assert max(errs) < BARS["prefill"], errs
+
+
+# (query heads, KV heads) of the GQA-ratio cases: every ratio from 1 to 8, ratio 4 over 2 and over 3 KV heads, hidden =
+# 64 * query heads <= 896 (the widest the persistent kernel plans for).  gqa7 is NeuTTS-Air's attention, gqa4 the Nano
+# shape's.
+RATIO_MODELS = {"gqa1": (8, 8), "gqa2": (4, 2), "gqa3": (9, 3), "gqa4": (8, 2), "gqa4kv3": (12, 3), "gqa5": (10, 2),
+                "gqa6": (12, 2), "gqa7": (14, 2), "gqa8": (8, 1)}
+
+
+def row_head_err(got, ref) -> float:
+    """Worst relative RMS error over (row, head); got / ref: [rows, heads, 64].  inf when ``got`` is not finite."""
+    if not torch.isfinite(got).all():
+        return math.inf
+    g, r = got.double(), ref.double()
+    return float(((g - r).pow(2).sum(-1) / r.pow(2).sum(-1).clamp_min(1e-300)).sqrt().max())
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("model", list(RATIO_MODELS))
+def test_prefill_rope_rows_vs_float64(cuda, model):
+    """rope_append_kernel: the prefill's rotated q buffer and every cached K and V row, per (row, head), against
+    rope64(bf16(rmsnorm(e) * ln1) @ W + b, pos) in float64 (K and V rounded to bf16 as cached).  Two ragged prefills:
+    the first PREFILL_LENS, few rows, where the qkv GEMM splits K into slices that the kernel sums (at hidden >= 512),
+    then all of PREFILL_LENS, where it does not."""
+    n_heads, n_kv = RATIO_MODELS[model]
+    cfg, w = transparent_model(n_heads, n_kv, seed=200 + n_heads + n_kv, qk_std=2.5)
+    H, QN = cfg.hidden_size, (n_heads + 2 * n_kv) * 64
+    lm = make_lm(cfg, w, max_batch=len(PREFILL_LENS), max_ctx=2048, page_shuffle_seed=n_kv)
+    g = torch.Generator().manual_seed(n_heads)
+    sp = lm.sampling(cfg.vocab_size - 1, min_new_tokens=0, max_new_tokens=2)
+    for lens in (PREFILL_LENS[:4], PREFILL_LENS):
+        T = sum(lens)
+        splits = gemm_splits(T, QN, H, 8 * 128 * max(QN, H))          # lm->splitk_floats
+        assert (splits > 1) == (T < 100 and H >= 512), splits
+        prompts = [torch.randint(0, cfg.vocab_size, (n,), generator=g).tolist() for n in lens]
+        lm.prefill(prompts, sp)
+        torch.cuda.synchronize()
+        q = lm.debug_buffer("q", (T, n_heads * 64)).double().cpu().view(T, n_heads, 64)
+        K, V = (torch.cat(t) for t in zip(*(gather_kv(lm, 0, b, n) for b, n in enumerate(lens))))
+        rq, rk, rv = project_rows(cfg, w, [t for p in prompts for t in p], torch.cat([torch.arange(n) for n in lens]))
+        errs = (row_head_err(q, rq), row_head_err(K, rk.bfloat16()), row_head_err(V, rv.bfloat16()))
+        print(f"PREFILL-ROPE {model} ({n_heads}/{n_kv}) T={T} split-K {splits}: q {errs[0]:.2e} K {errs[1]:.2e} "
+              f"V {errs[2]:.2e}")
+        assert errs[0] < BARS["prefill-q"] and max(errs[1:]) < BARS["row-head"], (T, errs)
 
 
 @pytest.mark.gpu
@@ -374,32 +458,54 @@ def _lens(B, lo, hi, seed):
     return out
 
 
-DECODE_CASES = [
-    ("chain-fp32-b1", "perop", [2047], 2048, None, "fp32"),
-    ("chain-fp32-b4", "perop", [511, 512, 513, 1000], 2048, None, "fp32"),
-    ("chain-mma-b6", "perop", [2047, 1000, 513, 512, 511, 64], 2048, "mma", "mma"),
-    ("chain-mma-b34", "perop", [511, 512, 513] + _lens(31, 64, 2047, 1), 2048, "mma", "mma"),
-    ("persistent-b1", None, [2047], 2048, "mma", "tc-b1"),
-    ("persistent-b4", None, [2047, 1000, 513, 1500], 2048, "mma", "tc-hilo"),
-    ("persistent-b8", None, _lens(8, 900, 2047, 2), 2048, "mma", "tc-hilo"),
-    ("persistent-b16", None, _lens(16, 1200, 2047, 3), 2048, "mma", "tc-bf16"),
-    ("persistent-b34-ctx4096", "tc", _lens(34, 2049, 4095, 4), 4096, "mma", "tc-pagefallback"),
+_RATIO_PATHS = [   # (id, impl, lens, mirror, branch): the paths every RATIO_MODELS shape runs
+    ("chain-fp32-b1", "perop", [2047], None, "fp32"),
+    ("chain-fp32-b4", "perop", [511, 512, 513, 1000], None, "fp32"),
+    ("chain-mma-b6", "perop", [2047, 1000, 513, 512, 511, 64], "mma", "mma"),
+    ("persistent-b1", None, [2047], "mma", "tc-b1"),
+    ("persistent-b8", None, _lens(8, 900, 2047, 2), "mma", "tc-hilo"),
+    ("persistent-b16", None, _lens(16, 1200, 2047, 3), "mma", "tc-bf16"),
 ]
+# (id, model, impl, lens, max_ctx, mirror, branch); model: a RATIO_MODELS key.  8/8 at batch 16 has 128 (sequence, KV
+# head) pairs: on a 132-SM H100 each gets one attention split ("tc-bf16-cap1").  8/1 at batch 16 has 8 splits of at most
+# 4 pages, one page per attention warp ("tc-bf16-1page").
+DECODE_CASES = [
+    ("chain-fp32-b1", "gqa7", "perop", [2047], 2048, None, "fp32"),
+    ("chain-fp32-b4", "gqa7", "perop", [511, 512, 513, 1000], 2048, None, "fp32"),
+    ("chain-mma-b6", "gqa7", "perop", [2047, 1000, 513, 512, 511, 64], 2048, "mma", "mma"),
+    ("chain-mma-b34", "gqa7", "perop", [511, 512, 513] + _lens(31, 64, 2047, 1), 2048, "mma", "mma"),
+    ("persistent-b1", "gqa7", None, [2047], 2048, "mma", "tc-b1"),
+    ("persistent-b4", "gqa7", None, [2047, 1000, 513, 1500], 2048, "mma", "tc-hilo"),
+    ("persistent-b8", "gqa7", None, _lens(8, 900, 2047, 2), 2048, "mma", "tc-hilo"),
+    ("persistent-b16", "gqa7", None, _lens(16, 1200, 2047, 3), 2048, "mma", "tc-bf16"),
+    ("persistent-b34-ctx4096", "gqa7", "tc", _lens(34, 2049, 4095, 4), 4096, "mma", "tc-pagefallback"),
+] + [(f"{model}-{name}", model, impl, lens, 2048, mirror,
+      {("gqa1", "tc-bf16"): "tc-bf16-cap1", ("gqa8", "tc-bf16"): "tc-bf16-1page"}.get((model, branch), branch))
+     for model in RATIO_MODELS if model != "gqa7" for name, impl, lens, mirror, branch in _RATIO_PATHS]
 
 
-def _assert_branch(lm, branch, lens, launches, steps):
+def _assert_branch(lm, branch, lens, launches, steps, impl):
+    """The path the case meant to test: decode_branch's prediction, the launch count and the split-KV geometry."""
     B = len(lens)
+    s = lm.shape
+    sms = min(torch.cuda.get_device_properties(0).multi_processor_count, 256)
+    br = decode_branch((s.hidden_size, s.intermediate_size, s.num_heads, s.num_kv_heads, s.vocab_size), B, sms,
+                       lm.max_ctx, impl)
     npages = [-(-(L + 1) // PAGE) for L in lens]
     if branch in ("fp32", "mma"):
+        assert br["name"] == ("gemv" if branch == "fp32" else "gemm"), br
         assert launches > steps, launches                     # the per-op chain: several kernels per step
         # more than 8 pages: each of the 8 warp pairs (fp32) / warps (mma) walks several pages
         assert max(npages) > 8
-        return
+        return br
+    bf16 = branch.startswith("tc-bf16") or branch == "tc-pagefallback"
+    assert br["kind"] == "tc" and br["act"] == ("bf16" if bf16 else "hilo"), br
+    assert br["fold"] == (branch == "tc-b1"), br
     assert launches == 1, launches                            # one launch: the persistent kernel
-    sms = torch.cuda.get_device_properties(0).multi_processor_count
     geo = [tc_geometry(lm, B, L, sms) for L in lens]
     cap = geo[0][0]
-    if branch != "tc-pagefallback":
+    assert cap == br["split_cap"], (cap, br)
+    if branch not in ("tc-pagefallback", "tc-bf16-cap1"):
         assert cap > 1 and max(g[2] for g in geo) == cap      # the merge sees split_cap partials
     if branch == "tc-b1":
         assert cap == min(8, sms // lm.shape.num_kv_heads) and geo[0][3] == 2 and geo[0][1] > geo[0][3]
@@ -407,8 +513,13 @@ def _assert_branch(lm, branch, lens, launches, steps):
         assert 1 < B <= 8 and max(g[1] for g in geo) > 1
     elif branch == "tc-bf16":
         assert B > 8 and cap == min(8, sms // (B * lm.shape.num_kv_heads)) and max(g[1] for g in geo) > geo[0][3]
+    elif branch == "tc-bf16-1page":  # split_cap partials of at most one page per attention warp
+        assert B > 8 and cap == min(8, sms // (B * lm.shape.num_kv_heads)) and max(g[1] for g in geo) == geo[0][3]
+    elif branch == "tc-bf16-cap1":   # one split per (sequence, KV head): its warps walk every page, no merge
+        assert B > 8 and cap == 1 and all(g[2] == 1 for g in geo) and max(g[1] for g in geo) > geo[0][3]
     elif branch == "tc-pagefallback":
         assert cap == 1 and max(g[1] for g in geo) > 32       # pages past the 32-entry cache: page_of's global load
+    return br
 
 
 @pytest.mark.gpu
@@ -418,12 +529,14 @@ def test_decode_attention_vs_float64(cuda, case, monkeypatch):
     the first, far and last pages make every page and every split-KV partial count; poison behind the context makes a
     leaked row blow the error up by orders of magnitude.  Also checks the K/V row the step appended.  Worst errors
     measured: see BARS."""
-    name, impl, lens, max_ctx, mirror, branch = case
-    cfg, w = transparent_model(14, 2, seed=5)
+    name, model, impl, lens, max_ctx, mirror, branch = case
+    n_heads, n_kv = RATIO_MODELS[model]
+    cfg, w = transparent_model(n_heads, n_kv, seed=5 if model == "gqa7" else 5 + 16 * n_heads + n_kv)
     lm, forced, logits, launches, rb = run_crafted_decode(cfg, w, lens, 1, impl, max_ctx, monkeypatch, seed=len(lens))
-    _assert_branch(lm, branch, lens, launches, 1)
+    br = _assert_branch(lm, branch, lens, launches, 1, impl)
     attn_err, row_err = check_decode(cfg, w, lm, forced, logits, lens, 1, mirror, rb)
-    print(f"DECODE-ATTN {name}: attention {attn_err:.2e} appended row {row_err:.2e} (launches {launches})")
+    print(f"DECODE-ATTN {name}: ratio {n_heads // n_kv} ({n_heads}/{n_kv}) [{br['name']}, split_cap {br['split_cap']}, "
+          f"launches {launches}]: attention {attn_err:.2e} appended row {row_err:.2e}")
     assert attn_err < BARS["decode-" + ("fp32" if mirror is None else ("bf16" if rb else "mma"))], attn_err
     assert row_err < BARS["row"], row_err
 

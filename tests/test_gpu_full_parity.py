@@ -6,7 +6,8 @@ reference semantics) AND with the real ``transformers.Qwen2ForCausalLM`` forward
   (a) configs[1]: 500-token prompt + 16 teacher-forced decode steps, batch 1;
   (b) configs[2]: batch 64 with ragged prompts U{200..1400}, 4 of the 64 slots checked against the oracle;
   (c) context limit: a 2040-token prompt decoded to the max_ctx = 2048 stop (``done``, ``seq_lens``, logits);
-  (d) a Nano-like shape (hidden 576, 9 heads / 3 KV heads, inter 1536) to show the kernels are config-driven.
+  (d) a Nano-like shape (hidden 576, 9 heads / 3 KV heads, inter 1536) to show the kernels are config-driven;
+  (e) the Nano-like shape bench.py streams (hidden 512, 8 / 2 heads, inter 2048, 28 layers, V = 217 472) at batch 8.
 
 Bars (relative RMS error of the logits / max error in units of the logit spread), stated per test:
 vs the pure-fp32 reference 2e-2 / 1e-1 — the CUDA path keeps bf16 weights (shared with the oracle), a bf16 KV
@@ -19,7 +20,7 @@ import pytest
 import torch
 
 from oracle import lm_oracle as O
-from tests.helpers import make_lm, max_err, rel_err
+from tests.helpers import decode_branch, make_lm, max_err, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -160,3 +161,40 @@ def test_nano_like_shape(cuda, B):
     for b in range(B):
         _, ref = O.generate(cfg, w, prompts[b], cfg.vocab_size - 1, max_length=512, max_new_tokens=n_new, forced=forced[b], mirror=False)
         _bars(got[b], ref, f"nano-like B={B} slot {b}")
+
+
+# The Nano-like model bench.py measures in its streaming line: hidden 512, 8 query / 2 KV heads (GQA ratio 4), inter 2048
+BENCH_NANO = dict(vocab_size=217472, hidden_size=512, intermediate_size=2048, num_layers=28, num_heads=8, num_kv_heads=2)
+
+
+def test_bench_nano_shape_b8(cuda):
+    """The benchmark's streaming shape end to end: 28 layers, V = 217 472, batch 8, 500-token prompts, then 16
+    teacher-forced steps in one launch of the persistent kernel (hi + lo activations, whole-K plan); slots 0 and 5
+    against the oracle, prefill and decode rows."""
+    torch.set_num_threads(min(16, os.cpu_count() or 1))
+    cfg = O.LMConfig.tiny(**BENCH_NANO)
+    w = O.random_weights(cfg, 23, std=0.02, bf16_round=True)
+    B, P, n_new = 8, 500, 17
+    lm = make_lm(cfg, w, max_batch=B, max_ctx=2048, max_new=32, max_prefill_tokens=B * P, page_shuffle_seed=5)
+    g = torch.Generator().manual_seed(9)
+    prompts = [torch.randint(0, cfg.vocab_size, (P,), generator=g) for _ in range(B)]
+    forced = torch.randint(0, cfg.vocab_size, (B, n_new), generator=g)
+    eos = cfg.vocab_size - 1
+    sp = lm.sampling(eos, min_new_tokens=0, max_new_tokens=n_new, forced=forced)
+    l0 = lm.prefill([p.tolist() for p in prompts], sp, return_logits=True)
+    torch.cuda.synchronize()
+    n0 = lm.L.nt_launch_count()
+    ls = lm.decode(n_new - 1, sp, return_logits=True)
+    torch.cuda.synchronize()
+    launches = lm.L.nt_launch_count() - n0
+    got = torch.cat((l0[None], ls), 0).permute(1, 0, 2).float().cpu()
+    sms = min(torch.cuda.get_device_properties(0).multi_processor_count, 256)
+    br = decode_branch((cfg.hidden_size, cfg.intermediate_size, cfg.num_heads, cfg.num_kv_heads, cfg.vocab_size), B, sms,
+                       2048)
+    print(f"FULL-PARITY bench-nano B={B}: decode [{br['name']}, {launches} launches]")
+    assert br["name"] == "tc-hilo-n16-wholeK-phases" and launches == 1, (br, launches)
+    assert lm.out_tokens[:B, :n_new].cpu().tolist() == forced.tolist()
+    for b in (0, 5):
+        _, ref = O.generate(cfg, w, prompts[b], eos, max_length=2048, max_new_tokens=n_new, forced=forced[b], mirror=False)
+        _bars(got[b, :1], ref[:1], f"bench-nano B={B} slot {b} prefill(500)")
+        _bars(got[b, 1:], ref[1:], f"bench-nano B={B} slot {b} 16 decode steps")

@@ -48,7 +48,7 @@ import pytest
 import torch
 
 from oracle import lm_oracle as O
-from tests.helpers import (GEMV_MAX_BATCH, decode_branch, gather_kv, make_lm, plan_regime, plan_summary,
+from tests.helpers import (GEMV_MAX_BATCH, decode_branch, gather_kv, gemm_splits, make_lm, plan_regime, plan_summary,
                            regime_representatives, rel_rms, set_decode_impl)
 from tests.sampler_ref import prob_err, ref_window
 
@@ -72,7 +72,10 @@ LOUD0 = EOS - N_LOUD              # ids [LOUD0, EOS): embedding rows scaled by 2
 N_LAYERS = 3
 STEPS = 4
 MAX_CTX = 512
-SHAPES = {"air": (896, 4864, 14, 2), "nano": (576, 1536, 9, 3), "small": (256, 640, 4, 2)}
+# NeuTTS-Air and NeuTTS-Nano widths, a small model, the Nano-like model bench.py measures in its streaming line (8 query
+# / 2 KV heads: GQA ratio 4) and Air widths over 16 query / 4 KV heads
+SHAPES = {"air": (896, 4864, 14, 2), "nano": (576, 1536, 9, 3), "small": (256, 640, 4, 2), "bench": (512, 2048, 8, 2),
+          "air16x4": (896, 4864, 16, 4)}
 
 NONE = frozenset()
 PREFILL_GEMV = frozenset({"x", "attn", "act"})
@@ -315,6 +318,15 @@ DECODE_CASES = [
     ("nano-tc-b6", "nano", 6, None, "tc-hilo-n16-wholeK-phases"),
     ("small-tc-b1", "small", 1, None, "tc-hilo-n16-flat-fold"),
     ("small-tc-b12", "small", 12, None, "tc-bf16-n16-wholeK-phases"),
+    ("bench-tc-b1", "bench", 1, None, "tc-hilo-n16-wholeK-fold"),
+    ("bench-tc-b3", "bench", 3, None, "tc-hilo-n16-wholeK-phases"),
+    ("bench-tc-b8", "bench", 8, None, "tc-hilo-n16-wholeK-phases"),
+    ("bench-tc-b9", "bench", 9, None, "tc-bf16-n16-wholeK-phases"),
+    ("bench-tc-b16", "bench", 16, None, "tc-bf16-n16-wholeK-phases"),
+    ("bench-chain-b4", "bench", 4, "perop", "gemv"),
+    ("bench-chain-b6", "bench", 6, "perop", "gemm"),
+    ("air16x4-tc-b1", "air16x4", 1, None, "tc-hilo-n16-flat-fold"),
+    ("air16x4-tc-b8", "air16x4", 8, None, "tc-hilo-n16-wholeK-phases"),
 ]
 
 
@@ -521,24 +533,10 @@ def test_debug_set_sms_refuses_counts_the_device_cannot_run(cuda):
     lm.debug_set_sms(0)
 
 
-def _gemm_splits(M: int, N: int, K: int, ws_floats: int) -> int:
-    """Split-K slices gemm_dispatch picks for an M x N x K bf16 GEMM with a split workspace (restated)."""
-    sms = torch.cuda.get_device_properties(0).multi_processor_count
-    mt = -(-M // 128)
-    bn = 128
-    if mt * -(-N // 128) < sms * 13 // 16:
-        bn = 64
-    if mt * -(-N // 64) < sms * 11 // 16:
-        bn = 32
-    tiles, nkb = mt * -(-N // bn), -(-K // 64)
-    if tiles > 48 or nkb < 8:
-        return 1
-    sk = min((sms - 4) // tiles, nkb // 4, 8)
-    return sk if sk > 1 and M * N * sk <= ws_floats else 1
-
-
-# (id, lens, split-K GEMMs)
-PREFILL_CASES = [("air-prefill-b3-t70", [17, 1, 52], True), ("air-prefill-b6-t700", [200, 64, 129, 1, 250, 56], False)]
+# (id, shape, lens, split-K GEMMs)
+PREFILL_CASES = [("air-prefill-b3-t70", "air", [17, 1, 52], True),
+                 ("air-prefill-b6-t700", "air", [200, 64, 129, 1, 250, 56], False),
+                 ("bench-prefill-b5-t90", "bench", [33, 1, 17, 38, 1], True)]
 
 
 @pytest.mark.gpu
@@ -546,8 +544,8 @@ PREFILL_CASES = [("air-prefill-b3-t70", [17, 1, 52], True), ("air-prefill-b6-t70
 def test_prefill_projections_vs_float64(cuda, case):
     """A ragged prefill after a prefill of every slot with loud prompts: the last-row logits, the final residual of
     every token row at index >= max_batch and every V row, against the float64 model on the run's own cache."""
-    name, lens, split = case
-    shape, B = "air", len(lens)
+    name, shape, lens, split = case
+    B = len(lens)
     cfg, w = avg_model(shape)
     H, I, nh, nkv = SHAPES[shape]
     MB = B + 2
@@ -558,7 +556,7 @@ def test_prefill_projections_vs_float64(cuda, case):
     prompts = [torch.randint(0, LOUD0, (n,), generator=g).tolist() for n in lens]
     T = sum(lens)
     ws = 8 * 128 * max((nh + 2 * nkv) * 64, H)                      # lm->splitk_floats
-    splits = [_gemm_splits(T, N, K, ws) for N, K in (((nh + 2 * nkv) * 64, H), (H, 64 * nh), (H, I))]
+    splits = [gemm_splits(T, N, K, ws) for N, K in (((nh + 2 * nkv) * 64, H), (H, 64 * nh), (H, I))]
     assert all(s > 1 for s in splits) if split else all(s == 1 for s in splits), splits
     logits = lm.prefill(prompts, sp, return_logits=True)
     torch.cuda.synchronize()
