@@ -108,7 +108,7 @@ struct nt_lm {
   __nv_bfloat16 *xn, *attn_bf16, *act_bf16;
   // persistent decode kernel tables (device)
   const float** ptr_tab;   // [3][n_layers]: ln1, bqkv, ln2
-  unsigned* gbar;          // grid barrier counter (word 0) and the batch-1 tile arrival counters (words kTcCntOff..)
+  unsigned* gbar;          // grid barrier counter (word 0) and the batch-1 tile arrival counters (kTcBarWords words)
   // cached decode-step graph
   cudaGraphExec_t graph = nullptr;
   std::vector<uint8_t> graph_key;
@@ -130,7 +130,7 @@ struct nt_lm {
   __nv_bfloat16 *tc_xa = nullptr, *tc_act = nullptr;
   float* tmax = nullptr;              // [max_batch][ceil(V / 128)] tile maxima of the logits rows (see lm_head_rows)
   float2 *tc_pq2 = nullptr, *tc_po2 = nullptr, *tc_pd2 = nullptr, *tc_ao2 = nullptr, *tc_aml2 = nullptr, *tc_act2 = nullptr, *tc_pg2 = nullptr,
-         *tc_h2 = nullptr;
+         *tc_qkv2 = nullptr, *tc_h2 = nullptr;
   size_t tc_pair_bytes = 0;           // extent of the stamped buffers (contiguous, starting at tc_pq2)
   int tc_stamp = 0, tc_hstamp = 0;    // stamps handed out so far (see TcParams::stamp_base)
   // prefill into chosen slots (nt_lm_prefill_slots)
@@ -222,7 +222,7 @@ static size_t lm_carve(const nt_lm_config& c, void* ws, size_t bytes, F&& assign
     (L)->attn_bf16 = a.take<__nv_bfloat16>(size_t(rows) * c.n_heads * 64);                     \
     (L)->act_bf16 = a.take<__nv_bfloat16>(size_t(rows) * I);                                   \
     (L)->ptr_tab = a.take<const float*>(size_t(3) * c.n_layers);                               \
-    (L)->gbar = a.take<unsigned>(64);                                                          \
+    (L)->gbar = a.take<unsigned>(kTcBarWords);                                                 \
     (L)->splitk_floats = size_t(8) * 128 * (qkv_n > H ? qkv_n : H);                            \
     (L)->splitk_ws = a.take<float>(size_t(8) * 128 * (qkv_n > H ? qkv_n : H));                 \
     (L)->tc_rows = c.max_batch < kTcMaxBatch ? c.max_batch : kTcMaxBatch;                      \
@@ -238,6 +238,7 @@ static size_t lm_carve(const nt_lm_config& c, void* ws, size_t bytes, F&& assign
     (L)->tc_aml2 = a.take<float2>(size_t((L)->tc_rows) * c.n_heads * max_splits * 2);          \
     (L)->tc_act2 = a.take<float2>(size_t(4) * I);                                              \
     (L)->tc_pg2 = a.take<float2>(size_t(kTcMaxGuSlices) * 4 * 2 * I);                          \
+    (L)->tc_qkv2 = a.take<float2>(qkv_n);                                                      \
     (L)->tc_h2 = a.take<float2>(size_t(2) * 4 * H);                                            \
     (L)->tc_pair_bytes = size_t(reinterpret_cast<uint8_t*>((L)->tc_h2 + size_t(2) * 4 * H) - reinterpret_cast<uint8_t*>((L)->tc_pq2)); \
     (L)->slot_key = a.take<int>(c.max_batch);                                                  \
@@ -280,7 +281,7 @@ static int tc_setup(nt_lm* lm) {
   std::vector<unsigned char> nsl(4096, 0);
   TcShape ts{c.hidden, c.inter, c.n_heads, c.n_kv_heads, lm->qkv_n, c.vocab_size};
   const int G = lm->num_sms;
-  lm->tc_flat_ok = (2 * c.inter + 127) / 128 <= 4096 &&
+  lm->tc_flat_ok = (2 * c.inter + 127) / 128 <= kTcMaxGuTiles &&
                    tc_build_plan(ts, G, true, plan.data() + 256, nsl.data(), &lm->tc_info[1]) == NT_OK;
   if (tc_build_plan(ts, G, false, plan.data(), nullptr, &lm->tc_info[0]) != NT_OK) return NT_OK;
   if (!lm->tc_maps_ok) {
@@ -976,7 +977,7 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
     P.h = lm->h, P.xa = lm->tc_xa, P.act = lm->tc_act;
     P.pq2 = lm->tc_pq2, P.po2 = lm->tc_po2, P.pd2 = lm->tc_pd2;
     P.sq = info.sq, P.so = info.so, P.sd = info.sd;
-    P.ao2 = lm->tc_ao2, P.aml2 = lm->tc_aml2, P.act2 = lm->tc_act2, P.h2 = lm->tc_h2, P.max_splits = lm->max_splits;
+    P.ao2 = lm->tc_ao2, P.aml2 = lm->tc_aml2, P.act2 = lm->tc_act2, P.h2 = lm->tc_h2, P.qkv2 = lm->tc_qkv2, P.max_splits = lm->max_splits;
     // (value, stamp) hand-offs: every launch takes a fresh range of stamps, so nothing left in the buffers by an
     // earlier launch (or by another batch size) can ever match
     const int need_s = n_steps * (tc_layers + 1) + 2, need_h = n_steps * (2 * tc_layers + 1) + 4;

@@ -19,7 +19,8 @@
 //       [fold+RMSNorm] qkv -> RoPE/KV-append + split-KV attention -> merge + o_proj -> [fold+RMSNorm] gate/up+SwiGLU
 //       -> down
 //     batch 1: no grid barrier inside a layer; the last producer of each o_proj / down_proj row tile folds it into the
-//     residual stream, and the consumers normalise that row while staging their B operand; larger batches:
+//     residual stream, and the consumers normalise that row while staging their B operand; the last producer of each
+//     qkv / gate/up row tile hands attention (bias + RoPE applied) and down_proj (SwiGLU applied) finished rows; larger batches:
 //     token-owner CTAs fold + normalise into bf16 rows that the consumers fetch by TMA (3 barriers per layer, no
 //     per-CTA re-reading of the whole batch).
 //   lm_head epilogue: logits -> HBM once, plus the processed maximum of every 128-row tile; the sampler then needs
@@ -96,6 +97,13 @@ NT_DEVINL void split_hilo(float x, __nv_bfloat16& hi, __nv_bfloat16& lo) {
 
 NT_DEVINL void tc_spin_check(uint32_t& spins, const char* what) {
   if (++spins > (1u << 22)) nt_timeout(what);
+}
+
+// RoPE of the adjacent qkv rows (2i, 2i + 1) = dims (i, i + 32) of a head, sc = rope_sincos(pos, inv_freq[i]):
+// rope_pair's rotation, but dim i + 32 fuses x sin and rounds y cos where rope_pair does the opposite -- the rounding
+// this kernel has always had, which keeps its decode output bit-identical
+NT_DEVINL float2 tc_rope(float2 a, float2 sc) {
+  return make_float2(__fmaf_rn(a.x, sc.y, -__fmul_rn(a.y, sc.x)), __fmaf_rn(a.x, sc.x, __fmul_rn(a.y, sc.y)));
 }
 
 // 4 consecutive elements of row b: residual pairs (or nothing) + the split-K slices in slice order; polls the stamps
@@ -284,11 +292,17 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
     //     writer of n polls version n - 1 of tile t before it writes;
     //   * the consumers of fold n - 2, which read the whole row.  A consumer has items in the GEMM that follows its
     //     fold and runs them after the read.  Version n - 1 of tile t needs the slices of every item of that GEMM:
-    //     gate/up items feed down_proj k-blocks, and every down tile's slices cover all of them; qkv items feed the
-    //     attention of every split (q rows) or of the appending split (k/v rows; split 0 reads them when no split
-    //     appends), and every o_proj tile's slices cover all heads and merge all their splits.  The writer of n polls
-    //     version n - 1 of tile t, so it comes after every such read.
+    //     every slice of a gate/up or qkv tile is read by the tile's last producer, which publishes the tile only
+    //     after that read.  Gate/up tiles feed down_proj k-blocks, and every down tile's slices cover all of them; qkv
+    //     tiles feed the attention of every split (q rows) or of the appending split (k/v rows; split 0 reads them
+    //     when no split appends), and every o_proj tile's slices cover all heads and merge all their splits.  The
+    //     writer of n polls version n - 1 of tile t, so it comes after every such read.
     //   After the final norm the sampler writes the next version behind a grid barrier.
+    // qkv2 and act2 (the finished qkv and SwiGLU rows, stamp of the layer) hold one version.  The next layer's writer
+    // of a qkv2 tile is elected by qkv items that read the residual version behind this layer's down_proj, and the
+    // writer of an act2 tile by gate/up items behind the next layer's o_proj: by the chains above, those versions need
+    // every attention split's partials (which come after its qkv2 read) and every down item's slice (which comes
+    // after its act2 read).  The stamps reject whatever an earlier layer or launch left.
     int fold_no = 0;
 
     // ---- grid barrier; `post` runs on thread 0 between the release and the trailing CTA barrier
@@ -358,33 +372,40 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
       }
     };
 
-    // ---- batch 1, o_proj and down_proj: the CTA that stores the last of a row tile's S slices folds the tile into
-    //      the residual stream (epilogue warps; lane = row of the tile).  It reads residual version fold_no - 1 and the
-    //      S slices and adds them in the order every consumer used to: acc = residual, then slice 0 .. S - 1, plus the
-    //      zero padding of tc_fold4's batches of eight -- the same fp32 additions, so the same bits.  The result is
-    //      residual version fold_no, which the consumers of fold fold_no poll (one pair per element, tc_fold4 with no
-    //      slices).  It is stored kTcH2Copies times: with one copy every CTA of the grid polled the same 7 KB, and on
-    //      H100 that hot spot cost more than the L2 traffic the fold saves (bench.py measured 885-895 us per step with
-    //      one copy, 825-836 us with four).
+    // ---- batch 1: the CTA that stores the last of a row tile's S split-K slices folds the tile (epilogue warps; lane =
+    //      row of the tile) and publishes finished rows, which the consumers poll as one pair per element:
+    //        o_proj, down_proj: residual version fold_no - 1 plus the slices -> residual version fold_no (h2), read by
+    //          the consumers of fold fold_no (tc_fold4 with no slices);
+    //        qkv: the slices plus the bias, RoPE on q and k rows -> qkv2, read by the attention prologue;
+    //        gate/up (flat plan): the slices, then SwiGLU of the (gate, up) row pairs -> act2, read by stage_act.
+    //      The additions are the ones every consumer used to do, in the same order: acc = residual (or 0), then slice
+    //      0 .. S - 1, plus the zero padding of the readers' batches of eight (none for gate/up), then the bias -- the
+    //      same fp32 additions, so the same bits.  The residual is stored kTcH2Copies times: with one copy every CTA of
+    //      the grid polled the same 7 KB, and on H100 that hot spot cost more than the L2 traffic the fold saves
+    //      (bench.py measured 885-895 us per step with one copy, 825-836 us with four).  qkv2 and act2 have at most 8
+    //      and 7 readers per line and are stored once.
     //      The counter only elects the last arriver (S arrivals per tile and layer; it wraps to 0 on the last one, and
     //      the next layer's arrivals all depend on this fold).  Every value read is a (value, stamp) pair polled until
     //      its stamp matches, so the arrival needs no release/acquire: a slice whose store is not yet visible to the
     //      elected CTA is simply polled again.  Each lane issues its loads before the election returns, so the
     //      arrival's round trip and the reads overlap; the other S - 1 producers drop what they loaded.
     uint32_t tf_n = 0;   // tile_fold calls (parity of ms->tile_last)
-    auto tile_fold = [&](const float2* part, int S, int stamp, unsigned* cnt, int tile) {
+    auto tile_fold = [&](int ph, const float2* part, int rows, int S, int stamp, int tile, int l) {
+      const bool resid = ph == kPhO || ph == kPhD;
+      unsigned* cnt = P.tile_cnt + (ph == kPhQ ? kTcQkvCnt : (ph == kPhG ? kTcGuCnt : (ph == kPhD ? kTcMaxTiles : 0))) + tile;
       int* last = &ms->tile_last[tf_n++ & 1];   // two slots: a lane still reading one never sees the next election
       if (tid == 0) *last = tc_arrive_inc(cnt, static_cast<unsigned>(S - 1)) == static_cast<unsigned>(S - 1);
       const int row = tile * 128 + warp * 32 + lane;
-      const bool in = row < H;
+      const bool in = row < rows;
       const int hstamp = P.hstamp_base + fold_no;
       const float2* hsrc = P.h2 + static_cast<long long>((fold_no - 1) & 1) * kTcH2Copies * H + row;
       const float2* psrc = part + row;
       const float pad = __int_as_float(stamp);
-      float2 r = in ? ldp1(hsrc) : make_float2(0.f, __int_as_float(hstamp - 1));
+      float2 r = in && resid ? ldp1(hsrc) : make_float2(0.f, __int_as_float(hstamp - 1));
+      const float bias = in && ph == kPhQ ? __ldg(P.bqkv[l] + row) : 0.f;
       float2 t[kTcMaxSlices];
 #pragma unroll
-      for (int j = 0; j < kTcMaxSlices; ++j) t[j] = in && j < S ? ldp1(psrc + static_cast<long long>(j) * H) : make_float2(0.f, pad);
+      for (int j = 0; j < kTcMaxSlices; ++j) t[j] = in && j < S ? ldp1(psrc + static_cast<long long>(j) * rows) : make_float2(0.f, pad);
       bar_epi();
       if (!*last) return;
       pm(11);
@@ -402,24 +423,39 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
         tc_spin_check(spins, "split-K slices");
 #pragma unroll
         for (int j = 0; j < kTcMaxSlices; ++j)
-          if (in && j < S && __float_as_int(t[j].y) != stamp) t[j] = ldp1(psrc + static_cast<long long>(j) * H);
+          if (in && j < S && __float_as_int(t[j].y) != stamp) t[j] = ldp1(psrc + static_cast<long long>(j) * rows);
       }
-      // tc_fold4's order: slices in batches of eight, the last batch padded with zeros
-      const int nadd = (S + 7) & ~7;
+      // the readers' order: slices in batches of eight, the last batch padded with zeros (gate/up: no padding)
+      const int nadd = ph == kPhG ? S : (S + 7) & ~7;
       float acc = r.x;
 #pragma unroll
       for (int j = 0; j < kTcMaxSlices; ++j)
         if (j < nadd) acc += t[j].x;
-      if (in) {
-        float2* dst = P.h2 + static_cast<long long>(fold_no & 1) * kTcH2Copies * H + row;
+      if (resid) {
+        if (in) {
+          float2* dst = P.h2 + static_cast<long long>(fold_no & 1) * kTcH2Copies * H + row;
 #pragma unroll
-        for (int c = 0; c < kTcH2Copies; ++c) dst[static_cast<long long>(c) * H] = make_float2(acc, __int_as_float(hstamp));
+          for (int c = 0; c < kTcH2Copies; ++c) dst[static_cast<long long>(c) * H] = make_float2(acc, __int_as_float(hstamp));
+        }
+      } else {
+        // rows (2j, 2j + 1) pair up on adjacent lanes: q/k dims (j, j + 32) of a head, v dims, or (gate_j, up_j)
+        if (ph == kPhQ) acc += bias;
+        const float odd = __shfl_down_sync(0xffffffffu, acc, 1);
+        if (in && !(lane & 1)) {
+          if (ph == kPhG) {
+            P.act2[row >> 1] = make_float2(silu(acc) * odd, pad);
+          } else {
+            float2 v = make_float2(acc, odd);
+            if (row < (P.n_heads + P.n_kv) * 64) v = tc_rope(v, rope_sincos(ms->pos[0], __ldg(P.inv_freq + ((row & 63) >> 1))));
+            *reinterpret_cast<float4*>(P.qkv2 + row) = make_float4(v.x, pad, v.y, pad);
+          }
+        }
       }
       pm(12);
     };
 
     // ---- epilogue of the split-K phases: raw partial sums as (value, stamp) pairs, one row per lane
-    auto epi_partials = [&](int ph, float2* part, int rows, int stamp) {
+    auto epi_partials = [&](int ph, float2* part, int rows, int stamp, int l) {
       if (warp >= 4) return;
       const float sf = __int_as_float(stamp);
       for (int i = 0; i < plan.n[ph]; ++i) {
@@ -435,8 +471,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
             if (n < B) dst[static_cast<long long>(n) * rows] = make_float2(v[n], sf);
         }
         if constexpr (FOLD) {
-          if (ph == kPhO || ph == kPhD)
-            tile_fold(part, ph == kPhO ? P.so : P.sd, stamp, P.tile_cnt + (ph == kPhD ? kTcMaxTiles : 0) + it.tile, it.tile);
+          const int S = ph == kPhQ ? P.sq : (ph == kPhO ? P.so : (ph == kPhG ? __ldg(P.gu_nsl + it.tile) : P.sd));
+          tile_fold(ph, part, rows, S, stamp, it.tile, l);
         }
       }
     };
@@ -579,7 +615,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
       const int b = my_b, kvh = my_kvh;
       const int p0 = my_split * geo.pps, p1 = min(p0 + geo.pps, geo.npages);
       const bool appends = pos < P.kv.max_ctx && (pos >> 6) >= p0 && (pos >> 6) < p1;
-      // in-CTA fold: every qkv slice must be read by some split, or the h2 ping-pong loses its ordering (see fold_no)
+      // batch 1: every finished qkv row tile must be read by some split, or the h2 ping-pong and the single qkv2 version
+      // lose their ordering (see fold_no)
       const bool kv_rows = appends || (FOLD && pos >= P.kv.max_ctx && my_split == 0);
       if (!att_separate) {
         // the pages do not depend on this layer's projections (the new row is patched in below): fetch the first round now
@@ -587,7 +624,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
         if (warp < AW && p0 + warp < p1) issue_page(l, p0 + warp, p0, true);
       }
       pm(21);
-      // prologue: fold the qkv slices (slice order) + bias, RoPE; q of the group -> shared; new K/V row
+      // prologue: q of the group -> shared; new K/V row.  Batch 1 reads the rows the last producer of each qkv tile
+      // finished (tile_fold); larger batches fold the qkv slices (slice order) + bias and apply RoPE here.
       const float* bias = P.bqkv[l];
       const int QN = P.qkv_n;
       const float2* pq = P.pq2 + static_cast<long long>(b) * QN;
@@ -600,36 +638,44 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
         else if (which == 1) row0 = (P.n_heads + kvh) * 64 + 2 * i;
         else row0 = (P.n_heads + P.n_kv + kvh) * 64 + 2 * i;
         if (which != 0 && !kv_rows) continue;
-        const float2 bia = __ldg(reinterpret_cast<const float2*>(bias + row0));
-        // ahead of the wait for the slices, which hides its latency
-        const float2 sc = which != 2 ? rope_sincos(pos, __ldg(P.inv_freq + i)) : make_float2(0.f, 1.f);
-        float2 a = make_float2(0.f, 0.f);
-        for (int s0 = 0; s0 < P.sq; s0 += 8) {
-          float4 t[8];
+        float2 r;
+        if constexpr (FOLD) {
           uint32_t spins = 0;
           for (;;) {
-            bool ok = true;
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              t[j] = (s0 + j < P.sq) ? ldp2(pq + (s0 + j) * sstride + row0) : make_float4(0.f, __int_as_float(stamp), 0.f, __int_as_float(stamp));
-#pragma unroll
-            for (int j = 0; j < 8; ++j) ok = ok && __float_as_int(t[j].y) == stamp && __float_as_int(t[j].w) == stamp;
-            if (ok) break;
-            tc_spin_check(spins, "qkv slices");
+            const float4 t = ldp2(P.qkv2 + row0);
+            if (__float_as_int(t.y) == stamp && __float_as_int(t.w) == stamp) {
+              r = make_float2(t.x, t.z);
+              break;
+            }
+            tc_spin_check(spins, "qkv rows");
           }
-#pragma unroll
-          for (int j = 0; j < 8; ++j) a.x += t[j].x, a.y += t[j].z;
-        }
-        a.x += bia.x, a.y += bia.y;
-        if (which == 2) {
-          att_vnew[2 * i] = a.x, att_vnew[2 * i + 1] = a.y;
         } else {
-          // rope_pair's rotation, but dim i + 32 fuses x sin and rounds y cos where rope_pair does the opposite: the
-          // rounding this kernel has always had, which keeps its decode output bit-identical
-          const float2 r = make_float2(__fmaf_rn(a.x, sc.y, -__fmul_rn(a.y, sc.x)), __fmaf_rn(a.x, sc.x, __fmul_rn(a.y, sc.y)));
-          if (which == 0) att_q[(idx >> 5) * 64 + i] = r.x, att_q[(idx >> 5) * 64 + i + 32] = r.y;
-          else att_knew[i] = r.x, att_knew[i + 32] = r.y;
+          const float2 bia = __ldg(reinterpret_cast<const float2*>(bias + row0));
+          // ahead of the wait for the slices, which hides its latency
+          const float2 sc = which != 2 ? rope_sincos(pos, __ldg(P.inv_freq + i)) : make_float2(0.f, 1.f);
+          float2 a = make_float2(0.f, 0.f);
+          for (int s0 = 0; s0 < P.sq; s0 += 8) {
+            float4 t[8];
+            uint32_t spins = 0;
+            for (;;) {
+              bool ok = true;
+#pragma unroll
+              for (int j = 0; j < 8; ++j)
+                t[j] = (s0 + j < P.sq) ? ldp2(pq + (s0 + j) * sstride + row0) : make_float4(0.f, __int_as_float(stamp), 0.f, __int_as_float(stamp));
+#pragma unroll
+              for (int j = 0; j < 8; ++j) ok = ok && __float_as_int(t[j].y) == stamp && __float_as_int(t[j].w) == stamp;
+              if (ok) break;
+              tc_spin_check(spins, "qkv slices");
+            }
+#pragma unroll
+            for (int j = 0; j < 8; ++j) a.x += t[j].x, a.y += t[j].z;
+          }
+          a.x += bia.x, a.y += bia.y;
+          r = which == 2 ? a : tc_rope(a, sc);
         }
+        if (which == 2) att_vnew[2 * i] = r.x, att_vnew[2 * i + 1] = r.y;
+        else if (which == 0) att_q[(idx >> 5) * 64 + i] = r.x, att_q[(idx >> 5) * 64 + i + 32] = r.y;
+        else att_knew[i] = r.x, att_knew[i + 32] = r.y;
       }
       pm(22);
       csync();
@@ -721,7 +767,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
       pm(32);
     };
 
-    // ---- batch <= 4: down_proj input from the (value, stamp) SwiGLU outputs, two elements per thread
+    // ---- batch 1: down_proj input from the (value, stamp) SwiGLU outputs, two elements per thread.  They come from
+    //      epi_swiglu (whole-K gate/up) or, in the flat plan, from the last producer of each gate/up tile (tile_fold).
     auto stage_act = [&](int stamp) {
       csync();   // the B chunks of the gate/up phase are free (see stage_attn)
       const int nch = ms->bchunks[kPhD];
@@ -730,39 +777,12 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
         const int c = e / per, r = e - c * per, b = r >> 5, k = (r & 31) * 2;
         const int kbd = ms->ckb[kPhD][c];
         float4 t;
-        if (plan.gu_split) {
-          // flat plan: activations j, j + 1 = gate/up rows 2j .. 2j + 3 of tile kbd; fold its K slices (slice order), then SwiGLU
-          const int nsl = __ldg(P.gu_nsl + kbd);
-          const float2* p = P.pg2 + static_cast<long long>(b) * 2 * I + 2 * (kbd * 64 + k);
-          const long long sstride = static_cast<long long>(B) * 2 * I;
-          float4 u0[kTcMaxGuSlices], u1[kTcMaxGuSlices];
-          uint32_t spins = 0;
-          for (;;) {
-            bool ok = true;
-#pragma unroll
-            for (int sl = 0; sl < kTcMaxGuSlices; ++sl)
-              if (sl < nsl) u0[sl] = ldp2(p + sl * sstride), u1[sl] = ldp2(p + sl * sstride + 2);
-#pragma unroll
-            for (int sl = 0; sl < kTcMaxGuSlices; ++sl)
-              if (sl < nsl)
-                ok = ok && __float_as_int(u0[sl].y) == stamp && __float_as_int(u0[sl].w) == stamp && __float_as_int(u1[sl].y) == stamp &&
-                     __float_as_int(u1[sl].w) == stamp;
-            if (ok) break;
-            tc_spin_check(spins, "gate/up slices");
-          }
-          float g0 = 0.f, up0 = 0.f, g1 = 0.f, up1 = 0.f;
-#pragma unroll
-          for (int sl = 0; sl < kTcMaxGuSlices; ++sl)
-            if (sl < nsl) g0 += u0[sl].x, up0 += u0[sl].z, g1 += u1[sl].x, up1 += u1[sl].z;
-          t.x = silu(g0) * up0, t.z = silu(g1) * up1;
-        } else {
-          const float2* p = P.act2 + static_cast<long long>(b) * I + kbd * 64 + k;
-          uint32_t spins = 0;
-          for (;;) {
-            t = ldp2(p);
-            if (__float_as_int(t.y) == stamp && __float_as_int(t.w) == stamp) break;
-            tc_spin_check(spins, "SwiGLU outputs");
-          }
+        const float2* p = P.act2 + static_cast<long long>(b) * I + kbd * 64 + k;
+        uint32_t spins = 0;
+        for (;;) {
+          t = ldp2(p);
+          if (__float_as_int(t.y) == stamp && __float_as_int(t.w) == stamp) break;
+          tc_spin_check(spins, "SwiGLU outputs");
         }
         __nv_bfloat16 h0, l0, h1, l1;
         split_hilo(t.x, h0, l0);
@@ -936,7 +956,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
             const int rows = ph == kPhQ ? P.qkv_n : (ph == kPhG ? 2 * I : H);
             // one call site each: the down epilogue (with its tile fold) is inlined once
             if (ph == kPhG && !plan.gu_split) epi_swiglu(st);   // whole-K gate/up: SwiGLU in the epilogue
-            else epi_partials(ph, part, rows, st);
+            else epi_partials(ph, part, rows, st, l);
             if (tid == 0) prof.mark(100 + ph + (ph > 0 ? 1 : 0));   // 100 qkv, 102 o_proj, 103 gate/up, 104 down
           }
         }
@@ -974,7 +994,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
               if (plan.n[kPhO] > 0) stage_attn(st);
             }
             float2* part = ph == kPhQ ? P.pq2 : (ph == kPhO ? P.po2 : P.pd2);
-            epi_partials(ph, part, ph == kPhQ ? P.qkv_n : H, st);
+            epi_partials(ph, part, ph == kPhQ ? P.qkv_n : H, st, l);
             if (tid == 0) prof.mark(100 + ph + (ph > 0 ? 1 : 0));   // 100 qkv, 102 o_proj, 103 gate/up, 104 down
           }
           const bool last = l + 1 == L;
@@ -1254,7 +1274,7 @@ static int launch_tc(TcParams& P, int num_sms, cudaStream_t stream) {
   int per_sm = 0;
   NT_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kTcThreads, smem));
   if (per_sm < 1) return set_error(NT_ERR_CUDA, "decode_tc: a CTA does not fit on an SM (%zu B shared memory)", smem);
-  NT_CUDA_CHECK(cudaMemsetAsync(P.gbar, 0, sizeof(unsigned) * 64, stream));
+  NT_CUDA_CHECK(cudaMemsetAsync(P.gbar, 0, sizeof(unsigned) * kTcBarWords, stream));
   void* args[] = {&P};
   cudaError_t e = cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kern), dim3(num_sms), dim3(kTcThreads), args, smem, stream);
   if (e != cudaSuccess) return set_error(NT_ERR_CUDA, "decode_tc launch failed: %s", cudaGetErrorString(e));
@@ -1275,6 +1295,7 @@ int launch_decode_tc(TcParams& P, int B, int num_sms, const TcPlanInfo& info, cu
   const int nt = B <= 16 ? 16 : (B <= 32 ? 32 : 64);
   if (info.max_chunks > 14) return set_error(NT_ERR_INVALID, "decode_tc: %d k-blocks per CTA exceed the staging area", info.max_chunks);
   P.fold_in_cta = tc_fold_in_cta(B, P.hidden) ? 1 : 0;
+  if (P.fold_in_cta && (P.qkv_n + 127) / 128 > kTcMaxQkvTiles) return set_error(NT_ERR_INVALID, "decode_tc: qkv width %d has too many row tiles", P.qkv_n);
   P.weights_evict_first = 1;
   if (info.gu_split && !P.fold_in_cta) return set_error(NT_ERR_INVALID, "decode_tc: the flat plan needs the in-CTA fold (batch <= 4)");
   const bool hilo = B <= 8;

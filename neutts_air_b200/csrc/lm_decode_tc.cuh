@@ -18,8 +18,16 @@ constexpr int kTcDefaultMaxBatch = 16;  // nt_lm_decode's default: larger batche
 constexpr int kTcMaxSlices = 16;
 constexpr int kTcMaxGuSlices = 4;   // K slices of one gate/up tile in the flat plan (batch <= 4)
 constexpr int kTcMaxTiles = 8;      // row tiles of a hidden-sized output (hidden <= 1024)
+constexpr int kTcMaxQkvTiles = 32;  // row tiles of the qkv output (hidden <= 896: at most 21)
+constexpr int kTcMaxGuTiles = 4096; // row tiles of the gate/up output in the flat plan (the gu_nsl table's extent)
+// Grid-barrier block (zeroed before every launch): word 0 is the grid barrier; the batch-1 tile arrival counters
+// start at word kTcCntOff: o_proj [0, kTcMaxTiles), down_proj [kTcMaxTiles, 2 kTcMaxTiles), then qkv (kTcQkvCnt)
+// and gate/up (kTcGuCnt) row tiles, relative to kTcCntOff.
 constexpr int kTcCntOff = 32;
-constexpr int kTcH2Copies = 4;      // batch 1: copies of each tile-folded residual version in the h2 buffers       // the tile counters sit at words [32, 32 + 2 kTcMaxTiles) of the grid barrier block
+constexpr int kTcQkvCnt = 2 * kTcMaxTiles;
+constexpr int kTcGuCnt = kTcQkvCnt + kTcMaxQkvTiles;
+constexpr int kTcBarWords = kTcCntOff + kTcGuCnt + kTcMaxGuTiles;
+constexpr int kTcH2Copies = 4;      // batch 1: copies of each tile-folded residual version in the h2 buffers
 
 // One GEMM work item: rows [tile*128, tile*128+128) of a weight matrix times k-blocks [kb0, kb0+nkb) of the
 // activations (a k-block = 64 elements = one 128-byte swizzle row).  Items of the split-K phases (qkv, o, down)
@@ -69,11 +77,12 @@ struct TcParams {
   float2 *pq2, *po2, *pd2;        // split-K partial sums [slice][B][rows]
   int sq, so, sd;                 // slices per phase
   float2 *ao2, *aml2;             // split-KV attention partials [B][n_heads][max_splits][64] / [..][2] = ((m, .), (l, .))
-  float2* act2;                   // batch <= 4, whole-K gate/up: SwiGLU output [B][inter] (fp32 value, stamp)
+  float2* act2;                   // batch 1: SwiGLU output [inter] (fp32 value, stamp), one version
   float2* pg2;                    // batch <= 4, flat plan: gate/up partial sums [slice][B][2 * inter]
   const unsigned char* gu_nsl;    // flat plan: K slices of every gate/up tile (device, [tiles])
   float2* h2;                     // batch 1: residual stream, ping-pong [2][kTcH2Copies][hidden]
-  unsigned* tile_cnt;             // batch 1: arrival counters of the o_proj [0, kTcMaxTiles) and down_proj row tiles
+  float2* qkv2;                   // batch 1: finished q/k/v rows [qkv_n] (slices + bias, RoPE on q and k), one version
+  unsigned* tile_cnt;             // batch 1: arrival counters of the row tiles (layout: kTcCntOff)
   int stamp_base, hstamp_base;    // stamps of this launch lie above these (host counters)
   int max_splits, split_cap;
   KVLayout kv;

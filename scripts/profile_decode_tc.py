@@ -4,7 +4,7 @@ The Air shape with synthetic weights, one 500-token prompt and the 249-step deco
 ``nt_lm_debug_set_profile`` makes thread 0 of CTAs 0 and 1 record a mark at the end of every phase of one chosen step,
 and fine marks inside layer 2 and the sampler.  CTA 0 owns qkv, o_proj and down_proj items and the first attention
 split; CTA 1 owns gate/up units and the second attention split.  Marks 11 and 12 bracket a tile fold, recorded only when
-the CTA stores the last slice of an o_proj or down_proj tile.  The marks cost a global
+the CTA stores the last slice of a qkv, o_proj, gate/up or down_proj tile.  The marks cost a global
 store each, so the timeline runs in launches of its own, never on the bench path.
 
     python scripts/profile_decode_tc.py [--repeats 3] [--step 100]
@@ -30,7 +30,7 @@ PROMPT, STEPS = 500, 249
 # coarse marks (every layer): the end of each phase; 104 closes a layer
 COARSE = {100: "qkv (ln1 fold + projection)", 101: "attention", 102: "o_proj (merge + projection)",
           103: "gate/up (ln2 fold + projection)", 104: "down (SwiGLU staging + projection)"}
-FINE = {1: "fold: start", 2: "fold: rows read", 4: "fold: staged", 5: "bop ready", 10: "split-K item out", 11: "tile fold: last arrival", 12: "tile fold: residual out", 21: "attention: start", 22: "attention: prologue done", 23: "attention: page in",
+FINE = {1: "fold: start", 2: "fold: rows read", 4: "fold: staged", 5: "bop ready", 10: "split-K item out", 11: "tile fold: last arrival", 12: "tile fold: rows out", 21: "attention: start", 22: "attention: prologue done", 23: "attention: page in",
         25: "attention: partials out", 31: "o_proj input: staged", 32: "o_proj input: bop ready",
         41: "down input: staged", 42: "down input: bop ready", 50: "gate/up item out", 110: "lm_head done",
         111: "sampler done", 200: "grid barrier passed", 0: "step start"}
