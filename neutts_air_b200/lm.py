@@ -497,14 +497,16 @@ class Settings:
         elif getattr(lm, "_guidance_host", None) is not None:
             lm.set_guidance(None)
 
-    def pair(self, pairs) -> "Settings":
+    def pair(self, pairs, n: int | None = None) -> "Settings":
         """The settings of a batch with guided pairs ((c, u, scale) from ``guided_layout``): the u slots, above the
         prompts in pair order, repeat their c's rows (they are never sampled, but every launch checks their entries),
-        and ``guidance`` holds the table of every slot."""
-        if not pairs:
-            return self
-        n = pairs[0][1]
-        rows = lambda r: None if r is None else list(r) + [r[c] for c, _, _ in pairs]
+        and ``guidance`` holds the table of every slot.  ``n``: the batch holds only the first n prompts (a queue's
+        first wave of a call with guidance); their table is on even without a pair."""
+        if n is None:
+            if not pairs:
+                return self
+            n = pairs[0][1]
+        rows = lambda r: None if r is None else list(r[:n]) + [r[c] for c, _, _ in pairs]
         table = [NO_GUIDANCE] * (n + len(pairs))
         for c, u, g in pairs:
             table[c] = (u, g)
@@ -670,10 +672,12 @@ class SpeechLM:
         self._write_slot_table("_slot_sp_host", self.L.nt_lm_set_slot_sampling, _lib.SlotSampling, check_controls,
                                DEFAULT_CONTROLS, rows, slots)
 
-    def _write_slot_table(self, mirror: str, setter, entry, check, default, rows, slots) -> None:
-        """Behind ``set_slot_sampling`` / ``set_repetition_penalty`` / ``set_length_control``: validates ``rows`` (``check``) and ``slots``,
-        merges them into the host mirror (attribute ``mirror``; ``default`` fills a table that was off), and hands the
-        whole table of ``entry`` structs to the C ``setter`` on the current stream.  ``rows=None``: the table goes off."""
+    def _write_slot_table(self, mirror: str, setter, entry, check, default, rows, slots, check_table=None) -> None:
+        """Behind the ``set_*`` methods of per-slot tables: validates ``rows`` (``check``) and ``slots``, merges them
+        into the host mirror (attribute ``mirror``; ``default`` fills a table that was off), validates the merged table
+        (``check_table(table, max_batch)``, when given), and hands the whole table of ``entry`` structs to the C
+        ``setter`` on the current stream.  ``rows=None``: the table goes off.  A bad table raises before anything is
+        written."""
         table = arr = None
         if rows is not None:
             rows = [check(*r) for r in rows]
@@ -683,6 +687,8 @@ class SpeechLM:
             table = list(getattr(self, mirror) or [default] * self.max_batch)
             for s, r in zip(slots, rows):
                 table[s] = r
+            if check_table is not None:
+                table = check_table(table, self.max_batch)
             arr = (entry * self.max_batch)(*(entry(*r) for r in table))
         with torch.cuda.device(self.device):
             _lib.check(setter(self.handle, arr, _lib.current_stream_ptr()))
@@ -752,20 +758,8 @@ class SpeechLM:
         (the next call's settings replace it); a caller that then prefills or decodes directly switches it off first,
         or its launches must include both slots of every pair still in the table.  The merged table is validated first (``check_guidance_table``); a bad one
         raises ValueError and leaves the previous table in force.  Copied on the current stream."""
-        table = arr = None
-        if rows is not None:
-            rows = [(int(p), float(g)) for p, g in rows]
-            slots = list(range(len(rows))) if slots is None else [int(s) for s in slots]
-            if len(slots) != len(rows) or len(set(slots)) != len(slots) or any(not 0 <= s < self.max_batch for s in slots):
-                raise ValueError(f"slots must be distinct, in 0..{self.max_batch - 1} and one per row")
-            table = list(getattr(self, "_guidance_host", None) or [NO_GUIDANCE] * self.max_batch)
-            for s, r in zip(slots, rows):
-                table[s] = r
-            table = check_guidance_table(table, self.max_batch)
-            arr = (_lib.SlotGuidance * self.max_batch)(*(_lib.SlotGuidance(*r) for r in table))
-        with torch.cuda.device(self.device):
-            _lib.check(self.L.nt_lm_set_guidance(self.handle, arr, _lib.current_stream_ptr()))
-        self._guidance_host = table
+        self._write_slot_table("_guidance_host", self.L.nt_lm_set_guidance, _lib.SlotGuidance,
+                               lambda p, g: (int(p), float(g)), NO_GUIDANCE, rows, slots, check_guidance_table)
 
     def _stage_ids(self, prompts) -> torch.Tensor:
         """The prompts' ids, range-checked, back to back in a persistent pinned buffer (so their H2D copy is
@@ -1030,10 +1024,6 @@ class SpeechLM:
         checks, the generated-token cap per prompt and the resolved ``settings`` -> (caps, Settings, guidance), with
         guidance as ``per_prompt_guidance`` and every guided prompt's cap shortened so its negative prompt fits."""
         guidance = per_prompt_guidance(prompts, guidance_scale, negative_prompt_ids)
-        caps, st = self._prepare_caps(prompts, max_length, max_new_tokens, **settings)
-        return guided_caps(caps, guidance, self.max_ctx), st, guidance
-
-    def _prepare_caps(self, prompts, max_length, max_new_tokens, **settings) -> tuple:
         max_length = max_length or self.max_ctx
         if max_length > self.max_ctx:
             raise ValueError(f"max_length {max_length} exceeds the engine context {self.max_ctx}")
@@ -1043,7 +1033,8 @@ class SpeechLM:
         # max_length counts prompt + generated PER SEQUENCE (stopping_criteria.py:73-84): a long prompt in the batch
         # must not shorten its neighbours, so every slot gets its own cap and the loop runs to the largest one
         caps = self._caps(lens, max_length, max_new_tokens)
-        return caps, resolve_settings(self, len(prompts), max_new=max(caps, default=0), **settings)
+        st = resolve_settings(self, len(prompts), max_new=max(caps, default=0), **settings)
+        return guided_caps(caps, guidance, self.max_ctx), st, guidance
 
     def generate_batch(self, prompts, eos_token_id: int, max_length: int | None = None, min_new_tokens: int = 50,
                        temperature: float = 1.0, top_k: int = 50, max_new_tokens: int | None = None, seed: int = 0,
@@ -1146,99 +1137,40 @@ class SpeechLM:
             top_p=top_p, min_p=min_p, vocab_range=vocab_range, repetition_penalty=repetition_penalty,
             penalize_prompt=penalize_prompt, logprobs=return_logprobs, min_new_tokens=min_new_tokens,
             exponential_decay_length_penalty=exponential_decay_length_penalty)
-        n = len(prompts)
+        n, M = len(prompts), self.max_batch
         if n == 0:
             return ([], []) if return_logprobs else []
         if check_every < 1:
             raise ValueError("check_every must be >= 1")
-        if guidance is not None:
-            return self._generate_queue_guided(prompts, eos_token_id, caps, settings, guidance, seed, greedy, check_every,
-                                               slot_base, return_logprobs)
-        S = min(n, self.max_batch)
-        sp = self.sampling(eos_token_id, settings.min_new_tokens, max(caps), settings.top_k, settings.temperature, seed,
-                           greedy, limits=caps[:S], slot_base=slot_base)
-        settings.apply(self, S)
-        self.prefill([prompts[i] for i in range(S)], sp)
-        occ = list(range(S))   # prompt held by each slot, None once harvested
-        ngen = [1] * S         # generated tokens per slot, as of the last read
-        nxt = S                # next prompt to admit
-        out = [None] * n
-        out_lp = [None] * n
-        # a sequence can finish inside its prefill: a cap of 1, or EOS when it is not masked at step 0
-        floors = settings.floors(n)
-        at_prefill = lambda idx: min(floors[i] for i in idx) <= 0 or min(caps[i] for i in idx) <= 1
-        read = at_prefill(range(S))
-        while True:
-            if read:
-                st = torch.stack((self.n_generated[:S], self.done[:S])).cpu()   # the one small D2H read per launch
-                ngen = st[0].tolist()
-                fin = [s for s in range(S) if occ[s] is not None and int(st[1, s])]
-                if fin:
-                    ids, lps = self._results(fin, [ngen[s] for s in fin], return_logprobs)
-                    for r, s in enumerate(fin):
-                        out[occ[s]] = ids[r]
-                        if return_logprobs:
-                            out_lp[occ[s]] = lps[r]
-                        occ[s] = None
-                    take = fin[: n - nxt]
-                    if take:
-                        idx = list(range(nxt, nxt + len(take)))
-                        nxt += len(take)
-                        settings.admit(self, take, idx)   # before their prefill, on the same stream
-                        self.prefill_slots(take, [prompts[i] for i in idx], sp, [slot_base + i for i in idx],
-                                           limits=[caps[i] for i in idx])
-                        for s, i in zip(take, idx):
-                            occ[s], ngen[s] = i, 1
-                        if at_prefill(idx):
-                            continue   # read again before decoding: a newcomer may be done already
-            live = [s for s in range(S) if occ[s] is not None]
-            if not live:
-                break
-            left = [caps[occ[s]] - ngen[s] for s in live]
-            steps = max(1, min(check_every, min(left) if nxt < n else max(left)))
-            self.decode(steps, sp)
-            read = True
-        self.release_pages()
-        return (out, out_lp) if return_logprobs else out
-
-    def _generate_queue_guided(self, prompts, eos_token_id, caps, settings, guidance, seed, greedy, check_every, slot_base,
-                               return_logprobs):
-        """``generate_queue`` with some prompts guided: the first prompts that fit go in by one ``prefill`` in the
-        ``generate_batch`` layout (prompt i in slot i, u slots above), later ones by ``prefill_slots`` into free slots."""
-        n, M = len(prompts), self.max_batch
-        need = [1 + (g != 1.0) for g, _ in guidance]
+        guided = guidance is not None
+        need = [1 + (g != 1.0) for g, _ in guidance] if guided else [1] * n   # slots per prompt: c, and u when guided
         if max(need) > M:
             raise ValueError(f"a guided prompt needs 2 slots; the engine has {M}")
-        k = 0
-        while k < n and sum(need[: k + 1]) <= M:   # prompts 0..k-1 and their u slots fit
+        k = 0   # the first wave: prompts 0..k-1 and their u slots, in the generate_batch layout
+        while k < n and sum(need[: k + 1]) <= M:
             k += 1
-        pairs = guided_layout(k, guidance[:k])
+        pairs = guided_layout(k, guidance[:k]) if guided else []
         slot_caps = caps[:k] + [caps[c] for c, _, _ in pairs]
         sp = self.sampling(eos_token_id, settings.min_new_tokens, max(caps), settings.top_k, settings.temperature, seed,
                            greedy, limits=slot_caps, slot_base=slot_base)
-        first = dataclasses.replace(settings, controls=None if settings.controls is None else settings.controls[:k],
-                                    penalty=None if settings.penalty is None else settings.penalty[:k],
-                                    length=None if settings.length is None else settings.length[:k]).pair(pairs)
-        if first.guidance is None:
-            first = dataclasses.replace(first, guidance=[NO_GUIDANCE] * k)
-        first.apply(self, len(slot_caps))
+        # with guidance the table is on from the first prefill, pair or not: the decode path depends on it, so switching
+        # it on at a later refill would change the kernels of the slots already decoding
+        (settings.pair(pairs, k) if guided else settings).apply(self, len(slot_caps))
         self.prefill(list(prompts[:k]) + [guidance[c][1] for c, _, _ in pairs], sp)
-        occ = [None] * M           # prompt held by each c slot
-        for i in range(k):
-            occ[i] = i
-        partner = {c: u for c, u, _ in pairs}   # c slot -> u slot
+        occ = list(range(k)) + [None] * (M - k)   # prompt held by each c slot, None once harvested
+        partner = {c: u for c, u, _ in pairs}     # c slot -> its u slot
         busy = set(range(k)) | set(partner.values())
-        ngen = [1] * M
-        nxt = k
+        ngen = [1] * M   # generated tokens per slot, as of the last read
+        nxt = k          # next prompt to admit
         out, out_lp = [None] * n, [None] * n
+        # a sequence can finish inside its prefill: a cap of 1, or EOS when it is not masked at step 0
         floors = settings.floors(n)
         at_prefill = lambda idx: min(floors[i] for i in idx) <= 0 or min(caps[i] for i in idx) <= 1
         read = at_prefill(range(k))
         while True:
             if read:
-                st = torch.stack((self.n_generated, self.done)).cpu()
-                ngen = st[0].tolist()
-                fin = [s for s in range(M) if occ[s] is not None and int(st[1, s])]
+                ngen, done = torch.stack((self.n_generated, self.done)).cpu().tolist()   # the one small D2H read per launch
+                fin = [s for s in range(M) if occ[s] is not None and done[s]]
                 freed = []
                 if fin:
                     ids, lps = self._results(fin, [ngen[s] for s in fin], return_logprobs)
@@ -1249,34 +1181,31 @@ class SpeechLM:
                         occ[s] = None
                         freed += [s] + ([partner.pop(s)] if s in partner else [])
                     busy -= set(freed)
-                free = [s for s in range(M) if s not in busy]
-                slots, idx, neg_rows, take_u = [], [], [], []
-                while nxt < n and need[nxt] <= len(free) - len(slots) - len(take_u):
-                    rest = [s for s in free if s not in slots and s not in take_u]
-                    slots.append(rest[0])
-                    idx.append(nxt)
-                    if need[nxt] == 2:
-                        take_u.append(rest[1])
-                        neg_rows.append((len(slots) - 1, rest[1]))
+                # FIFO, the head of the queue waiting for room: each prompt takes the lowest free slot, its u slot the next
+                free, room = (s for s in range(M) if s not in busy), M - len(busy)
+                new = []   # (c slot, u slot or None, prompt) of every admitted prompt
+                while nxt < n and need[nxt] <= room:
+                    new.append((next(free), next(free) if need[nxt] == 2 else None, nxt))
+                    room -= need[nxt]
                     nxt += 1
-                if slots:
-                    all_slots = slots + take_u
-                    all_idx = idx + [idx[j] for j, _ in neg_rows]
-                    # every freed slot's entry is rewritten in the same call, so no finished pair survives
-                    guide = {s: NO_GUIDANCE for s in freed + all_slots}
-                    for j, u in neg_rows:
-                        guide[slots[j]] = (u, guidance[idx[j]][0])
-                    settings.admit(self, all_slots, all_idx, guide=guide)
-                    prompts_in = [prompts[i] for i in idx] + [guidance[idx[j]][1] for j, _ in neg_rows]
-                    self.prefill_slots(all_slots, prompts_in, sp, [slot_base + i for i in all_idx],
-                                       limits=[caps[i] for i in all_idx])
-                    for s, i in zip(slots, idx):
-                        occ[s], ngen[s] = i, 1
-                    for j, u in neg_rows:
-                        partner[slots[j]] = u
-                    busy |= set(all_slots)
-                    if at_prefill(idx):
-                        continue
+                if new:
+                    new_pairs = [(c, u, i) for c, u, i in new if u is not None]
+                    slots = [c for c, _, _ in new] + [u for _, u, _ in new_pairs]
+                    idx = [i for _, _, i in new] + [i for _, _, i in new_pairs]
+                    guide = None
+                    if guided:   # every freed slot's entry is rewritten in the same call, so no finished pair survives
+                        guide = {s: NO_GUIDANCE for s in freed + slots}
+                        guide.update((c, (u, guidance[i][0])) for c, u, i in new_pairs)
+                    settings.admit(self, slots, idx, guide=guide)   # before their prefill, on the same stream
+                    self.prefill_slots(slots, [prompts[i] for _, _, i in new] + [guidance[i][1] for _, _, i in new_pairs],
+                                       sp, [slot_base + i for i in idx], limits=[caps[i] for i in idx])
+                    for c, u, i in new:
+                        occ[c], ngen[c] = i, 1
+                        if u is not None:
+                            partner[c] = u
+                    busy |= set(slots)
+                    if at_prefill([i for _, _, i in new]):
+                        continue   # read again before decoding: a newcomer may be done already
             live = [s for s in range(M) if occ[s] is not None]
             if not live:
                 break

@@ -210,50 +210,7 @@ def test_admit_writes_pair_entries():
 
 
 # ---------------------------------------------------------------------------------------------- engine host on stubs
-from tests.fakes import EOS, FakeTokenizer, GenerateBackbone, KwBackbone, QueueStub, _facade  # noqa: E402
-
-
-class GuidedStub(QueueStub):
-    """QueueStub with guidance: prompt i is i + 1 repeated, its negative prompt -(i + 1) repeated.  A u slot emits
-    nothing itself (it mirrors its c on the device); the stub records where each negative prompt went."""
-
-    def __init__(self, max_batch, eos_at=None):
-        super().__init__(max_batch, eos_at)
-        self._guidance_host = None
-        self.u_at = {}   # u slot -> tag of the prompt whose negative prompt it holds
-        self.done[:] = 1   # a slot no prefill has filled yet holds nothing to decode: the queue may fill it
-
-    def sampling(self, eos, min_new, max_new, top_k, temperature, seed, greedy, forced=None, limits=None, slot_base=0):
-        return super().sampling(eos, min_new, max_new, top_k, temperature, seed, greedy,
-                                limits=list(limits) if limits is not None else [max_new] * self.max_batch,
-                                slot_base=slot_base)
-
-    def set_guidance(self, rows, slots=None):
-        if rows is not None:
-            slots = list(range(len(rows))) if slots is None else list(slots)
-            table = list(self._guidance_host or [NO_GUIDANCE] * self.max_batch)
-            for s, r in zip(slots, rows):
-                table[s] = r
-            rows = check_guidance_table(table, self.max_batch)
-        self.log.append(("guide", None if rows is None else list(rows)))
-        self._guidance_host = rows
-
-    def _start(self, s, prompt, key):
-        if prompt[0] > 0:
-            self.u_at.pop(s, None)
-            return super()._start(s, prompt, key)
-        tag = -prompt[0]   # u is never sampled: its key is whatever the launch gives its slot
-        self._slot_pages[s] = self.pool.alloc((len(prompt) + self.limit_table[s] + self.PAGE - 1) // self.PAGE)
-        self.u_at[s] = tag
-        self.who[s], self.cap[s] = None, self.limit_table[s]
-        self.n_generated[s], self.done[s] = 1, 1   # u never emits here; the queue only reads c slots
-
-    def prefill_slots(self, slots, prompts, sp, stream_ids, return_logits=False, limits=None):
-        super().prefill_slots(slots, prompts, sp, stream_ids, return_logits, limits)
-        self._B = max(self._B, max(slots) + 1)   # as SpeechLM.prefill_slots: decode covers every slot filled so far
-
-    def set_logprobs(self, on=True):
-        self.logprobs = None
+from tests.fakes import EOS, FakeTokenizer, GenerateBackbone, GuidedStub, KwBackbone, _facade  # noqa: E402
 
 
 def _negs(lens):
