@@ -27,6 +27,7 @@ from typing import Generator, Sequence
 import numpy as np
 import torch
 
+from neutts_air_b200 import longform
 from neutts_air_b200.lm import check_guidance_scale, per_item, per_prompt_decay, resolve_settings
 
 SPEECH_RE = re.compile(r"<\|speech_(\d+)\|>")
@@ -514,16 +515,18 @@ class NeuTTS:
               min_p: float = 0.0, repetition_penalty: float = 1.0, penalize_prompt: bool = True,
               return_logprobs: bool = False, takes: int = 1, min_new_tokens: int = 50,
               exponential_decay_length_penalty=None, guidance_scale: float = 1.0, negative_text: str | None = None,
-              speed: float = 1.0):
+              speed: float = 1.0, long_form: bool = False, pause: float = 0.0):
         """Text + reference voice -> 24 kHz float32 waveform (``neutts/neutts.py:216-243``).  The sampling controls
         default to the reference's values; see ``infer_batch``.  ``return_logprobs``: returns (waveform, log-probs).
         ``takes``: generate that many takes and keep the most probable one (``infer_batch``).  ``guidance_scale`` and
-        ``negative_text``: classifier-free guidance (``infer_batch``).  ``speed``: speaking rate (``infer_batch``)."""
+        ``negative_text``: classifier-free guidance (``infer_batch``).  ``speed``: speaking rate (``infer_batch``).
+        ``long_form`` and ``pause``: a text longer than the context, in segments (``infer_batch``)."""
         out = self.infer_batch([text], [ref_codes], [ref_text], temperature=temperature, top_k=top_k, top_p=top_p,
                                min_p=min_p, repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt,
                                return_logprobs=return_logprobs, takes=takes, min_new_tokens=min_new_tokens,
                                exponential_decay_length_penalty=exponential_decay_length_penalty,
-                               guidance_scale=guidance_scale, negative_text=negative_text, speed=speed)
+                               guidance_scale=guidance_scale, negative_text=negative_text, speed=speed,
+                               long_form=long_form, pause=pause)
         return (out[0][0], out[1][0]) if return_logprobs else out[0]
 
     def infer_from_prompt_ids(self, prompts: Sequence[Sequence[int]], max_new_tokens: int | None = None,
@@ -558,7 +561,7 @@ class NeuTTS:
     def infer_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], distributed: bool = False, *,
                     temperature=1.0, top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0, penalize_prompt=True,
                     return_logprobs: bool = False, takes: int = 1, min_new_tokens=50, exponential_decay_length_penalty=None,
-                    guidance_scale=1.0, negative_text=None, speed=1.0):
+                    guidance_scale=1.0, negative_text=None, speed=1.0, long_form: bool = False, pause: float = 0.0):
         """List in / list out.  With ``distributed=True`` (inside an initialised torch.distributed job) the
         utterances are sharded over ranks and every rank returns all waveforms (one all-gather).
 
@@ -609,9 +612,28 @@ class NeuTTS:
         time-stretched at 24 kHz on the GPU right after the codec (librosa's ``time_stretch``, a phase vocoder: the
         pitch is kept, a waveform of L samples becomes round(L / speed)), before the watermark and any resampling.  A
         list follows its utterances through chunking, the queue, takes (the kept take is stretched) and the sharding
-        over ranks.  An utterance at exactly 1.0 is not stretched; with every speed at 1.0 nothing changes."""
+        over ranks.  An utterance at exactly 1.0 is not stretched; with every speed at 1.0 nothing changes.
+
+        ``long_form=True``: a text too long for one prompt is split into segments that fit (``segments``); the
+        segments of all texts run as one batch (segment 0 of every text first, then segment 1 of every text that has
+        one, and so on; segment j of that order draws from random stream j), each with its text's controls, and each
+        text's waveforms are joined after the codec, stretch, watermark and resampler with 10 ms fades at every seam
+        and ``pause`` seconds (in [0, 10]) of silence between segments.  A text that fits is one segment and comes back
+        as without ``long_form``.  With ``return_logprobs`` a text's rows are its segments' rows, concatenated."""
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
+        pause = longform.check_pause(pause, long_form)
+        if long_form:
+            owners, flat, refs, rts, kw = self._long_form_plan(
+                texts, ref_codes, ref_texts, temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p,
+                repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt, min_new_tokens=min_new_tokens,
+                exponential_decay_length_penalty=exponential_decay_length_penalty, guidance_scale=guidance_scale,
+                negative_text=negative_text, speed=speed)
+            out = self.infer_batch(flat, refs, rts, distributed, return_logprobs=return_logprobs, takes=takes, **kw)
+            wavs, lps = out if return_logprobs else (out, None)
+            idx = [[j for j, o in enumerate(owners) if o == t] for t in range(len(texts))]
+            joined = [longform.join([wavs[j] for j in js], self.sample_rate, pause) for js in idx]
+            return (joined, [np.concatenate([lps[j] for j in js]) for js in idx]) if return_logprobs else joined
         speeds = _speeds(len(texts), speed)
         ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
                         exponential_decay_length_penalty)
@@ -683,6 +705,61 @@ class NeuTTS:
             lps += r[1] if return_logprobs else []
         return (out, lps) if return_logprobs else out
 
+    # ------------------------------------------------------------------ long-form synthesis
+    def segments(self, text: str, ref_codes, ref_text: str) -> list:
+        """The segments ``long_form=True`` synthesises ``text`` in, with the voice (``ref_codes``, ``ref_text``):
+        ``[text]`` when it fits whole, else its sentences packed greedily per line (``neutts_air_b200.longform``).  A
+        segment fits when the room ``max_context`` leaves after its prompt covers its text at the reference's pace
+        (reference codes per reference-text token) with a 1.25 margin; every candidate is measured on the prompt that
+        would run.  ValueError when a single word does not fit."""
+        codes = ref_codes.tolist() if hasattr(ref_codes, "tolist") else list(ref_codes)
+        lens = {}
+
+        def prompt_len(s: str) -> int:
+            if s not in lens:
+                lens[s] = len(self._apply_chat_template(codes, ref_text, s))
+            return lens[s]
+
+        return longform.segment(text, longform.fit_rule(prompt_len, ref_text, len(codes), self.max_context))
+
+    def _long_form_plan(self, texts, ref_codes, ref_texts, **controls):
+        """The flattened segments of ``texts`` in round-robin order -> (owning text of each segment, segment texts,
+        reference codes, reference texts, controls): every per-text control list becomes one entry per segment,
+        scalars stay."""
+        segs = [self.segments(t, c, rt) for t, c, rt in zip(texts, ref_codes, ref_texts)]
+        order = longform.round_robin([len(s) for s in segs])
+        owners = [t for t, _ in order]
+        n = len(texts)
+        decay = controls.pop("exponential_decay_length_penalty")
+        per = per_prompt_decay(n, decay)
+        kw = {k: [v[t] for t in owners] if isinstance(v, list) else v for k, v in per_item(n, "text", **controls).items()}
+        kw["exponential_decay_length_penalty"] = decay if per[0] is decay else [per[t] for t in owners]
+        return (owners, [segs[t][k] for t, k in order], [ref_codes[t] for t in owners], [ref_texts[t] for t in owners],
+                kw)
+
+    def _long_form_stream(self, texts, ref_codes, ref_texts, pause: float, **controls) -> Generator[list, None, None]:
+        """``infer_stream_batch`` with ``long_form=True``: the flattened segments stream through ``_stream_batch`` and
+        ``longform.StreamJoin`` turns the rounds into one stream per text.  Planned here, streamed lazily."""
+        owners, flat, refs, rts, kw = self._long_form_plan(texts, ref_codes, ref_texts, **controls)
+        speeds = _speeds(len(flat), kw.pop("speed"))
+        ctl = _controls(len(flat), **kw)
+        prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(flat, refs, rts)]
+        ids = [[int(c) for c in (rc.tolist() if hasattr(rc, "tolist") else rc)] for rc in refs]
+        seams = longform.StreamJoin(owners, self.sample_rate, pause, np.int16 if self.pcm_format == "int16" else np.float32)
+
+        def run():
+            ends = []
+            rounds = self._stream_batch(prompts, ids, ctl, speeds, ends=ends)
+            try:
+                for out in rounds:
+                    got = seams.push(out, ends)
+                    if any(g is not None for g in got):
+                        yield got
+            finally:
+                rounds.close()   # every KV page back in the pool when the consumer stops early
+
+        return run()
+
     # ------------------------------------------------------------------ scoring
     def score(self, text: str, ref_codes, ref_text: str, codes, *, include_eos: bool = True) -> np.ndarray:
         """How likely the speech codes ``codes`` are as this model's rendering of ``text`` in the voice of
@@ -739,18 +816,26 @@ class NeuTTS:
                      top_p: float = 1.0, min_p: float = 0.0, repetition_penalty: float = 1.0,
                      penalize_prompt: bool = True, takes: int = 1, min_new_tokens: int = 50,
                      exponential_decay_length_penalty=None, guidance_scale=1.0,
-                     speed: float = 1.0) -> Generator[np.ndarray, None, None]:
+                     speed: float = 1.0, long_form: bool = False, pause: float = 0.0) -> Generator[np.ndarray, None, None]:
         """Streaming synthesis with the reference's window geometry (``neutts/neutts.py:373-465``):
         every 25 new frames (once 5 look-ahead frames exist) the codec re-decodes
         [n - 50 - 1, n + 25 + 5 + 1) and the chunk is cross-faded with triangular weights.  Sampling controls as in
         ``infer_batch``; streaming returns no per-token log-probabilities (``return_logprobs`` is not supported here)
         and generates one take per utterance (``takes`` other than 1 raises ValueError); classifier-free guidance is not
         supported (``guidance_scale`` other than 1 raises ValueError).  ``speed``: speaking rate (``infer_batch``); each
-        cross-faded chunk goes through the stretcher's stream, so the chunks concatenate to the stretched stream."""
+        cross-faded chunk goes through the stretcher's stream, so the chunks concatenate to the stretched stream.
+        ``long_form`` and ``pause``: a text longer than the context, in segments (``infer_stream_batch``)."""
         self._no_takes(takes)
         self._no_guidance(guidance_scale, "streaming synthesis")
         if self._is_quantized_model:  # kept for signature parity; never true on this build
             raise NotImplementedError("GGUF streaming is not part of the H100 build")
+        pause = longform.check_pause(pause, long_form)
+        if long_form:
+            rounds = self._long_form_stream([text], [ref_codes], [ref_text], pause, temperature=temperature, top_k=top_k,
+                                            top_p=top_p, min_p=min_p, repetition_penalty=repetition_penalty,
+                                            penalize_prompt=penalize_prompt, min_new_tokens=min_new_tokens,
+                                            exponential_decay_length_penalty=exponential_decay_length_penalty, speed=speed)
+            return self._only_text(rounds)
         ctl = _controls(1, temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
                         exponential_decay_length_penalty)
         speeds = _speeds(1, speed)
@@ -761,7 +846,8 @@ class NeuTTS:
     def infer_stream_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], *, temperature=1.0,
                            top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0,
                            penalize_prompt=True, takes: int = 1, min_new_tokens=50,
-                           exponential_decay_length_penalty=None, guidance_scale=1.0, speed=1.0) -> Generator[list, None, None]:
+                           exponential_decay_length_penalty=None, guidance_scale=1.0, speed=1.0, long_form: bool = False,
+                           pause: float = 0.0) -> Generator[list, None, None]:
         """Streaming synthesis of many utterances at once (BASELINE.json configs[4]; the reference streams one
         utterance, ``neutts/neutts.py:373-465``).  Every yield is a list with one entry per utterance, as many entries
         as ``texts``: the next audio chunk (float32, cross-faded exactly as in ``infer_stream``) or ``None`` when that
@@ -780,17 +866,38 @@ class NeuTTS:
         per utterance (``takes`` other than 1 raises ValueError); ``guidance_scale`` other than 1 raises ValueError.
         ``speed`` (a number or one per utterance): speaking rate, as in ``infer_batch``; it follows its utterance into
         whichever slot it takes.  Chunks go codec -> cross-fade -> stretch -> resample, and concatenate to the stretched
-        stream."""
+        stream.
+
+        ``long_form=True``: the texts are split and their segments ordered as in ``infer_batch``, and all segments stream
+        as one queue; each text still gets one entry per yield.  A text plays its segments in order: chunks of a later
+        segment, decoding in another slot already, are held until every earlier segment of the text has ended, and each
+        segment holds back its last 10 ms until its next chunk or its end, for the seam's fade-out and ``pause``.  The
+        chunks of a text concatenate to ``infer_batch``'s join of its segments' streams."""
         self._no_takes(takes)
         self._no_guidance(guidance_scale, "streaming synthesis")
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
+        pause = longform.check_pause(pause, long_form)
+        if long_form:
+            return self._long_form_stream(texts, ref_codes, ref_texts, pause, temperature=temperature, top_k=top_k,
+                                          top_p=top_p, min_p=min_p, repetition_penalty=repetition_penalty,
+                                          penalize_prompt=penalize_prompt, min_new_tokens=min_new_tokens,
+                                          exponential_decay_length_penalty=exponential_decay_length_penalty, speed=speed)
         self._stream_slots(len(texts))
         ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
                         exponential_decay_length_penalty)
         prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(texts, ref_codes, ref_texts)]
         refs = [[int(c) for c in (rc.tolist() if hasattr(rc, "tolist") else rc)] for rc in ref_codes]
         return self._stream_batch(prompts, refs, ctl, _speeds(len(texts), speed))
+
+    @staticmethod
+    def _only_text(rounds) -> Generator[np.ndarray, None, None]:
+        """The chunks of a one-text long-form stream (its rounds yield only when the text has new audio)."""
+        try:
+            for out in rounds:
+                yield out[0]
+        finally:
+            rounds.close()
 
     def _stream(self, prompt, ref_codes, ctl: dict | None = None, speeds=None) -> Generator[np.ndarray, None, None]:
         for out in self._stream_batch([prompt], [list(ref_codes)], ctl, speeds):
@@ -806,7 +913,8 @@ class NeuTTS:
                              "(neutts_air_b200.SpeechLM)")
         return min(n, slots)
 
-    def _stream_batch(self, prompts, refs, ctl: dict | None = None, speeds=None) -> Generator[list, None, None]:
+    def _stream_batch(self, prompts, refs, ctl: dict | None = None, speeds=None, ends: list | None = None
+                      ) -> Generator[list, None, None]:
         """Window geometry of the reference (``neutts/neutts.py:87-91,401-421,443-465``): once F + LA undecoded frames
         exist, the codec decodes [n_dec - LB - OV, n_dec + F + LA) and the slice [n_dec - OV, n_dec + F + OV) is
         cross-faded at stride F * hop; a ragged tail closes the stream.  ``streaming_frames_per_chunk`` may be set to
@@ -820,7 +928,10 @@ class NeuTTS:
         More utterances than the engine's ``max_batch`` run as a queue on its S slots: utterance i is admitted FIFO and
         draws from Philox stream i (the first S through ``prefill``, later ones through ``prefill_slots``); a slot is
         refilled once its utterance's tail has been decoded from its history row.  Every KV page is back in the pool
-        when the generator ends, closed early included."""
+        when the generator ends, closed early included.
+
+        ``ends``: None, or a list that holds, at every yield, the utterances whose stream ends with it; a round in which
+        one ends is then yielded even when it has no new audio."""
         hop, F, LA, LB, OV = self.hop_length, self.streaming_frames_per_chunk, self.streaming_lookforward, \
             self.streaming_lookback, self.streaming_overlap_frames
         eos = self._tok_id("<|SPEECH_GENERATION_END|>")
@@ -963,6 +1074,8 @@ class NeuTTS:
                 # ragged tail of an utterance that finished (neutts/neutts.py:443-465), once its regular chunks are out
                 tails, ending = [], []
                 all_finished = nxt == N and all(finished.values())
+                if ends is not None:
+                    ends.clear()
                 for b in held:
                     u = occ[b]
                     if finished[b] and not tail_done[u] and (all_finished or out[u] is None):
@@ -986,7 +1099,9 @@ class NeuTTS:
                         t = fades[occ[b]].push(wavs[0], final=True)
                         out[occ[b]] = t if out[occ[b]] is None else np.concatenate((out[occ[b]], t))
                 out = at_rate(at_speed(out, ending), ending)
-                if any(o is not None for o in out):
+                if ends is not None:
+                    ends += ending
+                if any(o is not None for o in out) or (ends is not None and ending):
                     yield out
                 if all_finished:
                     break
