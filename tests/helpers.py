@@ -168,6 +168,73 @@ def decode_branch(shape: tuple, B: int, G: int, max_ctx: int, impl=None) -> dict
                 name=f"tc-{act}-n{nt}-{plan}-{'fold' if fold else 'phases'}")
 
 
+def head_list(V: int, eos: int, rng=None) -> tuple:
+    """The persistent kernel's lm_head tile list for vocabulary V under the vocabulary range ``rng`` = (lo, hi) (None:
+    off), restated from vocab_tiles and nt_lm_decode (lm_api.cu): (head_n, head_lo, head_eos, head_eos_at).  The range's
+    tiles head_lo, head_lo + 1, ... in order, with EOS's tile head_eos inserted at position head_eos_at (0 when it lies
+    below the range, last when above) when EOS lies outside the range's tiles; head_eos = head_eos_at = -1 otherwise."""
+    t_lo = rng[0] // 128 if rng else 0
+    t_hi = -(-(rng[1] if rng else V) // 128)
+    et = eos // 128
+    head_eos = et if rng and (et < t_lo or et >= t_hi) else -1
+    head_eos_at = -1 if head_eos < 0 else (0 if head_eos < t_lo else t_hi - t_lo)
+    return t_hi - t_lo + (head_eos >= 0), t_lo, head_eos, head_eos_at
+
+
+def head_partition(head_n: int, head_eos_at: int, G: int, head_lo: int = 0, head_eos: int = -1) -> list:
+    """The lm_head work of the persistent kernel on G CTAs, restated from decode_tc_kernel (lm_decode_tc.cu): CTA c
+    takes list positions [head_n c / G, head_n (c + 1) / G).  Returns, per CTA, (t0, t1, row tiles of t0..t1-1)."""
+    def tile(v):
+        return head_eos if v == head_eos_at else head_lo + v - (1 if 0 <= head_eos_at < v else 0)
+
+    out = []
+    for c in range(G):
+        t0, t1 = head_n * c // G, head_n * (c + 1) // G
+        out.append((t0, t1, [tile(v) for v in range(t0, t1)]))
+    return out
+
+
+def head_grid_features(head: tuple, G: int) -> set:
+    """What the lm_head partition of ``head`` = head_list(...) looks like on G CTAs: "empty" (some CTA holds no tile),
+    "one-each" (G = head_n), "even" / "odd" (some CTA holds an even / odd count above 1), "eos-alone" / "eos-shared"
+    (the inserted EOS tile is the only tile of its CTA / shares it with range tiles)."""
+    head_n, head_lo, head_eos, head_eos_at = head
+    f = set()
+    for t0, t1, tiles in head_partition(head_n, head_eos_at, G, head_lo, head_eos):
+        n = t1 - t0
+        if n == 0:
+            f.add("empty")
+        elif n > 1:
+            f.add("even" if n % 2 == 0 else "odd")
+        if head_eos >= 0 and head_eos in tiles:
+            f.add("eos-alone" if n == 1 else "eos-shared")
+    if G == head_n:
+        f.add("one-each")
+    return f
+
+
+def head_grid_counts(shape: tuple, head: tuple, B: int, max_ctx: int, dev: int, impl=None) -> list:
+    """CTA counts to run a decode of B sequences of ``shape`` on, with the lm_head tile list ``head``: among the counts
+    in [max(8, B n_kv), dev] where ``decode_branch`` takes the persistent kernel, the smallest, the device's count
+    ``dev``, every plan regime's representative (``regime_representatives``), at batch 1 a flat-plan and a whole-K-plan
+    count, the H100 PCIe's 114 and head_n +- 1 (a CTA count next to the list length), and the smallest count showing
+    each ``head_grid_features`` feature some accepted count shows.  Sorted."""
+    ok = [G for G in range(max(8, B * shape[3]), dev + 1) if decode_branch(shape, B, G, max_ctx, impl)["kind"] == "tc"]
+    assert dev in ok, (shape, B, dev)
+    want = {ok[0], dev} | {G for G in regime_representatives(shape, dev).values() if G in ok}
+    want |= {G for G in (114, head[0] - 1, head[0] + 1) if G in ok}
+    if B == 1:
+        for plan in ("flat", "wholeK"):
+            want |= {next((G for G in ok if decode_branch(shape, B, G, max_ctx, impl)["plan"] == plan), dev)}
+    have = set().union(*(head_grid_features(head, G) for G in want))
+    for G in ok:
+        new = head_grid_features(head, G) - have
+        if new:
+            want.add(G)
+            have |= new
+    return sorted(want)
+
+
 def gemm_splits(M: int, N: int, K: int, ws_floats: int) -> int:
     """Split-K slices gemm_dispatch (gemm_tc.cu) picks for an M x N x K bf16 GEMM with a split workspace of
     ``ws_floats`` floats, on the device's SM count (restated)."""

@@ -21,39 +21,11 @@ import torch
 from neutts_air_b200 import synthetic
 from neutts_air_b200.lm import LMShape, SpeechLM
 from tests.helpers import make_lm, runs_persistent, set_decode_impl
-from tests.sampler_ref import (BARS, MARGIN, MIN_NEW, PATTERNS, SEED, Checker, _range, draw_u, fp32_logits, prob_err,
+from tests.processors_ref import bits_equal, hf_chain, ranked
+from tests.sampler_ref import (BARS, MARGIN, MIN_NEW, PATTERNS, SEED, Checker, _range, draw_u, prob_err,
                                processed_scores, programmable, ref_token, ref_window, ref_window_cut, tile_maxima)
 
 pytestmark = pytest.mark.gpu
-
-
-def hf_chain(row, prompt, gen, n, penalty=1.0, decay=None):
-    """transformers' RepetitionPenaltyLogitsProcessor then ExponentialDecayLengthPenalty on one fp32 logits row (torch,
-    CPU): the scores the engine stores.  n: tokens generated before this draw; gen: those tokens."""
-    from transformers.generation.logits_process import ExponentialDecayLengthPenalty, RepetitionPenaltyLogitsProcessor
-
-    x = torch.from_numpy(np.asarray(row, dtype=np.float32).copy())[None]
-    ids = torch.tensor([int(t) for t in list(prompt) + list(gen)][: len(prompt) + n], dtype=torch.long)
-    ids = torch.cat((ids, torch.zeros(len(prompt) + n - ids.numel(), dtype=torch.long)))[None]
-    if penalty != 1.0:
-        x = RepetitionPenaltyLogitsProcessor(float(np.float32(penalty)))(ids, x)
-    if decay is not None and decay[1] != 1.0:
-        x = ExponentialDecayLengthPenalty(decay, EOS_HOLDER[0], len(prompt))(ids, x)
-    return x[0].numpy()
-
-
-EOS_HOLDER = [0]
-
-
-def bits_equal(a, b) -> bool:
-    return np.array_equal(np.asarray(a, dtype=np.float32).view(np.uint32), np.asarray(b, dtype=np.float32).view(np.uint32))
-
-
-def ranked(m, name):
-    lg = fp32_logits(m, name)
-    ids = m.owned[name]
-    ids = ids[ids != m.eos]
-    return ids[np.lexsort((ids, -lg[ids].astype(np.float64)))]
 
 
 # per-slot (min_new_tokens, decay_start, decay_factor): floors 0..3, starts at or after floor - 1, factors on both
@@ -108,7 +80,6 @@ TF_CASES = [
 def test_length_control_every_path(cuda, case, monkeypatch):
     name, V, B, impl, rkind, ctl, pen = case
     m = programmable(V)
-    EOS_HOLDER[0] = m.eos
     cfg, w = m.oracle()
     lm = make_lm(cfg, w, max_batch=B, max_ctx=256, max_new=64)
     set_decode_impl(monkeypatch, impl)
@@ -152,7 +123,7 @@ def test_length_control_every_path(cuda, case, monkeypatch):
         tv, ti, _ = on["cap"]
         for b in range(B):
             mn, start, f = rows[b]
-            want = hf_chain(res["off"][j]["logits"][b], prompts[b], forced[b, :j].tolist(), j, 1.0, (start, f))
+            want = hf_chain(res["off"][j]["logits"][b], prompts[b], forced[b, :j].tolist(), j, 1.0, (start, f), m.eos)
             assert bits_equal(on["logits"][b], want), (name, j, b, np.nonzero(on["logits"][b] != want)[0][:5])
             decayed += not bits_equal(want, off["logits"][b])
             if j > 0 and persistent:
@@ -180,7 +151,7 @@ def _predict(m, first, steps_logits, prompt, mn, decay, n):
     toks = []
     for s in range(n + 1):
         row = first if s == 0 else steps_logits[s - 1]
-        want = hf_chain(row, prompt, toks, s, 1.0, decay)
+        want = hf_chain(row, prompt, toks, s, 1.0, decay, m.eos)
         sc = want.astype(np.float64)
         if s < mn:
             sc[m.eos] = -np.inf
@@ -197,7 +168,6 @@ def test_multistep_launch_ends_at_the_predicted_step(cuda, impl, B, monkeypatch)
     processors predict from the table-off logits."""
     V, n = 217472, 40
     m = programmable(V)
-    EOS_HOLDER[0] = m.eos
     cfg, w = m.oracle()
     lm = make_lm(cfg, w, max_batch=B, max_ctx=256, max_new=64)
     set_decode_impl(monkeypatch, impl)
@@ -229,7 +199,7 @@ def test_multistep_launch_ends_at_the_predicted_step(cuda, impl, B, monkeypatch)
         if pats[b] == "eos":
             assert len(pred) == mn + 1, (b, pred)          # EOS at the first draw the floor allows
         for s in range(len(pred) - 1):                     # the stored logits of every step before EOS
-            want = hf_chain(off[s, b], prompts[b], pred, s + 1, 1.0, (start, f))
+            want = hf_chain(off[s, b], prompts[b], pred, s + 1, 1.0, (start, f), m.eos)
             assert bits_equal(on[s, b], want), (b, s)
 
 
@@ -426,7 +396,6 @@ def test_full_size_teacher_forced(cuda, B, monkeypatch):
     set_decode_impl(monkeypatch, None)
     shape = LMShape()
     V, eos, steps = shape.vocab_size, 151670, 250
-    EOS_HOLDER[0] = eos
     sd = synthetic.lm_state_dict(shape, 0)
     eng = [SpeechLM(shape, sd, device="cuda:0", max_batch=B, max_ctx=1024, max_new=256, max_prefill_tokens=B * 520)
            for _ in range(2)]
@@ -442,7 +411,7 @@ def test_full_size_teacher_forced(cuda, B, monkeypatch):
     for s in range(steps + 1):
         off, on = (x.cpu().numpy() for x in lgs)
         for b in range(B):
-            want = hf_chain(off[b], prompts[b], forced[b, :s].tolist(), s, 1.0, rows[b][1:])
+            want = hf_chain(off[b], prompts[b], forced[b, :s].tolist(), s, 1.0, rows[b][1:], eos)
             assert bits_equal(on[b], want), (B, s, b)
             moved += not bits_equal(want[eos], off[b][eos])
         if s < steps:

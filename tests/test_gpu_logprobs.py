@@ -9,7 +9,7 @@ on, from the same prefill and seed:
   3. ``sampled`` at the steps whose window is captured (the last step of each launch) against float64 over that
      window's processed scores, ``exp(sampled)`` against the captured kept probability, and -inf for forced ids
      outside the window.  Greedy runs: ``sampled`` equals ``model``.
-BARS lists the worst values measured on the H100 and the bars.
+BARS (LOGPROB_BARS of processors_ref.py) lists the worst values measured on the H100 and the bars.
 """
 from __future__ import annotations
 
@@ -22,37 +22,14 @@ import torch
 from neutts_air_b200 import synthetic
 from neutts_air_b200.lm import LMShape, SpeechLM
 from tests.helpers import _tts, make_lm, set_decode_impl
+from tests.processors_ref import LOGPROB_BARS as BARS
+from tests.processors_ref import model_ref, sampled_ref
 from tests.sampler_ref import PATTERNS, PATTERNS_ALL, SEED, _prompts, programmable
 
 pytestmark = pytest.mark.gpu
 
-# Worst errors measured on one H100 80GB HBM3 over this file (see DESIGN.md §4, per-token log-probabilities), and bars:
-BARS = {"model": 5e-5, "sampled": 2e-5, "prob": 4e-7}
 MIN_NEW = 3
 WORST = {k: 0.0 for k in BARS}
-
-
-def lse64(x) -> float:
-    x = np.asarray(x, dtype=np.float64)
-    m = x.max()
-    return float(m + np.log(np.exp(x - m).sum())) if m > -np.inf else -math.inf
-
-
-def model_ref(row, tok: int, eos: int, masked: bool) -> float:
-    """float64 log-softmax of ``tok`` over the processed logits row (EOS left out while masked)."""
-    s = np.asarray(row, dtype=np.float64).copy()
-    if masked:
-        s[eos] = -np.inf
-    return float(s[tok] - lse64(s)) if s[tok] > -np.inf else -math.inf
-
-
-def sampled_ref(row, ids, tok: int, temperature: float) -> float:
-    """float64 log-probability of ``tok`` in the kept window ``ids`` (processed scores fp32(logit * fp32(1 / T)))."""
-    ids = [int(i) for i in ids if i >= 0]
-    if tok not in ids:
-        return -math.inf
-    sc = (np.asarray(row, dtype=np.float32)[ids] * (np.float32(1) / np.float32(temperature))).astype(np.float64)
-    return float(sc[ids.index(tok)] - lse64(sc))
 
 
 def _note(key, err, tag):

@@ -27,34 +27,11 @@ from neutts_air_b200 import synthetic
 from neutts_air_b200.lm import LMShape, SpeechLM
 from tests.fakes import AlignedTok
 from tests.helpers import make_lm, runs_persistent, set_decode_impl
-from tests.sampler_ref import (BARS, MARGIN, MIN_NEW, PATTERNS, SEED, Checker, _range, fp32_logits, prob_err,
+from tests.processors_ref import bits_equal, hf_penalty, ranked
+from tests.sampler_ref import (BARS, MARGIN, MIN_NEW, PATTERNS, SEED, Checker, _range, prob_err,
                                processed_scores, programmable, ref_window, ref_window_cut, tile_maxima)
 
 pytestmark = pytest.mark.gpu
-
-
-def hf_penalty(logits_row, prompt, gen, penalty: float, include: bool):
-    """transformers' RepetitionPenaltyLogitsProcessor on one fp32 logits row (torch, CPU)."""
-    x = torch.from_numpy(np.asarray(logits_row, dtype=np.float32).copy())[None]
-    if penalty == 1.0:
-        return x[0].numpy()
-    from transformers.generation.logits_process import RepetitionPenaltyLogitsProcessor
-
-    ids = torch.tensor([int(t) for t in list(prompt) + list(gen)], dtype=torch.long)[None]
-    proc = RepetitionPenaltyLogitsProcessor(float(np.float32(penalty)), prompt_ignore_length=None if include else len(prompt))
-    return proc(ids, x)[0].numpy()
-
-
-def bits_equal(a, b) -> bool:
-    return np.array_equal(np.asarray(a, dtype=np.float32).view(np.uint32), np.asarray(b, dtype=np.float32).view(np.uint32))
-
-
-def ranked(m, name):
-    """The ids a pattern owns (EOS excluded), by fp32 logit descending: forced tokens that keep a row on its pattern."""
-    lg = fp32_logits(m, name)
-    ids = m.owned[name]
-    ids = ids[ids != m.eos]
-    return ids[np.lexsort((ids, -lg[ids].astype(np.float64)))]
 
 
 PENS = [1.3, 0.7, 2.0, 1.0, 1.15, 0.9, 3.0, 1.05]
