@@ -298,6 +298,26 @@ typedef struct {
  * nt_op_topk_sample, nt_lm_head_gemv and nt_lm_score ignore the table. */
 int nt_lm_set_length_control(nt_lm* lm, const nt_slot_length* host_table, void* stream);
 
+/* Per-slot Repetition Aware Sampling (VALL-E 2; CosyVoice 2's ras_sampling).  At every sampled draw of a slot whose
+ * entry is on, with n the slot's n_generated: the sampler draws token t as usual (u1 = Philox word 0 of counter
+ * {n, stream key, 0, 0}); if t occurs at least min_count times among the slot's generated tokens [max(0, n - window), n)
+ * (its prompt never counts), t is replaced by one draw from the full distribution, the softmax of the processed scores
+ * times 1 / T over the whole vocabulary row (no top-k / top-p / min-p cut), by inverse CDF in ascending id order with
+ * u2 = (Philox word 1 of the same block >> 8) * 2^-24.  Suppressed ids (vocabulary range, EOS while masked) stay out.
+ * The redrawn token is kept even if it repeats too.  Greedy and teacher-forced runs never redraw, nor does token 0
+ * (its window is empty).  With nt_lm_set_logprobs on, a redrawn token's `sampled` value is its log-probability in the
+ * full distribution.  Every draw that does not trigger is bit-identical to the table off. */
+typedef struct {
+  int32_t window;     /* 0 = off for this slot, else 1..64 */
+  int32_t min_count;  /* 1..window */
+} nt_slot_ras;
+
+/* host_table: max_batch entries (row s = slot s), or NULL = off (the default).  Every entry is validated first; a bad
+ * one returns NT_ERR_INVALID and leaves the previous table in force.  The table is copied on `stream`; new values take
+ * effect at the next launch.  nt_lm_debug_ptr(lm, "ras_redraws") is a device int32 [max_batch] count of each slot's
+ * redraws since the prefill that filled it.  nt_op_topk_sample, nt_lm_head_gemv and nt_lm_score ignore the table. */
+int nt_lm_set_repetition_aware_sampling(nt_lm* lm, const nt_slot_ras* host_table, void* stream);
+
 /* Per-token log-probabilities.  out: caller-owned device fp32 [max_batch][max_new][2] (8-byte aligned); entry [s][n]
  * belongs to out_tokens[s][n] and is written wherever that token is (every sampler launch of nt_lm_prefill,
  * nt_lm_prefill_slots and nt_lm_decode); nothing else is written.  NULL switches it off (the default).

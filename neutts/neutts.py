@@ -28,7 +28,7 @@ import numpy as np
 import torch
 
 from neutts_air_b200 import longform
-from neutts_air_b200.lm import check_guidance_scale, per_item, per_prompt_decay, resolve_settings
+from neutts_air_b200.lm import check_guidance_scale, per_item, per_prompt_decay, per_prompt_ras, resolve_settings
 
 SPEECH_RE = re.compile(r"<\|speech_(\d+)\|>")
 CHAT = "user: Convert the text to speech:<|TEXT_REPLACE|>\nassistant:<|SPEECH_REPLACE|>"
@@ -36,10 +36,19 @@ CONTROL_DEFAULTS = dict(temperature=1.0, top_k=50, top_p=1.0, min_p=0.0)   # the
 PENALTY_DEFAULTS = dict(repetition_penalty=1.0, penalize_prompt=True)       # no repetition penalty, as the reference
 
 
+def _ras_arg(n: int, ras):
+    """``repetition_aware_sampling`` of n utterances, validated: None when no utterance has it (nothing is forwarded),
+    one (win_size, tau_r) tuple, or a list with one None / tuple per utterance."""
+    per = per_prompt_ras(n, ras)
+    if per is None:
+        return None
+    return per[0] if not isinstance(ras[0], (list, tuple, type(None))) else per   # one pair, or one entry per utterance
+
+
 def _controls(n: int, temperature, top_k, top_p, min_p, repetition_penalty=1.0, penalize_prompt=True, min_new_tokens=50,
-              exponential_decay_length_penalty=None) -> dict:
-    """Sampling controls of n utterances: each a scalar or one value per utterance (a list then).  The length decay is
-    None, one (start, factor) tuple, or a list with one None / pair per utterance."""
+              exponential_decay_length_penalty=None, repetition_aware_sampling=None) -> dict:
+    """Sampling controls of n utterances: each a scalar or one value per utterance (a list then).  The length decay and
+    the repetition-aware sampling are each None, one pair (a tuple), or a list with one None / pair per utterance."""
     ctl = per_item(n, "utterance", temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p,
                    repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt, min_new_tokens=min_new_tokens)
     decay = exponential_decay_length_penalty
@@ -50,6 +59,7 @@ def _controls(n: int, temperature, top_k, top_p, min_p, repetition_penalty=1.0, 
         else:
             decay = tuple(decay) if per[0] is decay else [None if d is None else tuple(d) for d in per]
     ctl["exponential_decay_length_penalty"] = decay
+    ctl["repetition_aware_sampling"] = _ras_arg(n, repetition_aware_sampling)
     return ctl
 
 
@@ -99,6 +109,8 @@ def _backbone_kw(ctl: dict) -> dict:
         kw.update(pen)
     if ctl.get("exponential_decay_length_penalty") is not None:
         kw["exponential_decay_length_penalty"] = ctl["exponential_decay_length_penalty"]
+    if ctl.get("repetition_aware_sampling") is not None:
+        kw["repetition_aware_sampling"] = ctl["repetition_aware_sampling"]
     if "guidance_scale" in ctl:
         kw["guidance_scale"] = ctl["guidance_scale"]
         kw["negative_prompt_ids"] = ctl["negative_prompt_ids"]
@@ -515,25 +527,26 @@ class NeuTTS:
               min_p: float = 0.0, repetition_penalty: float = 1.0, penalize_prompt: bool = True,
               return_logprobs: bool = False, takes: int = 1, min_new_tokens: int = 50,
               exponential_decay_length_penalty=None, guidance_scale: float = 1.0, negative_text: str | None = None,
-              speed: float = 1.0, long_form: bool = False, pause: float = 0.0):
+              speed: float = 1.0, long_form: bool = False, pause: float = 0.0, repetition_aware_sampling=None):
         """Text + reference voice -> 24 kHz float32 waveform (``neutts/neutts.py:216-243``).  The sampling controls
         default to the reference's values; see ``infer_batch``.  ``return_logprobs``: returns (waveform, log-probs).
         ``takes``: generate that many takes and keep the most probable one (``infer_batch``).  ``guidance_scale`` and
         ``negative_text``: classifier-free guidance (``infer_batch``).  ``speed``: speaking rate (``infer_batch``).
-        ``long_form`` and ``pause``: a text longer than the context, in segments (``infer_batch``)."""
+        ``long_form`` and ``pause``: a text longer than the context, in segments (``infer_batch``).
+        ``repetition_aware_sampling``: redraw a token that loops (``infer_batch``)."""
         out = self.infer_batch([text], [ref_codes], [ref_text], temperature=temperature, top_k=top_k, top_p=top_p,
                                min_p=min_p, repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt,
                                return_logprobs=return_logprobs, takes=takes, min_new_tokens=min_new_tokens,
                                exponential_decay_length_penalty=exponential_decay_length_penalty,
                                guidance_scale=guidance_scale, negative_text=negative_text, speed=speed,
-                               long_form=long_form, pause=pause)
+                               long_form=long_form, pause=pause, repetition_aware_sampling=repetition_aware_sampling)
         return (out[0][0], out[1][0]) if return_logprobs else out[0]
 
     def infer_from_prompt_ids(self, prompts: Sequence[Sequence[int]], max_new_tokens: int | None = None,
                               min_new_tokens: int = 50, slot_base: int = 0, *, temperature=1.0, top_k=50, top_p=1.0,
                               min_p=0.0, repetition_penalty=1.0, penalize_prompt=True, return_logprobs: bool = False,
                               takes: int = 1, exponential_decay_length_penalty=None, guidance_scale=1.0,
-                              negative_prompt_ids=None, speed=1.0):
+                              negative_prompt_ids=None, speed=1.0, repetition_aware_sampling=None):
         """Hot path only: prompt ids (host) -> waveforms (host).  Used by bench.py's end-to-end leg.
         ``slot_base`` offsets the sampler's Philox slot index so chunks / ranks under one seed draw independently.
         More prompts than ``max_batch`` go through the backbone's ``generate_queue`` when it has one.  Sampling
@@ -542,10 +555,12 @@ class NeuTTS:
         ``negative_prompt_ids`` (None, or one id list or None per prompt; None: the prompt's last token) add
         classifier-free guidance (``SpeechLM.generate_batch``; transformers' ``guidance_scale`` and
         ``negative_prompt_ids`` on an injected transformers backbone).  ``speed``: speaking rate of each waveform (a
-        number or one per prompt, ``infer_batch``); it acts on the PCM alone and never reaches the backbone."""
+        number or one per prompt, ``infer_batch``); it acts on the PCM alone and never reaches the backbone.
+        ``repetition_aware_sampling`` as in ``infer_batch``."""
         speeds = _speeds(len(prompts), speed)
         ctl = _controls(len(prompts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
-                        exponential_decay_length_penalty)
+                        exponential_decay_length_penalty, repetition_aware_sampling)
+        self._check_ras(ctl)
         ctl = _add_guidance(ctl, len(prompts), guidance_scale, negative_prompt_ids)
         min_new_tokens = ctl.pop("min_new_tokens")
         takes = self._check_takes(takes)
@@ -561,7 +576,8 @@ class NeuTTS:
     def infer_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], distributed: bool = False, *,
                     temperature=1.0, top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0, penalize_prompt=True,
                     return_logprobs: bool = False, takes: int = 1, min_new_tokens=50, exponential_decay_length_penalty=None,
-                    guidance_scale=1.0, negative_text=None, speed=1.0, long_form: bool = False, pause: float = 0.0):
+                    guidance_scale=1.0, negative_text=None, speed=1.0, long_form: bool = False, pause: float = 0.0,
+                    repetition_aware_sampling=None):
         """List in / list out.  With ``distributed=True`` (inside an initialised torch.distributed job) the
         utterances are sharded over ranks and every rank returns all waveforms (one all-gather).
 
@@ -586,6 +602,13 @@ class NeuTTS:
         end-of-speech score s becomes s + |s| * (factor ** k - 1) at step k past it, so an utterance that runs on ends
         at a point the model picks near the length the caller expects, instead of being cut at the hard cap.  None, one
         pair, or one None / pair per utterance; start must be >= min_new_tokens - 1.
+
+        ``repetition_aware_sampling`` (VALL-E 2's Repetition Aware Sampling, CosyVoice 2's ``ras_sampling``): None (the
+        default), one (win_size, tau_r) pair, or one None / pair per utterance, win_size an int in 1..64 and tau_r in
+        (0, 1].  A drawn code that already occurs at least ceil(win_size * tau_r) times among the utterance's last
+        win_size generated codes is thrown away and drawn again from the whole distribution (no top-k / top-p / min-p
+        cut), which breaks a loop of one repeated code where it happens and leaves every other step alone.  Needs a
+        ``SpeechLM`` backbone (ValueError otherwise: transformers' ``generate`` has no such option).
 
         ``return_logprobs=True`` (not with ``distributed``; needs a ``SpeechLM`` backbone) returns (waveforms,
         log-probs): per utterance a float32 array [n_generated, 2] with the (sampled, model) log-probability of every
@@ -628,7 +651,7 @@ class NeuTTS:
                 texts, ref_codes, ref_texts, temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p,
                 repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt, min_new_tokens=min_new_tokens,
                 exponential_decay_length_penalty=exponential_decay_length_penalty, guidance_scale=guidance_scale,
-                negative_text=negative_text, speed=speed)
+                negative_text=negative_text, speed=speed, repetition_aware_sampling=repetition_aware_sampling)
             out = self.infer_batch(flat, refs, rts, distributed, return_logprobs=return_logprobs, takes=takes, **kw)
             wavs, lps = out if return_logprobs else (out, None)
             idx = [[j for j, o in enumerate(owners) if o == t] for t in range(len(texts))]
@@ -636,7 +659,8 @@ class NeuTTS:
             return (joined, [np.concatenate([lps[j] for j in js]) for js in idx]) if return_logprobs else joined
         speeds = _speeds(len(texts), speed)
         ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
-                        exponential_decay_length_penalty)
+                        exponential_decay_length_penalty, repetition_aware_sampling)
+        self._check_ras(ctl)
         ctl = _add_guidance(ctl, len(texts), guidance_scale,
                             self._negatives(len(texts), guidance_scale, negative_text, ref_codes, ref_texts))
         if takes != 1 and "guidance_scale" in ctl:
@@ -732,8 +756,10 @@ class NeuTTS:
         n = len(texts)
         decay = controls.pop("exponential_decay_length_penalty")
         per = per_prompt_decay(n, decay)
+        ras = _ras_arg(n, controls.pop("repetition_aware_sampling", None))
         kw = {k: [v[t] for t in owners] if isinstance(v, list) else v for k, v in per_item(n, "text", **controls).items()}
         kw["exponential_decay_length_penalty"] = decay if per[0] is decay else [per[t] for t in owners]
+        kw["repetition_aware_sampling"] = [ras[t] for t in owners] if isinstance(ras, list) else ras
         return (owners, [segs[t][k] for t, k in order], [ref_codes[t] for t in owners], [ref_texts[t] for t in owners],
                 kw)
 
@@ -743,6 +769,7 @@ class NeuTTS:
         owners, flat, refs, rts, kw = self._long_form_plan(texts, ref_codes, ref_texts, **controls)
         speeds = _speeds(len(flat), kw.pop("speed"))
         ctl = _controls(len(flat), **kw)
+        self._check_ras(ctl)
         prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(flat, refs, rts)]
         ids = [[int(c) for c in (rc.tolist() if hasattr(rc, "tolist") else rc)] for rc in refs]
         seams = longform.StreamJoin(owners, self.sample_rate, pause, np.int16 if self.pcm_format == "int16" else np.float32)
@@ -802,6 +829,13 @@ class NeuTTS:
         out = self.backbone.score(seqs, [len(p) for p in prompts])
         return [np.asarray(o, dtype=np.float32) for o in out]
 
+    def _check_ras(self, ctl: dict) -> None:
+        """Repetition-aware sampling needs an engine that runs it (``SpeechLM.set_repetition_aware_sampling``):
+        transformers' ``generate`` has no such option, so asking for it elsewhere fails before any generation."""
+        if ctl.get("repetition_aware_sampling") is not None and not hasattr(self.backbone, "set_repetition_aware_sampling"):
+            raise ValueError("repetition_aware_sampling needs a backbone with set_repetition_aware_sampling "
+                             "(neutts_air_b200.SpeechLM)")
+
     def _check_score(self) -> None:
         """Scoring needs an engine that scores (``SpeechLM.score``)."""
         if not hasattr(self.backbone, "score"):
@@ -816,7 +850,8 @@ class NeuTTS:
                      top_p: float = 1.0, min_p: float = 0.0, repetition_penalty: float = 1.0,
                      penalize_prompt: bool = True, takes: int = 1, min_new_tokens: int = 50,
                      exponential_decay_length_penalty=None, guidance_scale=1.0,
-                     speed: float = 1.0, long_form: bool = False, pause: float = 0.0) -> Generator[np.ndarray, None, None]:
+                     speed: float = 1.0, long_form: bool = False, pause: float = 0.0,
+                     repetition_aware_sampling=None) -> Generator[np.ndarray, None, None]:
         """Streaming synthesis with the reference's window geometry (``neutts/neutts.py:373-465``):
         every 25 new frames (once 5 look-ahead frames exist) the codec re-decodes
         [n - 50 - 1, n + 25 + 5 + 1) and the chunk is cross-faded with triangular weights.  Sampling controls as in
@@ -834,10 +869,12 @@ class NeuTTS:
             rounds = self._long_form_stream([text], [ref_codes], [ref_text], pause, temperature=temperature, top_k=top_k,
                                             top_p=top_p, min_p=min_p, repetition_penalty=repetition_penalty,
                                             penalize_prompt=penalize_prompt, min_new_tokens=min_new_tokens,
-                                            exponential_decay_length_penalty=exponential_decay_length_penalty, speed=speed)
+                                            exponential_decay_length_penalty=exponential_decay_length_penalty, speed=speed,
+                                            repetition_aware_sampling=repetition_aware_sampling)
             return self._only_text(rounds)
         ctl = _controls(1, temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
-                        exponential_decay_length_penalty)
+                        exponential_decay_length_penalty, repetition_aware_sampling)
+        self._check_ras(ctl)
         speeds = _speeds(1, speed)
         prompt = self._apply_chat_template(ref_codes, ref_text, text)
         return self._stream(prompt, [int(c) for c in (ref_codes.tolist() if hasattr(ref_codes, "tolist") else ref_codes)], ctl,
@@ -847,7 +884,7 @@ class NeuTTS:
                            top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0,
                            penalize_prompt=True, takes: int = 1, min_new_tokens=50,
                            exponential_decay_length_penalty=None, guidance_scale=1.0, speed=1.0, long_form: bool = False,
-                           pause: float = 0.0) -> Generator[list, None, None]:
+                           pause: float = 0.0, repetition_aware_sampling=None) -> Generator[list, None, None]:
         """Streaming synthesis of many utterances at once (BASELINE.json configs[4]; the reference streams one
         utterance, ``neutts/neutts.py:373-465``).  Every yield is a list with one entry per utterance, as many entries
         as ``texts``: the next audio chunk (float32, cross-faded exactly as in ``infer_stream``) or ``None`` when that
@@ -882,10 +919,12 @@ class NeuTTS:
             return self._long_form_stream(texts, ref_codes, ref_texts, pause, temperature=temperature, top_k=top_k,
                                           top_p=top_p, min_p=min_p, repetition_penalty=repetition_penalty,
                                           penalize_prompt=penalize_prompt, min_new_tokens=min_new_tokens,
-                                          exponential_decay_length_penalty=exponential_decay_length_penalty, speed=speed)
+                                          exponential_decay_length_penalty=exponential_decay_length_penalty, speed=speed,
+                                          repetition_aware_sampling=repetition_aware_sampling)
         self._stream_slots(len(texts))
         ctl = _controls(len(texts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
-                        exponential_decay_length_penalty)
+                        exponential_decay_length_penalty, repetition_aware_sampling)
+        self._check_ras(ctl)
         prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(texts, ref_codes, ref_texts)]
         refs = [[int(c) for c in (rc.tolist() if hasattr(rc, "tolist") else rc)] for rc in ref_codes]
         return self._stream_batch(prompts, refs, ctl, _speeds(len(texts), speed))

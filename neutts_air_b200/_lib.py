@@ -73,6 +73,10 @@ class SlotLength(C.Structure):
     _fields_ = [("min_new_tokens", C.c_int32), ("decay_start", C.c_int32), ("decay_factor", C.c_double)]
 
 
+class SlotRAS(C.Structure):
+    _fields_ = [("window", C.c_int32), ("min_count", C.c_int32)]
+
+
 class SlotGuidance(C.Structure):
     _fields_ = [("partner", C.c_int32), ("scale", C.c_float)]
 
@@ -118,6 +122,7 @@ EXPORTS = [
     "nt_lm_workspace_bytes", "nt_lm_create", "nt_lm_destroy", "nt_lm_prefill", "nt_lm_prefill_slots", "nt_lm_prefill_fork",
     "nt_lm_score_scratch_bytes", "nt_lm_score", "nt_lm_decode",
     "nt_lm_set_slot_sampling", "nt_lm_set_vocab_range", "nt_lm_set_repetition_penalty", "nt_lm_set_length_control",
+    "nt_lm_set_repetition_aware_sampling",
     "nt_lm_set_logprobs", "nt_lm_set_guidance",
     "nt_lm_head_gemv",
     "nt_lm_debug_set_layers", "nt_lm_debug_set_sms", "nt_lm_debug_ptr", "nt_lm_debug_set_profile", "nt_lm_debug_capture_sampler",
@@ -173,6 +178,7 @@ def lib() -> C.CDLL:
     L.nt_lm_set_vocab_range.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
     L.nt_lm_set_repetition_penalty.argtypes = [C.c_void_p, C.POINTER(SlotPenalty), C.c_void_p]
     L.nt_lm_set_length_control.argtypes = [C.c_void_p, C.POINTER(SlotLength), C.c_void_p]
+    L.nt_lm_set_repetition_aware_sampling.argtypes = [C.c_void_p, C.POINTER(SlotRAS), C.c_void_p]
     L.nt_lm_set_logprobs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     L.nt_lm_set_guidance.argtypes = [C.c_void_p, C.POINTER(SlotGuidance), C.c_void_p]
     L.nt_lm_head_gemv.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]

@@ -87,6 +87,7 @@ struct StepSettings {
   bool len_on = false;                // length-control table (nt_lm_set_length_control)
   bool len_decay = false;             // ... and some entry decays (decay_factor != 1): the chain's fix-up launch
   float* logprob_out = nullptr;       // per-token log-probabilities (nt_lm_set_logprobs): nullptr = off
+  bool ras_on = false;                // repetition-aware sampling table (nt_lm_set_repetition_aware_sampling)
   bool guide_on = false;              // classifier-free guidance table (nt_lm_set_guidance): per-op chain, combine + follow
 };
 
@@ -160,6 +161,11 @@ struct nt_lm {
   float2* guide_part = nullptr;            // [max_batch][2][kGuideSplit]
   std::vector<nt_slot_guidance> guide_host;   // host copies of guide_tab and guide_of while the table is on
   std::vector<int> guide_of_host;
+  // repetition-aware sampling (nt_lm_set_repetition_aware_sampling): the per-slot table, every slot's ring of its last
+  // kRasRing generated tokens (written by every sampler launch, table on or off) and its redraw counter
+  nt_slot_ras* ras_tab = nullptr;     // [max_batch]
+  int* ras_ring = nullptr;            // [max_batch][kRasRing]
+  int* ras_redraws = nullptr;         // [max_batch]
 };
 
 // The lm_head tiles a launch computes under the vocabulary range: [t_lo, t_hi), plus eos_tile when EOS lies outside
@@ -256,6 +262,9 @@ static size_t lm_carve(const nt_lm_config& c, void* ws, size_t bytes, F&& assign
     (L)->guide_rows = a.take<nt_slot_guidance>(c.max_batch);                                   \
     (L)->guide_of = a.take<int>(c.max_batch);                                                  \
     (L)->guide_part = a.take<float2>(size_t(c.max_batch) * 2 * kGuideSplit);                   \
+    (L)->ras_tab = a.take<nt_slot_ras>(c.max_batch);                                           \
+    (L)->ras_ring = a.take<int>(size_t(c.max_batch) * kRasRing);                               \
+    (L)->ras_redraws = a.take<int>(c.max_batch);                                               \
   }
 
 static int lm_check_config(const nt_lm_config* c) {
@@ -442,6 +451,9 @@ static SamplerParams make_sampler(const nt_lm* lm, const nt_lm_state* st, const 
   s.len_c = lm->len_c;
   s.len_pitch = lm->cfg.max_ctx;
   s.logprob_out = ss.logprob_out;
+  s.ras_tab = ss.ras_on ? lm->ras_tab : nullptr;
+  s.ras_ring = lm->ras_ring;
+  s.ras_redraws = lm->ras_redraws;
   s.dbg_topk_val = ss.dbg_topk_val, s.dbg_topk_idx = ss.dbg_topk_idx, s.dbg_token = ss.dbg_token;
   return s;
 }
@@ -724,7 +736,7 @@ extern "C" int nt_lm_prefill_slots(nt_lm* lm, const nt_lm_state* st, const int32
   NT_CUDA_CHECK(cudaMemcpyAsync(lm->slot_args, args.data(), args.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
   const int max_pages = c.max_ctx / c.page_size;
   if ((rc = launch_slots_setup(lm->slot_args, B, st->page_table, max_pages, lm->slot_table, st->seq_lens, st->n_generated, st->done,
-                               lm->slot_key, stream)))
+                               lm->slot_key, lm->ras_redraws, stream)))
     return rc;
   if ((rc = prefill_forward(lm, st, ids, cu, B, max_len, lm->slot_table, logits_out, sp->eos_id, stream, lm->slot_args,
                              lm->step.guide_on ? lm->guide_rows : nullptr)))
@@ -770,10 +782,11 @@ static int prefill_fork(nt_lm* lm, const nt_lm_state* st, const int32_t* ids, co
   NT_CUDA_CHECK(cudaMemsetAsync(lm->slot_key, 0xff, size_t(c.max_batch) * sizeof(int), stream));
   NT_CUDA_CHECK(cudaMemsetAsync(st->n_generated, 0, size_t(c.max_batch) * sizeof(int), stream));
   NT_CUDA_CHECK(cudaMemsetAsync(st->done, 0, size_t(c.max_batch) * sizeof(int), stream));
+  NT_CUDA_CHECK(cudaMemsetAsync(lm->ras_redraws, 0, size_t(c.max_batch) * sizeof(int), stream));
   NT_CUDA_CHECK(cudaMemcpyAsync(st->seq_lens, seq.data(), N * sizeof(int), cudaMemcpyHostToDevice, stream));
   const int max_pages = c.max_ctx / c.page_size;
   if ((rc = launch_slots_setup(lm->slot_args, B, st->page_table, max_pages, lm->slot_table, st->seq_lens, st->n_generated, st->done,
-                               lm->slot_key, stream)))
+                               lm->slot_key, nullptr, stream)))   // the memset above zeroed every slot's redraw counter
     return rc;
   if ((rc = prefill_forward(lm, st, ids, cu, B, max_len, lm->slot_table, logits_out, sp->eos_id, stream, lm->slot_args,
                              lm->step.guide_on ? lm->guide_tab : nullptr)))
@@ -1020,8 +1033,8 @@ extern "C" int nt_lm_decode(nt_lm* lm, const nt_lm_state* st, int B, int n_steps
     return NT_OK;
   }
   // The graph is keyed by every input decode_step bakes into its launches: the batch, the state and sampling params,
-  // and the host settings in lm->step.  The slot_sp / rep_tab / len_tab / guide_tab contents stay out: the graph reads
-  // them at replay.
+  // and the host settings in lm->step.  The slot_sp / rep_tab / len_tab / guide_tab / ras_tab contents stay out: the
+  // graph reads them at replay.
   // prof / prof_step stay out: only the persistent kernel reads them, and it never runs from the graph.
   std::vector<uint8_t> key(sizeof(int) + sizeof(nt_lm_state) + sizeof(nt_sampling) + sizeof(StepSettings));
   uint8_t* k = key.data();
@@ -1190,6 +1203,25 @@ extern "C" int nt_lm_set_guidance(nt_lm* lm, const nt_slot_guidance* table, void
   return NT_OK;
 }
 
+extern "C" int nt_lm_set_repetition_aware_sampling(nt_lm* lm, const nt_slot_ras* table, void* stream_) {
+  if (!lm) return set_error(NT_ERR_INVALID, "nt_lm_set_repetition_aware_sampling: null handle");
+  const bool on = table != nullptr;
+  if (on) {
+    for (int s = 0; s < lm->cfg.max_batch; ++s) {
+      const nt_slot_ras& e = table[s];
+      if (e.window < 0 || e.window > kRasRing)
+        return set_error(NT_ERR_INVALID, "slot %d: window %d not in 0..%d (0: off)", s, e.window, kRasRing);
+      if (e.window > 0 && (e.min_count < 1 || e.min_count > e.window))
+        return set_error(NT_ERR_INVALID, "slot %d: min_count %d not in 1..%d (the window)", s, e.min_count, e.window);
+    }
+    // pageable source: the runtime has staged it by the time the call returns
+    NT_CUDA_CHECK(cudaMemcpyAsync(lm->ras_tab, table, size_t(lm->cfg.max_batch) * sizeof(nt_slot_ras), cudaMemcpyHostToDevice,
+                                  reinterpret_cast<cudaStream_t>(stream_)));
+  }
+  lm->step.ras_on = on;
+  return NT_OK;
+}
+
 extern "C" int nt_lm_set_logprobs(nt_lm* lm, float* out, void* stream) {
   (void)stream;   // host state only: read by the launches enqueued after this call
   if (!lm) return set_error(NT_ERR_INVALID, "nt_lm_set_logprobs: null handle");
@@ -1277,7 +1309,7 @@ extern "C" void* nt_lm_debug_ptr(nt_lm* lm, const char* name) {
   const struct { const char* n; void* p; } tab[] = {
       {"h", lm->h}, {"q", lm->q}, {"qkv", lm->qkv}, {"attn", lm->attn}, {"act", lm->act}, {"logits", lm->logits},
       {"xn", lm->xn}, {"attn_bf16", lm->attn_bf16}, {"act_bf16", lm->act_bf16}, {"h_last", lm->h_last},
-      {"tmax", lm->tmax}};
+      {"tmax", lm->tmax}, {"ras_redraws", lm->ras_redraws}};
   for (const auto& e : tab)
     if (!strcmp(e.n, name)) return e.p;
   return nullptr;

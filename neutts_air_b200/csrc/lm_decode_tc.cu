@@ -187,7 +187,9 @@ __host__ __device__ constexpr size_t tc_attn_layout_bytes(int aw) {
 }
 
 // ------------------------------------------------------------------------------------------ the kernel
-template <int NT, bool HILO, bool FOLD>
+// RAS: repetition-aware sampling compiled in (launches with the table on); without it the table-off sampler carries
+// none of its code
+template <int NT, bool HILO, bool FOLD, bool RAS>
 __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_constant__ TcParams P) {
   constexpr int CHUNK = NT * 128;            // bytes of one B-operand k-block
   constexpr int NTOK = HILO ? 8 : NT;        // token slots on the N axis
@@ -890,7 +892,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) decode_tc_kernel(const __grid_c
       float2* h2dst = fold_cta ? P.h2 + static_cast<long long>(fold_no & 1) * kTcH2Copies * H : nullptr;   // copy 0 (B = 1)
       const float h2stamp = __int_as_float(P.hstamp_base + fold_no);
       // the epilogue stored PROCESSED maxima (temperature, EOS mask): no scale, no tile to fix up
-      sample_tiles_seq(P.samp, b, P.tmax, P.ntiles, 1.0f, -1, 0.f, P.logits, P.vocab, ms->mask_eos[b] != 0, uni, P.uni_bytes, ms->sel,
+      sample_tiles_seq<RAS>(P.samp, b, P.tmax, P.ntiles, 1.0f, -1, 0.f, P.logits, P.vocab, ms->mask_eos[b] != 0, uni, P.uni_bytes, ms->sel,
                        csync, pm, h2dst, h2stamp, false);
     };
 
@@ -1249,7 +1251,7 @@ int tc_build_plan(const TcShape& s, int G, bool flat, TcPlan* plan, unsigned cha
 
 template <int NT, bool HILO, bool FOLD>
 static int launch_tc(TcParams& P, int num_sms, cudaStream_t stream) {
-  auto kern = decode_tc_kernel<NT, HILO, FOLD>;
+  auto kern = P.samp.ras_tab ? decode_tc_kernel<NT, HILO, FOLD, true> : decode_tc_kernel<NT, HILO, FOLD, false>;
   const size_t budget = 227 * 1024;
   const size_t misc = (sizeof(TcMisc) + 127) & ~size_t(127);
   const size_t acc = (size_t(128) * (NT + 4) * 4 + 127) & ~size_t(127);   // accumulator tile [128][NT + 4] fp32

@@ -482,16 +482,200 @@ NT_DEVINL float row_logsumexp(const float* lg, int V, int eos, bool mask_eos, fl
   return m + logf(s);
 }
 
+// Repetition-aware redraw on the 256 consumer threads: one draw from the softmax of the whole processed row lg[0, V)
+// times inv_t (id `eos` left out while mask_eos; ids the vocabulary range suppresses hold -inf and add nothing), by
+// inverse CDF in ascending id order with uniform u2.  Thread t sums exp(s * inv_t - m) over its chunk of consecutive
+// ids (ceil(V / 256) rounded up to a multiple of 4, read as float4 when the row is 16-byte aligned); a block scan of
+// the chunk sums in thread order bounds every chunk, and warp 0 walks the one chunk that holds u2 * total, 32 ids per
+// scan, 256 ids per round trip to L2.  Fixed order, no float atomics: a rerun is bit-identical.  m: the row's processed
+// maximum (so every term is <= 1 and the top id's is exactly 1).  sh: sample_finish's ras_sh (24 words).  Every thread
+// returns the token; thread 0 also leaves its log-probability s * inv_t - logsumexp(s * inv_t) in sh[4].
+template <typename Sync>
+NT_DEVINL int ras_full_row_draw(const SamplerParams& p, const float* lg, bool mask_eos, float inv_t, float m, float u2, int* sh,
+                                Sync sync) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int V = p.V, skip = mask_eos ? p.sp.eos_id : -1;
+  const int per = ((V + kConsumerThreads - 1) / kConsumerThreads + 3) & ~3;
+  const int lo = min(V, tid * per), hi = min(V, lo + per);
+  auto term = [&](int i, float x) { return i == skip ? 0.f : __expf(__fmul_rn(x, inv_t) - m); };
+  float part = 0.f;
+  if ((reinterpret_cast<uintptr_t>(lg) & 15) == 0) {   // CTA-uniform; chunks start at multiples of 4
+    for (int i0 = lo; i0 < hi; i0 += 32) {               // 8 float4 loads in flight per thread
+      float4 x[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int i = i0 + 4 * u;
+        if (i + 3 < hi) {
+          x[u] = __ldcg(reinterpret_cast<const float4*>(lg + i));
+        } else {
+          x[u].x = i < hi ? __ldcg(lg + i) : -INFINITY;
+          x[u].y = i + 1 < hi ? __ldcg(lg + i + 1) : -INFINITY;
+          x[u].z = i + 2 < hi ? __ldcg(lg + i + 2) : -INFINITY;
+          x[u].w = -INFINITY;   // i + 3 >= hi
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int i = i0 + 4 * u;
+        part += term(i, x[u].x);
+        part += term(i + 1, x[u].y);
+        part += term(i + 2, x[u].z);
+        part += term(i + 3, x[u].w);
+      }
+    }
+  } else {
+    for (int i0 = lo; i0 < hi; i0 += 8) {
+      float x[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) x[u] = i0 + u < hi ? __ldcg(lg + i0 + u) : -INFINITY;
+#pragma unroll
+      for (int u = 0; u < 8; ++u) part += term(i0 + u, x[u]);
+    }
+  }
+  float incl = part;   // inclusive scan over the warp's chunks
+#pragma unroll
+  for (int off = 1; off < 32; off <<= 1) {
+    const float t = __shfl_up_sync(0xffffffffu, incl, off);
+    if (lane >= off) incl += t;
+  }
+  float excl = __shfl_up_sync(0xffffffffu, incl, 1);
+  if (lane == 0) excl = 0.f;
+  const unsigned mass = __ballot_sync(0xffffffffu, part > 0.f);
+  float* wsum = reinterpret_cast<float*>(sh + 8);
+  unsigned* wmass = reinterpret_cast<unsigned*>(sh + 16);
+  if (lane == 31) wsum[warp] = incl;
+  if (lane == 0) wmass[warp] = mass;
+  sync();
+  float base = 0.f, total = 0.f;   // the same sequential sum for every thread: chunk bounds meet exactly
+  int last_t = -1;                 // the last thread whose chunk has mass
+#pragma unroll
+  for (int w = 0; w < kConsumerWarps; ++w) {
+    if (w == warp) base = total;
+    total += wsum[w];
+    if (wmass[w]) last_t = 32 * w + 31 - __clz(static_cast<int>(wmass[w]));
+  }
+  const float target = u2 * total, lo_cdf = base + excl, hi_cdf = base + incl;
+  // the chunk holding the target; when rounding puts the target at the total, the last chunk with mass
+  if (part > 0.f && lo_cdf <= target && (target < hi_cdf || tid == last_t)) sh[5] = tid, sh[6] = __float_as_int(lo_cdf);
+  sync();
+  if (warp == 0) {
+    const int t = sh[5], wlo = min(V, t * per), whi = min(V, wlo + per);
+    float cum = __int_as_float(sh[6]);
+    int tok = -1, last = -1;   // warp-uniform
+    for (int i0 = wlo; i0 < whi && tok < 0; i0 += 8 * 32) {
+      float x[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int i = i0 + 32 * u + lane;
+        x[u] = i < whi ? __ldcg(lg + i) : -INFINITY;
+      }
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int i = i0 + 32 * u + lane;
+        const float e = i < whi ? term(i, x[u]) : 0.f;
+        float c = e;   // inclusive scan of the 32 ids
+#pragma unroll
+        for (int off = 1; off < 32; off <<= 1) {
+          const float a = __shfl_up_sync(0xffffffffu, c, off);
+          if (lane >= off) c += a;
+        }
+        const unsigned hit = __ballot_sync(0xffffffffu, e > 0.f && cum + c > target);
+        const unsigned pos = __ballot_sync(0xffffffffu, e > 0.f);
+        if (tok < 0) {
+          if (hit) {
+            tok = i0 + 32 * u + __ffs(hit) - 1;
+          } else {
+            if (pos) last = i0 + 32 * u + 31 - __clz(static_cast<int>(pos));
+            cum += __shfl_sync(0xffffffffu, c, 31);
+          }
+        }
+      }
+    }
+    if (lane == 0) sh[3] = tok >= 0 ? tok : last;
+  }
+  sync();
+  const int tok = sh[3];
+  if (tid == 0) sh[4] = __float_as_int((__fmul_rn(__ldcg(lg + tok), inv_t) - m) - logf(total));
+  return tok;
+}
+
+// Whether token tok occurs at least min_count times among slot s's generated tokens [max(0, ngen - window), ngen) (its
+// repetition-aware entry; window 0 = off), read from the slot's ring 16 entries per round trip to L2 (one thread).
+NT_DEVINL bool ras_window_hit(const SamplerParams& p, int s, int ngen, int tok) {
+  const nt_slot_ras re = p.ras_tab[s];
+  const int lo = max(0, ngen - re.window);
+  const int32_t* ring = p.ras_ring + static_cast<long long>(s) * kRasRing;
+  int c = 0;
+  for (int j0 = ngen - 1; j0 >= lo; j0 -= 16) {
+#pragma unroll
+    for (int u = 0; u < 16; ++u) {
+      const int j = j0 - u;
+      c += (j >= lo && __ldcg(ring + (j & (kRasRing - 1))) == tok) ? 1 : 0;
+    }
+  }
+  return re.window > 0 && c >= re.min_count;
+}
+
+// model log-probability of token tok: log-softmax over the processed logits row lg (penalty, EOS mask, range; no
+// temperature or warpers), lse = row_logsumexp of that row
+NT_DEVINL float model_logprob(const SamplerParams& p, const float* lg, int tok, bool mask_eos, float lse) {
+  const float st = (tok < 0 || tok >= p.V || (mask_eos && tok == p.sp.eos_id)) ? -INFINITY : __ldcg(lg + tok);
+  return st - lse;
+}
+
+// Thread 0 of the sampler: the drawn token of sample row b into slot s, at n_generated ngen -- the capture, its
+// log-probabilities (when on), and unless the row is stateless or finished, out_tokens and the state that goes with it.
+// redrawn: a repetition-aware redraw (counted per slot).
+NT_DEVINL void sample_commit(const SamplerParams& p, int b, int s, int ngen, int tok, bool logprobs, float sampled, float model,
+                             bool write_state, bool redrawn, int* s_tok) {
+  *s_tok = tok;
+  if (p.dbg_token) p.dbg_token[b] = tok;
+  if (logprobs) reinterpret_cast<float2*>(p.logprob_out)[static_cast<long long>(s) * p.max_new + ngen] = make_float2(sampled, model);
+  if (write_state) {
+    p.out_tokens[static_cast<long long>(s) * p.max_new + ngen] = tok;
+    // the history bit of this token: the persistent kernel's epi_head reads it at the next step, behind the grid
+    // barrier this thread arrives at after the sampler (see DESIGN.md §4, repetition penalty)
+    if (p.rep_hist) atomicOr(p.rep_hist + static_cast<long long>(s) * p.rep_words + (tok >> 5), 1u << (tok & 31));
+    // the repetition-aware window's entry, read by later steps behind the same barrier
+    if (p.ras_ring) p.ras_ring[static_cast<long long>(s) * kRasRing + (ngen & (kRasRing - 1))] = tok;
+    if (redrawn) p.ras_redraws[s] = __ldcg(p.ras_redraws + s) + 1;
+    p.n_generated[s] = ngen + 1;
+    p.cur_token[s] = tok;
+    const int cached = __ldcg(p.seq_lens + s) + p.advance;  // decode: this step's input token is now in the KV cache
+    if (p.advance) p.seq_lens[s] = cached;
+    const int total = cached + 1;  // tokens in context once `tok` is appended
+    const int lim = p.sp.limits ? min(p.sp.max_new_tokens, __ldg(p.sp.limits + s)) : p.sp.max_new_tokens;
+    if (tok == p.sp.eos_id || ngen + 1 >= lim || ngen + 1 >= p.max_new || total >= p.max_ctx) p.done[s] = 1;
+  }
+}
+
+// The repetition-aware redraw of a live, sampled row (all 256 consumer threads; sample_finish's ras_sh holds u2 and the
+// row's processed maximum): the full-row draw, then thread 0 commits the new token with its log-probability in the
+// full distribution.  Out of line, so that the kernels' register allocation of the common path does not carry it.  p is
+// taken by reference: every kernel that samples declares its parameters __grid_constant__, so the reference points at
+// the kernel's parameter space (otherwise each thread would copy the parameters to local memory at entry).
+template <typename Sync>
+__device__ __noinline__ void ras_redraw(const SamplerParams& p, int b, int s, int ngen, const float* lg, bool mask_eos, float lse,
+                                        bool logprobs, int* s_tok, int* sh, Sync sync) {
+  const int tok = ras_full_row_draw(p, lg, mask_eos, row_sampling(p, s).inv_t, __int_as_float(sh[2]), __int_as_float(sh[1]), sh, sync);
+  if (threadIdx.x == 0)
+    sample_commit(p, b, s, ngen, tok, logprobs, __int_as_float(sh[4]), logprobs ? model_logprob(p, lg, tok, mask_eos, lse) : 0.f,
+                  true, true, s_tok);
+  sync();
+}
+
 // Tail of the sampler for sequence b, given the k kept candidates sorted (score desc, index asc) in win[0..k):
 // softmax over them (TopK processor + softmax, utils.py:2789), the slot's top-p and min-p cuts (which keep a prefix
 // k' <= k of the window, renormalised), Philox draw over the prefix, state update, stop flags, and the next
 // token's embedding -> residual stream row (fp32; optionally also as (value, stamp) pairs for the polled hand-off).
 // With p.logprob_out, the written token's (sampled, model) log-probabilities go next to it (DESIGN.md §4, per-token
 // log-probabilities); the model one takes one extra pass over logits row b.
+// kRas = false compiles repetition-aware sampling out (the persistent kernel's instantiations for a launch with the
+// table off); the ring entry is written either way.
 // Clobbers win[kTopKeep .. 2 kTopKeep) (exponentials).  b: sample row; slot >= 0: the slot whose state row b updates
 // (prefill into chosen slots), else slot b; src >= 0: the logits row sample row b reads (several takes of one
 // prompt), else row b.
-template <typename Sync>
+template <bool kRas = true, typename Sync>
 NT_DEVINL void sample_finish(const SamplerParams& p, int b, int k, Cand* win, int* s_tok, bool stateless, int ngen, bool is_done, Sync sync,
                              float2* h2dst = nullptr, float h2stamp = 0.f, int slot = -1, int src = -1) {
   const int tid = threadIdx.x;
@@ -502,6 +686,10 @@ NT_DEVINL void sample_finish(const SamplerParams& p, int b, int k, Cand* win, in
   const float* lg = p.logits + static_cast<long long>(src >= 0 ? src : b) * p.V;
   float lse = 0.f;
   if (logprobs) lse = row_logsumexp(lg, p.V, p.sp.eos_id, mask_eos, reinterpret_cast<float2*>(ev + kTopKeep), sync);
+  // repetition-aware sampling's shared words, behind row_logsumexp's pairs: [0] redraw flag (CTA-uniform after the
+  // barrier), [1] u2, [2] the row's processed maximum, [3] redrawn token, [4] its log-probability, [5, 6] the chunk
+  // holding the target and its lower bound, [8, 16) warp sums, [16, 24) warp masks of chunks with mass
+  int* ras_sh = reinterpret_cast<int*>(ev + kTopKeep + 2 * kConsumerWarps);
   if (tid < 32) {
     const float m = win[0].v;
     float e0 = (tid < k) ? __expf(win[tid].v - m) : 0.f;
@@ -540,6 +728,7 @@ NT_DEVINL void sample_finish(const SamplerParams& p, int b, int k, Cand* win, in
     __syncwarp();
     if (tid == 0) {
       int tok;
+      uint32_t word1 = 0;   // Philox word 1 of the draw's block: the repetition-aware redraw's uniform
       if (p.sp.forced && !stateless) {
         tok = p.sp.forced[static_cast<long long>(s) * p.max_new + ngen];
       } else if (p.sp.greedy) {
@@ -562,39 +751,38 @@ NT_DEVINL void sample_finish(const SamplerParams& p, int b, int k, Cand* win, in
             break;
           }
         }
+        word1 = ctr[1];
       }
-      *s_tok = tok;
-      if (p.dbg_token) p.dbg_token[b] = tok;
-      if (logprobs) {
-        // model: log-softmax over the processed logits row (penalty, EOS mask, range; no temperature or warpers)
-        const float st = (tok < 0 || tok >= p.V || (mask_eos && tok == p.sp.eos_id)) ? -INFINITY : __ldcg(lg + tok);
-        const float model = st - lse;
-        // sampled: the token's log-probability in the kept window the draw used (greedy: transformers applies no
-        // warpers, so it is the model value); -inf for a forced id outside the window
-        float sampled = model;
-        if (p.sp.forced || !p.sp.greedy) {
-          int j = 0;
-          while (j < k && win[j].i != tok) ++j;
-          sampled = j < k ? (win[j].v - win[0].v) - logf(sum) : -INFINITY;
+      // Repetition-aware sampling: the drawn token's count among the slot's last `window` generated tokens (ring
+      // entries written by earlier steps' samplers, behind the grid barrier or launch boundary that followed them).
+      // Thread 0 counts on its own, so that nothing stands between its draw and its state update.
+      bool redraw = false;
+      if (kRas && p.ras_tab) {
+        if (!stateless && !is_done && !p.sp.forced && !p.sp.greedy) redraw = ras_window_hit(p, s, ngen, tok);
+        ras_sh[0] = redraw ? 1 : 0;
+      }
+      if (redraw) {
+        ras_sh[1] = __float_as_int((word1 >> 8) * (1.0f / 16777216.0f));
+        ras_sh[2] = __float_as_int(win[0].v);   // the processed maximum of the row: the full pass's shift
+      } else {
+        float model = 0.f, sampled = 0.f;
+        if (logprobs) {
+          model = model_logprob(p, lg, tok, mask_eos, lse);
+          // sampled: the token's log-probability in the kept window the draw used (greedy: transformers applies no
+          // warpers, so it is the model value); -inf for a forced id outside the window
+          sampled = model;
+          if (p.sp.forced || !p.sp.greedy) {
+            int j = 0;
+            while (j < k && win[j].i != tok) ++j;
+            sampled = j < k ? (win[j].v - win[0].v) - logf(sum) : -INFINITY;
+          }
         }
-        reinterpret_cast<float2*>(p.logprob_out)[static_cast<long long>(s) * p.max_new + ngen] = make_float2(sampled, model);
-      }
-      if (!stateless && !is_done) {
-        p.out_tokens[static_cast<long long>(s) * p.max_new + ngen] = tok;
-        // the history bit of this token: the persistent kernel's epi_head reads it at the next step, behind the grid
-        // barrier this thread arrives at after the sampler (see DESIGN.md §4, repetition penalty)
-        if (p.rep_hist) atomicOr(p.rep_hist + static_cast<long long>(s) * p.rep_words + (tok >> 5), 1u << (tok & 31));
-        p.n_generated[s] = ngen + 1;
-        p.cur_token[s] = tok;
-        const int cached = __ldcg(p.seq_lens + s) + p.advance;  // decode: this step's input token is now in the KV cache
-        if (p.advance) p.seq_lens[s] = cached;
-        const int total = cached + 1;  // tokens in context once `tok` is appended
-        const int lim = p.sp.limits ? min(p.sp.max_new_tokens, __ldg(p.sp.limits + s)) : p.sp.max_new_tokens;
-        if (tok == p.sp.eos_id || ngen + 1 >= lim || ngen + 1 >= p.max_new || total >= p.max_ctx) p.done[s] = 1;
+        sample_commit(p, b, s, ngen, tok, logprobs, sampled, model, !stateless && !is_done, false, s_tok);
       }
     }
   }
   sync();
+  if (kRas && p.ras_tab && ras_sh[0]) ras_redraw(p, b, s, ngen, lg, mask_eos, lse, logprobs, s_tok, ras_sh, sync);   // CTA-uniform
   if (!stateless && !is_done && p.h) {
     const int tok = *s_tok;
     const __nv_bfloat16* e = p.embed + static_cast<long long>(tok) * p.hidden;
@@ -612,7 +800,7 @@ NT_DEVINL void sample_finish(const SamplerParams& p, int b, int k, Cand* win, in
 // processed) in row b of the candidate arrays, softmax, draw, state update, next embedding.  keys: [ncand] uint32
 // shared; scratch: [kSelScratch]; win: [2*kTopKeep].  Stateless (see sample_tiles_seq) when p.n_generated_override is
 // set: a run-time test here, where a caller's compile-time flag shifts ptxas's spills in the persistent kernel.
-template <typename Sync>
+template <bool kRas = true, typename Sync>
 NT_DEVINL void sample_stage2_seq(const SamplerParams& p, int b, int ncand, uint32_t* keys, uint32_t* scratch, Cand* win, int* s_tok,
                                  Sync sync, int slot = -1, int src = -1) {
   const int tid = threadIdx.x;
@@ -658,7 +846,7 @@ NT_DEVINL void sample_stage2_seq(const SamplerParams& p, int b, int ncand, uint3
     win[rank] = me;
   }
   sync();
-  sample_finish(p, b, k, win, s_tok, stateless, ngen, is_done, sync, nullptr, 0.f, slot, src);
+  sample_finish<kRas>(p, b, k, win, s_tok, stateless, ngen, is_done, sync, nullptr, 0.f, slot, src);
 }
 
 // Sampler of the tile-max schemes, for sequence b, on 256 threads (0..255) of one CTA.  The lm_head epilogue left the
@@ -673,7 +861,7 @@ NT_DEVINL void sample_stage2_seq(const SamplerParams& p, int b, int ncand, uint3
 //   uni / uni_bytes: >= 16 KB of shared scratch (1024-byte aligned); sel: >= 4 ints of shared memory.
 //   stateless (nt_op_topk_sample): n_generated_override[b] is the row's count, the row is live and no state is written.
 //   src >= 0: the logits and tile-maxima row sample row b reads (see sample_finish), else row b.
-template <typename Sync, typename Mark>
+template <bool kRas = true, typename Sync, typename Mark>
 NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax, int nt, float tmax_scale, int fix_tile, float fix_val,
                                 const float* logits, int V, bool mask_eos, uint8_t* uni, unsigned uni_bytes, int* sel, Sync sync, Mark pm,
                                 float2* h2dst, float h2stamp, bool stateless, int slot = -1, int src = -1) {
@@ -811,7 +999,7 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
             }
             sync();
             pm(124);
-            sample_finish(p, b, k2, win, s_tok, stateless, ngen, is_done, sync, h2dst, h2stamp, slot, src);
+            sample_finish<kRas>(p, b, k2, win, s_tok, stateless, ngen, is_done, sync, h2dst, h2stamp, slot, src);
             pm(125);
             return;
           }
@@ -895,7 +1083,7 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
       if (rank < k2) win[rank] = me;
     }
     sync();
-    sample_finish(p, b, k2, win, s_tok, stateless, ngen, is_done, sync, h2dst, h2stamp, slot, src);
+    sample_finish<kRas>(p, b, k2, win, s_tok, stateless, ngen, is_done, sync, h2dst, h2stamp, slot, src);
     return;
   }
   // ---- general path (thousands of candidates: tiny vocabularies, or exact ties at the threshold)
@@ -970,7 +1158,7 @@ NT_DEVINL void sample_tiles_seq(const SamplerParams& p, int b, const float* tmax
     }
   }
   sync();
-  sample_stage2_seq(p, b, ncand, keys, scratch, win, s_tok, sync, slot, src);
+  sample_stage2_seq<kRas>(p, b, ncand, keys, scratch, win, s_tok, sync, slot, src);
   if (h2dst) {  // the next token's embedding becomes the residual stream of the next step's first fold
     sync();
     for (int i = tid; i < H; i += kConsumerThreads) h2dst[i] = make_float2(p.h[static_cast<long long>(b) * H + i], h2stamp);

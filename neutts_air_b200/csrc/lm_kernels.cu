@@ -682,7 +682,7 @@ struct NoMarkI {
   NT_DEVINL void operator()(int) const {}
 };
 constexpr unsigned kTilesScratch = 96 * 1024;
-__global__ void __launch_bounds__(kConsumerThreads) topk_tiles_kernel(const SamplerParams p, const float* tmax, const int nt,
+__global__ void __launch_bounds__(kConsumerThreads) topk_tiles_kernel(const __grid_constant__ SamplerParams p, const float* tmax, const int nt,
                                                                       const int32_t* skip) {
   extern __shared__ uint8_t tiles_raw[];
   uint8_t* uni = tiles_raw + ((1024u - (smem_u32(tiles_raw) & 1023u)) & 1023u);
@@ -1321,7 +1321,7 @@ int launch_score_combine(const float2* lse, long long ld, int nt, const float* z
 
 // one CTA per listed slot: compact page-table row + the slot's fresh length, counters and Philox key
 __global__ void slots_setup_kernel(const int32_t* args, int B, const int32_t* page_table, int max_pages, int32_t* table,
-                                   int32_t* seq_lens, int32_t* n_generated, int32_t* done, int32_t* slot_key) {
+                                   int32_t* seq_lens, int32_t* n_generated, int32_t* done, int32_t* slot_key, int32_t* ras_redraws) {
   pdl_launch_dependents();
   pdl_wait();
   const int i = blockIdx.x, s = args[i];
@@ -1332,12 +1332,13 @@ __global__ void slots_setup_kernel(const int32_t* args, int B, const int32_t* pa
     seq_lens[s] = args[2 * B + i];
     n_generated[s] = 0;
     done[s] = 0;
+    if (ras_redraws) ras_redraws[s] = 0;
   }
 }
 int launch_slots_setup(const int32_t* args, int B, const int32_t* page_table, int max_pages, int32_t* table, int32_t* seq_lens,
-                       int32_t* n_generated, int32_t* done, int32_t* slot_key, cudaStream_t s) {
+                       int32_t* n_generated, int32_t* done, int32_t* slot_key, int32_t* ras_redraws, cudaStream_t s) {
   return launch_kernel(slots_setup_kernel, dim3(B), dim3(128), 0, s, true, args, B, page_table, max_pages, table, seq_lens, n_generated,
-                       done, slot_key);
+                       done, slot_key, ras_redraws);
 }
 
 // grid (children, n_layers * 2 * n_kv [+ 1 with hist]), 128 threads.  CTA (c, y < n_layers * 2 * n_kv) copies the first

@@ -118,7 +118,14 @@ struct SamplerParams {
   // per-token log-probabilities (nt_lm_set_logprobs): [max_batch][max_new][2] (sampled, model), nullptr = off.
   // sample_finish writes the pair of every token it writes to out_tokens.
   float* logprob_out;
+  // repetition-aware sampling (nt_lm_set_repetition_aware_sampling): per-slot (window, min_count) table, nullptr = off.
+  // ras_ring [max_batch][kRasRing]: sample_finish writes entry n % kRasRing of every token n it writes to out_tokens,
+  // table on or off; ras_redraws [max_batch]: redraws of the slot since the prefill that filled it.
+  const nt_slot_ras* ras_tab;
+  int32_t* ras_ring;
+  int32_t* ras_redraws;
 };
+constexpr int kRasRing = 64;   // generated tokens each slot keeps for the repetition window (the largest window)
 int launch_sampler_check(const SamplerParams& p);
 // tmax: [B][nt] RAW maxima of the 128-column tiles of p.logits (GEMM epilogue, gemm_dispatch(..., tile_max), or
 // launch_tile_max).  p.n_generated_override set: stateless (nt_op_topk_sample).  skip (optional, [max_batch]): rows
@@ -194,9 +201,10 @@ int launch_attn_prefill(const AttnPrefillParams& p, int B, int n_layers, cudaStr
 int kv_pool_tmap(const KVLayout& kv, int n_layers, ::CUtensorMap_st* out);
 int launch_gather_rows(const float* src, const int32_t* rows, int n, int cols, float* dst, cudaStream_t s);
 // Prefill into chosen slots.  args: device [3][B] = slots, Philox stream keys, prompt lengths.  Gathers the listed
-// slots' page-table rows into table [B][max_pages] and resets those slots' seq_lens / n_generated / done / slot_key.
+// slots' page-table rows into table [B][max_pages] and resets those slots' seq_lens / n_generated / done / slot_key, and
+// their repetition-aware redraw counters when ras_redraws is given.
 int launch_slots_setup(const int32_t* args, int B, const int32_t* page_table, int max_pages, int32_t* table, int32_t* seq_lens,
-                       int32_t* n_generated, int32_t* done, int32_t* slot_key, cudaStream_t s);
+                       int32_t* n_generated, int32_t* done, int32_t* slot_key, int32_t* ras_redraws, cudaStream_t s);
 // Several takes of one prompt.  args: device [3][nc] = parent slot, child slot, prompt length P of each child.  For
 // every child with P % 64 != 0, rows [0, P % 64) of the parent's page P / 64 (its partly filled last prompt page) are
 // copied into the child's page P / 64, in every layer, K and V, every KV head; full prompt pages are shared through

@@ -367,6 +367,54 @@ def per_prompt_length(n: int, min_new_tokens, decay, max_new: int | None = None)
             for m, d in zip(floors, decays)]
 
 
+RAS_OFF = (0, 0)   # (window, min_count) of a slot without repetition-aware sampling
+RAS_MAX_WINDOW = 64   # the generated tokens each slot keeps on the device for its window
+
+
+def check_ras(win_size, tau_r) -> tuple:
+    """One prompt's repetition-aware sampling (VALL-E 2's RAS, CosyVoice 2's ``ras_sampling(win_size, tau_r)``),
+    validated as ``nt_lm_set_repetition_aware_sampling`` does -> the slot entry (window, min_count).  ``win_size``: an
+    int in 1..64, the generated tokens the window looks back over; ``tau_r``: finite in (0, 1], not a bool.  A draw
+    is redrawn from the whole distribution when it occurs at least ``min_count = ceil(win_size * tau_r)`` times in the
+    window (float64, exactly CosyVoice's ``rep_num >= win_size * tau_r``)."""
+    if not _is_int(win_size) or not 1 <= win_size <= RAS_MAX_WINDOW:
+        raise ValueError(f"repetition_aware_sampling win_size {win_size!r} must be an integer in 1..{RAS_MAX_WINDOW}")
+    if isinstance(tau_r, (bool, np.bool_)) or not isinstance(tau_r, (int, float, np.integer, np.floating)):
+        raise ValueError(f"repetition_aware_sampling tau_r {tau_r!r} must be a number")
+    t = float(tau_r)
+    if not (math.isfinite(t) and 0 < t <= 1):
+        raise ValueError(f"repetition_aware_sampling tau_r {tau_r} must be finite and in (0, 1]")
+    return int(win_size), int(math.ceil(int(win_size) * t))
+
+
+def ras_entry(row) -> tuple:
+    """The slot entry of one prompt's setting: None -> ``RAS_OFF``, a (win_size, tau_r) pair -> ``check_ras``."""
+    if row is None:
+        return RAS_OFF
+    if not isinstance(row, (list, tuple)) or len(row) != 2:
+        raise ValueError(f"repetition_aware_sampling must be None or one (win_size, tau_r) pair; got {row!r}")
+    return check_ras(*row)
+
+
+def per_prompt_ras(n: int, ras):
+    """``repetition_aware_sampling`` of n prompts: None, one (win_size, tau_r) pair, or one None / pair per prompt.
+    Returns None when no prompt has it (no engine call), else one validated pair (a tuple) or None per prompt."""
+    pair = lambda r: isinstance(r, (list, tuple)) and len(r) == 2 and not any(isinstance(x, (list, tuple)) or x is None
+                                                                             for x in r)
+    if ras is None:
+        return None
+    if pair(ras):
+        rows = [tuple(ras)] * n
+    elif isinstance(ras, (list, tuple)) and len(ras) == n and all(r is None or pair(r) for r in ras):
+        rows = [None if r is None else tuple(r) for r in ras]
+    else:
+        raise ValueError(f"repetition_aware_sampling must be None, one (win_size, tau_r) pair, or one None / pair per "
+                         f"prompt ({n}); got {ras!r}")
+    for r in rows:
+        ras_entry(r)
+    return None if all(r is None for r in rows) else rows
+
+
 NO_GUIDANCE = (-1, 1.0)   # (partner, scale) of a slot outside every guided pair
 
 
@@ -471,6 +519,7 @@ class Settings:
     min_new_tokens: int = 50   # the launch scalar, row 0's while the length table is on
     guidance: list | None = None  # one (partner slot, scale) per slot of the prefill (NO_GUIDANCE outside a pair);
                                   # None: guidance off
+    ras: list | None = None    # one (win_size, tau_r) or None per prompt; None: repetition-aware sampling off
 
     def floors(self, n: int) -> list:
         """The min_new_tokens of each of the n prompts."""
@@ -478,7 +527,7 @@ class Settings:
 
     def apply(self, lm, n: int) -> None:
         """Before a prefill of prompts 0..n-1 into slots 0..n-1, on its stream: controls, then range, then penalty, then
-        length control, then log-probabilities.  Each setting is applied, or switched off when an earlier call left it on, or makes no call when it is off and
+        length control, then repetition-aware sampling, then log-probabilities.  Each setting is applied, or switched off when an earlier call left it on, or makes no call when it is off and
         stays off.  ``lm`` needs the ``set_*`` methods only when a call is due; a missing mirror counts as off."""
         if self.controls is not None or getattr(lm, "_slot_sp_host", None) is not None:
             lm.set_slot_sampling(None if self.controls is None else self.controls[:n])
@@ -490,6 +539,8 @@ class Settings:
             lm.set_repetition_penalty(None if self.penalty is None else self.penalty[:n])
         if self.length is not None or getattr(lm, "_length_host", None) is not None:
             lm.set_length_control(None if self.length is None else self.length[:n])
+        if self.ras is not None or getattr(lm, "_ras_host", None) is not None:
+            lm.set_repetition_aware_sampling(None if self.ras is None else self.ras[:n])
         if self.logprobs != (getattr(lm, "logprobs", None) is not None):
             lm.set_logprobs(self.logprobs)
         if self.guidance is not None:   # the whole table: no pair of an earlier call survives
@@ -511,13 +562,14 @@ class Settings:
         for c, u, g in pairs:
             table[c] = (u, g)
         return dataclasses.replace(self, controls=rows(self.controls), penalty=rows(self.penalty), length=rows(self.length),
-                                   guidance=table)
+                                   ras=rows(self.ras), guidance=table)
 
     def repeat(self, n: int) -> "Settings":
         """The settings of n takes of every prompt: each prompt's row repeated n times, in slot order (take j of prompt
         i in slot i * n + j), so that ``apply`` writes it into all of the prompt's take slots."""
         rows = lambda r: None if r is None else [x for x in r for _ in range(n)]
-        return dataclasses.replace(self, controls=rows(self.controls), penalty=rows(self.penalty), length=rows(self.length))
+        return dataclasses.replace(self, controls=rows(self.controls), penalty=rows(self.penalty), length=rows(self.length),
+                                   ras=rows(self.ras))
 
     def admit(self, lm, slots, idx, guide=None) -> None:
         """Before a refill of prompts ``idx`` into ``slots``: writes their rows; every other slot keeps its own, and
@@ -529,25 +581,29 @@ class Settings:
             lm.set_repetition_penalty([self.penalty[i] for i in idx], slots=slots)
         if self.length is not None:
             lm.set_length_control([self.length[i] for i in idx], slots=slots)
+        if self.ras is not None:
+            lm.set_repetition_aware_sampling([self.ras[i] for i in idx], slots=slots)
         if guide is not None:
             lm.set_guidance(list(guide.values()), slots=list(guide))
 
 
 def resolve_settings(lm, n: int, temperature=1.0, top_k=50, top_p=1.0, min_p=0.0, vocab_range=None,
                      repetition_penalty=1.0, penalize_prompt=True, logprobs=False, min_new_tokens=50,
-                     exponential_decay_length_penalty=None, max_new: int | None = None) -> Settings:
+                     exponential_decay_length_penalty=None, max_new: int | None = None,
+                     repetition_aware_sampling=None) -> Settings:
     """The settings of n prompts on engine ``lm``, each control a scalar or one value per prompt
-    (``per_prompt_controls``, ``per_prompt_penalty``, ``per_prompt_length``, ``check_vocab_range``; ``lm.shape`` is
-    read only for a range).  ``max_new``: the call's largest generated-token cap, against which a decay is checked."""
+    (``per_prompt_controls``, ``per_prompt_penalty``, ``per_prompt_length``, ``per_prompt_ras``,
+    ``check_vocab_range``; ``lm.shape`` is read only for a range).  ``max_new``: the call's largest generated-token cap, against which a decay is checked."""
     if vocab_range is not None:
         vocab_range = check_vocab_range(vocab_range, lm.shape.vocab_size)
     penalty = per_prompt_penalty(n, repetition_penalty, penalize_prompt)
     length = per_prompt_length(n, min_new_tokens, exponential_decay_length_penalty, max_new)
+    ras = per_prompt_ras(n, repetition_aware_sampling)
     controls = per_prompt_controls(n, temperature, top_k, top_p, min_p)
     if controls:
         temperature, top_k = controls[0][0], controls[0][1]
     floor = length[0][0] if length else int(min_new_tokens)
-    return Settings(controls, penalty, vocab_range, temperature, top_k, bool(logprobs), length, floor)
+    return Settings(controls, penalty, vocab_range, temperature, top_k, bool(logprobs), length, floor, ras=ras)
 
 
 PLAN_PHASES = ("qkv", "o", "gu", "d")   # phase order of the persistent kernel's work plan
@@ -631,6 +687,7 @@ class SpeechLM:
         self._vocab_range = None    # (lo, hi) while the vocabulary range is on
         self._penalty_host = None   # host mirror of the per-slot repetition penalties (None: off)
         self._length_host = None    # host mirror of the per-slot length control (None: off)
+        self._ras_host = None       # host mirror of the per-slot repetition-aware sampling (None: off)
         self.logprobs = None        # per-token log-probabilities, [max_batch][max_new][2] on the device (None: off)
         self._guidance_host = None  # host mirror of the guidance table (None: off)
 
@@ -731,6 +788,22 @@ class SpeechLM:
         or decode."""
         self._write_slot_table("_length_host", self.L.nt_lm_set_length_control, _lib.SlotLength, check_length,
                                DEFAULT_LENGTH, rows, slots)
+
+    def set_repetition_aware_sampling(self, rows, slots=None) -> None:
+        """Per-slot Repetition Aware Sampling (VALL-E 2; CosyVoice 2's ``ras_sampling``).  ``rows``: one
+        (win_size, tau_r) pair or None (off) per slot of ``slots`` (default: slots 0..len(rows) - 1); every other slot
+        keeps its entry, or none when the table was off.  While a slot's entry is on, a sampled draw that occurs at
+        least ceil(win_size * tau_r) times among the slot's last win_size generated tokens (never its prompt) is
+        replaced by one draw from the whole distribution: the softmax of the processed scores times 1 / T, without the
+        top-k, top-p and min-p cuts.  Greedy and teacher-forced runs, and every slot's first token, never redraw.
+        ``None`` switches the table off.  Rules: ``check_ras``.  The table is copied on the current stream, so it is
+        ordered before the next prefill or decode."""
+        self._write_slot_table("_ras_host", self.L.nt_lm_set_repetition_aware_sampling, _lib.SlotRAS, ras_entry,
+                               RAS_OFF, None if rows is None else [(r,) for r in rows], slots)
+
+    def ras_redraws(self) -> torch.Tensor:
+        """Each slot's repetition-aware redraws since the prefill that filled it (int32 CPU tensor [max_batch])."""
+        return self.debug_buffer("ras_redraws", (self.max_batch,), torch.int32).cpu()
 
     def set_logprobs(self, on: bool = True):
         """Per-token log-probabilities.  While on, every later sampler launch writes, for each token it writes to
@@ -1041,7 +1114,8 @@ class SpeechLM:
                        greedy: bool = False, forced: torch.Tensor | None = None, check_every: int = 64, slot_base: int = 0,
                        top_p: float = 1.0, min_p: float = 0.0, vocab_range=None, repetition_penalty=1.0,
                        penalize_prompt=True, return_logprobs: bool = False, num_return_sequences: int = 1,
-                       exponential_decay_length_penalty=None, guidance_scale=1.0, negative_prompt_ids=None):
+                       exponential_decay_length_penalty=None, guidance_scale=1.0, negative_prompt_ids=None,
+                       repetition_aware_sampling=None):
         """Returns a list of int64 CPU tensors with the generated ids of each prompt (EOS included
         when it was sampled), following transformers' stopping rules (stopping_criteria.py:73-84,
         467-471): stop at EOS or when prompt + generated reaches max_length.  ``max_new_tokens`` may also be a
@@ -1064,13 +1138,19 @@ class SpeechLM:
         (``set_guidance``): prompt i stays in slot i and the unconditional sequence of each guided prompt, its negative
         prompt (default: the prompt's last token) followed by its draws, takes a slot above the prompts, so
         len(prompts) + guided prompts <= max_batch.  A guided prompt's cap is at most max_ctx - len(negative prompt).
-        Guidance with ``num_return_sequences`` > 1 raises ValueError."""
+        Guidance with ``num_return_sequences`` > 1 raises ValueError.
+
+        ``repetition_aware_sampling``: None, one (win_size, tau_r) pair or one None / pair per prompt
+        (``set_repetition_aware_sampling``): a sampled token that repeats at least ceil(win_size * tau_r) times among
+        the prompt's last win_size generated tokens is redrawn once from the whole distribution.  It follows its
+        prompt into every take and into a guided prompt's slot."""
         n_takes = check_takes(len(prompts), num_return_sequences, self.max_batch)
         caps, settings, guidance = self._prepare(
             prompts, max_length, max_new_tokens, guidance_scale, negative_prompt_ids, temperature=temperature, top_k=top_k,
             top_p=top_p, min_p=min_p, vocab_range=vocab_range, repetition_penalty=repetition_penalty,
             penalize_prompt=penalize_prompt, logprobs=return_logprobs, min_new_tokens=min_new_tokens,
-            exponential_decay_length_penalty=exponential_decay_length_penalty)
+            exponential_decay_length_penalty=exponential_decay_length_penalty,
+            repetition_aware_sampling=repetition_aware_sampling)
         pairs = guided_layout(len(prompts), guidance)
         if pairs and n_takes > 1:
             raise ValueError("classifier-free guidance takes one sequence per prompt (num_return_sequences=1)")
@@ -1106,7 +1186,8 @@ class SpeechLM:
                        greedy: bool = False, check_every: int = 32, slot_base: int = 0, top_p: float = 1.0,
                        min_p: float = 0.0, vocab_range=None, repetition_penalty=1.0, penalize_prompt=True,
                        return_logprobs: bool = False, num_return_sequences: int = 1,
-                       exponential_decay_length_penalty=None, guidance_scale=1.0, negative_prompt_ids=None):
+                       exponential_decay_length_penalty=None, guidance_scale=1.0, negative_prompt_ids=None,
+                       repetition_aware_sampling=None):
         """Continuous batching over any number of prompts: ``generate_batch``'s results and stopping rules, but a slot
         whose sequence finished is refilled with the next waiting prompt while the other slots keep decoding.
 
@@ -1128,7 +1209,8 @@ class SpeechLM:
 
         ``guidance_scale`` and ``negative_prompt_ids`` as in ``generate_batch``.  A guided prompt needs two free slots,
         filled by one ``prefill_slots`` call with the others admitted at that read; admission stays FIFO (the head of
-        the queue waits for room), and the pair's slots free together."""
+        the queue waits for room), and the pair's slots free together.  ``repetition_aware_sampling`` as in
+        ``generate_batch``; a newcomer's entry is written before its prefill."""
         if num_return_sequences != 1:
             raise ValueError("generate_queue returns one sequence per prompt; use generate_batch(num_return_sequences=n) "
                              "for several takes of each prompt")
@@ -1136,7 +1218,8 @@ class SpeechLM:
             prompts, max_length, max_new_tokens, guidance_scale, negative_prompt_ids, temperature=temperature, top_k=top_k,
             top_p=top_p, min_p=min_p, vocab_range=vocab_range, repetition_penalty=repetition_penalty,
             penalize_prompt=penalize_prompt, logprobs=return_logprobs, min_new_tokens=min_new_tokens,
-            exponential_decay_length_penalty=exponential_decay_length_penalty)
+            exponential_decay_length_penalty=exponential_decay_length_penalty,
+            repetition_aware_sampling=repetition_aware_sampling)
         n, M = len(prompts), self.max_batch
         if n == 0:
             return ([], []) if return_logprobs else []
@@ -1222,7 +1305,7 @@ class SpeechLM:
                  min_new_tokens: int = 0, max_new_tokens: int | None = None, seed: int | None = None,
                  top_p: float = 1.0, min_p: float = 0.0, vocab_range=None, repetition_penalty: float = 1.0,
                  num_return_sequences: int = 1, exponential_decay_length_penalty=None, guidance_scale=None,
-                 negative_prompt_ids=None, negative_prompt_attention_mask=None, **_):
+                 negative_prompt_ids=None, negative_prompt_attention_mask=None, repetition_aware_sampling=None, **_):
         """transformers-compatible seam used by ``NeuTTS._infer_torch`` (neutts/neutts.py:338-347).  ``top_p`` and
         ``min_p`` act as transformers' TopPLogitsWarper / MinPLogitsWarper; ``vocab_range`` (lo, hi) suppresses every
         id outside [lo, hi) and EOS (``set_vocab_range``); ``repetition_penalty`` acts as transformers'
@@ -1231,7 +1314,8 @@ class SpeechLM:
         from one prefill, [B * n, P + gen] with take j of row b at row b * n + j, as transformers; ``guidance_scale``
         with ``negative_prompt_ids`` ([1 or B, L]; default: each prompt's last token) acts as transformers'
         UnbatchedClassifierFreeGuidanceLogitsProcessor (``generate_batch``), and ``negative_prompt_attention_mask`` must
-        be None or all ones; other generation kwargs are ignored."""
+        be None or all ones; ``repetition_aware_sampling`` (win_size, tau_r) redraws repeating tokens
+        (``set_repetition_aware_sampling``); other generation kwargs are ignored."""
         if eos_token_id is None:
             raise ValueError("eos_token_id is required")
         if input_ids.dim() != 2:
@@ -1260,6 +1344,8 @@ class SpeechLM:
             cuts["num_return_sequences"] = num_return_sequences
         if exponential_decay_length_penalty is not None:
             cuts["exponential_decay_length_penalty"] = tuple(exponential_decay_length_penalty)
+        if repetition_aware_sampling is not None:
+            cuts["repetition_aware_sampling"] = tuple(repetition_aware_sampling)
         outs = self.generate_batch(prompts, eos_token_id, max_length, min_new_tokens, temperature, top_k,
                                    max_new_tokens, seed, greedy=not do_sample, **cuts, **guided)
         n = max(len(o) for o in outs)
