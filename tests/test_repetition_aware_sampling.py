@@ -11,6 +11,7 @@
 from __future__ import annotations
 
 import math
+from types import SimpleNamespace
 
 import numpy as np
 import pytest
@@ -18,9 +19,10 @@ import torch
 
 from neutts_air_b200.lm import RAS_OFF, Settings, check_ras, per_prompt_ras, ras_entry, resolve_settings
 from tests.fakes import EOS, FakeTokenizer, GenerateBackbone, GuidedStub, KwBackbone, QueueStub, _facade, _prompts
-from tests.ras_ref import (cosyvoice_redraws, draw_u2, full_logprobs, kernel_full_draw, min_count, ref_full_token,
-                           window_count)
-from tests.sampler_ref import SEED, draw_u, philox4x32_10
+from tests.processors_ref import model_ref
+from tests.ras_ref import (RasChecker, chunk_of, chunk_per, cosyvoice_redraws, draw_u2, full_logprobs, full_scores,
+                           kernel_full_draw, min_count, ref_full_token, window_count, window_cut)
+from tests.sampler_ref import SEED, draw_u, philox4x32_10, ref_token, ref_window_cut
 
 TAUS = [1e-9, 0.01, 0.05, 0.1, 1 / 3, 0.2, 0.25, 0.3, 0.5, 0.7, 0.75, 0.9, 0.99, 1.0, 0.1 + 0.2, 2 / 3]
 
@@ -78,6 +80,125 @@ def test_kernel_draw_lands_on_float64_cdf(V):
             tok, ok = ref_full_token(s, u2)
             got = kernel_full_draw(s, m, u2)
             assert got in ok and np.isfinite(s[got]), (V, case, u2, got, tok, ok)
+
+
+def _sp(eos, top_k=1):
+    return SimpleNamespace(eos_id=eos, seed=SEED, top_k=top_k)
+
+
+def _device_token(row, s, n, key, history, entry, floor, ctl):
+    """What a correct sampler draws: the cut window's inverse CDF of u1, or on a trigger the full row's of u2."""
+    T, k, tp, mp = ctl
+    ids, q, _ = ref_window_cut(row, n, EOS_V, floor, T, k, tp, mp)
+    t = ref_token((ids, q), draw_u(SEED, n, key))[0]
+    if entry is not None and n > 0 and window_count(history, n, entry[0], t) >= entry[1]:
+        return ref_full_token(full_scores(row, n, EOS_V, floor, T), draw_u2(SEED, n, key))[0], True
+    return t, False
+
+
+EOS_V = 4000   # the EOS id of the CPU rows below (V = 4142)
+
+
+def _loop_row(rng, V=4142, top=1234):
+    row = rng.normal(0.0, 1.5, V).astype(np.float32)
+    row[top] = 6.0
+    return row
+
+
+def test_neutral_controls_reduce_to_the_launch_checker():
+    """Per-slot entries (T, top_k, 1.0, 0.0) and floors equal to min_new check exactly as the launch-wide checker: the
+    same verdicts, redraws and windows over looping slots at several temperatures and top_k."""
+    rng = np.random.default_rng(5)
+    entries = [(4, 2), (1, 1), None, (10, 1)]
+    temps, top_k, min_new = [1.0, 0.7, 1.3, 2.0], 3, 2
+    old = RasChecker(_sp(EOS_V, top_k), entries, temps, min_new)
+    new = RasChecker(_sp(EOS_V, top_k), entries, temps, min_new, controls=[(T, top_k, 1.0, 0.0) for T in temps],
+                     floors=[min_new] * 4)
+    rows = [_loop_row(rng, top=100 + 7 * s) for s in range(4)]
+    hist = [[] for _ in range(4)]
+    for n in range(12):
+        for s in range(4):
+            got, _ = _device_token(rows[s], s, n, s, hist[s], entries[s], min_new, (temps[s], top_k, 1.0, 0.0))
+            hist[s].append(got)
+            verdict = old.check(rows[s], s, n, s, hist[s], got)
+            assert verdict is not None and new.check(rows[s], s, n, s, hist[s], got) == verdict, (s, n)
+    assert old.redrawn == new.redrawn and old.redraws > 0 and old.skipped == new.skipped == 0
+    assert old.windows.keys() == new.windows.keys()
+    assert all(np.array_equal(old.windows[x], new.windows[x]) for x in old.windows)
+
+
+def test_top_p_redraw_reads_the_whole_row():
+    """A slot whose top-p keeps one id (q0 > top_p): the draw is that id, and a triggered redraw lands on the full
+    row's inverse CDF of u2, outside the kept window; the window's id is refused there."""
+    rng = np.random.default_rng(7)
+    row = rng.normal(0.0, 1.0, 4142).astype(np.float32)
+    row[[50, 900, 3000]] = [9.0, 7.5, 8.0]
+    ctl = (0.9, 64, 0.3, 0.0)
+    ids, _, margin = ref_window_cut(row, 5, EOS_V, 0, *ctl)
+    assert ids.tolist() == [50] and margin > 1e-2
+    ck = RasChecker(_sp(EOS_V), [(2, 1)], [1.0], 0, controls=[ctl], floors=[0])
+    seen = 0
+    for n in range(1, 40):
+        tok, redrawn = _device_token(row, 0, n, 0, [50] * n, (2, 1), 0, ctl)
+        assert redrawn
+        ok = ref_full_token(full_scores(row, n, EOS_V, 0, ctl[0]), draw_u2(SEED, n, 0))[1]
+        if 50 in ok:
+            continue
+        assert ck.check(row, 0, n, 0, [50] * n, tok, sampled_lp=full_logprobs(full_scores(row, n, EOS_V, 0, ctl[0]))[tok],
+                        model_lp=model_ref(row, tok, EOS_V, False)) is True
+        with pytest.raises(AssertionError):
+            ck.check(row, 0, n, 0, [50] * n, 50)
+        seen += tok not in ids
+    assert seen >= 3 and ck.worst_lp == 0.0
+
+
+def test_floor_masks_eos_in_the_redraw():
+    """Below a slot's floor the redraw's row leaves EOS out: where the unmasked full row draws EOS, the checker wants
+    the next id with mass and refuses EOS; at or above the floor it accepts EOS."""
+    row = np.full(4142, -30.0, dtype=np.float32)
+    row[EOS_V - 10], row[EOS_V] = 6.0, 5.0              # EOS (19 % of the mass) sorts after the looping id
+    row[EOS_V + 7] = 5.5
+    ctl = (1.0, 1, 1.0, 0.0)
+    for floor in (3, 30):
+        ck = RasChecker(_sp(EOS_V), [(3, 1)], [1.0], 0, controls=[ctl], floors=[floor])
+        hits = 0
+        for n in range(1, 30):
+            hist = [EOS_V - 10] * n
+            open_tok = ref_full_token(full_scores(row, n, EOS_V, 0, 1.0), draw_u2(SEED, n, 0))[0]
+            tok, redrawn = _device_token(row, 0, n, 0, hist, (3, 1), floor, ctl)
+            assert redrawn and (tok != EOS_V if n < floor else tok == open_tok)
+            if open_tok == EOS_V and n < floor:
+                hits += 1
+                assert ck.check(row, 0, n, 0, hist, tok) is True
+                with pytest.raises(AssertionError):
+                    ck.check(row, 0, n, 0, hist, EOS_V)
+            elif open_tok == EOS_V:
+                hits += 1
+                assert ck.check(row, 0, n, 0, hist, EOS_V) is True
+        assert hits >= 2, floor
+
+
+def test_full_row_chunks_at_v4142():
+    """V = 4142: 20 ids per thread, threads 208..255 hold no id and thread 207 the 2-id chunk [4140, 4142).  The
+    kernel's fp32 draw restated (``kernel_full_draw``) lands on the float64 CDF when the mass sits in that last chunk,
+    in a chunk boundary's neighbours and in an empty thread's range; ``window_cut`` equals ``ref_window_cut``."""
+    V = 4142
+    assert chunk_per(V) == 20 and chunk_of(V, 4141) == (207, (4140, 4142)) and chunk_of(V, 4139) == (206, (4120, 4140))
+    assert all(chunk_of(V, 0)[0] == 0 and min(V, t * 20) == V for t in range(208, 256))
+    rng = np.random.default_rng(11)
+    for hot in ([4140], [4141], [4140, 4141], [4139, 4140], [19, 20], [4100, 4141]):
+        s = (rng.normal(0, 1, V) - 8).astype(np.float32)
+        s[hot] = 4.0
+        m = float(s.max())
+        for u2 in (0.0, 0.3, 0.5, 0.97, 1 - 2 ** -24, float(rng.random())):
+            tok, ok = ref_full_token(s, u2)
+            assert kernel_full_draw(s, m, u2) in ok, (hot, u2, tok, ok)
+    for case in range(6):
+        row = rng.normal(0, 2, V).astype(np.float32)
+        row[rng.integers(V, size=5)] = 3.0                  # ties across the window's edge
+        args = (case, EOS_V, 2, (0.7, 1.3)[case % 2], (1, 8, 64)[case % 3], (1.0, 0.6)[case % 2], (0.0, 0.1)[case % 3 == 2])
+        a, b = window_cut(row, *args), ref_window_cut(row, *args)
+        assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1]) and a[2] == b[2]
 
 
 # ---------------------------------------------------------------------------------------- host validation
