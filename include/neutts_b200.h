@@ -573,6 +573,47 @@ int nt_stretch_push(nt_stretch* st, int n, const int32_t* rows, const int32_t* f
 void* nt_stretch_debug_ptr(nt_stretch* st, const char* name);
 
 /* ------------------------------------------------------------------------------------------
+ * Loudness: ITU-R BS.1770-4 integrated loudness of mono rows, and normalisation to a target
+ * ------------------------------------------------------------------------------------------
+ * Input: mono fp32 PCM at rate r, r a multiple of 10 Hz in [8000, 192000] (so a gating block is exactly four steps;
+ * any other rate is NT_ERR_INVALID).  Everything below is computed in fp64.
+ *   K-weighting: two biquads in cascade, zero initial state, no clamping; coefficients as torchaudio's formulas,
+ *     normalised by a0: treble_biquad(gain 4.0, central_freq 1500, Q 1/sqrt(2)), then highpass_biquad(38, Q 0.5).
+ *   Blocks: gate = round(0.4 r), step = gate / 4; nb = floor((n - gate) / step) + 1 full blocks (none when n < gate);
+ *     block j is y[j step, j step + gate) and z_j the mean of y^2 over it.
+ *   Gating: l_j = -0.691 + 10 log10(z_j); absolute gate l_j > -70; G_r = -0.691 + 10 log10(mean z over the blocks
+ *     above the absolute gate) - 10; relative gate l_j > G_r and l_j > -70;
+ *     L = -0.691 + 10 log10(mean z over the blocks that pass both).  L is NaN when no block passes (silence, n < gate).
+ * L equals torchaudio.functional.loudness(x[None], r) in float64 whenever both K-weighting stages stay inside [-1, 1].
+ * Two differences are deliberate: torchaudio's lfilter clamps every stage's output to [-1, 1] (BS.1770 does not, and
+ * neither does this meter), and torchaudio raises for n < gate where this meter returns NaN.
+ * Normalisation to a target T: g = 10^((T - L) / 20) in fp64 and each output sample is float32(g * (double)x), rounded
+ * once.  A row whose L or T is NaN comes back bit for bit unchanged.  There is no limiter: outputs may exceed +-1.
+ * The recursion runs in chunks of info.chunk samples (chunk divides step): pass 1 runs every chunk from zero state,
+ * the true start states follow exactly by linearity (per step, then along the row), and pass 2 re-runs every chunk from
+ * its true state.  No float atomics: two runs give the same bits. */
+typedef struct {
+  int32_t gate, step;          /* samples per gating block and per 100 ms step */
+  int32_t chunk;               /* samples one thread filters */
+  int32_t chunks_per_step;     /* step / chunk */
+} nt_loudness_info;
+
+/* Geometry for a rate (needs no GPU); NT_ERR_INVALID, with the reason, for a rejected rate. */
+int nt_loudness_query(int sample_rate, nt_loudness_info* info);
+/* Device workspace bytes nt_loudness_run needs for these rows (host offsets, n + 1 non-decreasing entries); 0 for
+ * n == 0 or invalid arguments (the reason in nt_last_error). */
+size_t nt_loudness_workspace_bytes(int sample_rate, int n, const int64_t* in_offsets);
+/* Measure n rows and optionally normalise them, stateless, on `stream`.  in: device fp32, row i at
+ * in[in_offsets[i] .. in_offsets[i + 1]) (host offsets).  lufs: device fp64 [n], L of every row.  targets: host fp64
+ * [n] in LUFS, or NULL to measure only; a NaN target leaves its row unchanged, an infinite one is NT_ERR_INVALID.  out:
+ * device fp32 at the same offsets (may equal in), written only when targets is not NULL.  workspace: device memory,
+ * 16-byte aligned, of at least nt_loudness_workspace_bytes (NT_ERR_NOMEM otherwise).  Rows go in groups of 128; each
+ * group is one host-to-device copy of the chunk transition powers followed by up to six launches.  Nothing
+ * synchronises the host. */
+int nt_loudness_run(int sample_rate, int n, const float* in, const int64_t* in_offsets, const double* targets,
+                    double* lufs, float* out, void* workspace, size_t bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Single-op entry points (unit tests; each mirrors one row of SURVEY.md §8a)
  * ------------------------------------------------------------------------------------------ */
 int nt_op_rmsnorm(const float* x, const float* w, float eps, int rows, int cols, float* out_f32, void* out_bf16,

@@ -93,6 +93,18 @@ def _speeds(n: int, speed):
     return s if any(x != 1.0 for x in s) else None
 
 
+def _targets(n: int, loudness):
+    """One loudness target per utterance (``loudness`` None, a number, or one number / None per utterance, each finite
+    and in [-70, 0] LUFS; ValueError otherwise), or None when no utterance has one: then nothing is measured."""
+    from neutts_air_b200.loudness import check_target
+
+    if loudness is None:
+        return None
+    t = per_item(n, "utterance", loudness=loudness)["loudness"]
+    t = [None if x is None else check_target(x) for x in t] if isinstance(t, list) else [check_target(t)] * n
+    return t if any(x is not None for x in t) else None
+
+
 def _pick(ctl: dict, idx) -> dict:
     """The controls of the utterances ``idx`` (lists are indexed, scalars stay)."""
     return {k: [v[i] for i in idx] if isinstance(v, list) else v for k, v in ctl.items()}
@@ -440,13 +452,14 @@ class NeuTTS:
             self._stretcher = TimeStretch(device=self.codec.device, max_rows=rows)
         return self._stretcher
 
-    def _decode_codes(self, codes: Sequence[torch.Tensor], watermark: bool = False, speeds=None) -> list:
+    def _decode_codes(self, codes: Sequence[torch.Tensor], watermark: bool = False, speeds=None, targets=None) -> list:
         """codes: list of 1-D int tensors -> list of numpy waveforms at ``sample_rate`` in ``pcm_format`` (batched by
         equal length).  ``watermark``: each waveform is watermarked at 24 kHz, before any resampling.  ``speeds``: None
         or one speaking rate per waveform; a waveform whose rate is not 1.0 is stretched at 24 kHz right after the
-        codec, before the watermark and the resampler."""
-        if speeds is not None:
-            return self._decode_stretched(codes, watermark, speeds)
+        codec, before the watermark and the resampler.  ``targets``: None or one loudness target (LUFS, or None) per
+        waveform; a waveform with one is normalised to it at 24 kHz after the stretch, before the watermark."""
+        if speeds is not None or targets is not None:
+            return self._decode_stretched(codes, watermark, speeds, targets)
         rs = self._output_resampler()
         out = [None] * len(codes)
         by_len: dict = {}
@@ -477,10 +490,14 @@ class NeuTTS:
             out = [self._watermark(w) for w in out]
         return out
 
-    def _decode_stretched(self, codes, watermark: bool, speeds) -> list:
-        """``_decode_codes`` with speaking rates: per waveform codec -> stretch (rate != 1.0) -> watermark -> resample,
-        the stretch and the resampler on the device; a waveform at 1.0 gets the bytes it gets without rates."""
-        rs, ts = self._output_resampler(), self._time_stretch()
+    def _decode_stretched(self, codes, watermark: bool, speeds, targets=None) -> list:
+        """``_decode_codes`` with speaking rates or loudness targets (either may be None): per waveform codec -> stretch
+        (rate != 1.0) -> loudness (a target) -> watermark -> resample, all but the watermark on the device; a waveform
+        at 1.0 without a target gets the bytes it gets without either."""
+        from neutts_air_b200.loudness import normalize
+
+        rs = self._output_resampler()
+        ts = self._time_stretch() if speeds is not None else None
         out = [None] * len(codes)
         by_len: dict = {}
         for i, c in enumerate(codes):
@@ -495,9 +512,14 @@ class NeuTTS:
                 with torch.no_grad():
                     pcm = self.codec.decode_code(batch)[:, 0, :]
                 rows = list(pcm)
-                fast = [r for r, i in enumerate(grp) if speeds[i] != 1.0]
-                for r, y in zip(fast, ts.stretch([rows[r] for r in fast], [speeds[grp[r]] for r in fast])):
-                    rows[r] = y
+                fast = [r for r, i in enumerate(grp) if speeds is not None and speeds[i] != 1.0]
+                if fast:
+                    for r, y in zip(fast, ts.stretch([rows[r] for r in fast], [speeds[grp[r]] for r in fast])):
+                        rows[r] = y
+                level = [r for r, i in enumerate(grp) if targets is not None and targets[i] is not None]
+                if level:
+                    for r, y in zip(level, normalize([rows[r] for r in level], [targets[grp[r]] for r in level])):
+                        rows[r] = y
                 for r, i in enumerate(grp):
                     w = rows[r]
                     if watermark and self.watermarker is not None:
@@ -527,26 +549,29 @@ class NeuTTS:
               min_p: float = 0.0, repetition_penalty: float = 1.0, penalize_prompt: bool = True,
               return_logprobs: bool = False, takes: int = 1, min_new_tokens: int = 50,
               exponential_decay_length_penalty=None, guidance_scale: float = 1.0, negative_text: str | None = None,
-              speed: float = 1.0, long_form: bool = False, pause: float = 0.0, repetition_aware_sampling=None):
+              speed: float = 1.0, long_form: bool = False, pause: float = 0.0, repetition_aware_sampling=None,
+              loudness=None):
         """Text + reference voice -> 24 kHz float32 waveform (``neutts/neutts.py:216-243``).  The sampling controls
         default to the reference's values; see ``infer_batch``.  ``return_logprobs``: returns (waveform, log-probs).
         ``takes``: generate that many takes and keep the most probable one (``infer_batch``).  ``guidance_scale`` and
         ``negative_text``: classifier-free guidance (``infer_batch``).  ``speed``: speaking rate (``infer_batch``).
         ``long_form`` and ``pause``: a text longer than the context, in segments (``infer_batch``).
-        ``repetition_aware_sampling``: redraw a token that loops (``infer_batch``)."""
+        ``repetition_aware_sampling``: redraw a token that loops (``infer_batch``).  ``loudness``: a target in LUFS
+        (``infer_batch``)."""
         out = self.infer_batch([text], [ref_codes], [ref_text], temperature=temperature, top_k=top_k, top_p=top_p,
                                min_p=min_p, repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt,
                                return_logprobs=return_logprobs, takes=takes, min_new_tokens=min_new_tokens,
                                exponential_decay_length_penalty=exponential_decay_length_penalty,
                                guidance_scale=guidance_scale, negative_text=negative_text, speed=speed,
-                               long_form=long_form, pause=pause, repetition_aware_sampling=repetition_aware_sampling)
+                               long_form=long_form, pause=pause, repetition_aware_sampling=repetition_aware_sampling,
+                               loudness=loudness)
         return (out[0][0], out[1][0]) if return_logprobs else out[0]
 
     def infer_from_prompt_ids(self, prompts: Sequence[Sequence[int]], max_new_tokens: int | None = None,
                               min_new_tokens: int = 50, slot_base: int = 0, *, temperature=1.0, top_k=50, top_p=1.0,
                               min_p=0.0, repetition_penalty=1.0, penalize_prompt=True, return_logprobs: bool = False,
                               takes: int = 1, exponential_decay_length_penalty=None, guidance_scale=1.0,
-                              negative_prompt_ids=None, speed=1.0, repetition_aware_sampling=None):
+                              negative_prompt_ids=None, speed=1.0, repetition_aware_sampling=None, loudness=None):
         """Hot path only: prompt ids (host) -> waveforms (host).  Used by bench.py's end-to-end leg.
         ``slot_base`` offsets the sampler's Philox slot index so chunks / ranks under one seed draw independently.
         More prompts than ``max_batch`` go through the backbone's ``generate_queue`` when it has one.  Sampling
@@ -556,8 +581,9 @@ class NeuTTS:
         classifier-free guidance (``SpeechLM.generate_batch``; transformers' ``guidance_scale`` and
         ``negative_prompt_ids`` on an injected transformers backbone).  ``speed``: speaking rate of each waveform (a
         number or one per prompt, ``infer_batch``); it acts on the PCM alone and never reaches the backbone.
-        ``repetition_aware_sampling`` as in ``infer_batch``."""
+        ``repetition_aware_sampling`` and ``loudness`` (a target or one per prompt) as in ``infer_batch``."""
         speeds = _speeds(len(prompts), speed)
+        targets = _targets(len(prompts), loudness)
         ctl = _controls(len(prompts), temperature, top_k, top_p, min_p, repetition_penalty, penalize_prompt, min_new_tokens,
                         exponential_decay_length_penalty, repetition_aware_sampling)
         self._check_ras(ctl)
@@ -570,14 +596,14 @@ class NeuTTS:
                                  takes=takes)
         if return_logprobs:
             gen, lps = gen
-        wavs = self._decode_codes([self._ids_to_codes(g) for g in gen], watermark=True, speeds=speeds)
+        wavs = self._decode_codes([self._ids_to_codes(g) for g in gen], watermark=True, speeds=speeds, targets=targets)
         return (wavs, [lp.numpy() for lp in lps]) if return_logprobs else wavs
 
     def infer_batch(self, texts: Sequence[str], ref_codes: Sequence, ref_texts: Sequence[str], distributed: bool = False, *,
                     temperature=1.0, top_k=50, top_p=1.0, min_p=0.0, repetition_penalty=1.0, penalize_prompt=True,
                     return_logprobs: bool = False, takes: int = 1, min_new_tokens=50, exponential_decay_length_penalty=None,
                     guidance_scale=1.0, negative_text=None, speed=1.0, long_form: bool = False, pause: float = 0.0,
-                    repetition_aware_sampling=None):
+                    repetition_aware_sampling=None, loudness=None):
         """List in / list out.  With ``distributed=True`` (inside an initialised torch.distributed job) the
         utterances are sharded over ranks and every rank returns all waveforms (one all-gather).
 
@@ -637,21 +663,34 @@ class NeuTTS:
         list follows its utterances through chunking, the queue, takes (the kept take is stretched) and the sharding
         over ranks.  An utterance at exactly 1.0 is not stretched; with every speed at 1.0 nothing changes.
 
+        ``loudness`` (None, a target in LUFS, or one target or None per utterance; each finite and in [-70, 0], e.g.
+        -16 for podcasts and streaming, -23 for EBU R128 broadcast) normalises each waveform on the GPU to that
+        ITU-R BS.1770-4 integrated loudness (``neutts_air_b200.loudness``), measured at 24 kHz after the stretch and
+        before the watermark and any resampling: the waveform is scaled by 10^((target - L) / 20).  There is no limiter,
+        so float32 samples may exceed +-1 (int16 output clips).  A waveform that is silent or shorter than 400 ms has no
+        loudness and comes back unchanged; one where the gain moves a 400 ms block across the -70 LUFS absolute gate
+        re-measures slightly off its target.  A list follows its utterances through chunking, the queue, takes (the kept
+        take is normalised), long-form segments and the sharding over ranks.  With ``loudness=None`` nothing changes.
+
         ``long_form=True``: a text too long for one prompt is split into segments that fit (``segments``); the
         segments of all texts run as one batch (segment 0 of every text first, then segment 1 of every text that has
         one, and so on; segment j of that order draws from random stream j), each with its text's controls, and each
         text's waveforms are joined after the codec, stretch, watermark and resampler with 10 ms fades at every seam
         and ``pause`` seconds (in [0, 10]) of silence between segments.  A text that fits is one segment and comes back
-        as without ``long_form``.  With ``return_logprobs`` a text's rows are its segments' rows, concatenated."""
+        as without ``long_form``.  With ``return_logprobs`` a text's rows are its segments' rows, concatenated.  Each
+        segment is normalised to its text's ``loudness`` target before the join, so a joined text sits near its target
+        but not exactly on it (the fades and pauses change its blocks)."""
         if not (len(texts) == len(ref_codes) == len(ref_texts)):
             raise ValueError("texts, ref_codes and ref_texts must have the same length")
         pause = longform.check_pause(pause, long_form)
+        targets = _targets(len(texts), loudness)
         if long_form:
             owners, flat, refs, rts, kw = self._long_form_plan(
                 texts, ref_codes, ref_texts, temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p,
                 repetition_penalty=repetition_penalty, penalize_prompt=penalize_prompt, min_new_tokens=min_new_tokens,
                 exponential_decay_length_penalty=exponential_decay_length_penalty, guidance_scale=guidance_scale,
-                negative_text=negative_text, speed=speed, repetition_aware_sampling=repetition_aware_sampling)
+                negative_text=negative_text, speed=speed, repetition_aware_sampling=repetition_aware_sampling,
+                loudness=targets)
             out = self.infer_batch(flat, refs, rts, distributed, return_logprobs=return_logprobs, takes=takes, **kw)
             wavs, lps = out if return_logprobs else (out, None)
             idx = [[j for j, o in enumerate(owners) if o == t] for t in range(len(texts))]
@@ -670,7 +709,7 @@ class NeuTTS:
             self._check_logprobs(distributed)
         prompts = [self._apply_chat_template(c, rt, t) for t, c, rt in zip(texts, ref_codes, ref_texts)]
         if takes > 1:
-            return self._infer_takes(prompts, ctl, takes, return_logprobs, speeds)
+            return self._infer_takes(prompts, ctl, takes, return_logprobs, speeds, targets)
         queue = hasattr(self.backbone, "generate_queue")
 
         def run(idx, slot_base):
@@ -678,7 +717,8 @@ class NeuTTS:
             g, neg = c.pop("guidance_scale", 1.0), c.pop("negative_prompt_ids", None)
             return self.infer_from_prompt_ids([prompts[i] for i in idx], slot_base=slot_base, return_logprobs=return_logprobs,
                                               guidance_scale=g, negative_prompt_ids=neg,
-                                              speed=1.0 if speeds is None else [speeds[i] for i in idx], **c)
+                                              speed=1.0 if speeds is None else [speeds[i] for i in idx],
+                                              loudness=None if targets is None else [targets[i] for i in idx], **c)
 
         # chunks of prompts whose slots (two for a guided one) fit the engine; prompt i keeps Philox stream i
         chunks, j = [], 0
@@ -719,11 +759,12 @@ class NeuTTS:
         per = max_batch // takes
         return [(range(j, min(j + per, n_utterances)), j * takes) for j in range(0, n_utterances, per)]
 
-    def _infer_takes(self, prompts, ctl: dict, takes: int, return_logprobs: bool, speeds=None):
+    def _infer_takes(self, prompts, ctl: dict, takes: int, return_logprobs: bool, speeds=None, targets=None):
         out, lps = [], []
         for idx, slot_base in self.take_chunks(len(prompts), takes, self.max_batch):
             r = self.infer_from_prompt_ids([prompts[i] for i in idx], slot_base=slot_base, return_logprobs=return_logprobs,
                                            takes=takes, speed=1.0 if speeds is None else [speeds[i] for i in idx],
+                                           loudness=None if targets is None else [targets[i] for i in idx],
                                            **_pick(ctl, idx))
             out += r[0] if return_logprobs else r
             lps += r[1] if return_logprobs else []
@@ -859,7 +900,8 @@ class NeuTTS:
         and generates one take per utterance (``takes`` other than 1 raises ValueError); classifier-free guidance is not
         supported (``guidance_scale`` other than 1 raises ValueError).  ``speed``: speaking rate (``infer_batch``); each
         cross-faded chunk goes through the stretcher's stream, so the chunks concatenate to the stretched stream.
-        ``long_form`` and ``pause``: a text longer than the context, in segments (``infer_stream_batch``)."""
+        ``long_form`` and ``pause``: a text longer than the context, in segments (``infer_stream_batch``).  There is
+        no ``loudness``: integrated loudness needs the whole utterance before its first sample can be scaled."""
         self._no_takes(takes)
         self._no_guidance(guidance_scale, "streaming synthesis")
         if self._is_quantized_model:  # kept for signature parity; never true on this build
@@ -903,7 +945,8 @@ class NeuTTS:
         per utterance (``takes`` other than 1 raises ValueError); ``guidance_scale`` other than 1 raises ValueError.
         ``speed`` (a number or one per utterance): speaking rate, as in ``infer_batch``; it follows its utterance into
         whichever slot it takes.  Chunks go codec -> cross-fade -> stretch -> resample, and concatenate to the stretched
-        stream.
+        stream.  Streams take no ``loudness`` target: integrated loudness needs the whole utterance before its first
+        sample can be scaled (normalise the finished waveforms with ``neutts_air_b200.loudness.normalize`` instead).
 
         ``long_form=True``: the texts are split and their segments ordered as in ``infer_batch``, and all segments stream
         as one queue; each text still gets one entry per yield.  A text plays its segments in order: chunks of a later

@@ -105,6 +105,10 @@ class StretchInfo(C.Structure):
                 ("table_bytes", C.c_size_t), ("row_bytes", C.c_size_t), ("scratch_bytes", C.c_size_t)]
 
 
+class LoudnessInfo(C.Structure):
+    _fields_ = [("gate", C.c_int32), ("step", C.c_int32), ("chunk", C.c_int32), ("chunks_per_step", C.c_int32)]
+
+
 class CodecWeights(C.Structure):
     _fields_ = [
         ("fsq_w", C.c_void_p), ("fsq_b", C.c_void_p), ("embed_w", C.c_void_p), ("embed_b", C.c_void_p),
@@ -132,6 +136,7 @@ EXPORTS = [
     "nt_resampler_query", "nt_resampler_create", "nt_resampler_destroy", "nt_resampler_reset", "nt_resampler_push",
     "nt_stretch_query", "nt_stretch_create", "nt_stretch_destroy", "nt_stretch_reset", "nt_stretch_push",
     "nt_stretch_debug_ptr",
+    "nt_loudness_query", "nt_loudness_workspace_bytes", "nt_loudness_run",
     "nt_op_rmsnorm", "nt_op_topk_sample",
 ]
 
@@ -212,6 +217,11 @@ def lib() -> C.CDLL:
                                   C.c_void_p, C.POINTER(C.c_int64), C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]
     L.nt_stretch_debug_ptr.restype = C.c_void_p
     L.nt_stretch_debug_ptr.argtypes = [C.c_void_p, C.c_char_p]
+    L.nt_loudness_query.argtypes = [C.c_int, C.POINTER(LoudnessInfo)]
+    L.nt_loudness_workspace_bytes.restype = C.c_size_t
+    L.nt_loudness_workspace_bytes.argtypes = [C.c_int, C.c_int, C.POINTER(C.c_int64)]
+    L.nt_loudness_run.argtypes = [C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_double), C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.nt_op_rmsnorm.argtypes = [C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     L.nt_op_topk_sample.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(Sampling), C.c_void_p, C.c_int32,
                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
